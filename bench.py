@@ -2,7 +2,7 @@
 """bench.py -- BASELINE.json metric: utterances/sec, ECAPA-TDNN + Fbank-80, 3 s @ 16 kHz, waveform -> 192-d
 embedding (configs[1]: batch 256 x 3 s synthetic audio per GPU).
 
-  python bench.py [--gpus N --steps K --warmup W] [--impl ours|reference] [--precision bf16x3|bf16]
+  python bench.py [--gpus N --steps K --warmup W] [--impl ours|reference] [--precision bf16x3|bf16] [--dump-outputs DIR]
 
 One "step" = one batch of 256 utterances through the whole hot path.
   value     device-resident waveforms -> embeddings on device, CUDA events around the K timed steps, LANES batches in
@@ -10,6 +10,8 @@ One "step" = one batch of 256 utterances through the whole hot path.
             kernels leave idle at their tails and between dependent launches); `single_lane` = one batch at a time
   e2e       the same through PPVectorPredictor.extract_embeddings_stream: pinned host fp32 waveforms -> H2D (copy
             stream) -> hot path (LANES lanes) -> D2H embeddings, every step
+  --dump-outputs DIR  after the timed steps, rank 0 writes the embeddings of the last timed step (float32 [256, 192]) to
+            DIR/embeddings.npy; the inputs are seeded, so two builds can be compared output for output
   roofline  tensor-core gather-GEMM (the dominant kernel): algorithmic FLOPs / its summed launch time, measured
             with CUDA events on the launching stream around every kernel of the K steps of the single-lane pass
   cpu_baseline  the oracle (torch CPU port of the reference path; Paddle is not installable) on a bounded sample
@@ -59,8 +61,8 @@ def synth_wave(batch, seed):
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region (B200_PROFILING.md recipe), polled through NVML every 50 ms in a
-    thread (in-process: an nvidia-smi subprocess needs ~100 ms before its first sample); falls back to nvidia-smi -lms."""
+    """SM clock / throttle reasons DURING the timed region, polled through NVML every 50 ms in a thread (in-process: an
+    nvidia-smi subprocess needs ~100 ms before its first sample); falls back to nvidia-smi -lms."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -96,7 +98,7 @@ class ClockSampler:
                 self.power.append(n.nvmlDeviceGetPowerUsage(self.h) / 1000.0)
             except Exception:
                 pass
-            time.sleep(0.05)  # B200_PROFILING.md samples at 200 ms; a 2 ms poll from a Python thread was measured to disturb the host-paced multi-lane pass
+            time.sleep(0.05)  # a 2 ms poll from a Python thread disturbs the host-paced multi-lane pass
 
     def start(self):
         if self.nvml is not None:
@@ -153,7 +155,7 @@ def bench_config(world):
     return {"workload": "ECAPA-TDNN (configs/ecapa_tdnn.yml) Fbank-80 embedding extraction, batch 256 x 3 s @ 16 kHz synthetic audio per GPU (BASELINE configs[1])",
             "batch_per_gpu": BATCH, "global_batch": BATCH * world, "samples": SAMPLES, "frames": FRAMES,
             "parallelism": f"dp{world} (independent utterance shards, no collective)",
-            "l2": "two alternating input batches; per-step working set ~2.2 GB >> 126 MB L2"}
+            "l2": "two alternating input batches; per-step working set ~2.2 GB >> 50 MB L2"}
 
 
 def seeded_ecapa_weights():
@@ -240,6 +242,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "bf16"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the embeddings of the last timed step to DIR/embeddings.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -247,6 +251,8 @@ def main():
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":
+        if args.dump_outputs:  # the CPU arm times a calibrated sample whose size varies from run to run: nothing comparable to dump
+            ap.error("--dump-outputs needs --impl ours")
         return run_reference(args, rank, world)
 
     import ctypes as C
@@ -269,7 +275,7 @@ def main():
     model, fz = pred.predictor, pred._audio_featurizer
     lib = _lib.load()
 
-    # two distinct device-resident batches; working set per step (49 MB waveforms + ~2.2 GB activations) >> 126 MB L2
+    # two distinct device-resident batches; working set per step (49 MB waveforms + ~2.2 GB activations) >> 50 MB L2
     wavs = [synth_wave(BATCH, 1000 + rank * 10 + i).to(dev) for i in range(2)]
     host = [synth_wave(BATCH, 2000 + rank * 10 + i).pin_memory() for i in range(2)]
 
@@ -314,6 +320,9 @@ def main():
     clk = clocks.stop() if rank == 0 else None
     assert torch.isfinite(last).all() and torch.equal(last, emb)  # the last batch of both passes is the same input: bitwise equal embeddings
     del last
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "embeddings.npy"), emb.float().cpu().numpy())
 
     # ---- end to end through the public API (host buffers) -----------------------------------------------------
     for out in pred.extract_embeddings_stream((host[i % 2] for i in range(2 * LANES)), lanes=LANES):
@@ -338,20 +347,15 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_sus = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_burst = peaks.get("bf16_tflops", 1700.0)
+        # fallback: NVIDIA's H100 SXM data sheet, dense BF16 (700 W card); a data-sheet figure, not a measured one
+        peak_sus = peaks.get("bf16_tflops_sustained", 989.0)
+        peak_burst = peaks.get("bf16_tflops", 989.0)
         # which peak applies: the timed region is short (K steps x ~3 ms); if the SM clock stayed near its maximum the cuBLAS
         # figure measured under the same conditions is the BURST one, a long (power-capped) run compares with the sustained one.
         burst = bool(clk and clk.get("sm_mhz") and clk.get("sm_max_mhz") and clk["sm_mhz"] >= 0.93 * clk["sm_max_mhz"])
         peak_tf = peak_burst if burst else peak_sus
-        src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"
+        src = "MEASURED_PEAKS.json" if peaks else "fallback (H100 SXM data sheet, dense BF16)"
         peak_src = (f"{src} {'bf16_tflops (burst: SM clock stayed >= 93 % of max during the timed region)' if burst else 'bf16_tflops_sustained (SM clock below 93 % of max during the timed region)'}")
-        traffic, traffic_src = None, None
-        try:  # per-launch DRAM bytes of the tensor-core kernels from the committed ncu --set full capture
-            tj = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-            traffic, traffic_src = tj["traffic_bytes_per_launch"], tj["source"]
-        except Exception:
-            pass
         flops_step = algorithmic_flops_per_utt() * BATCH
         gemm_s_per_step = g_ms.value / 1000.0 / args.steps
         achieved = flops_step / gemm_s_per_step / 1e12
@@ -383,8 +387,7 @@ def main():
                          "frac_vs_burst_peak": achieved / peak_burst, "frac_vs_sustained_peak": achieved / peak_sus,
                          "whole_step_tflops": step_tf, "whole_step_frac": step_tf / peak_tf,
                          "peak_burst": peak_burst, "peak_sustained": peak_sus, "sm_mhz_observed": clk.get("sm_mhz") if clk else None,
-                         "traffic": traffic, "traffic_source": traffic_src,
-                         "kernel": "tcgen05 gather-GEMM family: gemm_tcgen05_kernel + res2chain_kernel + asp_fused_kernel (every conv / linear layer)",
+                         "kernel": "wgmma gather-GEMM family: gemm_wgmma_kernel + res2chain_kernel + asp_fused_kernel (every conv / linear layer)",
                          "launches_per_step": g_n.value / args.steps, "ms_per_step_in_kernel": 1000.0 * gemm_s_per_step,
                          "timed_in": f"pass A ({args.steps} steps, one batch at a time, a CUDA event pair around every kernel on the launching stream); "
                                      "with several batches in flight the kernels of different batches share the SMs and their elapsed times overlap",

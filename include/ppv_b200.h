@@ -1,4 +1,4 @@
-/* libppv_b200 -- C ABI of the B200-native ppvector hot path.
+/* libppv_b200 -- C ABI of the H100-native ppvector hot path.
  *
  * The reference (yeyupiaoling/VoiceprintRecognition-PaddlePaddle) has NO plugin / FFI interface:
  * its boundary is the Python class surface.  Each entry point below names the reference
@@ -9,7 +9,7 @@
  *     (per-call scratch is the caller's workspace);
  *   - every call is asynchronous on `stream` (a cudaStream_t passed as void*), no hidden sync;
  *   - return value: 0 = PPV_OK, negative = error; ppv_last_error() gives the text;
- *   - sm_100a only; there is no CPU fallback.
+ *   - sm_90a (H100) only; there is no CPU fallback.
  */
 #ifndef PPV_B200_H
 #define PPV_B200_H
@@ -249,7 +249,7 @@ int64_t ppv_trainer_stat_count(const ppv_trainer_t* h);  /* floats in the runnin
 int ppv_trainer_lookup(const ppv_trainer_t* h, const char* name, int64_t* offset, int64_t* numel, int* is_stat);
 int ppv_trainer_bind(ppv_trainer_t* h, float* params, float* grads, float* stats);
 /* Operand precision of the step's GEMMs (forward, data gradients, weight gradients): PPV_PREC_BF16X3 (default, fp32-grade) or
- * PPV_PREC_BF16 -- the B200 form of train_conf.enable_amp (ppvector/trainer.py:167, 209-229: paddle.amp.auto_cast level O1 + GradScaler
+ * PPV_PREC_BF16 -- the single-pass bf16 form of train_conf.enable_amp (ppvector/trainer.py:167, 209-229: paddle.amp.auto_cast level O1 + GradScaler
  * around the same step): single-pass bf16 operands, fp32 accumulation, fp32 BatchNorm / pooling / loss / master weights / Adam; bf16
  * keeps fp32's exponent range, so there is no loss scaling. */
 int ppv_trainer_set_precision(ppv_trainer_t* h, int precision);
@@ -338,7 +338,7 @@ int ppv_aam_backward(const float* emb, const float* W, const int64_t* labels, co
 
 /* ---------------------------------------------------------------------------------------------
  * Test hook for the tensor-core GEMM (not a reference entry point): out[M,N] = A[M,K] * W[N,K]^T
- * (+bias, ReLU, BN affine as flagged) through the same tcgen05/TMA kernel the model uses.
+ * (+bias, ReLU, BN affine as flagged) through the same wgmma/TMA kernel the model uses.
  * A, W, out fp32 device; ws >= ppv_gemm_test_workspace_bytes.  block_n in {64,128,256}; block_k in {64,32}
  * (K elements per pipeline stage: SWIZZLE_128B / SWIZZLE_64B tiles).
  * ------------------------------------------------------------------------------------------- */

@@ -1,4 +1,4 @@
-"""GPU: ResNetSE forward (conv2d as tcgen05 gather-GEMMs over zero-bordered NHWC images) vs the fp64 oracle and golden
+"""GPU: ResNetSE forward (conv2d as wgmma gather-GEMMs over zero-bordered NHWC images) vs the fp64 oracle and golden
 embeddings; SURVEY.md §8 row a6.  Tolerance: cosine scores within 1e-4 of the reference path."""
 import numpy as np
 import pytest
@@ -77,7 +77,7 @@ def test_batch_independence(cuda, model):
 
 
 def test_pointwise_kernel_equals_gather_gemm(cuda, W64, monkeypatch):
-    """The K <= 64 1x1 convs run on pointwise.cu (CUDA cores, exact hi + lo inputs); PPV_POINTWISE=0 keeps them on the tcgen05 gather-GEMM.
+    """The K <= 64 1x1 convs run on pointwise.cu (CUDA cores, exact hi + lo inputs); PPV_POINTWISE=0 keeps them on the wgmma gather-GEMM.
     Both must agree to the split-bf16 product rounding (~2^-17 per product), far inside the embedding tolerance."""
     gi = torch.Generator().manual_seed(77)
     f = torch.randn(3, 149, 80, generator=gi).to(cuda)

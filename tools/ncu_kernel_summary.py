@@ -1,4 +1,4 @@
-"""Selected `ncu --set full` metrics of the kernels of a report, one block per launch -- the evidence format of profiles/*_ncu_r2.txt.
+"""Selected `ncu --set full` metrics of the kernels of a report, one block per launch.
 Usage: python tools/ncu_kernel_summary.py report.ncu-rep [name-regex]"""
 import csv
 import io

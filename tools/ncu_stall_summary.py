@@ -3,7 +3,7 @@
     python tools/ncu_stall_summary.py gpurun_out/gemm_pair_r2.ncu-rep [launch_index] [top_n]
 
 Prints the stall-reason totals and the most sampled SASS instructions (address suffix, samples, executions, top stall reason).
-Used to find what the epilogue / producer / MMA warps of the tcgen05 kernels wait on (profiles/gemm_pair_stalls_r2.txt)."""
+Used to find what the producer / MMA / epilogue warps of the tensor-core kernels wait on."""
 import csv
 import io
 import subprocess

@@ -1,6 +1,6 @@
-"""Per-kernel SASS instruction counts that prove the Blackwell paths (profiles/sass_r2.txt): UTCHMMA (tcgen05.mma), UTMALDG /
-UTMASTG / UTMAPF (TMA load / store / prefetch), UBLKCP (cp.async.bulk 1-D), LDTM (tcgen05.ld), UTCBAR (tcgen05.commit), SYNCS (mbarrier),
-plus the classic pipes for contrast (HMMA / FFMA / SHFL).  Usage: python tools/sass_counts.py [lib.so] > profiles/sass_r2.txt"""
+"""Per-kernel SASS instruction counts that show the Hopper paths: HGMMA (wgmma.mma_async), WARPSYNC / WARPGROUP (warpgroup
+fences), UTMALDG / UTMASTG / UTMAPF (TMA load / store / prefetch), UBLKCP (cp.async.bulk 1-D), SYNCS (mbarrier), plus the classic
+pipes for contrast (HMMA / FFMA / SHFL).  Usage: python tools/sass_counts.py [lib.so] > sass_counts.txt"""
 import collections
 import os
 import re
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "voiceprintrecognition-paddlepaddle_b200", "lib", "libppv_b200.so")
-OPS = ["UTCHMMA", "UTCQMMA", "UTMALDG", "UTMASTG", "UTMAPF", "UBLKCP", "LDTM", "UTCBAR", "UTCATOMSWS", "SYNCS", "HMMA", "FFMA", "SHFL", "LDS", "STS"]
+OPS = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "UBLKCP", "SYNCS", "HMMA", "FFMA", "SHFL", "LDS", "STS"]
 
 
 def main():
@@ -38,8 +38,8 @@ def main():
         demangle = dict(zip(names, dm))
     except Exception:
         pass
-    print(f"# {os.path.relpath(LIB, ROOT)}: SASS instruction counts per kernel (cuobjdump -sass, sm_100a).  Columns: " + " ".join(OPS) + " | total")
-    for n in sorted(names, key=lambda k: -counts[k]["UTCHMMA"] * 100000 - counts[k]["_total"]):
+    print(f"# {os.path.relpath(LIB, ROOT)}: SASS instruction counts per kernel (cuobjdump -sass, sm_90a).  Columns: " + " ".join(OPS) + " | total")
+    for n in sorted(names, key=lambda k: -counts[k]["HGMMA"] * 100000 - counts[k]["_total"]):
         c = counts[n]
         short = re.sub(r"\(.*", "", demangle.get(n, n).replace("(int)", "").replace("(bool)", "")).replace("void ", "").replace("ppv::", "")
         print(f"{short:60s} " + " ".join(f"{c[o]:5d}" for o in OPS) + f" | {c['_total']:6d}")

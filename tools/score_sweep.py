@@ -7,7 +7,7 @@ What runs (matches the reference's eval loop, ppvector/trainer.py:416-423: a ful
   1. every rank embeds ITS shard of the M trial and N enrolment utterances (synthetic 3 s audio -> Fbank -> ResNetSE);
   2. ONE collective: all_gather of the enrolment embedding shards ([N/n, 192] fp32 per rank -- 768 kB total for N = 1000) so that
      every rank holds the replicated enrolment matrix; trial rows stay sharded;
-  3. timed scoring step: each rank's [M/n, N] slice by ppv_cosine_matrix (row-normalise + tcgen05 GEMM).  `pairs_per_s` counts the
+  3. timed scoring step: each rank's [M/n, N] slice by ppv_cosine_matrix (row-normalise + wgmma GEMM).  `pairs_per_s` counts the
      whole job (M*N pairs / max-over-ranks device time).  Assembling the full [M, N] matrix on every rank (what
      ppvector.parallel.sharded_score_rows returns) is a second all_gather of [M/n, N] fp32 slices (4 MB total) and is timed
      separately as `with_gather`;

@@ -4,18 +4,19 @@
 // mean = sum(a x); std = sqrt(clip(sum(a (x - mean)^2), eps))) and ppvector/models/ecapa_tdnn.py:271 (asp_bn).
 //
 // The GEMM is TRANSPOSED relative to the other layers: D[channel, frame] = W2[channel, :] . att[frame, :], i.e.
-// A = conv weight slab (128 channels x K=128, K-major), B = attention-TDNN activations (128 frames x K, K-major:
-// the activation matrix is already laid out that way).  A TMEM lane is then a CHANNEL and its columns are FRAMES, so
-// each epilogue thread owns one channel and walks the frames of the utterance sequentially: the softmax over time and
-// the weighted moments are per-thread running sums -- no cross-thread reduction, no atomics, deterministic.
-//   * online softmax (running max, rescale once per 32-frame chunk)
+// A = conv weight slab (128 channels x K=128, K-major), B = attention-TDNN activations (64 frames x K, K-major:
+// the activation matrix is already laid out that way).  Accumulator rows are then CHANNELS and columns FRAMES: each of the
+// two MMA warpgroups owns 64 channels of the slab, and a thread holds two channels x 16 frames of every 64-frame tile
+// (wgmma fragment, ptx.cuh).  The softmax over time and the weighted moments are per-thread running sums over the thread's
+// frames, merged across the four threads that share a channel at the end of the utterance -- no atomics, deterministic.
+//   * online softmax (running max, rescale once per tile)
 //   * moments about the channel's global mean g (from asp_global): S0 = sum e, S1 = sum e (x-g), S2 = sum e (x-g)^2,
 //     mean = g + S1/S0, var = S2/S0 - (S1/S0)^2   (shifted one-pass; the reference is two-pass)
 //   * the conv bias is constant over time and cancels in the softmax: it is not even loaded.
 // Work item = (utterance b, 128-channel slab); a CTA keeps the weight slab in smem for the item and streams the
 // utterance in 64-frame tiles through a 2-deep TMA ring.  A ring stage carries BOTH the attention activations (the
-// MMA's B operand) and the matching [64 frames x 128 channels] tile of x (un-swizzled, read by the epilogue with
-// plain ld.shared), so the epilogue never waits on global memory; the accumulator is double-buffered in TMEM.
+// MMA's B operand) and the matching [64 frames x 128 channels] tile of x (un-swizzled, read with plain ld.shared), so the
+// epilogue never waits on global memory.
 #include <stdio.h>
 #include <string.h>
 
@@ -44,14 +45,10 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
     const uint32_t a_base = smem_base;
     const uint32_t s_base = smem_base + a_bytes;
     const uint32_t bar_base = s_base + AF_STAGES * stage_bytes;
-    // barriers: a_full, a_empty, b_full[2], b_empty[2], tfull[2], tempty[2], tmem slot
+    // barriers: a_full, a_empty, b_full[2], b_empty[2]
     const uint32_t a_full = bar_base, a_empty = bar_base + 8;
     auto b_full = [&](int s) { return bar_base + 16u + 8u * s; };
     auto b_empty = [&](int s) { return bar_base + 32u + 8u * s; };
-    auto tfull = [&](int a) { return bar_base + 48u + 8u * a; };
-    auto tempty = [&](int a) { return bar_base + 64u + 8u * a; };
-    const uint32_t tmem_slot = bar_base + 80u;
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
@@ -61,25 +58,14 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
     }
     if (warp == 1 && lane == 0) {
         mbar_init(a_full, 1);
-        mbar_init(a_empty, 1);
+        mbar_init(a_empty, 256);  // every MMA thread, after the last MMA of the slab
         for (int s = 0; s < AF_STAGES; ++s) {
             mbar_init(b_full(s), 1);
-            mbar_init(b_empty(s), 1 + 256);  // MMA commit + the 256 epilogue threads that read the x tile
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull(a), 1);
-            mbar_init(tempty(a), 256);
+            mbar_init(b_empty(s), 256);  // every MMA thread, after its MMAs retired and it has read the x tile
         }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, 128);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
     griddep_launch_dependents();  // PDL
     griddep_wait();
 
@@ -133,14 +119,18 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = make_idesc_bf16(128, AF_NT);
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_phase = 0, a_phase = 0;
+    } else if (warp >= 4) {
+        // ===================== MMA + softmax / moments: warpgroup g owns channels [64 g, 64 g + 64) of the slab =====================
+        const int g = (warp - 4) >> 2, t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+        const int cl0 = 64 * g + 16 * w + (l >> 2);  // this thread's channels within the slab: cl0 and cl0 + 8
+        float acc[AF_NT / 2];
+#pragma unroll
+        for (int i = 0; i < AF_NT / 2; ++i) acc[i] = 0.f;
+        int stage = 0;
+        uint32_t phase = 0, a_phase = 0;
         int cur_slab = -1;
         for (int item = blockIdx.x; item < items; item += gridDim.x) {
-            const int slab = item % slabs;
+            const int b = item / slabs, slab = item - b * slabs;
             if (slab != cur_slab) {
                 mbar_wait(a_full, a_phase);
                 a_phase ^= 1u;
@@ -148,155 +138,119 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
             }
             const int nitem = item + gridDim.x;
             const bool last_of_slab = (nitem >= items) || (nitem % slabs != slab);
-            for (int ft = 0; ft < ntiles; ++ft) {
-                mbar_wait(tempty(acc), acc_phase ^ 1u);
-                mbar_wait(b_full(stage), phase);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t d_tmem = tmem_base + acc * AF_NT;
-                    const uint32_t sb = s_base + stage * stage_bytes;
-                    uint32_t accumulate = 0;
-                    for (int ks = 0; ks < ksteps; ++ks) {
-                        const uint64_t a_hi = make_sw128_kmajor_desc(a_base + (ks * NP) * AF_A_TILE);
-                        const uint64_t b_hi = make_sw128_kmajor_desc(sb + (ks * NP) * AF_B_TILE);
+            float gm[2], m[2], S0[2], S1[2], S2[2];
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            umma_bf16(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc, accumulate);
-                            accumulate = 1;
-                        }
-                        if (NSPLIT == 3) {
-                            const uint64_t a_lo = make_sw128_kmajor_desc(a_base + (ks * NP + 1) * AF_A_TILE);
-                            const uint64_t b_lo = make_sw128_kmajor_desc(sb + (ks * NP + 1) * AF_B_TILE);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-                        }
-                    }
-                    umma_commit(b_empty(stage));  // one of the 129 arrivals: the att tiles are consumed
-                    umma_commit(tfull(acc));
-                    if (ft == ntiles - 1 && last_of_slab) umma_commit(a_empty);  // weight slab free once its last item's MMAs retire
-                }
-                __syncwarp();
-                if (++stage == AF_STAGES) {
-                    stage = 0;
-                    phase ^= 1u;
-                }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1u;
+            for (int rr = 0; rr < 2; ++rr) {
+                const int64_t goff = int64_t(b) * p.gstat.ld + slab * 128 + cl0 + 8 * rr;
+                gm[rr] = __bfloat162float(p.gstat.hi()[goff]) + __bfloat162float(p.gstat.lo()[goff]);
+                m[rr] = -INFINITY;
+                S0[rr] = S1[rr] = S2[rr] = 0.f;
             }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue: one thread = one channel =====================
-        // 8 warps: warps 4-7 take the first 32 frames of every 64-frame tile, warps 8-11 the second 32; the two
-        // partial (max, S0, S1, S2) of a channel are merged through shared memory at the end of the item.
-        const int q = warp & 3;
-        const int half = (warp - 4) >> 2;
-        const int cl = q * 32 + lane;  // channel within the slab == TMEM lane
-        float4* s_merge = reinterpret_cast<float4*>(smem_gen + (bar_base - smem_base) + 96);  // [128]
-        int acc = 0, stage = 0;
-        uint32_t acc_phase = 0, phase = 0;
-        for (int item = blockIdx.x; item < items; item += gridDim.x) {
-            const int b = item / slabs, slab = item - b * slabs;
-            const int c = slab * 128 + cl;
-            const int64_t goff = int64_t(b) * p.gstat.ld + c;
-            const float g = __bfloat162float(p.gstat.hi()[goff]) + __bfloat162float(p.gstat.lo()[goff]);
-            float m = -INFINITY, S0 = 0.f, S1 = 0.f, S2 = 0.f;
             const int Tb = p.nvalid ? max(1, min(p.T, p.nvalid[b])) : p.T;  // masked frames: softmax weight exactly 0
             for (int ft = 0; ft < ntiles; ++ft) {
-                mbar_wait(b_full(stage), phase);  // acquire the TMA-written x tile directly (already complete by now)
-                mbar_wait(tfull(acc), acc_phase);
-                tc_fence_after();
-                const uint32_t t_addr = tmem_base + (uint32_t(q * 32) << 16) + acc * AF_NT;
-                const __nv_bfloat16* xs_hi = reinterpret_cast<const __nv_bfloat16*>(smem_gen + (s_base - smem_base) + stage * stage_bytes + b_bytes);
-                const __nv_bfloat16* xs_lo = xs_hi + AF_X_TILE / 2;
-                {
-                    const int ch = half;
-                    const int t0 = ft * AF_NT + ch * 32;
-                    uint32_t v[32];
-                    __syncwarp();
-                    tmem_ld32(t_addr + ch * 32, v);
-                    tmem_ld_wait();
-                    const int nvalid = min(32, Tb - t0);  // warp-uniform
-                    if (nvalid > 0) {
-                        // chunk max as a 4-way tree (the serial fmax chain is latency-bound with 2 warps per scheduler)
-                        float cm4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+                mbar_wait(b_full(stage), phase);
+                const uint32_t sb = s_base + stage * stage_bytes;
+                wgmma_fence_acc(acc);
+                wgmma_fence();
+                for (int ks = 0; ks < ksteps; ++ks) {
+                    const uint64_t a_hi = make_sw128_kmajor_desc(a_base + (ks * NP) * AF_A_TILE + g * 64 * 128);
+                    const uint64_t b_hi = make_sw128_kmajor_desc(sb + (ks * NP) * AF_B_TILE);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < nvalid) cm4[j & 3] = fmaxf(cm4[j & 3], __uint_as_float(v[j]));
-                        const float cm = fmaxf(fmaxf(cm4[0], cm4[1]), fmaxf(cm4[2], cm4[3]));
-                        if (cm > m) {
-                            const float r = exp2f((m - cm) * LOG2E);  // exp(-inf) = 0 on the first chunk
-                            S0 *= r;
-                            S1 *= r;
-                            S2 *= r;
-                            m = cm;
-                        }
-                        // four independent accumulator sets (ILP), exp as one FFMA + ex2.approx
-                        const float ms = m * LOG2E;
-                        float a0[4] = {0.f, 0.f, 0.f, 0.f}, a1[4] = {0.f, 0.f, 0.f, 0.f}, a2[4] = {0.f, 0.f, 0.f, 0.f};
+                    for (int k = 0; k < 4; ++k) wgmma_bf16<AF_NT>(acc, a_hi + 2 * k, b_hi + 2 * k, (ks > 0 || k > 0) ? 1u : 0u);
+                    if (NSPLIT == 3) {
+                        const uint64_t a_lo = make_sw128_kmajor_desc(a_base + (ks * NP + 1) * AF_A_TILE + g * 64 * 128);
+                        const uint64_t b_lo = make_sw128_kmajor_desc(sb + (ks * NP + 1) * AF_B_TILE);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            if (j < nvalid) {
-                                const int o = (ch * 32 + j) * 128 + cl;
-                                const float xv = __bfloat162float(xs_hi[o]) + __bfloat162float(xs_lo[o]);
-                                const float e = exp2f(fmaf(__uint_as_float(v[j]), LOG2E, -ms));
-                                const float d = xv - g;
-                                const float ed = e * d;
-                                a0[j & 3] += e;
-                                a1[j & 3] += ed;
-                                a2[j & 3] = fmaf(ed, d, a2[j & 3]);
-                            }
-                        }
-                        S0 += (a0[0] + a0[1]) + (a0[2] + a0[3]);
-                        S1 += (a1[0] + a1[1]) + (a1[2] + a1[3]);
-                        S2 += (a2[0] + a2[1]) + (a2[2] + a2[3]);
+                        for (int k = 0; k < 4; ++k) wgmma_bf16<AF_NT>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) wgmma_bf16<AF_NT>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
                     }
                 }
-                tc_fence_before();
-                mbar_arrive(tempty(acc));
-                mbar_arrive(b_empty(stage));  // done reading the x tile of this stage
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1u;
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
+                if (ft == ntiles - 1 && last_of_slab) mbar_arrive(a_empty);  // weight slab free once its last item's MMAs retired
+                const __nv_bfloat16* xs_hi = reinterpret_cast<const __nv_bfloat16*>(smem_gen + (sb - smem_base) + b_bytes);
+                const __nv_bfloat16* xs_lo = xs_hi + AF_X_TILE / 2;
+                const int f0 = ft * AF_NT;
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    float cm = -INFINITY;
+#pragma unroll
+                    for (int i = 0; i < AF_NT / 8; ++i)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e)
+                            if (f0 + 8 * i + 2 * (l & 3) + e < Tb) cm = fmaxf(cm, acc[4 * i + 2 * rr + e]);
+                    if (cm > m[rr]) {
+                        const float r = exp2f((m[rr] - cm) * LOG2E);  // exp(-inf) = 0 on the first frames
+                        S0[rr] *= r;
+                        S1[rr] *= r;
+                        S2[rr] *= r;
+                        m[rr] = cm;
+                    }
+                    const float ms = m[rr] * LOG2E;
+                    const int cl = cl0 + 8 * rr;
+#pragma unroll
+                    for (int i = 0; i < AF_NT / 8; ++i)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int fl = 8 * i + 2 * (l & 3) + e;
+                            if (f0 + fl < Tb) {
+                                const int o = fl * 128 + cl;
+                                const float xv = __bfloat162float(xs_hi[o]) + __bfloat162float(xs_lo[o]);
+                                const float ev = exp2f(fmaf(acc[4 * i + 2 * rr + e], LOG2E, -ms));
+                                const float d = xv - gm[rr];
+                                const float ed = ev * d;
+                                S0[rr] += ev;
+                                S1[rr] += ed;
+                                S2[rr] = fmaf(ed, d, S2[rr]);
+                            }
+                        }
+                }
+                mbar_arrive(b_empty(stage));  // done with the att and x tiles of this stage
                 if (++stage == AF_STAGES) {
                     stage = 0;
                     phase ^= 1u;
                 }
             }
-            // merge the two halves of the channel
-            if (half == 1) s_merge[cl] = make_float4(m, S0, S1, S2);
-            named_bar_sync(2, 256);
-            if (half == 0) {
-                const float4 o = s_merge[cl];
-                const float mm = fmaxf(m, o.x);
-                const float ra = exp2f((m - mm) * LOG2E), rb = (o.y > 0.f) ? exp2f((o.x - mm) * LOG2E) : 0.f;
-                S0 = S0 * ra + o.y * rb;
-                S1 = S1 * ra + o.z * rb;
-                S2 = S2 * ra + o.w * rb;
+            // merge the four threads of a channel (lanes 4 k .. 4 k + 3 hold the same two channels)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+#pragma unroll
+                for (int off = 1; off <= 2; off <<= 1) {
+                    const float om = __shfl_xor_sync(0xffffffffu, m[rr], off), o0 = __shfl_xor_sync(0xffffffffu, S0[rr], off),
+                                o1 = __shfl_xor_sync(0xffffffffu, S1[rr], off), o2 = __shfl_xor_sync(0xffffffffu, S2[rr], off);
+                    const float mm = fmaxf(m[rr], om);
+                    const float ra = S0[rr] > 0.f ? exp2f((m[rr] - mm) * LOG2E) : 0.f, rb = o0 > 0.f ? exp2f((om - mm) * LOG2E) : 0.f;
+                    S0[rr] = S0[rr] * ra + o0 * rb;
+                    S1[rr] = S1[rr] * ra + o1 * rb;
+                    S2[rr] = S2[rr] * ra + o2 * rb;
+                    m[rr] = mm;
+                }
             }
-            named_bar_sync(2, 256);  // s_merge may be overwritten by the next item
-            if (half == 1) continue;
-            const float inv = 1.f / S0;
-            const float dm = S1 * inv;
-            const float mean = g + dm;
-            const float sd = sqrtf(fmaxf(S2 * inv - dm * dm, p.eps));
+            if ((l & 3) != 0) continue;
             const int C = p.C;
-            if (p.out_raw) {
-                p.out_raw[int64_t(b) * 2 * C + c] = mean;
-                p.out_raw[int64_t(b) * 2 * C + C + c] = sd;
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int c = slab * 128 + cl0 + 8 * rr;
+                const float inv = 1.f / S0[rr];
+                const float dm = S1[rr] * inv;
+                const float mean = gm[rr] + dm;
+                const float sd = sqrtf(fmaxf(S2[rr] * inv - dm * dm, p.eps));
+                if (p.out_raw) {
+                    p.out_raw[int64_t(b) * 2 * C + c] = mean;
+                    p.out_raw[int64_t(b) * 2 * C + C + c] = sd;
+                }
+                __nv_bfloat16 h, lo;
+                split_bf16(fmaf(mean, p.bn_scale[c], p.bn_shift[c]), h, lo);
+                p.out.hi()[int64_t(b) * p.out.ld + c] = h;
+                p.out.lo()[int64_t(b) * p.out.ld + c] = lo;
+                split_bf16(fmaf(sd, p.bn_scale[C + c], p.bn_shift[C + c]), h, lo);
+                p.out.hi()[int64_t(b) * p.out.ld + C + c] = h;
+                p.out.lo()[int64_t(b) * p.out.ld + C + c] = lo;
             }
-            __nv_bfloat16 h, l;
-            split_bf16(fmaf(mean, p.bn_scale[c], p.bn_shift[c]), h, l);
-            p.out.hi()[int64_t(b) * p.out.ld + c] = h;
-            p.out.lo()[int64_t(b) * p.out.ld + c] = l;
-            split_bf16(fmaf(sd, p.bn_scale[C + c], p.bn_shift[C + c]), h, l);
-            p.out.hi()[int64_t(b) * p.out.ld + C + c] = h;
-            p.out.lo()[int64_t(b) * p.out.ld + C + c] = l;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 128);
 }
 
 int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const Planes& x, const Planes& gstat, const float* bn_scale,

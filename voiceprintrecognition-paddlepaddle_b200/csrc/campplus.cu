@@ -205,7 +205,7 @@ struct CamppModel {
     WeightMap raw;
     bool finalized = false;
     int precision = PPV_PREC_BF16X3;
-    int num_sms = 148;
+    int num_sms = 132;
     void* arena = nullptr;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<ResBlockW> res;

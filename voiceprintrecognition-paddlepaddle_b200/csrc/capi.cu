@@ -20,7 +20,7 @@ int device_sm_count() {
     int dev = 0, n = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
         cudaGetLastError();
-        return 148;
+        return 132;  // H100 SXM
     }
     return n;
 }
@@ -31,7 +31,7 @@ static int check_device() {
     int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-    if (major != 10) return fail(PPV_EUNSUPPORTED, "libppv_b200 is built for sm_100a only (found sm_" + std::to_string(major * 10 + minor) + ")");
+    if (major != 9 || minor != 0) return fail(PPV_EUNSUPPORTED, "libppv_b200 is built for sm_90a only (found sm_" + std::to_string(major * 10 + minor) + ")");
     return PPV_OK;
 }
 

@@ -138,23 +138,19 @@ struct Epilogue {
     // (context-aware mask of CAM++, campplus.py:88-93); applied after the biases, before the activations
     const float* seg_scale = nullptr;
     int seg_len = 0, nseg = 0;
-    int zero_invalid = 0;  // TMA-store path: rows outside the valid frames are stored as zeros (zero-padded convs read them)
-    int f32_vec_ok = 0;  // set by gemm_build: OUT_F32 rows are 16-byte (1) / 32-byte (2) aligned
-    int tma_store = 0;   // set by gemm_build: planes output without halo goes through a shared-memory staging tile + TMA store
+    int zero_invalid = 0;  // planes output without halo on the input grid: rows outside the valid frames are stored as zeros (zero-padded convs read them)
+    int f32_vec_ok = 0;  // set by gemm_build: OUT_F32 rows and columns are 8-byte aligned (paired stores)
     int debug_nostore = 0;  // PPV_GEMM_NOSTORE=1 (tools/gemm_bench.py only): skip the epilogue stores
 };
 
 struct GemmParams {
     CUtensorMap mapA[GEMM_MAX_MAPS];
     CUtensorMap mapB;
-    CUtensorMap mapOut;  // output planes, box {64, 128, 1}, SWIZZLE_128B (TMA-store epilogue)
-    CUtensorMap mapBh;   // weight planes, box {BK, BN / 2, 1}: the half tile a CTA of a cta_group::2 pair loads (pair mode)
     KStep ksteps[GEMM_MAX_KSTEPS];
     int num_ksteps;
     int bk;  // K elements per k-step (64 or 32)
     int l2_prefetch;  // producer prefetches the next tile's activation rows into L2
     int ws;           // weight-stationary mode (set by gemm_build): W resident in shared memory, the ring carries activations only
-    int pair;         // pair mode (set by gemm_build): cta_group::2 MMAs, the two CTAs of a cluster own the two 128-row halves of a 256 x BN tile
     int lin_splits;   // > 0: weight-gradient mode (see gemm_build_wgrad): K runs over operand columns, split in lin_splits parts
     int lin_b_row0, lin_b_col0;
     int64_t lin_split_rows;

@@ -1,21 +1,17 @@
 // 3x3 conv (padding 1) with 32 input and 32 output channels over zero-bordered NHWC image grids: the stride-1 stages of
 // ResNetSE (ppvector/models/resnet_se.py:24-45, conv2 of layer1), CAM++'s FCM head (ppvector/models/campplus.py:211-281) and
-// ERes2Net's 32-wide Res2Net convs (ppvector/models/eres2net.py:85-108).  Same contraction as the gather-GEMM of gemm_tcgen05.cu
+// ERes2Net's 32-wide Res2Net convs (ppvector/models/eres2net.py:85-108).  Same contraction as the gather-GEMM of gemm_wgmma.cu
 // (M = grid positions, N = 32, K = 9 taps x 32), restructured around what bounds it.  The generic kernel loads every
 // activation row nine times from L2 (one TMA tile per tap) for an N = 32 tile: it is L2 -> shared-memory bound.  Here
 //   * the whole weight matrix (9 taps x hi/lo x 2 KB = 36 KB) is loaded once per CTA and stays in shared memory;
 //   * ONE image patch of 8 x 64 grid positions (6 x 62 outputs + a one-position halo) is loaded per work item by a single 5-D
 //     TMA box per plane ({32 ch, 64 w, 8 h}: out-of-range coordinates are zero-filled, and the zero border of the grid is the
 //     conv's padding), landing as 512 consecutive 64-byte rows in the SWIZZLE_64B layout;
-//   * the nine taps are the SAME shared-memory patch read at row offsets dh * 64 + dw: the UMMA descriptor start address
+//   * the nine taps are the SAME shared-memory patch read at row offsets dh * 64 + dw: the wgmma descriptor start address
 //     moves by whole 64-byte rows (the swizzle XOR is a function of the absolute shared-memory address, as in res2conv.cu);
-//   * three M = 128 accumulator tiles cover the 384 patch rows that hold outputs; the epilogue maps a patch row back to its
-//     grid position (halo columns are computed and dropped);
-//   * an M128 x N32 x K16 MMA keeps the tensor pipe busy for ~80 cycles (measured: it is bound by the 4 KB A-operand read, not by its
-//     65 k MACs), and so does N = 64.  The split-bf16 product A_hi W_hi + A_hi W_lo + A_lo W_hi therefore runs as TWO instructions per
-//     k-step instead of three: A_hi x [W_hi | W_lo] with N = 64 (the hi and lo weight tiles of a tap are adjacent in shared memory:
-//     one 64-row B operand) into accumulator columns [0,64), and A_lo x W_hi with N = 32 into columns [0,32); the epilogue adds the
-//     two column blocks.
+//   * three M = 128 accumulator tiles cover the 384 patch rows that hold outputs; the two MMA warpgroups take them in turn
+//     (two m64 x n32 accumulators each), and the epilogue maps a patch row back to its grid position (halo columns are
+//     computed and dropped).
 // L2 -> SM traffic per output position: 512 / 372 = 1.4 rows instead of 9.
 #include <stdio.h>
 #include <stdlib.h>
@@ -38,7 +34,6 @@ constexpr int C3_PLANE_BYTES = C3_ROWS * 64;             // 32 KB per plane
 constexpr int C3_W_TILE = 32 * 64;                       // [32 out ch x 32 k] bf16 per tap per plane
 constexpr int C3_STAGES = 2;
 constexpr int C3_BN = 32;
-constexpr int C3_ACC_COLS = 64;                          // accumulator columns per tile: [hi-part | lo-part]
 static_assert((C3_OH * C3_PW) % GEMM_BM == 0, "patch rows with outputs must be whole accumulator tiles");
 
 template <int NSPLIT>
@@ -50,15 +45,6 @@ struct C3Cfg {
     static constexpr int SMEM_BYTES = 1024 + ((W_BYTES + 1023) & ~1023) + C3_STAGES * STAGE_BYTES + 1024 + 256;
 };
 
-__device__ __forceinline__ uint64_t sw64_desc(uint32_t smem_addr) {  // K-major, rows of 32 bf16, 8-row groups 512 B apart
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3fff);
-    d |= static_cast<uint64_t>(1) << 16;
-    d |= static_cast<uint64_t>(512 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(4) << 61;  // SWIZZLE_64B
-    return d;
-}
 __device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
     asm volatile(
         "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
@@ -74,17 +60,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv3x3_c32_kernel(const __gr
     constexpr int NP = Cfg::NP;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t w_base = smem_base;
     const uint32_t a_base = smem_base + ((Cfg::W_BYTES + 1023) & ~1023);
     const uint32_t bar_base = a_base + C3_STAGES * Cfg::STAGE_BYTES + 1024;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C3_STAGES + s); };
-    auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C3_STAGES + a); };
-    auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C3_STAGES + 2 + a); };
-    const uint32_t w_full = bar_base + 8u * (2 * C3_STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C3_STAGES + 5);
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
+    const uint32_t w_full = bar_base + 8u * (2 * C3_STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
@@ -94,23 +75,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv3x3_c32_kernel(const __gr
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < C3_STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull_bar(a), 1);
-            mbar_init(tempty_bar(a), EPI_WARP_ARRIVALS / 2);  // one epilogue warp group (4 warps) per accumulator, one arrival per warp
+            mbar_init(empty_bar(s), GEMM_MMA_THREADS / 128);  // one arrival per MMA warpgroup
         }
         mbar_init(w_full, 1);
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, 2 * C3_ACC_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
     griddep_launch_dependents();  // PDL
 
     const int per_img = cp.nph * cp.npw;
@@ -141,81 +111,68 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv3x3_c32_kernel(const __gr
                 phase ^= 1u;
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc32 = make_idesc_bf16(GEMM_BM, C3_BN), idesc64 = make_idesc_bf16(GEMM_BM, 2 * C3_BN);
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup g takes every other 128-row accumulator tile =====================
+        const int g = (warp - 4) >> 2, t = threadIdx.x & 127;
+        griddep_wait();  // the epilogue writes buffers that upstream kernels may still be reading
         mbar_wait(w_full, 0);
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_phase[2] = {0, 0};
+        int stage = 0;
+        uint32_t phase = 0;
+        int tcount = 0;  // running accumulator-tile counter of this CTA: tile n goes to warpgroup n & 1
+        float acc0[C3_BN / 2], acc1[C3_BN / 2];
+#pragma unroll
+        for (int i = 0; i < C3_BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
         for (int item = blockIdx.x; item < cp.patches; item += gridDim.x) {
+            const int b = item / per_img, r = item - b * per_img;
+            const int ih = r / cp.npw, iw = r - ih * cp.npw;
             mbar_wait(full_bar(stage), phase);
-            tc_fence_after();
             const uint32_t slot = a_base + stage * Cfg::STAGE_BYTES;
-            for (int t = 0; t < C3_TILES; ++t) {
-                mbar_wait(tempty_bar(acc), acc_phase[acc] ^ 1u);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t d_tmem = tmem_base + acc * C3_ACC_COLS;
-                    uint32_t accumulate = 0;
+            for (int tt = 0; tt < C3_TILES; ++tt, ++tcount) {
+                if ((tcount & 1) != g) continue;
+                wgmma_fence_acc(acc0);
+                wgmma_fence_acc(acc1);
+                wgmma_fence();
+                auto issue = [&](float (&acc)[C3_BN / 2], int mb) {
 #pragma unroll
                     for (int tap = 0; tap < 9; ++tap) {
-                        const int roff = C3_ROW0 + t * GEMM_BM + (tap / 3 - 1) * C3_PW + (tap % 3 - 1);
-                        const uint64_t a_hi = sw64_desc(slot + uint32_t(roff) * 64u);
-                        const uint64_t b_hi = sw64_desc(w_base + (tap * NP) * C3_W_TILE);  // NSPLIT 3: rows 0-31 = W_hi, rows 32-63 = W_lo
+                        const int roff = C3_ROW0 + tt * GEMM_BM + mb * 64 + (tap / 3 - 1) * C3_PW + (tap % 3 - 1);
+                        const uint64_t a_hi = make_sw64_kmajor_desc(slot + uint32_t(roff) * 64u);
+                        const uint64_t b_hi = make_sw64_kmajor_desc(w_base + (tap * NP) * C3_W_TILE);
+#pragma unroll
+                        for (int k = 0; k < 2; ++k) wgmma_bf16<C3_BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (tap > 0 || k > 0) ? 1u : 0u);
                         if (NSPLIT == 3) {
-                            const uint64_t a_lo = sw64_desc(slot + C3_PLANE_BYTES + uint32_t(roff) * 64u);
+                            const uint64_t a_lo = make_sw64_kmajor_desc(slot + C3_PLANE_BYTES + uint32_t(roff) * 64u);
+                            const uint64_t b_lo = make_sw64_kmajor_desc(w_base + (tap * NP + 1) * C3_W_TILE);
 #pragma unroll
-                            for (int k = 0; k < 2; ++k) {
-                                umma_bf16(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc64, accumulate);  // [A_hi W_hi | A_hi W_lo]
-                                accumulate = 1;
-                            }
+                            for (int k = 0; k < 2; ++k) wgmma_bf16<C3_BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-                            for (int k = 0; k < 2; ++k) umma_bf16(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc32, 1u);  // + A_lo W_hi
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < 2; ++k) {
-                                umma_bf16(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc32, accumulate);
-                                accumulate = 1;
-                            }
+                            for (int k = 0; k < 2; ++k) wgmma_bf16<C3_BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
                         }
                     }
-                    umma_commit(tfull_bar(acc));
-                    if (t == C3_TILES - 1) umma_commit(empty_bar(stage));
-                }
-                __syncwarp();
-                acc_phase[acc] ^= 1u;
-                acc ^= 1;
+                };
+                issue(acc0, 0);
+                issue(acc1, 1);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc0);
+                wgmma_fence_acc(acc1);
+                auto row_of = [&](int mb, int rr) -> int64_t {
+                    const int prow = C3_ROW0 + tt * GEMM_BM + mb * 64 + rr;  // patch row of this accumulator row
+                    const int ph = prow / C3_PW, pw = prow - ph * C3_PW;
+                    const int hp = ih * C3_OH + ph, wp = iw * C3_OW + pw;  // padded grid coordinates
+                    if (pw >= 1 && pw <= C3_OW && ph <= C3_OH && hp <= cp.H && wp <= cp.W) return (int64_t(b) * cp.Hp + hp) * cp.Wp + wp;
+                    return -1;
+                };
+                epilogue_frag<C3_BN>(cp.epi, C3_BN, 0, acc0, [&](int rr) { return row_of(0, rr); }, t);
+                epilogue_frag<C3_BN>(cp.epi, C3_BN, 0, acc1, [&](int rr) { return row_of(1, rr); }, t);
             }
+            if (t == 0) mbar_arrive(empty_bar(stage));  // this warpgroup is done with the patch
             if (++stage == C3_STAGES) {
                 stage = 0;
                 phase ^= 1u;
             }
         }
-    } else if (warp >= 4) {
-        // ===================== epilogue: warps 4-7 take accumulator 0, warps 8-11 accumulator 1 =====================
-        const int q = warp & 3, grp = (warp - 4) >> 2;
-        griddep_wait();  // the epilogue writes buffers that upstream kernels may still be reading
-        uint32_t acc_phase = 0;
-        int tcount = 0;  // running accumulator-tile counter of this CTA: tile n uses accumulator n & 1
-        for (int item = blockIdx.x; item < cp.patches; item += gridDim.x) {
-            const int b = item / per_img, r = item - b * per_img;
-            const int ih = r / cp.npw, iw = r - ih * cp.npw;
-            for (int t = 0; t < C3_TILES; ++t, ++tcount) {
-                if ((tcount & 1) != grp) continue;
-                const int prow = C3_ROW0 + t * GEMM_BM + q * 32 + lane;  // patch row of this thread's accumulator lane
-                const int ph = prow / C3_PW, pw = prow - ph * C3_PW;
-                const int hp = ih * C3_OH + ph, wp = iw * C3_OW + pw;  // padded grid coordinates
-                int64_t row = -1;
-                if (pw >= 1 && pw <= C3_OW && ph <= C3_OH && hp <= cp.H && wp <= cp.W) row = (int64_t(b) * cp.Hp + hp) * cp.Wp + wp;
-                epilogue_tile<C3_BN>(cp.epi, nullptr, 0, C3_BN, 0, 0, tmem_base + grp * C3_ACC_COLS, tfull_bar(grp), acc_phase, tempty_bar(grp), q, lane,
-                                     0, threadIdx.x - 128, 0u, nullptr, 0, row, NSPLIT == 3 ? C3_BN : 0);
-                acc_phase ^= 1u;
-            }
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 2 * C3_ACC_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -265,7 +222,6 @@ int conv3x3_build(Conv3x3Params* cp, const Planes& x, int x_col0, const Planes& 
     cp->npw = (W + C3_OW - 1) / C3_OW;
     cp->patches = B * cp->nph * cp->npw;
     cp->epi = epi;
-    cp->epi.tma_store = 0;
     return PPV_OK;
 }
 

@@ -2,7 +2,7 @@
 // Reference: ppvector/predict.py:279-283 (contrast: dot / (|a||b|)), predict.py:173-187 (retrieval through
 // sklearn cosine_similarity), ppvector/trainer.py:416-423 (eval: one 1-vs-all-enrol cosine row per trial in a
 // Python loop).  Two forms:
-//   all-pairs  [M,D] x [N,D] -> [M,N] : rows are L2-normalised into split-bf16 planes, then the same tcgen05
+//   all-pairs  [M,D] x [N,D] -> [M,N] : rows are L2-normalised into split-bf16 planes, then the same wgmma
 //              gather-GEMM as the model (K = D, fp32 out).  Tensor-core bound, 384 FLOP / pair.
 //   pair-list  idx[P,2] -> [P]        : 8 lanes per pair, gather both rows (1536 B / pair), HBM/L2-bound.
 #include "common.h"

@@ -68,7 +68,7 @@ struct EcapaModel {
     std::map<std::string, HostW> raw;
     bool finalized = false;
     int precision = PPV_PREC_BF16X3;
-    int num_sms = 148;
+    int num_sms = 132;
     int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0;
     // device weights
     void* arena = nullptr;
@@ -460,7 +460,7 @@ static int build_plan(EcapaModel* m, int B, int T, void* ws, size_t ws_bytes, cu
     const bool use_res2_chain = use_res2_kernel && m->scale == 8 && res2chain_fits(T, P) && !(rcenv && rcenv[0] == '0');
     const char* skenv = getenv("PPV_SKINNY");  // 0 = the per-utterance linear layers through the tensor-core gather-GEMM (A-B timing)
     const bool use_skinny = !(skenv && skenv[0] == '0');
-    const char* bkenv = getenv("PPV_GEMM_BK32");  // experiment: 1 = 32-wide k-steps (SWIZZLE_64B) on the wide-N layers; measured slower
+    const char* bkenv = getenv("PPV_GEMM_BK32");  // experiment: 1 = 32-wide k-steps (SWIZZLE_64B) on the wide-N layers
     const bool bk32_enabled = (bkenv && bkenv[0] == '1');
 
     auto add_gemm = [&](const ConvW& cw, const std::vector<KSpec>& ks, const Planes* src_override, int override_col0, int M,

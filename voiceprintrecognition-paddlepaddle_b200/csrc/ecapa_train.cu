@@ -8,7 +8,7 @@
 // out in the reference's state_dict order, so that the optimizer is one elementwise kernel (ppv_adam_step) and data-parallel
 // training is ONE all-reduce over the gradient buffer (the reference's fleet.distributed_model, trainer.py:318-320).
 //
-// Every convolution is three tensor-core GEMMs on the tcgen05 kernel of gemm_tcgen05.cu:
+// Every convolution is three tensor-core GEMMs on the wgmma kernel of gemm_wgmma.cu:
 //   forward   A = input planes (taps = row offsets),      B = Wf [Cout][taps*Cin]
 //   dgrad     A = dz planes (taps = negated row offsets),  B = Wd [Cin][taps*Cout]      -> gradient of the PADDED input
 //   wgrad     A = dz^T [Cout][rows], B = x^T [Cin][rows] (tap = column offset), split-K partials summed in a fixed order
@@ -83,7 +83,7 @@ struct Trainer {
     ppv_ecapa_cfg cfg;
     int S = 0;  // classes
     int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0, D = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     int precision = PPV_PREC_BF16X3;  // PPV_PREC_BF16: single-pass bf16 operands for every forward / data-gradient / weight-gradient GEMM (AMP mode)
     // flat layout
     std::map<std::string, std::pair<int64_t, int64_t>> pmap, smap;  // name -> (offset, numel)

@@ -407,7 +407,7 @@ __global__ void planes_to_f32_kernel(Planes x, int col0, int C, int B, int T, in
 
 int launch_planes_to_f32(const Planes& x, int col0, int C, int B, int T, int P, int Tp, float* out, cudaStream_t st) {
     const int64_t total = int64_t(B) * T * C;
-    const int grid = int(std::min<int64_t>((total + 255) / 256, 148 * 32));
+    const int grid = int(std::min<int64_t>((total + 255) / 256, 132 * 32));
     planes_to_f32_kernel<<<grid, 256, 0, st>>>(x, col0, C, B, T, P, Tp, out);
     PPV_LAUNCH_OK("planes_to_f32_kernel");
     return PPV_OK;
@@ -428,7 +428,7 @@ __global__ void f32_to_planes_kernel(const float* __restrict__ src, int64_t rows
 
 int launch_f32_to_planes(const float* src, int64_t rows, int cols, const Planes& out, cudaStream_t st) {
     const int64_t total = rows * cols;
-    const int grid = int(std::min<int64_t>((total + 255) / 256, 148 * 32));
+    const int grid = int(std::min<int64_t>((total + 255) / 256, 132 * 32));
     f32_to_planes_kernel<<<grid, 256, 0, st>>>(src, rows, cols, out);
     PPV_LAUNCH_OK("f32_to_planes_kernel");
     return PPV_OK;

@@ -60,7 +60,7 @@ struct ERes2NetModel {
     WeightMap raw;
     bool finalized = false;
     int precision = PPV_PREC_BF16X3;
-    int num_sms = 148;
+    int num_sms = 132;
     void* arena = nullptr;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<EBlockW> blocks;

@@ -1,248 +1,125 @@
-// Shared epilogue of the tcgen05 kernels (gemm_tcgen05.cu, res2conv.cu): one 128 x BN fp32 accumulator tile in TMEM ->
-// bias / per-utterance bias / ReLU / BatchNorm affine / tanh / sigmoid -> split-bf16 planes (incl. the reflect-halo rows of
-// the padded time layout) or fp32.  Runs on warps 4..11 of the CTA: two warps per TMEM lane quarter alternate over the
-// 32-column chunks.
+// Shared epilogue of the wgmma kernels (gemm_wgmma.cu, res2conv.cu, conv3x3.cu): one warpgroup's 64 x BN fp32 accumulator
+// fragment (registers, layout in ptx.cuh) -> bias / per-utterance bias / ReLU / BatchNorm affine / tanh / sigmoid -> split-bf16
+// planes (incl. the reflect-halo rows of the padded time layout) or fp32.  Each thread owns two rows and BN / 4 columns of the
+// tile, in pairs of adjacent columns; every pair is processed and stored straight from the registers.
+// Not tuned on H100: a warp's store covers 16 B of each of 8 rows (half of a 32-byte sector).  Gathering a row's 8 columns into one
+// 16-byte store per lane (a 4 x 4 exchange of column pairs inside each quad of lanes) is the obvious next step; it is not measured.
 #pragma once
 #include "common.h"
 #include "ptx.cuh"
 
 namespace ppv {
 
-constexpr int GEMM_EPI_THREADS = 256;                 // 8 epilogue warps
-constexpr int GEMM_THREADS = 128 + GEMM_EPI_THREADS;  // + TMA, MMA, TMEM-alloc, spare warps
+constexpr int GEMM_MMA_THREADS = 256;                 // two MMA warpgroups: rows 0-63 and 64-127 of a 128-row tile
+constexpr int GEMM_THREADS = 128 + GEMM_MMA_THREADS;  // + the producer warpgroup (warp 0: TMA)
 
-constexpr int EPI_STAGING_BYTES = 2 * GEMM_BM * 128;
-constexpr int EPI_WARP_ARRIVALS = GEMM_EPI_THREADS / 32;  // accumulator-empty barrier: ONE arrival per epilogue warp (lane 0, after its last TMEM read)  // [hi | lo] x 128 rows x 64 bf16 columns, SWIZZLE_128B
-
-// per-column epilogue math on 32 accumulator columns starting at global column `col`
-__device__ __forceinline__ void epilogue_math(const Epilogue& ep, int N, int col, int64_t grp, int64_t sgrp, const uint32_t (&v)[32],
-                                              float (&x)[32]) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-    if (ep.bias) {
-        const float4* b = reinterpret_cast<const float4*>(ep.bias + col);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float4 b4 = __ldg(b + j);
-            x[4 * j + 0] += b4.x;
-            x[4 * j + 1] += b4.y;
-            x[4 * j + 2] += b4.z;
-            x[4 * j + 3] += b4.w;
-        }
-    }
-    if (ep.rowgrp_bias) {
-        const float4* rg = reinterpret_cast<const float4*>(ep.rowgrp_bias + grp * N + col);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float4 b4 = __ldg(rg + j);
-            x[4 * j + 0] += b4.x;
-            x[4 * j + 1] += b4.y;
-            x[4 * j + 2] += b4.z;
-            x[4 * j + 3] += b4.w;
-        }
-    }
-    if (ep.seg_scale) {
-        const float4* sg = reinterpret_cast<const float4*>(ep.seg_scale + sgrp * N + col);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float4 s4 = __ldg(sg + j);
-            x[4 * j + 0] *= s4.x;
-            x[4 * j + 1] *= s4.y;
-            x[4 * j + 2] *= s4.z;
-            x[4 * j + 3] *= s4.w;
-        }
-    }
+// per-column epilogue math on one accumulator value of global column `col`.  The per-column vectors are re-read for each of
+// the thread's two rows (L1 hits): holding them for all BN / 4 columns costs the BN = 256 tile more spills than the loads cost.
+__device__ __forceinline__ float epilogue_math1(const Epilogue& ep, int N, int col, int64_t grp, int64_t sgrp, float x) {
+    if (ep.bias) x += __ldg(ep.bias + col);
+    if (ep.rowgrp_bias) x += __ldg(ep.rowgrp_bias + grp * N + col);
+    if (ep.seg_scale) x *= __ldg(ep.seg_scale + sgrp * N + col);
     if (ep.relu) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.f);
-        if (ep.relu_max > 0.f) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = fminf(x[j], ep.relu_max);
-        }
+        x = fmaxf(x, 0.f);
+        if (ep.relu_max > 0.f) x = fminf(x, ep.relu_max);
     }
-    if (ep.silu_) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = x[j] / (1.f + expf(-x[j]));
-    }
-    if (ep.bn_scale) {
-        const float4* sc = reinterpret_cast<const float4*>(ep.bn_scale + col);
-        const float4* sh = reinterpret_cast<const float4*>(ep.bn_shift + col);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const float4 a = __ldg(sc + j), b = __ldg(sh + j);
-            x[4 * j + 0] = fmaf(x[4 * j + 0], a.x, b.x);
-            x[4 * j + 1] = fmaf(x[4 * j + 1], a.y, b.y);
-            x[4 * j + 2] = fmaf(x[4 * j + 2], a.z, b.z);
-            x[4 * j + 3] = fmaf(x[4 * j + 3], a.w, b.w);
-        }
-    }
-    if (ep.tanh_) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = tanhf(x[j]);
-    }
-    if (ep.sigmoid_) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = 1.f / (1.f + expf(-x[j]));
-    }
+    if (ep.silu_) x = x / (1.f + expf(-x));
+    if (ep.bn_scale) x = fmaf(x, __ldg(ep.bn_scale + col), __ldg(ep.bn_shift + col));
+    if (ep.tanh_) x = tanhf(x);
+    if (ep.sigmoid_) x = 1.f / (1.f + expf(-x));
+    return x;
 }
 
-// `staging`: shared-memory address (1024-aligned) of EPI_STAGING_BYTES for the TMA-store path, 0 if unavailable.
-// `tempty_remote`: shared::cluster address of the accumulator-empty barrier when it lives in the pair leader's CTA (0: local).
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const Epilogue& ep, const CUtensorMap* map_out, int M, int N, int m0, int n0,
-                                              uint32_t tmem_acc, uint32_t tfull_bar, uint32_t acc_phase, uint32_t tempty_bar, int q,
-                                              int lane, int ehalf, int etid, uint32_t staging, uint8_t* staging_gen, int64_t out_row_shift = 0,
-                                              int64_t row_override = INT64_MIN, int sum_cols = 0, uint32_t tempty_remote = 0) {
-    // row bookkeeping
-    const int rloc = q * 32 + lane;  // row within the tile == TMEM lane
-    // row_override (conv3x3.cu): the caller maps this accumulator lane to its GEMM row itself (-1: the lane holds no output)
-    const int64_t row = row_override == INT64_MIN ? int64_t(m0) + rloc : (row_override < 0 ? 0 : row_override);
-    bool valid = row_override == INT64_MIN ? row < M : row_override >= 0;
-    int64_t mirror_a = -1, mirror_b = -1;
-    int64_t grp = 0, sgrp = 0;
-    int64_t out_row = row + out_row_shift;  // wgrad mode: partial block of this K split
+// Where one GEMM row goes: validity, destination row, reflect-halo mirror rows, per-utterance / per-segment groups.
+struct EpiRow {
+    bool valid = false;
+    int64_t out_row = 0, mirror_a = -1, mirror_b = -1, grp = 0, sgrp = 0;
+    int64_t zero_row = -1;  // an invalid row that must hold zeros (ep.zero_invalid: zero-padded convs read it)
+};
+// row < 0: this accumulator row holds no output
+__device__ __forceinline__ EpiRow epilogue_row(const Epilogue& ep, int64_t row, int64_t out_row_shift) {
+    EpiRow r;
+    r.valid = row >= 0;
+    const int64_t row_in = row;
+    if (row < 0) row = 0;
+    r.out_row = row + out_row_shift;  // wgrad mode: partial block of this K split
     if (ep.img_Wp > 0) {
         const int64_t img = int64_t(ep.img_Hp) * ep.img_Wp;
-        grp = row / img;
-        const int rem = int(row - grp * img);
+        r.grp = row / img;
+        const int rem = int(row - r.grp * img);
         const int h = rem / ep.img_Wp - 1, w = rem % ep.img_Wp - 1;
-        valid = valid && h >= 0 && h < ep.img_H && w >= 0 && w < ep.img_W;
+        r.valid = r.valid && h >= 0 && h < ep.img_H && w >= 0 && w < ep.img_W;
         const int sw = ep.img_stride_w ? ep.img_stride_w : ep.img_stride;
-        valid = valid && (h % ep.img_stride) == 0 && (w % sw) == 0;
-        out_row = (grp * ep.out_Hp + h / ep.img_stride + 1) * ep.out_Wp + w / sw + 1;
+        r.valid = r.valid && (h % ep.img_stride) == 0 && (w % sw) == 0;
+        r.out_row = (r.grp * ep.out_Hp + h / ep.img_stride + 1) * ep.out_Wp + w / sw + 1;
     } else if (ep.Tp > 0) {
-        grp = row / ep.Tp;
-        const int t = int(row - grp * ep.Tp) - ep.P;
-        valid = valid && t >= 0 && t < ep.T;
-        if (ep.seg_scale && valid) sgrp = grp * ep.nseg + t / ep.seg_len;
-        if (ep.halo && valid) {
-            if (t >= 1 && t <= ep.P) mirror_a = row - 2 * t;
+        r.grp = row / ep.Tp;
+        const int t = int(row - r.grp * ep.Tp) - ep.P;
+        r.valid = r.valid && t >= 0 && t < ep.T;
+        if (ep.seg_scale && r.valid) r.sgrp = r.grp * ep.nseg + t / ep.seg_len;
+        if (ep.halo && r.valid) {
+            if (t >= 1 && t <= ep.P) r.mirror_a = row - 2 * t;
             const int u = ep.T - 1 - t;  // distance from the last frame
-            if (u >= 1 && u <= ep.P) mirror_b = row + 2 * u;
+            if (u >= 1 && u <= ep.P) r.mirror_b = row + 2 * u;
         }
     }
+    const bool same_grid = ep.img_Wp == 0 || (ep.img_stride == 1 && ep.img_stride_w <= 1 && ep.out_Hp == ep.img_Hp && ep.out_Wp == ep.img_Wp);
+    if (!r.valid && row_in >= 0 && ep.zero_invalid && ep.out_mode == OUT_PLANES && !ep.halo && same_grid) r.zero_row = row_in + out_row_shift;
+    return r;
+}
 
-    mbar_wait(tfull_bar, acc_phase);
-    tc_fence_after();
-    const uint32_t t_addr = tmem_acc + (uint32_t(q * 32) << 16);
-
-    if (ep.tma_store && staging != 0) {
-        // ---- planes output without halo: each half of the epilogue (ehalf: four warps = the 128 rows of the tile) streams ITS 32-column
-        // chunks through its own swizzled staging tile ([hi | lo] x 128 rows x 64 B, SWIZZLE_64B) and writes them out by TMA; the two halves
-        // share nothing (own named barrier, own bulk groups), so one half's store drain / barrier wait overlaps the other's math.
-        // Garbage rows (time padding, rows >= M) are stored too: their consumers never read them.
-        const int64_t gsafe = valid ? grp : 0;
-        const uint32_t stg = staging + ehalf * (EPI_STAGING_BYTES / 2);
-        uint8_t* sh = staging_gen + ehalf * (EPI_STAGING_BYTES / 2) + rloc * 64;
-        const bool issuer = (etid & 127) == 0;
-#pragma unroll 1
-        for (int s = 0; s < BN / 64; ++s) {
-            const int c = 2 * s + ehalf;
-            const int col = n0 + c * 32;
-            uint32_t v[32];
-            __syncwarp();
-            tmem_ld32(t_addr + c * 32, v);
-            tmem_ld_wait();
-            if (s == BN / 64 - 1) {  // this warp's last read of the accumulator: hand it back before the math / staging / store of the chunk
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if (tempty_remote) mbar_arrive_cluster(tempty_remote); else mbar_arrive(tempty_bar);
-                }
-            }
-            float x[32];
-            if (col < N && (valid || !ep.zero_invalid)) {
-                epilogue_math(ep, N, col, gsafe, sgrp, v, x);
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) x[j] = 0.f;
-            }
-            uint32_t hw[16], lw[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) split_pack_bf16x2(x[2 * j], x[2 * j + 1], hw[j], lw[j]);
-            if (issuer) bulk_wait_read0();  // this half's previous stores have drained its staging tile
-            named_bar_sync(1 + ehalf, GEMM_EPI_THREADS / 2);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {  // four 16-byte chunks (8 columns each); SWIZZLE_64B: chunk index XOR ((row >> 1) & 3)
-                const int chunk = (k ^ ((rloc >> 1) & 3)) << 4;
-                *reinterpret_cast<uint4*>(sh + chunk) = make_uint4(hw[4 * k], hw[4 * k + 1], hw[4 * k + 2], hw[4 * k + 3]);
-                *reinterpret_cast<uint4*>(sh + GEMM_BM * 64 + chunk) = make_uint4(lw[4 * k], lw[4 * k + 1], lw[4 * k + 2], lw[4 * k + 3]);
-            }
-            fence_proxy_async_smem();
-            named_bar_sync(1 + ehalf, GEMM_EPI_THREADS / 2);
-            if (issuer && col < N && !ep.debug_nostore) {
-                tma_store_3d(map_out, stg, ep.out_col0 + col, m0, 0);
-                tma_store_3d(map_out, stg + GEMM_BM * 64, ep.out_col0 + col, m0, 1);
-                bulk_commit_group();
-            }
+// two adjacent columns (col, col + 1) of one row
+__device__ __forceinline__ void epilogue_pair(const Epilogue& ep, int N, int col, const EpiRow& r, float a, float b) {
+    if (col >= N) return;
+    if (!r.valid) {
+        if (r.zero_row >= 0) {
+            __nv_bfloat16* ph = static_cast<__nv_bfloat16*>(ep.out) + r.zero_row * ep.out_ld + ep.out_col0 + col;
+            *reinterpret_cast<uint32_t*>(ph) = 0u;
+            *reinterpret_cast<uint32_t*>(ph + ep.out_plane_stride) = 0u;
         }
         return;
     }
-
-#pragma unroll 1
-    for (int c = ehalf; c < BN / 32; c += GEMM_EPI_THREADS / 128) {
-        uint32_t v[32];
-        __syncwarp();  // tcgen05.ld is warp-collective: reconverge after the divergent stores
-        tmem_ld32(t_addr + c * 32, v);
-        tmem_ld_wait();
-        if (sum_cols) {  // the accumulator is split in two column blocks `sum_cols` apart (conv3x3.cu: A_hi x [W_hi | W_lo]): add them
-            uint32_t v2[32];
-            tmem_ld32(t_addr + c * 32 + sum_cols, v2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-        }
-        const int col = n0 + c * 32;
-        if (!valid || col >= N || ep.debug_nostore) continue;
-        float x[32];
-        if (col + 32 <= N) {
-            epilogue_math(ep, N, col, grp, sgrp, v, x);
-        } else {  // ragged N (cosine scoring): no per-column vectors on this path
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-        }
-        if (ep.out_mode == OUT_F32) {
-            float* dstf = static_cast<float*>(ep.out) + out_row * ep.out_ld + ep.out_col0 + col;
-            if (ep.f32_vec_ok == 2 && col + 32 <= N) {  // 32-byte aligned rows: full-sector stores
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    st_global_v8(dstf + 8 * j, __float_as_uint(x[8 * j]), __float_as_uint(x[8 * j + 1]), __float_as_uint(x[8 * j + 2]),
-                                 __float_as_uint(x[8 * j + 3]), __float_as_uint(x[8 * j + 4]), __float_as_uint(x[8 * j + 5]),
-                                 __float_as_uint(x[8 * j + 6]), __float_as_uint(x[8 * j + 7]));
-            } else if (ep.f32_vec_ok && col + 32 <= N) {
-                float4* dst = reinterpret_cast<float4*>(dstf);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) dst[j] = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-            } else {  // ragged N (cosine scoring): guarded scalar stores
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (col + j < N) dstf[j] = x[j];
-            }
+    const bool two = col + 1 < N;
+    a = epilogue_math1(ep, N, col, r.grp, r.sgrp, a);
+    if (two) b = epilogue_math1(ep, N, col + 1, r.grp, r.sgrp, b);
+    if (ep.out_mode == OUT_F32) {
+        float* dst = static_cast<float*>(ep.out) + r.out_row * ep.out_ld + ep.out_col0 + col;
+        if (two && ep.f32_vec_ok) {
+            *reinterpret_cast<float2*>(dst) = make_float2(a, b);
         } else {
-            uint32_t h[16], l[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) split_pack_bf16x2(x[2 * j], x[2 * j + 1], h[j], l[j]);
-            __nv_bfloat16* obase = static_cast<__nv_bfloat16*>(ep.out) + ep.out_col0 + col;
-            auto store_row = [&](int64_t r) {  // 64 B per plane = two full 32-byte sectors
-                __nv_bfloat16* ph = obase + r * ep.out_ld;
-                __nv_bfloat16* pl = ph + ep.out_plane_stride;
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    st_global_v8(ph + 16 * j, h[8 * j], h[8 * j + 1], h[8 * j + 2], h[8 * j + 3], h[8 * j + 4], h[8 * j + 5], h[8 * j + 6],
-                                 h[8 * j + 7]);
-                    st_global_v8(pl + 16 * j, l[8 * j], l[8 * j + 1], l[8 * j + 2], l[8 * j + 3], l[8 * j + 4], l[8 * j + 5], l[8 * j + 6],
-                                 l[8 * j + 7]);
-                }
-            };
-            store_row(out_row);
-            if (mirror_a >= 0) store_row(mirror_a);
-            if (mirror_b >= 0) store_row(mirror_b);
+            dst[0] = a;
+            if (two) dst[1] = b;
         }
+        return;
     }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-        if (tempty_remote) mbar_arrive_cluster(tempty_remote); else mbar_arrive(tempty_bar);  // pair mode: the leader CTA's barrier
+    uint32_t h, l;
+    split_pack_bf16x2(a, b, h, l);
+    __nv_bfloat16* obase = static_cast<__nv_bfloat16*>(ep.out) + ep.out_col0 + col;
+    auto store_row = [&](int64_t row) {
+        uint32_t* ph = reinterpret_cast<uint32_t*>(obase + row * ep.out_ld);
+        ph[0] = h;
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ph) + ep.out_plane_stride) = l;
+    };
+    store_row(r.out_row);
+    if (r.mirror_a >= 0) store_row(r.mirror_a);
+    if (r.mirror_b >= 0) store_row(r.mirror_b);
+}
+
+// The whole 64 x BN fragment of this warpgroup.  `row_of(r)`, r in [0, 64): the GEMM row of warpgroup-local row r, or -1 if it
+// holds no output; `t`: thread index inside the warpgroup; columns are n0 + [0, BN).
+template <int BN, typename RowOf>
+__device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0, const float (&acc)[BN / 2], RowOf&& row_of, int t,
+                                              int64_t out_row_shift = 0) {
+    if (ep.debug_nostore) return;
+    const int w = t >> 5, l = t & 31;
+    const int r0 = 16 * w + (l >> 2);
+    const EpiRow ra = epilogue_row(ep, row_of(r0), out_row_shift);
+    const EpiRow rb = epilogue_row(ep, row_of(r0 + 8), out_row_shift);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+        const int col = n0 + 8 * i + 2 * (l & 3);
+        epilogue_pair(ep, N, col, ra, acc[4 * i + 0], acc[4 * i + 1]);
+        epilogue_pair(ep, N, col, rb, acc[4 * i + 2], acc[4 * i + 3]);
     }
 }
 

@@ -1,0 +1,392 @@
+// Gather-GEMM on the Hopper tensor cores (wgmma + TMA + mbarrier), the contraction behind every Conv1d / Linear of the
+// ppvector hot path (reference: ppvector/models/utils.py:65-77 Conv1d.forward, reached from TDNNBlock utils.py:147,
+// Res2NetBlock ecapa_tdnn.py:36-47, ASP pooling.py:107, fc).
+//
+//   out[r, n] = epilogue( sum_s  A_{map(s)}[r + row_off(s), a_col(s) : a_col(s)+64] . W[n, 64 s : 64 s + 64] )
+//
+// A "k-step" s is one 64-wide K slice: a conv tap is a row offset in the padded time layout, a channel
+// concat is a different source tensor, `x_i + y_{i-1}` (Res2Net) is two sources sharing the same weights.
+// Operands are split-bf16 planes (hi, lo); PPV_PREC_BF16X3 issues hi*hi + lo*hi + hi*lo into one fp32
+// register accumulator (fp32-grade), PPV_PREC_BF16 issues hi*hi only.
+//
+// Warp roles (384 threads, 1 CTA / SM, persistent over 128 x BN tiles):
+//   warp 0        TMA producer : cp.async.bulk.tensor 3-D tiles (SWIZZLE_128B / 64B) into a STAGES-deep smem ring
+//   warps 4-7     MMA + epilogue of tile rows 0-63 : wgmma m64 x BN x 16 from the ring, then bias / ReLU / BN affine / tanh ->
+//   warps 8-11    MMA + epilogue of tile rows 64-127  split-bf16 (or fp32) stores incl. the reflect-halo rows
+// The producer runs ahead into the next tile while the two warpgroups drain their accumulators.
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <algorithm>
+#include <mutex>
+
+#include "common.h"
+#include "gemm_epilogue.cuh"
+#include "ptx.cuh"
+
+namespace ppv {
+
+// BK = K elements per pipeline stage: 64 (128-byte rows, SWIZZLE_128B) or 32 (64-byte rows, SWIZZLE_64B).  The smaller
+// stage keeps the same bytes per MMA but doubles the number of ring slots, i.e. more TMA bytes in flight for the same
+// shared memory.
+template <int BN, int NSPLIT, int BK>
+struct GemmCfg {
+    static constexpr int NA = (NSPLIT == 3) ? 2 : 1;  // A tiles per stage (hi[, lo])
+    static constexpr int NB = NA;
+    static constexpr int A_BYTES = GEMM_BM * BK * 2;
+    static constexpr int B_BYTES = BN * BK * 2;
+    static constexpr int STAGE_BYTES = NA * A_BYTES + NB * B_BYTES;
+    static constexpr int BAR_BYTES = 256;
+    static constexpr int MAX_SMEM = 232448;  // 227 KB
+    static constexpr int STAGES_RAW = (MAX_SMEM - 1024 - BAR_BYTES) / STAGE_BYTES;
+    static constexpr int MAX_STAGES = 8;  // barrier slots
+    static constexpr int STAGES = STAGES_RAW > MAX_STAGES ? MAX_STAGES : STAGES_RAW;
+    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + BAR_BYTES;
+    static_assert(STAGES >= 2, "need at least a double buffer");
+    static_assert(BN == 64 || BN == 128 || BN == 256, "BN");
+    static_assert(BK == 64 || BK == 32, "BK");
+};
+
+template <int BK>
+__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr) {
+    return BK == 64 ? make_sw128_kmajor_desc(smem_addr) : make_sw64_kmajor_desc(smem_addr);
+}
+
+template <int BN, int NSPLIT, int BK>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GemmParams gp) {
+    using Cfg = GemmCfg<BN, NSPLIT, BK>;
+    constexpr int STAGES = Cfg::STAGES;
+    extern __shared__ uint8_t smem_raw[];
+    // SWIZZLE_128B tiles need 1024-byte alignment.
+    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const uint32_t tiles_base = smem_base;
+    const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
+    // barrier layout (8 B each): full[8], empty[8], resident-weights barrier
+    constexpr int MAXST = Cfg::MAX_STAGES;
+    auto full_bar = [&](int s) { return bar_base + 8u * s; };
+    auto empty_bar = [&](int s) { return bar_base + 8u * (MAXST + s); };
+    const uint32_t w_full = bar_base + 8u * (2 * MAXST);
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    // Weight-stationary mode (gp.ws, narrow convs with one n-tile and a small K): the whole weight matrix is loaded ONCE per CTA
+    // into the upper part of the ring's shared memory and the ring (4 slots) carries activation tiles only -- for the
+    // 32-channel 3x3 convs of the 2-D models the per-tile reload of the weights was a third of the L2 -> SM traffic.
+    const int nst = gp.ws ? GEMM_WS_STAGES : STAGES;
+    const uint32_t w_res = tiles_base + GEMM_WS_STAGES * Cfg::STAGE_BYTES;
+
+    if (warp == 0 && lane == 0) {
+        for (int i = 0; i < GEMM_MAX_MAPS; ++i) prefetch_tmap(&gp.mapA[i]);
+        prefetch_tmap(&gp.mapB);
+    }
+    if (warp == 1 && lane == 0) {
+        for (int s = 0; s < MAXST; ++s) {
+            mbar_init(full_bar(s), 1);
+            mbar_init(empty_bar(s), GEMM_MMA_THREADS / 128);  // one arrival per MMA warpgroup
+        }
+        mbar_init(w_full, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    griddep_launch_dependents();  // PDL: the next kernel may begin its prologue
+    griddep_wait();               // PDL: upstream activations are complete and visible
+
+    // lin_splits > 0: "wgrad" mode -- the contraction runs over the COLUMNS of both operands (two transposed matrices
+    // [M][R] and [N][R]), k-step s of split z reads columns (z * nk + s) * BK; there is no k-step table, and split z of
+    // tile (m, n) accumulates into its own partial output block (rows shifted by z * lin_split_rows).
+    const int mn_tiles = gp.m_tiles * gp.n_tiles;
+    const int num_tiles = mn_tiles * (gp.lin_splits > 0 ? gp.lin_splits : 1);
+    const int nk = gp.num_ksteps;
+    auto tile_m = [&](int t) { return (t % mn_tiles) / gp.n_tiles; };
+    auto tile_n = [&](int t) { return (t % mn_tiles) % gp.n_tiles; };
+
+    if (warp == 0) {
+        // ===================== TMA producer =====================
+        int stage = 0;
+        uint32_t phase = 0;
+        if (gp.ws && lane == 0) {  // resident weights: every k-slice, once
+            mbar_arrive_expect_tx(w_full, nk * Cfg::NB * Cfg::B_BYTES);
+            for (int s = 0; s < nk; ++s)
+                for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(w_res + (s * Cfg::NB + p) * Cfg::B_BYTES, &gp.mapB, w_full, s * BK, 0, p);
+        }
+        __syncwarp();
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            const int zsplit = tile / mn_tiles;
+            const int m0 = tile_m(tile) * GEMM_BM;
+            const int n0 = tile_n(tile) * BN;
+            // L2 prefetch of the activation rows of this CTA's NEXT tile (one CTA per m-tile issues it): they come
+            // from HBM, and a 2-4 slot ring alone cannot hide that latency.
+            const int ntile = tile + gridDim.x;
+            if (gp.l2_prefetch && ntile < num_tiles && tile_n(ntile) == 0 && lane < nk && gp.lin_splits == 0) {
+                const int nm0 = tile_m(ntile) * GEMM_BM;
+                for (int s = lane; s < nk; s += 32) {
+                    const KStep ks = gp.ksteps[s];
+#pragma unroll
+                    for (int p = 0; p < Cfg::NA; ++p) tma_prefetch_l2_3d(&gp.mapA[ks.map], ks.a_col, nm0 + ks.row_off, p);
+                }
+            }
+            __syncwarp();
+            for (int s = 0; s < nk; ++s) {
+                mbar_wait(empty_bar(stage), phase ^ 1u);
+                if (lane == 0) {
+                    const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
+                    const uint32_t sb = sa + Cfg::NA * Cfg::A_BYTES;
+                    const uint32_t fb = full_bar(stage);
+                    mbar_arrive_expect_tx(fb, gp.ws ? Cfg::NA * Cfg::A_BYTES : Cfg::STAGE_BYTES);
+                    if (gp.ws) {
+                        const KStep ks = gp.ksteps[s];
+#pragma unroll
+                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[ks.map], fb, ks.a_col, m0 + ks.row_off, p);
+                    } else if (gp.lin_splits > 0) {
+                        const int kcol = (zsplit * nk + s) * BK;
+#pragma unroll
+                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[0], fb, kcol, m0, p);
+#pragma unroll
+                        for (int p = 0; p < Cfg::NB; ++p)
+                            tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, kcol + gp.lin_b_col0, gp.lin_b_row0 + n0, p);
+                    } else {
+                        const KStep ks = gp.ksteps[s];
+                        const CUtensorMap* ma = &gp.mapA[ks.map];
+#pragma unroll
+                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, ma, fb, ks.a_col, m0 + ks.row_off, p);
+#pragma unroll
+                        for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, s * BK, n0, p);
+                    }
+                }
+                __syncwarp();
+                if (++stage == nst) {
+                    stage = 0;
+                    phase ^= 1u;
+                }
+            }
+        }
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup g owns rows [64 g, 64 g + 64) of every tile =====================
+        const int g = (warp - 4) >> 2;
+        const int t = threadIdx.x & 127;
+        constexpr uint32_t A_WG_OFF = 64 * BK * 2;  // 64 rows of the A tile (a whole number of 8-row swizzle groups)
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        if (gp.ws) mbar_wait(w_full, 0);
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            const int m0 = tile_m(tile) * GEMM_BM;
+            const int n0 = tile_n(tile) * BN;
+            int prev = -1;
+            wgmma_fence_acc(acc);
+            for (int s = 0; s < nk; ++s) {
+                mbar_wait(full_bar(stage), phase);
+                const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
+                const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
+                const uint64_t a_hi = make_kmajor_desc<BK>(sa + g * A_WG_OFF);
+                const uint64_t b_hi = make_kmajor_desc<BK>(sb);
+                wgmma_fence();
+                // K advance inside the swizzle atom: +32 B (16 bf16) per MMA => +2 in the descriptor's start field
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
+                if (NSPLIT == 3) {
+                    const uint64_t a_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES + g * A_WG_OFF);
+                    const uint64_t b_lo = make_kmajor_desc<BK>(sb + Cfg::B_BYTES);
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
+                if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+                prev = stage;
+                if (++stage == nst) {
+                    stage = 0;
+                    phase ^= 1u;
+                }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (t == 0) mbar_arrive(empty_bar(prev));
+            const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
+            const int rbase = m0 + 64 * g;
+            epilogue_frag<BN>(gp.epi, gp.N, n0, acc, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ host
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static EncodeTiledFn get_encode_fn() {
+    static EncodeTiledFn fn = nullptr;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+            q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeTiledFn>(p);
+    });
+    return fn;
+}
+
+int encode_planes_map_ex(CUtensorMap* m, const Planes& t, int box_cols, int box_rows, int swizzle_bytes) {
+    EncodeTiledFn enc = get_encode_fn();
+    if (!enc) return fail(PPV_ECUDA, "cuTensorMapEncodeTiled entry point not available");
+    if ((reinterpret_cast<uintptr_t>(t.base) & 15) || (t.ld % 8) || (t.plane_stride % 8))
+        return fail(PPV_EINVAL, "planes tensor not 16-byte aligned");
+    cuuint64_t dims[3] = {cuuint64_t(t.ld), cuuint64_t(t.rows), 2};
+    cuuint64_t strides[2] = {cuuint64_t(t.ld) * 2, cuuint64_t(t.plane_stride) * 2};
+    cuuint32_t box[3] = {cuuint32_t(box_cols), cuuint32_t(box_rows), 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, t.base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(PPV_ECUDA, "cuTensorMapEncodeTiled failed, CUresult " + std::to_string(int(r)));
+    return PPV_OK;
+}
+
+// 3-D map over split planes [2][rows][ld] bf16, box = {64 cols, box_rows, 1 plane}, SWIZZLE_128B.
+int encode_planes_map(CUtensorMap* m, const Planes& t, int box_rows) { return encode_planes_map_ex(m, t, GEMM_BK, box_rows, 128); }
+
+int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W, int M, int N, const Epilogue& epi,
+               int BN, int BK) {
+    PPV_REQUIRE(BK == 64 || BK == 32, "gemm_build: BK must be 64 or 32");
+    PPV_REQUIRE(BN == 64 || BN == 128 || BN == 256, "gemm_build: BN must be 64/128/256");
+    PPV_REQUIRE(epi.out_mode == OUT_F32 || N % 32 == 0, "gemm_build: planes output needs N % 32 == 0");
+    PPV_REQUIRE(!epi.rowgrp_bias || N % 32 == 0, "gemm_build: row-group bias needs N % 32 == 0");
+    memset(gp, 0, sizeof(*gp));
+    // distinct A tensors -> maps
+    const __nv_bfloat16* bases[GEMM_MAX_MAPS];
+    int nmaps = 0;
+    int ks = 0;
+    for (int i = 0; i < nsrc; ++i) {
+        const GemmSource& s = srcs[i];
+        PPV_REQUIRE(s.ncols % BK == 0 && s.col0 % 8 == 0, "gemm_build: source K slice must be a multiple of the k-step");
+        PPV_REQUIRE(s.col0 + s.ncols <= s.t.ld, "gemm_build: source K slice exceeds the row");
+        int mi = -1;
+        for (int j = 0; j < nmaps; ++j)
+            if (bases[j] == s.t.base) mi = j;
+        if (mi < 0) {
+            PPV_REQUIRE(nmaps < GEMM_MAX_MAPS, "gemm_build: too many distinct A tensors");
+            mi = nmaps++;
+            bases[mi] = s.t.base;
+            int rc = encode_planes_map_ex(&gp->mapA[mi], s.t, BK, GEMM_BM, BK * 2);
+            if (rc) return rc;
+        }
+        for (int c = 0; c < s.ncols; c += BK) {
+            PPV_REQUIRE(ks < GEMM_MAX_KSTEPS, "gemm_build: too many k-steps");
+            gp->ksteps[ks].map = int16_t(mi);
+            gp->ksteps[ks].row_off = int16_t(s.row_off);
+            gp->ksteps[ks].a_col = s.col0 + c;
+            ++ks;
+        }
+    }
+    for (int j = nmaps; j < GEMM_MAX_MAPS; ++j) gp->mapA[j] = gp->mapA[0];
+    PPV_REQUIRE(ks > 0, "gemm_build: empty K");
+    PPV_REQUIRE(W.ld == ks * BK, "gemm_build: weight K does not match the k-steps");
+    PPV_REQUIRE(W.rows >= N, "gemm_build: weight rows < N");
+    int rc = encode_planes_map_ex(&gp->mapB, W, BK, BN, BK * 2);
+    if (rc) return rc;
+    gp->num_ksteps = ks;
+    gp->bk = BK;
+    gp->M = M;
+    gp->N = N;
+    gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
+    gp->n_tiles = (N + BN - 1) / BN;
+    gp->epi = epi;
+    {
+        // weight-stationary: one n-tile, all k-slices of W (both planes) fit next to a 4-slot ring, and enough tiles per CTA to pay
+        // (two per SM of a 132-SM H100)
+        const size_t stage_bytes = size_t(2) * GEMM_BM * BK * 2 + size_t(2) * BN * BK * 2;
+        const size_t stages_full = std::min<size_t>(8, (232448 - 1024 - 256) / stage_bytes);
+        const size_t w_bytes = size_t(ks) * 2 * BN * BK * 2;
+        const char* wsenv = getenv("PPV_GEMM_WS");
+        gp->ws = (gp->n_tiles == 1 && stages_full > GEMM_WS_STAGES && w_bytes <= (stages_full - GEMM_WS_STAGES) * stage_bytes && gp->m_tiles >= 264 &&
+                  !(wsenv && wsenv[0] == '0'))
+                     ? 1
+                     : 0;
+    }
+    {
+        const char* ns = getenv("PPV_GEMM_NOSTORE");
+        gp->epi.debug_nostore = (ns && ns[0] == '1') ? 1 : 0;
+        const char* pf = getenv("PPV_GEMM_NO_L2PREFETCH");
+        gp->l2_prefetch = (pf && pf[0] == '1') ? 0 : 1;
+    }
+    if (epi.out_mode == OUT_PLANES) {
+        PPV_REQUIRE((epi.out_ld % 16) == 0 && (epi.out_col0 % 16) == 0 && (epi.out_plane_stride % 16) == 0 &&
+                        (reinterpret_cast<uintptr_t>(epi.out) & 15) == 0,
+                    "gemm_build: planes output must be 16-byte aligned");
+    } else {
+        gp->epi.f32_vec_ok = ((epi.out_ld % 2) == 0 && (epi.out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(epi.out) & 7) == 0) ? 1 : 0;
+    }
+    return PPV_OK;
+}
+
+// Weight-gradient GEMM: out[z][m, out_col0 + n] = sum over columns r of split z of  At[m, r] * Bt[b_row0 + n, r + b_col0]
+// (At = transposed output gradient [M][R], Bt = transposed layer input [*][R]; b_col0 = conv tap offset in rows of the
+// padded time layout).  Partial blocks are `split_rows` output rows apart; the caller sums them.
+int gemm_build_wgrad(GemmParams* gp, const Planes& At, const Planes& Bt, int M, int N, int b_row0, int b_col0, int splits, float* out,
+                     int64_t out_ld, int out_col0, int64_t split_rows, int BN) {
+    PPV_REQUIRE(BN == 64 || BN == 128 || BN == 256, "gemm_build_wgrad: BN must be 64/128/256");
+    PPV_REQUIRE(At.ld == Bt.ld && splits >= 1, "gemm_build_wgrad: operands must share the contraction length");
+    memset(gp, 0, sizeof(*gp));
+    int rc = encode_planes_map_ex(&gp->mapA[0], At, GEMM_BK, GEMM_BM, 128);
+    if (rc) return rc;
+    for (int j = 1; j < GEMM_MAX_MAPS; ++j) gp->mapA[j] = gp->mapA[0];
+    rc = encode_planes_map_ex(&gp->mapB, Bt, GEMM_BK, BN, 128);
+    if (rc) return rc;
+    const int nk_total = (At.ld + GEMM_BK - 1) / GEMM_BK;
+    gp->lin_splits = std::min(splits, nk_total);
+    gp->num_ksteps = (nk_total + gp->lin_splits - 1) / gp->lin_splits;
+    gp->lin_b_row0 = b_row0;
+    gp->lin_b_col0 = b_col0;
+    gp->lin_split_rows = split_rows;
+    gp->bk = GEMM_BK;
+    gp->M = M;
+    gp->N = N;
+    gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
+    gp->n_tiles = (N + BN - 1) / BN;
+    Epilogue ep;
+    ep.out_mode = OUT_F32;
+    ep.out = out;
+    ep.out_ld = out_ld;
+    ep.out_col0 = out_col0;
+    gp->epi = ep;
+    gp->epi.f32_vec_ok = ((out_ld % 2) == 0 && (out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 1 : 0;
+    PPV_REQUIRE(N % 32 == 0, "gemm_build_wgrad: N % 32 == 0 required");
+    return PPV_OK;
+}
+
+template <int BN, int NSPLIT, int BK>
+static int launch_one(const GemmParams& gp, int num_sms, cudaStream_t stream) {
+    using Cfg = GemmCfg<BN, NSPLIT, BK>;
+    PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, NSPLIT, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::SMEM_BYTES)));
+    const int tiles = gp.m_tiles * gp.n_tiles * (gp.lin_splits > 0 ? gp.lin_splits : 1);
+    const int grid = std::min(tiles, num_sms);
+    PPV_PDL_OK(launch_pdl(gemm_wgmma_kernel<BN, NSPLIT, BK>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, gp),
+               "gemm_wgmma_kernel");
+    return PPV_OK;
+}
+
+template <int BN>
+static int launch_bn(const GemmParams& gp, bool x3, int num_sms, cudaStream_t stream) {
+    if (gp.bk == 32) return x3 ? launch_one<BN, 3, 32>(gp, num_sms, stream) : launch_one<BN, 1, 32>(gp, num_sms, stream);
+    return x3 ? launch_one<BN, 3, 64>(gp, num_sms, stream) : launch_one<BN, 1, 64>(gp, num_sms, stream);
+}
+
+int gemm_launch(const GemmParams& gp, int BN, int precision, int num_sms, cudaStream_t stream) {
+    const bool x3 = (precision == PPV_PREC_BF16X3);
+    switch (BN) {
+        case 64: return launch_bn<64>(gp, x3, num_sms, stream);
+        case 128: return launch_bn<128>(gp, x3, num_sms, stream);
+        case 256: return launch_bn<256>(gp, x3, num_sms, stream);
+    }
+    return fail(PPV_EINVAL, "gemm_launch: bad BN");
+}
+
+}  // namespace ppv

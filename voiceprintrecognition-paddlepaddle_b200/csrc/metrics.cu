@@ -329,7 +329,7 @@ int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_la
     uint32_t* tsum = reinterpret_cast<uint32_t*>(take(size_t(nb) * 4));
     uint32_t* tsum_raw = reinterpret_cast<uint32_t*>(take(size_t(nb) * 4));
     EerAcc* acc = reinterpret_cast<EerAcc*>(take(sizeof(EerAcc)));
-    const int pack_grid = int(std::min<int64_t>((n + 255) / 256, 148 * 8));
+    const int pack_grid = int(std::min<int64_t>((n + 255) / 256, 132 * 8));
     eer_pack_kernel<<<pack_grid, 256, 0, st>>>(scores, labels, row_labels, col_labels, ncols, n, ka);
     PPV_LAUNCH_OK("eer_pack_kernel");
     for (int pass = 0; pass < RS_PASSES; ++pass) {

@@ -2,12 +2,11 @@
 // ResNetSE's first-stage conv1 / conv3 / downsample where the input is the 32-channel stem (ppvector/models/resnet_se.py:24-45),
 // ERes2Net's layer-1 conv1 / shortcut (ppvector/models/eres2net.py:85-108) and CAM++'s FCM shortcuts (ppvector/models/campplus.py:232-238).
 //
-// On the tcgen05 gather-GEMM these layers run one 128-row tile per pipeline step with a single 32-wide k-step: 49 200 tiles of 16 KB at
-// the 80 x 298 resolution, paced by the per-tile epilogue chain (~950 us per launch against a ~300 us HBM floor:
-// profiles/eres2net_launches_r2_summary.txt).  Here one thread owns one grid position, keeps its 32 input values (exact hi + lo) in
-// registers and walks the fp32 weight matrix in shared memory with broadcast 16-byte loads: 2 K N FLOP per position on the FMA pipe.
-// Measured 870 us at K = 32; the same kernel at K = 64 took 1670 us (every 4 FMAs cost one broadcast LDS.128 = 4 LSU cycles per warp, i.e.
-// shared-memory bound at 4x its FMA time) against 1020 us on the tensor path, so only K = 32 is routed here.
+// On the tensor-core gather-GEMM these layers run one 128-row tile per pipeline step with a single 32-wide k-step: 49 200 tiles of 16 KB at
+// the 80 x 298 resolution, paced by the per-tile epilogue chain rather than by HBM.  Here one thread owns one grid position, keeps its
+// 32 input values (exact hi + lo) in registers and walks the fp32 weight matrix in shared memory with broadcast 16-byte loads: 2 K N FLOP
+// per position on the FMA pipe.  At K = 64 every 4 FMAs cost one broadcast LDS.128 (4 LSU cycles per warp), so the kernel would be
+// shared-memory bound at 4x its FMA time: only K = 32 is routed here.
 #include <type_traits>
 
 #include "common.h"
@@ -110,9 +109,9 @@ __global__ void __launch_bounds__(256, 2) pw_conv_kernel(const PwParams p) {
             __nv_bfloat16* oh = static_cast<__nv_bfloat16*>(ep.out) + out_row * ep.out_ld + ep.out_col0 + n0;
             __nv_bfloat16* ol = oh + ep.out_plane_stride;
 #pragma unroll
-            for (int j = 0; j < PW_NCH / 16; ++j) {  // 64 B per plane = two full 32-byte sectors
-                st_global_v8(oh + 16 * j, h[8 * j], h[8 * j + 1], h[8 * j + 2], h[8 * j + 3], h[8 * j + 4], h[8 * j + 5], h[8 * j + 6], h[8 * j + 7]);
-                st_global_v8(ol + 16 * j, l[8 * j], l[8 * j + 1], l[8 * j + 2], l[8 * j + 3], l[8 * j + 4], l[8 * j + 5], l[8 * j + 6], l[8 * j + 7]);
+            for (int j = 0; j < PW_NCH / 8; ++j) {  // 16-byte stores, 64 B per plane
+                *reinterpret_cast<uint4*>(oh + 8 * j) = make_uint4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
+                *reinterpret_cast<uint4*>(ol + 8 * j) = make_uint4(l[4 * j], l[4 * j + 1], l[4 * j + 2], l[4 * j + 3]);
             }
         }
     }

@@ -1,16 +1,16 @@
 // The whole Res2Net chain of one SE-Res2Net block in ONE kernel: y_1 = f_1(x_1), y_j = f_j(x_j + y_{j-1}), j = 2..7, with
 // f_j = BN(ReLU(conv_k3,d(.))) on 64-channel chunks (ppvector/models/ecapa_tdnn.py:36-47, TDNNBlock utils.py:147).
 //
-// The seven convs are strictly sequential, and as seven launches each one costs a full kernel latency (~24 us for 4 us of
-// tensor work; profiles/launches_r1_final_summary.txt).  Here one CTA owns one UTTERANCE: its whole padded time axis
-// (<= 384 rows x 64 channels, split-bf16) lives in shared memory in the SWIZZLE_128B layout the UMMA descriptors read, so
+// The seven convs are strictly sequential, and as seven launches each one costs a full kernel latency.  Here one CTA owns one
+// UTTERANCE: its whole padded time axis (<= 384 rows x 64 channels, split-bf16) lives in shared memory in the SWIZZLE_128B
+// layout the wgmma descriptors read, so
 //   * conv taps are descriptor row offsets into that resident tile (as in res2conv.cu),
 //   * the epilogue of conv j writes BN(ReLU(.)) to HBM once (the tdnn2 GEMM reads it) and writes x_{j+1} + y_j -- including
 //     the reflect-padding halo rows -- straight back into the shared-memory tile as the A operand of conv j+1:
 //     the intermediate sums never touch HBM and there is no inter-CTA dependency at all,
-//   * the 48 KB of weights of conv j+1 stream into a second slot by TMA while conv j runs.
-// Warp roles: warp 0 TMA, warp 1 MMA issue, warp 2 TMEM, warps 4-19 epilogue (640 threads).  TMEM holds three
-// 128 x 64 fp32 accumulators (the three 128-row tiles of the utterance).
+//   * the 48 KB of weights of conv j+1 stream into the weight slot by TMA while the epilogue of conv j runs.
+// Warp roles: warp 0 TMA, warp 3 TMA store, warps 4-15 three MMA warpgroups (512 threads): warpgroup t owns the 128-row
+// output tile t of the utterance (two m64 x n64 register accumulators) and runs its epilogue.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -29,8 +29,8 @@ constexpr int RC_W_TILE = 64 * 128;             // [64 out ch x 64 k] bf16
 constexpr int RC_MAX_TILES = 3;                 // 128-row output tiles per utterance
 constexpr int RC_MAX_TP = RC_MAX_TILES * GEMM_BM;  // 384
 constexpr int RC_S_PLANE = GEMM_BM * 128;       // staging tile: 128 rows x 64 channels bf16, SWIZZLE_128B
-constexpr int RC_EPI_THREADS = 512;             // 16 epilogue warps: four per TMEM lane quarter, 16 channels each
-constexpr int RC_THREADS = 128 + RC_EPI_THREADS;
+constexpr int RC_MMA_THREADS = 128 * RC_MAX_TILES;  // one MMA warpgroup per 128-row tile
+constexpr int RC_THREADS = 128 + RC_MMA_THREADS;
 
 template <int NSPLIT>
 struct RCCfg {
@@ -47,9 +47,9 @@ struct RCCfg {
     } while (0)
 
 // Per (conv, tile) a 32 KB staging tile S carries both directions of HBM traffic through TMA: the producer loads the slice
-// of the NEXT chunk x_{j+2} into it, the epilogue reads its 16 channels from it and overwrites them with y_{j+1}, and warp 3
-// stores the tile to HBM.  (Measured: with one row per thread every global load / store instruction touches 32 different
-// cache lines, and the LSU wavefronts, not the tensor core, paced the kernel.)
+// of the NEXT chunk x_{j+2} into it, the epilogue reads its values from it and overwrites them with y_{j+1}, and warp 3
+// stores the tile to HBM.  Two staging tiles serve the (up to) three output tiles of a conv: tiles 0 and 1 run their epilogues
+// together, tile 2 after them.
 template <int NSPLIT>
 __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_constant__ Res2ChainParams cp) {
     using Cfg = RCCfg<NSPLIT>;
@@ -61,15 +61,10 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
     const uint32_t w_base = a_base + Cfg::A_BYTES;
     const uint32_t s_base = w_base + Cfg::W_SLOT;
     const uint32_t bar_base = s_base + 2 * Cfg::S_BYTES;
-    const uint32_t x_full = bar_base, a_ready = bar_base + 8, a_free = bar_base + 16, x_free = bar_base + 24, w_full = bar_base + 32,
-                   w_empty = bar_base + 40;
+    const uint32_t x_full = bar_base, x_free = bar_base + 24, w_full = bar_base + 32, w_empty = bar_base + 40;
     auto s_full = [&](int i) { return bar_base + 48u + 8u * i; };
     auto s_empty = [&](int i) { return bar_base + 64u + 8u * i; };
     auto y_ready = [&](int i) { return bar_base + 80u + 8u * i; };
-    auto tfull = [&](int t) { return bar_base + 96u + 8u * t; };
-    auto tempty = [&](int t) { return bar_base + 120u + 8u * t; };
-    const uint32_t tmem_slot = bar_base + 144u;
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
@@ -81,30 +76,17 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
     }
     if (warp == 1 && lane == 0) {
         mbar_init(x_full, 1);
-        mbar_init(a_ready, RC_EPI_THREADS);
-        mbar_init(a_free, 1);
         mbar_init(x_free, 1);
         mbar_init(w_full, 1);
         mbar_init(w_empty, 1);
         for (int i = 0; i < 2; ++i) {
             mbar_init(s_full(i), 1);
             mbar_init(s_empty(i), 1);
-            mbar_init(y_ready(i), RC_EPI_THREADS);
-        }
-        for (int t = 0; t < RC_MAX_TILES; ++t) {
-            mbar_init(tfull(t), 1);
-            mbar_init(tempty(t), RC_EPI_THREADS);
+            mbar_init(y_ready(i), 128);  // the warpgroup of the tile
         }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, 512);  // 3 accumulator tiles x (64 + 64) columns: [A_hi W_hi + A_lo W_hi | A_hi W_lo]
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
     griddep_launch_dependents();
     const int nconv = cp.nconv, ntiles = cp.ntiles;
 
@@ -142,57 +124,6 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // split-bf16 product as TWO instructions per k-step (see conv3x3.cu): A_hi x [W_hi | W_lo] with N = 128 -- the hi and lo weight
-        // tiles of a tap are adjacent in shared memory -- and A_lo x W_hi with N = 64; an N = 64 MMA is bound by its A-operand read,
-        // so the N = 128 one costs the same.  The epilogue adds the two 64-column blocks.
-        constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM, BN), idesc2 = make_idesc_bf16(GEMM_BM, 2 * BN);
-        int g = 0, u = 0;
-        uint32_t aready_count = 0;
-        for (int b = blockIdx.x; b < cp.B; b += gridDim.x, ++u) {
-            for (int j = 0; j < nconv; ++j, ++g) {
-                if (j == 0) mbar_wait(x_full, uint32_t(u) & 1u);
-                mbar_wait(a_ready, aready_count & 1u);  // conv 0: reflect halo rows of the TMA-loaded tile are in place; else: operand rewritten
-                ++aready_count;
-                if (lane == 0) RC_STAMP(1, j, 0);  // operand ready
-                mbar_wait(w_full, uint32_t(g) & 1u);
-                if (lane == 0) RC_STAMP(1, j, 1);  // weights ready
-                tc_fence_after();
-                for (int t = 0; t < ntiles; ++t) {
-                    if (g > 0) mbar_wait(tempty(t), uint32_t(g - 1) & 1u);  // epilogue drained this accumulator
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t d_tmem = tmem_base + t * 2 * BN;
-                        uint32_t accumulate = 0;
-#pragma unroll
-                        for (int tap = 0; tap < 3; ++tap) {
-                            const uint32_t roff = uint32_t(t * GEMM_BM + RC_PAD + (tap - 1) * cp.dil);
-                            const uint64_t a_hi = make_sw128_kmajor_desc(a_base + roff * 128u);
-                            const uint64_t b_hi = make_sw128_kmajor_desc(w_base + (tap * NP) * RC_W_TILE);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                umma_bf16(d_tmem, a_hi + 2 * k, b_hi + 2 * k, NSPLIT == 3 ? idesc2 : idesc, accumulate);
-                                accumulate = 1;
-                            }
-                            if (NSPLIT == 3) {
-                                const uint64_t a_lo = make_sw128_kmajor_desc(a_base + RC_A_PLANE + roff * 128u);
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-                            }
-                        }
-                        umma_commit(tfull(t));
-                        RC_STAMP(1, j, 2 + t);  // tile t issued
-                    }
-                    __syncwarp();
-                }
-                if (lane == 0) {
-                    umma_commit(w_empty);  // weight slot reusable
-                    if (j == nconv - 1) umma_commit(x_free);
-                }
-                __syncwarp();
-            }
-        }
     } else if (warp == 3) {
         // ===================== store warp: staging tile -> HBM =====================
         if (lane == 0) {
@@ -214,21 +145,22 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
             bulk_wait_all();
         }
     } else if (warp >= 4) {
-        // ===================== epilogue: 16 warps, each thread one row x 16 channels =====================
-        const int q = warp & 3, cq = (warp - 4) >> 2;
-        const int c0 = cq * 16;
+        // ===================== MMA + epilogue: warpgroup tw owns output tile tw of the utterance =====================
+        const int tw = (warp - 4) >> 2, tid = threadIdx.x & 127, w = tid >> 5, l = tid & 31;
+        const int e = threadIdx.x - 128;  // 0 .. RC_MMA_THREADS - 1
+        const bool has_tile = tw < ntiles;
         griddep_wait();
-        uint32_t g = 0, sn = 0;
         uint8_t* const a_gen = smem_gen;  // a_base == smem_base
         uint8_t* const s_gen = smem_gen + (s_base - smem_base);
-        const int rloc = q * 32 + lane;  // row inside the tile == TMEM lane
-        uint32_t ucount = 0;
+        float acc0[BN / 2], acc1[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+        uint32_t g = 0, ucount = 0;
         for (int b = blockIdx.x; b < cp.B; b += gridDim.x, ++ucount) {
             {
-                // The producing GEMM stores valid frames only (TMA-store epilogue): build the reflect halo rows of the resident
-                // tile here -- 2 P rows x 8 chunks x planes, one 16-byte copy per thread, in the swizzled layout.
+                // The producing GEMM stores valid frames only: build the reflect halo rows of the resident tile here --
+                // 2 P rows x 8 chunks x planes, one 16-byte copy per thread, in the swizzled layout.
                 mbar_wait(x_full, ucount & 1u);
-                const int e = threadIdx.x - 128;
                 if (e < 2 * cp.P * 8 * NP) {
                     const int pl = e / (2 * cp.P * 8), r = (e / 8) % (2 * cp.P), c = e % 8;
                     const int k = (r % cp.P) + 1;
@@ -237,114 +169,119 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
                     *reinterpret_cast<uint4*>(a_gen + pl * RC_A_PLANE + dst * 128 + ((c ^ (dst & 7)) << 4)) = val;
                 }
                 fence_proxy_async_smem();
-                mbar_arrive(a_ready);
+                named_bar_sync(1, RC_MMA_THREADS);
             }
             for (int j = 0; j < nconv; ++j, ++g) {
-                const float* bias = cp.bias[j] + c0;
-                const float* bsc = cp.bn_scale[j] + c0;
-                const float* bsh = cp.bn_shift[j] + c0;
+                mbar_wait(w_full, g & 1u);
+                if (tid == 0 && tw == 0) RC_STAMP(1, j, 1);  // weights ready
+                if (has_tile) {
+                    wgmma_fence_acc(acc0);
+                    wgmma_fence_acc(acc1);
+                    wgmma_fence();
+                    auto issue = [&](float (&acc)[BN / 2], int mb) {
+#pragma unroll
+                        for (int tap = 0; tap < 3; ++tap) {
+                            const uint32_t roff = uint32_t(tw * GEMM_BM + mb * 64 + RC_PAD + (tap - 1) * cp.dil);
+                            const uint64_t a_hi = make_sw128_kmajor_desc(a_base + roff * 128u);
+                            const uint64_t b_hi = make_sw128_kmajor_desc(w_base + (tap * NP) * RC_W_TILE);
+#pragma unroll
+                            for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (tap > 0 || k > 0) ? 1u : 0u);
+                            if (NSPLIT == 3) {
+                                const uint64_t a_lo = make_sw128_kmajor_desc(a_base + RC_A_PLANE + roff * 128u);
+                                const uint64_t b_lo = make_sw128_kmajor_desc(w_base + (tap * NP + 1) * RC_W_TILE);
+#pragma unroll
+                                for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+#pragma unroll
+                                for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
+                            }
+                        }
+                    };
+                    issue(acc0, 0);
+                    issue(acc1, 1);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_acc(acc0);
+                    wgmma_fence_acc(acc1);
+                }
+                // every MMA of this conv has read the operand tile and the weights: both may be overwritten now
+                named_bar_sync(1, RC_MMA_THREADS);
+                if (e == 0) {
+                    RC_STAMP(1, j, 2);
+                    mbar_arrive(w_empty);
+                    if (j == nconv - 1) mbar_arrive(x_free);
+                }
+                const float* bias = cp.bias[j];
+                const float* bsc = cp.bn_scale[j];
+                const float* bsh = cp.bn_shift[j];
                 const bool has_next = j + 1 < nconv;
-                for (int t = 0; t < ntiles; ++t, ++sn) {
-                    const int p = t * GEMM_BM + rloc;  // padded row inside the utterance
-                    const int tt = p - cp.P;
-                    const bool valid = tt >= 0 && tt < cp.T;
-                    const int i = sn & 1;
-                    uint8_t* const srow = s_gen + i * Cfg::S_BYTES + rloc * 128;
-                    const int ch0 = ((cq * 2) ^ (rloc & 7)) << 4, ch1 = ((cq * 2 + 1) ^ (rloc & 7)) << 4;  // SWIZZLE_128B chunk offsets
-                    mbar_wait(s_full(i), (sn >> 1) & 1u);
-                    uint4 nh[2], nl[2];
-                    if (has_next) {
-                        nh[0] = *reinterpret_cast<const uint4*>(srow + ch0);
-                        nh[1] = *reinterpret_cast<const uint4*>(srow + ch1);
-                        if (NP == 2) {
-                            nl[0] = *reinterpret_cast<const uint4*>(srow + RC_S_PLANE + ch0);
-                            nl[1] = *reinterpret_cast<const uint4*>(srow + RC_S_PLANE + ch1);
-                        } else {
-                            nl[0] = nl[1] = make_uint4(0, 0, 0, 0);
-                        }
-                    }
-                    mbar_wait(tfull(t), g & 1u);
-                    if (threadIdx.x == 128) RC_STAMP(2, j, t);  // accumulator t complete
-                    tc_fence_after();
-                    uint32_t v[16];
-                    __syncwarp();
-                    tmem_ld16(tmem_base + t * 2 * BN + c0 + (uint32_t(q * 32) << 16), v);
-                    if (NSPLIT == 3) {  // + the A_hi W_lo block
-                        uint32_t v2[16];
-                        tmem_ld16(tmem_base + t * 2 * BN + BN + c0 + (uint32_t(q * 32) << 16), v2);
-                        tmem_ld_wait();
+                const uint32_t sn = g * uint32_t(ntiles) + uint32_t(tw);
+                const int i = sn & 1;
+                uint8_t* const sbuf = s_gen + i * Cfg::S_BYTES;
+                auto epilogue = [&](const float (&acc)[BN / 2], int mb) {
 #pragma unroll
-                        for (int k = 0; k < 16; ++k) v[k] = __float_as_uint(__uint_as_float(v[k]) + __uint_as_float(v2[k]));
-                    }
-                    tmem_ld_wait();
-                    tc_fence_before();
-                    mbar_arrive(tempty(t));  // values are in registers: the accumulator may be reused
-                    float x[16];
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {  // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
-                        const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias) + k);
-                        const float4 s4 = __ldg(reinterpret_cast<const float4*>(bsc) + k);
-                        const float4 h4 = __ldg(reinterpret_cast<const float4*>(bsh) + k);
-                        x[4 * k + 0] = fmaf(fmaxf(__uint_as_float(v[4 * k + 0]) + b4.x, 0.f), s4.x, h4.x);
-                        x[4 * k + 1] = fmaf(fmaxf(__uint_as_float(v[4 * k + 1]) + b4.y, 0.f), s4.y, h4.y);
-                        x[4 * k + 2] = fmaf(fmaxf(__uint_as_float(v[4 * k + 2]) + b4.z, 0.f), s4.z, h4.z);
-                        x[4 * k + 3] = fmaf(fmaxf(__uint_as_float(v[4 * k + 3]) + b4.w, 0.f), s4.w, h4.w);
-                    }
-                    {  // y_{j+1} -> staging tile (every row: rows outside the valid frames are halo / padding rows of the y buffer)
-                        uint32_t h[8], l[8];
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) split_pack_bf16x2(x[2 * k], x[2 * k + 1], h[k], l[k]);
-                        *reinterpret_cast<uint4*>(srow + ch0) = make_uint4(h[0], h[1], h[2], h[3]);
-                        *reinterpret_cast<uint4*>(srow + ch1) = make_uint4(h[4], h[5], h[6], h[7]);
-                        if (NP == 2) {
-                            *reinterpret_cast<uint4*>(srow + RC_S_PLANE + ch0) = make_uint4(l[0], l[1], l[2], l[3]);
-                            *reinterpret_cast<uint4*>(srow + RC_S_PLANE + ch1) = make_uint4(l[4], l[5], l[6], l[7]);
-                        }
-                        fence_proxy_async_smem();
-                        mbar_arrive(y_ready(i));
-                    }
-                    // The resident tile is rewritten IN PLACE while later tiles of this conv are still being multiplied: the MMAs of
-                    // tiles <= t are complete (tfull(t) was committed after them), and those of tile t+1 read this tile's last
-                    // `dil` rows only.  So only the warps holding those rows (lane quarter 3) wait for tile t+1 -- which every
-                    // warp is about to wait for anyway -- and nobody waits for the whole conv.
-                    if (has_next && q == 3 && t + 1 < ntiles) mbar_wait(tfull(t + 1), g & 1u);
-                    if (threadIdx.x == 128) RC_STAMP(2, j, 3 + (t > 0));
-                    if (has_next && valid) {  // x_{j+2} + y_{j+1} -> operand of the next conv, in place, with its reflect halo rows
+                    for (int h = 0; h < 2; ++h) {
+                        const int rloc = mb * 64 + 16 * w + (l >> 2) + 8 * h;  // row inside the 128-row tile
+                        const int p = tw * GEMM_BM + rloc;                      // padded row inside the utterance
+                        const int tt = p - cp.P;
+                        const bool valid = tt >= 0 && tt < cp.T;
                         int rows[3] = {p + RC_PAD, -1, -1};
                         if (tt >= 1 && tt <= cp.P) rows[1] = cp.P - tt + RC_PAD;
                         const int uu = cp.T - 1 - tt;
                         if (uu >= 1 && uu <= cp.P) rows[2] = cp.P + cp.T - 1 + uu + RC_PAD;
 #pragma unroll
-                        for (int k = 0; k < 2; ++k) {
-                            const uint32_t hw[4] = {nh[k].x, nh[k].y, nh[k].z, nh[k].w}, lw[4] = {nl[k].x, nl[k].y, nl[k].z, nl[k].w};
-                            uint32_t oh[4], ol[4];
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 hf = unpack_bf16x2(hw[e]), lf = unpack_bf16x2(lw[e]);
-                                split_pack_bf16x2(x[8 * k + 2 * e] + (hf.x + lf.x), x[8 * k + 2 * e + 1] + (hf.y + lf.y), oh[e], ol[e]);
+                        for (int q = 0; q < BN / 8; ++q) {
+                            const int col = 8 * q + 2 * (l & 3);
+                            const int off = ((q ^ (rloc & 7)) << 4) + 4 * (l & 3);  // SWIZZLE_128B: 16-byte chunk q of the row
+                            // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
+                            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+                            const float2 s2 = __ldg(reinterpret_cast<const float2*>(bsc + col));
+                            const float2 h2 = __ldg(reinterpret_cast<const float2*>(bsh + col));
+                            const float x0 = fmaf(fmaxf(acc[4 * q + 2 * h] + b2.x, 0.f), s2.x, h2.x);
+                            const float x1 = fmaf(fmaxf(acc[4 * q + 2 * h + 1] + b2.y, 0.f), s2.y, h2.y);
+                            uint32_t nh = 0, nl = 0;
+                            if (has_next) {
+                                nh = *reinterpret_cast<const uint32_t*>(sbuf + rloc * 128 + off);
+                                if (NP == 2) nl = *reinterpret_cast<const uint32_t*>(sbuf + RC_S_PLANE + rloc * 128 + off);
                             }
+                            uint32_t yh, yl;  // y_{j+1} -> staging tile (every row: rows outside the valid frames are halo / padding rows of y)
+                            split_pack_bf16x2(x0, x1, yh, yl);
+                            *reinterpret_cast<uint32_t*>(sbuf + rloc * 128 + off) = yh;
+                            if (NP == 2) *reinterpret_cast<uint32_t*>(sbuf + RC_S_PLANE + rloc * 128 + off) = yl;
+                            if (has_next && valid) {  // x_{j+2} + y_{j+1} -> operand of the next conv, in place, with its reflect halo rows
+                                const float2 hf = unpack_bf16x2(nh), lf = unpack_bf16x2(nl);
+                                uint32_t oh, ol;
+                                split_pack_bf16x2(x0 + (hf.x + lf.x), x1 + (hf.y + lf.y), oh, ol);
 #pragma unroll
-                            for (int r = 0; r < 3; ++r) {
-                                if (rows[r] < 0) continue;
-                                const int chunk = ((cq * 2 + k) ^ (rows[r] & 7)) << 4;
-                                uint8_t* dst = a_gen + rows[r] * 128 + chunk;
-                                *reinterpret_cast<uint4*>(dst) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-                                if (NP == 2) *reinterpret_cast<uint4*>(dst + RC_A_PLANE) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+                                for (int r = 0; r < 3; ++r) {
+                                    if (rows[r] < 0) continue;
+                                    uint8_t* dst = a_gen + rows[r] * 128 + ((q ^ (rows[r] & 7)) << 4) + 4 * (l & 3);
+                                    *reinterpret_cast<uint32_t*>(dst) = oh;
+                                    if (NP == 2) *reinterpret_cast<uint32_t*>(dst + RC_A_PLANE) = ol;
+                                }
                             }
                         }
                     }
+                };
+                // tiles 0 and 1 use the two staging tiles, tile 2 reuses the first one after them
+#pragma unroll 1
+                for (int round = 0; round < 2; ++round) {
+                    if (has_tile && (tw == 2) == (round == 1)) {
+                        mbar_wait(s_full(i), (sn >> 1) & 1u);
+                        epilogue(acc0, 0);
+                        epilogue(acc1, 1);
+                        fence_proxy_async_smem();
+                        mbar_arrive(y_ready(i));
+                    }
+                    if (ntiles > 2 && round == 0) named_bar_sync(2, RC_MMA_THREADS);
                 }
-                if (threadIdx.x == 128) RC_STAMP(2, j, 5);  // all tiles written back
+                if (tid == 0 && tw == 0) RC_STAMP(2, j, 5);  // all tiles written back
                 if (has_next) {
                     fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-                    mbar_arrive(a_ready);
+                    named_bar_sync(1, RC_MMA_THREADS);
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 int res2chain_build(Res2ChainParams* cp, const Planes& x, const Planes& y, const Planes* W, const float* const* bias, const float* const* bn_scale,

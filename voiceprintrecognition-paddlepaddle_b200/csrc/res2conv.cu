@@ -1,15 +1,14 @@
 // Res2Net dilated conv (K3): y_j = BN(ReLU(conv_k3,d(x_j + y_{j-1}))) for one 64-channel chunk.
 // Reference: ppvector/models/ecapa_tdnn.py:36-47 (Res2NetBlock.forward) -> TDNNBlock (ppvector/models/utils.py:147).
 //
-// Same contraction as gemm_tcgen05.cu (N = 64, K = nsrc * 3 taps * 64), restructured around what bounds it -- the
+// Same contraction as gemm_wgmma.cu (N = 64, K = nsrc * 3 taps * 64), restructured around what bounds it -- the
 // L2 -> shared-memory fill, not the tensor pipe:
 //   * the whole weight matrix of the layer (<= 6 k-slices x hi/lo = 96 KB) is loaded ONCE per CTA and stays in
 //     shared memory for all of the CTA's tiles (weight-stationary);
 //   * per source (x_j, y_{j-1}) ONE tall activation tile of 128 + 2*4 rows is loaded per output tile; the three
-//     conv taps are the SAME shared-memory tile read at row offsets 4-d, 4, 4+d: the UMMA descriptor's start
-//     address simply moves by whole 128-byte rows.  Measured on B200: the SWIZZLE_128B XOR phase is a function of the
-//     absolute shared-memory address (bits [7,10)), exactly as TMA wrote it, so any row of a 1024-byte-aligned slot is a
-//     valid matrix start with base_offset = 0 (setting base_offset = row mod 8 gives WRONG results).
+//     conv taps are the SAME shared-memory tile read at row offsets 4-d, 4, 4+d: the wgmma descriptor's start
+//     address simply moves by whole 128-byte rows (the SWIZZLE_128B XOR is a function of the absolute shared-memory
+//     address, exactly as TMA wrote it, so any row of a 1024-byte-aligned slot is a valid matrix start).
 // L2 -> SM traffic per 128-row tile: 2 x 2 x 17 KB = 70 KB instead of 288 KB.
 #include <stdio.h>
 #include <stdlib.h>
@@ -36,31 +35,18 @@ struct R2Cfg {
     static constexpr int SMEM_BYTES = 1024 + W_BYTES + STAGES * STAGE_BYTES + 256;
 };
 
-// descriptor for rows [roff, roff+128) of a tall SWIZZLE_128B tile whose slot is 1024-byte aligned
-__device__ __forceinline__ uint64_t tall_tile_desc(uint32_t slot_addr, int roff) {
-    // The 128B-swizzle XOR is a function of the absolute shared-memory address bits [7,10) (as TMA wrote it), so a
-    // row-shifted start address needs no base_offset as long as the slot itself is 1024-byte aligned.
-    const uint32_t addr = slot_addr + uint32_t(roff) * 128u;
-    return make_sw128_kmajor_desc(addr);
-}
-
 template <int NSPLIT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) res2conv_kernel(const __grid_constant__ Res2Params rp) {
     using Cfg = R2Cfg<NSPLIT>;
     constexpr int NP = Cfg::NP, STAGES = Cfg::STAGES, BN = 64;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t w_base = smem_base;
     const uint32_t a_base = smem_base + Cfg::W_BYTES;
     const uint32_t bar_base = a_base + STAGES * Cfg::STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-    auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-    const uint32_t w_full = bar_base + 8u * (2 * STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 5);
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
+    const uint32_t w_full = bar_base + 8u * (2 * STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
@@ -71,23 +57,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) res2conv_kernel(const __grid_
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull_bar(a), 1);
-            mbar_init(tempty_bar(a), EPI_WARP_ARRIVALS);
+            mbar_init(empty_bar(s), GEMM_MMA_THREADS / 128);  // one arrival per MMA warpgroup
         }
         mbar_init(w_full, 1);
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, 2 * BN);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
     const int nsrc = rp.nsrc;
     const int wslices = nsrc * 3;
     griddep_launch_dependents();  // PDL
@@ -126,69 +101,56 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) res2conv_kernel(const __grid_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM, BN);
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup g owns rows [64 g, 64 g + 64) of every tile =====================
+        const int g = (warp - 4) >> 2, t = threadIdx.x & 127;
+        griddep_wait();  // the epilogue writes buffers that upstream kernels may still be reading
         mbar_wait(w_full, 0);
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_phase = 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         for (int tile = blockIdx.x; tile < rp.m_tiles; tile += gridDim.x) {
-            mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * BN;
-            uint32_t accumulate = 0;
+            int prev = -1;
+            wgmma_fence_acc(acc);
             for (int s = 0; s < nsrc; ++s) {
                 mbar_wait(full_bar(stage), phase);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t slot = a_base + stage * Cfg::STAGE_BYTES;
+                const uint32_t slot = a_base + stage * Cfg::STAGE_BYTES;
+                wgmma_fence();
 #pragma unroll
-                    for (int tap = 0; tap < 3; ++tap) {
-                        const int roff = R2_PAD + (tap - 1) * rp.dil;
-                        const uint64_t a_hi = tall_tile_desc(slot, roff);
-                        const uint64_t b_hi = make_sw128_kmajor_desc(w_base + ((s * 3 + tap) * NP) * R2_W_TILE);
+                for (int tap = 0; tap < 3; ++tap) {
+                    // rows [roff, roff + 64) of the tall tile: whole 128-byte rows of a 1024-byte-aligned slot
+                    const uint32_t roff = uint32_t(R2_PAD + (tap - 1) * rp.dil + 64 * g);
+                    const uint64_t a_hi = make_sw128_kmajor_desc(slot + roff * 128u);
+                    const uint64_t b_hi = make_sw128_kmajor_desc(w_base + ((s * 3 + tap) * NP) * R2_W_TILE);
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            umma_bf16(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc, accumulate);
-                            accumulate = 1;
-                        }
-                        if (NSPLIT == 3) {
-                            const uint64_t a_lo = tall_tile_desc(slot + R2_A_SLOT, roff);
-                            const uint64_t b_lo = make_sw128_kmajor_desc(w_base + ((s * 3 + tap) * NP + 1) * R2_W_TILE);
+                    for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (s > 0 || tap > 0 || k > 0) ? 1u : 0u);
+                    if (NSPLIT == 3) {
+                        const uint64_t a_lo = make_sw128_kmajor_desc(slot + R2_A_SLOT + roff * 128u);
+                        const uint64_t b_lo = make_sw128_kmajor_desc(w_base + ((s * 3 + tap) * NP + 1) * R2_W_TILE);
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
+                        for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-                        }
+                        for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
                     }
-                    umma_commit(empty_bar(stage));
-                    if (s == nsrc - 1) umma_commit(tfull_bar(acc));
                 }
-                __syncwarp();
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+                prev = stage;
                 if (++stage == STAGES) {
                     stage = 0;
                     phase ^= 1u;
                 }
             }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue (shared with the gather-GEMM) =====================
-        const int q = warp & 3, etid = threadIdx.x - 128, ehalf = (warp - 4) >> 2;
-        griddep_wait();  // the epilogue writes buffers that upstream kernels may still be reading
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x; tile < rp.m_tiles; tile += gridDim.x) {
-            epilogue_tile<BN>(rp.epi, nullptr, rp.M, BN, tile * GEMM_BM, 0, tmem_base + acc * BN, tfull_bar(acc), acc_phase, tempty_bar(acc),
-                              q, lane, ehalf, etid, 0u, nullptr);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (t == 0) mbar_arrive(empty_bar(prev));
+            const int rbase = tile * GEMM_BM + 64 * g;
+            epilogue_frag<BN>(rp.epi, BN, 0, acc, [&](int r) -> int64_t { return rbase + r < rp.M ? int64_t(rbase + r) : -1; }, t);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 2 * BN);
 }
 
 int res2conv_build(Res2Params* rp, const GemmSource* srcs, int nsrc, const Planes& W, int M, int dil, const Epilogue& epi) {

@@ -55,7 +55,7 @@ struct ResNetSEModel {
     WeightMap raw;
     bool finalized = false;
     int precision = PPV_PREC_BF16X3;
-    int num_sms = 148;
+    int num_sms = 132;
     void* arena = nullptr;
     // weights
     float* conv1_w = nullptr;  // [32][9] BN folded
@@ -178,7 +178,7 @@ int launch_flatten_image(const Planes& in, int B, int H, int W, int Hp, int Wp, 
 }
 int launch_image_to_f32(const Planes& in, int B, int H, int W, int Hp, int Wp, int C, float* out, cudaStream_t st) {
     const int64_t total = int64_t(B) * H * W * C;
-    rs_image_to_f32_kernel<<<int(std::min<int64_t>((total + 255) / 256, 148 * 32)), 256, 0, st>>>(in, B, H, W, Hp, Wp, C, out);
+    rs_image_to_f32_kernel<<<int(std::min<int64_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(in, B, H, W, Hp, Wp, C, out);
     PPV_LAUNCH_OK("rs_image_to_f32_kernel");
     return PPV_OK;
 }
@@ -740,7 +740,7 @@ int resnetse_read_tap(ResNetSEModel* m, const char* name, float* out, size_t out
     const Geo& g = m->geo[stage];
     const int64_t total = int64_t(B) * g.H * g.W * C;
     PPV_REQUIRE(out_elems >= size_t(total), "resnetse_read_tap: output too small");
-    rs_image_to_f32_kernel<<<int(std::min<int64_t>((total + 255) / 256, 148 * 32)), 256, 0, st>>>(src, B, g.H, g.W, g.Hp, g.Wp, C, out);
+    rs_image_to_f32_kernel<<<int(std::min<int64_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(src, B, g.H, g.W, g.Hp, g.Wp, C, out);
     PPV_LAUNCH_OK("rs_image_to_f32_kernel");
     return PPV_OK;
 }

@@ -2,9 +2,8 @@
 // excitation MLP (ppvector/models/ecapa_tdnn.py:79-80), ASP's global-context bias and the final fc of EcapaTdnn.forward
 // (ecapa_tdnn.py:274), each [256 x K] x [K x N] with K <= 3072, N <= 512.
 //
-// On the tensor-core gather-GEMM these layers occupy 2-6 CTAs and take 20-35 us each (eight launches = 200 us of a 3.1 ms step,
-// measured: profiles/launches_r1_final_summary.txt): with M = 256 rows there are only two 128-row tiles, and the k-loop is a
-// latency chain.  They are 17-150 MFLOP: here every SM takes a 16 x 16 output tile and walks K on the CUDA cores with fp32 FMAs over
+// On the tensor-core gather-GEMM these layers would occupy 2-6 CTAs: with M = 256 rows there are only two 128-row tiles, and the
+// k-loop is a latency chain.  They are 17-150 MFLOP: here every SM takes a 16 x 16 output tile and walks K on the CUDA cores with fp32 FMAs over
 // the exact hi + lo values of the split-bf16 operands (at least as accurate as the three-product tensor path).  128-192 CTAs, no
 // split-K, no atomics: deterministic.
 #include "common.h"
@@ -106,9 +105,7 @@ __global__ void __launch_bounds__(256) skinny_linear_kernel(Planes x, int x_col0
 
 }  // namespace
 
-// K <= 1024: with 16 x 16 output tiles every CTA re-reads 32 operand rows, so the L2 -> SM traffic is M N K / 2 bytes: measured on B200 the
-// K = 3072 layers (ASP context bias, fc) take 30 / 51 us here against 35 / 31 us on the tensor cores, the K <= 512 SE layers 8 / 10 us
-// against 20 / 24 us.
+// K <= 1024: with 16 x 16 output tiles every CTA re-reads 32 operand rows, so the L2 -> SM traffic is M N K / 2 bytes.
 bool skinny_linear_supported(int M, int N, int K, const Epilogue& ep) {
     return M <= 4096 && K % 8 == 0 && K <= 1024 && !ep.rowgrp_bias && !ep.seg_scale && !ep.bn_scale && !ep.tanh_ && !ep.silu_ && ep.Tp == 0 && ep.img_Wp == 0 &&
            ep.relu_max == 0.f;

@@ -35,7 +35,7 @@ class WaveAugmentor:
         self.speed, self.volume, self.noise = _conf(conf.get('speed')), _conf(conf.get('volume')), _conf(conf.get('noise'))
         reverb = _conf(conf.get('reverb'))
         if reverb and reverb.get('prob', 0) > 0 and os.path.isdir(str(reverb.get('reverb_dir', ''))) and os.listdir(reverb['reverb_dir']):
-            raise NotImplementedError('reverb augmentation is not implemented on the B200 path; set reverb.prob to 0')
+            raise NotImplementedError('reverb augmentation is not implemented on the H100 path; set reverb.prob to 0')
         self.num_speakers = num_speakers
         self.device = torch.device(device)
         self.noise_bank, self.noise_clips = None, []

@@ -50,7 +50,7 @@ class AudioFeaturizer(torch.nn.Module):
                 cfg.htk = int(bool(v))
             elif k == 'norm':
                 if v not in ('slaney', None):
-                    raise _lib.PPVError(f'{method}: norm={v!r} is not supported by the B200 kernel (slaney or None)')
+                    raise _lib.PPVError(f'{method}: norm={v!r} is not supported by the CUDA kernel (slaney or None)')
                 cfg.norm_slaney = int(v == 'slaney')
             elif k == 'center':
                 cfg.center = int(bool(v))
@@ -58,7 +58,7 @@ class AudioFeaturizer(torch.nn.Module):
                     or k == 'top_db' and v is None:
                 pass
             else:
-                raise _lib.PPVError(f'{method} argument {k}={v!r} is not supported by the B200 kernel')
+                raise _lib.PPVError(f'{method} argument {k}={v!r} is not supported by the CUDA kernel')
         return cfg
 
     @staticmethod
@@ -73,7 +73,7 @@ class AudioFeaturizer(torch.nn.Module):
                  'high_freq': 'high_freq'}
         for k, v in args.items():
             if k not in known:
-                raise _lib.PPVError(f'Fbank argument {k!r} is not supported by the B200 kernel')
+                raise _lib.PPVError(f'Fbank argument {k!r} is not supported by the CUDA kernel')
             setattr(cfg, known[k], type(getattr(cfg, known[k]))(v))
         return cfg
 

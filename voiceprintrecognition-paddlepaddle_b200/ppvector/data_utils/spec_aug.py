@@ -19,7 +19,7 @@ class SpecAugmentor:
     def __init__(self, prob=0.5, freq_mask_ratio=0.15, n_freq_masks=2, time_mask_ratio=0.05, n_time_masks=2, inplace=True,
                  max_time_warp=0, replace_with_zero=True):
         if max_time_warp:
-            raise NotImplementedError('SpecAugmentor on B200: max_time_warp must be 0 (configs/augmentation.yml:48)')
+            raise NotImplementedError('SpecAugmentor on the H100 path: max_time_warp must be 0 (configs/augmentation.yml:48)')
         if 2 + 2 * (n_freq_masks + n_time_masks) > _lib.PPV_SPECAUG_NPARAM:
             raise ValueError('too many masks')
         self.prob, self.freq_mask_ratio, self.n_freq_masks = prob, freq_mask_ratio, n_freq_masks

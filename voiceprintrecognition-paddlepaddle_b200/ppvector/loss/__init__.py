@@ -17,7 +17,7 @@ def build_loss(configs):
     name = configs.loss_conf.get('loss', 'AAMLoss')
     kwargs = dict(configs.loss_conf.get('loss_args', {}) or {})
     if name not in _IMPLEMENTED:
-        hint = 'exists in the reference but is not implemented on the B200 path' if name in _REFERENCE_ONLY else 'is not a known loss'
+        hint = 'exists in the reference but is not implemented on the H100 path' if name in _REFERENCE_ONLY else 'is not a known loss'
         raise NotImplementedError(f'loss {name!r} {hint} (implemented: {sorted(_IMPLEMENTED)})')
     loss = _IMPLEMENTED[name](**kwargs)
     logger.info(f'loss: {name} {kwargs}')

@@ -78,7 +78,7 @@ class AAMLoss(nn.Module):
         features = inputs['features']
         weight = inputs.get('_weight')
         if weight is None:
-            raise _lib.PPVError("AAMLoss on B200 needs the classifier weight: pass SpeakerIdentification's output dict")
+            raise _lib.PPVError("AAMLoss on the H100 path needs the classifier weight: pass SpeakerIdentification's output dict")
         return _AAMFunction.apply(features, weight, labels, self.margin, self.scale, self.easy_margin, self.label_smoothing)
 
     def update(self, margin=0.2):

@@ -28,7 +28,7 @@ class _MarginHead(nn.Module):
     def forward(self, inputs, labels):
         weight = inputs.get('_weight')
         if weight is None:
-            raise _lib.PPVError(f"{type(self).__name__} on B200 needs the classifier weight: pass SpeakerIdentification's output dict")
+            raise _lib.PPVError(f"{type(self).__name__} on the H100 path needs the classifier weight: pass SpeakerIdentification's output dict")
         return _AAMFunction.apply(inputs['features'], weight, labels, self.margin, self.scale, self.head, self.label_smoothing)
 
     def update(self, margin=0.2):

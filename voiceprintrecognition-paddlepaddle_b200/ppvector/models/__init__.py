@@ -19,7 +19,7 @@ def build_model(input_size, configs):
     kwargs = dict(configs.model_conf.get('model_args', {}) or {})
     if name not in _BACKBONES:
         if name in _REFERENCE_ONLY:
-            raise NotImplementedError(f'{name} is not implemented on the B200 path (implemented: {sorted(_BACKBONES)}); there is no fallback')
+            raise NotImplementedError(f'{name} is not implemented on the H100 path (implemented: {sorted(_BACKBONES)}); there is no fallback')
         raise Exception(f'unknown model {name!r}')
     model = _BACKBONES[name](input_size=input_size, **kwargs)
     logger.info(f'model: {name} {kwargs}')

@@ -75,7 +75,7 @@ class NativeBackbone(nn.Module):
         if lengths is not None:
             raise NotImplementedError('lengths masking is never used by the reference callers and is not implemented')
         if self.training:
-            raise _lib.PPVError(f'{type(self).__name__} on B200 implements the eval-mode forward only; call .eval()')
+            raise _lib.PPVError(f'{type(self).__name__} on the H100 path implements the eval-mode forward only; call .eval()')
         _lib.require_cuda(x, 'x')
         x = x.to(torch.float32).contiguous()
         B, T, F = x.shape

@@ -113,9 +113,9 @@ class CAMPPlus(NativeBackbone):
                  memory_efficient=True, precision='bf16x3'):
         super().__init__(precision)
         if config_str != 'batchnorm-relu':
-            raise NotImplementedError("CAMPPlus on B200 implements config_str='batchnorm-relu' (configs/cam++.yml)")
+            raise NotImplementedError("CAMPPlus on the H100 path implements config_str='batchnorm-relu' (configs/cam++.yml)")
         if (growth_rate, bn_size, init_channels) != (32, 4, 128):
-            raise NotImplementedError('CAMPPlus on B200 implements growth_rate=32, bn_size=4, init_channels=128 (configs/cam++.yml)')
+            raise NotImplementedError('CAMPPlus on the H100 path implements growth_rate=32, bn_size=4, init_channels=128 (configs/cam++.yml)')
         self.input_size, self.embd_dim = input_size, embd_dim
         self.growth_rate, self.bn_size, self.init_channels = growth_rate, bn_size, init_channels
         self.head = _FCM(feat_dim=input_size)

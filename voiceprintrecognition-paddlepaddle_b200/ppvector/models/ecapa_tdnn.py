@@ -2,7 +2,7 @@
 
 The module tree and parameter names equal the reference's Paddle ``state_dict`` (``blocks.0.conv.conv.weight``,
 ``blocks.1.res2net_block.blocks.3.norm.norm._variance`` ...), so reference checkpoints map 1:1.  The modules
-hold parameters only; ``forward`` is ONE call into libppv_b200 (``ppv_model_forward``): tcgen05/TMA gather-GEMMs
+hold parameters only; ``forward`` is ONE call into libppv_b200 (``ppv_model_forward``): wgmma/TMA gather-GEMMs
 with fused bias/ReLU/BatchNorm epilogues plus the SE / ASP reductions (csrc/ecapa.cu).  This module is the eval-mode
 forward; the training step (SURVEY.md §8 row a11) runs through ppvector/train_engine.py on the same parameter names.
 There is no torch fallback.
@@ -74,7 +74,7 @@ class SERes2NetBlock(nn.Module):
         self.tdnn2 = TDNNBlock(out_channels, out_channels, 1, 1)
         self.se_block = SEBlock(out_channels, se_channels, out_channels)
         if in_channels != out_channels:
-            raise NotImplementedError('SERes2NetBlock shortcut conv (in != out channels) is not implemented on B200')
+            raise NotImplementedError('SERes2NetBlock shortcut conv (in != out channels) is not implemented on the H100 path')
 
 
 class AttentiveStatisticsPooling(nn.Module):
@@ -153,9 +153,9 @@ class EcapaTdnn(NativeBackbone):
         if lengths is None:
             return super().forward(x)
         if self.pooling_type != "ASP":  # pooling.py:17,39,60: the other pooling layers accept and ignore `lengths`; SEBlock does not
-            raise NotImplementedError('lengths with pooling_type != "ASP" is not implemented on B200')
+            raise NotImplementedError('lengths with pooling_type != "ASP" is not implemented on the H100 path')
         if self.training:
-            raise _lib.PPVError('EcapaTdnn on B200 implements the eval-mode forward only; call .eval()')
+            raise _lib.PPVError('EcapaTdnn on the H100 path implements the eval-mode forward only; call .eval()')
         _lib.require_cuda(x, 'x')
         x = x.to(torch.float32).contiguous()
         B, T, F = x.shape

@@ -51,7 +51,7 @@ class ERes2Net(NativeBackbone):
         if pooling_type != 'TSTP':
             raise Exception(f'没有{pooling_type}池化层！')  # eres2net.py:218-221
         if (mul_channel, expansion, base_width, scale, two_emb_layer) != (1, 2, 32, 2, False):
-            raise NotImplementedError('ERes2Net on B200 implements mul_channel=1, expansion=2, base_width=32, scale=2, '
+            raise NotImplementedError('ERes2Net on the H100 path implements mul_channel=1, expansion=2, base_width=32, scale=2, '
                                       'two_emb_layer=False (configs/eres2net.yml)')
         self.input_size, self.embd_dim, self.m_channels, self.num_blocks = input_size, embd_dim, m_channels, list(num_blocks)
         self.in_planes = m_channels
@@ -110,7 +110,7 @@ class ERes2NetV2(NativeBackbone):
         if pooling_type != 'TSTP':
             raise Exception(f'没有{pooling_type}池化层！')  # eres2net.py:411-414
         if (expansion, scale, two_emb_layer) != (2, 2, False) or not 8 <= int(base_width) <= 32:
-            raise NotImplementedError('ERes2NetV2 on B200 implements expansion=2, scale=2, two_emb_layer=False, 8 <= base_width <= 32')
+            raise NotImplementedError('ERes2NetV2 on the H100 path implements expansion=2, scale=2, two_emb_layer=False, 8 <= base_width <= 32')
         self.input_size, self.embd_dim, self.m_channels, self.num_blocks = input_size, embd_dim, m_channels, list(num_blocks)
         self.base_width = int(base_width)
         self.in_planes = m_channels

@@ -33,7 +33,7 @@ class SpeakerIdentification(nn.Module):
     def __init__(self, input_dim, num_speakers, classifier_type='Cosine', K=1, num_blocks=0, inter_dim=512):
         super().__init__()
         if classifier_type != 'Cosine' or num_blocks != 0:
-            raise NotImplementedError('only classifier_type="Cosine" with num_blocks=0 is implemented on B200')
+            raise NotImplementedError('only classifier_type="Cosine" with num_blocks=0 is implemented on the H100 path')
         self.classifier_type = classifier_type
         # XavierUniform on a [input_dim, num_speakers*K] tensor (fc.py:31-33)
         bound = math.sqrt(6.0 / (input_dim + num_speakers * K))

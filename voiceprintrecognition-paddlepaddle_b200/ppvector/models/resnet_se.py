@@ -2,7 +2,7 @@
 
 Module tree / parameter names equal the reference's Paddle ``state_dict`` (``layer2.0.downsample.0.weight``,
 ``layer1.1.se.fc.2.bias``, ``pooling.tdnn.norm.norm._variance``, ``linear.weight`` [in,out] ...).  ``forward`` is one
-call into libppv_b200 (csrc/resnet_se.cu): 2-D convolutions as tcgen05 gather-GEMMs over zero-bordered NHWC images,
+call into libppv_b200 (csrc/resnet_se.cu): 2-D convolutions as wgmma gather-GEMMs over zero-bordered NHWC images,
 SE as column sums + two small GEMMs, the ASP head shared with ECAPA-TDNN.  Eval mode only."""
 import ctypes as C
 
@@ -77,7 +77,7 @@ class ResNetSE(NativeBackbone):
                  precision='bf16x3'):
         super().__init__(precision)
         if pooling_type != "ASP":
-            raise NotImplementedError(f'pooling_type {pooling_type} is not implemented on B200 (ASP only)')
+            raise NotImplementedError(f'pooling_type {pooling_type} is not implemented on the H100 path (ASP only)')
         self.input_size, self.embd_dim = input_size, embd_dim
         self.layers_cfg, self.num_filters = list(layers), list(num_filters)
         self.inplanes = num_filters[0]

@@ -13,7 +13,7 @@ def build_lr_scheduler(step_per_epoch, configs):
     use_scheduler = configs.optimizer_conf.get('scheduler', 'WarmupCosineSchedulerLR')
     scheduler_args = dict(configs.optimizer_conf.get('scheduler_args', {}))
     if use_scheduler != 'WarmupCosineSchedulerLR':
-        raise NotImplementedError(f'学习率衰减 {use_scheduler}: only WarmupCosineSchedulerLR is implemented on the B200 path')
+        raise NotImplementedError(f'学习率衰减 {use_scheduler}: only WarmupCosineSchedulerLR is implemented on the H100 path')
     scheduler_args.setdefault('fix_epoch', configs.train_conf.max_epoch)
     scheduler_args.setdefault('step_per_epoch', step_per_epoch)
     scheduler = cosine_decay_with_warmup(**scheduler_args)

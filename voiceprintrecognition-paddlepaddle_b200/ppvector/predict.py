@@ -6,7 +6,7 @@ Same constructor arguments and the same ``predict`` / ``predict_batch`` / ``cont
     embedding is ONE library call (``ppv_model_forward_wav``); the reference featurises per utterance in a Python
     loop and runs the model in chunks of 32 (predict.py:262-267);
   * cosine scoring runs on the GPU (``ppvector.metric.cosine``);
-  * ``use_gpu=False`` raises: the B200 build has no CPU path.
+  * ``use_gpu=False`` raises: this build has no CPU path.
 Not carried over (SURVEY.md §2 rows 12, 21: out of scope): the enrolment DB, recognition and diarization.
 """
 import os
@@ -31,7 +31,7 @@ class PPVectorPredictor:
                  use_gpu=True, state_dict=None):
         """reference: predict.py:25-67.  ``state_dict`` (extension): weights given in memory instead of a file."""
         if not use_gpu:
-            raise _lib.PPVError('use_gpu=False: the B200 build of ppvector has no CPU path')
+            raise _lib.PPVError('use_gpu=False: this build of ppvector has no CPU path')
         assert torch.cuda.is_available(), 'GPU不可用'
         self.device = torch.device('cuda', torch.cuda.current_device())
         self.threshold = threshold
@@ -54,7 +54,7 @@ class PPVectorPredictor:
         self._pinned = None
         self._pinned_out = None
         if audio_db_path is not None:
-            logger.warning('audio_db_path: the enrolment database is out of scope of the B200 hot path (ignored)')
+            logger.warning('audio_db_path: the enrolment database is out of scope of the CUDA hot path (ignored)')
 
     # ---- audio loading: predict.py:189-216 ----------------------------------------------------------------
     def _load_audio(self, audio_data, sample_rate=16000):

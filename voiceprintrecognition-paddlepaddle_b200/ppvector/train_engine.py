@@ -49,7 +49,7 @@ class TrainEngine:
             pass
 
     def set_precision(self, precision):
-        """'bf16x3' (default, fp32-grade split-bf16) or 'bf16' (single-pass bf16 operands: the B200 form of train_conf.enable_amp,
+        """'bf16x3' (default, fp32-grade split-bf16) or 'bf16' (single-pass bf16 operands: the single-pass bf16 form of train_conf.enable_amp,
         reference trainer.py:167, 209-229)."""
         prec = {'bf16x3': _lib.PPV_PREC_BF16X3, 'bf16': _lib.PPV_PREC_BF16}[precision]
         _lib.check(_lib.load().ppv_trainer_set_precision(self._h, prec), 'ppv_trainer_set_precision')

@@ -31,7 +31,7 @@ class PPVectorTrainer(object):
     def __init__(self, configs, use_gpu=True, data_augment_configs=None, state_dict=None):
         """reference: trainer.py:34-81.  ``state_dict`` (extension): backbone weights given in memory."""
         if not use_gpu:
-            raise _lib.PPVError('use_gpu=False: the B200 build of ppvector has no CPU path')
+            raise _lib.PPVError('use_gpu=False: this build of ppvector has no CPU path')
         assert torch.cuda.is_available(), 'GPU不可用'
         self.use_gpu = use_gpu
         self.device = torch.device('cuda', torch.cuda.current_device())
@@ -122,7 +122,7 @@ class PPVectorTrainer(object):
         # EER / minDCF on the device too (metrics.py:4-37 definitions; csrc/metrics.cu): the M x N scores never visit the host
         eer, min_dcf, threshold = eer_mindcf_from_matrix_gpu(scores, trials_labels, enroll_labels)
         if save_image_path:
-            logger.warning('save_image_path: plotting is out of scope of the B200 hot path (ignored)')
+            logger.warning('save_image_path: plotting is out of scope of the CUDA hot path (ignored)')
         return float(eer), float(min_dcf), float(threshold)
 
     # ---- trainer.py:281-365, step :206-229 ---------------------------------------------------------------------
@@ -151,11 +151,11 @@ class PPVectorTrainer(object):
         cf = self.configs
         use_model = cf.model_conf.get('model', 'CAMPPlus')
         if use_model != 'EcapaTdnn':
-            raise NotImplementedError(f'training on the B200 path is implemented for EcapaTdnn (got {use_model}); no fallback')
+            raise NotImplementedError(f'training on the H100 path is implemented for EcapaTdnn (got {use_model}); no fallback')
         if cf.loss_conf.get('loss', 'AAMLoss') not in ('AAMLoss', 'AMLoss', 'ARMLoss', 'CELoss', 'SubCenterLoss', 'SphereFace2') or cf.optimizer_conf.get('optimizer', 'Adam') != 'Adam':
-            raise NotImplementedError('training on the B200 path implements AAMLoss / AMLoss / ARMLoss / CELoss / SubCenterLoss / SphereFace2 + Adam (configs/ecapa_tdnn.yml)')
+            raise NotImplementedError('training on the H100 path implements AAMLoss / AMLoss / ARMLoss / CELoss / SubCenterLoss / SphereFace2 + Adam (configs/ecapa_tdnn.yml)')
         if cf.dataset_conf.get('is_use_pksampler', False):
-            raise NotImplementedError('PKSampler is out of scope of the B200 path')
+            raise NotImplementedError('PKSampler is out of scope of the H100 path')
         torch.manual_seed(1000)  # trainer.py:290
         np.random.seed(1000)
         _random.seed(1000)
@@ -172,9 +172,9 @@ class PPVectorTrainer(object):
         backbone = build_model(input_size=fz.feature_dim, configs=cf)  # random init with the mirror's initialisers, names = state_dict
         cls_conf = dict(cf.model_conf.get('classifier', {}))
         if model_args.get('pooling_type', 'ASP') != 'ASP' or not model_args.get('global_context', True):
-            raise NotImplementedError('the B200 training step implements pooling_type="ASP" with global_context')
+            raise NotImplementedError('the CUDA training step implements pooling_type="ASP" with global_context')
         if cls_conf.get('classifier_type', 'Cosine') != 'Cosine' or int(cls_conf.get('num_blocks', 0)) != 0:
-            raise NotImplementedError('the B200 training step implements classifier_type="Cosine", num_blocks=0')
+            raise NotImplementedError('the CUDA training step implements classifier_type="Cosine", num_blocks=0')
         cls_K = int(cls_conf.get('K', 1))  # fc.py:33: K sub-centres per class (SubCenterLoss); the classifier has num_speakers * K columns
         loss_K = int((cf.loss_conf.get('loss_args', {}) or {}).get('K', 3)) if cf.loss_conf.get('loss', 'AAMLoss') == 'SubCenterLoss' else 1
         if cls_K != loss_K:
