@@ -20,7 +20,7 @@ if __name__ == "__main__":
     tag = " ".join(f"{k}={v}" for k, v in os.environ.items() if k.startswith("PPV_"))
     for (N, K) in [(512, 512), (1536, 1536), (128, 1536), (512, 640)]:
         for prec in (0, 1):
-            for bn, bk in [(256, 64), (128, 64), (256, 32)]:
+            for bn, bk in [(256, 64), (128, 64), (256, 32), (128, 32)]:
                 if N < bn:
                     continue
                 us = run(M, N, K, bn, bk, prec)

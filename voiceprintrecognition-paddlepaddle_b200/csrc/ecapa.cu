@@ -427,7 +427,10 @@ void carve(EcapaModel* m, Carver& cv, int B, int T) {
     m->Tp = Tp;
 }
 
-inline int pick_bn(int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : 64; }
+// 128-wide n-tiles even where N allows 256: on an H100 SXM at 700 W (tools/gemm_bench.py, M = 78 336, profiles/gemm_bench_after.txt)
+// BN = 128 with 64-wide k-steps takes 15-18 % less time than BN = 256 at every large layer of the model (N x K = 512 x 512 / 640,
+// 1536 x 1536, split-bf16 x3), and no BN = 256 variant beats it by more than run-to-run noise.
+inline int pick_bn(int N) { return (N % 128 == 0) ? 128 : 64; }
 
 }  // namespace
 
@@ -504,7 +507,7 @@ static int build_plan(EcapaModel* m, int B, int T, void* ws, size_t ws_bytes, cu
         stp.kind = Step::GEMM;
         stp.BN = pick_bn(cw.N);
         // 32-wide k-steps (twice the ring slots) for the wide-N layers whose K fits the k-step table
-        const int bk = (stp.BN == 256 && cw.Ktot <= 32 * GEMM_MAX_KSTEPS && bk32_enabled) ? 32 : 64;
+        const int bk = (cw.N >= 512 && cw.Ktot <= 32 * GEMM_MAX_KSTEPS && bk32_enabled) ? 32 : 64;
         int rc = gemm_build(&stp.gp, srcs.data(), int(srcs.size()), cw.W, M, cw.N, ep, stp.BN, bk);
         if (rc) return rc;
         m->steps.push_back(stp);

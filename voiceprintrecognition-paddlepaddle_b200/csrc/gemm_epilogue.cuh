@@ -106,20 +106,31 @@ __device__ __forceinline__ void epilogue_pair(const Epilogue& ep, int N, int col
 }
 
 // The whole 64 x BN fragment of this warpgroup.  `row_of(r)`, r in [0, 64): the GEMM row of warpgroup-local row r, or -1 if it
-// holds no output; `t`: thread index inside the warpgroup; columns are n0 + [0, BN).
+// holds no output; `t`: thread index inside the warpgroup; columns are n0 + [0, BN).  The accumulators are consumed: on return
+// `acc` holds garbage.
+// The fragment is walked EPI_GROUPS column groups (8 columns, 4 registers) at a time by a loop that is not unrolled; after each trip the
+// remaining accumulators move down by one chunk (register moves), so the per-pair code exists once per position inside a chunk
+// instead of once per column group.  Unrolled over the whole fragment, the BN = 256 epilogue is ~25 k SASS instructions run straight
+// through once per tile, and fetching them, not the tensor cores, sets the GEMM's pace (DESIGN.md §5).
 template <int BN, typename RowOf>
-__device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0, const float (&acc)[BN / 2], RowOf&& row_of, int t,
+__device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0, float (&acc)[BN / 2], RowOf&& row_of, int t,
                                               int64_t out_row_shift = 0) {
     if (ep.debug_nostore) return;
     const int w = t >> 5, l = t & 31;
     const int r0 = 16 * w + (l >> 2);
     const EpiRow ra = epilogue_row(ep, row_of(r0), out_row_shift);
     const EpiRow rb = epilogue_row(ep, row_of(r0 + 8), out_row_shift);
+    constexpr int EPI_GROUPS = BN / 8 < 4 ? BN / 8 : 4;
+#pragma unroll 1
+    for (int c = 0; c < BN / 8; c += EPI_GROUPS) {
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-        const int col = n0 + 8 * i + 2 * (l & 3);
-        epilogue_pair(ep, N, col, ra, acc[4 * i + 0], acc[4 * i + 1]);
-        epilogue_pair(ep, N, col, rb, acc[4 * i + 2], acc[4 * i + 3]);
+        for (int i = 0; i < EPI_GROUPS; ++i) {
+            const int col = n0 + 8 * (c + i) + 2 * (l & 3);
+            epilogue_pair(ep, N, col, ra, acc[4 * i + 0], acc[4 * i + 1]);
+            epilogue_pair(ep, N, col, rb, acc[4 * i + 2], acc[4 * i + 3]);
+        }
+#pragma unroll
+        for (int j = 0; j + 4 * EPI_GROUPS < BN / 2; ++j) acc[j] = acc[j + 4 * EPI_GROUPS];
     }
 }
 

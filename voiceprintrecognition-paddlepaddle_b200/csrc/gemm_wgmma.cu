@@ -13,7 +13,8 @@
 //   warp 0        TMA producer : cp.async.bulk.tensor 3-D tiles (SWIZZLE_128B / 64B) into a STAGES-deep smem ring
 //   warps 4-7     MMA + epilogue of tile rows 0-63 : wgmma m64 x BN x 16 from the ring, then bias / ReLU / BN affine / tanh ->
 //   warps 8-11    MMA + epilogue of tile rows 64-127  split-bf16 (or fp32) stores incl. the reflect-halo rows
-// The producer runs ahead into the next tile while the two warpgroups drain their accumulators.
+// The producer runs ahead into the next tile while the two warpgroups drain their accumulators.  The producer warpgroup hands its
+// registers to the MMA warpgroups (setmaxnreg 40 / 232): a BN = 256 accumulator alone is 128 registers per thread.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -101,67 +102,71 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     auto tile_m = [&](int t) { return (t % mn_tiles) / gp.n_tiles; };
     auto tile_n = [&](int t) { return (t % mn_tiles) % gp.n_tiles; };
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        int stage = 0;
-        uint32_t phase = 0;
-        if (gp.ws && lane == 0) {  // resident weights: every k-slice, once
-            mbar_arrive_expect_tx(w_full, nk * Cfg::NB * Cfg::B_BYTES);
-            for (int s = 0; s < nk; ++s)
-                for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(w_res + (s * Cfg::NB + p) * Cfg::B_BYTES, &gp.mapB, w_full, s * BK, 0, p);
-        }
-        __syncwarp();
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            const int zsplit = tile / mn_tiles;
-            const int m0 = tile_m(tile) * GEMM_BM;
-            const int n0 = tile_n(tile) * BN;
-            // L2 prefetch of the activation rows of this CTA's NEXT tile (one CTA per m-tile issues it): they come
-            // from HBM, and a 2-4 slot ring alone cannot hide that latency.
-            const int ntile = tile + gridDim.x;
-            if (gp.l2_prefetch && ntile < num_tiles && tile_n(ntile) == 0 && lane < nk && gp.lin_splits == 0) {
-                const int nm0 = tile_m(ntile) * GEMM_BM;
-                for (int s = lane; s < nk; s += 32) {
-                    const KStep ks = gp.ksteps[s];
-#pragma unroll
-                    for (int p = 0; p < Cfg::NA; ++p) tma_prefetch_l2_3d(&gp.mapA[ks.map], ks.a_col, nm0 + ks.row_off, p);
-                }
+    if (warp < 4) {
+        setmaxnreg_dec<40>();  // all four producer warps; warps 1-3 have nothing else to do
+        if (warp == 0) {
+            // ===================== TMA producer =====================
+            int stage = 0;
+            uint32_t phase = 0;
+            if (gp.ws && lane == 0) {  // resident weights: every k-slice, once
+                mbar_arrive_expect_tx(w_full, nk * Cfg::NB * Cfg::B_BYTES);
+                for (int s = 0; s < nk; ++s)
+                    for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(w_res + (s * Cfg::NB + p) * Cfg::B_BYTES, &gp.mapB, w_full, s * BK, 0, p);
             }
             __syncwarp();
-            for (int s = 0; s < nk; ++s) {
-                mbar_wait(empty_bar(stage), phase ^ 1u);
-                if (lane == 0) {
-                    const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
-                    const uint32_t sb = sa + Cfg::NA * Cfg::A_BYTES;
-                    const uint32_t fb = full_bar(stage);
-                    mbar_arrive_expect_tx(fb, gp.ws ? Cfg::NA * Cfg::A_BYTES : Cfg::STAGE_BYTES);
-                    if (gp.ws) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int zsplit = tile / mn_tiles;
+                const int m0 = tile_m(tile) * GEMM_BM;
+                const int n0 = tile_n(tile) * BN;
+                // L2 prefetch of the activation rows of this CTA's NEXT tile (one CTA per m-tile issues it): they come
+                // from HBM, and a 2-4 slot ring alone cannot hide that latency.
+                const int ntile = tile + gridDim.x;
+                if (gp.l2_prefetch && ntile < num_tiles && tile_n(ntile) == 0 && lane < nk && gp.lin_splits == 0) {
+                    const int nm0 = tile_m(ntile) * GEMM_BM;
+                    for (int s = lane; s < nk; s += 32) {
                         const KStep ks = gp.ksteps[s];
 #pragma unroll
-                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[ks.map], fb, ks.a_col, m0 + ks.row_off, p);
-                    } else if (gp.lin_splits > 0) {
-                        const int kcol = (zsplit * nk + s) * BK;
-#pragma unroll
-                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[0], fb, kcol, m0, p);
-#pragma unroll
-                        for (int p = 0; p < Cfg::NB; ++p)
-                            tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, kcol + gp.lin_b_col0, gp.lin_b_row0 + n0, p);
-                    } else {
-                        const KStep ks = gp.ksteps[s];
-                        const CUtensorMap* ma = &gp.mapA[ks.map];
-#pragma unroll
-                        for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, ma, fb, ks.a_col, m0 + ks.row_off, p);
-#pragma unroll
-                        for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, s * BK, n0, p);
+                        for (int p = 0; p < Cfg::NA; ++p) tma_prefetch_l2_3d(&gp.mapA[ks.map], ks.a_col, nm0 + ks.row_off, p);
                     }
                 }
                 __syncwarp();
-                if (++stage == nst) {
-                    stage = 0;
-                    phase ^= 1u;
+                for (int s = 0; s < nk; ++s) {
+                    mbar_wait(empty_bar(stage), phase ^ 1u);
+                    if (lane == 0) {
+                        const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
+                        const uint32_t sb = sa + Cfg::NA * Cfg::A_BYTES;
+                        const uint32_t fb = full_bar(stage);
+                        mbar_arrive_expect_tx(fb, gp.ws ? Cfg::NA * Cfg::A_BYTES : Cfg::STAGE_BYTES);
+                        if (gp.ws) {
+                            const KStep ks = gp.ksteps[s];
+#pragma unroll
+                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[ks.map], fb, ks.a_col, m0 + ks.row_off, p);
+                        } else if (gp.lin_splits > 0) {
+                            const int kcol = (zsplit * nk + s) * BK;
+#pragma unroll
+                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[0], fb, kcol, m0, p);
+#pragma unroll
+                            for (int p = 0; p < Cfg::NB; ++p)
+                                tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, kcol + gp.lin_b_col0, gp.lin_b_row0 + n0, p);
+                        } else {
+                            const KStep ks = gp.ksteps[s];
+                            const CUtensorMap* ma = &gp.mapA[ks.map];
+#pragma unroll
+                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, ma, fb, ks.a_col, m0 + ks.row_off, p);
+#pragma unroll
+                            for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, s * BK, n0, p);
+                        }
+                    }
+                    __syncwarp();
+                    if (++stage == nst) {
+                        stage = 0;
+                        phase ^= 1u;
+                    }
                 }
             }
         }
-    } else if (warp >= 4) {
+    } else {
+        setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
         // ===================== MMA + epilogue: warpgroup g owns rows [64 g, 64 g + 64) of every tile =====================
         const int g = (warp - 4) >> 2;
         const int t = threadIdx.x & 127;
