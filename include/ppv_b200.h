@@ -347,7 +347,16 @@ int ppv_gemm_test(const float* A, const float* W, const float* bias, const float
                   int relu, int M, int N, int K, int block_n, int block_k, int precision, float* out, void* ws,
                   size_t ws_bytes, void* stream);
 
-/* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N) bytes. */
+/* The same with split-bf16 planes output out[2][M][N] (bf16, N % 32 == 0, 16-byte aligned) and the epilogue of the ECAPA layers:
+ * + bias, + rowgrp_bias[row / Tp] (may be NULL), ReLU (relu), BN affine (may be NULL), tanh (tanh_).  Tp > 0: padded time layout
+ * (Tp = T + 2 P, M % Tp == 0), only the T valid rows of each group are written.  block_k is 64. */
+int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, const float* rowgrp_bias, const float* bn_scale,
+                         const float* bn_shift, int relu, int tanh_, int Tp, int P, int M, int N, int K, int block_n,
+                         int precision, void* out, void* ws, size_t ws_bytes, void* stream);
+
+/* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N)
+ * bytes + 4*(3 + M/306)*N rounded up to 256.  planes_out: 0 ReLU to fp32, 1 ReLU to planes, 2 bias + ReLU + BN to planes over the
+ * padded time layout (Tp = 306, P = 4), 3 the same + per-utterance bias + tanh (ASP attention TDNN); 2 and 3 need M % 306 == 0. */
 int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision, int planes_out, int iters, void* ws,
                    size_t ws_bytes, float* ms_per_launch, void* stream);
 

@@ -96,44 +96,56 @@ def main():
     assert len(gemm_idx) == len(GEMM_LAYERS), f"expected {len(GEMM_LAYERS)} gather-GEMM launches per step, got {len(gemm_idx)}: {seqs[0]}"
 
     dur = collections.defaultdict(float)  # per launch position, us summed over steps
+    # exclusive time: end - max(start, end of the kernel before it).  Under programmatic dependent launch a kernel starts while
+    # its predecessor still runs and waits in griddepcontrol.wait; its plain duration counts that wait, the exclusive time does not.
+    excl = collections.defaultdict(float)
+    prev_end = None
     for s in range(args.steps):
         for i, e in enumerate(kern[s * per:(s + 1) * per]):
             dur[i] += e.time_range.elapsed_us()
+            start, end = e.time_range.start, e.time_range.end
+            excl[i] += max(0.0, end - (start if prev_end is None else max(start, prev_end)))
+            prev_end = end if prev_end is None else max(prev_end, end)
     kernel_us = sum(dur.values()) / args.steps
     M = BATCH * (FRAMES + 8)  # GEMM rows: padded time layout, Tp = T + 2 P, P = 4
     valid = BATCH * FRAMES
     layers = []
     for (name, rows, N, Ka, Kx), i in zip(GEMM_LAYERS, gemm_idx):
         us = dur[i] / args.steps
+        ex = excl[i] / args.steps
         m_alg, m_exec = (valid, M) if rows == "frames" else (BATCH, BATCH)
         flops = 2.0 * m_alg * N * Ka
         hbm = 4.0 * (m_exec * Kx + N * Kx + m_exec * N)  # two bf16 planes of A, W and the output
         t_min_us = max(flops * 3 / (PEAK_BF16_TFLOPS * 1e12), hbm / (PEAK_HBM_TBS * 1e12)) * 1e6  # x3: split-bf16 executes three MMAs
-        layers.append({"layer": name, "kernel": seqs[0][i], "us": us, "algorithmic_gflop": flops / 1e9, "hbm_mb": hbm / 1e6,
+        layers.append({"layer": name, "kernel": seqs[0][i], "us": us, "exclusive_us": ex, "algorithmic_gflop": flops / 1e9, "hbm_mb": hbm / 1e6,
                        "algorithmic_tflops": flops / us / 1e6, "executed_x3_tflops": 3 * flops * (Kx / Ka) * (m_exec / m_alg) / us / 1e6,
-                       "share_of_peak": t_min_us / us})
+                       "share_of_peak": t_min_us / us, "share_of_peak_exclusive": t_min_us / ex})
     gemm_us = sum(l["us"] for l in layers)
-    others = collections.defaultdict(lambda: [0.0, 0])
+    gemm_excl_us = sum(l["exclusive_us"] for l in layers)
+    others = collections.defaultdict(lambda: [0.0, 0, 0.0])
     for i, n in enumerate(seqs[0]):
         if i not in gemm_idx:
             others[n][0] += dur[i] / args.steps
             others[n][1] += 1
+            others[n][2] += excl[i] / args.steps
     res = {"card": card(), "steps": args.steps, "step_ms": step_ms, "kernel_ms_per_step": kernel_us / 1000.0,
            "launches_per_step": per, "gemm_layers_ms": gemm_us / 1000.0, "gemm_share_of_step": gemm_us / 1000.0 / step_ms,
-           "layers": layers, "other_kernels": {k: {"us": v[0], "launches": v[1]} for k, v in sorted(others.items(), key=lambda kv: -kv[1][0])}}
+           "gemm_layers_exclusive_ms": gemm_excl_us / 1000.0,
+           "layers": layers, "other_kernels": {k: {"us": v[0], "launches": v[1], "exclusive_us": v[2]} for k, v in sorted(others.items(), key=lambda kv: -kv[1][0])}}
 
     print(f"card: {res['card']}")
     print(f"step {step_ms:.3f} ms (events, no profiler), kernels {kernel_us / 1000:.3f} ms summed, {per} launches per step")
-    print(f"{'layer':10s} {'us':>9s} {'GFLOP':>8s} {'MB':>8s} {'TF/s alg':>9s} {'TF/s x3':>8s} {'peak %':>7s}")
+    print(f"{'layer':10s} {'us':>9s} {'excl us':>9s} {'GFLOP':>8s} {'MB':>8s} {'TF/s alg':>9s} {'TF/s x3':>8s} {'peak %':>7s}")
     for l in layers:
-        print(f"{l['layer']:10s} {l['us']:9.1f} {l['algorithmic_gflop']:8.1f} {l['hbm_mb']:8.1f} {l['algorithmic_tflops']:9.1f} "
-              f"{l['executed_x3_tflops']:8.1f} {100 * l['share_of_peak']:6.1f}%")
+        print(f"{l['layer']:10s} {l['us']:9.1f} {l['exclusive_us']:9.1f} {l['algorithmic_gflop']:8.1f} {l['hbm_mb']:8.1f} "
+              f"{l['algorithmic_tflops']:9.1f} {l['executed_x3_tflops']:8.1f} {100 * l['share_of_peak']:6.1f}%")
     big = sum(l["us"] for l in layers if l["layer"] in ("conv0", "mfa", "att1") or l["layer"].startswith("tdnn"))
     res["conv0_tdnn_mfa_att1_ms"] = big / 1000.0
     print(f"conv0 + tdnn + mfa + att1: {big / 1000:.3f} ms = {100 * big / 1000 / step_ms:.1f} % of the step")
-    print(f"gather-GEMM layers: {gemm_us / 1000:.3f} ms = {100 * res['gemm_share_of_step']:.1f} % of the step")
+    print(f"gather-GEMM layers: {gemm_us / 1000:.3f} ms = {100 * res['gemm_share_of_step']:.1f} % of the step "
+          f"({gemm_excl_us / 1000:.3f} ms exclusive)")
     for k, v in res["other_kernels"].items():
-        print(f"  {v['us']:9.1f} us  x{v['launches']:<3d} {k}")
+        print(f"  {v['us']:9.1f} us  {v['exclusive_us']:9.1f} us excl  x{v['launches']:<3d} {k}")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "step_profile.json"), "w") as f:

@@ -508,18 +508,77 @@ int ppv_gemm_test(const float* A, const float* W, const float* bias, const float
     PPV_GUARD_END
 }
 
+// Planes-output variant of the test hook: out is a split-bf16 planes buffer [2][M][N] (N % 32 == 0, 16-byte aligned) written by the
+// epilogue the ECAPA layers use: + bias, + rowgrp_bias[row / Tp] (if given), ReLU (if relu), BN affine (if given), tanh (if tanh_).
+// Tp > 0: rows follow the padded time layout (Tp = T + 2 P, M % Tp == 0) and only the T valid rows of each group are stored.
+int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, const float* rowgrp_bias, const float* bn_scale,
+                         const float* bn_shift, int relu, int tanh_, int Tp, int P, int M, int N, int K, int block_n, int precision,
+                         void* out, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(A && W && out && ws, "ppv_gemm_test_planes: null argument");
+    PPV_REQUIRE(ws_bytes >= ppv_gemm_test_workspace_bytes(M, N, K), "ppv_gemm_test_planes: workspace too small");
+    PPV_REQUIRE(N % 32 == 0 && (Tp == 0 || (M % Tp == 0 && Tp > 2 * P)), "ppv_gemm_test_planes: bad shape");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Kp = int(au(size_t(K), 64));
+    Planes pa, pw;
+    pa.rows = int64_t(au(size_t(M), 128));
+    pa.ld = Kp;
+    pa.plane_stride = pa.rows * Kp;
+    pa.base = static_cast<__nv_bfloat16*>(ws);
+    pw.rows = int64_t(au(size_t(N), 256));
+    pw.ld = Kp;
+    pw.plane_stride = pw.rows * Kp;
+    pw.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + au(size_t(pa.plane_stride) * 4, 256));
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, ppv_gemm_test_workspace_bytes(M, N, K), st));
+    rc = launch_f32_to_planes(A, M, K, pa, st);
+    if (rc) return rc;
+    rc = launch_f32_to_planes(W, N, K, pw, st);
+    if (rc) return rc;
+    GemmSource src{pa, 0, Kp, 0};
+    Epilogue ep;
+    ep.bias = bias;
+    ep.rowgrp_bias = rowgrp_bias;
+    ep.relu = relu;
+    ep.tanh_ = tanh_;
+    ep.bn_scale = bn_scale;
+    ep.bn_shift = bn_shift;
+    ep.out_mode = OUT_PLANES;
+    ep.out = out;
+    ep.out_ld = N;
+    ep.out_plane_stride = int64_t(M) * N;
+    if (Tp > 0) {
+        ep.Tp = Tp;
+        ep.P = P;
+        ep.T = Tp - 2 * P;
+    }
+    GemmParams gp;
+    rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, 64);
+    if (rc) return rc;
+    return gemm_launch(gp, block_n, precision, device_sm_count(), st);
+    PPV_GUARD_END
+}
+
 // Kernel-only timing of the gather-GEMM (tools/gemm_bench.py): operands are converted once, the kernel is launched
-// `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  out is fp32 [M,N] or, when
-// planes_out != 0, a split-bf16 planes buffer inside ws (the layout every model layer writes).
+// `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  planes_out selects the epilogue:
+//   0  ReLU, fp32 [M,N];   1  ReLU, split-bf16 planes (the layout every model layer writes);
+//   2  the ECAPA TDNN layers: bias + ReLU + BN affine into planes over the padded time layout (Tp = 306, P = 4: T = 298);
+//   3  the ASP attention TDNN (att1): bias + per-utterance bias + ReLU + BN affine + tanh, same layout.
+// Modes 2 and 3 need M % 306 == 0.
 int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision, int planes_out, int iters, void* ws, size_t ws_bytes,
                    float* ms_per_launch, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(ws && ms_per_launch && iters > 0, "ppv_gemm_bench: bad argument");
+    PPV_REQUIRE(planes_out >= 0 && planes_out <= 3, "ppv_gemm_bench: planes_out must be 0-3");
+    constexpr int kTp = 306, kP = 4;
+    PPV_REQUIRE(planes_out < 2 || M % kTp == 0, "ppv_gemm_bench: model epilogues need M % 306 == 0");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t Kp = au(size_t(K), 64);
     const size_t a_bytes = au(au(size_t(M), 128) * Kp * 4, 256), w_bytes = au(au(size_t(N), 256) * Kp * 4, 256);
     const size_t o_bytes = au(au(size_t(M), 128) * size_t(N) * 4, 256);
-    PPV_REQUIRE(ws_bytes >= a_bytes + w_bytes + o_bytes, "ppv_gemm_bench: workspace too small");
+    const size_t v_bytes = au((3 + size_t(M / kTp)) * size_t(N) * 4, 256);  // bias, BN scale / shift, per-utterance bias
+    PPV_REQUIRE(ws_bytes >= a_bytes + w_bytes + o_bytes + v_bytes, "ppv_gemm_bench: workspace too small");
     Planes pa, pw, po;
     pa.rows = int64_t(au(size_t(M), 128)); pa.ld = int(Kp); pa.plane_stride = pa.rows * pa.ld; pa.base = static_cast<__nv_bfloat16*>(ws);
     pw.rows = int64_t(au(size_t(N), 256)); pw.ld = int(Kp); pw.plane_stride = pw.rows * pw.ld;
@@ -527,11 +586,18 @@ int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision,
     po.rows = pa.rows; po.ld = N; po.plane_stride = po.rows * po.ld;
     po.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + a_bytes + w_bytes);
     PPV_CUDA_OK(cudaMemsetAsync(ws, 0x11, a_bytes + w_bytes, st));  // small finite bf16 values
+    float* vec = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + a_bytes + w_bytes + o_bytes);
+    PPV_CUDA_OK(cudaMemsetAsync(vec, 0x3c, v_bytes, st));  // small finite floats (0.0115)
     GemmSource src{pa, 0, int(Kp), 0};
     Epilogue ep;
     ep.relu = 1;
     if (planes_out) {
         ep.out_mode = OUT_PLANES; ep.out = po.base; ep.out_ld = po.ld; ep.out_plane_stride = po.plane_stride;
+        if (planes_out >= 2) {
+            ep.Tp = kTp; ep.P = kP; ep.T = kTp - 2 * kP;
+            ep.bias = vec; ep.bn_scale = vec + N; ep.bn_shift = vec + 2 * N;
+            if (planes_out == 3) { ep.rowgrp_bias = vec + 3 * N; ep.tanh_ = 1; }
+        }
     } else {
         ep.out_mode = OUT_F32; ep.out = po.base; ep.out_ld = N;
     }

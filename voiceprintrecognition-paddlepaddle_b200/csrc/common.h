@@ -141,6 +141,7 @@ struct Epilogue {
     int zero_invalid = 0;  // planes output without halo on the input grid: rows outside the valid frames are stored as zeros (zero-padded convs read them)
     int f32_vec_ok = 0;  // set by gemm_build: OUT_F32 rows and columns are 8-byte aligned (paired stores)
     int debug_nostore = 0;  // PPV_GEMM_NOSTORE=1 (tools/gemm_bench.py only): skip the epilogue stores
+    int lean = 0;  // set by gemm_build: the epilogue needs only what epilogue_frag_lean does (gemm_epilogue.cuh)
 };
 
 struct GemmParams {

@@ -532,7 +532,7 @@ static int build_plan(EcapaModel* m, int B, int T, void* ws, size_t ws_bytes, cu
     for (int b = 1; b <= 3; ++b) {
         const Planes& X = (b == 1) ? m->bufs[B_X0] : m->bufs[B_CAT];
         const int xcol = (b == 1) ? 0 : (b - 2) * C;
-        // the fused Res2Net chain builds the reflect halo rows itself, so tdnn1 may use the faster halo-free TMA-store epilogue
+        // the fused Res2Net chain builds the reflect halo rows itself, so tdnn1 writes no halo rows (and gets the lean epilogue)
         rc = add_gemm(m->tdnn1[b - 1], {{-1, 0, C, 0, 0, C, 0}}, &X, xcol, int(R), planes_out(m->bufs[B_H], 0, !use_res2_chain));
         if (rc) return rc;
         if (use_res2_chain) {  // all seven convs in one kernel, one utterance per CTA, operands resident in shared memory (res2chain.cu)

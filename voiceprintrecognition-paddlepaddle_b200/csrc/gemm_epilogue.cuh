@@ -10,7 +10,7 @@
 
 namespace ppv {
 
-constexpr int GEMM_MMA_THREADS = 256;                 // two MMA warpgroups: rows 0-63 and 64-127 of a 128-row tile
+constexpr int GEMM_MMA_THREADS = 256;                 // two MMA warpgroups (whole tiles in turn, or rows 0-63 / 64-127 of each)
 constexpr int GEMM_THREADS = 128 + GEMM_MMA_THREADS;  // + the producer warpgroup (warp 0: TMA)
 
 // per-column epilogue math on one accumulator value of global column `col`.  The per-column vectors are re-read for each of
@@ -132,6 +132,71 @@ __device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0,
 #pragma unroll
         for (int j = 0; j + 4 * EPI_GROUPS < BN / 2; ++j) acc[j] = acc[j + 4 * EPI_GROUPS];
     }
+}
+
+// The epilogues of the ECAPA-TDNN layers (gemm_build sets ep.lean): split-bf16 planes on the input row grid, bias / per-utterance
+// bias / ReLU / BN affine / tanh, no halo, mirror or zero rows, no segment scale, SiLU, sigmoid or clipped ReLU.  The two rows'
+// mapping and store addresses are computed once per fragment, and each column's bias / BN vectors are loaded once for both rows.
+// Per element the arithmetic is epilogue_math1's, in the same order.
+template <int BN, typename RowOf>
+__device__ __forceinline__ void epilogue_frag_lean(const Epilogue& ep, int N, int n0, float (&acc)[BN / 2], RowOf&& row_of, int t) {
+    const int w = t >> 5, l = t & 31;
+    const int r0 = 16 * w + (l >> 2);
+    const EpiRow ra = epilogue_row(ep, row_of(r0), 0);
+    const EpiRow rb = epilogue_row(ep, row_of(r0 + 8), 0);
+    const int c0 = n0 + 2 * (l & 3);  // this thread's first column; its columns are c0 + 8 j + {0, 1}
+    __nv_bfloat16* const obase = static_cast<__nv_bfloat16*>(ep.out) + ep.out_col0 + c0;
+    uint32_t* const pa = reinterpret_cast<uint32_t*>(obase + ra.out_row * ep.out_ld);
+    uint32_t* const pb = reinterpret_cast<uint32_t*>(obase + rb.out_row * ep.out_ld);
+    const int64_t lo_off = ep.out_plane_stride / 2;  // the lo plane, in 32-bit words (gemm_build: plane stride % 16 == 0)
+    const float* const ga = ep.rowgrp_bias ? ep.rowgrp_bias + ra.grp * N + c0 : nullptr;
+    const float* const gb = ep.rowgrp_bias ? ep.rowgrp_bias + rb.grp * N + c0 : nullptr;
+    constexpr int EPI_GROUPS = BN / 8 < 4 ? BN / 8 : 4;
+#pragma unroll 1
+    for (int c = 0; c < BN / 8; c += EPI_GROUPS) {
+#pragma unroll
+        for (int i = 0; i < EPI_GROUPS; ++i) {
+            const int j = 8 * (c + i);
+            if (c0 + j >= N) continue;  // planes output: N % 32 == 0, so column c0 + j + 1 exists too
+            float xa0 = acc[4 * i + 0], xa1 = acc[4 * i + 1], xb0 = acc[4 * i + 2], xb1 = acc[4 * i + 3];
+            if (ep.bias) {
+                const float b0 = __ldg(ep.bias + c0 + j), b1 = __ldg(ep.bias + c0 + j + 1);
+                xa0 += b0, xa1 += b1, xb0 += b0, xb1 += b1;
+            }
+            if (ga) {
+                xa0 += __ldg(ga + j), xa1 += __ldg(ga + j + 1);
+                xb0 += __ldg(gb + j), xb1 += __ldg(gb + j + 1);
+            }
+            if (ep.relu) xa0 = fmaxf(xa0, 0.f), xa1 = fmaxf(xa1, 0.f), xb0 = fmaxf(xb0, 0.f), xb1 = fmaxf(xb1, 0.f);
+            if (ep.bn_scale) {
+                const float s0 = __ldg(ep.bn_scale + c0 + j), s1 = __ldg(ep.bn_scale + c0 + j + 1);
+                const float h0 = __ldg(ep.bn_shift + c0 + j), h1 = __ldg(ep.bn_shift + c0 + j + 1);
+                xa0 = fmaf(xa0, s0, h0), xa1 = fmaf(xa1, s1, h1), xb0 = fmaf(xb0, s0, h0), xb1 = fmaf(xb1, s1, h1);
+            }
+            if (ep.tanh_) xa0 = tanhf(xa0), xa1 = tanhf(xa1), xb0 = tanhf(xb0), xb1 = tanhf(xb1);
+            uint32_t h, lo;
+            if (ra.valid) {
+                split_pack_bf16x2(xa0, xa1, h, lo);
+                pa[j / 2] = h;
+                pa[j / 2 + lo_off] = lo;
+            }
+            if (rb.valid) {
+                split_pack_bf16x2(xb0, xb1, h, lo);
+                pb[j / 2] = h;
+                pb[j / 2 + lo_off] = lo;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j + 4 * EPI_GROUPS < BN / 2; ++j) acc[j] = acc[j + 4 * EPI_GROUPS];
+    }
+}
+
+// The lean path where gemm_build selected it, else the general one.
+template <int BN, typename RowOf>
+__device__ __forceinline__ void gemm_epilogue(const Epilogue& ep, int N, int n0, float (&acc)[BN / 2], RowOf&& row_of, int t,
+                                              int64_t out_row_shift) {
+    if (ep.lean) epilogue_frag_lean<BN>(ep, N, n0, acc, row_of, t);
+    else epilogue_frag<BN>(ep, N, n0, acc, row_of, t, out_row_shift);
 }
 
 }  // namespace ppv

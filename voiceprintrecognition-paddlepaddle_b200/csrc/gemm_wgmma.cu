@@ -10,11 +10,12 @@
 // register accumulator (fp32-grade), PPV_PREC_BF16 issues hi*hi only.
 //
 // Warp roles (384 threads, 1 CTA / SM, persistent over 128 x BN tiles):
-//   warp 0        TMA producer : cp.async.bulk.tensor 3-D tiles (SWIZZLE_128B / 64B) into a STAGES-deep smem ring
-//   warps 4-7     MMA + epilogue of tile rows 0-63 : wgmma m64 x BN x 16 from the ring, then bias / ReLU / BN affine / tanh ->
-//   warps 8-11    MMA + epilogue of tile rows 64-127  split-bf16 (or fp32) stores incl. the reflect-halo rows
-// The producer runs ahead into the next tile while the two warpgroups drain their accumulators.  The producer warpgroup hands its
-// registers to the MMA warpgroups (setmaxnreg 40 / 232): a BN = 256 accumulator alone is 128 registers per thread.
+//   warp 0        TMA producer : cp.async.bulk.tensor 3-D tiles (SWIZZLE_128B / 64B) into a STAGES-deep smem ring, in tile order
+//   warps 4-7     MMA warpgroup 0 : wgmma m64 x BN x 16 from the ring, then bias / ReLU / BN affine / tanh ->
+//   warps 8-11    MMA warpgroup 1   split-bf16 (or fp32) stores incl. the reflect-halo rows
+// BN <= 128 (ping-pong): warpgroup g owns the CTA's tiles g, g + 2, ... whole (two m64 accumulators), so one warpgroup's epilogue
+// runs while the other's MMAs keep the tensor cores busy.  BN = 256 (cooperative): warpgroup g owns rows [64 g, 64 g + 64) of every
+// tile and both run their epilogues together.  The producer warpgroup hands its registers to the MMA warpgroups (setmaxnreg 40 / 232).
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -44,6 +45,10 @@ struct GemmCfg {
     static constexpr int MAX_STAGES = 8;  // barrier slots
     static constexpr int STAGES = STAGES_RAW > MAX_STAGES ? MAX_STAGES : STAGES_RAW;
     static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + BAR_BYTES;
+    // Ping-pong schedule (each MMA warpgroup owns whole tiles, two m64 x BN accumulators) where a tile fits in registers: BN <= 128.
+    // BN = 256 would need 256 accumulator registers per thread and keeps the cooperative schedule (both warpgroups share every tile).
+    static constexpr bool PINGPONG = BN <= 128;
+    static constexpr int EMPTY_ARRIVALS = PINGPONG ? 1 : GEMM_MMA_THREADS / 128;  // consumers that release one ring slot
     static_assert(STAGES >= 2, "need at least a double buffer");
     static_assert(BN == 64 || BN == 128 || BN == 256, "BN");
     static_assert(BK == 64 || BK == 32, "BK");
@@ -84,7 +89,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < MAXST; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), GEMM_MMA_THREADS / 128);  // one arrival per MMA warpgroup
+            mbar_init(empty_bar(s), Cfg::EMPTY_ARRIVALS);
         }
         mbar_init(w_full, 1);
         fence_mbar_init();
@@ -165,6 +170,90 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 }
             }
         }
+    } else if constexpr (Cfg::PINGPONG) {
+        setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
+        // ===================== MMA + epilogue, ping-pong: warpgroup g owns the CTA's tiles g, g + 2, g + 4, ... =====================
+        // A tile is two m64 x BN accumulators (rows 0-63 and 64-127).  The producer fills the ring in tile order and the warpgroup that
+        // consumes a slot releases it.  Ordered hand-off: a warpgroup starts its k-loop only once the other has waited for every k-step of
+        // the tile before (named barrier 1 + g, arrived at by the other warpgroup).  So the k-loops run one after the other, one
+        // warpgroup's epilogue runs under the other's MMAs, and no warpgroup ever waits for a ring slot more than one fill ahead of the
+        // last completed one (an mbarrier parity wait cannot tell fill k from fill k + 2).
+        const int g = (warp - 4) >> 2;
+        const int t = threadIdx.x & 127;
+        constexpr uint32_t A_HALF = 64 * BK * 2;  // 64 rows of the A tile (a whole number of 8-row swizzle groups)
+        const int my_tiles = blockIdx.x < num_tiles ? (num_tiles - 1 - int(blockIdx.x)) / int(gridDim.x) + 1 : 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc0[BN / 2], acc1[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+        if (gp.ws) mbar_wait(w_full, 0);
+        int local = 0;  // index of the tile among this CTA's tiles
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
+            if ((local & 1) != g) {  // the other warpgroup's tile: skip its nk ring positions
+                const int adv = stage + nk;
+                phase ^= uint32_t((adv / nst) & 1);
+                stage = adv % nst;
+                continue;
+            }
+            const int m0 = tile_m(tile) * GEMM_BM;
+            const int n0 = tile_n(tile) * BN;
+            named_bar_sync_if(local > 0, 1 + g, 2 * 128);  // the other warpgroup has taken every k-step of tile local - 1
+            int prev = -1;
+            wgmma_fence_acc(acc0);
+            wgmma_fence_acc(acc1);
+            for (int s = 0; s < nk; ++s) {
+                mbar_wait(full_bar(stage), phase);
+                const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
+                const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
+                const uint64_t a0_hi = make_kmajor_desc<BK>(sa), a1_hi = make_kmajor_desc<BK>(sa + A_HALF);
+                const uint64_t b_hi = make_kmajor_desc<BK>(sb);
+                wgmma_fence();
+                // per accumulator the same order as the cooperative schedule: hi*hi, lo*hi, hi*lo, k ascending in each
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    wgmma_bf16<BN>(acc0, a0_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
+                    wgmma_bf16<BN>(acc1, a1_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
+                }
+                if (NSPLIT == 3) {
+                    const uint64_t a0_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES), a1_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES + A_HALF);
+                    const uint64_t b_lo = make_kmajor_desc<BK>(sb + Cfg::B_BYTES);
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) {
+                        wgmma_bf16<BN>(acc0, a0_lo + 2 * k, b_hi + 2 * k, 1u);
+                        wgmma_bf16<BN>(acc1, a1_lo + 2 * k, b_hi + 2 * k, 1u);
+                    }
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) {
+                        wgmma_bf16<BN>(acc0, a0_hi + 2 * k, b_lo + 2 * k, 1u);
+                        wgmma_bf16<BN>(acc1, a1_hi + 2 * k, b_lo + 2 * k, 1u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
+                if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+                prev = stage;
+                if (++stage == nst) {
+                    stage = 0;
+                    phase ^= 1u;
+                }
+            }
+            wgmma_wait<0>();
+            // the other warpgroup may start tile local + 1
+            named_bar_arrive_if(local + 1 < my_tiles, 1 + (g ^ 1), 2 * 128);
+            wgmma_fence_acc(acc0);
+            wgmma_fence_acc(acc1);
+            if (t == 0) mbar_arrive(empty_bar(prev));
+            const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
+            // rows 0-63 from acc0, then rows 64-127 moved down into acc0: one copy of the epilogue code
+#pragma unroll 1
+            for (int h = 0; h < 2; ++h) {
+                const int rbase = m0 + 64 * h;
+                gemm_epilogue<BN>(gp.epi, gp.N, n0, acc0, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
+            }
+        }
     } else {
         setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
         // ===================== MMA + epilogue: warpgroup g owns rows [64 g, 64 g + 64) of every tile =====================
@@ -214,7 +303,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             if (t == 0) mbar_arrive(empty_bar(prev));
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
             const int rbase = m0 + 64 * g;
-            epilogue_frag<BN>(gp.epi, gp.N, n0, acc, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
+            gemm_epilogue<BN>(gp.epi, gp.N, n0, acc, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
         }
     }
 }
@@ -325,6 +414,11 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
         PPV_REQUIRE((epi.out_ld % 16) == 0 && (epi.out_col0 % 16) == 0 && (epi.out_plane_stride % 16) == 0 &&
                         (reinterpret_cast<uintptr_t>(epi.out) & 15) == 0,
                     "gemm_build: planes output must be 16-byte aligned");
+        // the layers of the ECAPA plan: the lean epilogue path covers everything they ask for
+        gp->epi.lean = (!epi.halo && !epi.zero_invalid && epi.img_Wp == 0 && !epi.seg_scale && !epi.silu_ && !epi.sigmoid_ &&
+                        !(epi.relu && epi.relu_max > 0.f) && !gp->epi.debug_nostore)
+                           ? 1
+                           : 0;
     } else {
         gp->epi.f32_vec_ok = ((epi.out_ld % 2) == 0 && (epi.out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(epi.out) & 7) == 0) ? 1 : 0;
     }

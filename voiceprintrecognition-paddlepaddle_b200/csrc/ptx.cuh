@@ -212,6 +212,24 @@ __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wa
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Predicated named-barrier wait / signal.  A branch around bar.sync makes ptxas serialise the wgmma pipeline of the MMA warpgroups;
+// a predicate does not.  arrive signals without waiting (the other `nthreads - arrivals` threads wait with named_bar_sync_if).
+__device__ __forceinline__ void named_bar_sync_if(bool pred, int id, int nthreads) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %2, 0;\n\t"
+        "@p bar.sync %0, %1;\n\t}\n" ::"r"(id),
+        "r"(nthreads), "r"(uint32_t(pred))
+        : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive_if(bool pred, int id, int nthreads) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %2, 0;\n\t"
+        "@p bar.arrive %0, %1;\n\t}\n" ::"r"(id),
+        "r"(nthreads), "r"(uint32_t(pred))
+        : "memory");
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -136,6 +136,8 @@ SIGNATURES = {
                                  C.POINTER(C.c_float), _P]),
     "ppv_gemm_test": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
                                 C.c_size_t, _P]),
+    "ppv_gemm_test_planes": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
 }
 
 _lib = None
