@@ -2,12 +2,14 @@
 
 python tools/model_bench.py [--models EcapaTdnn,ResNetSE,ERes2Net,CAMPPlus] [--batch 256] [--frames 298] [--iters 10]
                             [--precision bf16x3] [--once MODEL]   (--once: one warm forward only, for ncu launch lists)
-Prints one JSON line per model."""
+                            [--dump-outputs DIR]   (each model's last embeddings as float32 DIR/<model>.npy)
+Prints one JSON line per model.  Weights and inputs are seeded, so two builds can be compared output for output."""
 import argparse
 import json
 import os
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -44,13 +46,14 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--precision", default="bf16x3")
     ap.add_argument("--once", default="")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write each model's last embeddings to DIR/<model>.npy")
     ap.add_argument("--lanes", type=int, default=1, help="batches in flight: replica models on their own streams (see PPVectorPredictor._lanes)")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
     names = [a.once] if a.once else a.models.split(",")
     for name in names:
         m = randomize(MODELS[name](input_size=80, precision=a.precision).eval()).to(dev)
-        x = torch.randn(a.batch, a.frames, 80, device=dev)
+        x = torch.randn(a.batch, a.frames, 80, generator=torch.Generator().manual_seed(1)).to(dev)
         for _ in range(3):
             e = m(x)
         torch.cuda.synchronize()
@@ -66,6 +69,9 @@ def main():
         t1.record()
         torch.cuda.synchronize()
         ms = t0.elapsed_time(t1) / a.iters
+        if a.dump_outputs:
+            os.makedirs(a.dump_outputs, exist_ok=True)
+            np.save(os.path.join(a.dump_outputs, name + ".npy"), e.float().cpu().numpy())
         ws = _lib.load().ppv_model_workspace_bytes(m._get_handle(), a.batch, a.frames)
         line = {"model": name, "precision": a.precision, "batch": a.batch, "frames": a.frames, "ms_per_forward": round(ms, 3),
                 "utt_per_s": round(a.batch / ms * 1e3, 1), "workspace_GB": round(ws / 2**30, 2), "finite": bool(torch.isfinite(e).all())}

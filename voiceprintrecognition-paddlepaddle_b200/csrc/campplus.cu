@@ -60,7 +60,6 @@ struct CStep {
     PwStep pw;  // PW: 1x1 conv with K <= 64 on the CUDA cores (pointwise.cu)
     GemmParams gp;
     Conv3x3Params c3;  // CONV3: the 32 -> 32 channel 3x3 convs of the FCM head (conv3x3.cu)
-    int BN = 0;
     Planes a, b, d;
     const float *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr, *p4 = nullptr, *p5 = nullptr;
     float* fout = nullptr;
@@ -200,13 +199,8 @@ __global__ void __launch_bounds__(256) cp_flatten_pairs_kernel(Planes in, int B,
 
 }  // namespace
 
-struct CamppModel {
+struct CamppModel : Model {
     ppv_campplus_cfg cfg;
-    WeightMap raw;
-    bool finalized = false;
-    int precision = PPV_PREC_BF16X3;
-    int num_sms = 132;
-    void* arena = nullptr;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<ResBlockW> res;
     GemmWeights head_conv2, tdnn, dense;
@@ -216,13 +210,21 @@ struct CamppModel {
     int head_ch = 0, final_ch = 0;
     // plan
     std::vector<CStep> steps;
-    void* plan_ws = nullptr;
-    int plan_B = 0, plan_T = 0, T2 = 0, Tp = 0, nseg = 0;
+    int T2 = 0, Tp = 0, nseg = 0;
     ImageGeo geo[4];
     Planes stem_out, flat, tdnn_view, stats, final_x;
     Planes stage_out[4];
     Planes xblk[CP_NB], tr_out[CP_NB];
-    float* emb_out = nullptr;
+
+    explicit CamppModel(const ppv_campplus_cfg& c) : Model("campplus", c.precision), cfg(c) {}
+    int embd_dim() const override { return cfg.embd_dim; }
+    size_t workspace_bytes(int B, int T) const override;
+
+  protected:
+    bool prepare_weights(ArenaBuilder& ab) override;
+    int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
+    int run_steps(const float* feat, cudaStream_t st) override;
+    int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
 void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c) {
@@ -234,43 +236,21 @@ void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c) {
     c->precision = PPV_PREC_BF16X3;
 }
 
-int campplus_create(const ppv_campplus_cfg* cfg, CamppModel** out) {
+int campplus_create(const ppv_campplus_cfg* cfg, Model** out) {
     PPV_REQUIRE(cfg && out, "campplus_create: null argument");
     if (cfg->growth_rate != 32 || cfg->bn_size != 4 || cfg->init_channels != 128)
         return fail(PPV_EUNSUPPORTED, "campplus: growth_rate 32, bn_size 4, init_channels 128 (configs/cam++.yml) are implemented");
     if (cfg->input_size % 8 || cfg->input_size < 8 || cfg->embd_dim % 32)
         return fail(PPV_EUNSUPPORTED, "campplus: input_size % 8 and embd_dim % 32 required");
-    CamppModel* m = new CamppModel();
-    m->cfg = *cfg;
-    m->precision = cfg->precision;
+    CamppModel* m = new CamppModel(*cfg);
     m->head_ch = 32 * (cfg->input_size / 8);
-    m->num_sms = device_sm_count();
     *out = m;
     return PPV_OK;
 }
-void campplus_destroy(CamppModel* m) {
-    if (!m) return;
-    cudaFree(m->arena);
-    delete m;
-}
-int campplus_embd_dim(const CamppModel* m) { return m->cfg.embd_dim; }
-int campplus_set_precision(CamppModel* m, int precision) {
-    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "bad precision");
-    m->precision = precision;
-    return PPV_OK;
-}
-int campplus_load_weight(CamppModel* m, const char* name, const float* data, const int64_t* shape, int ndim) {
-    PPV_REQUIRE(m, "campplus_load_weight: null model");
-    if (m->finalized) return fail(PPV_ESTATE, "campplus_load_weight: model already finalized");
-    return weight_map_load(&m->raw, name, data, shape, ndim);
-}
 
 // ------------------------------------------------------------------------------------------------ finalize
-int campplus_finalize(CamppModel* m) {
-    PPV_REQUIRE(m, "campplus_finalize: null model");
-    if (m->finalized) return PPV_OK;
-    ArenaBuilder ab;
-    ab.wm = &m->raw;
+bool CamppModel::prepare_weights(ArenaBuilder& ab) {
+    CamppModel* const m = this;
     const ppv_campplus_cfg& cf = m->cfg;
     bool ok = true;
     const int G = cf.growth_rate, BC = cf.bn_size * cf.growth_rate;  // 32, 128
@@ -412,12 +392,7 @@ int campplus_finalize(CamppModel* m) {
     }
     m->final_ch = channels;
     if (ok) conv1d_matrix(&m->dense, "xvector.dense.linear", "xvector.dense.nonlinear.batchnorm", cf.embd_dim, 2 * channels, 1, 2 * channels);
-    if (!ok) return fail(PPV_EINVAL, "campplus_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
-    int rc = ab.upload(&m->arena);
-    if (rc) return rc;
-    m->raw.clear();
-    m->finalized = true;
-    return PPV_OK;
+    return ok;
 }
 
 // ------------------------------------------------------------------------------------------------ workspace / plan
@@ -469,21 +444,20 @@ void cp_carve(const CamppModel* m, WsCarver& cv, int B, int T, ImageGeo* geo, Cp
     cb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
-inline int cp_pick_bn(int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : 64; }
-
 }  // namespace
 
-size_t campplus_workspace_bytes(const CamppModel* m, int B, int T) {
-    if (!m || !m->finalized || B <= 0 || T <= 0) return 0;
+size_t CamppModel::workspace_bytes(int B, int T) const {
+    if (!finalized || B <= 0 || T <= 0) return 0;
     WsCarver cv;
-    ImageGeo geo[4];
+    ImageGeo g[4];
     CpBuffers cb;
-    cp_carve(m, cv, B, T, geo, &cb);
+    cp_carve(this, cv, B, T, g, &cb);
     return mc_align_up(cv.off, 256);
 }
 
-static int cp_build_plan(CamppModel* m, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-    const size_t need = campplus_workspace_bytes(m, B, T);
+int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+    CamppModel* const m = this;
+    const size_t need = workspace_bytes(B, T);
     PPV_REQUIRE(ws && ws_bytes >= need, "campplus: workspace too small (see ppv_model_workspace_bytes)");
     PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "campplus: workspace must be 256-byte aligned");
     PPV_REQUIRE(T >= 3, "campplus: too few frames (the statistics pooling needs at least two frames after the stride-2 TDNN)");
@@ -530,26 +504,14 @@ static int cp_build_plan(CamppModel* m, int B, int T, void* ws, size_t ws_bytes,
     };
     auto add_gemm = [&](const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) -> int {
         ep.bias = gw.bias;
-        if (pointwise_enabled() && ep.img_Wp > 0 && pointwise_supported(srcs.data(), int(srcs.size()), gw.N, ep)) {
-            CStep sp;
-            sp.kind = CStep::PW;
-            for (size_t i = 0; i < srcs.size(); ++i) sp.pw.srcs[i] = srcs[i];
-            sp.pw.nsrc = int(srcs.size());
-            sp.pw.N = gw.N;
-            sp.pw.M = M;
-            sp.pw.W = gw.W;
-            sp.pw.ep = ep;
-            m->steps.push_back(sp);
-            return PPV_OK;
-        }
         CStep s;
-        s.kind = CStep::GEMM;
-        s.BN = cp_pick_bn(gw.N);
-        int bk = 64;
-        for (const GemmSource& g : srcs)
-            if (g.ncols % 64) bk = 32;
-        int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, s.BN, bk);
-        if (rc) return rc;
+        if (pointwise_step_build(&s.pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) {
+            s.kind = CStep::PW;
+        } else {
+            s.kind = CStep::GEMM;
+            int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N));
+            if (rc) return rc;
+        }
         m->steps.push_back(s);
         return PPV_OK;
     };
@@ -700,31 +662,20 @@ static int cp_build_plan(CamppModel* m, int B, int T, void* ws, size_t ws_bytes,
     m->T2 = T2;
     m->Tp = Tp;
     m->nseg = nseg;
-    m->plan_ws = ws;
-    m->plan_B = B;
-    m->plan_T = T;
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int campplus_forward(CamppModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(m && feat && emb, "campplus_forward: null argument");
-    if (!m->finalized) return fail(PPV_ESTATE, "campplus_forward: call ppv_model_finalize first");
-    PPV_REQUIRE(B > 0 && T > 0, "campplus_forward: empty batch");
-    if (m->plan_ws != ws || m->plan_B != B || m->plan_T != T) {
-        int rc = cp_build_plan(m, B, T, ws, ws_bytes, st);
-        if (rc) {
-            m->plan_ws = nullptr;
-            return rc;
-        }
-    }
+int CamppModel::run_steps(const float* feat, cudaStream_t st) {
+    CamppModel* const m = this;
+    const int B = m->plan_B, T = m->plan_T;
     int rc = PPV_OK;
     for (const CStep& s : m->steps) {
         switch (s.kind) {
             case CStep::STEM:
                 rc = launch_stem_conv(feat, B, T, m->cfg.input_size, m->stem_w, m->stem_b, 32, m->stem_out, m->geo[0].Hp, m->geo[0].Wp, st);
                 break;
-            case CStep::GEMM: rc = gemm_launch(s.gp, s.BN, m->precision, m->num_sms, st); break;
+            case CStep::GEMM: rc = gemm_launch(s.gp, m->precision, m->num_sms, st); break;
             case CStep::CONV3: rc = conv3x3_launch(s.c3, m->precision, m->num_sms, st); break;
             case CStep::PW: rc = pointwise_launch(s.pw, m->num_sms, st); break;
             case CStep::ADD_RELU: rc = launch_se_scale_res(s.a, nullptr, s.b, 0, s.d, 0, s.C, s.img_rows, s.rows, m->num_sms, st, 1, 0.f); break;
@@ -752,16 +703,13 @@ int campplus_forward(CamppModel* m, const float* feat, int B, int T, float* emb,
         }
         if (rc) return rc;
     }
-    PPV_CUDA_OK(cudaMemcpyAsync(emb, m->emb_out, size_t(B) * m->cfg.embd_dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return PPV_OK;
 }
 
 // taps: "head.layer1", "head.layer2" -> fp32 [B,H,W,32]; "tdnn" [B,T2,128]; "block1".."block3" [B,T2,C]; "transit1", "transit2"
 // [B,T2,C/2]; "out_nonlinear" [B,T2,512] (transit3 + BN + ReLU); "stats" [B, 2*512]
-int campplus_read_tap(CamppModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st) {
-    PPV_REQUIRE(m && name && out, "campplus_read_tap: null argument");
-    if (!m->plan_ws) return fail(PPV_ESTATE, "campplus_read_tap: no forward has run");
-    const std::string n(name);
+int CamppModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {
+    CamppModel* const m = this;
     const int B = m->plan_B;
     if (n == "stats") {
         PPV_REQUIRE(out_elems >= size_t(B) * 2 * m->final_ch, "campplus_read_tap: output too small");

@@ -5,6 +5,7 @@
 #include <new>
 
 #include "common.h"
+#include "model_common.h"
 
 namespace ppv {
 
@@ -52,11 +53,11 @@ struct ppv_trainer {
 
 struct ppv_model {
     int kind;
-    EcapaModel* ecapa;
-    ResNetSEModel* resnet;
-    ERes2NetModel* eres;
-    CamppModel* campp;
+    Model* m;
 };
+
+// The model behind an ECAPA-TDNN handle, else null: the entry points that only ECAPA-TDNN has.
+static Model* ecapa_of(const ppv_model* h) { return h && h->kind == PPV_MODEL_ECAPA_TDNN ? h->m : nullptr; }
 
 #define PPV_GUARD_BEGIN try {
 #define PPV_GUARD_END                                                        \
@@ -143,23 +144,8 @@ int ppv_audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, con
 
 // ---------------------------------------------------------------- model
 void ppv_ecapa_default_cfg(ppv_ecapa_cfg* c) {
-    if (!c) return;
-    c->input_size = 80;
-    c->embd_dim = 192;
-    const int ch[5] = {512, 512, 512, 512, 1536}, ks[5] = {5, 3, 3, 3, 1}, dl[5] = {1, 2, 3, 4, 1};
-    for (int i = 0; i < 5; ++i) {
-        c->channels[i] = ch[i];
-        c->kernel_sizes[i] = ks[i];
-        c->dilations[i] = dl[i];
-    }
-    c->attention_channels = 128;
-    c->res2net_scale = 8;
-    c->se_channels = 128;
-    c->precision = PPV_PREC_BF16X3;
-    c->pooling = PPV_POOL_ASP;
-    c->global_context = 1;
+    if (c) ppv_ecapa_default_cfg_impl(c);
 }
-
 void ppv_eres2net_default_cfg(ppv_eres2net_cfg* c) {
     if (c) ppv_eres2net_default_cfg_impl(c);
 }
@@ -178,113 +164,71 @@ int ppv_model_create(int kind, const void* cfg, ppv_model_t** out) {
                     "ppv_model_create: implemented kinds are PPV_MODEL_ECAPA_TDNN, PPV_MODEL_RESNET_SE, PPV_MODEL_ERES2NET, PPV_MODEL_CAMPPLUS");
     int rc = check_device();
     if (rc) return rc;
-    if (kind == PPV_MODEL_RESNET_SE) {
-        ResNetSEModel* r = nullptr;
-        rc = resnetse_create(static_cast<const ppv_resnetse_cfg*>(cfg), &r);
-        if (rc) return rc;
-        *out = new ppv_model{kind, nullptr, r, nullptr, nullptr};
-        return PPV_OK;
+    Model* m = nullptr;
+    switch (kind) {
+        case PPV_MODEL_ECAPA_TDNN: rc = ecapa_create(static_cast<const ppv_ecapa_cfg*>(cfg), &m); break;
+        case PPV_MODEL_RESNET_SE: rc = resnetse_create(static_cast<const ppv_resnetse_cfg*>(cfg), &m); break;
+        case PPV_MODEL_ERES2NET: rc = eres2net_create(static_cast<const ppv_eres2net_cfg*>(cfg), &m); break;
+        default: rc = campplus_create(static_cast<const ppv_campplus_cfg*>(cfg), &m); break;
     }
-    if (kind == PPV_MODEL_ERES2NET) {
-        ERes2NetModel* e = nullptr;
-        rc = eres2net_create(static_cast<const ppv_eres2net_cfg*>(cfg), &e);
-        if (rc) return rc;
-        *out = new ppv_model{kind, nullptr, nullptr, e, nullptr};
-        return PPV_OK;
-    }
-    if (kind == PPV_MODEL_CAMPPLUS) {
-        CamppModel* c = nullptr;
-        rc = campplus_create(static_cast<const ppv_campplus_cfg*>(cfg), &c);
-        if (rc) return rc;
-        *out = new ppv_model{kind, nullptr, nullptr, nullptr, c};
-        return PPV_OK;
-    }
-    EcapaModel* m = nullptr;
-    rc = ecapa_create(static_cast<const ppv_ecapa_cfg*>(cfg), &m);
     if (rc) return rc;
-    *out = new ppv_model{kind, m, nullptr, nullptr, nullptr};
+    *out = new ppv_model{kind, m};
     return PPV_OK;
     PPV_GUARD_END
 }
 int ppv_model_destroy(ppv_model_t* h) {
     if (!h) return PPV_OK;
-    ecapa_destroy(h->ecapa);
-    resnetse_destroy(h->resnet);
-    eres2net_destroy(h->eres);
-    campplus_destroy(h->campp);
+    delete h->m;
     delete h;
     return PPV_OK;
 }
 int ppv_model_load_weight(ppv_model_t* h, const char* name, const float* data, const int64_t* shape, int ndim) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h, "ppv_model_load_weight: null model");
-    if (h->resnet) return resnetse_load_weight(h->resnet, name, data, shape, ndim);
-    if (h->eres) return eres2net_load_weight(h->eres, name, data, shape, ndim);
-    if (h->campp) return campplus_load_weight(h->campp, name, data, shape, ndim);
-    return ecapa_load_weight(h->ecapa, name, data, shape, ndim);
+    return h->m->load_weight(name, data, shape, ndim);
     PPV_GUARD_END
 }
 int ppv_model_finalize(ppv_model_t* h) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h, "ppv_model_finalize: null model");
-    if (h->resnet) return resnetse_finalize(h->resnet);
-    if (h->eres) return eres2net_finalize(h->eres);
-    if (h->campp) return campplus_finalize(h->campp);
-    return ecapa_finalize(h->ecapa);
+    return h->m->finalize();
     PPV_GUARD_END
 }
 int ppv_model_set_precision(ppv_model_t* h, int precision) {
     PPV_REQUIRE(h, "ppv_model_set_precision: null model");
-    if (h->resnet) return resnetse_set_precision(h->resnet, precision);
-    if (h->eres) return eres2net_set_precision(h->eres, precision);
-    if (h->campp) return campplus_set_precision(h->campp, precision);
-    return ecapa_set_precision(h->ecapa, precision);
+    return h->m->set_precision(precision);
 }
-int ppv_model_embd_dim(const ppv_model_t* h) {
-    if (!h) return 0;
-    if (h->campp) return campplus_embd_dim(h->campp);
-    return h->resnet ? resnetse_embd_dim(h->resnet) : h->eres ? eres2net_embd_dim(h->eres) : ecapa_embd_dim(h->ecapa);
-}
-size_t ppv_model_workspace_bytes(const ppv_model_t* h, int B, int T) {
-    if (h && h->campp) return campplus_workspace_bytes(h->campp, B, T);
-    return !h ? 0 : h->resnet ? resnetse_workspace_bytes(h->resnet, B, T) : h->eres ? eres2net_workspace_bytes(h->eres, B, T)
-                                                                              : ecapa_workspace_bytes(h->ecapa, B, T);
-}
+int ppv_model_embd_dim(const ppv_model_t* h) { return h ? h->m->embd_dim() : 0; }
+size_t ppv_model_workspace_bytes(const ppv_model_t* h, int B, int T) { return h ? h->m->workspace_bytes(B, T) : 0; }
 
 int ppv_model_forward(ppv_model_t* h, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && feat && emb, "ppv_model_forward: null argument");
-    if (h->resnet) return resnetse_forward(h->resnet, feat, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
-    if (h->eres) return eres2net_forward(h->eres, feat, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
-    if (h->campp) return campplus_forward(h->campp, feat, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
-    return ecapa_forward(h->ecapa, feat, nullptr, nullptr, nullptr, B, T, 0, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    return h->m->forward(feat, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 int ppv_model_forward_lengths(ppv_model_t* h, const float* feat, const float* lengths, int B, int T, float* emb, void* ws, size_t ws_bytes,
                               void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && feat && emb, "ppv_model_forward_lengths: null argument");
-    if (!h->ecapa) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_lengths: only EcapaTdnn.forward takes lengths in the reference");
-    return ecapa_forward(h->ecapa, feat, nullptr, nullptr, nullptr, B, T, 0, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream), lengths);
+    if (!ecapa_of(h)) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_lengths: only EcapaTdnn.forward takes lengths in the reference");
+    return ecapa_forward(h->m, feat, nullptr, nullptr, nullptr, B, T, 0, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream), lengths);
     PPV_GUARD_END
 }
 int ppv_model_forward_wav(ppv_model_t* h, ppv_fbank_t* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb,
                           void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && fb && wav && emb, "ppv_model_forward_wav: null argument");
-    if (h->resnet || h->eres || h->campp) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_wav: the fused waveform path exists for ECAPA-TDNN only; call ppv_fbank_forward + ppv_model_forward");
+    if (!ecapa_of(h)) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_wav: the fused waveform path exists for ECAPA-TDNN only; call ppv_fbank_forward + ppv_model_forward");
     const int T = fbank_num_frames(fb->impl, L);
     PPV_REQUIRE(T > 0, "ppv_model_forward_wav: waveform shorter than one frame");
-    return ecapa_forward(h->ecapa, nullptr, fb->impl, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    return ecapa_forward(h->m, nullptr, fb->impl, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 int ppv_model_read_tap(ppv_model_t* h, const char* name, float* out, size_t out_elems, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h, "ppv_model_read_tap: null model");
-    if (h->resnet) return resnetse_read_tap(h->resnet, name, out, out_elems, static_cast<cudaStream_t>(stream));
-    if (h->eres) return eres2net_read_tap(h->eres, name, out, out_elems, static_cast<cudaStream_t>(stream));
-    if (h->campp) return campplus_read_tap(h->campp, name, out, out_elems, static_cast<cudaStream_t>(stream));
-    return ecapa_read_tap(h->ecapa, name, out, out_elems, static_cast<cudaStream_t>(stream));
+    return h->m->read_tap(name, out, out_elems, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 
@@ -311,13 +255,13 @@ int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* be
 }
 
 int ppv_model_profile(ppv_model_t* h, int enable) {
-    PPV_REQUIRE(h && h->ecapa, "ppv_model_profile: ECAPA-TDNN model required");
-    return ecapa_profile(h->ecapa, enable);
+    PPV_REQUIRE(ecapa_of(h), "ppv_model_profile: ECAPA-TDNN model required");
+    return ecapa_profile(h->m, enable);
 }
 int ppv_model_profile_read(ppv_model_t* h, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(h && h->ecapa, "ppv_model_profile_read: ECAPA-TDNN model required");
-    return ecapa_profile_read(h->ecapa, gemm_ms, other_ms, gemm_launches, other_launches);
+    PPV_REQUIRE(ecapa_of(h), "ppv_model_profile_read: ECAPA-TDNN model required");
+    return ecapa_profile_read(h->m, gemm_ms, other_ms, gemm_launches, other_launches);
     PPV_GUARD_END
 }
 
@@ -504,7 +448,7 @@ int ppv_gemm_test(const float* A, const float* W, const float* bias, const float
     GemmParams gp;
     rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, block_k);
     if (rc) return rc;
-    return gemm_launch(gp, block_n, precision, device_sm_count(), st);
+    return gemm_launch(gp, precision, device_sm_count(), st);
     PPV_GUARD_END
 }
 
@@ -556,7 +500,7 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
     GemmParams gp;
     rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, 64);
     if (rc) return rc;
-    return gemm_launch(gp, block_n, precision, device_sm_count(), st);
+    return gemm_launch(gp, precision, device_sm_count(), st);
     PPV_GUARD_END
 }
 
@@ -605,12 +549,12 @@ int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision,
     int rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, block_k);
     if (rc) return rc;
     const int sms = device_sm_count();
-    for (int i = 0; i < 3; ++i) { rc = gemm_launch(gp, block_n, precision, sms, st); if (rc) return rc; }
+    for (int i = 0; i < 3; ++i) { rc = gemm_launch(gp, precision, sms, st); if (rc) return rc; }
     cudaEvent_t e0, e1;
     PPV_CUDA_OK(cudaEventCreate(&e0));
     PPV_CUDA_OK(cudaEventCreate(&e1));
     PPV_CUDA_OK(cudaEventRecord(e0, st));
-    for (int i = 0; i < iters; ++i) { rc = gemm_launch(gp, block_n, precision, sms, st); if (rc) return rc; }
+    for (int i = 0; i < iters; ++i) { rc = gemm_launch(gp, precision, sms, st); if (rc) return rc; }
     PPV_CUDA_OK(cudaEventRecord(e1, st));
     PPV_CUDA_OK(cudaEventSynchronize(e1));
     float ms = 0.f;

@@ -158,6 +158,7 @@ struct GemmParams {
     int M, N;
     int m_tiles, n_tiles;
     Epilogue epi;
+    int bn;  // n-tile width (64, 128 or 256): selects the kernel instance.  Last, so that no kernel parameter offset depends on it.
 };
 
 struct GemmSource {
@@ -170,11 +171,18 @@ struct GemmSource {
 // Precision of the tensor-core contraction.
 //   PPV_PREC_BF16X3: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo  (fp32-grade, ~2^-16 relative per product)
 //   PPV_PREC_BF16  : A_hi*B_hi only
+// BK = 0: 64, or 32 where a source's K slice is not a multiple of 64.
 int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W, int M, int N, const Epilogue& epi,
-               int BN, int BK = GEMM_BK);
+               int BN, int BK = 0);
 int gemm_build_wgrad(GemmParams* gp, const Planes& At, const Planes& Bt, int M, int N, int b_row0, int b_col0, int splits, float* out,
                      int64_t out_ld, int out_col0, int64_t split_rows, int BN);
-int gemm_launch(const GemmParams& gp, int BN, int precision, int num_sms, cudaStream_t stream);
+int gemm_launch(const GemmParams& gp, int precision, int num_sms, cudaStream_t stream);
+// The widest n-tile, up to max_bn, that divides N (64 at least).
+inline int gemm_pick_bn(int N, int max_bn = 256) {
+    for (int bn = max_bn; bn > 64; bn /= 2)
+        if (N % bn == 0) return bn;
+    return 64;
+}
 int gemm_max_smem_setup();
 
 int encode_planes_map(CUtensorMap* m, const Planes& t, int box_rows);  // 3-D TMA map over split planes, box {64, box_rows, 1}, SWIZZLE_128B
@@ -227,7 +235,6 @@ bool res2chain_fits(int T, int P);
 void res2chain_trace_dump(const Res2ChainParams& cp);
 
 // ---- 1x1 convs with K <= 64 on the CUDA cores, one thread per grid position (pointwise.cu) ----------------------------
-bool pointwise_supported(const GemmSource* srcs, int nsrc, int N, const Epilogue& ep);
 int pointwise_launch(const GemmSource* srcs, int nsrc, const Planes& W, int64_t M, int N, const Epilogue& ep, int num_sms, cudaStream_t st);
 struct PwStep {  // a planned pointwise conv (the model plans keep these next to their GemmParams)
     GemmSource srcs[2];
@@ -237,11 +244,9 @@ struct PwStep {  // a planned pointwise conv (the model plans keep these next to
     Epilogue ep;
 };
 inline int pointwise_launch(const PwStep& s, int num_sms, cudaStream_t st) { return pointwise_launch(s.srcs, s.nsrc, s.W, s.M, s.N, s.ep, num_sms, st); }
-// PPV_POINTWISE=0 keeps these layers on the gather-GEMM (A-B timing)
-inline bool pointwise_enabled() {
-    const char* e = getenv("PPV_POINTWISE");
-    return !(e && e[0] == '0');
-}
+// Plans a 1x1 conv over an image grid on the CUDA cores where pointwise_launch supports it; false: it takes the gather-GEMM.
+// PPV_POINTWISE=0 keeps every such layer on the gather-GEMM (A-B timing).
+bool pointwise_step_build(PwStep* s, const GemmSource* srcs, int nsrc, const Planes& W, int N, int64_t M, const Epilogue& ep);
 
 // ---- skinny linear layers on the CUDA cores (skinny.cu): [B x K] x [K x N] with one row per utterance ----------------
 bool skinny_linear_supported(int M, int N, int K, const Epilogue& ep);
@@ -303,20 +308,21 @@ int spectral_feature_dim(const Spectral* h);
 int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st);
 int spec_augment_run(float* feat, const int32_t* params, int B, int T, int F, int n_freq_masks, int n_time_masks, int fill_mode, cudaStream_t st);
 
-// ---- ecapa.cu ---------------------------------------------------------------------------------------
-struct EcapaModel;
-int ecapa_create(const ppv_ecapa_cfg* cfg, EcapaModel** out);
-void ecapa_destroy(EcapaModel* m);
-int ecapa_load_weight(EcapaModel* m, const char* name, const float* data, const int64_t* shape, int ndim);
-int ecapa_finalize(EcapaModel* m);
-int ecapa_set_precision(EcapaModel* m, int precision);
-int ecapa_embd_dim(const EcapaModel* m);
-size_t ecapa_workspace_bytes(const EcapaModel* m, int B, int T);
-int ecapa_forward(EcapaModel* m, const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L,
-                  float* emb, void* ws, size_t ws_bytes, cudaStream_t st, const float* lengths = nullptr);
-int ecapa_read_tap(EcapaModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st);
-int ecapa_profile(EcapaModel* m, int enable);
-int ecapa_profile_read(EcapaModel* m, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches);
+// ---- model factories (ecapa.cu, resnet_se.cu, eres2net.cu, campplus.cu; the Model interface is in model_common.h) -------------
+struct Model;
+void ppv_ecapa_default_cfg_impl(ppv_ecapa_cfg* c);
+int ecapa_create(const ppv_ecapa_cfg* cfg, Model** out);
+// ECAPA-TDNN only (m must be one): waveform input through `fb`, `lengths`, and the launch-group profile
+int ecapa_forward(Model* m, const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb,
+                  void* ws, size_t ws_bytes, cudaStream_t st, const float* lengths = nullptr);
+int ecapa_profile(Model* m, int enable);
+int ecapa_profile_read(Model* m, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches);
+void ppv_resnetse_default_cfg_impl(ppv_resnetse_cfg* c);
+int resnetse_create(const ppv_resnetse_cfg* cfg, Model** out);
+void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c);
+int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out);
+void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);
+int campplus_create(const ppv_campplus_cfg* cfg, Model** out);
 
 // ---- conv2d models: zero-bordered NHWC image grids (resnet_se.cu, eres2net.cu) ------------------------
 struct ImageGeo {
@@ -332,45 +338,6 @@ int launch_image_to_f32(const Planes& in, int B, int H, int W, int Hp, int Wp, i
 // xo = x * (1 + t) + y * (1 - t)  (AFF blend, eres2net.py:50-51 with t = tanh(att)); all rows
 int launch_aff_combine(const Planes& x, int xc0, const Planes& y, int yc0, const Planes& t, const Planes& out, int C, int64_t rows, int num_sms,
                        cudaStream_t st);
-
-// ---- resnet_se.cu -----------------------------------------------------------------------------------
-struct ResNetSEModel;
-void ppv_resnetse_default_cfg_impl(ppv_resnetse_cfg* c);
-int resnetse_create(const ppv_resnetse_cfg* cfg, ResNetSEModel** out);
-void resnetse_destroy(ResNetSEModel* m);
-int resnetse_load_weight(ResNetSEModel* m, const char* name, const float* data, const int64_t* shape, int ndim);
-int resnetse_finalize(ResNetSEModel* m);
-int resnetse_set_precision(ResNetSEModel* m, int precision);
-int resnetse_embd_dim(const ResNetSEModel* m);
-size_t resnetse_workspace_bytes(const ResNetSEModel* m, int B, int T);
-int resnetse_forward(ResNetSEModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st);
-int resnetse_read_tap(ResNetSEModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st);
-
-// ---- eres2net.cu ------------------------------------------------------------------------------------
-struct ERes2NetModel;
-void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c);
-int eres2net_create(const ppv_eres2net_cfg* cfg, ERes2NetModel** out);
-void eres2net_destroy(ERes2NetModel* m);
-int eres2net_load_weight(ERes2NetModel* m, const char* name, const float* data, const int64_t* shape, int ndim);
-int eres2net_finalize(ERes2NetModel* m);
-int eres2net_set_precision(ERes2NetModel* m, int precision);
-int eres2net_embd_dim(const ERes2NetModel* m);
-size_t eres2net_workspace_bytes(const ERes2NetModel* m, int B, int T);
-int eres2net_forward(ERes2NetModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st);
-int eres2net_read_tap(ERes2NetModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st);
-
-// ---- campplus.cu ------------------------------------------------------------------------------------
-struct CamppModel;
-void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);
-int campplus_create(const ppv_campplus_cfg* cfg, CamppModel** out);
-void campplus_destroy(CamppModel* m);
-int campplus_load_weight(CamppModel* m, const char* name, const float* data, const int64_t* shape, int ndim);
-int campplus_finalize(CamppModel* m);
-int campplus_set_precision(CamppModel* m, int precision);
-int campplus_embd_dim(const CamppModel* m);
-size_t campplus_workspace_bytes(const CamppModel* m, int B, int T);
-int campplus_forward(CamppModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st);
-int campplus_read_tap(CamppModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st);
 
 // ---- ecapa_train.cu / train_kernels.cu ---------------------------------------------------------------
 struct Trainer;

@@ -65,10 +65,9 @@ int cosine_matrix(const float* A, const float* Bm, int M, int N, int D, float* o
     ep.out = out;
     ep.out_ld = N;
     GemmParams gp;
-    const int BN = 128;
-    int rc = gemm_build(&gp, &src, 1, pb, M, N, ep, BN);
+    int rc = gemm_build(&gp, &src, 1, pb, M, N, ep, 128);
     if (rc) return rc;
-    return gemm_launch(gp, BN, precision, device_sm_count(), st);
+    return gemm_launch(gp, precision, device_sm_count(), st);
 }
 
 // pair list: 8 lanes per pair, float4 loads

@@ -57,7 +57,6 @@ struct TStep {
         HEAD_BWD, ASP_BWD, COLSUM, BN_BWD, WGRAD, ASP_CTX_BWD, GRAD_SUM, SE_BWD
     } kind;
     GemmParams gp;
-    int BN = 0;
     int a = 0, b = 0;  // small integer arguments (block index, split counts)
     GradSrcList gl;
     BnApplyArgs ap;
@@ -375,7 +374,6 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
     int rc;
 
     auto push = [&](const TStep& s) { t->steps.push_back(s); };
-    auto pick_bn = [](int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : 64; };
     // forward conv: bias + ReLU -> post-activation planes (valid frames)
     auto fwd_gemm = [&](const TConv& c, const std::vector<GemmSource>& srcs, const Planes& out, int out_col0, bool relu, const float* rowgrp,
                         float* out_f32) -> int {
@@ -399,8 +397,7 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         ep.T = T;
         TStep s;
         s.kind = TStep::GEMM;
-        s.BN = pick_bn(c.Cout);
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wf, M, c.Cout, ep, s.BN);
+        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wf, M, c.Cout, ep, gemm_pick_bn(c.Cout));
         if (r) return r;
         push(s);
         return PPV_OK;
@@ -438,9 +435,8 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         ep.out_col0 = out_col0;
         TStep s;
         s.kind = TStep::GEMM;
-        s.BN = pick_bn(c.Cinp);
         std::vector<GemmSource> srcs = taps_of(c, dz, dz_col0, -1);
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wd, M, c.Cinp, ep, s.BN);
+        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wd, M, c.Cinp, ep, gemm_pick_bn(c.Cinp));
         if (r) return r;
         push(s);
         return PPV_OK;
@@ -460,14 +456,13 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
             s.trs.push_back(tr);
         }
         const int N = c.taps * c.Cinp;
-        const int BNw = pick_bn(N);
+        const int BNw = gemm_pick_bn(N);
         const int mt = (c.Cout + 127) / 128, nt = (N + BNw - 1) / BNw;
         const int splits = std::max(1, std::min((t->num_sms + mt * nt - 1) / (mt * nt), int((t->Rp + 63) / 64)));
         GemmParams gp;
         int r = gemm_build_wgrad(&gp, t->TA, t->TB, c.Cout, N, 0, 0, splits, t->wpart, N, 0, int64_t(mt) * 128, BNw);
         if (r) return r;
         s.wg.push_back(gp);
-        s.BN = BNw;
         s.a = gp.lin_splits;
         s.b = mt * 128;
         push(s);
@@ -737,7 +732,7 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
                 break;
             }
             case TStep::PACK: rc = launch_pack_features(feat, B, T, t->cfg.input_size, t->X0, P, Tp, st); break;
-            case TStep::GEMM: rc = gemm_launch(s.gp, s.BN, t->precision, t->num_sms, st); break;
+            case TStep::GEMM: rc = gemm_launch(s.gp, t->precision, t->num_sms, st); break;
             case TStep::BN_FWD: {
                 const TBN& bn = t->L[s.layer].bn;
                 rc = tr_bn_forward(s.p0, s.c0, bn.C, B, T, P, Tp, TR_BN_EPS, TR_BN_MOMENTUM, par + bn.g_off, par + bn.b_off, bn.mean, bn.rstd, bn.scale,
@@ -839,7 +834,7 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
                     if (rc) return rc;
                 }
                 for (const GemmParams& gp : s.wg) {
-                    rc = gemm_launch(gp, s.BN, t->precision, t->num_sms, st);
+                    rc = gemm_launch(gp, t->precision, t->num_sms, st);
                     if (rc) return rc;
                 }
                 rc = tr_wgrad_unpack(t->wpart, s.a, s.b, c.Cout, c.Cin, c.Cinp, c.taps, grd + c.w_off, int64_t(c.CinTotal) * c.taps, st);

@@ -47,7 +47,6 @@ struct EStep {
     PwStep pw;  // PW: 1x1 conv with K <= 64 on the CUDA cores (pointwise.cu)
     Conv3x3Params c3;  // CONV3: single-source 3x3 conv over a 32-channel (padded) chunk, conv3x3.cu
     GemmParams gp;
-    int BN = 0;
     Planes a, b, c, d;
     int ac0 = 0, bc0 = 0, C = 0, img_rows = 0;
     int64_t rows = 0;
@@ -55,13 +54,8 @@ struct EStep {
 
 }  // namespace
 
-struct ERes2NetModel {
+struct ERes2NetModel : Model {
     ppv_eres2net_cfg cfg;
-    WeightMap raw;
-    bool finalized = false;
-    int precision = PPV_PREC_BF16X3;
-    int num_sms = 132;
-    void* arena = nullptr;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<EBlockW> blocks;
     EFuseW fuse[3];
@@ -70,14 +64,21 @@ struct ERes2NetModel {
     int stats_ch = 0;  // 512 * F'
     // plan
     std::vector<EStep> steps;
-    void* plan_ws = nullptr;
-    int plan_B = 0, plan_T = 0;
     ImageGeo geo[5];
     Planes stem_out, flat, stats;
     std::vector<Planes> blk_out;
     Planes fuse_out[3];
-    float* emb_out = nullptr;
     int Tf = 0;
+
+    explicit ERes2NetModel(const ppv_eres2net_cfg& c) : Model("eres2net", c.precision), cfg(c) {}
+    int embd_dim() const override { return cfg.embd_dim; }
+    size_t workspace_bytes(int B, int T) const override;
+
+  protected:
+    bool prepare_weights(ArenaBuilder& ab) override;
+    int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
+    int run_steps(const float* feat, cudaStream_t st) override;
+    int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
 void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c) {
@@ -91,7 +92,7 @@ void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c) {
     c->base_width = 32;
 }
 
-int eres2net_create(const ppv_eres2net_cfg* cfg, ERes2NetModel** out) {
+int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out) {
     PPV_REQUIRE(cfg && out, "eres2net_create: null argument");
     int nblocks = 0;
     for (int i = 0; i < 4; ++i) {
@@ -104,37 +105,15 @@ int eres2net_create(const ppv_eres2net_cfg* cfg, ERes2NetModel** out) {
     if (cfg->version != 0 && cfg->version != 1 && cfg->version != 2) return fail(PPV_EUNSUPPORTED, "eres2net: version must be 1 (ERes2Net) or 2 (ERes2NetV2)");
     if (cfg->version != 2 && cfg->base_width != 0 && cfg->base_width != 32) return fail(PPV_EUNSUPPORTED, "eres2net: ERes2Net is built for base_width 32");
     if (cfg->version == 2 && cfg->base_width != 0 && (cfg->base_width < 8 || cfg->base_width > 32)) return fail(PPV_EUNSUPPORTED, "eres2net: ERes2NetV2 base_width must be in [8, 32]");
-    ERes2NetModel* m = new ERes2NetModel();
-    m->cfg = *cfg;
-    m->precision = cfg->precision;
+    ERes2NetModel* m = new ERes2NetModel(*cfg);
     m->stats_ch = (cfg->input_size / 8) * cfg->m_channels * 16;
-    m->num_sms = device_sm_count();
     *out = m;
     return PPV_OK;
 }
-void eres2net_destroy(ERes2NetModel* m) {
-    if (!m) return;
-    cudaFree(m->arena);
-    delete m;
-}
-int eres2net_embd_dim(const ERes2NetModel* m) { return m->cfg.embd_dim; }
-int eres2net_set_precision(ERes2NetModel* m, int precision) {
-    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "bad precision");
-    m->precision = precision;
-    return PPV_OK;
-}
-int eres2net_load_weight(ERes2NetModel* m, const char* name, const float* data, const int64_t* shape, int ndim) {
-    PPV_REQUIRE(m, "eres2net_load_weight: null model");
-    if (m->finalized) return fail(PPV_ESTATE, "eres2net_load_weight: model already finalized");
-    return weight_map_load(&m->raw, name, data, shape, ndim);
-}
 
 // ------------------------------------------------------------------------------------------------ finalize
-int eres2net_finalize(ERes2NetModel* m) {
-    PPV_REQUIRE(m, "eres2net_finalize: null model");
-    if (m->finalized) return PPV_OK;
-    ArenaBuilder ab;
-    ab.wm = &m->raw;
+bool ERes2NetModel::prepare_weights(ArenaBuilder& ab) {
+    ERes2NetModel* const m = this;
     const ppv_eres2net_cfg& cf = m->cfg;
     bool ok = true;
     // One K group of a dense weight matrix: `ncols` source columns per tap, of which columns [pos, pos+cnt) carry the conv's
@@ -259,12 +238,7 @@ int eres2net_finalize(ERes2NetModel* m) {
             ok = false;
         }
     }
-    if (!ok) return fail(PPV_EINVAL, "eres2net_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
-    int rc = ab.upload(&m->arena);
-    if (rc) return rc;
-    m->raw.clear();
-    m->finalized = true;
-    return PPV_OK;
+    return ok;
 }
 
 // ------------------------------------------------------------------------------------------------ workspace / plan
@@ -345,21 +319,20 @@ void er_carve(const ERes2NetModel* m, WsCarver& cv, int B, int T, ImageGeo* geo,
     eb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
-inline int er_pick_bn(int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : 64; }
-
 }  // namespace
 
-size_t eres2net_workspace_bytes(const ERes2NetModel* m, int B, int T) {
-    if (!m || !m->finalized || B <= 0 || T <= 0) return 0;
+size_t ERes2NetModel::workspace_bytes(int B, int T) const {
+    if (!finalized || B <= 0 || T <= 0) return 0;
     WsCarver cv;
-    ImageGeo geo[5];
+    ImageGeo g[5];
     ErBuffers eb;
-    er_carve(m, cv, B, T, geo, &eb);
+    er_carve(this, cv, B, T, g, &eb);
     return mc_align_up(cv.off, 256);
 }
 
-static int er_build_plan(ERes2NetModel* m, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-    const size_t need = eres2net_workspace_bytes(m, B, T);
+int ERes2NetModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+    ERes2NetModel* const m = this;
+    const size_t need = workspace_bytes(B, T);
     PPV_REQUIRE(ws && ws_bytes >= need, "eres2net: workspace too small (see ppv_model_workspace_bytes)");
     PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "eres2net: workspace must be 256-byte aligned");
     PPV_REQUIRE(T >= 16, "eres2net: too few frames (TSTP needs at least two pooled frames)");
@@ -388,26 +361,14 @@ static int er_build_plan(ERes2NetModel* m, int B, int T, void* ws, size_t ws_byt
     };
     auto add_gemm = [&](const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) -> int {
         ep.bias = gw.bias;
-        if (pointwise_enabled() && ep.img_Wp > 0 && pointwise_supported(srcs.data(), int(srcs.size()), gw.N, ep)) {
-            EStep sp;
-            sp.kind = EStep::PW;
-            for (size_t i = 0; i < srcs.size(); ++i) sp.pw.srcs[i] = srcs[i];
-            sp.pw.nsrc = int(srcs.size());
-            sp.pw.N = gw.N;
-            sp.pw.M = M;
-            sp.pw.W = gw.W;
-            sp.pw.ep = ep;
-            m->steps.push_back(sp);
-            return PPV_OK;
-        }
         EStep s;
-        s.kind = EStep::GEMM;
-        s.BN = er_pick_bn(gw.N);
-        int bk = 64;
-        for (const GemmSource& g : srcs)
-            if (g.ncols % 64) bk = 32;
-        int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, s.BN, bk);
-        if (rc) return rc;
+        if (pointwise_step_build(&s.pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) {
+            s.kind = EStep::PW;
+        } else {
+            s.kind = EStep::GEMM;
+            int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N));
+            if (rc) return rc;
+        }
         m->steps.push_back(s);
         return PPV_OK;
     };
@@ -550,31 +511,20 @@ static int er_build_plan(ERes2NetModel* m, int B, int T, void* ws, size_t ws_byt
     for (int i = m->fuse_first; i < 3; ++i) m->fuse_out[i] = eb.fout[i];
     m->emb_out = eb.emb_out;
     m->Tf = m->geo[4].W;
-    m->plan_ws = ws;
-    m->plan_B = B;
-    m->plan_T = T;
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int eres2net_forward(ERes2NetModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(m && feat && emb, "eres2net_forward: null argument");
-    if (!m->finalized) return fail(PPV_ESTATE, "eres2net_forward: call ppv_model_finalize first");
-    PPV_REQUIRE(B > 0 && T > 0, "eres2net_forward: empty batch");
-    if (m->plan_ws != ws || m->plan_B != B || m->plan_T != T) {
-        int rc = er_build_plan(m, B, T, ws, ws_bytes, st);
-        if (rc) {
-            m->plan_ws = nullptr;
-            return rc;
-        }
-    }
+int ERes2NetModel::run_steps(const float* feat, cudaStream_t st) {
+    ERes2NetModel* const m = this;
+    const int B = m->plan_B, T = m->plan_T;
     int rc = PPV_OK;
     for (const EStep& s : m->steps) {
         switch (s.kind) {
             case EStep::STEM:
                 rc = launch_stem_conv(feat, B, T, m->cfg.input_size, m->stem_w, m->stem_b, m->cfg.m_channels, m->stem_out, m->geo[1].Hp, m->geo[1].Wp, st);
                 break;
-            case EStep::GEMM: rc = gemm_launch(s.gp, s.BN, m->precision, m->num_sms, st); break;
+            case EStep::GEMM: rc = gemm_launch(s.gp, m->precision, m->num_sms, st); break;
             case EStep::CONV3: rc = conv3x3_launch(s.c3, m->precision, m->num_sms, st); break;
             case EStep::PW: rc = pointwise_launch(s.pw, m->num_sms, st); break;
             case EStep::ADD_RELU:
@@ -590,15 +540,12 @@ int eres2net_forward(ERes2NetModel* m, const float* feat, int B, int T, float* e
         }
         if (rc) return rc;
     }
-    PPV_CUDA_OK(cudaMemcpyAsync(emb, m->emb_out, size_t(B) * m->cfg.embd_dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return PPV_OK;
 }
 
 // taps: "layer1".."layer4", "fuse12", "fuse123", "fuse1234" -> fp32 [B,H,W,C]; "stats" -> [B, 2*512*F']
-int eres2net_read_tap(ERes2NetModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st) {
-    PPV_REQUIRE(m && name && out, "eres2net_read_tap: null argument");
-    if (!m->plan_ws) return fail(PPV_ESTATE, "eres2net_read_tap: no forward has run");
-    const std::string n(name);
+int ERes2NetModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {
+    ERes2NetModel* const m = this;
     const int B = m->plan_B;
     if (n == "stats") {
         PPV_REQUIRE(out_elems >= size_t(B) * 2 * m->stats_ch, "eres2net_read_tap: output too small");

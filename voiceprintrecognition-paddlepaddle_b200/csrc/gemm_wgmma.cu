@@ -348,6 +348,11 @@ int encode_planes_map(CUtensorMap* m, const Planes& t, int box_rows) { return en
 
 int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W, int M, int N, const Epilogue& epi,
                int BN, int BK) {
+    if (BK == 0) {
+        BK = 64;
+        for (int i = 0; i < nsrc; ++i)
+            if (srcs[i].ncols % 64) BK = 32;
+    }
     PPV_REQUIRE(BK == 64 || BK == 32, "gemm_build: BK must be 64 or 32");
     PPV_REQUIRE(BN == 64 || BN == 128 || BN == 256, "gemm_build: BN must be 64/128/256");
     PPV_REQUIRE(epi.out_mode == OUT_F32 || N % 32 == 0, "gemm_build: planes output needs N % 32 == 0");
@@ -391,6 +396,7 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
     gp->N = N;
     gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
     gp->n_tiles = (N + BN - 1) / BN;
+    gp->bn = BN;
     gp->epi = epi;
     {
         // weight-stationary: one n-tile, all k-slices of W (both planes) fit next to a 4-slot ring, and enough tiles per CTA to pay
@@ -449,6 +455,7 @@ int gemm_build_wgrad(GemmParams* gp, const Planes& At, const Planes& Bt, int M, 
     gp->N = N;
     gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
     gp->n_tiles = (N + BN - 1) / BN;
+    gp->bn = BN;
     Epilogue ep;
     ep.out_mode = OUT_F32;
     ep.out = out;
@@ -478,9 +485,9 @@ static int launch_bn(const GemmParams& gp, bool x3, int num_sms, cudaStream_t st
     return x3 ? launch_one<BN, 3, 64>(gp, num_sms, stream) : launch_one<BN, 1, 64>(gp, num_sms, stream);
 }
 
-int gemm_launch(const GemmParams& gp, int BN, int precision, int num_sms, cudaStream_t stream) {
+int gemm_launch(const GemmParams& gp, int precision, int num_sms, cudaStream_t stream) {
     const bool x3 = (precision == PPV_PREC_BF16X3);
-    switch (BN) {
+    switch (gp.bn) {
         case 64: return launch_bn<64>(gp, x3, num_sms, stream);
         case 128: return launch_bn<128>(gp, x3, num_sms, stream);
         case 256: return launch_bn<256>(gp, x3, num_sms, stream);

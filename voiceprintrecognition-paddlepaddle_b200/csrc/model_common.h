@@ -144,4 +144,89 @@ struct WsCarver {
     }
 };
 
+// An inference model behind ppv_model_*: weights are loaded by name, prepared into one device arena by finalize(), and each
+// forward runs a plan of launches that is built for (workspace, B, T) and rebuilt whenever one of them changes.
+struct Model {
+    const char* prefix;  // error-message prefix, e.g. "resnetse"
+    WeightMap raw;
+    bool finalized = false;
+    int precision;
+    int num_sms;
+    void* arena = nullptr;
+    void* plan_ws = nullptr;  // the plan's key (plan_ws, plan_B, plan_T); null and zeros when no plan is built
+    int plan_B = 0, plan_T = 0;
+    float* emb_out = nullptr;  // workspace buffer the plan's last step writes the embeddings [B][embd_dim] to
+
+    Model(const char* prefix, int precision) : prefix(prefix), precision(precision), num_sms(device_sm_count()) {}
+    virtual ~Model() { cudaFree(arena); }
+    virtual int embd_dim() const = 0;
+    virtual size_t workspace_bytes(int B, int T) const = 0;
+
+    int load_weight(const char* name, const float* data, const int64_t* shape, int ndim) {
+        if (finalized) return fail(PPV_ESTATE, std::string(prefix) + "_load_weight: model already finalized");
+        return weight_map_load(&raw, name, data, shape, ndim);
+    }
+    int set_precision(int p) {
+        PPV_REQUIRE(p == PPV_PREC_BF16X3 || p == PPV_PREC_BF16, "bad precision");
+        precision = p;
+        return PPV_OK;
+    }
+    int finalize() {
+        if (finalized) return PPV_OK;
+        ArenaBuilder ab;
+        ab.wm = &raw;
+        if (!prepare_weights(ab))
+            return fail(PPV_EINVAL, std::string(prefix) + "_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
+        int rc = ab.upload(&arena);
+        if (rc) return rc;
+        raw.clear();
+        finalized = true;
+        return PPV_OK;
+    }
+    int forward(const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
+        int rc = forward_begin(emb, B, T);
+        if (!rc) rc = update_plan(B, T, ws, ws_bytes, st);
+        if (!rc) rc = run_steps(feat, st);
+        return rc ? rc : copy_embeddings(emb, st);
+    }
+    int read_tap(const char* name, float* out, size_t out_elems, cudaStream_t st) {
+        PPV_REQUIRE(name && out, std::string(prefix) + "_read_tap: null argument");
+        if (!plan_ws) return fail(PPV_ESTATE, std::string(prefix) + "_read_tap: no forward has run");
+        return tap(name, out, out_elems, st);
+    }
+
+  protected:
+    // The steps of forward(), for models whose forward takes more inputs.
+    int forward_begin(const float* emb, int B, int T) {
+        PPV_REQUIRE(emb, std::string(prefix) + "_forward: null argument");
+        if (!finalized) return fail(PPV_ESTATE, std::string(prefix) + "_forward: call ppv_model_finalize first");
+        PPV_REQUIRE(B > 0 && T > 0, std::string(prefix) + "_forward: empty batch");
+        return PPV_OK;
+    }
+    int update_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+        if (plan_ws == ws && plan_B == B && plan_T == T) return PPV_OK;
+        int rc = build_plan(B, T, ws, ws_bytes, st);
+        if (rc) {  // no plan: B > 0 in every forward, so no key matches this one and the next forward rebuilds
+            plan_ws = nullptr;
+            plan_B = plan_T = 0;
+            return rc;
+        }
+        plan_ws = ws;
+        plan_B = B;
+        plan_T = T;
+        return PPV_OK;
+    }
+    int copy_embeddings(float* emb, cudaStream_t st) {
+        PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(plan_B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        return PPV_OK;
+    }
+    // Puts the prepared weights into the arena image; false, with ab.err set where known, on a missing or misshapen weight.
+    virtual bool prepare_weights(ArenaBuilder& ab) = 0;
+    // Carves `ws` and plans the launches of a forward over B utterances of T frames.
+    virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
+    // Launches the planned steps on features [plan_B, plan_T, input_size].
+    virtual int run_steps(const float* feat, cudaStream_t st) = 0;
+    virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
+};
+
 }  // namespace ppv

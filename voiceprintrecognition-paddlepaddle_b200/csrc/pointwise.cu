@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256, 2) pw_conv_kernel(const PwParams p) {
 
 // A 1x1 conv qualifies when its single source is a 32-column window at row offset 0, N is 32 or 64, the output goes to split planes (plain
 // rows or an image grid, any stride) and the epilogue is bias (+ ReLU / clipped ReLU).
-bool pointwise_supported(const GemmSource* srcs, int nsrc, int N, const Epilogue& ep) {
+static bool pointwise_supported(const GemmSource* srcs, int nsrc, int N, const Epilogue& ep) {
     if (nsrc != 1 || N % 32 != 0 || N > 64) return false;
     if (srcs[0].row_off != 0 || srcs[0].ncols != 32 || srcs[0].col0 % 8 != 0 || srcs[0].t.ld % 8 != 0) return false;
     if (ep.out_mode != OUT_PLANES || ep.rowgrp_bias || ep.seg_scale || ep.bn_scale || ep.tanh_ || ep.sigmoid_ || ep.silu_ || ep.Tp != 0 || ep.halo) return false;
@@ -148,6 +148,18 @@ int pointwise_launch(const GemmSource* srcs, int nsrc, const Planes& W, int64_t 
     const int grid = int(std::min<int64_t>((M + 255) / 256, int64_t(num_sms) * 8));
     PPV_PDL_OK(launch_pdl(pw_conv_kernel<32>, dim3(grid), dim3(256), smem, st, p), "pw_conv_kernel<32>");
     return PPV_OK;
+}
+
+bool pointwise_step_build(PwStep* s, const GemmSource* srcs, int nsrc, const Planes& W, int N, int64_t M, const Epilogue& ep) {
+    const char* e = getenv("PPV_POINTWISE");
+    if ((e && e[0] == '0') || ep.img_Wp == 0 || !pointwise_supported(srcs, nsrc, N, ep)) return false;
+    for (int i = 0; i < nsrc; ++i) s->srcs[i] = srcs[i];
+    s->nsrc = nsrc;
+    s->N = N;
+    s->M = M;
+    s->W = W;
+    s->ep = ep;
+    return true;
 }
 
 }  // namespace ppv

@@ -34,12 +34,10 @@ struct BlockW {
 };
 
 struct RStep {
-    enum Kind { CONV1, GEMM, CONV3, PW, POOL, SCALE_RES, FLATTEN, ASP_GLOBAL, ASP_FUSED } kind;
-    PwStep pw;  // PW: 1x1 conv with K <= 64 on the CUDA cores (pointwise.cu)
+    enum Kind { CONV1, GEMM, CONV3, POOL, SCALE_RES, FLATTEN, ASP_GLOBAL, ASP_FUSED } kind;
     Conv3x3Params c3;  // CONV3: 3x3 conv with 32 -> 32 channels (layer1), conv3x3.cu
     GemmParams gp;
     AspFusedParams ap;
-    int BN = 0;
     // POOL / SCALE_RES operands
     Planes a, b, c;
     const float* scale = nullptr;
@@ -50,13 +48,8 @@ struct RStep {
 
 }  // namespace
 
-struct ResNetSEModel {
+struct ResNetSEModel : Model {
     ppv_resnetse_cfg cfg;
-    WeightMap raw;
-    bool finalized = false;
-    int precision = PPV_PREC_BF16X3;
-    int num_sms = 132;
-    void* arena = nullptr;
     // weights
     float* conv1_w = nullptr;  // [32][9] BN folded
     float* conv1_b = nullptr;  // [32]
@@ -66,14 +59,21 @@ struct ResNetSEModel {
     int att = 128, cat = 0, Hf = 0;
     // plan
     std::vector<RStep> steps;
-    void* plan_ws = nullptr;
-    int plan_B = 0, plan_T = 0;
     Geo geo[5];  // geo[l] = grid of stage l (1..4); geo[1] is also conv1's
     Planes conv1_out, flat, gstat, pooled, attp, se_mean, se_hid;
     std::vector<Planes> blk_out;  // per block
-    float *se_scale = nullptr, *fold_out = nullptr, *pooled_raw = nullptr, *emb_out = nullptr;
+    float *se_scale = nullptr, *fold_out = nullptr, *pooled_raw = nullptr;
     int Tf = 0;
-    const float* feat_in = nullptr;
+
+    explicit ResNetSEModel(const ppv_resnetse_cfg& c) : Model("resnetse", c.precision), cfg(c) {}
+    int embd_dim() const override { return cfg.embd_dim; }
+    size_t workspace_bytes(int B, int T) const override;
+
+  protected:
+    bool prepare_weights(ArenaBuilder& ab) override;
+    int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
+    int run_steps(const float* feat, cudaStream_t st) override;
+    int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
 // ------------------------------------------------------------------------------------------------ small kernels
@@ -197,7 +197,7 @@ void ppv_resnetse_default_cfg_impl(ppv_resnetse_cfg* c) {
     c->precision = PPV_PREC_BF16X3;
 }
 
-int resnetse_create(const ppv_resnetse_cfg* cfg, ResNetSEModel** out) {
+int resnetse_create(const ppv_resnetse_cfg* cfg, Model** out) {
     PPV_REQUIRE(cfg && out, "resnetse_create: null argument");
     int nblocks = 0;
     for (int i = 0; i < 4; ++i) {
@@ -212,40 +212,17 @@ int resnetse_create(const ppv_resnetse_cfg* cfg, ResNetSEModel** out) {
         if ((2 * cfg->num_filters[i]) / cfg->reduction > 64 || (2 * cfg->num_filters[i]) % cfg->reduction)
             return fail(PPV_EUNSUPPORTED, "resnetse: SE hidden width must be <= 64");
     if ((2 * cfg->num_filters[3] * (cfg->input_size / 8)) % 128) return fail(PPV_EUNSUPPORTED, "resnetse: pooled channels must be a multiple of 128");
-    ResNetSEModel* m = new ResNetSEModel();
-    m->cfg = *cfg;
-    m->precision = cfg->precision;
+    ResNetSEModel* m = new ResNetSEModel(*cfg);
     m->att = cfg->attention_channels;
     m->Hf = cfg->input_size / 8;
     m->cat = 2 * cfg->num_filters[3] * m->Hf;
-    m->num_sms = device_sm_count();
     *out = m;
     return PPV_OK;
 }
 
-void resnetse_destroy(ResNetSEModel* m) {
-    if (!m) return;
-    cudaFree(m->arena);
-    delete m;
-}
-int resnetse_embd_dim(const ResNetSEModel* m) { return m->cfg.embd_dim; }
-int resnetse_set_precision(ResNetSEModel* m, int precision) {
-    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "bad precision");
-    m->precision = precision;
-    return PPV_OK;
-}
-int resnetse_load_weight(ResNetSEModel* m, const char* name, const float* data, const int64_t* shape, int ndim) {
-    PPV_REQUIRE(m, "resnetse_load_weight: null model");
-    if (m->finalized) return fail(PPV_ESTATE, "resnetse_load_weight: model already finalized");
-    return weight_map_load(&m->raw, name, data, shape, ndim);
-}
-
 // ------------------------------------------------------------------------------------------------ finalize
-int resnetse_finalize(ResNetSEModel* m) {
-    PPV_REQUIRE(m, "resnetse_finalize: null model");
-    if (m->finalized) return PPV_OK;
-    ArenaBuilder ab;
-    ab.wm = &m->raw;
+bool ResNetSEModel::prepare_weights(ArenaBuilder& ab) {
+    ResNetSEModel* const m = this;
     const ppv_resnetse_cfg& cf = m->cfg;
     bool ok = true;
     // conv (+ directly following BN) -> dense [N][taps*Cin] with BN folded; K order = (tap, cin)
@@ -360,12 +337,7 @@ int resnetse_finalize(ResNetSEModel* m) {
             ab.put_f32(&m->bn2_shift, f4);
         }
     }
-    if (!ok) return fail(PPV_EINVAL, "resnetse_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
-    int rc = ab.upload(&m->arena);
-    if (rc) return rc;
-    m->raw.clear();
-    m->finalized = true;
-    return PPV_OK;
+    return ok;
 }
 
 // ------------------------------------------------------------------------------------------------ workspace / plan
@@ -443,21 +415,20 @@ void rs_carve(const ResNetSEModel* m, WsCarver& cv, int B, int T, Geo* geo, RsBu
     rb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
-inline int rs_pick_bn(int N) { return (N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : 64; }
-
 }  // namespace
 
-size_t resnetse_workspace_bytes(const ResNetSEModel* m, int B, int T) {
-    if (!m || !m->finalized || B <= 0 || T <= 0) return 0;
+size_t ResNetSEModel::workspace_bytes(int B, int T) const {
+    if (!finalized || B <= 0 || T <= 0) return 0;
     WsCarver cv;
-    Geo geo[5];
+    Geo g[5];
     RsBuffers rb;
-    rs_carve(m, cv, B, T, geo, &rb);
+    rs_carve(this, cv, B, T, g, &rb);
     return mc_align_up(cv.off, 256);
 }
 
-static int rs_build_plan(ResNetSEModel* m, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-    const size_t need = resnetse_workspace_bytes(m, B, T);
+int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+    ResNetSEModel* const m = this;
+    const size_t need = workspace_bytes(B, T);
     PPV_REQUIRE(ws && ws_bytes >= need, "resnetse: workspace too small (see ppv_model_workspace_bytes)");
     PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "resnetse: workspace must be 256-byte aligned");
     PPV_REQUIRE(T >= 8, "resnetse: too few frames");
@@ -489,11 +460,7 @@ static int rs_build_plan(ResNetSEModel* m, int B, int T, void* ws, size_t ws_byt
         ep.bias = gw.bias;
         RStep s;
         s.kind = RStep::GEMM;
-        s.BN = rs_pick_bn(n_gemm);
-        int bk = 64;
-        for (const GemmSource& g : srcs)
-            if (g.ncols % 64) bk = 32;
-        int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, n_gemm, ep, s.BN, bk);
+        int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, n_gemm, ep, gemm_pick_bn(n_gemm));
         if (rc) return rc;
         m->steps.push_back(s);
         return PPV_OK;
@@ -651,25 +618,13 @@ static int rs_build_plan(ResNetSEModel* m, int B, int T, void* ws, size_t ws_byt
     m->pooled_raw = rb.pooled_raw;
     m->emb_out = rb.emb_out;
     m->Tf = Tf;
-    m->plan_ws = ws;
-    m->plan_B = B;
-    m->plan_T = T;
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int resnetse_forward(ResNetSEModel* m, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(m && feat && emb, "resnetse_forward: null argument");
-    if (!m->finalized) return fail(PPV_ESTATE, "resnetse_forward: call ppv_model_finalize first");
-    PPV_REQUIRE(B > 0 && T > 0, "resnetse_forward: empty batch");
-    if (m->plan_ws != ws || m->plan_B != B || m->plan_T != T) {
-        int rc = rs_build_plan(m, B, T, ws, ws_bytes, st);
-        if (rc) {
-            m->plan_ws = nullptr;
-            return rc;
-        }
-    }
-    const int F = m->cfg.input_size, cat = m->cat;
+int ResNetSEModel::run_steps(const float* feat, cudaStream_t st) {
+    ResNetSEModel* const m = this;
+    const int B = m->plan_B, T = m->plan_T, F = m->cfg.input_size, cat = m->cat;
     int rc = PPV_OK;
     for (const RStep& s : m->steps) {
         switch (s.kind) {
@@ -680,9 +635,8 @@ int resnetse_forward(ResNetSEModel* m, const float* feat, int B, int T, float* e
                            "rs_conv1_kernel");
                 break;
             }
-            case RStep::GEMM: rc = gemm_launch(s.gp, s.BN, m->precision, m->num_sms, st); break;
+            case RStep::GEMM: rc = gemm_launch(s.gp, m->precision, m->num_sms, st); break;
             case RStep::CONV3: rc = conv3x3_launch(s.c3, m->precision, m->num_sms, st); break;
-            case RStep::PW: rc = pointwise_launch(s.pw, m->num_sms, st); break;
             case RStep::POOL:
                 rc = launch_colstats(s.a, 0, s.C, B, s.img_rows, 0, s.img_rows, 0, 0.f, nullptr, s.b, st, s.inv_count);
                 break;
@@ -702,15 +656,12 @@ int resnetse_forward(ResNetSEModel* m, const float* feat, int B, int T, float* e
         }
         if (rc) return rc;
     }
-    PPV_CUDA_OK(cudaMemcpyAsync(emb, m->emb_out, size_t(B) * m->cfg.embd_dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return PPV_OK;
 }
 
 // taps: "conv1", "layer1".."layer4" -> fp32 [B,H,W,C]; "flat" -> [B,T',cat]; "asp" -> [B, 2*cat]
-int resnetse_read_tap(ResNetSEModel* m, const char* name, float* out, size_t out_elems, cudaStream_t st) {
-    PPV_REQUIRE(m && name && out, "resnetse_read_tap: null argument");
-    if (!m->plan_ws) return fail(PPV_ESTATE, "resnetse_read_tap: no forward has run");
-    const std::string n(name);
+int ResNetSEModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {
+    ResNetSEModel* const m = this;
     const int B = m->plan_B;
     if (n == "asp") {
         PPV_REQUIRE(out_elems >= size_t(B) * 2 * m->cat, "resnetse_read_tap: output too small");
