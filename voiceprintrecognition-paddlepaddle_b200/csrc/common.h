@@ -214,11 +214,12 @@ bool conv3x3_c32_supported(int Cin, int Cout, int H, int W);
 int conv3x3_build(Conv3x3Params* cp, const Planes& x, int x_col0, const Planes& Wt, int B, int H, int W, int Hp, int Wp, const Epilogue& epi);
 int conv3x3_launch(const Conv3x3Params& cp, int precision, int num_sms, cudaStream_t st);
 
-// ---- the whole Res2Net chain of a block, one utterance per CTA, operands resident in shared memory (res2chain.cu) ----------
+// ---- the whole Res2Net chain of a block, operands resident in shared memory (res2chain.cu): two utterances per CTA up to
+// Tp = 320 ("paired"), else one utterance per CTA up to Tp = 384 ----------
 constexpr int RES2CHAIN_MAX = 7;
 struct Res2ChainParams {
-    CUtensorMap mapX;                  // tdnn1 output planes, box {64, 200, 1} (the resident tile of conv 1)
-    CUtensorMap mapXt, mapY, mapYtail; // 128-row staging tiles: next-chunk load, y store, y store of the utterance's last tile
+    CUtensorMap mapX;                  // tdnn1 output planes, box {64, 200 (one utterance per CTA) or 168 (paired), 1}: the resident tile of conv 1
+    CUtensorMap mapXt, mapY, mapYtail; // one utterance per CTA only, 128-row staging tiles: next-chunk load, y store, y store of the utterance's last tile
     CUtensorMap mapW[RES2CHAIN_MAX];   // per-conv weight planes [2][>=64][>=192], box {64, 64, 1}
     const float* bias[RES2CHAIN_MAX];
     const float* bn_scale[RES2CHAIN_MAX];
@@ -226,12 +227,14 @@ struct Res2ChainParams {
     Planes x;  // tdnn1 output [rows][>= 8*64]: chunk j at columns 64 j
     Planes y;  // Res2Net output [rows][>= 8*64]: conv j (1-based) -> columns 64 j
     int nconv, width, B, T, P, Tp, dil, ntiles;
-    unsigned long long* trace;  // debug (PPV_RES2_TRACE): clock64 stamps of CTA 0's first utterance, [role][conv][event]
+    int paired;                 // 1: res2chain_pair_kernel, 0: res2chain_kernel
+    unsigned long long* trace;  // debug (PPV_RES2_TRACE): clock64 stamps of CTA 0's first utterance (pair), [role][conv][event]
 };
 int res2chain_build(Res2ChainParams* cp, const Planes& x, const Planes& y, const Planes* W, const float* const* bias, const float* const* bn_scale,
-                    const float* const* bn_shift, int nconv, int B, int T, int P, int Tp, int dil);
+                    const float* const* bn_shift, int nconv, int B, int T, int P, int Tp, int dil, bool paired);
 int res2chain_launch(const Res2ChainParams& cp, int precision, int num_sms, cudaStream_t st);
-bool res2chain_fits(int T, int P);
+bool res2chain_fits(int T, int P);       // one utterance per CTA: Tp <= 384
+bool res2chain_pair_fits(int T, int P);  // two utterances per CTA: Tp <= 320
 void res2chain_trace_dump(const Res2ChainParams& cp);
 
 // ---- 1x1 convs with K <= 64 on the CUDA cores, one thread per grid position (pointwise.cu) ----------------------------

@@ -13,6 +13,7 @@
 //     is one tiny GEMM, so the attention TDNN runs with K = 1536 (2.857 GFLOP / utterance executed
 //     instead of 3.090).
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.h"
 #include "model_common.h"
@@ -339,8 +340,11 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     const int64_t R = int64_t(B) * Tp;
     const char* r2env = getenv("PPV_RES2_GEMM");  // debugging aid: 1 = run the Res2Net convs through the generic gather-GEMM
     const bool use_res2_kernel = (w == 64) && !(r2env && r2env[0] == '1');
-    const char* rcenv = getenv("PPV_RES2_CHAIN");  // 0 = one launch per Res2Net conv (res2conv.cu) instead of the fused chain
+    // 0 = one launch per Res2Net conv (res2conv.cu) instead of the fused chain; single = the fused chain with one utterance per CTA
+    // even where two fit (tests and A/B timing)
+    const char* rcenv = getenv("PPV_RES2_CHAIN");
     const bool use_res2_chain = use_res2_kernel && m->scale == 8 && res2chain_fits(T, P) && !(rcenv && rcenv[0] == '0');
+    const bool res2_paired = use_res2_chain && res2chain_pair_fits(T, P) && !(rcenv && strcmp(rcenv, "single") == 0);
     const char* skenv = getenv("PPV_SKINNY");  // 0 = the per-utterance linear layers through the tensor-core gather-GEMM (A-B timing)
     const bool use_skinny = !(skenv && skenv[0] == '0');
     const char* bkenv = getenv("PPV_GEMM_BK32");  // experiment: 1 = 32-wide k-steps (SWIZZLE_64B) on the wide-N layers
@@ -414,7 +418,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         // the fused Res2Net chain builds the reflect halo rows itself, so tdnn1 writes no halo rows (and gets the lean epilogue)
         rc = add_gemm(m->tdnn1[b - 1], {{-1, 0, C, 0, 0, C, 0}}, &X, xcol, int(R), planes_out(m->buf.bufs[B_H], 0, !use_res2_chain));
         if (rc) return rc;
-        if (use_res2_chain) {  // all seven convs in one kernel, one utterance per CTA, operands resident in shared memory (res2chain.cu)
+        if (use_res2_chain) {  // all seven convs in one kernel, one or two utterances per CTA, operands resident in shared memory (res2chain.cu)
             Planes Wj[RES2CHAIN_MAX];
             const float *bj[RES2CHAIN_MAX], *sj[RES2CHAIN_MAX], *hj[RES2CHAIN_MAX];
             for (int j = 1; j < m->scale; ++j) {
@@ -426,7 +430,8 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             }
             Step stp;
             stp.kind = Step::RES2CHAIN;
-            rc = res2chain_build(&stp.cp, m->buf.bufs[B_H], m->buf.bufs[B_Y], Wj, bj, sj, hj, m->scale - 1, B, T, P, Tp, m->cfg.dilations[b]);
+            rc = res2chain_build(&stp.cp, m->buf.bufs[B_H], m->buf.bufs[B_Y], Wj, bj, sj, hj, m->scale - 1, B, T, P, Tp, m->cfg.dilations[b],
+                                 res2_paired);
             if (rc) return rc;
             m->steps.push_back(stp);
         }

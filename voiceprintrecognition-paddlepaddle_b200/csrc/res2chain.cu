@@ -41,6 +41,21 @@ struct RCCfg {
     static constexpr int SMEM_BYTES = 1024 + A_BYTES + W_SLOT + 2 * S_BYTES + 256;
 };
 
+// Predicated stores, in program order (volatile asm is not reordered): with branches around plain stores the scheduler computes
+// many columns ahead of their stores and runs out of registers.
+__device__ __forceinline__ void rp_st_global(bool pred, uint32_t* p, uint32_t v) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.u32 [%0], %1;\n\t}" ::"l"(p), "r"(v), "r"(uint32_t(pred)) : "memory");
+}
+__device__ __forceinline__ void rp_st_shared(bool pred, uint32_t a, uint32_t v) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.shared.u32 [%0], %1;\n\t}" ::"r"(a), "r"(v), "r"(uint32_t(pred)) : "memory");
+}
+
+__device__ __forceinline__ uint32_t rc_ld_shared(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+
 #define RC_STAMP(role, conv, ev)                                                                   \
     do {                                                                                          \
         if (cp.trace && blockIdx.x == 0 && b == 0) cp.trace[((role) * 8 + (conv)) * 8 + (ev)] = clock64(); \
@@ -151,7 +166,6 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
         const bool has_tile = tw < ntiles;
         griddep_wait();
         uint8_t* const a_gen = smem_gen;  // a_base == smem_base
-        uint8_t* const s_gen = smem_gen + (s_base - smem_base);
         float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
@@ -216,49 +230,52 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
                 const bool has_next = j + 1 < nconv;
                 const uint32_t sn = g * uint32_t(ntiles) + uint32_t(tw);
                 const int i = sn & 1;
-                uint8_t* const sbuf = s_gen + i * Cfg::S_BYTES;
+                // One row per trip of a loop that is not unrolled (acc indexed by selects), the mirror rows as scalars and the
+                // shared-memory stores predicated in program order: unrolled, the compiler computes values far ahead of their
+                // stores and spills.
                 auto epilogue = [&](const float (&acc)[BN / 2], int mb) {
-#pragma unroll
+#pragma unroll 1
                     for (int h = 0; h < 2; ++h) {
                         const int rloc = mb * 64 + 16 * w + (l >> 2) + 8 * h;  // row inside the 128-row tile
                         const int p = tw * GEMM_BM + rloc;                      // padded row inside the utterance
-                        const int tt = p - cp.P;
-                        const bool valid = tt >= 0 && tt < cp.T;
-                        int rows[3] = {p + RC_PAD, -1, -1};
-                        if (tt >= 1 && tt <= cp.P) rows[1] = cp.P - tt + RC_PAD;
-                        const int uu = cp.T - 1 - tt;
-                        if (uu >= 1 && uu <= cp.P) rows[2] = cp.P + cp.T - 1 + uu + RC_PAD;
+                        const int tt = p - cp.P, uu = cp.T - 1 - tt;
+                        const bool next = has_next && tt >= 0 && tt < cp.T;
+                        const int m0 = p + RC_PAD;
+                        const int m1 = (tt >= 1 && tt <= cp.P) ? cp.P - tt + RC_PAD : -1;
+                        const int m2 = (uu >= 1 && uu <= cp.P) ? cp.P + cp.T - 1 + uu + RC_PAD : -1;
+                        const uint32_t srow = s_base + i * Cfg::S_BYTES + rloc * 128 + 4 * (l & 3);
 #pragma unroll
                         for (int q = 0; q < BN / 8; ++q) {
                             const int col = 8 * q + 2 * (l & 3);
-                            const int off = ((q ^ (rloc & 7)) << 4) + 4 * (l & 3);  // SWIZZLE_128B: 16-byte chunk q of the row
+                            const uint32_t so = srow + ((q ^ (rloc & 7)) << 4);  // SWIZZLE_128B: 16-byte chunk q of the row
                             // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
                             const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
                             const float2 s2 = __ldg(reinterpret_cast<const float2*>(bsc + col));
                             const float2 h2 = __ldg(reinterpret_cast<const float2*>(bsh + col));
-                            const float x0 = fmaf(fmaxf(acc[4 * q + 2 * h] + b2.x, 0.f), s2.x, h2.x);
-                            const float x1 = fmaf(fmaxf(acc[4 * q + 2 * h + 1] + b2.y, 0.f), s2.y, h2.y);
+                            const float a0 = h ? acc[4 * q + 2] : acc[4 * q], a1 = h ? acc[4 * q + 3] : acc[4 * q + 1];
+                            const float x0 = fmaf(fmaxf(a0 + b2.x, 0.f), s2.x, h2.x);
+                            const float x1 = fmaf(fmaxf(a1 + b2.y, 0.f), s2.y, h2.y);
                             uint32_t nh = 0, nl = 0;
                             if (has_next) {
-                                nh = *reinterpret_cast<const uint32_t*>(sbuf + rloc * 128 + off);
-                                if (NP == 2) nl = *reinterpret_cast<const uint32_t*>(sbuf + RC_S_PLANE + rloc * 128 + off);
+                                nh = rc_ld_shared(so);
+                                if (NP == 2) nl = rc_ld_shared(so + RC_S_PLANE);
                             }
                             uint32_t yh, yl;  // y_{j+1} -> staging tile (every row: rows outside the valid frames are halo / padding rows of y)
                             split_pack_bf16x2(x0, x1, yh, yl);
-                            *reinterpret_cast<uint32_t*>(sbuf + rloc * 128 + off) = yh;
-                            if (NP == 2) *reinterpret_cast<uint32_t*>(sbuf + RC_S_PLANE + rloc * 128 + off) = yl;
-                            if (has_next && valid) {  // x_{j+2} + y_{j+1} -> operand of the next conv, in place, with its reflect halo rows
-                                const float2 hf = unpack_bf16x2(nh), lf = unpack_bf16x2(nl);
-                                uint32_t oh, ol;
-                                split_pack_bf16x2(x0 + (hf.x + lf.x), x1 + (hf.y + lf.y), oh, ol);
-#pragma unroll
-                                for (int r = 0; r < 3; ++r) {
-                                    if (rows[r] < 0) continue;
-                                    uint8_t* dst = a_gen + rows[r] * 128 + ((q ^ (rows[r] & 7)) << 4) + 4 * (l & 3);
-                                    *reinterpret_cast<uint32_t*>(dst) = oh;
-                                    if (NP == 2) *reinterpret_cast<uint32_t*>(dst + RC_A_PLANE) = ol;
-                                }
-                            }
+                            rp_st_shared(true, so, yh);
+                            if (NP == 2) rp_st_shared(true, so + RC_S_PLANE, yl);
+                            // x_{j+2} + y_{j+1} -> operand of the next conv, in place, with its reflect halo rows
+                            const float2 hf = unpack_bf16x2(nh), lf = unpack_bf16x2(nl);
+                            uint32_t oh, ol;
+                            split_pack_bf16x2(x0 + (hf.x + lf.x), x1 + (hf.y + lf.y), oh, ol);
+                            auto put = [&](bool pred, int row) {
+                                const uint32_t d = a_base + row * 128 + ((q ^ (row & 7)) << 4) + 4 * (l & 3);
+                                rp_st_shared(pred, d, oh);
+                                if (NP == 2) rp_st_shared(pred, d + RC_A_PLANE, ol);
+                            };
+                            put(next, m0);
+                            put(next && m1 >= 0, m1);
+                            put(next && m2 >= 0, m2);
                         }
                     }
                 };
@@ -284,22 +301,267 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Paired variant (Tp <= 320): one CTA holds TWO utterances, A and B, resident in shared memory and alternates them through the
+// convs, so that the MMAs of one utterance run on the tensor cores while the warps run the epilogue of the other:
+//   MMA_A(j) | epilogue_B(j-1)  ->  MMA_B(j) | epilogue_A(j)  ->  W[j+1] lands  ->  MMA_A(j+1) | epilogue_B(j)  -> ...
+// B = 256 utterances are 128 CTAs, one wave.  Five MMA warpgroups (640 threads, 96 registers each): warpgroup w owns the
+// m64 row block w of BOTH utterances, one 64 x 64 accumulator per utterance.  The operands (2 x 336 rows x planes) and one
+// conv's weights (shared by both utterances) leave no room for staging tiles, so the epilogue reads x_{j+2} and writes y_{j+1}
+// with plain global accesses; x_{j+2} is prefetched into L2 when conv j-1 starts.  Per row, the MMA order, the epilogue formulas
+// and the reflect halo rows are those of the one-utterance kernel above, so the outputs are bitwise equal to its outputs.
+constexpr int RP_BLOCKS = 5;                          // m64 row blocks per utterance, one per MMA warpgroup
+constexpr int RP_MAX_TP = RP_BLOCKS * 64;             // 320
+constexpr int RP_BOX_ROWS = 168;                      // two boxes: 336 >= 4 + 320 + 4 rows; 168 * 128 B is a multiple of 1024
+constexpr int RP_A_PLANE = 2 * RP_BOX_ROWS * 128;     // 43008 B per plane
+constexpr int RP_THREADS = 128 * RP_BLOCKS;           // 640
+constexpr int RP_VEC_FLOATS = 3 * RES2CHAIN_MAX * 64;  // bias, BN scale, BN shift of every conv
+
+template <int NSPLIT>
+struct RPCfg {
+    static constexpr int NP = (NSPLIT == 3) ? 2 : 1;
+    static constexpr int U_BYTES = NP * RP_A_PLANE;     // one utterance's operand tile
+    static constexpr int W_SLOT = 3 * NP * RC_W_TILE;   // 3 taps x planes of one conv
+    static constexpr int SMEM_BYTES = 1024 + 2 * U_BYTES + W_SLOT + RP_VEC_FLOATS * 4 + 64;
+};
+static_assert(RPCfg<3>::SMEM_BYTES <= 232448, "paired res2chain exceeds the H100 shared-memory opt-in");
+
+// trace (PPV_RES2_TRACE) of CTA 0's first pair: role 0 / 1 = utterance A / B, events 0 MMA issued, 1 MMA retired (every
+// warpgroup), 2 epilogue start, 3 epilogue end (warpgroup 0); role 2 = weights, events 0 load issued, 1 landed
+#define RP_STAMP(role, conv, ev)                                                                                \
+    do {                                                                                                        \
+        if (trace_on) cp.trace[((role) * 8 + (conv)) * 8 + (ev)] = clock64();                                   \
+    } while (0)
+
+// An opaque copy: what is computed from it stays inside the loop that computes it.  Without it the compiler hoists the operand
+// descriptors and the row addresses of both utterances out of the conv loop and spills them.
+__device__ __forceinline__ int rp_opaque(int v) {
+    asm volatile("mov.b32 %0, %0;" : "+r"(v));
+    return v;
+}
+
+template <int NSPLIT>
+__global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __grid_constant__ Res2ChainParams cp) {
+    using Cfg = RPCfg<NSPLIT>;
+    constexpr int NP = Cfg::NP, BN = 64;
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* const a_gen = smem_raw + (smem_base - smem_u32(smem_raw));  // utterance u's tile at u * U_BYTES, plane pl at + pl * RP_A_PLANE
+    const uint32_t w_base = smem_base + 2 * Cfg::U_BYTES;
+    float* const vec = reinterpret_cast<float*>(a_gen + 2 * Cfg::U_BYTES + Cfg::W_SLOT);  // [conv][bias, scale, shift][64]
+    const uint32_t bar_base = w_base + Cfg::W_SLOT + RP_VEC_FLOATS * 4;
+    const uint32_t x_full = bar_base, w_full = bar_base + 8;
+
+    const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, l = tid & 31;
+    const int nconv = cp.nconv, T = cp.T, P = cp.P, Tp = cp.Tp;
+    if (tid == 0) {
+        prefetch_tmap(&cp.mapX);
+        for (int j = 0; j < nconv; ++j) prefetch_tmap(&cp.mapW[j]);
+        mbar_init(x_full, 1);
+        mbar_init(w_full, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    griddep_launch_dependents();
+    griddep_wait();  // x comes from the previous kernel
+    for (int i = tid; i < 3 * 64 * nconv; i += RP_THREADS) {
+        const int j = i / 192, k = (i / 64) % 3, c = i % 64;
+        vec[i] = (k == 0 ? cp.bias[j] : k == 1 ? cp.bn_scale[j] : cp.bn_shift[j])[c];
+    }
+
+    auto load_w = [&](int j) {
+        mbar_arrive_expect_tx(w_full, 3 * NP * RC_W_TILE);
+        for (int tap = 0; tap < 3; ++tap)
+            for (int pl = 0; pl < NP; ++pl) tma_load_3d(w_base + (tap * NP + pl) * RC_W_TILE, &cp.mapW[j], w_full, tap * 64, 0, pl);
+    };
+    // x_{c} (c = chunk) of both utterances of the pair -> L2, for the epilogue's global loads
+    auto prefetch_chunk = [&](int b0, int c) {
+        for (int u = 0; u < 2 && b0 + u < cp.B; ++u)
+            for (int pl = 0; pl < NP; ++pl)
+                for (int h = 0; h < 2; ++h) tma_prefetch_l2_3d(&cp.mapX, c * cp.width, (b0 + u) * Tp - RC_PAD + h * RP_BOX_ROWS, pl);
+    };
+    // D(64 x 64) of row block wg of utterance u, conv taps in the one-utterance kernel's order
+    auto issue = [&](float (&acc)[BN / 2], int u) {
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 3; ++tap) {
+            const uint32_t a_row = smem_base + rp_opaque(u * Cfg::U_BYTES) + uint32_t(wg * 64 + RC_PAD + (tap - 1) * cp.dil) * 128u;
+            const uint64_t a_hi = make_sw128_kmajor_desc(a_row);
+            const uint64_t b_hi = make_sw128_kmajor_desc(w_base + (tap * NP) * RC_W_TILE);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (tap > 0 || k > 0) ? 1u : 0u);
+            if (NSPLIT == 3) {
+                const uint64_t a_lo = make_sw128_kmajor_desc(a_row + RP_A_PLANE);
+                const uint64_t b_lo = make_sw128_kmajor_desc(w_base + (tap * NP + 1) * RC_W_TILE);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
+            }
+        }
+        wgmma_commit();
+    };
+    // conv j of utterance b (slot u): y_{j+1} -> HBM on rows [0, Tp); x_{j+2} + y_{j+1} -> the operand tile on the valid rows and
+    // their reflect mirrors.  An absent utterance (odd B) stores nothing and loads nothing.
+    auto epilogue = [&](const float (&acc)[BN / 2], int u, int b, int j) {
+        b = rp_opaque(b);
+        const bool present = b < cp.B, has_next = j + 1 < nconv;
+        const float* const vb = vec + j * 192 + 2 * (l & 3);
+        const uint32_t tile = smem_base + u * Cfg::U_BYTES;
+        // an eighth of the fragment (one row, two column pairs) per trip of a loop that is not unrolled: unrolled, the compiler
+        // computes values far ahead of their stores and spills them.  acc is read through selects, never with a runtime index.
+#pragma unroll 1
+        for (int part = 0; part < 8; ++part) {
+            const int h = part >> 2, qh = 2 * (part & 3);
+            const int r = wg * 64 + 16 * wq + (l >> 2) + 8 * h;  // padded row inside the utterance
+            const int tt = r - P, uu = T - 1 - tt;
+            const bool store = present && r < Tp;
+            const bool next = has_next && store && tt >= 0 && tt < T;
+            const int m0 = r + RC_PAD;
+            const int m1 = (tt >= 1 && tt <= P) ? P - tt + RC_PAD : -1;
+            const int m2 = (uu >= 1 && uu <= P) ? P + T - 1 + uu + RC_PAD : -1;
+            const int64_t grow = int64_t(b) * Tp + r;
+            const uint32_t* const xh = reinterpret_cast<const uint32_t*>(cp.x.hi() + grow * cp.x.ld + (j + 2) * cp.width + 2 * (l & 3)) + 4 * qh;
+            uint32_t* const yh = reinterpret_cast<uint32_t*>(cp.y.hi() + grow * cp.y.ld + (j + 1) * cp.width + 2 * (l & 3)) + 4 * qh;
+            // the lo planes, in 32-bit words (encode_planes_map_ex: plane strides are multiples of 8 elements)
+            const int64_t xlo = cp.x.plane_stride / 2, ylo = cp.y.plane_stride / 2;
+            uint32_t nh[2], nl[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                nh[i] = next ? __ldg(xh + 4 * i) : 0u;
+                nl[i] = (next && NP == 2) ? __ldg(xh + 4 * i + xlo) : 0u;
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int q = qh + i;
+                // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
+                const float2 b2 = *reinterpret_cast<const float2*>(vb + 8 * q);
+                const float2 s2 = *reinterpret_cast<const float2*>(vb + 64 + 8 * q);
+                const float2 h2 = *reinterpret_cast<const float2*>(vb + 128 + 8 * q);
+                float a0 = acc[4 * i], a1 = acc[4 * i + 1];
+#pragma unroll
+                for (int k = 0; k < 8; ++k)
+                    if (part == k) a0 = acc[4 * (2 * (k & 3) + i) + 2 * (k >> 2)], a1 = acc[4 * (2 * (k & 3) + i) + 2 * (k >> 2) + 1];
+                const float x0 = fmaf(fmaxf(a0 + b2.x, 0.f), s2.x, h2.x);
+                const float x1 = fmaf(fmaxf(a1 + b2.y, 0.f), s2.y, h2.y);
+                uint32_t vh, vl;
+                split_pack_bf16x2(x0, x1, vh, vl);
+                rp_st_global(store, yh + 4 * i, vh);
+                if (NP == 2) rp_st_global(store, yh + 4 * i + ylo, vl);
+                const float2 hf = unpack_bf16x2(nh[i]), lf = unpack_bf16x2(nl[i]);
+                uint32_t oh, ol;
+                split_pack_bf16x2(x0 + (hf.x + lf.x), x1 + (hf.y + lf.y), oh, ol);
+                auto put = [&](bool pred, int row) {
+                    const uint32_t d = tile + row * 128 + ((q ^ (row & 7)) << 4) + 4 * (l & 3);
+                    rp_st_shared(pred, d, oh);
+                    if (NP == 2) rp_st_shared(pred, d + RP_A_PLANE, ol);
+                };
+                put(next, m0);
+                put(next && m1 >= 0, m1);
+                put(next && m2 >= 0, m2);
+            }
+        }
+    };
+
+    float accA[BN / 2], accB[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) accA[i] = accB[i] = 0.f;
+    const int npairs = (cp.B + 1) / 2;
+    uint32_t g = 0, it = 0;
+    for (int pi = blockIdx.x; pi < npairs; pi += gridDim.x, ++it) {
+        const int b0 = 2 * pi;  // utterances b0 (A) and b0 + 1 (B, absent when B is odd and this is the last pair)
+        const bool trace_on = cp.trace && blockIdx.x == 0 && it == 0 && tid == 0;
+        if (tid == 0) {
+            // rows [-4, 332) around each utterance; an absent B loads out-of-range rows, which TMA fills with zeros
+            mbar_arrive_expect_tx(x_full, 2 * NP * RP_A_PLANE);
+            for (int u = 0; u < 2; ++u)
+                for (int pl = 0; pl < NP; ++pl)
+                    for (int h = 0; h < 2; ++h)
+                        tma_load_3d(smem_base + u * Cfg::U_BYTES + pl * RP_A_PLANE + h * RP_BOX_ROWS * 128, &cp.mapX, x_full,
+                                    cp.width /* chunk 1 */, (b0 + u) * Tp - RC_PAD + h * RP_BOX_ROWS, pl);
+            RP_STAMP(2, 0, 0);
+            load_w(0);
+            for (int c = 2; c <= 3 && c <= nconv; ++c) prefetch_chunk(b0, c);
+        }
+        {
+            // The producing GEMM stores valid frames only: build the reflect halo rows of both resident tiles here --
+            // 2 utterances x 2 P rows x 8 chunks x planes, one 16-byte copy per thread, in the swizzled layout.
+            mbar_wait(x_full, it & 1u);
+            const int per_u = 2 * P * 8 * NP;
+            if (tid < 2 * per_u) {
+                const int u = tid / per_u, e = tid % per_u;
+                const int pl = e / (2 * P * 8), r = (e / 8) % (2 * P), c = e % 8;
+                const int k = (r % P) + 1;
+                const int dst = (r < P ? P - k : P + T - 1 + k) + RC_PAD, src = (r < P ? P + k : P + T - 1 - k) + RC_PAD;
+                uint8_t* const base = a_gen + u * Cfg::U_BYTES + pl * RP_A_PLANE;
+                *reinterpret_cast<uint4*>(base + dst * 128 + ((c ^ (dst & 7)) << 4)) =
+                    *reinterpret_cast<const uint4*>(base + src * 128 + ((c ^ (src & 7)) << 4));
+            }
+            fence_proxy_async_smem();
+            __syncthreads();
+        }
+        for (int j = 0; j < nconv; ++j, ++g) {
+            mbar_wait(w_full, g & 1u);
+            RP_STAMP(2, j, 1);
+            if (tid == 0 && j + 3 <= nconv) prefetch_chunk(b0, j + 3);  // one conv ahead of the epilogue that reads it
+            issue(accA, 0);  // MMA_A(j)
+            // MMA_A(j) is the only group in flight, so this returns at once.  It tells ptxas so: without it ptxas waits for MMA_A(j)
+            // inside epilogue_B(j-1) below, and that epilogue no longer runs under the MMAs.
+            wgmma_wait<1>();
+            RP_STAMP(0, j, 0);
+            if (j > 0) {
+                RP_STAMP(1, j - 1, 2);
+                epilogue(accB, 1, b0 + 1, j - 1);  // under MMA_A(j)
+                RP_STAMP(1, j - 1, 3);
+                fence_proxy_async_smem();
+            }
+            __syncthreads();  // B's operand of conv j is complete
+            issue(accB, 1);   // MMA_B(j)
+            RP_STAMP(1, j, 0);
+            wgmma_wait<1>();
+            wgmma_fence_acc(accA);
+            __syncthreads();  // every warpgroup's MMA_A(j) has retired: A's tile may be overwritten
+            RP_STAMP(0, j, 1);
+            RP_STAMP(0, j, 2);
+            epilogue(accA, 0, b0, j);  // under MMA_B(j)
+            RP_STAMP(0, j, 3);
+            fence_proxy_async_smem();
+            wgmma_wait<0>();
+            wgmma_fence_acc(accB);
+            __syncthreads();  // A's operand of conv j+1 is complete, and every MMA_B(j) has retired: the weight slot is free
+            RP_STAMP(1, j, 1);
+            if (tid == 0 && j + 1 < nconv) {
+                RP_STAMP(2, j + 1, 0);
+                load_w(j + 1);
+            }
+        }
+        RP_STAMP(1, nconv - 1, 2);
+        epilogue(accB, 1, b0 + 1, nconv - 1);
+        RP_STAMP(1, nconv - 1, 3);
+        __syncthreads();  // the next pair's loads overwrite the tiles and the weight slot
+    }
+}
+
 int res2chain_build(Res2ChainParams* cp, const Planes& x, const Planes& y, const Planes* W, const float* const* bias, const float* const* bn_scale,
-                    const float* const* bn_shift, int nconv, int B, int T, int P, int Tp, int dil) {
+                    const float* const* bn_shift, int nconv, int B, int T, int P, int Tp, int dil, bool paired) {
     PPV_REQUIRE(nconv >= 1 && nconv <= RES2CHAIN_MAX, "res2chain: 1..7 convs");
     PPV_REQUIRE(P == RC_PAD && Tp == T + 2 * P && Tp <= RC_MAX_TP, "res2chain: padded utterance must fit 384 rows with P == 4");
+    PPV_REQUIRE(!paired || Tp <= RP_MAX_TP, "res2chain: the paired kernel needs a padded utterance of at most 320 rows");
     PPV_REQUIRE(dil >= 1 && dil <= RC_PAD, "res2chain: dilation must be in [1,4]");
     PPV_REQUIRE(x.ld >= (nconv + 1) * 64 && y.ld >= (nconv + 1) * 64, "res2chain: buffers narrower than the chunks");
     memset(static_cast<void*>(cp), 0, sizeof(*cp));
-    int rc = encode_planes_map_ex(&cp->mapX, x, 64, RC_BOX_ROWS, 128);
+    int rc = encode_planes_map_ex(&cp->mapX, x, 64, paired ? RP_BOX_ROWS : RC_BOX_ROWS, 128);
     if (rc) return rc;
     const int ntiles = (Tp + GEMM_BM - 1) / GEMM_BM;
-    rc = encode_planes_map_ex(&cp->mapXt, x, 64, GEMM_BM, 128);
-    if (rc) return rc;
-    rc = encode_planes_map_ex(&cp->mapY, y, 64, GEMM_BM, 128);
-    if (rc) return rc;
-    rc = encode_planes_map_ex(&cp->mapYtail, y, 64, Tp - (ntiles - 1) * GEMM_BM, 128);
-    if (rc) return rc;
+    if (!paired) {  // the paired kernel stages nothing: its epilogue reads x and writes y directly
+        rc = encode_planes_map_ex(&cp->mapXt, x, 64, GEMM_BM, 128);
+        if (rc) return rc;
+        rc = encode_planes_map_ex(&cp->mapY, y, 64, GEMM_BM, 128);
+        if (rc) return rc;
+        rc = encode_planes_map_ex(&cp->mapYtail, y, 64, Tp - (ntiles - 1) * GEMM_BM, 128);
+        if (rc) return rc;
+    }
     for (int j = 0; j < nconv; ++j) {
         PPV_REQUIRE(W[j].ld >= 192 && W[j].rows >= 64, "res2chain: weight layout mismatch");
         rc = encode_planes_map(&cp->mapW[j], W[j], 64);
@@ -318,6 +580,7 @@ int res2chain_build(Res2ChainParams* cp, const Planes& x, const Planes& y, const
     cp->Tp = Tp;
     cp->dil = dil;
     cp->ntiles = ntiles;
+    cp->paired = paired ? 1 : 0;
     if (getenv("PPV_RES2_TRACE")) {  // debug: leaked on purpose, read back by res2chain_trace_dump
         static unsigned long long* buf = nullptr;
         if (!buf) {
@@ -338,7 +601,17 @@ static int launch_rc(const Res2ChainParams& cp, int num_sms, cudaStream_t st) {
     return PPV_OK;
 }
 
+template <int NSPLIT>
+static int launch_rp(const Res2ChainParams& cp, int num_sms, cudaStream_t st) {
+    using Cfg = RPCfg<NSPLIT>;
+    PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(res2chain_pair_kernel<NSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES)));
+    const int grid = std::min((cp.B + 1) / 2, num_sms);
+    PPV_PDL_OK(launch_pdl(res2chain_pair_kernel<NSPLIT>, dim3(grid), dim3(RP_THREADS), Cfg::SMEM_BYTES, st, cp), "res2chain_pair_kernel");
+    return PPV_OK;
+}
+
 int res2chain_launch(const Res2ChainParams& cp, int precision, int num_sms, cudaStream_t st) {
+    if (cp.paired) return precision == PPV_PREC_BF16X3 ? launch_rp<3>(cp, num_sms, st) : launch_rp<1>(cp, num_sms, st);
     return precision == PPV_PREC_BF16X3 ? launch_rc<3>(cp, num_sms, st) : launch_rc<1>(cp, num_sms, st);
 }
 void res2chain_trace_dump(const Res2ChainParams& cp) {
@@ -349,7 +622,9 @@ void res2chain_trace_dump(const Res2ChainParams& cp) {
     unsigned long long t0 = ~0ull;
     for (unsigned long long v : h)
         if (v && v < t0) t0 = v;
-    static const char* roles[3] = {"tma", "mma", "epi"};
+    static const char* const single_roles[3] = {"tma", "mma", "epi"};
+    static const char* const pair_roles[3] = {"utt A", "utt B", "weights"};  // see RP_STAMP
+    const char* const* roles = cp.paired ? pair_roles : single_roles;
     for (int r = 0; r < 3; ++r)
         for (int j = 0; j < 7; ++j) {
             printf("res2chain trace %s conv %d:", roles[r], j);
@@ -358,5 +633,6 @@ void res2chain_trace_dump(const Res2ChainParams& cp) {
         }
 }
 bool res2chain_fits(int T, int P) { return P == RC_PAD && T + 2 * P <= RC_MAX_TP; }
+bool res2chain_pair_fits(int T, int P) { return P == RC_PAD && T + 2 * P <= RP_MAX_TP; }
 
 }  // namespace ppv
