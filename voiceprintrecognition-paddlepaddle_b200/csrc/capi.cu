@@ -561,6 +561,7 @@ int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision,
     PPV_CUDA_OK(cudaEventElapsedTime(&ms, e0, e1));
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
+    gemm_trace_dump(gp);  // PPV_GEMM_TRACE: the last timed launch
     *ms_per_launch = ms / float(iters);
     return PPV_OK;
     PPV_GUARD_END

@@ -144,6 +144,8 @@ struct Epilogue {
     int lean = 0;  // set by gemm_build: the epilogue needs only what epilogue_frag_lean does (gemm_epilogue.cuh)
 };
 
+constexpr int GEMM_TRACE_TILES = 16;  // PPV_GEMM_TRACE: CTA 0's first tiles stamped
+
 struct GemmParams {
     CUtensorMap mapA[GEMM_MAX_MAPS];
     CUtensorMap mapB;
@@ -158,8 +160,11 @@ struct GemmParams {
     int M, N;
     int m_tiles, n_tiles;
     Epilogue epi;
+    // debug (PPV_GEMM_TRACE): clock64 stamps of CTA 0, [role][tile][event] with role 0 = producer, 1 + g = MMA warpgroup g
+    unsigned long long* trace;
     int bn;  // n-tile width (64, 128 or 256): selects the kernel instance.  Last, so that no kernel parameter offset depends on it.
 };
+void gemm_trace_dump(const GemmParams& gp);
 
 struct GemmSource {
     Planes t;

@@ -1,9 +1,9 @@
 // Shared epilogue of the wgmma kernels (gemm_wgmma.cu, res2conv.cu, conv3x3.cu): one warpgroup's 64 x BN fp32 accumulator
 // fragment (registers, layout in ptx.cuh) -> bias / per-utterance bias / ReLU / BatchNorm affine / tanh / sigmoid -> split-bf16
 // planes (incl. the reflect-halo rows of the padded time layout) or fp32.  Each thread owns two rows and BN / 4 columns of the
-// tile, in pairs of adjacent columns; every pair is processed and stored straight from the registers.
-// Not tuned on H100: a warp's store covers 16 B of each of 8 rows (half of a 32-byte sector).  Gathering a row's 8 columns into one
-// 16-byte store per lane (a 4 x 4 exchange of column pairs inside each quad of lanes) is the obvious next step; it is not measured.
+// tile, in pairs of adjacent columns.  The general path (epilogue_frag) stores every pair straight from the registers: a warp's store
+// covers 16 B of each of 8 rows (half of a 32-byte sector).  The lean path of the gather-GEMM (epilogue_frag_lean) first exchanges the
+// pairs inside each quad of lanes so that every lane stores 8 columns of a row with one 16-byte store per plane.
 #pragma once
 #include "common.h"
 #include "ptx.cuh"
@@ -135,59 +135,82 @@ __device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0,
 }
 
 // The epilogues of the ECAPA-TDNN layers (gemm_build sets ep.lean): split-bf16 planes on the input row grid, bias / per-utterance
-// bias / ReLU / BN affine / tanh, no halo, mirror or zero rows, no segment scale, SiLU, sigmoid or clipped ReLU.  The two rows'
-// mapping and store addresses are computed once per fragment, and each column's bias / BN vectors are loaded once for both rows.
-// Per element the arithmetic is epilogue_math1's, in the same order.
+// bias / ReLU / BN affine / tanh, no halo, mirror or zero rows, no segment scale, SiLU, sigmoid or clipped ReLU.  Per element the
+// arithmetic is epilogue_math1's, in the same order; each column's bias / BN vectors are loaded once for both of a thread's rows.
+// The fragment is walked 32 columns (four 8-column groups) per trip.  The four lanes of a quad share two rows and hold two columns of
+// each group; a 4 x 4 transpose inside the quad (two butterfly stages of __shfl_xor_sync) gives lane q all 8 columns of group q of
+// both rows, so each row leaves as one 16-byte store per plane instead of four 4-byte ones (whole 32-byte sectors per warp store).
 template <int BN, typename RowOf>
 __device__ __forceinline__ void epilogue_frag_lean(const Epilogue& ep, int N, int n0, float (&acc)[BN / 2], RowOf&& row_of, int t) {
-    const int w = t >> 5, l = t & 31;
+    static_assert(BN % 32 == 0, "lean epilogue: whole 32-column trips");
+    const int w = t >> 5, l = t & 31, q = l & 3;
     const int r0 = 16 * w + (l >> 2);
     const EpiRow ra = epilogue_row(ep, row_of(r0), 0);
     const EpiRow rb = epilogue_row(ep, row_of(r0 + 8), 0);
-    const int c0 = n0 + 2 * (l & 3);  // this thread's first column; its columns are c0 + 8 j + {0, 1}
-    __nv_bfloat16* const obase = static_cast<__nv_bfloat16*>(ep.out) + ep.out_col0 + c0;
-    uint32_t* const pa = reinterpret_cast<uint32_t*>(obase + ra.out_row * ep.out_ld);
-    uint32_t* const pb = reinterpret_cast<uint32_t*>(obase + rb.out_row * ep.out_ld);
-    const int64_t lo_off = ep.out_plane_stride / 2;  // the lo plane, in 32-bit words (gemm_build: plane stride % 16 == 0)
-    const float* const ga = ep.rowgrp_bias ? ep.rowgrp_bias + ra.grp * N + c0 : nullptr;
-    const float* const gb = ep.rowgrp_bias ? ep.rowgrp_bias + rb.grp * N + c0 : nullptr;
-    constexpr int EPI_GROUPS = BN / 8 < 4 ? BN / 8 : 4;
+    const int cq = n0 + 8 * q;  // after the transpose this lane's columns are cq + 8 c + [0, 8) in trip c / 4
+    __nv_bfloat16* const obase = static_cast<__nv_bfloat16*>(ep.out) + ep.out_col0 + cq;
+    __nv_bfloat16* const pa = obase + ra.out_row * ep.out_ld;
+    __nv_bfloat16* const pb = obase + rb.out_row * ep.out_ld;
+    const int64_t lo_off = ep.out_plane_stride;  // gemm_build: out_ld, out_col0 and the plane stride are multiples of 16 elements
+    const float* const ga = ep.rowgrp_bias ? ep.rowgrp_bias + ra.grp * N + cq : nullptr;
+    const float* const gb = ep.rowgrp_bias ? ep.rowgrp_bias + rb.grp * N + cq : nullptr;
+    const bool q2 = (q & 2) != 0, q1 = (q & 1) != 0;
 #pragma unroll 1
-    for (int c = 0; c < BN / 8; c += EPI_GROUPS) {
+    for (int c = 0; c < BN / 8; c += 4) {
+        // a[2 i], a[2 i + 1]: this lane's two columns of group i, row a (b: row b)
+        float a[8], b[8];
 #pragma unroll
-        for (int i = 0; i < EPI_GROUPS; ++i) {
-            const int j = 8 * (c + i);
-            if (c0 + j >= N) continue;  // planes output: N % 32 == 0, so column c0 + j + 1 exists too
-            float xa0 = acc[4 * i + 0], xa1 = acc[4 * i + 1], xb0 = acc[4 * i + 2], xb1 = acc[4 * i + 3];
-            if (ep.bias) {
-                const float b0 = __ldg(ep.bias + c0 + j), b1 = __ldg(ep.bias + c0 + j + 1);
-                xa0 += b0, xa1 += b1, xb0 += b0, xb1 += b1;
-            }
-            if (ga) {
-                xa0 += __ldg(ga + j), xa1 += __ldg(ga + j + 1);
-                xb0 += __ldg(gb + j), xb1 += __ldg(gb + j + 1);
-            }
-            if (ep.relu) xa0 = fmaxf(xa0, 0.f), xa1 = fmaxf(xa1, 0.f), xb0 = fmaxf(xb0, 0.f), xb1 = fmaxf(xb1, 0.f);
-            if (ep.bn_scale) {
-                const float s0 = __ldg(ep.bn_scale + c0 + j), s1 = __ldg(ep.bn_scale + c0 + j + 1);
-                const float h0 = __ldg(ep.bn_shift + c0 + j), h1 = __ldg(ep.bn_shift + c0 + j + 1);
-                xa0 = fmaf(xa0, s0, h0), xa1 = fmaf(xa1, s1, h1), xb0 = fmaf(xb0, s0, h0), xb1 = fmaf(xb1, s1, h1);
-            }
-            if (ep.tanh_) xa0 = tanhf(xa0), xa1 = tanhf(xa1), xb0 = tanhf(xb0), xb1 = tanhf(xb1);
-            uint32_t h, lo;
-            if (ra.valid) {
-                split_pack_bf16x2(xa0, xa1, h, lo);
-                pa[j / 2] = h;
-                pa[j / 2 + lo_off] = lo;
-            }
-            if (rb.valid) {
-                split_pack_bf16x2(xb0, xb1, h, lo);
-                pb[j / 2] = h;
-                pb[j / 2 + lo_off] = lo;
-            }
+        for (int i = 0; i < 4; ++i) a[2 * i] = acc[4 * i], a[2 * i + 1] = acc[4 * i + 1], b[2 * i] = acc[4 * i + 2], b[2 * i + 1] = acc[4 * i + 3];
+#pragma unroll
+        for (int j = 0; j + 16 < BN / 2; ++j) acc[j] = acc[j + 16];
+        // stage 1, lanes q and q ^ 2 swap 2 x 2 blocks of column pairs; stage 2, lanes q and q ^ 1 swap single pairs
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {  // e = 2 j + f: pair j in {0, 1}, float f
+            const float sa = q2 ? a[e] : a[e + 4], sb = q2 ? b[e] : b[e + 4];
+            const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 2), rb_ = __shfl_xor_sync(0xffffffffu, sb, 2);
+            if (q2) a[e] = ra_, b[e] = rb_;
+            else a[e + 4] = ra_, b[e + 4] = rb_;
         }
 #pragma unroll
-        for (int j = 0; j + 4 * EPI_GROUPS < BN / 2; ++j) acc[j] = acc[j + 4 * EPI_GROUPS];
+        for (int e = 0; e < 8; e += 4) {
+#pragma unroll
+            for (int f = 0; f < 2; ++f) {
+                const float sa = q1 ? a[e + f] : a[e + 2 + f], sb = q1 ? b[e + f] : b[e + 2 + f];
+                const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 1), rb_ = __shfl_xor_sync(0xffffffffu, sb, 1);
+                if (q1) a[e + f] = ra_, b[e + f] = rb_;
+                else a[e + 2 + f] = ra_, b[e + 2 + f] = rb_;
+            }
+        }
+        const int j0 = 8 * c;  // this lane's first column of the trip, relative to cq
+        if (n0 + j0 >= N) continue;  // planes output: N % 32 == 0, so a trip's 32 columns are all in or all out
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int col = cq + j0 + k;
+            if (ep.bias) {
+                const float bb = __ldg(ep.bias + col);
+                a[k] += bb, b[k] += bb;
+            }
+            if (ga) a[k] += __ldg(ga + j0 + k), b[k] += __ldg(gb + j0 + k);
+            if (ep.relu) a[k] = fmaxf(a[k], 0.f), b[k] = fmaxf(b[k], 0.f);
+            if (ep.bn_scale) {
+                const float sc = __ldg(ep.bn_scale + col), sh = __ldg(ep.bn_shift + col);
+                a[k] = fmaf(a[k], sc, sh), b[k] = fmaf(b[k], sc, sh);
+            }
+            if (ep.tanh_) a[k] = tanhf(a[k]), b[k] = tanhf(b[k]);
+        }
+        uint4 ha, la, hb, lb;
+        split_pack_bf16x2(a[0], a[1], ha.x, la.x), split_pack_bf16x2(a[2], a[3], ha.y, la.y);
+        split_pack_bf16x2(a[4], a[5], ha.z, la.z), split_pack_bf16x2(a[6], a[7], ha.w, la.w);
+        split_pack_bf16x2(b[0], b[1], hb.x, lb.x), split_pack_bf16x2(b[2], b[3], hb.y, lb.y);
+        split_pack_bf16x2(b[4], b[5], hb.z, lb.z), split_pack_bf16x2(b[6], b[7], hb.w, lb.w);
+        if (ra.valid) {
+            *reinterpret_cast<uint4*>(pa + j0) = ha;
+            *reinterpret_cast<uint4*>(pa + j0 + lo_off) = la;
+        }
+        if (rb.valid) {
+            *reinterpret_cast<uint4*>(pb + j0) = hb;
+            *reinterpret_cast<uint4*>(pb + j0 + lo_off) = lb;
+        }
     }
 }
 

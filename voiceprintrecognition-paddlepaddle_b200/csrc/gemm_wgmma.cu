@@ -106,6 +106,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     const int nk = gp.num_ksteps;
     auto tile_m = [&](int t) { return (t % mn_tiles) / gp.n_tiles; };
     auto tile_n = [&](int t) { return (t % mn_tiles) % gp.n_tiles; };
+    // PPV_GEMM_TRACE stamps of CTA 0 (`on`: tracing, this CTA, the stamping thread, local tile in range).  Producer events: 0 / 1 its
+    // first / last ring-slot wait of the tile passed, 7 of tile 0 the kernel start.  MMA warpgroup events: 0 hand-off barrier passed,
+    // 1 first `full` wait passed, 2 last k-step issued, 3 wgmma_wait<0> returned, 4 / 5 epilogue start / end.
+    const bool trace_cta = gp.trace != nullptr && blockIdx.x == 0;
+    auto stamp = [&](bool on, int role, int local, int ev) {
+        if (on) gp.trace[(role * GEMM_TRACE_TILES + local) * 8 + ev] = clock64();
+    };
+    stamp(trace_cta && threadIdx.x == 0, 0, 0, 7);
 
     if (warp < 4) {
         setmaxnreg_dec<40>();  // all four producer warps; warps 1-3 have nothing else to do
@@ -119,7 +127,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                     for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(w_res + (s * Cfg::NB + p) * Cfg::B_BYTES, &gp.mapB, w_full, s * BK, 0, p);
             }
             __syncwarp();
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            int local = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
+                const bool tr = trace_cta && lane == 0 && local < GEMM_TRACE_TILES;
                 const int zsplit = tile / mn_tiles;
                 const int m0 = tile_m(tile) * GEMM_BM;
                 const int n0 = tile_n(tile) * BN;
@@ -137,6 +147,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 __syncwarp();
                 for (int s = 0; s < nk; ++s) {
                     mbar_wait(empty_bar(stage), phase ^ 1u);
+                    stamp(tr && s == 0, 0, local, 0);
+                    stamp(tr && s == nk - 1, 0, local, 1);
                     if (lane == 0) {
                         const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
                         const uint32_t sb = sa + Cfg::NA * Cfg::A_BYTES;
@@ -198,12 +210,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             }
             const int m0 = tile_m(tile) * GEMM_BM;
             const int n0 = tile_n(tile) * BN;
+            const bool tr = trace_cta && t == 0 && local < GEMM_TRACE_TILES;
             named_bar_sync_if(local > 0, 1 + g, 2 * 128);  // the other warpgroup has taken every k-step of tile local - 1
+            stamp(tr, 1 + g, local, 0);
             int prev = -1;
             wgmma_fence_acc(acc0);
             wgmma_fence_acc(acc1);
             for (int s = 0; s < nk; ++s) {
                 mbar_wait(full_bar(stage), phase);
+                stamp(tr && s == 0, 1 + g, local, 1);
                 const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
                 const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
                 const uint64_t a0_hi = make_kmajor_desc<BK>(sa), a1_hi = make_kmajor_desc<BK>(sa + A_HALF);
@@ -230,6 +245,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                     }
                 }
                 wgmma_commit();
+                stamp(tr && s == nk - 1, 1 + g, local, 2);
                 wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
                 if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
                 prev = stage;
@@ -239,11 +255,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 }
             }
             wgmma_wait<0>();
+            stamp(tr, 1 + g, local, 3);
             // the other warpgroup may start tile local + 1
             named_bar_arrive_if(local + 1 < my_tiles, 1 + (g ^ 1), 2 * 128);
             wgmma_fence_acc(acc0);
             wgmma_fence_acc(acc1);
             if (t == 0) mbar_arrive(empty_bar(prev));
+            stamp(tr, 1 + g, local, 4);
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
             // rows 0-63 from acc0, then rows 64-127 moved down into acc0: one copy of the epilogue code
 #pragma unroll 1
@@ -253,6 +271,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
                 for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
             }
+            stamp(tr, 1 + g, local, 5);
         }
     } else {
         setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
@@ -266,13 +285,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         if (gp.ws) mbar_wait(w_full, 0);
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int local = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
             const int m0 = tile_m(tile) * GEMM_BM;
             const int n0 = tile_n(tile) * BN;
+            const bool tr = trace_cta && t == 0 && local < GEMM_TRACE_TILES;
+            stamp(tr, 1 + g, local, 0);
             int prev = -1;
             wgmma_fence_acc(acc);
             for (int s = 0; s < nk; ++s) {
                 mbar_wait(full_bar(stage), phase);
+                stamp(tr && s == 0, 1 + g, local, 1);
                 const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
                 const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
                 const uint64_t a_hi = make_kmajor_desc<BK>(sa + g * A_WG_OFF);
@@ -290,6 +313,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                     for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
                 }
                 wgmma_commit();
+                stamp(tr && s == nk - 1, 1 + g, local, 2);
                 wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
                 if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
                 prev = stage;
@@ -299,11 +323,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 }
             }
             wgmma_wait<0>();
+            stamp(tr, 1 + g, local, 3);
             wgmma_fence_acc(acc);
             if (t == 0) mbar_arrive(empty_bar(prev));
+            stamp(tr, 1 + g, local, 4);
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
             const int rbase = m0 + 64 * g;
             gemm_epilogue<BN>(gp.epi, gp.N, n0, acc, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
+            stamp(tr, 1 + g, local, 5);
         }
     }
 }
@@ -416,6 +443,14 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
         const char* pf = getenv("PPV_GEMM_NO_L2PREFETCH");
         gp->l2_prefetch = (pf && pf[0] == '1') ? 0 : 1;
     }
+    if (getenv("PPV_GEMM_TRACE")) {  // debug: leaked on purpose, read back by gemm_trace_dump
+        static unsigned long long* buf = nullptr;
+        if (!buf) {
+            PPV_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&buf), 3 * GEMM_TRACE_TILES * 8 * sizeof(unsigned long long)));
+            PPV_CUDA_OK(cudaMemset(buf, 0, 3 * GEMM_TRACE_TILES * 8 * sizeof(unsigned long long)));
+        }
+        gp->trace = buf;
+    }
     if (epi.out_mode == OUT_PLANES) {
         PPV_REQUIRE((epi.out_ld % 16) == 0 && (epi.out_col0 % 16) == 0 && (epi.out_plane_stride % 16) == 0 &&
                         (reinterpret_cast<uintptr_t>(epi.out) & 15) == 0,
@@ -483,6 +518,33 @@ template <int BN>
 static int launch_bn(const GemmParams& gp, bool x3, int num_sms, cudaStream_t stream) {
     if (gp.bk == 32) return x3 ? launch_one<BN, 3, 32>(gp, num_sms, stream) : launch_one<BN, 1, 32>(gp, num_sms, stream);
     return x3 ? launch_one<BN, 3, 64>(gp, num_sms, stream) : launch_one<BN, 1, 64>(gp, num_sms, stream);
+}
+
+// Prints the stamps of the last traced launch in cycles from the kernel start, one line per role and tile, with the phases they give:
+// wait = hand-off passed -> first `full` passed, kloop = first `full` -> wgmma_wait<0> returned, epi = epilogue start -> end,
+// period = this tile's epilogue end - the previous tile's of the same warpgroup.
+void gemm_trace_dump(const GemmParams& gp) {
+    if (!gp.trace) return;
+    unsigned long long h[3 * GEMM_TRACE_TILES * 8];
+    cudaDeviceSynchronize();
+    cudaMemcpy(h, gp.trace, sizeof(h), cudaMemcpyDeviceToHost);
+    const unsigned long long t0 = h[7];
+    auto at = [&](int r, int i, int e) -> long long { const unsigned long long v = h[(r * GEMM_TRACE_TILES + i) * 8 + e]; return v ? (long long)(v - t0) : -1ll; };
+    printf("gemm trace M=%d N=%d nk=%d BN=%d (cycles from kernel start)\n", gp.M, gp.N, gp.num_ksteps, gp.bn);
+    for (int i = 0; i < GEMM_TRACE_TILES; ++i)
+        if (at(0, i, 0) >= 0) printf("gemm trace tma  tile %2d: first slot %8lld  last slot %8lld\n", i, at(0, i, 0), at(0, i, 1));
+    for (int r = 1; r < 3; ++r) {
+        long long prev_end = -1;
+        for (int i = 0; i < GEMM_TRACE_TILES; ++i) {
+            if (at(r, i, 0) < 0) continue;
+            printf("gemm trace wg%d  tile %2d:", r - 1, i);
+            for (int e = 0; e < 6; ++e) printf(" %8lld", at(r, i, e));
+            printf("   wait %6lld  kloop %6lld  epi %6lld  period %6lld\n", at(r, i, 1) - at(r, i, 0), at(r, i, 3) - at(r, i, 1),
+                   at(r, i, 5) - at(r, i, 4), prev_end >= 0 ? at(r, i, 5) - prev_end : -1ll);
+            prev_end = at(r, i, 5);
+        }
+    }
+    fflush(stdout);
 }
 
 int gemm_launch(const GemmParams& gp, int precision, int num_sms, cudaStream_t stream) {
