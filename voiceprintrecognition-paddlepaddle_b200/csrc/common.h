@@ -188,7 +188,6 @@ inline int gemm_pick_bn(int N, int max_bn = 256) {
         if (N % bn == 0) return bn;
     return 64;
 }
-int gemm_max_smem_setup();
 
 int encode_planes_map(CUtensorMap* m, const Planes& t, int box_rows);  // 3-D TMA map over split planes, box {64, box_rows, 1}, SWIZZLE_128B
 int encode_planes_map_ex(CUtensorMap* m, const Planes& t, int box_cols, int box_rows, int swizzle_bytes);  // 0 / 64 / 128

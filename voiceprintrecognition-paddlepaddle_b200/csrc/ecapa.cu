@@ -347,8 +347,6 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     const bool res2_paired = use_res2_chain && res2chain_pair_fits(T, P) && !(rcenv && strcmp(rcenv, "single") == 0);
     const char* skenv = getenv("PPV_SKINNY");  // 0 = the per-utterance linear layers through the tensor-core gather-GEMM (A-B timing)
     const bool use_skinny = !(skenv && skenv[0] == '0');
-    const char* bkenv = getenv("PPV_GEMM_BK32");  // experiment: 1 = 32-wide k-steps (SWIZZLE_64B) on the wide-N layers
-    const bool bk32_enabled = (bkenv && bkenv[0] == '1');
 
     auto add_gemm = [&](const ConvW& cw, const std::vector<KSpec>& ks, const Planes* src_override, int override_col0, int M,
                         Epilogue ep) -> int {
@@ -389,9 +387,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         }
         Step stp;
         stp.kind = Step::GEMM;
-        // 32-wide k-steps (twice the ring slots) for the wide-N layers whose K fits the k-step table
-        const int bk = (cw.N >= 512 && cw.Ktot <= 32 * GEMM_MAX_KSTEPS && bk32_enabled) ? 32 : 0;
-        int rc = gemm_build(&stp.gp, srcs.data(), int(srcs.size()), cw.W, M, cw.N, ep, gemm_pick_bn(cw.N, ECAPA_MAX_BN), bk);
+        int rc = gemm_build(&stp.gp, srcs.data(), int(srcs.size()), cw.W, M, cw.N, ep, gemm_pick_bn(cw.N, ECAPA_MAX_BN));
         if (rc) return rc;
         m->steps.push_back(stp);
         return PPV_OK;

@@ -332,7 +332,7 @@ void tr_carve(Trainer* t, TrCarve& k, int B, int T) {
     // weight-gradient partials: max over layers of splits * Mpad * Ktot; splits <= num_sms
     size_t wmax = 0;
     auto wsize = [&](const TConv& c) {
-        const size_t N = size_t(c.taps) * c.Cinp, mt = (c.Cout + 127) / 128, bn = N % 256 == 0 ? 256 : N % 128 == 0 ? 128 : 64, nt = (N + bn - 1) / bn;
+        const size_t N = size_t(c.taps) * c.Cinp, mt = (c.Cout + 127) / 128, bn = gemm_pick_bn(int(N)), nt = (N + bn - 1) / bn;
         const size_t splits = std::max<size_t>(1, std::min<size_t>((t->num_sms + mt * nt - 1) / (mt * nt), (Rp + 63) / 64));
         wmax = std::max(wmax, splits * mt * 128 * N);
     };
