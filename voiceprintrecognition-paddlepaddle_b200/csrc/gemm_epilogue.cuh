@@ -134,6 +134,31 @@ __device__ __forceinline__ void epilogue_frag(const Epilogue& ep, int N, int n0,
     }
 }
 
+// 4 x 4 transpose of column pairs inside each quad of lanes (two butterfly stages of __shfl_xor_sync), for 16-byte epilogue
+// accesses.  On entry a[2 i], a[2 i + 1] are this lane's two columns of 8-column group i of row a (b: row b), i in [0, 4), as the
+// wgmma fragment holds them; on return lane q = lane & 3 holds all 8 columns of group q of both rows, a[k] / b[k] = column 8 q + k.
+__device__ __forceinline__ void quad_transpose_pairs(float (&a)[8], float (&b)[8], int q) {
+    const bool q2 = (q & 2) != 0, q1 = (q & 1) != 0;
+    // stage 1, lanes q and q ^ 2 swap 2 x 2 blocks of column pairs; stage 2, lanes q and q ^ 1 swap single pairs
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {  // e = 2 j + f: pair j in {0, 1}, float f
+        const float sa = q2 ? a[e] : a[e + 4], sb = q2 ? b[e] : b[e + 4];
+        const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 2), rb_ = __shfl_xor_sync(0xffffffffu, sb, 2);
+        if (q2) a[e] = ra_, b[e] = rb_;
+        else a[e + 4] = ra_, b[e + 4] = rb_;
+    }
+#pragma unroll
+    for (int e = 0; e < 8; e += 4) {
+#pragma unroll
+        for (int f = 0; f < 2; ++f) {
+            const float sa = q1 ? a[e + f] : a[e + 2 + f], sb = q1 ? b[e + f] : b[e + 2 + f];
+            const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 1), rb_ = __shfl_xor_sync(0xffffffffu, sb, 1);
+            if (q1) a[e + f] = ra_, b[e + f] = rb_;
+            else a[e + 2 + f] = ra_, b[e + 2 + f] = rb_;
+        }
+    }
+}
+
 // The epilogues of the ECAPA-TDNN layers (gemm_build sets ep.lean): split-bf16 planes on the input row grid, bias / per-utterance
 // bias / ReLU / BN affine / tanh, no halo, mirror or zero rows, no segment scale, SiLU, sigmoid or clipped ReLU.  Per element the
 // arithmetic is epilogue_math1's, in the same order; each column's bias / BN vectors are loaded once for both of a thread's rows.
@@ -154,7 +179,6 @@ __device__ __forceinline__ void epilogue_frag_lean(const Epilogue& ep, int N, in
     const int64_t lo_off = ep.out_plane_stride;  // gemm_build: out_ld, out_col0 and the plane stride are multiples of 16 elements
     const float* const ga = ep.rowgrp_bias ? ep.rowgrp_bias + ra.grp * N + cq : nullptr;
     const float* const gb = ep.rowgrp_bias ? ep.rowgrp_bias + rb.grp * N + cq : nullptr;
-    const bool q2 = (q & 2) != 0, q1 = (q & 1) != 0;
 #pragma unroll 1
     for (int c = 0; c < BN / 8; c += 4) {
         // a[2 i], a[2 i + 1]: this lane's two columns of group i, row a (b: row b)
@@ -163,24 +187,7 @@ __device__ __forceinline__ void epilogue_frag_lean(const Epilogue& ep, int N, in
         for (int i = 0; i < 4; ++i) a[2 * i] = acc[4 * i], a[2 * i + 1] = acc[4 * i + 1], b[2 * i] = acc[4 * i + 2], b[2 * i + 1] = acc[4 * i + 3];
 #pragma unroll
         for (int j = 0; j + 16 < BN / 2; ++j) acc[j] = acc[j + 16];
-        // stage 1, lanes q and q ^ 2 swap 2 x 2 blocks of column pairs; stage 2, lanes q and q ^ 1 swap single pairs
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {  // e = 2 j + f: pair j in {0, 1}, float f
-            const float sa = q2 ? a[e] : a[e + 4], sb = q2 ? b[e] : b[e + 4];
-            const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 2), rb_ = __shfl_xor_sync(0xffffffffu, sb, 2);
-            if (q2) a[e] = ra_, b[e] = rb_;
-            else a[e + 4] = ra_, b[e + 4] = rb_;
-        }
-#pragma unroll
-        for (int e = 0; e < 8; e += 4) {
-#pragma unroll
-            for (int f = 0; f < 2; ++f) {
-                const float sa = q1 ? a[e + f] : a[e + 2 + f], sb = q1 ? b[e + f] : b[e + 2 + f];
-                const float ra_ = __shfl_xor_sync(0xffffffffu, sa, 1), rb_ = __shfl_xor_sync(0xffffffffu, sb, 1);
-                if (q1) a[e + f] = ra_, b[e + f] = rb_;
-                else a[e + 2 + f] = ra_, b[e + 2 + f] = rb_;
-            }
-        }
+        quad_transpose_pairs(a, b, q);
         const int j0 = 8 * c;  // this lane's first column of the trip, relative to cq
         if (n0 + j0 >= N) continue;  // planes output: N % 32 == 0, so a trip's 32 columns are all in or all out
 #pragma unroll

@@ -43,11 +43,24 @@ struct RCCfg {
 
 // Predicated stores, in program order (volatile asm is not reordered): with branches around plain stores the scheduler computes
 // many columns ahead of their stores and runs out of registers.
-__device__ __forceinline__ void rp_st_global(bool pred, uint32_t* p, uint32_t v) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.u32 [%0], %1;\n\t}" ::"l"(p), "r"(v), "r"(uint32_t(pred)) : "memory");
-}
 __device__ __forceinline__ void rp_st_shared(bool pred, uint32_t a, uint32_t v) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.shared.u32 [%0], %1;\n\t}" ::"r"(a), "r"(v), "r"(uint32_t(pred)) : "memory");
+}
+// 16-byte variants for the paired kernel's epilogue (8 bf16 columns of one row and plane)
+__device__ __forceinline__ void rp_st_global_v4(bool pred, const void* p, uint4 v) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t@p st.global.v4.u32 [%0], {%1, %2, %3, %4};\n\t}" ::"l"(p), "r"(v.x), "r"(v.y),
+                 "r"(v.z), "r"(v.w), "r"(uint32_t(pred))
+                 : "memory");
+}
+__device__ __forceinline__ void rp_st_shared_v4(bool pred, uint32_t a, uint4 v) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t@p st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n\t}" ::"r"(a), "r"(v.x), "r"(v.y),
+                 "r"(v.z), "r"(v.w), "r"(uint32_t(pred))
+                 : "memory");
+}
+__device__ __forceinline__ uint4 rp_ld_shared_v4(uint32_t a) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
+    return v;
 }
 
 __device__ __forceinline__ uint32_t rc_ld_shared(uint32_t a) {
@@ -307,9 +320,12 @@ __global__ void __launch_bounds__(RC_THREADS, 1) res2chain_kernel(const __grid_c
 //   MMA_A(j) | epilogue_B(j-1)  ->  MMA_B(j) | epilogue_A(j)  ->  W[j+1] lands  ->  MMA_A(j+1) | epilogue_B(j)  -> ...
 // B = 256 utterances are 128 CTAs, one wave.  Five MMA warpgroups (640 threads, 96 registers each): warpgroup w owns the
 // m64 row block w of BOTH utterances, one 64 x 64 accumulator per utterance.  The operands (2 x 336 rows x planes) and one
-// conv's weights (shared by both utterances) leave no room for staging tiles, so the epilogue reads x_{j+2} and writes y_{j+1}
-// with plain global accesses; x_{j+2} is prefetched into L2 when conv j-1 starts.  Per row, the MMA order, the epilogue formulas
-// and the reflect halo rows are those of the one-utterance kernel above, so the outputs are bitwise equal to its outputs.
+// conv's weights (shared by both utterances) leave no room for staging tiles.  Instead, once every MMA of conv j of an
+// utterance has retired, its operand tile is dead, and thread 0 loads chunk x_{j+2} into that tile by TMA (prefetched into L2
+// when conv j-1 starts).  The epilogue writes y_{j+1} to HBM straight from the registers, then waits for x_{j+2} and overwrites
+// the tile in place with x_{j+2} + y_{j+1}.  Both use 16-byte accesses after a transpose inside each quad of lanes.  Per row, the
+// MMA order, the epilogue formulas and the reflect halo rows are those of the one-utterance kernel above, so the outputs are
+// bitwise equal to its outputs.
 constexpr int RP_BLOCKS = 5;                          // m64 row blocks per utterance, one per MMA warpgroup
 constexpr int RP_MAX_TP = RP_BLOCKS * 64;             // 320
 constexpr int RP_BOX_ROWS = 168;                      // two boxes: 336 >= 4 + 320 + 4 rows; 168 * 128 B is a multiple of 1024
@@ -327,7 +343,8 @@ struct RPCfg {
 static_assert(RPCfg<3>::SMEM_BYTES <= 232448, "paired res2chain exceeds the H100 shared-memory opt-in");
 
 // trace (PPV_RES2_TRACE) of CTA 0's first pair: role 0 / 1 = utterance A / B, events 0 MMA issued, 1 MMA retired (every
-// warpgroup), 2 epilogue start, 3 epilogue end (warpgroup 0); role 2 = weights, events 0 load issued, 1 landed
+// warpgroup), 2 epilogue start, 3 epilogue end, 4 x_{j+2} load issued, 5 y_{j+1} stores done, 6 x_{j+2} barrier passed
+// (thread 0); role 2 = weights, events 0 load issued, 1 landed
 #define RP_STAMP(role, conv, ev)                                                                                \
     do {                                                                                                        \
         if (trace_on) cp.trace[((role) * 8 + (conv)) * 8 + (ev)] = clock64();                                   \
@@ -351,6 +368,7 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
     float* const vec = reinterpret_cast<float*>(a_gen + 2 * Cfg::U_BYTES + Cfg::W_SLOT);  // [conv][bias, scale, shift][64]
     const uint32_t bar_base = w_base + Cfg::W_SLOT + RP_VEC_FLOATS * 4;
     const uint32_t x_full = bar_base, w_full = bar_base + 8;
+    auto x_next = [&](int u) { return bar_base + 16u + 8u * u; };  // x_{j+2} of utterance u has landed in its tile
 
     const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, l = tid & 31;
     const int nconv = cp.nconv, T = cp.T, P = cp.P, Tp = cp.Tp;
@@ -359,6 +377,8 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
         for (int j = 0; j < nconv; ++j) prefetch_tmap(&cp.mapW[j]);
         mbar_init(x_full, 1);
         mbar_init(w_full, 1);
+        mbar_init(x_next(0), 1);
+        mbar_init(x_next(1), 1);
         fence_mbar_init();
     }
     __syncthreads();
@@ -374,7 +394,15 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
         for (int tap = 0; tap < 3; ++tap)
             for (int pl = 0; pl < NP; ++pl) tma_load_3d(w_base + (tap * NP + pl) * RC_W_TILE, &cp.mapW[j], w_full, tap * 64, 0, pl);
     };
-    // x_{c} (c = chunk) of both utterances of the pair -> L2, for the epilogue's global loads
+    // chunk c of utterance b -> slot u's operand tile: rows [-4, 332) around the utterance in two boxes, completing on `bar`.
+    // Rows past the end of the batch are filled with zeros by TMA.
+    auto load_x = [&](uint32_t bar, int u, int b, int c) {
+        for (int pl = 0; pl < NP; ++pl)
+            for (int h = 0; h < 2; ++h)
+                tma_load_3d(smem_base + u * Cfg::U_BYTES + pl * RP_A_PLANE + h * RP_BOX_ROWS * 128, &cp.mapX, bar, c * cp.width,
+                            b * Tp - RC_PAD + h * RP_BOX_ROWS, pl);
+    };
+    // x_{c} (c = chunk) of both utterances of the pair -> L2, where load_x of x_{c} one conv later finds it
     auto prefetch_chunk = [&](int b0, int c) {
         for (int u = 0; u < 2 && b0 + u < cp.B; ++u)
             for (int pl = 0; pl < NP; ++pl)
@@ -402,60 +430,82 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
         }
         wgmma_commit();
     };
-    // conv j of utterance b (slot u): y_{j+1} -> HBM on rows [0, Tp); x_{j+2} + y_{j+1} -> the operand tile on the valid rows and
-    // their reflect mirrors.  An absent utterance (odd B) stores nothing and loads nothing.
-    auto epilogue = [&](const float (&acc)[BN / 2], int u, int b, int j) {
+    // conv j of utterance b (slot u): y_{j+1} -> HBM on rows [0, Tp); then, once x_{j+2} has landed in the operand tile (load_x
+    // on x_next(u), completion `xpar`), x_{j+2} + y_{j+1} -> the tile in place on the valid rows and their reflect mirrors.  The
+    // load also overwrote the halo rows [0, P) and [P + T, Tp), which the mirrors rewrite, and the rows outside [0, Tp), which only
+    // feed halo rows of y (discarded by tdnn2).  An absent utterance (odd B) stores nothing and waits for nothing.
+    // After quad_transpose_pairs lane q holds columns 32 c + 8 q + [0, 8) of its two rows in half c: one 16-byte access per row,
+    // half and plane.  acc is consumed: pass 1 leaves the BN outputs of half c, row h in acc[16 c + 8 h + k] for pass 2.
+    bool trace_on = false;
+    auto epilogue = [&](float (&acc)[BN / 2], int u, int b, int j, uint32_t xpar) {
         b = rp_opaque(b);
         const bool present = b < cp.B, has_next = j + 1 < nconv;
-        const float* const vb = vec + j * 192 + 2 * (l & 3);
-        const uint32_t tile = smem_base + u * Cfg::U_BYTES;
-        // an eighth of the fragment (one row, two column pairs) per trip of a loop that is not unrolled: unrolled, the compiler
-        // computes values far ahead of their stores and spills them.  acc is read through selects, never with a runtime index.
-#pragma unroll 1
-        for (int part = 0; part < 8; ++part) {
-            const int h = part >> 2, qh = 2 * (part & 3);
-            const int r = wg * 64 + 16 * wq + (l >> 2) + 8 * h;  // padded row inside the utterance
-            const int tt = r - P, uu = T - 1 - tt;
-            const bool store = present && r < Tp;
-            const bool next = has_next && store && tt >= 0 && tt < T;
-            const int m0 = r + RC_PAD;
-            const int m1 = (tt >= 1 && tt <= P) ? P - tt + RC_PAD : -1;
-            const int m2 = (uu >= 1 && uu <= P) ? P + T - 1 + uu + RC_PAD : -1;
-            const int64_t grow = int64_t(b) * Tp + r;
-            const uint32_t* const xh = reinterpret_cast<const uint32_t*>(cp.x.hi() + grow * cp.x.ld + (j + 2) * cp.width + 2 * (l & 3)) + 4 * qh;
-            uint32_t* const yh = reinterpret_cast<uint32_t*>(cp.y.hi() + grow * cp.y.ld + (j + 1) * cp.width + 2 * (l & 3)) + 4 * qh;
-            // the lo planes, in 32-bit words (encode_planes_map_ex: plane strides are multiples of 8 elements)
-            const int64_t xlo = cp.x.plane_stride / 2, ylo = cp.y.plane_stride / 2;
-            uint32_t nh[2], nl[2];
+        j = rp_opaque(j);  // like b: the y column offset is computed here, not before the epilogue and held through it
+        const int q = l & 3, r0 = wg * 64 + 16 * wq + (l >> 2);  // padded rows r0 and r0 + 8 inside the utterance
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                nh[i] = next ? __ldg(xh + 4 * i) : 0u;
-                nl[i] = (next && NP == 2) ? __ldg(xh + 4 * i + xlo) : 0u;
+        for (int c = 0; c < 2; ++c) {
+            float a[8], bb[8];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                a[2 * i] = acc[16 * c + 4 * i], a[2 * i + 1] = acc[16 * c + 4 * i + 1], bb[2 * i] = acc[16 * c + 4 * i + 2],
+                bb[2 * i + 1] = acc[16 * c + 4 * i + 3];
+            quad_transpose_pairs(a, bb, q);
+            // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
+            const float* const vb = vec + j * 192 + 32 * c + 8 * q;
+#pragma unroll
+            for (int k4 = 0; k4 < 8; k4 += 4) {
+                const float4 b4 = *reinterpret_cast<const float4*>(vb + k4);
+                const float4 s4 = *reinterpret_cast<const float4*>(vb + 64 + k4);
+                const float4 h4 = *reinterpret_cast<const float4*>(vb + 128 + k4);
+                const float bv[4] = {b4.x, b4.y, b4.z, b4.w}, sv[4] = {s4.x, s4.y, s4.z, s4.w}, hv[4] = {h4.x, h4.y, h4.z, h4.w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    acc[16 * c + k4 + k] = fmaf(fmaxf(a[k4 + k] + bv[k], 0.f), sv[k], hv[k]);
+                    acc[16 * c + 8 + k4 + k] = fmaf(fmaxf(bb[k4 + k] + bv[k], 0.f), sv[k], hv[k]);
+                }
             }
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int q = qh + i;
-                // bias -> ReLU -> BatchNorm(eval) affine   (TDNNBlock, utils.py:147)
-                const float2 b2 = *reinterpret_cast<const float2*>(vb + 8 * q);
-                const float2 s2 = *reinterpret_cast<const float2*>(vb + 64 + 8 * q);
-                const float2 h2 = *reinterpret_cast<const float2*>(vb + 128 + 8 * q);
-                float a0 = acc[4 * i], a1 = acc[4 * i + 1];
+            for (int h = 0; h < 2; ++h) {
+                const float* const v = acc + 16 * c + 8 * h;
+                const int r = r0 + 8 * h;
+                const __nv_bfloat16* const yp = cp.y.hi() + (int64_t(b) * Tp + r) * cp.y.ld + (j + 1) * cp.width + 32 * c + 8 * q;
+                uint4 vh, vl;
+                split_pack_bf16x2(v[0], v[1], vh.x, vl.x), split_pack_bf16x2(v[2], v[3], vh.y, vl.y);
+                split_pack_bf16x2(v[4], v[5], vh.z, vl.z), split_pack_bf16x2(v[6], v[7], vh.w, vl.w);
+                rp_st_global_v4(present && r < Tp, yp, vh);
+                if (NP == 2) rp_st_global_v4(present && r < Tp, yp + cp.y.plane_stride, vl);
+            }
+        }
+        RP_STAMP(u, j, 5);
+        if (!(present && has_next)) return;  // uniform across the CTA
+        mbar_wait(x_next(u), xpar);
+        RP_STAMP(u, j, 6);
+        const uint32_t tile = smem_base + u * Cfg::U_BYTES;
+        const int r1 = rp_opaque(r0);  // the row arithmetic below stays after the wait instead of holding registers through pass 1
 #pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    if (part == k) a0 = acc[4 * (2 * (k & 3) + i) + 2 * (k >> 2)], a1 = acc[4 * (2 * (k & 3) + i) + 2 * (k >> 2) + 1];
-                const float x0 = fmaf(fmaxf(a0 + b2.x, 0.f), s2.x, h2.x);
-                const float x1 = fmaf(fmaxf(a1 + b2.y, 0.f), s2.y, h2.y);
-                uint32_t vh, vl;
-                split_pack_bf16x2(x0, x1, vh, vl);
-                rp_st_global(store, yh + 4 * i, vh);
-                if (NP == 2) rp_st_global(store, yh + 4 * i + ylo, vl);
-                const float2 hf = unpack_bf16x2(nh[i]), lf = unpack_bf16x2(nl[i]);
-                uint32_t oh, ol;
-                split_pack_bf16x2(x0 + (hf.x + lf.x), x1 + (hf.y + lf.y), oh, ol);
+        for (int c = 0; c < 2; ++c) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = r1 + 8 * h, tt = r - P, uu = T - 1 - tt;
+                const bool next = tt >= 0 && tt < T;
+                const int m0 = r + RC_PAD;
+                const int m1 = (tt >= 1 && tt <= P) ? P - tt + RC_PAD : -1;
+                const int m2 = (uu >= 1 && uu <= P) ? P + T - 1 + uu + RC_PAD : -1;
+                const int k16 = 4 * c + q;  // SWIZZLE_128B: 16-byte unit k16 of row m sits at m * 128 + ((k16 ^ (m & 7)) << 4)
+                const uint32_t s0 = tile + m0 * 128 + ((k16 ^ (m0 & 7)) << 4);
+                const uint4 xh = rp_ld_shared_v4(s0);
+                const uint4 xl = NP == 2 ? rp_ld_shared_v4(s0 + RP_A_PLANE) : make_uint4(0u, 0u, 0u, 0u);
+                const float* const v = acc + 16 * c + 8 * h;
+                uint4 oh, ol;
+                auto add = [&](uint32_t nh, uint32_t nl, int k, uint32_t& ph, uint32_t& pl) {
+                    const float2 hf = unpack_bf16x2(nh), lf = unpack_bf16x2(nl);
+                    split_pack_bf16x2(v[k] + (hf.x + lf.x), v[k + 1] + (hf.y + lf.y), ph, pl);
+                };
+                add(xh.x, xl.x, 0, oh.x, ol.x), add(xh.y, xl.y, 2, oh.y, ol.y), add(xh.z, xl.z, 4, oh.z, ol.z), add(xh.w, xl.w, 6, oh.w, ol.w);
                 auto put = [&](bool pred, int row) {
-                    const uint32_t d = tile + row * 128 + ((q ^ (row & 7)) << 4) + 4 * (l & 3);
-                    rp_st_shared(pred, d, oh);
-                    if (NP == 2) rp_st_shared(pred, d + RP_A_PLANE, ol);
+                    const uint32_t d = tile + row * 128 + ((k16 ^ (row & 7)) << 4);
+                    rp_st_shared_v4(pred, d, oh);
+                    if (NP == 2) rp_st_shared_v4(pred, d + RP_A_PLANE, ol);
                 };
                 put(next, m0);
                 put(next && m1 >= 0, m1);
@@ -471,15 +521,11 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
     uint32_t g = 0, it = 0;
     for (int pi = blockIdx.x; pi < npairs; pi += gridDim.x, ++it) {
         const int b0 = 2 * pi;  // utterances b0 (A) and b0 + 1 (B, absent when B is odd and this is the last pair)
-        const bool trace_on = cp.trace && blockIdx.x == 0 && it == 0 && tid == 0;
+        trace_on = cp.trace && blockIdx.x == 0 && it == 0 && tid == 0;
         if (tid == 0) {
-            // rows [-4, 332) around each utterance; an absent B loads out-of-range rows, which TMA fills with zeros
+            // chunk 1 of both utterances; an absent B loads out-of-range rows, which TMA fills with zeros
             mbar_arrive_expect_tx(x_full, 2 * NP * RP_A_PLANE);
-            for (int u = 0; u < 2; ++u)
-                for (int pl = 0; pl < NP; ++pl)
-                    for (int h = 0; h < 2; ++h)
-                        tma_load_3d(smem_base + u * Cfg::U_BYTES + pl * RP_A_PLANE + h * RP_BOX_ROWS * 128, &cp.mapX, x_full,
-                                    cp.width /* chunk 1 */, (b0 + u) * Tp - RC_PAD + h * RP_BOX_ROWS, pl);
+            for (int u = 0; u < 2; ++u) load_x(x_full, u, b0 + u, 1);
             RP_STAMP(2, 0, 0);
             load_w(0);
             for (int c = 2; c <= 3 && c <= nconv; ++c) prefetch_chunk(b0, c);
@@ -504,15 +550,17 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
         for (int j = 0; j < nconv; ++j, ++g) {
             mbar_wait(w_full, g & 1u);
             RP_STAMP(2, j, 1);
-            if (tid == 0 && j + 3 <= nconv) prefetch_chunk(b0, j + 3);  // one conv ahead of the epilogue that reads it
+            if (tid == 0 && j + 3 <= nconv) prefetch_chunk(b0, j + 3);  // one conv ahead of the load_x that reads it
             issue(accA, 0);  // MMA_A(j)
             // MMA_A(j) is the only group in flight, so this returns at once.  It tells ptxas so: without it ptxas waits for MMA_A(j)
             // inside epilogue_B(j-1) below, and that epilogue no longer runs under the MMAs.
             wgmma_wait<1>();
             RP_STAMP(0, j, 0);
+            // Each x_{j+2} load completes one phase of x_next(u).  Before conv j's, slot u has had it * (nconv - 1) loads in this
+            // CTA's earlier pairs (an absent B is always its CTA's last pair) and j in this one: g - it.
             if (j > 0) {
                 RP_STAMP(1, j - 1, 2);
-                epilogue(accB, 1, b0 + 1, j - 1);  // under MMA_A(j)
+                epilogue(accB, 1, b0 + 1, j - 1, (g - 1 - it) & 1u);  // under MMA_A(j)
                 RP_STAMP(1, j - 1, 3);
                 fence_proxy_async_smem();
             }
@@ -523,8 +571,13 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
             wgmma_fence_acc(accA);
             __syncthreads();  // every warpgroup's MMA_A(j) has retired: A's tile may be overwritten
             RP_STAMP(0, j, 1);
+            if (tid == 0 && j + 1 < nconv) {
+                mbar_arrive_expect_tx(x_next(0), NP * RP_A_PLANE);
+                load_x(x_next(0), 0, b0, j + 2);
+                RP_STAMP(0, j, 4);
+            }
             RP_STAMP(0, j, 2);
-            epilogue(accA, 0, b0, j);  // under MMA_B(j)
+            epilogue(accA, 0, b0, j, (g - it) & 1u);  // under MMA_B(j)
             RP_STAMP(0, j, 3);
             fence_proxy_async_smem();
             wgmma_wait<0>();
@@ -533,11 +586,16 @@ __global__ void __launch_bounds__(RP_THREADS, 1) res2chain_pair_kernel(const __g
             RP_STAMP(1, j, 1);
             if (tid == 0 && j + 1 < nconv) {
                 RP_STAMP(2, j + 1, 0);
-                load_w(j + 1);
+                load_w(j + 1);  // first: MMA_A(j+1) waits for the weights, only B's pass 2 for x
+                if (b0 + 1 < cp.B) {  // B's tile is dead as well; its epilogue runs under MMA_A(j+1)
+                    mbar_arrive_expect_tx(x_next(1), NP * RP_A_PLANE);
+                    load_x(x_next(1), 1, b0 + 1, j + 2);
+                    RP_STAMP(1, j, 4);
+                }
             }
         }
         RP_STAMP(1, nconv - 1, 2);
-        epilogue(accB, 1, b0 + 1, nconv - 1);
+        epilogue(accB, 1, b0 + 1, nconv - 1, 0u);  // the last conv: nothing to load
         RP_STAMP(1, nconv - 1, 3);
         __syncthreads();  // the next pair's loads overwrite the tiles and the weight slot
     }
@@ -554,7 +612,9 @@ int res2chain_build(Res2ChainParams* cp, const Planes& x, const Planes& y, const
     int rc = encode_planes_map_ex(&cp->mapX, x, 64, paired ? RP_BOX_ROWS : RC_BOX_ROWS, 128);
     if (rc) return rc;
     const int ntiles = (Tp + GEMM_BM - 1) / GEMM_BM;
-    if (!paired) {  // the paired kernel stages nothing: its epilogue reads x and writes y directly
+    if (paired) {  // the paired kernel stages nothing: its epilogue writes y from the registers, 16 bytes per row and plane
+        PPV_REQUIRE(!(reinterpret_cast<uintptr_t>(y.base) & 15) && y.ld % 8 == 0 && y.plane_stride % 8 == 0, "res2chain: y planes not 16-byte aligned");
+    } else {
         rc = encode_planes_map_ex(&cp->mapXt, x, 64, GEMM_BM, 128);
         if (rc) return rc;
         rc = encode_planes_map_ex(&cp->mapY, y, 64, GEMM_BM, 128);
