@@ -354,6 +354,19 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
                          const float* bn_shift, int relu, int tanh_, int Tp, int P, int M, int N, int K, int block_n,
                          int precision, void* out, void* ws, size_t ws_bytes, void* stream);
 
+/* Test hook for the conv2d kernels of ResNetSE, ERes2Net and CAM++ (not a reference entry point): one k x k conv (k 1 or 3, padding
+ * k / 2, stride (stride_h, stride_w)) of x [B,H,W,Cin] (fp32 NHWC) with w [Cout,Cin,k,k] (fp32), + bias (may be NULL), ReLU (relu).
+ * x is written as split planes at columns [x_col0, x_col0 + Cin) of a zero-bordered [B, H+2, W+2, x_ld] grid (x_ld 0: Cin); the
+ * other columns hold a non-zero fill.  path 0: the 3x3 patch kernel (32 -> 32 channels); 1: the pointwise kernel (1x1, Cin 32,
+ * Cout 32 or 64; it computes in fp32 over the exact hi + lo values at either precision); 2: the gather-GEMM in image mode (k x k
+ * row-offset taps).  A conv the chosen kernel does not take is an error.  out: split-bf16 planes [2][B][Ho+2][Wo+2][Cout] with
+ * Ho = (H-1)/stride_h + 1, Wo = (W-1)/stride_w + 1, 16-byte aligned; it is zeroed, then the kernel writes the interior positions.
+ * ws >= ppv_conv2d_test_workspace_bytes.  Synchronises `stream` while it prepares the weights. */
+size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k, int x_ld);
+int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
+                    int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
+                    size_t ws_bytes, void* stream);
+
 /* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N)
  * bytes + 4*(3 + M/306)*N rounded up to 256.  planes_out: 0 ReLU to fp32, 1 ReLU to planes, 2 bias + ReLU + BN to planes over the
  * padded time layout (Tp = 306, P = 4), 3 the same + per-utterance bias + tanh (ASP attention TDNN); 2 and 3 need M % 306 == 0. */

@@ -76,17 +76,14 @@ def test_batch_independence(cuda, model):
         assert torch.equal(model(f[b:b + 1]), emb[b:b + 1])
 
 
-def test_pointwise_kernel_equals_gather_gemm(cuda, W64, monkeypatch):
-    """The K <= 64 1x1 convs run on pointwise.cu (CUDA cores, exact hi + lo inputs); PPV_POINTWISE=0 keeps them on the wgmma gather-GEMM.
-    Both must agree to the split-bf16 product rounding (~2^-17 per product), far inside the embedding tolerance."""
-    gi = torch.Generator().manual_seed(77)
-    f = torch.randn(3, 149, 80, generator=gi).to(cuda)
-    sd = {k: v.float() for k, v in W64.items()}
-    embs = []
-    for flag in ("1", "0"):
-        monkeypatch.setenv("PPV_POINTWISE", flag)
-        m = ResNetSE(input_size=80).eval()
-        m.load_state_dict(sd, strict=True)
-        embs.append(m.to(cuda)(f).double().cpu())
-    rel = (embs[0] - embs[1]).norm(dim=1) / embs[1].norm(dim=1)
-    assert rel.max() < 2e-5, rel
+def test_plans_no_pointwise_step(cuda, model):
+    """ResNetSE runs every 1x1 conv on the wgmma gather-GEMM: its plan has no pointwise step (pointwise.cu), so PPV_POINTWISE does not
+    apply to it.  The profiler's kernel names show which kernels a forward ran."""
+    from torch.profiler import ProfilerActivity, profile
+    f = torch.randn(3, 149, 80, generator=torch.Generator().manual_seed(77)).to(cuda)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        model(f)
+        torch.cuda.synchronize()
+    names = {e.key for e in prof.key_averages()}
+    assert any("gemm_wgmma_kernel" in n for n in names) and any("conv3x3_c32_kernel" in n for n in names), names
+    assert not any("pw_conv_kernel" in n for n in names), names

@@ -504,6 +504,116 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- conv2d test hook
+// One conv2d of the 2-D models (ResNetSE, ERes2Net, CAM++), planned as their plans plan it: the input grid, the weight planes and the
+// image-mode epilogue are laid out as in resnet_se.cu / eres2net.cu / campplus.cu, and exactly the kernel `path` names runs, or an
+// error is returned.  Workspace: the input grid [2][pad128(B (H+2) (W+2))][x_ld], then the weight planes [2][pad256(Cout)][k k Cin].
+static size_t conv2d_test_x_bytes(int B, int H, int W, int x_ld) {
+    return au(au(size_t(B) * (H + 2) * (W + 2), 128) * size_t(x_ld) * 4, 256);
+}
+size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k, int x_ld) {
+    if (x_ld <= 0) x_ld = Cin;
+    return conv2d_test_x_bytes(B, H, W, x_ld) + au(au(size_t(Cout), 256) * k * k * Cin * 4, 256) + 256;
+}
+int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
+                    int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws, size_t ws_bytes,
+                    void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && w && out && ws, "ppv_conv2d_test: null argument");
+    if (x_ld <= 0) x_ld = Cin;
+    PPV_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && (k == 1 || k == 3) && stride_h >= 1 && stride_w >= 1,
+                "ppv_conv2d_test: bad shape");
+    PPV_REQUIRE(x_col0 >= 0 && x_col0 + Cin <= x_ld, "ppv_conv2d_test: the input columns exceed x_ld");
+    PPV_REQUIRE(path >= 0 && path <= 2, "ppv_conv2d_test: path must be 0 (3x3 patch kernel), 1 (pointwise kernel) or 2 (gather-GEMM)");
+    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "ppv_conv2d_test: bad precision");
+    PPV_REQUIRE(ws_bytes >= ppv_conv2d_test_workspace_bytes(B, H, W, Cin, Cout, k, x_ld), "ppv_conv2d_test: workspace too small");
+    const int Hp = H + 2, Wp = W + 2, Ho = (H - 1) / stride_h + 1, Wo = (W - 1) / stride_w + 1;
+    const int64_t M = int64_t(B) * Hp * Wp;
+    PPV_REQUIRE(M < (int64_t(1) << 31) && Wp + 1 < 32768, "ppv_conv2d_test: grid too large for 32-bit rows / 16-bit tap offsets");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // input grid: zero border; x at columns [x_col0, x_col0 + Cin) of the interior; the other columns hold 0x3f3f (0.746 in bf16) in
+    // both planes, so a kernel that reads outside its column window is visibly wrong
+    Planes xp;
+    xp.rows = int64_t(au(size_t(M), 128));
+    xp.ld = x_ld;
+    xp.plane_stride = xp.rows * x_ld;
+    xp.base = static_cast<__nv_bfloat16*>(ws);
+    const size_t x_bytes = conv2d_test_x_bytes(B, H, W, x_ld);
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, x_bytes, st));
+    const size_t pitch = size_t(x_ld) * sizeof(__nv_bfloat16), rows2 = size_t(2 * xp.rows);
+    if (x_col0 > 0) PPV_CUDA_OK(cudaMemset2DAsync(xp.base, pitch, 0x3f, size_t(x_col0) * sizeof(__nv_bfloat16), rows2, st));
+    if (x_col0 + Cin < x_ld)
+        PPV_CUDA_OK(cudaMemset2DAsync(xp.base + x_col0 + Cin, pitch, 0x3f, size_t(x_ld - x_col0 - Cin) * sizeof(__nv_bfloat16), rows2, st));
+    for (int b = 0; b < B; ++b)
+        for (int h = 0; h < H; ++h) {  // one image row: W consecutive grid positions
+            Planes row = xp;
+            row.base = xp.base + ((int64_t(b) * Hp + h + 1) * Wp + 1) * x_ld + x_col0;
+            rc = launch_f32_to_planes(x + (int64_t(b) * H + h) * W * Cin, W, Cin, row, st);
+            if (rc) return rc;
+        }
+    // weights [Cout][Cin][k][k] -> [Cout][tap][Cin] with tap = kh k + kw (the order of the plans' nine row-offset sources), split
+    // into planes on the host as the models prepare theirs
+    const int K = k * k * Cin;
+    std::vector<float> wh(size_t(Cout) * K);
+    PPV_CUDA_OK(cudaMemcpyAsync(wh.data(), w, wh.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    PPV_CUDA_OK(cudaStreamSynchronize(st));
+    std::vector<double> wm(wh.size());
+    for (int n = 0; n < Cout; ++n)
+        for (int c = 0; c < Cin; ++c)
+            for (int t = 0; t < k * k; ++t) wm[(size_t(n) * k * k + t) * Cin + c] = wh[(size_t(n) * Cin + c) * k * k + t];
+    ArenaBuilder ab;
+    GemmWeights gw;
+    ab.put_matrix(&gw, wm, Cout, K);
+    uint8_t* wdev = static_cast<uint8_t*>(ws) + x_bytes;
+    PPV_CUDA_OK(cudaMemcpyAsync(wdev, ab.host.data(), ab.host.size(), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaStreamSynchronize(st));
+    gw.W.base = reinterpret_cast<__nv_bfloat16*>(wdev + ab.patches[0].off);
+    // output grid, zeroed as a plan zeroes its workspace: the kernels store interior positions on the stride grid only
+    const int64_t out_plane = int64_t(B) * (Ho + 2) * (Wo + 2) * Cout;
+    PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2 * out_plane) * sizeof(__nv_bfloat16), st));
+    Epilogue ep;
+    ep.bias = bias;
+    ep.relu = relu ? 1 : 0;
+    ep.out_mode = OUT_PLANES;
+    ep.out = out;
+    ep.out_ld = Cout;
+    ep.out_plane_stride = out_plane;
+    ep.img_Hp = Hp;
+    ep.img_Wp = Wp;
+    ep.img_H = H;
+    ep.img_W = W;
+    ep.img_stride = stride_h;
+    ep.img_stride_w = stride_w == stride_h ? 0 : stride_w;  // 0 as ResNetSE / ERes2Net set it; CAM++'s FCM sets 1 with stride_h 2
+    ep.out_Hp = Ho + 2;
+    ep.out_Wp = Wo + 2;
+    const int sms = device_sm_count();
+    if (path == 0) {
+        PPV_REQUIRE(k == 3 && conv3x3_c32_supported(Cin, Cout, H, W), "ppv_conv2d_test: the patch kernel takes 3x3 convs with 32 -> 32 channels only");
+        Conv3x3Params cp;
+        rc = conv3x3_build(&cp, xp, x_col0, gw.W, B, H, W, Hp, Wp, ep);
+        if (rc) return rc;
+        return conv3x3_launch(cp, precision, sms, st);
+    }
+    if (path == 1) {  // fp32 FMAs over the exact hi + lo values whatever the precision
+        PPV_REQUIRE(k == 1, "ppv_conv2d_test: the pointwise kernel takes 1x1 convs only");
+        const GemmSource src{xp, x_col0, Cin, 0};
+        PwStep s;
+        if (!pointwise_step_build(&s, &src, 1, gw.W, Cout, M, ep))
+            return fail(PPV_EINVAL, "ppv_conv2d_test: the pointwise kernel does not take this conv (or PPV_POINTWISE=0)");
+        return pointwise_launch(s, sms, st);
+    }
+    std::vector<GemmSource> srcs;
+    for (int dh = -(k / 2); dh <= k / 2; ++dh)
+        for (int dw = -(k / 2); dw <= k / 2; ++dw) srcs.push_back(GemmSource{xp, x_col0, Cin, dh * Wp + dw});
+    GemmParams gp;
+    rc = gemm_build(&gp, srcs.data(), int(srcs.size()), gw.W, int(M), Cout, ep, gemm_pick_bn(Cout));
+    if (rc) return rc;
+    return gemm_launch(gp, precision, sms, st);
+    PPV_GUARD_END
+}
+
 // Kernel-only timing of the gather-GEMM (tools/gemm_bench.py): operands are converted once, the kernel is launched
 // `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  planes_out selects the epilogue:
 //   0  ReLU, fp32 [M,N];   1  ReLU, split-bf16 planes (the layout every model layer writes);

@@ -1,6 +1,6 @@
 // 1x1 convolutions with K = 32 input channels (one 32-channel source) and N <= 64 output channels over image grids or plain row ranges:
-// ResNetSE's first-stage conv1 / conv3 / downsample where the input is the 32-channel stem (ppvector/models/resnet_se.py:24-45),
 // ERes2Net's layer-1 conv1 / shortcut (ppvector/models/eres2net.py:85-108) and CAM++'s FCM shortcuts (ppvector/models/campplus.py:232-238).
+// ResNetSE plans no pointwise step: its 1x1 convs run on the gather-GEMM.
 //
 // On the tensor-core gather-GEMM these layers run one 128-row tile per pipeline step with a single 32-wide k-step: 49 200 tiles of 16 KB at
 // the 80 x 298 resolution, paced by the per-tile epilogue chain rather than by HBM.  Here one thread owns one grid position, keeps its

@@ -138,6 +138,8 @@ SIGNATURES = {
                                 C.c_size_t, _P]),
     "ppv_gemm_test_planes": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
+    "ppv_conv2d_test_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
+    "ppv_conv2d_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 13 + [_P, _P, C.c_size_t, _P]),
 }
 
 _lib = None
