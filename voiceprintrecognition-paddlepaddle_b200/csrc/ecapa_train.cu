@@ -105,6 +105,7 @@ struct Trainer {
           *cls_logits = nullptr, *loss = nullptr, *aspbn_mean = nullptr, *aspbn_rstd = nullptr;
     float *d_emb = nullptr, *dpn = nullptr, *dpooled = nullptr, *dgs = nullptr, *rs = nullptr, *rb = nullptr, *dg2 = nullptr, *dg1 = nullptr, *ds = nullptr,
           *part = nullptr, *wpart = nullptr;
+    size_t part_elems = 0;
     void* aam_ws = nullptr;
     size_t aam_ws_bytes = 0;
 };
@@ -248,6 +249,13 @@ struct TrCarve {
     float* f32(size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); }
 };
 
+// Frame splits of a layer's BatchNorm backward: narrow layers split the frames of an utterance over several CTAs so the
+// reduction fills the GPU.  The attention TDNN keeps per-utterance sums, which ASP_CTX_BWD reads back from `part`.
+int tr_bn_bwd_tsplit(const Trainer* t, int layer, int B) {
+    const int ctas = (t->L[layer].bn.C / 64) * B;
+    return (layer == t->l_att1 || ctas >= 2 * t->num_sms) ? 1 : std::min(8, std::max(1, (2 * t->num_sms + ctas - 1) / ctas));
+}
+
 void tr_carve(Trainer* t, TrCarve& k, int B, int T) {
     const int Tp = T + 2 * t->P;
     const int64_t R = int64_t(B) * Tp, Rp = int64_t(mc_align_up(size_t(R), 128));
@@ -328,7 +336,11 @@ void tr_carve(Trainer* t, TrCarve& k, int B, int T) {
     t->dg2 = k.f32(size_t(B) * C);
     t->dg1 = k.f32(size_t(B) * t->se);
     t->ds = k.f32(size_t(B) * C);
-    t->part = k.f32(size_t(3) * B * C3);
+    // partial sums: BatchNorm forward statistics [B][3][C], per-utterance column sums [B][C], BatchNorm backward [B * tsplit][2][C]
+    t->part_elems = size_t(3) * B * C3;
+    for (int l = 0; l < int(t->L.size()); ++l)
+        t->part_elems = std::max(t->part_elems, size_t(2) * B * tr_bn_bwd_tsplit(t, l, B) * t->L[l].bn.C);
+    t->part = k.f32(t->part_elems);
     // weight-gradient partials: max over layers of splits * Mpad * Ktot; splits <= num_sms
     size_t wmax = 0;
     auto wsize = [&](const TConv& c) {
@@ -484,6 +496,7 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         s.c0 = a_col0;
         s.p1 = dz;
         s.c1 = dz_col0;
+        s.a = tr_bn_bwd_tsplit(t, layer, B);
         push(s);
     };
     auto simple = [&](TStep::Kind kd, int a = 0) {
@@ -790,11 +803,8 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
             case TStep::GRAD_SUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, s.p0, s.c0, t->part, nullptr, st); break;
             case TStep::BN_BWD: {
                 const TLayer& l = t->L[s.layer];
-                // narrow layers: split the frames of an utterance over several CTAs (the attention TDNN keeps per-utterance sums)
-                const int ctas = (l.bn.C / 64) * B;
-                const int tsplit = (s.layer == t->l_att1 || ctas >= 2 * t->num_sms) ? 1 : std::min(8, std::max(1, (2 * t->num_sms + ctas - 1) / ctas));
                 rc = tr_bn_backward(s.gl, s.p0, s.c0, l.bn.C, B, T, P, Tp, l.bn.mean, l.bn.rstd, par + l.bn.g_off, grd + l.bn.g_off, grd + l.bn.b_off,
-                                    s.p1, s.c1, grd + l.conv.b_off, t->part, st, tsplit);
+                                    s.p1, s.c1, grd + l.conv.b_off, t->part, t->part_elems, st, s.a);
                 break;
             }
             case TStep::ASP_CTX_BWD: {
@@ -848,53 +858,113 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
     return PPV_OK;
 }
 
-// forward taps for tests: "blocks.0".."blocks.3", "mfa" -> fp32 [B,T,C]; "asp" -> pooled [B, 2*C3]; "emb" -> [B, D]
+// Taps for tests and debugging: every buffer of the step stays readable after it (tr_carve aliases none).
+//   planes -> fp32 [B, T, C], valid frames; with the prefix "pad:" all Tp = T + 2P rows of every utterance, halo rows included
+//     forward   "blocks.0".."blocks.3", "mfa" (block outputs); X0, A0, Y0, OUTCAT, Amfa, M, Aatt, A4; per block ("<name>:<0..2>")
+//               At1, Yt1, Ares, RC, IN, At2, Yt2.  A* are the post-ReLU, pre-BatchNorm activations the BatchNorm backward reads.
+//     gradients "g:<name>": dZ0, dOUTCAT, dMd, dMatt, dZmfa, dlogits, dZatt, dA4; per block D, dZt2, dRC, dZres, DIN, dZt1, dXt1
+//   fp32 as stored: "asp" (pooled) [B, 2*C3], "emb" and "d_emb" [B, D], "logits" [B, Tp, C3] (every row), gstat, dgs, pn, dpn, dpooled
+//     [B, 2*C3], rs, rb [B, C3]; per block se_s, se_g2 [B, C], se_g1 [B, se]; dg2, ds [B, C] and dg1 [B, se] are scratch that every
+//     block's SE backward overwrites, so they hold block 0's values.
+// A per-block name without a block suffix reads block 0.
 int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems, cudaStream_t st) {
     PPV_REQUIRE(t && name && out, "trainer_read_tap: null argument");
     if (!t->plan_ws) return fail(PPV_ESTATE, "trainer_read_tap: no step has run");
-    const std::string n(name);
-    const int B = t->plan_B, T = t->plan_T;
-    if (n == "asp" || n == "emb") {
-        const size_t cnt = size_t(B) * (n == "asp" ? 2 * t->C3 : t->D);
+    std::string n(name);
+    const bool padded = n.rfind("pad:", 0) == 0;
+    if (padded) n = n.substr(4);
+    const int B = t->plan_B, T = t->plan_T, C = t->C, C3 = t->C3;
+    int b = -1;  // block suffix
+    const size_t colon = n.rfind(':');
+    if (colon != std::string::npos && colon + 2 == n.size() && n.back() >= '0' && n.back() <= '9') {
+        b = n.back() - '0';
+        n.resize(colon);
+        PPV_REQUIRE(b < 3, "trainer_read_tap: bad block");
+    }
+    const bool per_block = b >= 0;
+    const int bk = per_block ? b : 0;
+    auto unknown = [&]() { return fail(PPV_EINVAL, std::string("trainer_read_tap: unknown tap ") + name); };
+
+    const float* vec = nullptr;
+    size_t cnt = 0;
+    bool vec_block = false;
+    if (n == "asp") vec = t->pooled, cnt = size_t(B) * 2 * C3;
+    else if (n == "emb") vec = t->emb, cnt = size_t(B) * t->D;
+    else if (n == "d_emb") vec = t->d_emb, cnt = size_t(B) * t->D;
+    else if (n == "logits") vec = t->logits, cnt = size_t(t->R) * C3;
+    else if (n == "gstat") vec = t->gstat, cnt = size_t(B) * 2 * C3;
+    else if (n == "dgs") vec = t->dgs, cnt = size_t(B) * 2 * C3;
+    else if (n == "pn") vec = t->pn, cnt = size_t(B) * 2 * C3;
+    else if (n == "dpn") vec = t->dpn, cnt = size_t(B) * 2 * C3;
+    else if (n == "dpooled") vec = t->dpooled, cnt = size_t(B) * 2 * C3;
+    else if (n == "rs") vec = t->rs, cnt = size_t(B) * C3;
+    else if (n == "rb") vec = t->rb, cnt = size_t(B) * C3;
+    else if (n == "dg2") vec = t->dg2, cnt = size_t(B) * C;
+    else if (n == "dg1") vec = t->dg1, cnt = size_t(B) * t->se;
+    else if (n == "ds") vec = t->ds, cnt = size_t(B) * C;
+    else if (n == "se_s") vec = t->se_s[bk], cnt = size_t(B) * C, vec_block = true;
+    else if (n == "se_g1") vec = t->se_g1[bk], cnt = size_t(B) * t->se, vec_block = true;
+    else if (n == "se_g2") vec = t->se_g2[bk], cnt = size_t(B) * C, vec_block = true;
+    if (vec) {
+        if (padded || (per_block && !vec_block)) return unknown();
         PPV_REQUIRE(out_elems >= cnt, "trainer_read_tap: output too small");
-        PPV_CUDA_OK(cudaMemcpyAsync(out, n == "asp" ? t->pooled : t->emb, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        PPV_CUDA_OK(cudaMemcpyAsync(out, vec, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return PPV_OK;
     }
+
     Planes src;
-    int col0 = 0, C = t->C;
-    if (n.rfind("g:", 0) == 0) {  // gradient buffers (debug / tests): "g:<name>" or "g:<name>:<block 0..2>", all rows valid frames only
-        const std::string nm = n.substr(2, n.find(':', 2) == std::string::npos ? std::string::npos : n.find(':', 2) - 2);
-        const int b = n.find(':', 2) == std::string::npos ? 0 : (n.back() - '0');
-        PPV_REQUIRE(b >= 0 && b < 3, "trainer_read_tap: bad block");
-        if (nm == "D") src = t->Dbuf[b];
-        else if (nm == "dZt2") src = t->dZt2[b];
-        else if (nm == "dRC") src = t->dRC[b];
-        else if (nm == "DIN") src = t->DIN[b];
-        else if (nm == "dZt1") src = t->dZt1[b];
-        else if (nm == "dXt1") src = t->dXt1[b];
-        else if (nm == "dZ0") src = t->dZ0;
-        else if (nm == "dOUTCAT") { src = t->dOUTCAT; C = t->C3; }
-        else if (nm == "dMd") { src = t->dMd; C = t->C3; }
-        else if (nm == "dMatt") { src = t->dMatt; C = t->C3; }
-        else if (nm == "dZmfa") { src = t->dZmfa; C = t->C3; }
-        else if (nm == "dlogits") { src = t->dlogits; C = t->C3; }
-        else return fail(PPV_EINVAL, "trainer_read_tap: unknown gradient tap " + n);
-        PPV_REQUIRE(out_elems >= size_t(B) * T * C, "trainer_read_tap: output too small");
-        return launch_planes_to_f32(src, 0, C, B, T, t->P, t->Tp, out, st);
-    }
-    if (n == "blocks.0") {
+    int col0 = 0, cols = C;
+    bool blocked = false;
+    if (n.rfind("g:", 0) == 0) {
+        const std::string g = n.substr(2);
+        if (g == "D") src = t->Dbuf[bk], blocked = true;
+        else if (g == "dZt2") src = t->dZt2[bk], blocked = true;
+        else if (g == "dRC") src = t->dRC[bk], blocked = true;
+        else if (g == "dZres") src = t->dZres[bk], blocked = true;
+        else if (g == "DIN") src = t->DIN[bk], blocked = true;
+        else if (g == "dZt1") src = t->dZt1[bk], blocked = true;
+        else if (g == "dXt1") src = t->dXt1[bk], blocked = true;
+        else if (g == "dZ0") src = t->dZ0;
+        else if (g == "dOUTCAT") src = t->dOUTCAT, cols = C3;
+        else if (g == "dMd") src = t->dMd, cols = C3;
+        else if (g == "dMatt") src = t->dMatt, cols = C3;
+        else if (g == "dZmfa") src = t->dZmfa, cols = C3;
+        else if (g == "dlogits") src = t->dlogits, cols = C3;
+        else if (g == "dZatt") src = t->dZatt, cols = t->att;
+        else if (g == "dA4") src = t->dA4, cols = t->att;
+        else return unknown();
+    } else if (n == "blocks.0" || n == "Y0") {
         src = t->Y0;
     } else if (n == "blocks.1" || n == "blocks.2" || n == "blocks.3") {
         src = t->OUTCAT;
-        col0 = t->C * (n[7] - '1');
-    } else if (n == "mfa") {
-        src = t->M;
-        C = t->C3;
+        col0 = C * (n[7] - '1');
+    } else if (n == "mfa" || n == "M") {
+        src = t->M, cols = C3;
+    } else if (n == "X0") {
+        src = t->X0, cols = t->cfg.input_size;
+    } else if (n == "A0") {
+        src = t->A0;
+    } else if (n == "OUTCAT") {
+        src = t->OUTCAT, cols = C3;
+    } else if (n == "Amfa") {
+        src = t->Amfa, cols = C3;
+    } else if (n == "Aatt" || n == "A4") {
+        src = n == "A4" ? t->A4 : t->Aatt, cols = t->att;
     } else {
-        return fail(PPV_EINVAL, "trainer_read_tap: unknown tap " + n);
+        blocked = true;
+        if (n == "At1") src = t->At1[bk];
+        else if (n == "Yt1") src = t->Yt1[bk];
+        else if (n == "Ares") src = t->Ares[bk];
+        else if (n == "RC") src = t->RC[bk];
+        else if (n == "IN") src = t->IN[bk];
+        else if (n == "At2") src = t->At2[bk];
+        else if (n == "Yt2") src = t->Yt2[bk];
+        else return unknown();
     }
-    PPV_REQUIRE(out_elems >= size_t(B) * T * C, "trainer_read_tap: output too small");
-    return launch_planes_to_f32(src, col0, C, B, T, t->P, t->Tp, out, st);
+    if (per_block && !blocked) return unknown();
+    const int rows = padded ? t->Tp : T;
+    PPV_REQUIRE(out_elems >= size_t(B) * rows * cols, "trainer_read_tap: output too small");
+    return launch_planes_to_f32(src, col0, cols, B, rows, padded ? 0 : t->P, t->Tp, out, st);
 }
 
 }  // namespace ppv

@@ -37,10 +37,11 @@ struct BnApplyArgs {
 int tr_bn_forward(const Planes& a, int a_col0, int C, int B, int T, int P, int Tp, float eps, float momentum, const float* gamma, const float* beta,
                   float* mean, float* rstd, float* scale, float* shift, float* run_mean, float* run_var, float* part, const BnApplyArgs& apply_in,
                   int num_sms, cudaStream_t st);
-// dz (valid frames) = d(conv output) through BatchNorm(train) and ReLU; dgamma / dbeta / dbias are [C] outputs
+// dz (valid frames) = d(conv output) through BatchNorm(train) and ReLU; dgamma / dbeta / dbias are [C] outputs.
+// `part` holds part_elems floats; the launch needs 2 * B * tsplit * C of them and is refused if they do not fit.
 int tr_bn_backward(const GradSrcList& gl, const Planes& a, int a_col0, int C, int B, int T, int P, int Tp, const float* mean, const float* rstd,
-                   const float* gamma, float* dgamma, float* dbeta, const Planes& dz, int dz_col0, float* dbias, float* part, cudaStream_t st,
-                   int tsplit = 1);  // tsplit > 1: `part` holds B * tsplit partial rows (no per-utterance sums)
+                   const float* gamma, float* dgamma, float* dbeta, const Planes& dz, int dz_col0, float* dbias, float* part, size_t part_elems,
+                   cudaStream_t st, int tsplit = 1);  // tsplit > 1: `part` holds B * tsplit partial rows (no per-utterance sums)
 // out (optional planes, valid frames) = summed sources; part [B][C] = per-utterance column sums; colsum (optional) [C]
 int tr_grad_sum(const GradSrcList& gl, int C, int B, int T, int P, int Tp, const Planes& out, int out_col0, float* part, float* colsum, cudaStream_t st);
 // out_bc [B][C] = sum_t grad(b,t,c) * y[b,t,c]

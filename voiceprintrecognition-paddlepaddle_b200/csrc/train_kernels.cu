@@ -593,6 +593,9 @@ __global__ void __launch_bounds__(256)
 }
 // global context statistics backward as a row scale / row bias on x (gstat = [mean | std] with std = sqrt(clamp(var_biased, eps))):
 //   dx_t += dmean / T + dstd (x_t - mean) / (T std)  =  rs * x_t + rb
+// No gradient passes through a clamped std.  gstat went through split-bf16 planes (2^-17 relative), so a std clamped to
+// sqrt(eps) can read back a few ulps above it; the clamp test allows that rounding.  Otherwise a channel that is constant over an
+// utterance (all frames ReLU-dead) gets rs ~ dstd / (T sqrt(eps)), and rs * x_t + rb cancels to fp32 noise of that size.
 __global__ void asp_global_bwd_kernel(const float* __restrict__ gstat, const float* __restrict__ dgstat, int B, int C, int T, float eps,
                                       float* __restrict__ rs, float* __restrict__ rb) {
     const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -600,7 +603,7 @@ __global__ void asp_global_bwd_kernel(const float* __restrict__ gstat, const flo
     const int b = int(i / C), c = int(i % C);
     const float mean = gstat[int64_t(b) * 2 * C + c], sd = gstat[int64_t(b) * 2 * C + C + c];
     const float dmean = dgstat[int64_t(b) * 2 * C + c], dstd = dgstat[int64_t(b) * 2 * C + C + c];
-    const float s = (sd * sd > eps) ? dstd / (float(T) * sd) : 0.f;
+    const float s = (sd * sd > eps * (1.f + 0x1p-14f)) ? dstd / (float(T) * sd) : 0.f;
     rs[i] = s;
     rb[i] = dmean / float(T) - s * mean;
 }
@@ -649,9 +652,10 @@ int tr_bn_forward(const Planes& a, int a_col0, int C, int B, int T, int P, int T
 }
 
 int tr_bn_backward(const GradSrcList& gl, const Planes& a, int a_col0, int C, int B, int T, int P, int Tp, const float* mean, const float* rstd,
-                   const float* gamma, float* dgamma, float* dbeta, const Planes& dz, int dz_col0, float* dbias, float* part, cudaStream_t st,
-                   int tsplit) {
+                   const float* gamma, float* dgamma, float* dbeta, const Planes& dz, int dz_col0, float* dbias, float* part, size_t part_elems,
+                   cudaStream_t st, int tsplit) {
     PPV_REQUIRE(C % 64 == 0 && tsplit >= 1 && tsplit <= 8, "bn_backward: C % 64 == 0 and 1 <= tsplit <= 8 required");
+    PPV_REQUIRE(size_t(2) * B * tsplit * C <= part_elems, "bn_backward: partial-sum scratch too small for B * tsplit * C");
     bn_bwd_reduce_kernel<<<dim3(C / 64, B, tsplit), TR_WARPS * 32, 0, st>>>(gl, a, a_col0, C, T, P, Tp, mean, rstd, part);
     TR_LAUNCH_OK("bn_bwd_reduce_kernel");
     part_finalize_kernel<<<(C + 7) / 8, 256, 0, st>>>(part, B * tsplit, C, 2, dbeta, dgamma);
