@@ -5,7 +5,7 @@
 // (growth 32, bn_size 4, init_channels 128, blocks 12/24/16 with dilations 1/2/2, 100-frame average segment pooling).
 //
 // Layouts:
-//   * FCM head: zero-bordered NHWC images (H = frequency, W = time) as in resnet_se.cu; its convs stride the frequency
+//   * FCM head: zero-bordered NHWC images (H = frequency, W = time), planned as in image_plan.h; its convs stride the frequency
 //     axis only, so a strided conv is computed on the input grid and stored on the (H/2, W) output grid;
 //   * the head output [B, 32, F/8, T] is flattened to a time-major matrix that holds frame PAIRS: row (b, t') has the
 //     320 channels of frame 2t' followed by those of frame 2t'+1.  The stride-2, kernel-5 TDNN conv is then five
@@ -20,9 +20,8 @@
 //   linear_local * mask     3-tap gather-GEMM whose epilogue multiplies by the mask of (utterance, segment)
 #include <math.h>
 
-#include <stdlib.h>
-
 #include "common.h"
+#include "image_plan.h"
 #include "model_common.h"
 #include "ptx.cuh"
 
@@ -55,17 +54,11 @@ struct TransitW {
     int C = 0;
 };
 
-struct CStep {
-    enum Kind { STEM, GEMM, CONV3, PW, ADD_RELU, FLATTEN, BN_RELU, CONTEXT, STATS } kind;
-    PwStep pw;  // PW: 1x1 conv with K <= 64 on the CUDA cores (pointwise.cu)
-    GemmParams gp;
-    Conv3x3Params c3;  // CONV3: the 32 -> 32 channel 3x3 convs of the FCM head (conv3x3.cu)
-    Planes a, b, d;
-    const float *p0 = nullptr, *p1 = nullptr, *p2 = nullptr, *p3 = nullptr, *p4 = nullptr, *p5 = nullptr;
-    float* fout = nullptr;
-    int C = 0, img_rows = 0;
-    int64_t rows = 0;
-};
+// CAM++'s own plan steps (PlanStep::MODEL):
+//   FLATTEN_PAIRS  x on grid g -> frame-pair matrix `out` (C channels, Tp / P time layout)
+//   BN_RELU        out = relu(x * vec[0] + vec[1]) over C columns of `rows` rows
+//   CONTEXT        x [B * Tp, 128] -> context mask out_f32 [B * n, 32] (MLP vec[0..3]), T frames from row P of each utterance
+enum CpKind { CP_FLATTEN_PAIRS, CP_BN_RELU, CP_CONTEXT };
 
 // ------------------------------------------------------------------------------------------------ kernels
 // out[r, c] = relu(x[r, c] * scale[c] + shift[c]) for c < C (C % 8 == 0), every row
@@ -199,7 +192,7 @@ __global__ void __launch_bounds__(256) cp_flatten_pairs_kernel(Planes in, int B,
 
 }  // namespace
 
-struct CamppModel : Model {
+struct CamppModel : ImagePlanModel {
     ppv_campplus_cfg cfg;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<ResBlockW> res;
@@ -208,22 +201,21 @@ struct CamppModel : Model {
     TransitW transit[CP_NB];
     int block_in[CP_NB], block_out[CP_NB];  // channels entering / leaving each dense block
     int head_ch = 0, final_ch = 0;
-    // plan
-    std::vector<CStep> steps;
-    int T2 = 0, Tp = 0, nseg = 0;
+    // plan (what the taps read)
+    int T2 = 0, Tp = 0;
     ImageGeo geo[4];
-    Planes stem_out, flat, tdnn_view, stats, final_x;
+    Planes stats, final_x;
     Planes stage_out[4];
     Planes xblk[CP_NB], tr_out[CP_NB];
 
-    explicit CamppModel(const ppv_campplus_cfg& c) : Model("campplus", c.precision), cfg(c) {}
+    explicit CamppModel(const ppv_campplus_cfg& c) : ImagePlanModel("campplus", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
     size_t workspace_bytes(int B, int T) const override;
 
   protected:
     bool prepare_weights(ArenaBuilder& ab) override;
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
-    int run_steps(const float* feat, cudaStream_t st) override;
+    int run_model_step(const PlanStep& s, cudaStream_t st) override;
     int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
@@ -252,80 +244,9 @@ int campplus_create(const ppv_campplus_cfg* cfg, Model** out) {
 bool CamppModel::prepare_weights(ArenaBuilder& ab) {
     CamppModel* const m = this;
     const ppv_campplus_cfg& cf = m->cfg;
-    bool ok = true;
     const int G = cf.growth_rate, BC = cf.bn_size * cf.growth_rate;  // 32, 128
 
-    // conv2d [N, Cin, k, k] + BN folded -> dense [N][k*k*Cin] (tap-major, taps in (dh, dw) order)
-    auto conv2d_matrix = [&](GemmWeights* gw, const std::string& conv, const std::string& bn, int N, int Cin, int k) {
-        const HostWeight* w = ab.get(conv + ".weight", {N, Cin, k, k});
-        const HostWeight* b = ab.get(conv + ".bias", {N});
-        std::vector<double> sc, sh;
-        if (!w || !b || !ab.bn_affine(bn, N, &sc, &sh)) {
-            ok = false;
-            return;
-        }
-        const int taps = k * k, K = taps * Cin;
-        std::vector<double> mtx(size_t(N) * K);
-        std::vector<float> bias(std::max(N, 64), 0.f);
-        for (int n = 0; n < N; ++n) {
-            for (int t = 0; t < taps; ++t)
-                for (int c = 0; c < Cin; ++c) mtx[size_t(n) * K + t * Cin + c] = double(w->v[(size_t(n) * Cin + c) * taps + t]) * sc[n];
-            bias[n] = float(double(b->v[n]) * sc[n] + sh[n]);
-        }
-        ab.put_matrix(gw, mtx, N, K);
-        ab.put_f32(&gw->bias, bias);
-    };
-    // conv1d [N, Cin, k] (+ optional BN folded) -> dense [N][k*Kp]; input channels beyond Cin (up to Kp) get zero weights
-    auto conv1d_matrix = [&](GemmWeights* gw, const std::string& conv, const std::string& bn, int N, int Cin, int k, int Kp) {
-        const HostWeight* w = ab.get(conv + ".weight", {N, Cin, k});
-        const HostWeight* b = ab.get(conv + ".bias", {N});
-        std::vector<double> sc(N, 1.0), sh(N, 0.0);
-        if (!w || !b || (!bn.empty() && !ab.bn_affine(bn, N, &sc, &sh))) {
-            ok = false;
-            return;
-        }
-        const int K = k * Kp;
-        std::vector<double> mtx(size_t(N) * K, 0.0);
-        std::vector<float> bias(std::max(N, 64), 0.f);
-        for (int n = 0; n < N; ++n) {
-            for (int t = 0; t < k; ++t)
-                for (int c = 0; c < Cin; ++c) mtx[size_t(n) * K + t * Kp + c] = double(w->v[(size_t(n) * Cin + c) * k + t]) * sc[n];
-            bias[n] = float(double(b->v[n]) * sc[n] + sh[n]);
-        }
-        ab.put_matrix(gw, mtx, N, K);
-        ab.put_f32(&gw->bias, bias);
-    };
-    auto bn_vectors = [&](const std::string& bn, int C, int Cp, float** scale, float** shift) {
-        std::vector<double> sc, sh;
-        if (!ab.bn_affine(bn, C, &sc, &sh)) {
-            ok = false;
-            return;
-        }
-        std::vector<float> s(Cp, 0.f), b(Cp, 0.f);
-        for (int i = 0; i < C; ++i) {
-            s[i] = float(sc[i]);
-            b[i] = float(sh[i]);
-        }
-        ab.put_f32(scale, s);
-        ab.put_f32(shift, b);
-    };
-
-    {  // head.conv1 + bn1 folded (1 -> 32 channels, CUDA-core stem)
-        const HostWeight* w = ab.get("head.conv1.weight", {32, 1, 3, 3});
-        const HostWeight* b = ab.get("head.conv1.bias", {32});
-        std::vector<double> sc, sh;
-        if (w && b && ab.bn_affine("head.bn1", 32, &sc, &sh)) {
-            std::vector<float> w9(32 * 9), bb(32);
-            for (int c = 0; c < 32; ++c) {
-                for (int k = 0; k < 9; ++k) w9[c * 9 + k] = float(double(w->v[c * 9 + k]) * sc[c]);
-                bb[c] = float(double(b->v[c]) * sc[c] + sh[c]);
-            }
-            ab.put_f32(&m->stem_w, w9);
-            ab.put_f32(&m->stem_b, bb);
-        } else {
-            ok = false;
-        }
-    }
+    bool ok = ab.fold_stem(&m->stem_w, &m->stem_b, "head.conv1", "head.bn1", 32);  // 1 -> 32 channels, CUDA-core stem
     m->res.clear();
     m->res.reserve(4);  // arena patches point into the elements
     for (int li = 1; li <= 2 && ok; ++li)
@@ -336,15 +257,13 @@ bool CamppModel::prepare_weights(ArenaBuilder& ab) {
             rw.stage = li;
             rw.has_sc = bi == 0;
             const std::string p = "head.layer" + std::to_string(li) + "." + std::to_string(bi);
-            conv2d_matrix(&rw.conv1, p + ".conv1", p + ".bn1", 32, 32, 3);
-            conv2d_matrix(&rw.conv2, p + ".conv2", p + ".bn2", 32, 32, 3);
-            if (rw.has_sc) conv2d_matrix(&rw.sc, p + ".shortcut.0", p + ".shortcut.1", 32, 32, 1);
+            ok &= ab.fold_conv(&rw.conv1, p + ".conv1", p + ".bn1", 32, 32, 3, 2);
+            ok &= ab.fold_conv(&rw.conv2, p + ".conv2", p + ".bn2", 32, 32, 3, 2);
+            if (rw.has_sc) ok &= ab.fold_conv(&rw.sc, p + ".shortcut.0", p + ".shortcut.1", 32, 32, 1, 2);
         }
-    if (ok) conv2d_matrix(&m->head_conv2, "head.conv2", "head.bn2", 32, 32, 3);
-    if (ok) {
-        // TDNN: out[t'] = sum_k w_k x[2t' + k - 2]; K-sources in tap order over the frame-pair matrix
-        conv1d_matrix(&m->tdnn, "xvector.tdnn.linear", "xvector.tdnn.nonlinear.batchnorm", cf.init_channels, m->head_ch, 5, m->head_ch);
-    }
+    if (ok) ok = ab.fold_conv(&m->head_conv2, "head.conv2", "head.bn2", 32, 32, 3, 2);
+    // TDNN: out[t'] = sum_k w_k x[2t' + k - 2]; K-sources in tap order over the frame-pair matrix
+    if (ok) ok = ab.fold_conv(&m->tdnn, "xvector.tdnn.linear", "xvector.tdnn.nonlinear.batchnorm", cf.init_channels, m->head_ch, 5, 1);
     m->layers.clear();
     m->layers.reserve(CP_MAX_LAYERS);
     int channels = cf.init_channels;
@@ -358,9 +277,9 @@ bool CamppModel::prepare_weights(ArenaBuilder& ab) {
             lw.in_ch = channels + li * G;
             lw.Kp = int(mc_align_up(size_t(lw.in_ch), 64));
             const std::string p = "xvector.block" + std::to_string(bi + 1) + ".tdnnd" + std::to_string(li + 1);
-            bn_vectors(p + ".nonlinear1.batchnorm", lw.in_ch, lw.Kp, &lw.bn1_scale, &lw.bn1_shift);
-            conv1d_matrix(&lw.linear1, p + ".linear1", p + ".nonlinear2.batchnorm", BC, lw.in_ch, 1, lw.Kp);
-            conv1d_matrix(&lw.local, p + ".cam_layer.linear_local", "", G, BC, 3, BC);
+            ok &= ab.put_bn(&lw.bn1_scale, &lw.bn1_shift, p + ".nonlinear1.batchnorm", lw.in_ch, lw.Kp);
+            ok &= ab.fold_conv(&lw.linear1, p + ".linear1", p + ".nonlinear2.batchnorm", BC, lw.in_ch, 1, 1, 0, {{1, lw.Kp, 0, lw.in_ch, 0}});
+            ok &= ab.fold_conv(&lw.local, p + ".cam_layer.linear_local", "", G, BC, 3, 1);
             const HostWeight* w1 = ab.get(p + ".cam_layer.linear1.weight", {BC / 2, BC, 1});
             const HostWeight* b1 = ab.get(p + ".cam_layer.linear1.bias", {BC / 2});
             const HostWeight* w2 = ab.get(p + ".cam_layer.linear2.weight", {G, BC / 2, 1});
@@ -385,13 +304,13 @@ bool CamppModel::prepare_weights(ArenaBuilder& ab) {
         TransitW& tw = m->transit[bi];
         tw.C = channels;
         const std::string p = "xvector.transit" + std::to_string(bi + 1);
-        bn_vectors(p + ".nonlinear.batchnorm", channels, channels, &tw.bn_scale, &tw.bn_shift);
+        ok &= ab.put_bn(&tw.bn_scale, &tw.bn_shift, p + ".nonlinear.batchnorm", channels, channels);
         // the last transit is followed directly by out_nonlinear (BN + ReLU): fold that BN into its weights
-        conv1d_matrix(&tw.linear, p + ".linear", bi == CP_NB - 1 ? "xvector.out_nonlinear.batchnorm" : "", channels / 2, channels, 1, channels);
+        ok &= ab.fold_conv(&tw.linear, p + ".linear", bi == CP_NB - 1 ? "xvector.out_nonlinear.batchnorm" : "", channels / 2, channels, 1, 1);
         channels /= 2;
     }
     m->final_ch = channels;
-    if (ok) conv1d_matrix(&m->dense, "xvector.dense.linear", "xvector.dense.nonlinear.batchnorm", cf.embd_dim, 2 * channels, 1, 2 * channels);
+    if (ok) ok = ab.fold_conv(&m->dense, "xvector.dense.linear", "xvector.dense.nonlinear.batchnorm", cf.embd_dim, 2 * channels, 1, 1);
     return ok;
 }
 
@@ -406,19 +325,8 @@ struct CpBuffers {
     float *mask, *emb_out;
 };
 
-void cp_geometry(const CamppModel* m, int T, ImageGeo* geo) {
-    int H = m->cfg.input_size;
-    for (int l = 0; l < 4; ++l) {
-        if (l > 0) H = (H - 1) / 2 + 1;
-        geo[l].H = H;
-        geo[l].W = T;
-        geo[l].Hp = H + 2;
-        geo[l].Wp = T + 2;
-    }
-}
-
 void cp_carve(const CamppModel* m, WsCarver& cv, int B, int T, ImageGeo* geo, CpBuffers* cb) {
-    cp_geometry(m, T, geo);
+    image_pyramid(geo, 4, m->cfg.input_size, T, false);
     const int T2 = (T - 1) / 2 + 1, Tp = T2 + 2 * CP_P, nseg = (T2 + CP_SEG - 1) / CP_SEG;
     const int64_t R = int64_t(B) * Tp;
     cb->stem_out = cv.planes(geo[0].rows(B), 32);
@@ -457,38 +365,21 @@ size_t CamppModel::workspace_bytes(int B, int T) const {
 
 int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
     CamppModel* const m = this;
-    const size_t need = workspace_bytes(B, T);
-    PPV_REQUIRE(ws && ws_bytes >= need, "campplus: workspace too small (see ppv_model_workspace_bytes)");
-    PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "campplus: workspace must be 256-byte aligned");
     PPV_REQUIRE(T >= 3, "campplus: too few frames (the statistics pooling needs at least two frames after the stride-2 TDNN)");
     const int T2 = (T - 1) / 2 + 1, Tp = T2 + 2 * CP_P, nseg = (T2 + CP_SEG - 1) / CP_SEG;
     PPV_REQUIRE(nseg <= CP_MAX_SEG, "campplus: utterance too long (more than 64 context segments of 100 frames)");
     PPV_REQUIRE(T + 3 < 32768, "campplus: utterance too long for 16-bit tap offsets");
+    image_pyramid(m->geo, 4, m->cfg.input_size, T, false);
+    PPV_REQUIRE(m->geo[0].rows(B) < (int64_t(1) << 31), "campplus: batch too large for 32-bit row indices");
+    int rc = claim_workspace(B, T, ws, ws_bytes, st);
+    if (rc) return rc;
     WsCarver cv;
     cv.base = static_cast<uint8_t*>(ws);
     CpBuffers cb;
     cp_carve(m, cv, B, T, m->geo, &cb);
-    PPV_REQUIRE(m->geo[0].rows(B) < (int64_t(1) << 31), "campplus: batch too large for 32-bit row indices");
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));  // zero borders, zero padding rows, zero padded columns
     m->steps.clear();
     const int M2 = int(int64_t(B) * Tp);
 
-    auto img_epi = [&](const Planes& out, const ImageGeo& gin, const ImageGeo& gout, int stride_h) {
-        Epilogue ep;
-        ep.out_mode = OUT_PLANES;
-        ep.out = out.base;
-        ep.out_ld = out.ld;
-        ep.out_plane_stride = out.plane_stride;
-        ep.img_Hp = gin.Hp;
-        ep.img_Wp = gin.Wp;
-        ep.img_H = gin.H;
-        ep.img_W = gin.W;
-        ep.img_stride = stride_h;
-        ep.img_stride_w = 1;
-        ep.out_Hp = gout.Hp;
-        ep.out_Wp = gout.Wp;
-        return ep;
-    };
     auto time_epi = [&](const Planes& out, int col0) {
         Epilogue ep;
         ep.out_mode = OUT_PLANES;
@@ -502,85 +393,52 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         ep.zero_invalid = 1;
         return ep;
     };
-    auto add_gemm = [&](const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) -> int {
-        ep.bias = gw.bias;
-        CStep s;
-        if (pointwise_step_build(&s.pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) {
-            s.kind = CStep::PW;
-        } else {
-            s.kind = CStep::GEMM;
-            int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N));
-            if (rc) return rc;
-        }
-        m->steps.push_back(s);
-        return PPV_OK;
-    };
-    auto taps9 = [&](const Planes& p, const ImageGeo& g, std::vector<GemmSource>* v) {
-        for (int dh = -1; dh <= 1; ++dh)
-            for (int dw = -1; dw <= 1; ++dw) v->push_back(GemmSource{p, 0, 32, dh * g.Wp + dw});
-    };
-    const char* c3env = getenv("PPV_CONV3X3");  // 0 = run the 3x3 convs through the generic gather-GEMM (debugging / A-B timing)
-    const bool use_c3 = !(c3env && c3env[0] == '0');
-    // 3x3 conv, 32 -> 32 channels, on grid `g` of buffer `p`: the patch kernel (conv3x3.cu), else nine taps of the gather-GEMM
-    auto add_conv3 = [&](const GemmWeights& gw, const Planes& p, const ImageGeo& g, Epilogue ep) -> int {
-        if (use_c3 && gw.N == 32 && conv3x3_c32_supported(32, gw.N, g.H, g.W)) {
-            ep.bias = gw.bias;
-            CStep s;
-            s.kind = CStep::CONV3;
-            int rc = conv3x3_build(&s.c3, p, 0, gw.W, B, g.H, g.W, g.Hp, g.Wp, ep);
-            if (rc) return rc;
-            m->steps.push_back(s);
-            return PPV_OK;
-        }
-        std::vector<GemmSource> t;
-        taps9(p, g, &t);
-        return add_gemm(gw, t, int(g.rows(B)), ep);
-    };
     auto relu = [](Epilogue ep) {
         ep.relu = 1;
         return ep;
     };
-    int rc;
-    // ---- FCM head
-    {
-        CStep s;
-        s.kind = CStep::STEM;
+    auto bn_relu = [&](const Planes& x, const float* scale, const float* shift, int C) {
+        PlanStep s = model_step(CP_BN_RELU);
+        s.x = x;
+        s.out = cb.tmp;
+        s.vec[0] = scale;
+        s.vec[1] = shift;
+        s.C = C;
+        s.rows = M2;
         m->steps.push_back(s);
-    }
+    };
+    // ---- FCM head: its convs stride the frequency axis only
+    m->steps.push_back(stem_step(m->stem_w, m->stem_b, 32, cb.stem_out, m->geo[0], B));
     Planes x = cb.stem_out;
     for (size_t i = 0; i < m->res.size(); ++i) {
         const ResBlockW& rw = m->res[i];
         const ImageGeo& gin = m->geo[rw.stride == 2 ? rw.stage - 1 : rw.stage];
         const ImageGeo& go = m->geo[rw.stage];
-        rc = add_conv3(rw.conv1, x, gin, relu(img_epi(cb.c1[i], gin, go, rw.stride)));
+        rc = plan_conv3x3(rw.conv1, x, 0, 32, gin, B, relu(image_epilogue(cb.c1[i], gin, go, rw.stride, 1)));
         if (rc) return rc;
-        rc = add_conv3(rw.conv2, cb.c1[i], go, img_epi(cb.c2[i], go, go, 1));
+        rc = plan_conv3x3(rw.conv2, cb.c1[i], 0, 32, go, B, image_epilogue(cb.c2[i], go, go, 1, 1));
         if (rc) return rc;
         Planes resid = x;
         if (rw.has_sc) {
-            rc = add_gemm(rw.sc, {GemmSource{x, 0, 32, 0}}, int(gin.rows(B)), img_epi(cb.sc[i], gin, go, rw.stride));
+            rc = plan_conv(rw.sc, {GemmSource{x, 0, 32, 0}}, int(gin.rows(B)), image_epilogue(cb.sc[i], gin, go, rw.stride, 1));
             if (rc) return rc;
             resid = cb.sc[i];
         }
-        CStep s;
-        s.kind = CStep::ADD_RELU;
-        s.a = cb.c2[i];
-        s.b = resid;
-        s.d = cb.out[i];
-        s.C = 32;
-        s.img_rows = go.Hp * go.Wp;
-        s.rows = go.rows(B);
-        m->steps.push_back(s);
+        m->steps.push_back(scale_res_step(cb.c2[i], nullptr, resid, cb.out[i], 32, go, B));
         x = cb.out[i];
         m->stage_out[rw.stage] = x;
     }
     {
-        rc = add_conv3(m->head_conv2, x, m->geo[2], relu(img_epi(cb.head_out, m->geo[2], m->geo[3], 2)));
+        rc = plan_conv3x3(m->head_conv2, x, 0, 32, m->geo[2], B, relu(image_epilogue(cb.head_out, m->geo[2], m->geo[3], 2, 1)));
         if (rc) return rc;
-        CStep s;
-        s.kind = CStep::FLATTEN;
-        s.a = cb.head_out;
-        s.d = cb.flat;
+        PlanStep s = model_step(CP_FLATTEN_PAIRS);
+        s.x = cb.head_out;
+        s.g = m->geo[3];
+        s.B = B;
+        s.C = 32;
+        s.out = cb.flat;
+        s.Tp = Tp;
+        s.P = CP_P;
         m->steps.push_back(s);
     }
     // ---- TDNN (k5, stride 2) over the frame-pair matrix -> first 128 columns of block 1's buffer
@@ -588,7 +446,7 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         const int HC = m->head_ch;
         std::vector<GemmSource> srcs = {GemmSource{cb.flat, 0, HC, -1}, GemmSource{cb.flat, HC, HC, -1}, GemmSource{cb.flat, 0, HC, 0},
                                         GemmSource{cb.flat, HC, HC, 0}, GemmSource{cb.flat, 0, HC, 1}};
-        rc = add_gemm(m->tdnn, srcs, M2, relu(time_epi(cb.xblk[0], 0)));
+        rc = plan_conv(m->tdnn, srcs, M2, relu(time_epi(cb.xblk[0], 0)));
         if (rc) return rc;
     }
     // ---- dense blocks
@@ -597,113 +455,81 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         const Planes& xb = cb.xblk[bi];
         for (int l = 0; l < CP_LAYERS[bi]; ++l, ++li) {
             const DenseLayerW& lw = m->layers[li];
-            CStep s;
-            s.kind = CStep::BN_RELU;
-            s.a = xb;
-            s.d = cb.tmp;
-            s.p0 = lw.bn1_scale;
-            s.p1 = lw.bn1_shift;
-            s.C = lw.Kp;
-            s.rows = M2;
-            m->steps.push_back(s);
-            rc = add_gemm(lw.linear1, {GemmSource{cb.tmp, 0, lw.Kp, 0}}, M2, relu(time_epi(cb.hbuf, 0)));
+            bn_relu(xb, lw.bn1_scale, lw.bn1_shift, lw.Kp);
+            rc = plan_conv(lw.linear1, {GemmSource{cb.tmp, 0, lw.Kp, 0}}, M2, relu(time_epi(cb.hbuf, 0)));
             if (rc) return rc;
-            CStep c;
-            c.kind = CStep::CONTEXT;
-            c.a = cb.hbuf;
-            c.p0 = lw.w1t;
-            c.p1 = lw.b1;
-            c.p2 = lw.w2t;
-            c.p3 = lw.b2;
-            c.fout = cb.mask;
+            PlanStep c = model_step(CP_CONTEXT);
+            c.x = cb.hbuf;
+            c.B = B;
+            c.T = T2;
+            c.P = CP_P;
+            c.Tp = Tp;
+            c.n = nseg;
+            c.vec[0] = lw.w1t;
+            c.vec[1] = lw.b1;
+            c.vec[2] = lw.w2t;
+            c.vec[3] = lw.b2;
+            c.out_f32 = cb.mask;
             m->steps.push_back(c);
             Epilogue ep = time_epi(xb, lw.in_ch);
             ep.seg_scale = cb.mask;
             ep.seg_len = CP_SEG;
             ep.nseg = nseg;
             const int BCc = cb.hbuf.ld;
-            rc = add_gemm(lw.local, {GemmSource{cb.hbuf, 0, BCc, -lw.dil}, GemmSource{cb.hbuf, 0, BCc, 0}, GemmSource{cb.hbuf, 0, BCc, lw.dil}}, M2, ep);
+            rc = plan_conv(lw.local, {GemmSource{cb.hbuf, 0, BCc, -lw.dil}, GemmSource{cb.hbuf, 0, BCc, 0}, GemmSource{cb.hbuf, 0, BCc, lw.dil}}, M2, ep);
             if (rc) return rc;
         }
         const TransitW& tw = m->transit[bi];
-        CStep s;
-        s.kind = CStep::BN_RELU;
-        s.a = xb;
-        s.d = cb.tmp;
-        s.p0 = tw.bn_scale;
-        s.p1 = tw.bn_shift;
-        s.C = tw.C;
-        s.rows = M2;
-        m->steps.push_back(s);
+        bn_relu(xb, tw.bn_scale, tw.bn_shift, tw.C);
         const bool last = bi == CP_NB - 1;
         Epilogue ep = time_epi(last ? cb.final_x : cb.xblk[bi + 1], 0);
         if (last) ep.relu = 1;  // out_nonlinear (BN folded into the transit weights) + ReLU
-        rc = add_gemm(tw.linear, {GemmSource{cb.tmp, 0, tw.C, 0}}, M2, ep);
+        rc = plan_conv(tw.linear, {GemmSource{cb.tmp, 0, tw.C, 0}}, M2, ep);
         if (rc) return rc;
         m->tr_out[bi] = last ? cb.final_x : cb.xblk[bi + 1];
     }
     {
-        CStep s;
-        s.kind = CStep::STATS;
-        m->steps.push_back(s);
+        m->steps.push_back(colstats_step(cb.final_x, m->final_ch, B, T2, CP_P, Tp, 2, 0.f, cb.stats));
         Epilogue ep;
         ep.out_mode = OUT_F32;
         ep.out = cb.emb_out;
         ep.out_ld = m->cfg.embd_dim;
-        rc = add_gemm(m->dense, {GemmSource{cb.stats, 0, 2 * m->final_ch, 0}}, B, ep);
+        rc = plan_conv(m->dense, {GemmSource{cb.stats, 0, 2 * m->final_ch, 0}}, B, ep);
         if (rc) return rc;
     }
-    m->stem_out = cb.stem_out;
-    m->flat = cb.flat;
     m->stats = cb.stats;
     m->final_x = cb.final_x;
     for (int bi = 0; bi < CP_NB; ++bi) m->xblk[bi] = cb.xblk[bi];
     m->emb_out = cb.emb_out;
     m->T2 = T2;
     m->Tp = Tp;
-    m->nseg = nseg;
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int CamppModel::run_steps(const float* feat, cudaStream_t st) {
-    CamppModel* const m = this;
-    const int B = m->plan_B, T = m->plan_T;
-    int rc = PPV_OK;
-    for (const CStep& s : m->steps) {
-        switch (s.kind) {
-            case CStep::STEM:
-                rc = launch_stem_conv(feat, B, T, m->cfg.input_size, m->stem_w, m->stem_b, 32, m->stem_out, m->geo[0].Hp, m->geo[0].Wp, st);
-                break;
-            case CStep::GEMM: rc = gemm_launch(s.gp, m->precision, m->num_sms, st); break;
-            case CStep::CONV3: rc = conv3x3_launch(s.c3, m->precision, m->num_sms, st); break;
-            case CStep::PW: rc = pointwise_launch(s.pw, m->num_sms, st); break;
-            case CStep::ADD_RELU: rc = launch_se_scale_res(s.a, nullptr, s.b, 0, s.d, 0, s.C, s.img_rows, s.rows, m->num_sms, st, 1, 0.f); break;
-            case CStep::FLATTEN: {
-                const ImageGeo& g = m->geo[3];
-                const int64_t total = int64_t(B) * g.W * 32 * g.H;
-                const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(m->num_sms) * 16));
-                PPV_PDL_OK(launch_pdl(cp_flatten_pairs_kernel, dim3(grid), dim3(256), 0, st, s.a, B, g.H, g.W, g.Hp, g.Wp, 32, s.d, m->Tp, CP_P),
-                           "cp_flatten_pairs_kernel");
-                break;
-            }
-            case CStep::BN_RELU: {
-                const int64_t total = s.rows * (s.C / 8);
-                const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(m->num_sms) * 16));
-                PPV_PDL_OK(launch_pdl(cp_bn_relu_kernel, dim3(grid), dim3(256), 0, st, s.a, s.p0, s.p1, s.d, s.C, s.rows), "cp_bn_relu_kernel");
-                break;
-            }
-            case CStep::CONTEXT:
-                PPV_PDL_OK(launch_pdl(cp_context_kernel, dim3(B), dim3(256), 0, st, s.a, m->T2, CP_P, m->Tp, m->nseg, s.p0, s.p1, s.p2, s.p3, s.fout),
-                           "cp_context_kernel");
-                break;
-            case CStep::STATS:
-                rc = launch_colstats(m->final_x, 0, m->final_ch, B, m->T2, CP_P, m->Tp, 2, 0.f, nullptr, m->stats, st);
-                break;
+int CamppModel::run_model_step(const PlanStep& s, cudaStream_t st) {
+    switch (s.model_kind) {
+        case CP_FLATTEN_PAIRS: {
+            const ImageGeo& g = s.g;
+            const int64_t total = int64_t(s.B) * g.W * s.C * g.H;
+            const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(num_sms) * 16));
+            PPV_PDL_OK(launch_pdl(cp_flatten_pairs_kernel, dim3(grid), dim3(256), 0, st, s.x, s.B, g.H, g.W, g.Hp, g.Wp, s.C, s.out, s.Tp, s.P),
+                       "cp_flatten_pairs_kernel");
+            return PPV_OK;
         }
-        if (rc) return rc;
+        case CP_BN_RELU: {
+            const int64_t total = s.rows * (s.C / 8);
+            const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(num_sms) * 16));
+            PPV_PDL_OK(launch_pdl(cp_bn_relu_kernel, dim3(grid), dim3(256), 0, st, s.x, s.vec[0], s.vec[1], s.out, s.C, s.rows), "cp_bn_relu_kernel");
+            return PPV_OK;
+        }
+        case CP_CONTEXT:
+            PPV_PDL_OK(launch_pdl(cp_context_kernel, dim3(s.B), dim3(256), 0, st, s.x, s.T, s.P, s.Tp, s.n, s.vec[0], s.vec[1], s.vec[2], s.vec[3],
+                                  s.out_f32),
+                       "cp_context_kernel");
+            return PPV_OK;
     }
-    return PPV_OK;
+    return ImagePlanModel::run_model_step(s, st);
 }
 
 // taps: "head.layer1", "head.layer2" -> fp32 [B,H,W,32]; "tdnn" [B,T2,128]; "block1".."block3" [B,T2,C]; "transit1", "transit2"
@@ -715,23 +541,18 @@ int CamppModel::tap(const std::string& n, float* out, size_t out_elems, cudaStre
         PPV_REQUIRE(out_elems >= size_t(B) * 2 * m->final_ch, "campplus_read_tap: output too small");
         return launch_planes_to_f32(m->stats, 0, 2 * m->final_ch, B, 1, 0, 1, out, st);
     }
-    if (n == "head.layer1" || n == "head.layer2") {
-        const int stage = n.back() - '0';
-        const ImageGeo& g = m->geo[stage];
-        PPV_REQUIRE(out_elems >= size_t(B) * g.H * g.W * 32, "campplus_read_tap: output too small");
-        return launch_image_to_f32(m->stage_out[stage], B, g.H, g.W, g.Hp, g.Wp, 32, out, st);
-    }
+    if (const int stage = name_index(n, "head.layer", 1, 2)) return image_tap(m->stage_out[stage], m->geo[stage], 32, out, out_elems, st);
     Planes src;
     int C = 0;
     if (n == "tdnn") {
         src = m->xblk[0];
         C = m->cfg.init_channels;
-    } else if (n.rfind("block", 0) == 0 && n.size() == 6 && n[5] >= '1' && n[5] <= '3') {
-        src = m->xblk[n[5] - '1'];
-        C = m->block_out[n[5] - '1'];
-    } else if (n.rfind("transit", 0) == 0 && n.size() == 8 && n[7] >= '1' && n[7] <= '2') {
-        src = m->tr_out[n[7] - '1'];
-        C = m->block_out[n[7] - '1'] / 2;
+    } else if (const int b = name_index(n, "block", 1, 3)) {
+        src = m->xblk[b - 1];
+        C = m->block_out[b - 1];
+    } else if (const int t = name_index(n, "transit", 1, 2)) {
+        src = m->tr_out[t - 1];
+        C = m->block_out[t - 1] / 2;
     } else if (n == "out_nonlinear") {
         src = m->final_x;
         C = m->final_ch;

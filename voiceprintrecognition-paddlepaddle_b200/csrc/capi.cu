@@ -5,6 +5,7 @@
 #include <new>
 
 #include "common.h"
+#include "image_plan.h"
 #include "model_common.h"
 
 namespace ppv {
@@ -505,9 +506,8 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
 }
 
 // ---------------------------------------------------------------- conv2d test hook
-// One conv2d of the 2-D models (ResNetSE, ERes2Net, CAM++), planned as their plans plan it: the input grid, the weight planes and the
-// image-mode epilogue are laid out as in resnet_se.cu / eres2net.cu / campplus.cu, and exactly the kernel `path` names runs, or an
-// error is returned.  Workspace: the input grid [2][pad128(B (H+2) (W+2))][x_ld], then the weight planes [2][pad256(Cout)][k k Cin].
+// One conv2d of the 2-D models (ResNetSE, ERes2Net, CAM++) on an input grid laid out as theirs, with their weight reorder, epilogue
+// and tap list (image_plan.h, model_common.h); exactly the kernel `path` names runs, or an error is returned.  Workspace: the input grid [2][pad128(B (H+2) (W+2))][x_ld], then the weight planes [2][pad256(Cout)][k k Cin].
 static size_t conv2d_test_x_bytes(int B, int H, int W, int x_ld) {
     return au(au(size_t(B) * (H + 2) * (W + 2), 128) * size_t(x_ld) * 4, 256);
 }
@@ -553,19 +553,14 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
             rc = launch_f32_to_planes(x + (int64_t(b) * H + h) * W * Cin, W, Cin, row, st);
             if (rc) return rc;
         }
-    // weights [Cout][Cin][k][k] -> [Cout][tap][Cin] with tap = kh k + kw (the order of the plans' nine row-offset sources), split
-    // into planes on the host as the models prepare theirs
+    // weights [Cout][Cin][k][k] -> [Cout][tap][Cin], split into planes on the host as the models prepare theirs
     const int K = k * k * Cin;
     std::vector<float> wh(size_t(Cout) * K);
     PPV_CUDA_OK(cudaMemcpyAsync(wh.data(), w, wh.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
     PPV_CUDA_OK(cudaStreamSynchronize(st));
-    std::vector<double> wm(wh.size());
-    for (int n = 0; n < Cout; ++n)
-        for (int c = 0; c < Cin; ++c)
-            for (int t = 0; t < k * k; ++t) wm[(size_t(n) * k * k + t) * Cin + c] = wh[(size_t(n) * Cin + c) * k * k + t];
     ArenaBuilder ab;
     GemmWeights gw;
-    ab.put_matrix(&gw, wm, Cout, K);
+    ab.put_matrix(&gw, conv_weight_matrix(wh.data(), Cout, Cin, k * k, Cout, {{k * k, Cin, 0, Cin, 0}}), Cout, K);
     uint8_t* wdev = static_cast<uint8_t*>(ws) + x_bytes;
     PPV_CUDA_OK(cudaMemcpyAsync(wdev, ab.host.data(), ab.host.size(), cudaMemcpyHostToDevice, st));
     PPV_CUDA_OK(cudaStreamSynchronize(st));
@@ -573,21 +568,14 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     // output grid, zeroed as a plan zeroes its workspace: the kernels store interior positions on the stride grid only
     const int64_t out_plane = int64_t(B) * (Ho + 2) * (Wo + 2) * Cout;
     PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2 * out_plane) * sizeof(__nv_bfloat16), st));
-    Epilogue ep;
+    Planes outp;
+    outp.base = static_cast<__nv_bfloat16*>(out);
+    outp.ld = Cout;
+    outp.plane_stride = out_plane;
+    const ImageGeo gin{H, W, Hp, Wp}, gout{Ho, Wo, Ho + 2, Wo + 2};
+    Epilogue ep = image_epilogue(outp, gin, gout, stride_h, stride_w);
     ep.bias = bias;
     ep.relu = relu ? 1 : 0;
-    ep.out_mode = OUT_PLANES;
-    ep.out = out;
-    ep.out_ld = Cout;
-    ep.out_plane_stride = out_plane;
-    ep.img_Hp = Hp;
-    ep.img_Wp = Wp;
-    ep.img_H = H;
-    ep.img_W = W;
-    ep.img_stride = stride_h;
-    ep.img_stride_w = stride_w == stride_h ? 0 : stride_w;  // 0 as ResNetSE / ERes2Net set it; CAM++'s FCM sets 1 with stride_h 2
-    ep.out_Hp = Ho + 2;
-    ep.out_Wp = Wo + 2;
     const int sms = device_sm_count();
     if (path == 0) {
         PPV_REQUIRE(k == 3 && conv3x3_c32_supported(Cin, Cout, H, W), "ppv_conv2d_test: the patch kernel takes 3x3 convs with 32 -> 32 channels only");
@@ -605,8 +593,10 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
         return pointwise_launch(s, sms, st);
     }
     std::vector<GemmSource> srcs;
-    for (int dh = -(k / 2); dh <= k / 2; ++dh)
-        for (int dw = -(k / 2); dw <= k / 2; ++dw) srcs.push_back(GemmSource{xp, x_col0, Cin, dh * Wp + dw});
+    if (k == 3)
+        image_taps(&srcs, xp, x_col0, Cin, gin);
+    else
+        srcs.push_back(GemmSource{xp, x_col0, Cin, 0});
     GemmParams gp;
     rc = gemm_build(&gp, srcs.data(), int(srcs.size()), gw.W, int(M), Cout, ep, gemm_pick_bn(Cout));
     if (rc) return rc;

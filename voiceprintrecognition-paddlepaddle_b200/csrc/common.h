@@ -331,7 +331,7 @@ int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out);
 void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);
 int campplus_create(const ppv_campplus_cfg* cfg, Model** out);
 
-// ---- conv2d models: zero-bordered NHWC image grids (resnet_se.cu, eres2net.cu) ------------------------
+// ---- conv2d models: zero-bordered NHWC image grids (image_plan.h / image_plan.cu) ------------------------
 struct ImageGeo {
     int H = 0, W = 0, Hp = 0, Wp = 0;
     int64_t rows(int B) const { return int64_t(B) * Hp * Wp; }

@@ -47,6 +47,33 @@ struct GemmWeights {  // one conv / linear layer prepared for the gather-GEMM
     int N = 0, Ktot = 0;
 };
 
+// One K group of a conv's dense weight matrix: `taps` taps of `ncols` source columns each, of which columns [pos, pos + cnt) carry
+// the conv's input channels [cin0, cin0 + cnt) and the rest are zero.
+struct ConvKGroup {
+    int taps, ncols, pos, cnt, cin0;
+};
+
+// Conv weights w [N][Cin][taps] (Paddle's Conv1D / Conv2D order, taps in (kh, kw) order) -> dense [Npad][sum taps * ncols] in
+// double, K order (group, tap, column), row n scaled by scale[n] (null: 1).  Output channel n lands in row n, or, with `chunk` > 0, in
+// row (n / chunk) * chunk_stride + n % chunk (zero-padded output chunks).  Rows and columns that carry no weight are zero.
+inline std::vector<double> conv_weight_matrix(const float* w, int N, int Cin, int taps, int Npad, const std::vector<ConvKGroup>& groups,
+                                              const double* scale = nullptr, int chunk = 0, int chunk_stride = 0) {
+    int K = 0;
+    for (const ConvKGroup& g : groups) K += g.taps * g.ncols;
+    std::vector<double> mtx(size_t(Npad) * K, 0.0);
+    for (int n = 0; n < N; ++n) {
+        const int row = chunk > 0 ? (n / chunk) * chunk_stride + n % chunk : n;
+        const double s = scale ? scale[n] : 1.0;
+        int kpos = 0;
+        for (const ConvKGroup& g : groups) {
+            for (int t = 0; t < g.taps; ++t)
+                for (int c = 0; c < g.cnt; ++c) mtx[size_t(row) * K + kpos + t * g.ncols + g.pos + c] = double(w[(size_t(n) * Cin + g.cin0 + c) * taps + t]) * s;
+            kpos += g.taps * g.ncols;
+        }
+    }
+    return mtx;
+}
+
 struct ArenaBuilder {
     const WeightMap* wm = nullptr;
     std::vector<uint8_t> host;
@@ -115,6 +142,52 @@ struct ArenaBuilder {
             (*scale)[i] = s;
             (*shift)[i] = double(b->v[i]) - double(mu->v[i]) * s;
         }
+        return true;
+    }
+    // Conv `conv` ([N][Cin][k] with dims 1, [N][Cin][k][k] with dims 2) with the BatchNorm `bn` folded in (none if empty) -> dense
+    // [Npad][K] split-bf16 matrix (see conv_weight_matrix; no groups: one group of all taps x Cin) and bias [max(Npad, 64)].
+    bool fold_conv(GemmWeights* gw, const std::string& conv, const std::string& bn, int N, int Cin, int k, int dims, int Npad = 0,
+                   std::vector<ConvKGroup> groups = {}, int chunk = 0, int chunk_stride = 0) {
+        const int taps = dims == 2 ? k * k : k;
+        if (Npad == 0) Npad = N;
+        if (groups.empty()) groups.push_back({taps, Cin, 0, Cin, 0});
+        const HostWeight* w = get(conv + ".weight", dims == 2 ? std::vector<int64_t>{N, Cin, k, k} : std::vector<int64_t>{N, Cin, k});
+        const HostWeight* b = get(conv + ".bias", {N});
+        std::vector<double> sc(N, 1.0), sh(N, 0.0);
+        if (!w || !b || (!bn.empty() && !bn_affine(bn, N, &sc, &sh))) return false;
+        const std::vector<double> mtx = conv_weight_matrix(w->v.data(), N, Cin, taps, Npad, groups, sc.data(), chunk, chunk_stride);
+        std::vector<float> bias(std::max(Npad, 64), 0.f);
+        for (int n = 0; n < N; ++n) bias[chunk > 0 ? (n / chunk) * chunk_stride + n % chunk : n] = float(double(b->v[n]) * sc[n] + sh[n]);
+        put_matrix(gw, mtx, Npad, int(mtx.size() / Npad));
+        put_f32(&gw->bias, bias);
+        return true;
+    }
+    // The 1 -> C0 channel 3x3 stem conv with its BatchNorm folded in: weights [C0][9], bias [C0] (launch_stem_conv)
+    bool fold_stem(float** w9, float** bias, const std::string& conv, const std::string& bn, int C0) {
+        const HostWeight* w = get(conv + ".weight", {C0, 1, 3, 3});
+        const HostWeight* b = get(conv + ".bias", {C0});
+        std::vector<double> sc, sh;
+        if (!w || !b || !bn_affine(bn, C0, &sc, &sh)) return false;
+        std::vector<float> wf(size_t(C0) * 9), bf(C0);
+        for (int c = 0; c < C0; ++c) {
+            for (int k = 0; k < 9; ++k) wf[c * 9 + k] = float(double(w->v[c * 9 + k]) * sc[c]);
+            bf[c] = float(double(b->v[c]) * sc[c] + sh[c]);
+        }
+        put_f32(w9, wf);
+        put_f32(bias, bf);
+        return true;
+    }
+    // BatchNorm `bn` as fp32 scale / shift vectors of Cp >= C entries, zero beyond C
+    bool put_bn(float** scale, float** shift, const std::string& bn, int C, int Cp) {
+        std::vector<double> sc, sh;
+        if (!bn_affine(bn, C, &sc, &sh)) return false;
+        std::vector<float> s(Cp, 0.f), b(Cp, 0.f);
+        for (int i = 0; i < C; ++i) {
+            s[i] = float(sc[i]);
+            b[i] = float(sh[i]);
+        }
+        put_f32(scale, s);
+        put_f32(shift, b);
         return true;
     }
     int upload(void** arena) {
@@ -214,6 +287,15 @@ struct Model {
         plan_ws = ws;
         plan_B = B;
         plan_T = T;
+        return PPV_OK;
+    }
+    // The opening of build_plan: `ws` must hold workspace_bytes(B, T) bytes at 256-byte alignment; it is zeroed on `st`, because the
+    // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
+    int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
+        const size_t need = workspace_bytes(B, T);
+        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see ppv_model_workspace_bytes)");
+        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
+        PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
         return PPV_OK;
     }
     int copy_embeddings(float* emb, cudaStream_t st) {
