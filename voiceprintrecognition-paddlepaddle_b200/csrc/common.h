@@ -144,7 +144,8 @@ struct Epilogue {
     int lean = 0;  // set by gemm_build: the epilogue needs only what epilogue_frag_lean does (gemm_epilogue.cuh)
 };
 
-constexpr int GEMM_TRACE_TILES = 16;  // PPV_GEMM_TRACE: CTA 0's first tiles stamped
+constexpr int GEMM_TRACE_TILES = 16;   // PPV_GEMM_TRACE: the traced CTA's first tiles stamped
+constexpr int GEMM_TRACE_EVENTS = 16;  // stamps per role and tile
 
 struct GemmParams {
     CUtensorMap mapA[GEMM_MAX_MAPS];
@@ -152,7 +153,6 @@ struct GemmParams {
     KStep ksteps[GEMM_MAX_KSTEPS];
     int num_ksteps;
     int bk;  // K elements per k-step (64 or 32)
-    int l2_prefetch;  // producer prefetches the next tile's activation rows into L2
     int ws;           // weight-stationary mode (set by gemm_build): W resident in shared memory, the ring carries activations only
     int lin_splits;   // > 0: weight-gradient mode (see gemm_build_wgrad): K runs over operand columns, split in lin_splits parts
     int lin_b_row0, lin_b_col0;
@@ -160,8 +160,10 @@ struct GemmParams {
     int M, N;
     int m_tiles, n_tiles;
     Epilogue epi;
-    // debug (PPV_GEMM_TRACE): clock64 stamps of CTA 0, [role][tile][event] with role 0 = producer, 1 + g = MMA warpgroup g
+    // debug (PPV_GEMM_TRACE=<cta>, default 0): clock64 stamps of CTA trace_cta, [role][tile][event] with role 0 = producer,
+    // 1 + g = MMA warpgroup g
     unsigned long long* trace;
+    int trace_cta;
     int bn;  // n-tile width (64, 128 or 256): selects the kernel instance.  Last, so that no kernel parameter offset depends on it.
 };
 void gemm_trace_dump(const GemmParams& gp);

@@ -106,13 +106,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     const int nk = gp.num_ksteps;
     auto tile_m = [&](int t) { return (t % mn_tiles) / gp.n_tiles; };
     auto tile_n = [&](int t) { return (t % mn_tiles) % gp.n_tiles; };
-    // PPV_GEMM_TRACE stamps of CTA 0 (`on`: tracing, this CTA, the stamping thread, local tile in range).  Producer events: 0 / 1 its
-    // first / last ring-slot wait of the tile passed, 7 of tile 0 the kernel start.  MMA warpgroup events: 0 hand-off barrier passed,
-    // 1 first `full` wait passed, 2 last k-step issued, 3 wgmma_wait<0> returned, 4 / 5 epilogue start / end.
-    const bool trace_cta = gp.trace != nullptr && blockIdx.x == 0;
+    // PPV_GEMM_TRACE stamps of one CTA (gp.trace_cta; `on`: tracing, this CTA, the stamping thread, local tile in range), GEMM_TRACE_EVENTS
+    // per tile.  Producer: 0-2 / 3-5 its ring-slot waits of k-steps 0-2 / nk-3..nk-1 passed, 8-10 / 11-13 their TMA loads issued, 7 of
+    // tile 0 the kernel start.  MMA warpgroup: 0 hand-off barrier passed, 1 first `full` wait passed, 2 last
+    // k-step issued, 3 wgmma_wait<0> returned, 4 / 5 epilogue start / end, 6-8 / 9-11 the `empty` arrivals releasing k-steps 0-2 /
+    // nk-3..nk-1.
+    const bool trace_cta = gp.trace != nullptr && int(blockIdx.x) == gp.trace_cta;
     auto stamp = [&](bool on, int role, int local, int ev) {
-        if (on) gp.trace[(role * GEMM_TRACE_TILES + local) * 8 + ev] = clock64();
+        if (on) gp.trace[(role * GEMM_TRACE_TILES + local) * GEMM_TRACE_EVENTS + ev] = clock64();
     };
+    // the first and last three k-steps of a tile: event base + 0..2 / base + 3..5
+    auto stamp_kstep = [&](bool on, int role, int local, int base, int s) {
+        if (s >= 0 && s < 3) stamp(on, role, local, base + s);
+        if (s >= nk - 3 && s >= 0) stamp(on, role, local, base + 3 + s - (nk - 3));
+    };
+    auto stamp_release = [&](bool on, int role, int local, int s) { stamp_kstep(on, role, local, 6, s); };
     stamp(trace_cta && threadIdx.x == 0, 0, 0, 7);
 
     if (warp < 4) {
@@ -133,22 +141,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 const int zsplit = tile / mn_tiles;
                 const int m0 = tile_m(tile) * GEMM_BM;
                 const int n0 = tile_n(tile) * BN;
-                // L2 prefetch of the activation rows of this CTA's NEXT tile (one CTA per m-tile issues it): they come
-                // from HBM, and a 2-4 slot ring alone cannot hide that latency.
-                const int ntile = tile + gridDim.x;
-                if (gp.l2_prefetch && ntile < num_tiles && tile_n(ntile) == 0 && lane < nk && gp.lin_splits == 0) {
-                    const int nm0 = tile_m(ntile) * GEMM_BM;
-                    for (int s = lane; s < nk; s += 32) {
-                        const KStep ks = gp.ksteps[s];
-#pragma unroll
-                        for (int p = 0; p < Cfg::NA; ++p) tma_prefetch_l2_3d(&gp.mapA[ks.map], ks.a_col, nm0 + ks.row_off, p);
-                    }
-                }
-                __syncwarp();
                 for (int s = 0; s < nk; ++s) {
                     mbar_wait(empty_bar(stage), phase ^ 1u);
-                    stamp(tr && s == 0, 0, local, 0);
-                    stamp(tr && s == nk - 1, 0, local, 1);
+                    stamp_kstep(tr, 0, local, 0, s);
                     if (lane == 0) {
                         const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
                         const uint32_t sb = sa + Cfg::NA * Cfg::A_BYTES;
@@ -173,6 +168,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
                             for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, s * BK, n0, p);
                         }
+                        stamp_kstep(tr, 0, local, 8, s);
                     }
                     __syncwarp();
                     if (++stage == nst) {
@@ -248,6 +244,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 stamp(tr && s == nk - 1, 1 + g, local, 2);
                 wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
                 if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+                stamp_release(tr, 1 + g, local, s - 1);
                 prev = stage;
                 if (++stage == nst) {
                     stage = 0;
@@ -261,6 +258,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             wgmma_fence_acc(acc0);
             wgmma_fence_acc(acc1);
             if (t == 0) mbar_arrive(empty_bar(prev));
+            stamp_release(tr, 1 + g, local, nk - 1);
             stamp(tr, 1 + g, local, 4);
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
             // rows 0-63 from acc0, then rows 64-127 moved down into acc0: one copy of the epilogue code
@@ -316,6 +314,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 stamp(tr && s == nk - 1, 1 + g, local, 2);
                 wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
                 if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
+                stamp_release(tr, 1 + g, local, s - 1);
                 prev = stage;
                 if (++stage == nst) {
                     stage = 0;
@@ -326,6 +325,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             stamp(tr, 1 + g, local, 3);
             wgmma_fence_acc(acc);
             if (t == 0) mbar_arrive(empty_bar(prev));
+            stamp_release(tr, 1 + g, local, nk - 1);
             stamp(tr, 1 + g, local, 4);
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
             const int rbase = m0 + 64 * g;
@@ -440,16 +440,14 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
     {
         const char* ns = getenv("PPV_GEMM_NOSTORE");
         gp->epi.debug_nostore = (ns && ns[0] == '1') ? 1 : 0;
-        const char* pf = getenv("PPV_GEMM_NO_L2PREFETCH");
-        gp->l2_prefetch = (pf && pf[0] == '1') ? 0 : 1;
     }
-    if (getenv("PPV_GEMM_TRACE")) {  // debug: leaked on purpose, read back by gemm_trace_dump
+    if (const char* tr = getenv("PPV_GEMM_TRACE")) {  // debug: leaked on purpose, read back by gemm_trace_dump
+        constexpr size_t n = 3 * GEMM_TRACE_TILES * GEMM_TRACE_EVENTS;
         static unsigned long long* buf = nullptr;
-        if (!buf) {
-            PPV_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&buf), 3 * GEMM_TRACE_TILES * 8 * sizeof(unsigned long long)));
-            PPV_CUDA_OK(cudaMemset(buf, 0, 3 * GEMM_TRACE_TILES * 8 * sizeof(unsigned long long)));
-        }
+        if (!buf) PPV_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&buf), n * sizeof(unsigned long long)));
+        PPV_CUDA_OK(cudaMemset(buf, 0, n * sizeof(unsigned long long)));
         gp->trace = buf;
+        gp->trace_cta = atoi(tr);
     }
     if (epi.out_mode == OUT_PLANES) {
         PPV_REQUIRE((epi.out_ld % 16) == 0 && (epi.out_col0 % 16) == 0 && (epi.out_plane_stride % 16) == 0 &&
@@ -522,25 +520,34 @@ static int launch_bn(const GemmParams& gp, bool x3, int num_sms, cudaStream_t st
 
 // Prints the stamps of the last traced launch in cycles from the kernel start, one line per role and tile, with the phases they give:
 // wait = hand-off passed -> first `full` passed, kloop = first `full` -> wgmma_wait<0> returned, epi = epilogue start -> end,
-// period = this tile's epilogue end - the previous tile's of the same warpgroup.
+// period = this tile's epilogue end - the previous tile's of the same warpgroup.  The producer lines give, for k-steps 0-2 and
+// nk-3..nk-1, when its ring-slot wait passed and when the TMA loads were issued; the MMA lines when the consumer released those
+// k-steps' slots (`empty` arrival).
 void gemm_trace_dump(const GemmParams& gp) {
     if (!gp.trace) return;
-    unsigned long long h[3 * GEMM_TRACE_TILES * 8];
+    constexpr int E = GEMM_TRACE_EVENTS;
+    unsigned long long h[3 * GEMM_TRACE_TILES * E];
     cudaDeviceSynchronize();
     cudaMemcpy(h, gp.trace, sizeof(h), cudaMemcpyDeviceToHost);
     const unsigned long long t0 = h[7];
-    auto at = [&](int r, int i, int e) -> long long { const unsigned long long v = h[(r * GEMM_TRACE_TILES + i) * 8 + e]; return v ? (long long)(v - t0) : -1ll; };
-    printf("gemm trace M=%d N=%d nk=%d BN=%d (cycles from kernel start)\n", gp.M, gp.N, gp.num_ksteps, gp.bn);
-    for (int i = 0; i < GEMM_TRACE_TILES; ++i)
-        if (at(0, i, 0) >= 0) printf("gemm trace tma  tile %2d: first slot %8lld  last slot %8lld\n", i, at(0, i, 0), at(0, i, 1));
+    auto at = [&](int r, int i, int e) -> long long { const unsigned long long v = h[(r * GEMM_TRACE_TILES + i) * E + e]; return v ? (long long)(v - t0) : -1ll; };
+    printf("gemm trace M=%d N=%d nk=%d BN=%d CTA %d (cycles from kernel start)\n", gp.M, gp.N, gp.num_ksteps, gp.bn, gp.trace_cta);
+    for (int i = 0; i < GEMM_TRACE_TILES; ++i) {
+        if (at(0, i, 0) < 0) continue;
+        printf("gemm trace tma  tile %2d: slot passed / loads issued, k-steps 0-2 and last 3:", i);
+        for (int e = 0; e < 6; ++e) printf(" %lld/%lld", at(0, i, e), at(0, i, 8 + e));
+        printf("\n");
+    }
     for (int r = 1; r < 3; ++r) {
         long long prev_end = -1;
         for (int i = 0; i < GEMM_TRACE_TILES; ++i) {
             if (at(r, i, 0) < 0) continue;
             printf("gemm trace wg%d  tile %2d:", r - 1, i);
             for (int e = 0; e < 6; ++e) printf(" %8lld", at(r, i, e));
-            printf("   wait %6lld  kloop %6lld  epi %6lld  period %6lld\n", at(r, i, 1) - at(r, i, 0), at(r, i, 3) - at(r, i, 1),
+            printf("   wait %6lld  kloop %6lld  epi %6lld  period %6lld   released", at(r, i, 1) - at(r, i, 0), at(r, i, 3) - at(r, i, 1),
                    at(r, i, 5) - at(r, i, 4), prev_end >= 0 ? at(r, i, 5) - prev_end : -1ll);
+            for (int e = 6; e < 12; ++e) printf(" %lld", at(r, i, e));
+            printf("\n");
             prev_end = at(r, i, 5);
         }
     }
