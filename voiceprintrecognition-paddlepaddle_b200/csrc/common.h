@@ -357,7 +357,7 @@ int64_t trainer_stat_count(const Trainer* t);
 int trainer_lookup(const Trainer* t, const char* name, int64_t* off, int64_t* numel, int* is_stat);
 int trainer_bind(Trainer* t, float* params, float* grads, float* stats);
 int trainer_set_precision(Trainer* t, int precision);
-size_t trainer_workspace_bytes(Trainer* t, int B, int T);
+size_t trainer_workspace_bytes(const Trainer* t, int B, int T);
 int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* labels, int B, int T, float margin, float scale, int easy_margin,
                              float label_smoothing, float* loss_out, float* logits_out, void* ws, size_t ws_bytes, cudaStream_t st);
 int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems, cudaStream_t st);

@@ -326,15 +326,12 @@ size_t EcapaModel::workspace_bytes(int B, int T) const {
 int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
     EcapaModel* const m = this;
     PPV_REQUIRE(T > m->P, "ecapa: too few frames for the reflect padding");
-    const size_t need = workspace_bytes(B, T);
-    PPV_REQUIRE(ws && ws_bytes >= need, "ecapa: workspace too small (see ppv_model_workspace_bytes)");
-    PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "ecapa: workspace must be 256-byte aligned");
+    int rc = claim_workspace(B, T, ws, ws_bytes, st);
+    if (rc) return rc;
     WsCarver cv;
     cv.base = static_cast<uint8_t*>(ws);
     carve(m, cv, B, T, &m->buf, &m->emb_out);
     m->Tp = T + 2 * m->P;
-    // garbage rows (halo of never-written buffers) must at least be finite
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
     m->steps.clear();
     const int Tp = m->Tp, P = m->P, C = m->C, C3 = m->C3, w = m->width;
     const int64_t R = int64_t(B) * Tp;
@@ -406,7 +403,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         ep.relu = 1;
         return ep;
     };
-    int rc = add_gemm(m->conv0, spec_conv0(m), nullptr, 0, int(R), planes_out(m->buf.bufs[B_X0], 0, false));
+    rc = add_gemm(m->conv0, spec_conv0(m), nullptr, 0, int(R), planes_out(m->buf.bufs[B_X0], 0, false));
     if (rc) return rc;
     for (int b = 1; b <= 3; ++b) {
         const Planes& X = (b == 1) ? m->buf.bufs[B_X0] : m->buf.bufs[B_CAT];

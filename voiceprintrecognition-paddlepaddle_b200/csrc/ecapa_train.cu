@@ -37,14 +37,12 @@ struct TConv {
     std::string name;  // e.g. "blocks.1.tdnn1.conv.conv" (weight [Cout, CinTotal, taps], bias [Cout])
     int Cout = 0, Cin = 0, CinTotal = 0, Cinp = 0, taps = 1, dil = 1;
     int64_t w_off = 0, b_off = 0;
-    Planes wf, wd;
     bool dgrad = true;
 };
 struct TBN {
     std::string name;  // e.g. "blocks.1.tdnn1.norm.norm"
     int C = 0;
     int64_t g_off = 0, b_off = 0, rm_off = 0, rv_off = 0;
-    float *mean = nullptr, *rstd = nullptr, *scale = nullptr, *shift = nullptr;  // workspace
 };
 struct TLayer {  // TDNNBlock
     TConv conv;
@@ -76,14 +74,43 @@ struct TStep {
     int layer = -1;
 };
 
+// The workspace views of one plan (tr_carve).  `layer` is indexed like Trainer::conv: the TDNN layers, then asp.conv.
+struct TrBuffers {
+    int Tp = 0;          // rows per utterance: T + 2P
+    int64_t R = 0, Rp = 0;  // rows of the padded time layout, B * Tp, and that rounded up to 128
+    struct Layer {
+        Planes wf, wd;  // weights in GEMM layouts
+        float *mean = nullptr, *rstd = nullptr, *scale = nullptr, *shift = nullptr;  // BatchNorm (none for asp.conv)
+    };
+    std::vector<Layer> layer;
+    Planes X0, A0, Y0, At1[3], Yt1[3], Ares[3], RC[3], IN[3], At2[3], Yt2[3], OUTCAT, Amfa, M, Aatt, A4, gstat_pl;
+    Planes dlogits, dMd, dA4, dZatt, dMatt, dZmfa, dOUTCAT, Dbuf[3], dZt2[3], dRC[3], dZres[3], DIN[3], dZt1[3], dXt1[3], dZ0, TA, TB;
+    float *logits = nullptr, *se_s[3], *se_g1[3], *se_g2[3], *gstat = nullptr, *fold = nullptr, *pooled = nullptr, *pn = nullptr, *emb = nullptr,
+          *cls_logits = nullptr, *loss = nullptr, *aspbn_mean = nullptr, *aspbn_rstd = nullptr;
+    float *d_emb = nullptr, *dpn = nullptr, *dpooled = nullptr, *dgs = nullptr, *rs = nullptr, *rb = nullptr, *dg2 = nullptr, *dg1 = nullptr, *ds = nullptr,
+          *part = nullptr, *wpart = nullptr;
+    size_t part_elems = 0;
+    void* aam_ws = nullptr;
+    size_t aam_ws_bytes = 0;
+};
+
+// One readable tap (trainer_read_tap): planes read as fp32 [B, T, cols] from column col0, or `count` fp32 values as stored.  A
+// per-block tap has one buffer per block; the others use index 0.
+struct TrTap {
+    bool per_block = false, f32 = false;
+    Planes pl[3];
+    int col0 = 0, cols = 0;
+    const float* vec[3] = {};
+    size_t count = 0;
+};
+
 }  // namespace
 
-struct Trainer {
+struct Trainer : PlanOwner {
     ppv_ecapa_cfg cfg;
     int S = 0;  // classes
     int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0, D = 0;
-    int num_sms = 132;
-    int precision = PPV_PREC_BF16X3;  // PPV_PREC_BF16: single-pass bf16 operands for every forward / data-gradient / weight-gradient GEMM (AMP mode)
+    // (PlanOwner::precision PPV_PREC_BF16: single-pass bf16 operands for every forward / data-gradient / weight-gradient GEMM, AMP mode)
     // flat layout
     std::map<std::string, std::pair<int64_t, int64_t>> pmap, smap;  // name -> (offset, numel)
     int64_t n_params = 0, n_stats = 0;
@@ -95,19 +122,17 @@ struct Trainer {
     int64_t se1_w[3], se1_b[3], se2_w[3], se2_b[3], aspbn_g = 0, aspbn_b = 0, aspbn_rm = 0, aspbn_rv = 0, fc_w = 0, fc_b = 0, cls_w = 0;
     // plan
     std::vector<TStep> steps;
-    void* plan_ws = nullptr;
-    int plan_B = 0, plan_T = 0, Tp = 0;
-    int64_t R = 0, Rp = 0;
-    // buffers
-    Planes X0, A0, Y0, At1[3], Yt1[3], Ares[3], RC[3], IN[3], At2[3], Yt2[3], OUTCAT, Amfa, M, Aatt, A4, gstat_pl;
-    Planes dlogits, dMd, dA4, dZatt, dMatt, dZmfa, dOUTCAT, Dbuf[3], dZt2[3], dRC[3], dZres[3], DIN[3], dZt1[3], dXt1[3], dZ0, TA, TB;  // per-block gradient buffers stay readable (taps)
-    float *logits = nullptr, *se_s[3], *se_g1[3], *se_g2[3], *gstat = nullptr, *fold = nullptr, *pooled = nullptr, *pn = nullptr, *emb = nullptr,
-          *cls_logits = nullptr, *loss = nullptr, *aspbn_mean = nullptr, *aspbn_rstd = nullptr;
-    float *d_emb = nullptr, *dpn = nullptr, *dpooled = nullptr, *dgs = nullptr, *rs = nullptr, *rb = nullptr, *dg2 = nullptr, *dg1 = nullptr, *ds = nullptr,
-          *part = nullptr, *wpart = nullptr;
-    size_t part_elems = 0;
-    void* aam_ws = nullptr;
-    size_t aam_ws_bytes = 0;
+    TrBuffers buf;
+    std::map<std::string, TrTap> taps;
+
+    Trainer() : PlanOwner("trainer", "ppv_trainer_workspace_bytes", PPV_PREC_BF16X3) {}
+    // convs by layer index: L's, then asp.conv
+    int l_att2() const { return int(L.size()); }
+    const TConv& conv(int layer) const { return layer == l_att2() ? att2 : L[layer].conv; }
+    size_t workspace_bytes(int B, int T) const override;
+
+  protected:
+    int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
 };
 
 // ------------------------------------------------------------------------------------------------ create: flat layout
@@ -144,7 +169,6 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
     int P = (cfg->kernel_sizes[0] - 1) / 2 * cfg->dilations[0];
     for (int i = 1; i <= 3; ++i) P = std::max(P, cfg->dilations[i]);
     t->P = P;
-    t->num_sms = device_sm_count();
 
     auto add_layer = [&](const std::string& p, int cin, int cout, int k, int dil, bool dgrad) {
         TLayer l;
@@ -236,18 +260,12 @@ int trainer_bind(Trainer* t, float* params, float* grads, float* stats) {
     t->params = params;
     t->grads = grads;
     t->stats = stats;
-    t->plan_ws = nullptr;  // pointers are baked into the plan
+    t->invalidate_plan();  // pointers are baked into the plan
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ workspace
 namespace {
-
-struct TrCarve {
-    WsCarver cv;
-    Planes act(int64_t Rp, int C) { return cv.planes(Rp, C); }
-    float* f32(size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); }
-};
 
 // Frame splits of a layer's BatchNorm backward: narrow layers split the frames of an utterance over several CTAs so the
 // reduction fills the GPU.  The attention TDNN keeps per-utterance sums, which ASP_CTX_BWD reads back from `part`.
@@ -256,139 +274,182 @@ int tr_bn_bwd_tsplit(const Trainer* t, int layer, int B) {
     return (layer == t->l_att1 || ctas >= 2 * t->num_sms) ? 1 : std::min(8, std::max(1, (2 * t->num_sms + ctas - 1) / ctas));
 }
 
-void tr_carve(Trainer* t, TrCarve& k, int B, int T) {
-    const int Tp = T + 2 * t->P;
-    const int64_t R = int64_t(B) * Tp, Rp = int64_t(mc_align_up(size_t(R), 128));
+// Split-K of a conv's weight-gradient GEMM [Cout] x [taps * Cinp] over the Rp frame rows: enough splits to fill the GPU, at most
+// one per 64 rows.  Each split writes an [Mpad][taps * Cinp] partial to `wpart`.
+struct WgradSplit {
+    int splits, Mpad, BN;
+};
+WgradSplit tr_wgrad_split(const Trainer* t, const TConv& c, int64_t Rp) {
+    const int N = c.taps * c.Cinp, BN = gemm_pick_bn(N);
+    const int mt = (c.Cout + 127) / 128, nt = (N + BN - 1) / BN;
+    return {std::max(1, std::min((t->num_sms + mt * nt - 1) / (mt * nt), int((Rp + 63) / 64))), mt * 128, BN};
+}
+
+void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
+    f->Tp = T + 2 * t->P;
+    f->R = int64_t(B) * f->Tp;
+    f->Rp = int64_t(mc_align_up(size_t(f->R), 128));
+    const int64_t Rp = f->Rp;
     const int C = t->C, C3 = t->C3;
-    t->Tp = Tp;
-    t->R = R;
-    t->Rp = Rp;
-    // weights in GEMM layouts
-    auto wplanes = [&](TConv& c) {
-        c.wf = k.cv.planes(int64_t(mc_align_up(size_t(c.Cout), 256)), c.taps * c.Cinp);
-        if (c.dgrad) c.wd = k.cv.planes(int64_t(mc_align_up(size_t(c.Cinp), 256)), c.taps * c.Cout);
+    auto f32 = [&](size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); };
+    f->layer.assign(t->l_att2() + 1, TrBuffers::Layer());
+    for (int l = 0; l <= t->l_att2(); ++l) {
+        const TConv& c = t->conv(l);
+        TrBuffers::Layer& w = f->layer[l];
+        w.wf = cv.planes(int64_t(mc_align_up(size_t(c.Cout), 256)), c.taps * c.Cinp);
+        if (c.dgrad) w.wd = cv.planes(int64_t(mc_align_up(size_t(c.Cinp), 256)), c.taps * c.Cout);
+        if (l == t->l_att2()) break;
+        const int Cb = t->L[l].bn.C;
+        w.mean = f32(Cb);
+        w.rstd = f32(Cb);
+        w.scale = f32(Cb);
+        w.shift = f32(Cb);
+    }
+    auto act = [&](std::initializer_list<Planes*> ps, int cols) {
+        for (Planes* p : ps) *p = cv.planes(Rp, cols);
     };
-    for (TLayer& l : t->L) {
-        wplanes(l.conv);
-        l.bn.mean = k.f32(l.bn.C);
-        l.bn.rstd = k.f32(l.bn.C);
-        l.bn.scale = k.f32(l.bn.C);
-        l.bn.shift = k.f32(l.bn.C);
-    }
-    wplanes(t->att2);
-    t->X0 = k.act(Rp, t->Fp);
-    t->A0 = k.act(Rp, C);
-    t->Y0 = k.act(Rp, C);
+    f->X0 = cv.planes(Rp, t->Fp);
+    act({&f->A0, &f->Y0}, C);
     for (int b = 0; b < 3; ++b) {
-        t->At1[b] = k.act(Rp, C);
-        t->Yt1[b] = k.act(Rp, C);
-        t->Ares[b] = k.act(Rp, C);
-        t->RC[b] = k.act(Rp, C);
-        t->IN[b] = k.act(Rp, C);
-        t->At2[b] = k.act(Rp, C);
-        t->Yt2[b] = k.act(Rp, C);
-        t->se_s[b] = k.f32(size_t(B) * C);
-        t->se_g1[b] = k.f32(size_t(B) * t->se);
-        t->se_g2[b] = k.f32(size_t(B) * C);
+        act({&f->At1[b], &f->Yt1[b], &f->Ares[b], &f->RC[b], &f->IN[b], &f->At2[b], &f->Yt2[b]}, C);
+        f->se_s[b] = f32(size_t(B) * C);
+        f->se_g1[b] = f32(size_t(B) * t->se);
+        f->se_g2[b] = f32(size_t(B) * C);
     }
-    t->OUTCAT = k.act(Rp, C3);
-    t->Amfa = k.act(Rp, C3);
-    t->M = k.act(Rp, C3);
-    t->Aatt = k.act(Rp, t->att);
-    t->A4 = k.act(Rp, t->att);
-    t->gstat_pl = k.cv.planes(B, 2 * C3);
-    t->logits = k.f32(size_t(Rp) * C3);
-    t->gstat = k.f32(size_t(B) * 2 * C3);
-    t->fold = k.f32(size_t(B) * t->att);
-    t->pooled = k.f32(size_t(B) * 2 * C3);
-    t->pn = k.f32(size_t(B) * 2 * C3);
-    t->emb = k.f32(size_t(B) * t->D);
-    t->cls_logits = k.f32(size_t(B) * t->S);
-    t->loss = k.f32(8);
-    t->aspbn_mean = k.f32(2 * C3);
-    t->aspbn_rstd = k.f32(2 * C3);
+    act({&f->OUTCAT, &f->Amfa, &f->M}, C3);
+    act({&f->Aatt, &f->A4}, t->att);
+    f->gstat_pl = cv.planes(B, 2 * C3);
+    f->logits = f32(size_t(Rp) * C3);
+    f->gstat = f32(size_t(B) * 2 * C3);
+    f->fold = f32(size_t(B) * t->att);
+    f->pooled = f32(size_t(B) * 2 * C3);
+    f->pn = f32(size_t(B) * 2 * C3);
+    f->emb = f32(size_t(B) * t->D);
+    f->cls_logits = f32(size_t(B) * t->S);
+    f->loss = f32(8);
+    f->aspbn_mean = f32(2 * C3);
+    f->aspbn_rstd = f32(2 * C3);
     // gradients
-    t->dlogits = k.act(Rp, C3);
-    t->dMd = k.act(Rp, C3);
-    t->dA4 = k.act(Rp, t->att);
-    t->dZatt = k.act(Rp, t->att);
-    t->dMatt = k.act(Rp, C3);
-    t->dZmfa = k.act(Rp, C3);
-    t->dOUTCAT = k.act(Rp, C3);
-    for (int b = 0; b < 3; ++b) {
-        t->Dbuf[b] = k.act(Rp, C);
-        t->dZt2[b] = k.act(Rp, C);
-        t->dRC[b] = k.act(Rp, C);
-        t->dZres[b] = k.act(Rp, C);
-        t->DIN[b] = k.act(Rp, C);
-        t->dZt1[b] = k.act(Rp, C);
-        t->dXt1[b] = k.act(Rp, C);
-    }
-    t->dZ0 = k.act(Rp, C);
-    t->TA = k.cv.planes(C3, int(Rp));
-    t->TB = k.cv.planes(C3, int(Rp));
-    t->d_emb = k.f32(size_t(B) * t->D);
-    t->dpn = k.f32(size_t(B) * 2 * C3);
-    t->dpooled = k.f32(size_t(B) * 2 * C3);
-    t->dgs = k.f32(size_t(B) * 2 * C3);
-    t->rs = k.f32(size_t(B) * C3);
-    t->rb = k.f32(size_t(B) * C3);
-    t->dg2 = k.f32(size_t(B) * C);
-    t->dg1 = k.f32(size_t(B) * t->se);
-    t->ds = k.f32(size_t(B) * C);
+    act({&f->dlogits, &f->dMd}, C3);
+    act({&f->dA4, &f->dZatt}, t->att);
+    act({&f->dMatt, &f->dZmfa, &f->dOUTCAT}, C3);
+    for (int b = 0; b < 3; ++b) act({&f->Dbuf[b], &f->dZt2[b], &f->dRC[b], &f->dZres[b], &f->DIN[b], &f->dZt1[b], &f->dXt1[b]}, C);
+    act({&f->dZ0}, C);
+    f->TA = cv.planes(C3, int(Rp));
+    f->TB = cv.planes(C3, int(Rp));
+    f->d_emb = f32(size_t(B) * t->D);
+    f->dpn = f32(size_t(B) * 2 * C3);
+    f->dpooled = f32(size_t(B) * 2 * C3);
+    f->dgs = f32(size_t(B) * 2 * C3);
+    f->rs = f32(size_t(B) * C3);
+    f->rb = f32(size_t(B) * C3);
+    f->dg2 = f32(size_t(B) * C);
+    f->dg1 = f32(size_t(B) * t->se);
+    f->ds = f32(size_t(B) * C);
     // partial sums: BatchNorm forward statistics [B][3][C], per-utterance column sums [B][C], BatchNorm backward [B * tsplit][2][C]
-    t->part_elems = size_t(3) * B * C3;
+    f->part_elems = size_t(3) * B * C3;
     for (int l = 0; l < int(t->L.size()); ++l)
-        t->part_elems = std::max(t->part_elems, size_t(2) * B * tr_bn_bwd_tsplit(t, l, B) * t->L[l].bn.C);
-    t->part = k.f32(t->part_elems);
-    // weight-gradient partials: max over layers of splits * Mpad * Ktot; splits <= num_sms
+        f->part_elems = std::max(f->part_elems, size_t(2) * B * tr_bn_bwd_tsplit(t, l, B) * t->L[l].bn.C);
+    f->part = f32(f->part_elems);
+    // weight-gradient partials: the largest split-K output of any conv
     size_t wmax = 0;
-    auto wsize = [&](const TConv& c) {
-        const size_t N = size_t(c.taps) * c.Cinp, mt = (c.Cout + 127) / 128, bn = gemm_pick_bn(int(N)), nt = (N + bn - 1) / bn;
-        const size_t splits = std::max<size_t>(1, std::min<size_t>((t->num_sms + mt * nt - 1) / (mt * nt), (Rp + 63) / 64));
-        wmax = std::max(wmax, splits * mt * 128 * N);
+    for (int l = 0; l <= t->l_att2(); ++l) {
+        const TConv& c = t->conv(l);
+        const WgradSplit w = tr_wgrad_split(t, c, Rp);
+        wmax = std::max(wmax, size_t(w.splits) * w.Mpad * c.taps * c.Cinp);
+    }
+    f->wpart = f32(wmax);
+    f->aam_ws_bytes = aam_workspace_bytes(B, t->D, t->S);
+    f->aam_ws = cv.take(f->aam_ws_bytes);
+}
+
+// The taps trainer_read_tap serves, by name without the "pad:" prefix and the block suffix.
+std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, int B) {
+    const int C = t->C, C3 = t->C3;
+    std::map<std::string, TrTap> m;
+    auto planes = [&](const std::string& name, const Planes* p, bool per_block, int cols, int col0 = 0) {
+        TrTap& e = m[name];
+        e.per_block = per_block;
+        for (int b = 0; b < (per_block ? 3 : 1); ++b) e.pl[b] = p[b];
+        e.cols = cols;
+        e.col0 = col0;
     };
-    for (const TLayer& l : t->L) wsize(l.conv);
-    wsize(t->att2);
-    t->wpart = k.f32(wmax);
-    t->aam_ws_bytes = aam_workspace_bytes(B, t->D, t->S);
-    t->aam_ws = k.cv.take(t->aam_ws_bytes);
+    auto vec = [&](const std::string& name, float* const* p, bool per_block, size_t count) {
+        TrTap& e = m[name];
+        e.per_block = per_block;
+        e.f32 = true;
+        for (int b = 0; b < (per_block ? 3 : 1); ++b) e.vec[b] = p[b];
+        e.count = count;
+    };
+    using NamedPlanes = std::initializer_list<std::pair<const char*, const Planes*>>;
+    using NamedVec = std::initializer_list<std::pair<const char*, float* const*>>;
+    // forward planes
+    planes("blocks.0", &f.Y0, false, C);
+    for (int b = 1; b <= 3; ++b) planes("blocks." + std::to_string(b), &f.OUTCAT, false, C, C * (b - 1));
+    planes("mfa", &f.M, false, C3);
+    planes("X0", &f.X0, false, t->cfg.input_size);
+    for (const auto& e : NamedPlanes{{"A0", &f.A0}, {"Y0", &f.Y0}}) planes(e.first, e.second, false, C);
+    for (const auto& e : NamedPlanes{{"OUTCAT", &f.OUTCAT}, {"Amfa", &f.Amfa}, {"M", &f.M}}) planes(e.first, e.second, false, C3);
+    for (const auto& e : NamedPlanes{{"Aatt", &f.Aatt}, {"A4", &f.A4}}) planes(e.first, e.second, false, t->att);
+    for (const auto& e : NamedPlanes{{"At1", f.At1}, {"Yt1", f.Yt1}, {"Ares", f.Ares}, {"RC", f.RC}, {"IN", f.IN}, {"At2", f.At2}, {"Yt2", f.Yt2}})
+        planes(e.first, e.second, true, C);
+    // gradient planes
+    planes("g:dZ0", &f.dZ0, false, C);
+    for (const auto& e : NamedPlanes{{"g:dOUTCAT", &f.dOUTCAT}, {"g:dMd", &f.dMd}, {"g:dMatt", &f.dMatt}, {"g:dZmfa", &f.dZmfa}, {"g:dlogits", &f.dlogits}})
+        planes(e.first, e.second, false, C3);
+    for (const auto& e : NamedPlanes{{"g:dZatt", &f.dZatt}, {"g:dA4", &f.dA4}}) planes(e.first, e.second, false, t->att);
+    for (const auto& e : NamedPlanes{{"g:D", f.Dbuf}, {"g:dZt2", f.dZt2}, {"g:dRC", f.dRC}, {"g:dZres", f.dZres}, {"g:DIN", f.DIN}, {"g:dZt1", f.dZt1},
+                                     {"g:dXt1", f.dXt1}})
+        planes(e.first, e.second, true, C);
+    // fp32 as stored
+    vec("asp", &f.pooled, false, size_t(B) * 2 * C3);
+    for (const auto& e : NamedVec{{"emb", &f.emb}, {"d_emb", &f.d_emb}}) vec(e.first, e.second, false, size_t(B) * t->D);
+    vec("logits", &f.logits, false, size_t(f.R) * C3);
+    for (const auto& e : NamedVec{{"gstat", &f.gstat}, {"dgs", &f.dgs}, {"pn", &f.pn}, {"dpn", &f.dpn}, {"dpooled", &f.dpooled}})
+        vec(e.first, e.second, false, size_t(B) * 2 * C3);
+    for (const auto& e : NamedVec{{"rs", &f.rs}, {"rb", &f.rb}}) vec(e.first, e.second, false, size_t(B) * C3);
+    for (const auto& e : NamedVec{{"dg2", &f.dg2}, {"ds", &f.ds}}) vec(e.first, e.second, false, size_t(B) * C);
+    vec("dg1", &f.dg1, false, size_t(B) * t->se);
+    for (const auto& e : NamedVec{{"se_s", f.se_s}, {"se_g2", f.se_g2}}) vec(e.first, e.second, true, size_t(B) * C);
+    vec("se_g1", f.se_g1, true, size_t(B) * t->se);
+    return m;
 }
 
 }  // namespace
 
-size_t trainer_workspace_bytes(Trainer* t, int B, int T) {
-    if (!t || B <= 0 || T <= 0) return 0;
-    TrCarve k;
-    tr_carve(t, k, B, T);
-    t->plan_ws = nullptr;  // carving overwrote the plan's buffer views
-    return mc_align_up(k.cv.off, 256);
+size_t Trainer::workspace_bytes(int B, int T) const {
+    if (B <= 0 || T <= 0) return 0;
+    WsCarver cv;
+    TrBuffers f;
+    tr_carve(this, cv, B, T, &f);
+    return mc_align_up(cv.off, 256);
 }
 
+size_t trainer_workspace_bytes(const Trainer* t, int B, int T) { return t ? t->workspace_bytes(B, T) : 0; }
+
 // ------------------------------------------------------------------------------------------------ plan
-static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+    Trainer* const t = this;
     PPV_REQUIRE(t->params, "trainer: call ppv_trainer_bind first");
     PPV_REQUIRE(T > 2 * t->P, "trainer: too few frames for the reflect padding");
-    TrCarve k;
-    tr_carve(t, k, B, T);
-    const size_t need = mc_align_up(k.cv.off, 256);
-    PPV_REQUIRE(ws && ws_bytes >= need, "trainer: workspace too small (see ppv_trainer_workspace_bytes)");
-    PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "trainer: workspace must be 256-byte aligned");
-    k = TrCarve();
-    k.cv.base = static_cast<uint8_t*>(ws);
-    tr_carve(t, k, B, T);
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
+    int rc = claim_workspace(B, T, ws, ws_bytes, st);
+    if (rc) return rc;
+    WsCarver cv;
+    cv.base = static_cast<uint8_t*>(ws);
+    TrBuffers& f = t->buf;
+    tr_carve(t, cv, B, T, &f);
+    t->taps = tr_tap_table(t, f, B);
     t->steps.clear();
-    const int C = t->C, C3 = t->C3, W = t->width, P = t->P, Tp = t->Tp;
-    const int M = int(t->R);
+    const int C = t->C, C3 = t->C3, W = t->width, P = t->P, Tp = f.Tp;
+    const int M = int(f.R);
     float* const par = t->params;
     float* const grd = t->grads;
-    int rc;
 
     auto push = [&](const TStep& s) { t->steps.push_back(s); };
     // forward conv: bias + ReLU -> post-activation planes (valid frames)
-    auto fwd_gemm = [&](const TConv& c, const std::vector<GemmSource>& srcs, const Planes& out, int out_col0, bool relu, const float* rowgrp,
+    auto fwd_gemm = [&](int li, const std::vector<GemmSource>& srcs, const Planes& out, int out_col0, bool relu, const float* rowgrp,
                         float* out_f32) -> int {
+        const TConv& c = t->conv(li);
         Epilogue ep;
         ep.bias = par + c.b_off;
         ep.rowgrp_bias = rowgrp;
@@ -409,7 +470,7 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         ep.T = T;
         TStep s;
         s.kind = TStep::GEMM;
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wf, M, c.Cout, ep, gemm_pick_bn(c.Cout));
+        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), f.layer[li].wf, M, c.Cout, ep, gemm_pick_bn(c.Cout));
         if (r) return r;
         push(s);
         return PPV_OK;
@@ -419,11 +480,11 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         for (int tp = 0; tp < c.taps; ++tp) v.push_back(GemmSource{x, col0, sign > 0 ? c.Cinp : c.Cout, sign * (tp - (c.taps - 1) / 2) * c.dil});
         return v;
     };
-    auto bn_fwd = [&](const TLayer& l, const Planes& a, int a_col0, const Planes& y, int y_col0, int tanh_, const Planes* add, int add_col0,
+    auto bn_fwd = [&](int li, const Planes& a, int a_col0, const Planes& y, int y_col0, int tanh_, const Planes* add, int add_col0,
                       const Planes* out2, int out2_col0) {
         TStep s;
         s.kind = TStep::BN_FWD;
-        s.layer = int(&l - t->L.data());
+        s.layer = li;
         s.p0 = a;
         s.c0 = a_col0;
         s.ap.y = y;
@@ -438,7 +499,8 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         push(s);
     };
     // data gradient: dx_pad[r, cin] = sum_tap dz[r - off_tap, :] . W[:, cin, tap]  -> planes on every row
-    auto dgrad_gemm = [&](const TConv& c, const Planes& dz, int dz_col0, const Planes& out, int out_col0) -> int {
+    auto dgrad_gemm = [&](int li, const Planes& dz, int dz_col0, const Planes& out, int out_col0) -> int {
+        const TConv& c = t->conv(li);
         Epilogue ep;
         ep.out_mode = OUT_PLANES;
         ep.out = out.base;
@@ -448,17 +510,18 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         TStep s;
         s.kind = TStep::GEMM;
         std::vector<GemmSource> srcs = taps_of(c, dz, dz_col0, -1);
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), c.wd, M, c.Cinp, ep, gemm_pick_bn(c.Cinp));
+        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), f.layer[li].wd, M, c.Cinp, ep, gemm_pick_bn(c.Cinp));
         if (r) return r;
         push(s);
         return PPV_OK;
     };
     // weight gradient: dz^T -> TA; one row-shifted transpose of the layer input per tap -> TB rows [tap * Cinp, ...); ONE GEMM
     // [Cout] x [taps * Cinp] over the frames (split-K partials); unpack into the flat gradient buffer
-    auto wgrad = [&](int layer, const TConv& c, const Planes& dz, int dz_col0, const std::vector<TStep::Tr>& xs) -> int {
+    auto wgrad = [&](int li, const Planes& dz, int dz_col0, const std::vector<TStep::Tr>& xs) -> int {
+        const TConv& c = t->conv(li);
         TStep s;
         s.kind = TStep::WGRAD;
-        s.layer = layer;
+        s.layer = li;
         s.trs.push_back(TStep::Tr{dz, dz_col0, c.Cout, 0, 0, 0});
         for (const TStep::Tr& x : xs) {
             TStep::Tr tr{x.in, x.col0, x.C, x.row0, 1, -((c.taps - 1) / 2) * c.dil};
@@ -468,15 +531,13 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
             s.trs.push_back(tr);
         }
         const int N = c.taps * c.Cinp;
-        const int BNw = gemm_pick_bn(N);
-        const int mt = (c.Cout + 127) / 128, nt = (N + BNw - 1) / BNw;
-        const int splits = std::max(1, std::min((t->num_sms + mt * nt - 1) / (mt * nt), int((t->Rp + 63) / 64)));
+        const WgradSplit sp = tr_wgrad_split(t, c, f.Rp);
         GemmParams gp;
-        int r = gemm_build_wgrad(&gp, t->TA, t->TB, c.Cout, N, 0, 0, splits, t->wpart, N, 0, int64_t(mt) * 128, BNw);
+        int r = gemm_build_wgrad(&gp, f.TA, f.TB, c.Cout, N, 0, 0, sp.splits, f.wpart, N, 0, sp.Mpad, sp.BN);
         if (r) return r;
         s.wg.push_back(gp);
         s.a = gp.lin_splits;
-        s.b = mt * 128;
+        s.b = sp.Mpad;
         push(s);
         return PPV_OK;
     };
@@ -510,36 +571,36 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
     simple(TStep::REPACK);
     simple(TStep::PACK);
     {
-        const TLayer& l = t->L[t->l_conv0];
-        rc = fwd_gemm(l.conv, taps_of(l.conv, t->X0, 0, +1), t->A0, 0, true, nullptr, nullptr);
+        const int li = t->l_conv0;
+        rc = fwd_gemm(li, taps_of(t->conv(li), f.X0, 0, +1), f.A0, 0, true, nullptr, nullptr);
         if (rc) return rc;
-        bn_fwd(l, t->A0, 0, t->Y0, 0, 0, nullptr, 0, nullptr, 0);
+        bn_fwd(li, f.A0, 0, f.Y0, 0, 0, nullptr, 0, nullptr, 0);
     }
     for (int b = 0; b < 3; ++b) {
-        const Planes u = b == 0 ? t->Y0 : t->OUTCAT;
+        const Planes u = b == 0 ? f.Y0 : f.OUTCAT;
         const int uc = b == 0 ? 0 : C * (b - 1);
         {
-            const TLayer& l = t->L[t->l_tdnn1[b]];
-            rc = fwd_gemm(l.conv, {GemmSource{u, uc, C, 0}}, t->At1[b], 0, true, nullptr, nullptr);
+            const int li = t->l_tdnn1[b];
+            rc = fwd_gemm(li, {GemmSource{u, uc, C, 0}}, f.At1[b], 0, true, nullptr, nullptr);
             if (rc) return rc;
-            bn_fwd(l, t->At1[b], 0, t->Yt1[b], 0, 0, nullptr, 0, nullptr, 0);
+            bn_fwd(li, f.At1[b], 0, f.Yt1[b], 0, 0, nullptr, 0, nullptr, 0);
         }
         for (int j = 1; j < 8; ++j) {
-            const TLayer& l = t->L[t->l_res[b][j]];
-            const Planes& xin = j == 1 ? t->Yt1[b] : t->IN[b];
-            rc = fwd_gemm(l.conv, taps_of(l.conv, xin, W * j, +1), t->Ares[b], W * j, true, nullptr, nullptr);
+            const int li = t->l_res[b][j];
+            const Planes& xin = j == 1 ? f.Yt1[b] : f.IN[b];
+            rc = fwd_gemm(li, taps_of(t->conv(li), xin, W * j, +1), f.Ares[b], W * j, true, nullptr, nullptr);
             if (rc) return rc;
             // r_j -> RC window j; in_{j+1} = r_j + chunk_{j+1}(tdnn1 output) -> IN window j+1   (ecapa_tdnn.py:41-45)
             if (j < 7)
-                bn_fwd(l, t->Ares[b], W * j, t->RC[b], W * j, 0, &t->Yt1[b], W * (j + 1), &t->IN[b], W * (j + 1));
+                bn_fwd(li, f.Ares[b], W * j, f.RC[b], W * j, 0, &f.Yt1[b], W * (j + 1), &f.IN[b], W * (j + 1));
             else
-                bn_fwd(l, t->Ares[b], W * j, t->RC[b], W * j, 0, nullptr, 0, nullptr, 0);
+                bn_fwd(li, f.Ares[b], W * j, f.RC[b], W * j, 0, nullptr, 0, nullptr, 0);
         }
         {
-            const TLayer& l = t->L[t->l_tdnn2[b]];
-            rc = fwd_gemm(l.conv, {GemmSource{t->Yt1[b], 0, W, 0}, GemmSource{t->RC[b], W, C - W, 0}}, t->At2[b], 0, true, nullptr, nullptr);
+            const int li = t->l_tdnn2[b];
+            rc = fwd_gemm(li, {GemmSource{f.Yt1[b], 0, W, 0}, GemmSource{f.RC[b], W, C - W, 0}}, f.At2[b], 0, true, nullptr, nullptr);
             if (rc) return rc;
-            bn_fwd(l, t->At2[b], 0, t->Yt2[b], 0, 0, nullptr, 0, nullptr, 0);
+            bn_fwd(li, f.At2[b], 0, f.Yt2[b], 0, 0, nullptr, 0, nullptr, 0);
         }
         simple(TStep::SE_FWD, b);
         {
@@ -552,18 +613,16 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         }
     }
     {
-        const TLayer& l = t->L[t->l_mfa];
-        rc = fwd_gemm(l.conv, {GemmSource{t->OUTCAT, 0, C3, 0}}, t->Amfa, 0, true, nullptr, nullptr);
+        rc = fwd_gemm(t->l_mfa, {GemmSource{f.OUTCAT, 0, C3, 0}}, f.Amfa, 0, true, nullptr, nullptr);
         if (rc) return rc;
-        bn_fwd(l, t->Amfa, 0, t->M, 0, 0, nullptr, 0, nullptr, 0);
+        bn_fwd(t->l_mfa, f.Amfa, 0, f.M, 0, 0, nullptr, 0, nullptr, 0);
     }
     simple(TStep::ASP_HEAD_FWD);  // global stats -> per-utterance bias of the attention TDNN
     {
-        const TLayer& l = t->L[t->l_att1];
-        rc = fwd_gemm(l.conv, {GemmSource{t->M, 0, C3, 0}}, t->Aatt, 0, true, t->fold, nullptr);
+        rc = fwd_gemm(t->l_att1, {GemmSource{f.M, 0, C3, 0}}, f.Aatt, 0, true, f.fold, nullptr);
         if (rc) return rc;
-        bn_fwd(l, t->Aatt, 0, t->A4, 0, 1, nullptr, 0, nullptr, 0);
-        rc = fwd_gemm(t->att2, {GemmSource{t->A4, 0, t->att, 0}}, Planes(), 0, false, nullptr, t->logits);
+        bn_fwd(t->l_att1, f.Aatt, 0, f.A4, 0, 1, nullptr, 0, nullptr, 0);
+        rc = fwd_gemm(t->l_att2(), {GemmSource{f.A4, 0, t->att, 0}}, Planes(), 0, false, nullptr, f.logits);
         if (rc) return rc;
     }
     simple(TStep::ASP_TAIL_FWD);  // softmax pooling, asp_bn (batch statistics), fc
@@ -577,60 +636,58 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
         TStep s;
         s.kind = TStep::COLSUM;
         s.gl.n = 1;
-        s.gl.s[0] = src1(t->dlogits, 0, 0);
+        s.gl.s[0] = src1(f.dlogits, 0, 0);
         s.C = C3;
         s.f0 = grd + t->att2.b_off;
         push(s);
-        rc = wgrad(-1, t->att2, t->dlogits, 0, {TStep::Tr{t->A4, 0, t->att, 0, 1}});
+        rc = wgrad(t->l_att2(), f.dlogits, 0, {TStep::Tr{f.A4, 0, t->att, 0, 1}});
         if (rc) return rc;
-        rc = dgrad_gemm(t->att2, t->dlogits, 0, t->dA4, 0);
+        rc = dgrad_gemm(t->l_att2(), f.dlogits, 0, f.dA4, 0);
         if (rc) return rc;
     }
     {
         // attention TDNN: tanh, BN, ReLU backward; frame-level weight / data gradients; per-utterance context gradients
         GradSrcList gl;
         gl.n = 1;
-        gl.s[0] = src1(t->dA4, 0, 0);
-        gl.s[0].dtanh = t->A4;
-        bn_bwd(t->l_att1, gl, t->Aatt, 0, t->dZatt, 0);
+        gl.s[0] = src1(f.dA4, 0, 0);
+        gl.s[0].dtanh = f.A4;
+        bn_bwd(t->l_att1, gl, f.Aatt, 0, f.dZatt, 0);
         simple(TStep::ASP_CTX_BWD);
-        const TConv& c = t->L[t->l_att1].conv;
-        rc = wgrad(t->l_att1, c, t->dZatt, 0, {TStep::Tr{t->M, 0, C3, 0, 1}});
+        rc = wgrad(t->l_att1, f.dZatt, 0, {TStep::Tr{f.M, 0, C3, 0, 1}});
         if (rc) return rc;
-        rc = dgrad_gemm(c, t->dZatt, 0, t->dMatt, 0);
+        rc = dgrad_gemm(t->l_att1, f.dZatt, 0, f.dMatt, 0);
         if (rc) return rc;
     }
     {
         // MFA: d(M) = ASP direct + attention path + global-context statistics (as row scale / bias on M itself)
         GradSrcList gl;
         gl.n = 3;
-        gl.s[0] = src1(t->dMd, 0, 0);
-        gl.s[1] = src1(t->dMatt, 0, 0);
-        gl.s[2] = src1(t->M, 0, 0);
-        gl.s[2].rowscale = t->rs;
-        gl.s[2].rowbias = t->rb;
+        gl.s[0] = src1(f.dMd, 0, 0);
+        gl.s[1] = src1(f.dMatt, 0, 0);
+        gl.s[2] = src1(f.M, 0, 0);
+        gl.s[2].rowscale = f.rs;
+        gl.s[2].rowbias = f.rb;
         gl.s[2].row_ld = C3;
-        bn_bwd(t->l_mfa, gl, t->Amfa, 0, t->dZmfa, 0);
-        const TConv& c = t->L[t->l_mfa].conv;
-        rc = wgrad(t->l_mfa, c, t->dZmfa, 0, {TStep::Tr{t->OUTCAT, 0, C3, 0, 1}});
+        bn_bwd(t->l_mfa, gl, f.Amfa, 0, f.dZmfa, 0);
+        rc = wgrad(t->l_mfa, f.dZmfa, 0, {TStep::Tr{f.OUTCAT, 0, C3, 0, 1}});
         if (rc) return rc;
-        rc = dgrad_gemm(c, t->dZmfa, 0, t->dOUTCAT, 0);
+        rc = dgrad_gemm(t->l_mfa, f.dZmfa, 0, f.dOUTCAT, 0);
         if (rc) return rc;
     }
     for (int b = 2; b >= 0; --b) {
-        const Planes u = b == 0 ? t->Y0 : t->OUTCAT;
+        const Planes u = b == 0 ? f.Y0 : f.OUTCAT;
         const int uc = b == 0 ? 0 : C * (b - 1);
-        const Planes& D = t->Dbuf[b];
+        const Planes& D = f.Dbuf[b];
         {
             // d(out_b) = MFA window + (next block: tdnn1 data gradient + its own residual gradient)
             TStep s;
             s.kind = TStep::GRAD_SUM;
             s.gl.n = 1;
-            s.gl.s[0] = src1(t->dOUTCAT, C * b, 0);
+            s.gl.s[0] = src1(f.dOUTCAT, C * b, 0);
             if (b < 2) {
                 s.gl.n = 3;
-                s.gl.s[1] = src1(t->dXt1[b + 1], 0, 0);
-                s.gl.s[2] = src1(t->Dbuf[b + 1], 0, 0);
+                s.gl.s[1] = src1(f.dXt1[b + 1], 0, 0);
+                s.gl.s[2] = src1(f.Dbuf[b + 1], 0, 0);
             }
             s.C = C;
             s.p0 = D;
@@ -642,30 +699,28 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
             GradSrcList gl;
             gl.n = 1;
             gl.s[0] = src1(D, 0, 0);
-            gl.s[0].rowscale = t->se_g2[b];
-            gl.s[0].rowbias = t->ds;
+            gl.s[0].rowscale = f.se_g2[b];
+            gl.s[0].rowbias = f.ds;
             gl.s[0].row_ld = C;
-            bn_bwd(t->l_tdnn2[b], gl, t->At2[b], 0, t->dZt2[b], 0);
-            const TConv& c = t->L[t->l_tdnn2[b]].conv;
-            rc = wgrad(t->l_tdnn2[b], c, t->dZt2[b], 0, {TStep::Tr{t->Yt1[b], 0, W, 0, 1}, TStep::Tr{t->RC[b], W, C - W, W, 1}});
+            bn_bwd(t->l_tdnn2[b], gl, f.At2[b], 0, f.dZt2[b], 0);
+            rc = wgrad(t->l_tdnn2[b], f.dZt2[b], 0, {TStep::Tr{f.Yt1[b], 0, W, 0, 1}, TStep::Tr{f.RC[b], W, C - W, W, 1}});
             if (rc) return rc;
-            rc = dgrad_gemm(c, t->dZt2[b], 0, t->dRC[b], 0);
+            rc = dgrad_gemm(t->l_tdnn2[b], f.dZt2[b], 0, f.dRC[b], 0);
             if (rc) return rc;
         }
         for (int j = 7; j >= 1; --j) {
             GradSrcList gl;
             gl.n = 1;
-            gl.s[0] = src1(t->dRC[b], W * j, 0);
+            gl.s[0] = src1(f.dRC[b], W * j, 0);
             if (j < 7) {
                 gl.n = 2;
-                gl.s[1] = src1(t->DIN[b], W * (j + 1), 1);
+                gl.s[1] = src1(f.DIN[b], W * (j + 1), 1);
             }
             const int li = t->l_res[b][j];
-            bn_bwd(li, gl, t->Ares[b], W * j, t->dZres[b], W * j);
-            const TConv& c = t->L[li].conv;
-            rc = wgrad(li, c, t->dZres[b], W * j, {TStep::Tr{j == 1 ? t->Yt1[b] : t->IN[b], W * j, W, 0, 1}});
+            bn_bwd(li, gl, f.Ares[b], W * j, f.dZres[b], W * j);
+            rc = wgrad(li, f.dZres[b], W * j, {TStep::Tr{j == 1 ? f.Yt1[b] : f.IN[b], W * j, W, 0, 1}});
             if (rc) return rc;
-            rc = dgrad_gemm(c, t->dZres[b], W * j, t->DIN[b], W * j);
+            rc = dgrad_gemm(li, f.dZres[b], W * j, f.DIN[b], W * j);
             if (rc) return rc;
         }
         {
@@ -673,37 +728,32 @@ static int tr_build_plan(Trainer* t, int B, int T, void* ws, size_t ws_bytes, cu
             TStep s;
             s.kind = TStep::GRAD_SUM;
             s.gl.n = 1;
-            s.gl.s[0] = src1(t->dRC[b], 0, 0);
+            s.gl.s[0] = src1(f.dRC[b], 0, 0);
             s.C = W;
-            s.p0 = t->DIN[b];
+            s.p0 = f.DIN[b];
             s.c0 = 0;
             push(s);
         }
         {
             GradSrcList gl;
             gl.n = 1;
-            gl.s[0] = src1(t->DIN[b], 0, 1);
-            bn_bwd(t->l_tdnn1[b], gl, t->At1[b], 0, t->dZt1[b], 0);
-            const TConv& c = t->L[t->l_tdnn1[b]].conv;
-            rc = wgrad(t->l_tdnn1[b], c, t->dZt1[b], 0, {TStep::Tr{u, uc, C, 0, 1}});
+            gl.s[0] = src1(f.DIN[b], 0, 1);
+            bn_bwd(t->l_tdnn1[b], gl, f.At1[b], 0, f.dZt1[b], 0);
+            rc = wgrad(t->l_tdnn1[b], f.dZt1[b], 0, {TStep::Tr{u, uc, C, 0, 1}});
             if (rc) return rc;
-            rc = dgrad_gemm(c, t->dZt1[b], 0, t->dXt1[b], 0);
+            rc = dgrad_gemm(t->l_tdnn1[b], f.dZt1[b], 0, f.dXt1[b], 0);
             if (rc) return rc;
         }
     }
     {
         GradSrcList gl;
         gl.n = 2;
-        gl.s[0] = src1(t->dXt1[0], 0, 0);
-        gl.s[1] = src1(t->Dbuf[0], 0, 0);
-        bn_bwd(t->l_conv0, gl, t->A0, 0, t->dZ0, 0);
-        const TConv& c = t->L[t->l_conv0].conv;
-        rc = wgrad(t->l_conv0, c, t->dZ0, 0, {TStep::Tr{t->X0, 0, t->Fp, 0, 1}});
+        gl.s[0] = src1(f.dXt1[0], 0, 0);
+        gl.s[1] = src1(f.Dbuf[0], 0, 0);
+        bn_bwd(t->l_conv0, gl, f.A0, 0, f.dZ0, 0);
+        rc = wgrad(t->l_conv0, f.dZ0, 0, {TStep::Tr{f.X0, 0, t->Fp, 0, 1}});
         if (rc) return rc;
     }
-    t->plan_ws = ws;
-    t->plan_B = B;
-    t->plan_T = T;
     return PPV_OK;
 }
 
@@ -712,18 +762,13 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
                              float label_smoothing, float* loss_out, float* logits_out, void* ws, size_t ws_bytes, cudaStream_t st) {
     PPV_REQUIRE(t && feat && labels, "trainer_forward_backward: null argument");
     PPV_REQUIRE(B > 1 && T > 0, "trainer_forward_backward: batch of at least 2 required (batch statistics)");
-    if (t->plan_ws != ws || t->plan_B != B || t->plan_T != T) {
-        int rc = tr_build_plan(t, B, T, ws, ws_bytes, st);
-        if (rc) {
-            t->plan_ws = nullptr;
-            return rc;
-        }
-    }
+    int rc = t->update_plan(B, T, ws, ws_bytes, st);
+    if (rc) return rc;
+    const TrBuffers& f = t->buf;
     float* const par = t->params;
     float* const grd = t->grads;
     float* const sta = t->stats;
-    const int C = t->C, C3 = t->C3, P = t->P, Tp = t->Tp, se = t->se, att = t->att, D = t->D;
-    int rc = PPV_OK;
+    const int C = t->C, C3 = t->C3, P = t->P, Tp = f.Tp, se = t->se, att = t->att, D = t->D;
     static const bool debug_sync = getenv("PPV_TRAIN_DEBUG") != nullptr;  // localise a faulting kernel: sync after every step
     int step_idx = 0;
     for (const TStep& s : t->steps) {
@@ -736,125 +781,124 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
         ++step_idx;
         switch (s.kind) {
             case TStep::REPACK: {
-                for (const TLayer& l : t->L) {
-                    rc = tr_repack_conv(par + l.conv.w_off, int64_t(l.conv.CinTotal) * l.conv.taps, l.conv.Cout, l.conv.Cin, l.conv.Cinp, l.conv.taps,
-                                        l.conv.wf, l.conv.dgrad ? l.conv.wd : Planes(), st);
-                    if (rc) return rc;
+                for (int l = 0; l <= t->l_att2() && !rc; ++l) {
+                    const TConv& c = t->conv(l);
+                    rc = tr_repack_conv(par + c.w_off, int64_t(c.CinTotal) * c.taps, c.Cout, c.Cin, c.Cinp, c.taps, f.layer[l].wf, f.layer[l].wd, st);
                 }
-                rc = tr_repack_conv(par + t->att2.w_off, t->att2.CinTotal, t->att2.Cout, t->att2.Cin, t->att2.Cinp, 1, t->att2.wf, t->att2.wd, st);
                 break;
             }
-            case TStep::PACK: rc = launch_pack_features(feat, B, T, t->cfg.input_size, t->X0, P, Tp, st); break;
+            case TStep::PACK: rc = launch_pack_features(feat, B, T, t->cfg.input_size, f.X0, P, Tp, st); break;
             case TStep::GEMM: rc = gemm_launch(s.gp, t->precision, t->num_sms, st); break;
             case TStep::BN_FWD: {
                 const TBN& bn = t->L[s.layer].bn;
-                rc = tr_bn_forward(s.p0, s.c0, bn.C, B, T, P, Tp, TR_BN_EPS, TR_BN_MOMENTUM, par + bn.g_off, par + bn.b_off, bn.mean, bn.rstd, bn.scale,
-                                   bn.shift, sta + bn.rm_off, sta + bn.rv_off, t->part, s.ap, t->num_sms, st);
+                const TrBuffers::Layer& w = f.layer[s.layer];
+                rc = tr_bn_forward(s.p0, s.c0, bn.C, B, T, P, Tp, TR_BN_EPS, TR_BN_MOMENTUM, par + bn.g_off, par + bn.b_off, w.mean, w.rstd, w.scale,
+                                   w.shift, sta + bn.rm_off, sta + bn.rv_off, f.part, s.ap, t->num_sms, st);
                 break;
             }
             case TStep::SE_FWD: {
                 const int b = s.a;
-                rc = launch_colstats(t->Yt2[b], 0, C, B, T, P, Tp, 0, 0.f, t->se_s[b], Planes(), st);
+                rc = launch_colstats(f.Yt2[b], 0, C, B, T, P, Tp, 0, 0.f, f.se_s[b], Planes(), st);
                 if (rc) return rc;
-                rc = tr_dense_fwd(t->se_s[b], C, par + t->se1_w[b], C, par + t->se1_b[b], B, se, C, 1, t->se_g1[b], se, st);
+                rc = tr_dense_fwd(f.se_s[b], C, par + t->se1_w[b], C, par + t->se1_b[b], B, se, C, 1, f.se_g1[b], se, st);
                 if (rc) return rc;
-                rc = tr_dense_fwd(t->se_g1[b], se, par + t->se2_w[b], se, par + t->se2_b[b], B, C, se, 2, t->se_g2[b], C, st);
+                rc = tr_dense_fwd(f.se_g1[b], se, par + t->se2_w[b], se, par + t->se2_b[b], B, C, se, 2, f.se_g2[b], C, st);
                 break;
             }
             case TStep::SCALE_RES:
-                rc = launch_se_scale_res(t->Yt2[s.a], t->se_g2[s.a], s.p0, s.c0, t->OUTCAT, C * s.a, C, Tp, t->R, t->num_sms, st);
+                rc = launch_se_scale_res(f.Yt2[s.a], f.se_g2[s.a], s.p0, s.c0, f.OUTCAT, C * s.a, C, Tp, f.R, t->num_sms, st);
                 break;
             case TStep::ASP_HEAD_FWD: {
-                rc = launch_colstats(t->M, 0, C3, B, T, P, Tp, 1, TR_ASP_EPS, nullptr, t->gstat_pl, st);
+                rc = launch_colstats(f.M, 0, C3, B, T, P, Tp, 1, TR_ASP_EPS, nullptr, f.gstat_pl, st);
                 if (rc) return rc;
-                rc = launch_planes_to_f32(t->gstat_pl, 0, 2 * C3, B, 1, 0, 1, t->gstat, st);
+                rc = launch_planes_to_f32(f.gstat_pl, 0, 2 * C3, B, 1, 0, 1, f.gstat, st);
                 if (rc) return rc;
                 const TConv& c = t->L[t->l_att1].conv;  // weight [att][3*C3]: columns C3.. multiply [mean | std]
-                rc = tr_dense_fwd(t->gstat, 2 * C3, par + c.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, t->fold, att, st);
+                rc = tr_dense_fwd(f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, f.fold, att, st);
                 break;
             }
             case TStep::ASP_TAIL_FWD: {
-                rc = launch_asp_pool(t->logits, C3, t->M, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), t->pooled, st);
+                rc = launch_asp_pool(f.logits, C3, f.M, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), f.pooled, st);
                 if (rc) return rc;
-                rc = tr_bn1d_fwd(t->pooled, B, 2 * C3, TR_BN_EPS, TR_BN_MOMENTUM, par + t->aspbn_g, par + t->aspbn_b, t->pn, t->aspbn_mean, t->aspbn_rstd,
+                rc = tr_bn1d_fwd(f.pooled, B, 2 * C3, TR_BN_EPS, TR_BN_MOMENTUM, par + t->aspbn_g, par + t->aspbn_b, f.pn, f.aspbn_mean, f.aspbn_rstd,
                                  sta + t->aspbn_rm, sta + t->aspbn_rv, st);
                 if (rc) return rc;
-                rc = tr_dense_fwd(t->pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, t->emb, D, st);
+                rc = tr_dense_fwd(f.pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, f.emb, D, st);
                 break;
             }
             case TStep::LOSS:
-                rc = aam_forward(t->emb, par + t->cls_w, labels, B, D, t->S, margin, scale, easy_margin, label_smoothing, t->cls_logits, t->loss,
-                                 t->aam_ws, t->aam_ws_bytes, st);
+                rc = aam_forward(f.emb, par + t->cls_w, labels, B, D, t->S, margin, scale, easy_margin, label_smoothing, f.cls_logits, f.loss,
+                                 f.aam_ws, f.aam_ws_bytes, st);
                 break;
             case TStep::HEAD_BWD: {
-                rc = aam_backward(t->emb, par + t->cls_w, labels, t->cls_logits, B, D, t->S, margin, scale, easy_margin, label_smoothing, t->d_emb,
-                                  grd + t->cls_w, t->aam_ws, t->aam_ws_bytes, st);
+                rc = aam_backward(f.emb, par + t->cls_w, labels, f.cls_logits, B, D, t->S, margin, scale, easy_margin, label_smoothing, f.d_emb,
+                                  grd + t->cls_w, f.aam_ws, f.aam_ws_bytes, st);
                 if (rc) return rc;
-                rc = tr_dense_bwd(t->d_emb, D, t->pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, t->dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b, st);
+                rc = tr_dense_bwd(f.d_emb, D, f.pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, f.dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b, st);
                 if (rc) return rc;
-                rc = tr_bn1d_bwd(t->dpn, t->pooled, B, 2 * C3, par + t->aspbn_g, t->aspbn_mean, t->aspbn_rstd, t->dpooled, grd + t->aspbn_g,
+                rc = tr_bn1d_bwd(f.dpn, f.pooled, B, 2 * C3, par + t->aspbn_g, f.aspbn_mean, f.aspbn_rstd, f.dpooled, grd + t->aspbn_g,
                                  grd + t->aspbn_b, st);
                 break;
             }
             case TStep::ASP_BWD:
-                rc = tr_asp_bwd(t->logits, C3, t->M, C3, B, T, P, Tp, TR_ASP_EPS, t->pooled, t->dpooled, t->dlogits, t->dMd, st);
+                rc = tr_asp_bwd(f.logits, C3, f.M, C3, B, T, P, Tp, TR_ASP_EPS, f.pooled, f.dpooled, f.dlogits, f.dMd, st);
                 break;
-            case TStep::COLSUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, Planes(), 0, t->part, s.f0, st); break;
-            case TStep::GRAD_SUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, s.p0, s.c0, t->part, nullptr, st); break;
+            case TStep::COLSUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, Planes(), 0, f.part, s.f0, st); break;
+            case TStep::GRAD_SUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, s.p0, s.c0, f.part, nullptr, st); break;
             case TStep::BN_BWD: {
                 const TLayer& l = t->L[s.layer];
-                rc = tr_bn_backward(s.gl, s.p0, s.c0, l.bn.C, B, T, P, Tp, l.bn.mean, l.bn.rstd, par + l.bn.g_off, grd + l.bn.g_off, grd + l.bn.b_off,
-                                    s.p1, s.c1, grd + l.conv.b_off, t->part, t->part_elems, st, s.a);
+                rc = tr_bn_backward(s.gl, s.p0, s.c0, l.bn.C, B, T, P, Tp, f.layer[s.layer].mean, f.layer[s.layer].rstd, par + l.bn.g_off, grd + l.bn.g_off, grd + l.bn.b_off,
+                                    s.p1, s.c1, grd + l.conv.b_off, f.part, f.part_elems, st, s.a);
                 break;
             }
             case TStep::ASP_CTX_BWD: {
-                // t->part holds sum_t dz per utterance [B][att] (left by the BN backward of the attention TDNN)
+                // f.part holds sum_t dz per utterance [B][att] (left by the BN backward of the attention TDNN)
                 const TConv& c = t->L[t->l_att1].conv;
-                rc = tr_dense_bwd(t->part, att, t->gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, t->dgs, 2 * C3, grd + c.w_off + C3, 3 * C3,
+                rc = tr_dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3,
                                   nullptr, st);
                 if (rc) return rc;
-                rc = tr_asp_global_bwd(t->gstat, t->dgs, B, C3, T, TR_ASP_EPS, t->rs, t->rb, st);
+                rc = tr_asp_global_bwd(f.gstat, f.dgs, B, C3, T, TR_ASP_EPS, f.rs, f.rb, st);
                 break;
             }
             case TStep::SE_BWD: {
                 const int b = s.a;
                 GradSrcList gl;
                 gl.n = 1;
-                gl.s[0].t = t->Dbuf[b];
-                rc = tr_grad_dot(gl, t->Yt2[b], 0, C, B, T, P, Tp, t->dg2, st);
+                gl.s[0].t = f.Dbuf[b];
+                rc = tr_grad_dot(gl, f.Yt2[b], 0, C, B, T, P, Tp, f.dg2, st);
                 if (rc) return rc;
-                rc = tr_act_bwd(t->dg2, t->se_g2[b], int64_t(B) * C, 2, 0.f, st);
+                rc = tr_act_bwd(f.dg2, f.se_g2[b], int64_t(B) * C, 2, 0.f, st);
                 if (rc) return rc;
-                rc = tr_dense_bwd(t->dg2, C, t->se_g1[b], se, par + t->se2_w[b], se, B, C, se, t->dg1, se, grd + t->se2_w[b], se, grd + t->se2_b[b], st);
+                rc = tr_dense_bwd(f.dg2, C, f.se_g1[b], se, par + t->se2_w[b], se, B, C, se, f.dg1, se, grd + t->se2_w[b], se, grd + t->se2_b[b], st);
                 if (rc) return rc;
-                rc = tr_act_bwd(t->dg1, t->se_g1[b], int64_t(B) * se, 1, 0.f, st);
+                rc = tr_act_bwd(f.dg1, f.se_g1[b], int64_t(B) * se, 1, 0.f, st);
                 if (rc) return rc;
-                rc = tr_dense_bwd(t->dg1, se, t->se_s[b], C, par + t->se1_w[b], C, B, se, C, t->ds, C, grd + t->se1_w[b], C, grd + t->se1_b[b], st);
+                rc = tr_dense_bwd(f.dg1, se, f.se_s[b], C, par + t->se1_w[b], C, B, se, C, f.ds, C, grd + t->se1_w[b], C, grd + t->se1_b[b], st);
                 if (rc) return rc;
-                rc = tr_act_bwd(t->ds, nullptr, int64_t(B) * C, 0, 1.f / float(T), st);
+                rc = tr_act_bwd(f.ds, nullptr, int64_t(B) * C, 0, 1.f / float(T), st);
                 break;
             }
             case TStep::WGRAD: {
-                const TConv& c = s.layer >= 0 ? t->L[s.layer].conv : t->att2;
+                const TConv& c = t->conv(s.layer);
                 for (const TStep::Tr& tr : s.trs) {
-                    Planes dst = tr.which == 0 ? t->TA : t->TB;
+                    Planes dst = tr.which == 0 ? f.TA : f.TB;
                     dst.base += int64_t(tr.row0) * dst.ld;
                     dst.rows -= tr.row0;
-                    rc = tr_transpose(tr.in, tr.col0, tr.C, t->R, dst, tr.shift, st, tr.ntaps, tr.shift_step, tr.row_step);
+                    rc = tr_transpose(tr.in, tr.col0, tr.C, f.R, dst, tr.shift, st, tr.ntaps, tr.shift_step, tr.row_step);
                     if (rc) return rc;
                 }
                 for (const GemmParams& gp : s.wg) {
                     rc = gemm_launch(gp, t->precision, t->num_sms, st);
                     if (rc) return rc;
                 }
-                rc = tr_wgrad_unpack(t->wpart, s.a, s.b, c.Cout, c.Cin, c.Cinp, c.taps, grd + c.w_off, int64_t(c.CinTotal) * c.taps, st);
+                rc = tr_wgrad_unpack(f.wpart, s.a, s.b, c.Cout, c.Cin, c.Cinp, c.taps, grd + c.w_off, int64_t(c.CinTotal) * c.taps, st);
                 break;
             }
         }
         if (rc) return rc;
     }
-    if (loss_out) PPV_CUDA_OK(cudaMemcpyAsync(loss_out, t->loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (logits_out) PPV_CUDA_OK(cudaMemcpyAsync(logits_out, t->cls_logits, size_t(B) * t->S * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (loss_out) PPV_CUDA_OK(cudaMemcpyAsync(loss_out, f.loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (logits_out) PPV_CUDA_OK(cudaMemcpyAsync(logits_out, f.cls_logits, size_t(B) * t->S * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return PPV_OK;
 }
 
@@ -873,7 +917,6 @@ int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems,
     std::string n(name);
     const bool padded = n.rfind("pad:", 0) == 0;
     if (padded) n = n.substr(4);
-    const int B = t->plan_B, T = t->plan_T, C = t->C, C3 = t->C3;
     int b = -1;  // block suffix
     const size_t colon = n.rfind(':');
     if (colon != std::string::npos && colon + 2 == n.size() && n.back() >= '0' && n.back() <= '9') {
@@ -881,90 +924,19 @@ int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems,
         n.resize(colon);
         PPV_REQUIRE(b < 3, "trainer_read_tap: bad block");
     }
-    const bool per_block = b >= 0;
-    const int bk = per_block ? b : 0;
-    auto unknown = [&]() { return fail(PPV_EINVAL, std::string("trainer_read_tap: unknown tap ") + name); };
-
-    const float* vec = nullptr;
-    size_t cnt = 0;
-    bool vec_block = false;
-    if (n == "asp") vec = t->pooled, cnt = size_t(B) * 2 * C3;
-    else if (n == "emb") vec = t->emb, cnt = size_t(B) * t->D;
-    else if (n == "d_emb") vec = t->d_emb, cnt = size_t(B) * t->D;
-    else if (n == "logits") vec = t->logits, cnt = size_t(t->R) * C3;
-    else if (n == "gstat") vec = t->gstat, cnt = size_t(B) * 2 * C3;
-    else if (n == "dgs") vec = t->dgs, cnt = size_t(B) * 2 * C3;
-    else if (n == "pn") vec = t->pn, cnt = size_t(B) * 2 * C3;
-    else if (n == "dpn") vec = t->dpn, cnt = size_t(B) * 2 * C3;
-    else if (n == "dpooled") vec = t->dpooled, cnt = size_t(B) * 2 * C3;
-    else if (n == "rs") vec = t->rs, cnt = size_t(B) * C3;
-    else if (n == "rb") vec = t->rb, cnt = size_t(B) * C3;
-    else if (n == "dg2") vec = t->dg2, cnt = size_t(B) * C;
-    else if (n == "dg1") vec = t->dg1, cnt = size_t(B) * t->se;
-    else if (n == "ds") vec = t->ds, cnt = size_t(B) * C;
-    else if (n == "se_s") vec = t->se_s[bk], cnt = size_t(B) * C, vec_block = true;
-    else if (n == "se_g1") vec = t->se_g1[bk], cnt = size_t(B) * t->se, vec_block = true;
-    else if (n == "se_g2") vec = t->se_g2[bk], cnt = size_t(B) * C, vec_block = true;
-    if (vec) {
-        if (padded || (per_block && !vec_block)) return unknown();
-        PPV_REQUIRE(out_elems >= cnt, "trainer_read_tap: output too small");
-        PPV_CUDA_OK(cudaMemcpyAsync(out, vec, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    const auto it = t->taps.find(n);
+    if (it == t->taps.end() || (b >= 0 && !it->second.per_block) || (padded && it->second.f32))
+        return fail(PPV_EINVAL, std::string("trainer_read_tap: unknown tap ") + name);
+    const TrTap& e = it->second;
+    const int bk = std::max(b, 0);
+    if (e.f32) {
+        PPV_REQUIRE(out_elems >= e.count, "trainer_read_tap: output too small");
+        PPV_CUDA_OK(cudaMemcpyAsync(out, e.vec[bk], e.count * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return PPV_OK;
     }
-
-    Planes src;
-    int col0 = 0, cols = C;
-    bool blocked = false;
-    if (n.rfind("g:", 0) == 0) {
-        const std::string g = n.substr(2);
-        if (g == "D") src = t->Dbuf[bk], blocked = true;
-        else if (g == "dZt2") src = t->dZt2[bk], blocked = true;
-        else if (g == "dRC") src = t->dRC[bk], blocked = true;
-        else if (g == "dZres") src = t->dZres[bk], blocked = true;
-        else if (g == "DIN") src = t->DIN[bk], blocked = true;
-        else if (g == "dZt1") src = t->dZt1[bk], blocked = true;
-        else if (g == "dXt1") src = t->dXt1[bk], blocked = true;
-        else if (g == "dZ0") src = t->dZ0;
-        else if (g == "dOUTCAT") src = t->dOUTCAT, cols = C3;
-        else if (g == "dMd") src = t->dMd, cols = C3;
-        else if (g == "dMatt") src = t->dMatt, cols = C3;
-        else if (g == "dZmfa") src = t->dZmfa, cols = C3;
-        else if (g == "dlogits") src = t->dlogits, cols = C3;
-        else if (g == "dZatt") src = t->dZatt, cols = t->att;
-        else if (g == "dA4") src = t->dA4, cols = t->att;
-        else return unknown();
-    } else if (n == "blocks.0" || n == "Y0") {
-        src = t->Y0;
-    } else if (n == "blocks.1" || n == "blocks.2" || n == "blocks.3") {
-        src = t->OUTCAT;
-        col0 = C * (n[7] - '1');
-    } else if (n == "mfa" || n == "M") {
-        src = t->M, cols = C3;
-    } else if (n == "X0") {
-        src = t->X0, cols = t->cfg.input_size;
-    } else if (n == "A0") {
-        src = t->A0;
-    } else if (n == "OUTCAT") {
-        src = t->OUTCAT, cols = C3;
-    } else if (n == "Amfa") {
-        src = t->Amfa, cols = C3;
-    } else if (n == "Aatt" || n == "A4") {
-        src = n == "A4" ? t->A4 : t->Aatt, cols = t->att;
-    } else {
-        blocked = true;
-        if (n == "At1") src = t->At1[bk];
-        else if (n == "Yt1") src = t->Yt1[bk];
-        else if (n == "Ares") src = t->Ares[bk];
-        else if (n == "RC") src = t->RC[bk];
-        else if (n == "IN") src = t->IN[bk];
-        else if (n == "At2") src = t->At2[bk];
-        else if (n == "Yt2") src = t->Yt2[bk];
-        else return unknown();
-    }
-    if (per_block && !blocked) return unknown();
-    const int rows = padded ? t->Tp : T;
-    PPV_REQUIRE(out_elems >= size_t(B) * rows * cols, "trainer_read_tap: output too small");
-    return launch_planes_to_f32(src, col0, cols, B, rows, padded ? 0 : t->P, t->Tp, out, st);
+    const int B = t->plan_B, Tp = t->buf.Tp, rows = padded ? Tp : t->plan_T;
+    PPV_REQUIRE(out_elems >= size_t(B) * rows * e.cols, "trainer_read_tap: output too small");
+    return launch_planes_to_f32(e.pl[bk], e.col0, e.cols, B, rows, padded ? 0 : t->P, Tp, out, st);
 }
 
 }  // namespace ppv

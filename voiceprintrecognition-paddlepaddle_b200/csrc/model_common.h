@@ -217,23 +217,65 @@ struct WsCarver {
     }
 };
 
-// An inference model behind ppv_model_*: weights are loaded by name, prepared into one device arena by finalize(), and each
-// forward runs a plan of launches that is built for (workspace, B, T) and rebuilt whenever one of them changes.
-struct Model {
-    const char* prefix;  // error-message prefix, e.g. "resnetse"
-    WeightMap raw;
-    bool finalized = false;
+// A plan of launches over a caller-owned workspace, built for (workspace, B, T) and rebuilt whenever one of them changes: the
+// inference models and the training step.
+struct PlanOwner {
+    const char* prefix;    // error-message prefix, e.g. "resnetse"
+    const char* ws_query;  // the C ABI entry point that sizes the workspace, named in the "workspace too small" error
     int precision;
     int num_sms;
-    void* arena = nullptr;
     void* plan_ws = nullptr;  // the plan's key (plan_ws, plan_B, plan_T); null and zeros when no plan is built
     int plan_B = 0, plan_T = 0;
+
+    PlanOwner(const char* prefix, const char* ws_query, int precision)
+        : prefix(prefix), ws_query(ws_query), precision(precision), num_sms(device_sm_count()) {}
+    virtual ~PlanOwner() = default;
+    // Bytes of workspace a plan for B utterances of T frames carves; computed without touching the current plan.
+    virtual size_t workspace_bytes(int B, int T) const = 0;
+
+    // No plan: B > 0 in every run, so no key matches this one and the next run rebuilds.
+    void invalidate_plan() {
+        plan_ws = nullptr;
+        plan_B = plan_T = 0;
+    }
+    int update_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+        if (plan_ws == ws && plan_B == B && plan_T == T) return PPV_OK;
+        int rc = build_plan(B, T, ws, ws_bytes, st);
+        if (rc) {
+            invalidate_plan();
+            return rc;
+        }
+        plan_ws = ws;
+        plan_B = B;
+        plan_T = T;
+        return PPV_OK;
+    }
+
+  protected:
+    // The opening of build_plan: `ws` must hold workspace_bytes(B, T) bytes at 256-byte alignment; it is zeroed on `st`, because the
+    // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
+    int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
+        const size_t need = workspace_bytes(B, T);
+        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see " + ws_query + ")");
+        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
+        PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
+        return PPV_OK;
+    }
+    // Carves `ws` and plans the launches of a run over B utterances of T frames.
+    virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
+};
+
+// An inference model behind ppv_model_*: weights are loaded by name, prepared into one device arena by finalize(), and each
+// forward runs the plan.
+struct Model : PlanOwner {
+    WeightMap raw;
+    bool finalized = false;
+    void* arena = nullptr;
     float* emb_out = nullptr;  // workspace buffer the plan's last step writes the embeddings [B][embd_dim] to
 
-    Model(const char* prefix, int precision) : prefix(prefix), precision(precision), num_sms(device_sm_count()) {}
-    virtual ~Model() { cudaFree(arena); }
+    Model(const char* prefix, int precision) : PlanOwner(prefix, "ppv_model_workspace_bytes", precision) {}
+    ~Model() override { cudaFree(arena); }
     virtual int embd_dim() const = 0;
-    virtual size_t workspace_bytes(int B, int T) const = 0;
 
     int load_weight(const char* name, const float* data, const int64_t* shape, int ndim) {
         if (finalized) return fail(PPV_ESTATE, std::string(prefix) + "_load_weight: model already finalized");
@@ -276,36 +318,12 @@ struct Model {
         PPV_REQUIRE(B > 0 && T > 0, std::string(prefix) + "_forward: empty batch");
         return PPV_OK;
     }
-    int update_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-        if (plan_ws == ws && plan_B == B && plan_T == T) return PPV_OK;
-        int rc = build_plan(B, T, ws, ws_bytes, st);
-        if (rc) {  // no plan: B > 0 in every forward, so no key matches this one and the next forward rebuilds
-            plan_ws = nullptr;
-            plan_B = plan_T = 0;
-            return rc;
-        }
-        plan_ws = ws;
-        plan_B = B;
-        plan_T = T;
-        return PPV_OK;
-    }
-    // The opening of build_plan: `ws` must hold workspace_bytes(B, T) bytes at 256-byte alignment; it is zeroed on `st`, because the
-    // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
-    int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
-        const size_t need = workspace_bytes(B, T);
-        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see ppv_model_workspace_bytes)");
-        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
-        PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
-        return PPV_OK;
-    }
     int copy_embeddings(float* emb, cudaStream_t st) {
         PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(plan_B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return PPV_OK;
     }
     // Puts the prepared weights into the arena image; false, with ab.err set where known, on a missing or misshapen weight.
     virtual bool prepare_weights(ArenaBuilder& ab) = 0;
-    // Carves `ws` and plans the launches of a forward over B utterances of T frames.
-    virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
     // Launches the planned steps on features [plan_B, plan_T, input_size].
     virtual int run_steps(const float* feat, cudaStream_t st) = 0;
     virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
