@@ -192,7 +192,7 @@ __global__ void __launch_bounds__(256) cp_flatten_pairs_kernel(Planes in, int B,
 
 }  // namespace
 
-struct CamppModel : ImagePlanModel {
+struct CamppModel : PlanModel {
     ppv_campplus_cfg cfg;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<ResBlockW> res;
@@ -208,7 +208,7 @@ struct CamppModel : ImagePlanModel {
     Planes stage_out[4];
     Planes xblk[CP_NB], tr_out[CP_NB];
 
-    explicit CamppModel(const ppv_campplus_cfg& c) : ImagePlanModel("campplus", c.precision), cfg(c) {}
+    explicit CamppModel(const ppv_campplus_cfg& c) : PlanModel("campplus", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
     size_t workspace_bytes(int B, int T) const override;
 
@@ -424,7 +424,7 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             if (rc) return rc;
             resid = cb.sc[i];
         }
-        m->steps.push_back(scale_res_step(cb.c2[i], nullptr, resid, cb.out[i], 32, go, B));
+        m->steps.push_back(scale_res_step(cb.c2[i], nullptr, resid, 0, cb.out[i], 0, 32, go.Hp * go.Wp, go.rows(B), true));
         x = cb.out[i];
         m->stage_out[rw.stage] = x;
     }
@@ -529,7 +529,7 @@ int CamppModel::run_model_step(const PlanStep& s, cudaStream_t st) {
                        "cp_context_kernel");
             return PPV_OK;
     }
-    return ImagePlanModel::run_model_step(s, st);
+    return PlanModel::run_model_step(s, st);
 }
 
 // taps: "head.layer1", "head.layer2" -> fp32 [B,H,W,32]; "tdnn" [B,T2,128]; "block1".."block3" [B,T2,C]; "transit1", "transit2"

@@ -16,7 +16,7 @@
 #include <string.h>
 
 #include "common.h"
-#include "model_common.h"
+#include "plan.h"
 
 namespace ppv {
 
@@ -27,55 +27,29 @@ struct ConvW : GemmWeights {  // + BatchNorm(eval) after the ReLU, as y = y * bn
     float* bn_shift = nullptr;
 };
 
-struct KSpec {  // one K group: `ncols` columns of a source at a row offset <- weight input channels
-    int src;    // buffer id
-    int col0, ncols, row_off;
-    int w_cin0, w_cnt, w_tap;
-};
-
-enum Buf { B_FEAT, B_X0, B_H, B_Y, B_Z, B_CAT, B_MFA, B_ATT, B_GSTAT, B_POOL, B_SEM, B_SEH, B_COUNT };
-
-struct Step {
-    enum Kind { GEMM, SKINNY, RES2, RES2CHAIN, SE_SQUEEZE, SE_SCALE, ASP_GLOBAL, ASP_FUSED, POOL_STATS } kind;
-    // SKINNY: one-row-per-utterance linear layer on the CUDA cores (skinny.cu)
-    Planes sk_x, sk_w;
-    int sk_col0 = 0, sk_M = 0, sk_N = 0, sk_K = 0;
-    Epilogue sk_ep;
-    GemmParams gp;
-    AspFusedParams ap;
-    Res2Params rp;
-    Res2ChainParams cp;
-    int blk = 0;  // block index for the SE steps
-};
-
 struct EcBuffers {  // the workspace of a plan
-    Planes bufs[B_COUNT];
+    Planes feat, x0, h, y, z, cat, mfa, att, gstat, pool, sem, seh;
     float *se_mean = nullptr, *se_scale = nullptr, *fold_out = nullptr, *pooled_raw = nullptr, *raw_logmel = nullptr;
     int* nvalid = nullptr;  // [B] valid-frame counts of the current forward (`lengths`)
 };
 
 }  // namespace
 
-struct EcapaModel : Model {
+struct EcapaModel : PlanModel {
     ppv_ecapa_cfg cfg;
     int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0;
     // device weights
     ConvW conv0, tdnn1[3], res2[3][8], tdnn2[3], se1[3], se2[3], mfa, fold, att1, att2, fc;
     float *aspbn_scale = nullptr, *aspbn_shift = nullptr;
     // plan
-    std::vector<Step> steps;
     EcBuffers buf;
     int Tp = 0;
-    // profiling (bench.py roofline): CUDA events around every launch group of the forward
-    bool prof_on = false;
-    std::vector<cudaEvent_t> prof_ev;   // pairs
-    std::vector<int> prof_kind;         // 0 = tensor-core GEMM, 1 = other kernels
-    size_t prof_used = 0;
-    int64_t launches_gemm = 0, launches_other = 0;
 
-    explicit EcapaModel(const ppv_ecapa_cfg& c) : Model("ecapa", c.precision), cfg(c) {}
-    ~EcapaModel() override {
-        for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
+    explicit EcapaModel(const ppv_ecapa_cfg& c) : PlanModel("ecapa", c.precision), cfg(c) {
+        // 128-wide n-tiles even where N allows 256: on an H100 SXM at 700 W (tools/gemm_bench.py, M = 78 336,
+        // profiles/gemm_bench_after.txt) BN = 128 with 64-wide k-steps takes 15-18 % less time than BN = 256 at every large layer of
+        // the model (N x K = 512 x 512 / 640, 1536 x 1536, split-bf16 x3), and no BN = 256 variant beats it by more than run-to-run noise.
+        max_bn = 128;
     }
     int embd_dim() const override { return cfg.embd_dim; }
     size_t workspace_bytes(int B, int T) const override;
@@ -140,125 +114,76 @@ int ecapa_create(const ppv_ecapa_cfg* cfg, Model** out) {
 }
 
 // ------------------------------------------------------------------------------------------------ finalize
-namespace {
-
-// conv weight [N, Cin, k] -> split planes [2][Npad][Ktot] following the K groups; rows padded to a multiple of 128
-void put_conv(ArenaBuilder& ab, ConvW* cw, const std::vector<float>& w, int N, int Cin, int k, const std::vector<KSpec>& ks) {
-    int Ktot = 0;
-    for (const KSpec& s : ks) Ktot += s.ncols;
-    std::vector<double> mtx(size_t(N) * Ktot, 0.0);
-    for (int n = 0; n < N; ++n) {
-        int kpos = 0;
-        for (const KSpec& s : ks) {
-            for (int c = 0; c < s.w_cnt; ++c) mtx[size_t(n) * Ktot + kpos + c] = w[(size_t(n) * Cin + s.w_cin0 + c) * k + s.w_tap];
-            kpos += s.ncols;
-        }
-    }
-    ab.put_matrix(cw, mtx, N, Ktot, 128);
-}
-
-// BatchNorm eval -> y = x * scale + shift  (ppvector/models/utils.py:96-119), rounded to fp32
-bool bn_affine_f32(ArenaBuilder& ab, const std::string& prefix, int C, std::vector<float>* scale, std::vector<float>* shift) {
-    std::vector<double> sc, sh;
-    if (!ab.bn_affine(prefix, C, &sc, &sh)) return false;
-    scale->assign(sc.begin(), sc.end());
-    shift->assign(sh.begin(), sh.end());
-    return true;
-}
-
-std::vector<KSpec> spec_conv0(const EcapaModel* m) {
-    std::vector<KSpec> ks;
-    const int k = m->cfg.kernel_sizes[0], d = m->cfg.dilations[0];
-    for (int j = 0; j < k; ++j) ks.push_back({B_FEAT, 0, m->Fp, (j - (k - 1) / 2) * d, 0, m->cfg.input_size, j});
-    return ks;
-}
-std::vector<KSpec> spec_res2(const EcapaModel* m, int blk, int j) {  // j = 1 .. scale-1
-    std::vector<KSpec> ks;
-    const int d = m->cfg.dilations[blk], w = m->width;
-    for (int tap = 0; tap < 3; ++tap) ks.push_back({B_H, j * w, w, (tap - 1) * d, 0, w, tap});
-    if (j >= 2)
-        for (int tap = 0; tap < 3; ++tap) ks.push_back({B_Y, (j - 1) * w, w, (tap - 1) * d, 0, w, tap});
-    return ks;
-}
-
-}  // namespace
-
 bool EcapaModel::prepare_weights(ArenaBuilder& ab) {
-    EcapaModel* const m = this;
-    const int C = m->C, C3 = m->C3, w = m->width, F = m->cfg.input_size, A = m->att, S = m->se, E = m->cfg.embd_dim;
-    const int k0 = m->cfg.kernel_sizes[0];
-    auto conv_layer = [&](ConvW* cw, const std::string& wname, int N, int Cin, int k, const std::vector<KSpec>& ks,
-                          const std::string& bn_prefix, bool has_bias) -> bool {
-        const HostWeight* hw = ab.get(wname + ".weight", {N, Cin, k});
-        if (!hw) return false;
-        put_conv(ab, cw, hw->v, N, Cin, k, ks);
-        if (has_bias) {
-            const HostWeight* hb = ab.get(wname + ".bias", {N});
-            if (!hb) return false;
-            ab.put_f32(&cw->bias, hb->v);
-        }
-        if (!bn_prefix.empty()) {
-            std::vector<float> sc, sh;
-            if (!bn_affine_f32(ab, bn_prefix, N, &sc, &sh)) return false;
-            ab.put_f32(&cw->bn_scale, sc);
-            ab.put_f32(&cw->bn_shift, sh);
-        }
-        return true;
+    const int w = width, F = cfg.input_size, A = att, S = se, E = cfg.embd_dim;
+    const int k0 = cfg.kernel_sizes[0];
+    // conv weight [N, Cin, k] -> split planes [2][N rounded up to 128][K], K in the order of `groups` (conv_weight_matrix)
+    auto put_weights = [&](ConvW* cw, const float* wv, int N, int Cin, int k, const std::vector<ConvKGroup>& groups) {
+        const std::vector<double> mtx = conv_weight_matrix(wv, N, Cin, k, N, groups);
+        ab.put_matrix(cw, mtx, N, int(mtx.size() / N), 128);
     };
-    bool ok = conv_layer(&m->conv0, "blocks.0.conv.conv", C, F, k0, spec_conv0(m), "blocks.0.norm.norm", true);
+    // a conv with its bias and, unless `bn` is empty, the BatchNorm after its ReLU
+    auto conv_layer = [&](ConvW* cw, const std::string& name, int N, int Cin, int k, const std::vector<ConvKGroup>& groups,
+                          const std::string& bn) -> bool {
+        const HostWeight* hw = ab.get(name + ".weight", {N, Cin, k});
+        if (!hw) return false;
+        put_weights(cw, hw->v.data(), N, Cin, k, groups);
+        const HostWeight* hb = ab.get(name + ".bias", {N});
+        if (!hb) return false;
+        ab.put_f32(&cw->bias, hb->v);
+        return bn.empty() || ab.put_bn(&cw->bn_scale, &cw->bn_shift, bn, N, N);
+    };
+    auto all_cols = [](int Cin) { return std::vector<ConvKGroup>{{1, Cin, 0, Cin, 0}}; };  // a 1x1 conv reading Cin columns
+    bool ok = conv_layer(&conv0, "blocks.0.conv.conv", C, F, k0, {{k0, Fp, 0, F, 0}}, "blocks.0.norm.norm");
     for (int b = 1; b <= 3 && ok; ++b) {
         const std::string p = "blocks." + std::to_string(b);
-        ok = ok && conv_layer(&m->tdnn1[b - 1], p + ".tdnn1.conv.conv", C, C, 1, {{-1, 0, C, 0, 0, C, 0}}, p + ".tdnn1.norm.norm", true);
-        for (int j = 1; j < m->scale && ok; ++j) {
+        ok = ok && conv_layer(&tdnn1[b - 1], p + ".tdnn1.conv.conv", C, C, 1, all_cols(C), p + ".tdnn1.norm.norm");
+        for (int j = 1; j < scale && ok; ++j) {
+            // three taps of chunk j, then from j = 2 the same weights again for the three taps of conv j-1's output (x_j + y_{j-1})
+            std::vector<ConvKGroup> groups = {{3, w, 0, w, 0}};
+            if (j >= 2) groups.push_back({3, w, 0, w, 0});
             const std::string q = p + ".res2net_block.blocks." + std::to_string(j - 1);
-            ok = ok && conv_layer(&m->res2[b - 1][j], q + ".conv.conv", w, w, 3, spec_res2(m, b, j), q + ".norm.norm", true);
+            ok = ok && conv_layer(&res2[b - 1][j], q + ".conv.conv", w, w, 3, groups, q + ".norm.norm");
         }
-        ok = ok && conv_layer(&m->tdnn2[b - 1], p + ".tdnn2.conv.conv", C, C, 1, {{B_H, 0, w, 0, 0, w, 0}, {B_Y, w, C - w, 0, w, C - w, 0}},
-                              p + ".tdnn2.norm.norm", true);
-        // SE excitation as two small gather-GEMMs over the [B, C] squeeze (ecapa_tdnn.py:79-80)
-        ok = ok && conv_layer(&m->se1[b - 1], p + ".se_block.conv1.conv", S, C, 1, {{B_SEM, 0, C, 0, 0, C, 0}}, "", true);
-        ok = ok && conv_layer(&m->se2[b - 1], p + ".se_block.conv2.conv", C, S, 1, {{B_SEH, 0, S, 0, 0, S, 0}}, "", true);
+        ok = ok && conv_layer(&tdnn2[b - 1], p + ".tdnn2.conv.conv", C, C, 1, {{1, w, 0, w, 0}, {1, C - w, 0, C - w, w}}, p + ".tdnn2.norm.norm");
+        // SE excitation as two small linear layers over the [B, C] squeeze (ecapa_tdnn.py:79-80)
+        ok = ok && conv_layer(&se1[b - 1], p + ".se_block.conv1.conv", S, C, 1, all_cols(C), "");
+        ok = ok && conv_layer(&se2[b - 1], p + ".se_block.conv2.conv", C, S, 1, all_cols(S), "");
     }
-    ok = ok && conv_layer(&m->mfa, "mfa.conv.conv", C3, C3, 1, {{B_CAT, 0, C3, 0, 0, C3, 0}}, "mfa.norm.norm", true);
-    const int pooling = m->cfg.pooling;
+    ok = ok && conv_layer(&mfa, "mfa.conv.conv", C3, C3, 1, all_cols(C3), "mfa.norm.norm");
+    const int pooling = cfg.pooling;
     // BatchNorm(eval) + Linear after a parameter-free or self-attentive pooling: fc(bn(p)) = (W diag(s)) p + (W t + b), folded here
     auto folded_fc = [&](int Kp) -> bool {
-        const HostWeight* w = ab.get("fc.conv.weight", {E, Kp, 1});
-        const HostWeight* b = ab.get("fc.conv.bias", {E});
-        std::vector<float> sc, sh;
-        if (!w || !b || !bn_affine_f32(ab, "asp_bn", Kp, &sc, &sh)) return false;  // paddle.nn.BatchNorm1D: keys asp_bn.weight / ._mean ...
+        const HostWeight* wt = ab.get("fc.conv.weight", {E, Kp, 1});
+        const HostWeight* bt = ab.get("fc.conv.bias", {E});
+        std::vector<double> scd, shd;
+        if (!wt || !bt || !ab.bn_affine("asp_bn", Kp, &scd, &shd)) return false;  // paddle.nn.BatchNorm1D: keys asp_bn.weight / ._mean ...
+        const std::vector<float> sc(scd.begin(), scd.end()), sh(shd.begin(), shd.end());  // rounded to fp32 first
         std::vector<float> wf(size_t(E) * Kp), bf(E);
         for (int n = 0; n < E; ++n) {
-            double acc = b->v[n];
+            double acc = bt->v[n];
             for (int k = 0; k < Kp; ++k) {
-                wf[size_t(n) * Kp + k] = w->v[size_t(n) * Kp + k] * sc[k];
-                acc += double(w->v[size_t(n) * Kp + k]) * sh[k];
+                wf[size_t(n) * Kp + k] = wt->v[size_t(n) * Kp + k] * sc[k];
+                acc += double(wt->v[size_t(n) * Kp + k]) * sh[k];
             }
             bf[n] = float(acc);
         }
-        put_conv(ab, &m->fc, wf, E, Kp, 1, {{B_POOL, 0, Kp, 0, 0, Kp, 0}});
-        ab.put_f32(&m->fc.bias, bf);
+        put_weights(&fc, wf.data(), E, Kp, 1, all_cols(Kp));
+        ab.put_f32(&fc.bias, bf);
         return true;
     };
     if (pooling == PPV_POOL_ASP) {
-    // ASP attention TDNN: weight [A, 3*C3, 1] split into the x part (cols 0..C3) and the [mean;std] part;
-    // global_context = False (pooling.py:77-78, 108-109): the TDNN sees x alone, weight [A, C3, 1], no per-utterance bias
-    const int ctx = m->cfg.global_context ? 3 : 1;
-    ok = ok && conv_layer(&m->att1, "asp.tdnn.conv.conv", A, ctx * C3, 1, {{B_MFA, 0, C3, 0, 0, C3, 0}}, "asp.tdnn.norm.norm", true);
-    if (ok && m->cfg.global_context) {
-        const HostWeight* hw = ab.get("asp.tdnn.conv.conv.weight", {A, 3 * C3, 1});
-        put_conv(ab, &m->fold, hw->v, A, 3 * C3, 1, {{B_GSTAT, 0, 2 * C3, 0, C3, 2 * C3, 0}});
-    }
-    ok = ok && conv_layer(&m->att2, "asp.conv.conv", C3, A, 1, {{B_ATT, 0, A, 0, 0, A, 0}}, "", true);
-    ok = ok && conv_layer(&m->fc, "fc.conv", E, 2 * C3, 1, {{B_POOL, 0, 2 * C3, 0, 0, 2 * C3, 0}}, "", true);
-    if (ok) {
-        std::vector<float> sc, sh;
-        ok = bn_affine_f32(ab, "asp_bn.norm", 2 * C3, &sc, &sh);
-        if (ok) {
-            ab.put_f32(&m->aspbn_scale, sc);
-            ab.put_f32(&m->aspbn_shift, sh);
+        // ASP attention TDNN: weight [A, 3*C3, 1] split into the x part (cols 0..C3) and the [mean;std] part;
+        // global_context = False (pooling.py:77-78, 108-109): the TDNN sees x alone, weight [A, C3, 1], no per-utterance bias
+        const int ctx = cfg.global_context ? 3 : 1;
+        ok = ok && conv_layer(&att1, "asp.tdnn.conv.conv", A, ctx * C3, 1, {{1, C3, 0, C3, 0}}, "asp.tdnn.norm.norm");
+        if (ok && cfg.global_context) {
+            const HostWeight* hw = ab.get("asp.tdnn.conv.conv.weight", {A, 3 * C3, 1});
+            put_weights(&fold, hw->v.data(), A, 3 * C3, 1, {{1, 2 * C3, 0, 2 * C3, C3}});
         }
-    }
+        ok = ok && conv_layer(&att2, "asp.conv.conv", C3, A, 1, all_cols(A), "");
+        ok = ok && conv_layer(&fc, "fc.conv", E, 2 * C3, 1, all_cols(2 * C3), "");
+        ok = ok && ab.put_bn(&aspbn_scale, &aspbn_shift, "asp_bn.norm", 2 * C3, 2 * C3);
     } else if (pooling == PPV_POOL_SAP) {
         // SelfAttentivePooling (pooling.py:50-66): alpha = softmax_t(linear2(tanh(linear1(x)))); mean = sum alpha x.  The fused ASP
         // kernel computes exactly this weighted mean (its std half is ignored); linear2's bias cancels in the softmax.
@@ -266,12 +191,12 @@ bool EcapaModel::prepare_weights(ArenaBuilder& ab) {
             ab.err = "SAP pooling uses a 128-channel bottleneck (ecapa_tdnn.py:222): attention_channels must be 128";
             ok = false;
         }
-        ok = ok && conv_layer(&m->att1, "asp.linear1", A, C3, 1, {{B_MFA, 0, C3, 0, 0, C3, 0}}, "", true);
-        ok = ok && conv_layer(&m->att2, "asp.linear2", C3, A, 1, {{B_ATT, 0, A, 0, 0, A, 0}}, "", true);
+        ok = ok && conv_layer(&att1, "asp.linear1", A, C3, 1, all_cols(C3), "");
+        ok = ok && conv_layer(&att2, "asp.linear2", C3, A, 1, all_cols(A), "");
         ok = ok && folded_fc(C3);
         if (ok) {
-            ab.put_f32(&m->aspbn_scale, std::vector<float>(2 * C3, 1.f));
-            ab.put_f32(&m->aspbn_shift, std::vector<float>(2 * C3, 0.f));
+            ab.put_f32(&aspbn_scale, std::vector<float>(2 * C3, 1.f));
+            ab.put_f32(&aspbn_shift, std::vector<float>(2 * C3, 0.f));
         }
     } else {
         ok = ok && folded_fc(pooling == PPV_POOL_TAP ? C3 : 2 * C3);
@@ -285,18 +210,18 @@ namespace {
 void carve(const EcapaModel* m, WsCarver& cv, int B, int T, EcBuffers* eb, float** emb_out) {
     const int64_t R = int64_t(B) * (T + 2 * m->P);
     const int C = m->C, C3 = m->C3;
-    eb->bufs[B_FEAT] = cv.planes(R, m->Fp);
-    eb->bufs[B_X0] = cv.planes(R, C);
-    eb->bufs[B_H] = cv.planes(R, C);
-    eb->bufs[B_Y] = cv.planes(R, C);
-    eb->bufs[B_Z] = cv.planes(R, C);
-    eb->bufs[B_CAT] = cv.planes(R, C3);
-    eb->bufs[B_MFA] = cv.planes(R, C3);
-    eb->bufs[B_ATT] = cv.planes(R, m->att);
-    eb->bufs[B_GSTAT] = cv.planes(B, 2 * C3);
-    eb->bufs[B_POOL] = cv.planes(B, 2 * C3);
-    eb->bufs[B_SEM] = cv.planes(B, C);
-    eb->bufs[B_SEH] = cv.planes(B, m->se);
+    eb->feat = cv.planes(R, m->Fp);
+    eb->x0 = cv.planes(R, C);
+    eb->h = cv.planes(R, C);
+    eb->y = cv.planes(R, C);
+    eb->z = cv.planes(R, C);
+    eb->cat = cv.planes(R, C3);
+    eb->mfa = cv.planes(R, C3);
+    eb->att = cv.planes(R, m->att);
+    eb->gstat = cv.planes(B, 2 * C3);
+    eb->pool = cv.planes(B, 2 * C3);
+    eb->sem = cv.planes(B, C);
+    eb->seh = cv.planes(B, m->se);
     eb->se_mean = static_cast<float*>(cv.take(size_t(B) * C * 4));
     eb->se_scale = static_cast<float*>(cv.take(size_t(B) * C * 4));
     eb->fold_out = static_cast<float*>(cv.take(mc_align_up(B, 128) * m->att * 4));
@@ -306,10 +231,13 @@ void carve(const EcapaModel* m, WsCarver& cv, int B, int T, EcBuffers* eb, float
     eb->nvalid = static_cast<int*>(cv.take(size_t(B) * sizeof(int)));
 }
 
-// 128-wide n-tiles even where N allows 256: on an H100 SXM at 700 W (tools/gemm_bench.py, M = 78 336, profiles/gemm_bench_after.txt)
-// BN = 128 with 64-wide k-steps takes 15-18 % less time than BN = 256 at every large layer of the model (N x K = 512 x 512 / 640,
-// 1536 x 1536, split-bf16 x3), and no BN = 256 variant beats it by more than run-to-run noise.
-constexpr int ECAPA_MAX_BN = 128;
+Epilogue f32_out(float* out, int ld) {
+    Epilogue ep;
+    ep.out_mode = OUT_F32;
+    ep.out = out;
+    ep.out_ld = ld;
+    return ep;
+}
 
 }  // namespace
 
@@ -324,72 +252,24 @@ size_t EcapaModel::workspace_bytes(int B, int T) const {
 
 // ------------------------------------------------------------------------------------------------ plan
 int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-    EcapaModel* const m = this;
-    PPV_REQUIRE(T > m->P, "ecapa: too few frames for the reflect padding");
+    PPV_REQUIRE(T > P, "ecapa: too few frames for the reflect padding");
     int rc = claim_workspace(B, T, ws, ws_bytes, st);
     if (rc) return rc;
     WsCarver cv;
     cv.base = static_cast<uint8_t*>(ws);
-    carve(m, cv, B, T, &m->buf, &m->emb_out);
-    m->Tp = T + 2 * m->P;
-    m->steps.clear();
-    const int Tp = m->Tp, P = m->P, C = m->C, C3 = m->C3, w = m->width;
-    const int64_t R = int64_t(B) * Tp;
-    const char* r2env = getenv("PPV_RES2_GEMM");  // debugging aid: 1 = run the Res2Net convs through the generic gather-GEMM
-    const bool use_res2_kernel = (w == 64) && !(r2env && r2env[0] == '1');
+    carve(this, cv, B, T, &buf, &emb_out);
+    Tp = T + 2 * P;
+    steps.clear();
+    const int w = width, R = int(int64_t(B) * Tp);
+    const bool use_res2_kernel = w == 64;
     // 0 = one launch per Res2Net conv (res2conv.cu) instead of the fused chain; single = the fused chain with one utterance per CTA
     // even where two fit (tests and A/B timing)
     const char* rcenv = getenv("PPV_RES2_CHAIN");
-    const bool use_res2_chain = use_res2_kernel && m->scale == 8 && res2chain_fits(T, P) && !(rcenv && rcenv[0] == '0');
+    const bool use_res2_chain = use_res2_kernel && scale == 8 && res2chain_fits(T, P) && !(rcenv && rcenv[0] == '0');
     const bool res2_paired = use_res2_chain && res2chain_pair_fits(T, P) && !(rcenv && strcmp(rcenv, "single") == 0);
-    const char* skenv = getenv("PPV_SKINNY");  // 0 = the per-utterance linear layers through the tensor-core gather-GEMM (A-B timing)
-    const bool use_skinny = !(skenv && skenv[0] == '0');
 
-    auto add_gemm = [&](const ConvW& cw, const std::vector<KSpec>& ks, const Planes* src_override, int override_col0, int M,
-                        Epilogue ep) -> int {
-        std::vector<GemmSource> srcs;
-        for (const KSpec& s : ks) {
-            GemmSource g;
-            if (s.src < 0) {
-                g.t = *src_override;
-                g.col0 = override_col0 + s.col0;
-            } else {
-                g.t = m->buf.bufs[s.src];
-                g.col0 = s.col0;
-            }
-            g.ncols = s.ncols;
-            g.row_off = s.row_off;
-            srcs.push_back(g);
-        }
-        ep.bias = cw.bias;
-        if (ep.relu) {
-            ep.bn_scale = cw.bn_scale;
-            ep.bn_shift = cw.bn_shift;
-        }
-        // one row per utterance (SE MLP, ASP context bias, fc): every SM takes a 16 x 16 output tile on the CUDA cores instead of 2-6
-        // CTAs walking a latency-bound k-loop on the tensor cores
-        if (use_skinny && M == B && srcs.size() == 1 && srcs[0].row_off == 0 && skinny_linear_supported(M, cw.N, srcs[0].ncols, ep) &&
-            cw.Ktot == srcs[0].ncols) {
-            Step sk;
-            sk.kind = Step::SKINNY;
-            sk.sk_x = srcs[0].t;
-            sk.sk_col0 = srcs[0].col0;
-            sk.sk_w = cw.W;
-            sk.sk_M = M;
-            sk.sk_N = cw.N;
-            sk.sk_K = srcs[0].ncols;
-            sk.sk_ep = ep;
-            m->steps.push_back(sk);
-            return PPV_OK;
-        }
-        Step stp;
-        stp.kind = Step::GEMM;
-        int rc = gemm_build(&stp.gp, srcs.data(), int(srcs.size()), cw.W, M, cw.N, ep, gemm_pick_bn(cw.N, ECAPA_MAX_BN));
-        if (rc) return rc;
-        m->steps.push_back(stp);
-        return PPV_OK;
-    };
-    auto planes_out = [&](const Planes& p, int col0, bool halo) {
+    // planes output in the padded time layout: ReLU, then the layer's BatchNorm
+    auto planes_out = [&](const Planes& p, int col0, bool halo, const ConvW& cw) {
         Epilogue ep;
         ep.out_mode = OUT_PLANES;
         ep.out = p.base;
@@ -401,133 +281,113 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         ep.T = T;
         ep.halo = halo ? 1 : 0;
         ep.relu = 1;
+        ep.bn_scale = cw.bn_scale;
+        ep.bn_shift = cw.bn_shift;
         return ep;
     };
-    rc = add_gemm(m->conv0, spec_conv0(m), nullptr, 0, int(R), planes_out(m->buf.bufs[B_X0], 0, false));
-    if (rc) return rc;
+    {
+        std::vector<GemmSource> taps;
+        const int k0 = cfg.kernel_sizes[0], d0 = cfg.dilations[0];
+        for (int j = 0; j < k0; ++j) taps.push_back(GemmSource{buf.feat, 0, Fp, (j - (k0 - 1) / 2) * d0});
+        rc = plan_gemm(conv0, taps, R, planes_out(buf.x0, 0, false, conv0));
+        if (rc) return rc;
+    }
     for (int b = 1; b <= 3; ++b) {
-        const Planes& X = (b == 1) ? m->buf.bufs[B_X0] : m->buf.bufs[B_CAT];
-        const int xcol = (b == 1) ? 0 : (b - 2) * C;
+        const Planes& X = (b == 1) ? buf.x0 : buf.cat;
+        const int xcol = (b == 1) ? 0 : (b - 2) * C, d = cfg.dilations[b];
         // the fused Res2Net chain builds the reflect halo rows itself, so tdnn1 writes no halo rows (and gets the lean epilogue)
-        rc = add_gemm(m->tdnn1[b - 1], {{-1, 0, C, 0, 0, C, 0}}, &X, xcol, int(R), planes_out(m->buf.bufs[B_H], 0, !use_res2_chain));
+        rc = plan_gemm(tdnn1[b - 1], {GemmSource{X, xcol, C, 0}}, R, planes_out(buf.h, 0, !use_res2_chain, tdnn1[b - 1]));
         if (rc) return rc;
         if (use_res2_chain) {  // all seven convs in one kernel, one or two utterances per CTA, operands resident in shared memory (res2chain.cu)
             Planes Wj[RES2CHAIN_MAX];
             const float *bj[RES2CHAIN_MAX], *sj[RES2CHAIN_MAX], *hj[RES2CHAIN_MAX];
-            for (int j = 1; j < m->scale; ++j) {
-                const ConvW& cw = m->res2[b - 1][j];
+            for (int j = 1; j < scale; ++j) {
+                const ConvW& cw = res2[b - 1][j];
                 Wj[j - 1] = cw.W;  // the first 3 x 64 columns are the taps of source 0; source 1 repeats the same weights
                 bj[j - 1] = cw.bias;
                 sj[j - 1] = cw.bn_scale;
                 hj[j - 1] = cw.bn_shift;
             }
-            Step stp;
-            stp.kind = Step::RES2CHAIN;
-            rc = res2chain_build(&stp.cp, m->buf.bufs[B_H], m->buf.bufs[B_Y], Wj, bj, sj, hj, m->scale - 1, B, T, P, Tp, m->cfg.dilations[b],
-                                 res2_paired);
+            PlanStep s;
+            s.kind = PlanStep::RES2CHAIN;
+            rc = res2chain_build(&s.cp, buf.h, buf.y, Wj, bj, sj, hj, scale - 1, B, T, P, Tp, d, res2_paired);
             if (rc) return rc;
-            m->steps.push_back(stp);
+            steps.push_back(s);
         }
-        for (int j = 1; j < m->scale && !use_res2_chain; ++j) {
+        for (int j = 1; j < scale && !use_res2_chain; ++j) {
+            const ConvW& cw = res2[b - 1][j];
+            Epilogue ep = planes_out(buf.y, j * w, true, cw);
             if (use_res2_kernel) {  // weight-stationary kernel, one tall tile per source (res2conv.cu)
-                GemmSource srcs[2];
-                srcs[0] = GemmSource{m->buf.bufs[B_H], j * w, w, 0};
-                srcs[1] = GemmSource{m->buf.bufs[B_Y], (j - 1) * w, w, 0};
-                Epilogue ep = planes_out(m->buf.bufs[B_Y], j * w, true);
-                const ConvW& cw = m->res2[b - 1][j];
+                const GemmSource srcs[2] = {GemmSource{buf.h, j * w, w, 0}, GemmSource{buf.y, (j - 1) * w, w, 0}};
                 ep.bias = cw.bias;
-                ep.bn_scale = cw.bn_scale;
-                ep.bn_shift = cw.bn_shift;
-                Step stp;
-                stp.kind = Step::RES2;
-                rc = res2conv_build(&stp.rp, srcs, j >= 2 ? 2 : 1, cw.W, int(R), m->cfg.dilations[b], ep);
+                PlanStep s;
+                s.kind = PlanStep::RES2;
+                rc = res2conv_build(&s.rp, srcs, j >= 2 ? 2 : 1, cw.W, R, d, ep);
                 if (rc) return rc;
-                m->steps.push_back(stp);
-            } else {
-                rc = add_gemm(m->res2[b - 1][j], spec_res2(m, b, j), nullptr, 0, int(R), planes_out(m->buf.bufs[B_Y], j * w, true));
+                steps.push_back(s);
+            } else {  // the gather-GEMM over the three taps of chunk j and, from j = 2, of conv j-1's output
+                std::vector<GemmSource> srcs;
+                for (int tap = 0; tap < 3; ++tap) srcs.push_back(GemmSource{buf.h, j * w, w, (tap - 1) * d});
+                if (j >= 2)
+                    for (int tap = 0; tap < 3; ++tap) srcs.push_back(GemmSource{buf.y, (j - 1) * w, w, (tap - 1) * d});
+                rc = plan_gemm(cw, srcs, R, ep);
                 if (rc) return rc;
             }
         }
-        rc = add_gemm(m->tdnn2[b - 1], {{B_H, 0, w, 0, 0, w, 0}, {B_Y, w, C - w, 0, w, C - w, 0}}, nullptr, 0, int(R),
-                      planes_out(m->buf.bufs[B_Z], 0, false));
+        rc = plan_gemm(tdnn2[b - 1], {GemmSource{buf.h, 0, w, 0}, GemmSource{buf.y, w, C - w, 0}}, R, planes_out(buf.z, 0, false, tdnn2[b - 1]));
         if (rc) return rc;
-        Step s;
-        s.blk = b;
-        s.kind = Step::SE_SQUEEZE;
-        m->steps.push_back(s);
+        steps.push_back(colstats_step(buf.z, C, B, T, P, Tp, 0, 0.f, buf.sem, 0.f, true));
         {  // s = sigmoid(W2 relu(W1 mean + b1) + b2): [B,C] -> [B,S] -> [B,C], plain (un-padded) row layout
             Epilogue e1;
             e1.out_mode = OUT_PLANES;
-            e1.out = m->buf.bufs[B_SEH].base;
-            e1.out_ld = m->buf.bufs[B_SEH].ld;
-            e1.out_plane_stride = m->buf.bufs[B_SEH].plane_stride;
+            e1.out = buf.seh.base;
+            e1.out_ld = buf.seh.ld;
+            e1.out_plane_stride = buf.seh.plane_stride;
             e1.relu = 1;
-            rc = add_gemm(m->se1[b - 1], {{B_SEM, 0, C, 0, 0, 0, 0}}, nullptr, 0, B, e1);
+            rc = plan_row_linear(se1[b - 1], GemmSource{buf.sem, 0, C, 0}, B, e1);
             if (rc) return rc;
-            Epilogue e2;
-            e2.out_mode = OUT_F32;
-            e2.out = m->buf.se_scale;
-            e2.out_ld = C;
+            Epilogue e2 = f32_out(buf.se_scale, C);
             e2.sigmoid_ = 1;
-            rc = add_gemm(m->se2[b - 1], {{B_SEH, 0, m->se, 0, 0, 0, 0}}, nullptr, 0, B, e2);
+            rc = plan_row_linear(se2[b - 1], GemmSource{buf.seh, 0, se, 0}, B, e2);
             if (rc) return rc;
         }
-        s.kind = Step::SE_SCALE;
-        m->steps.push_back(s);
+        steps.push_back(scale_res_step(buf.z, buf.se_scale, X, xcol, buf.cat, (b - 1) * C, C, Tp, R, false));
     }
-    rc = add_gemm(m->mfa, {{B_CAT, 0, C3, 0, 0, C3, 0}}, nullptr, 0, int(R), planes_out(m->buf.bufs[B_MFA], 0, false));
+    rc = plan_gemm(mfa, {GemmSource{buf.cat, 0, C3, 0}}, R, planes_out(buf.mfa, 0, false, mfa));
     if (rc) return rc;
-    const int pooling = m->cfg.pooling;
-    if (pooling == PPV_POOL_TAP || pooling == PPV_POOL_TSP) {
-        Step s;  // mean (TAP) or mean | unbiased variance (TSP) over time, straight into the fc operand
-        s.kind = Step::POOL_STATS;
-        m->steps.push_back(s);
-    } else {
-        Step s;
-        s.kind = Step::ASP_GLOBAL;
-        m->steps.push_back(s);
-    }
-    if (pooling == PPV_POOL_ASP && m->cfg.global_context) {  // fold: [B, 2*C3] . W[:, C3:3*C3]^T -> per-utterance bias [B, att]  (no conv bias here)
-        Epilogue ep;
-        ep.out_mode = OUT_F32;
-        ep.out = m->buf.fold_out;
-        ep.out_ld = m->att;
-        ConvW cw = m->fold;
-        cw.bias = nullptr;
-        rc = add_gemm(cw, {{B_GSTAT, 0, 2 * C3, 0, 0, 0, 0}}, nullptr, 0, B, ep);
+    const int pooling = cfg.pooling;
+    if (pooling == PPV_POOL_TAP || pooling == PPV_POOL_TSP)  // mean (TAP) or mean | unbiased variance (TSP) over time, straight into the fc operand
+        steps.push_back(colstats_step(buf.mfa, C3, B, T, P, Tp, pooling == PPV_POOL_TAP ? 0 : 3, 0.f, buf.pool));
+    else  // global mean | std: ASP's context statistics and the fused pooling's shift
+        steps.push_back(colstats_step(buf.mfa, C3, B, T, P, Tp, 1, 1e-12f, buf.gstat, 0.f, true));
+    if (pooling == PPV_POOL_ASP && cfg.global_context) {  // fold: [B, 2*C3] . W[:, C3:3*C3]^T -> per-utterance bias [B, att]  (no conv bias here)
+        rc = plan_row_linear(fold, GemmSource{buf.gstat, 0, 2 * C3, 0}, B, f32_out(buf.fold_out, att));
         if (rc) return rc;
     }
     if (pooling == PPV_POOL_ASP || pooling == PPV_POOL_SAP) {
         {  // ASP: attention TDNN (K = C3) + per-utterance bias -> ReLU -> BN -> tanh;  SAP: tanh(linear1(x))
-            Epilogue ep = planes_out(m->buf.bufs[B_ATT], 0, false);
+            Epilogue ep = planes_out(buf.att, 0, false, att1);
             if (pooling == PPV_POOL_ASP) {
-                if (m->cfg.global_context) ep.rowgrp_bias = m->buf.fold_out;
+                if (cfg.global_context) ep.rowgrp_bias = buf.fold_out;
             } else {
                 ep.relu = 0;
             }
             ep.tanh_ = 1;
-            rc = add_gemm(m->att1, {{B_MFA, 0, C3, 0, 0, 0, 0}}, nullptr, 0, int(R), ep);
+            rc = plan_gemm(att1, {GemmSource{buf.mfa, 0, C3, 0}}, R, ep);
             if (rc) return rc;
         }
         {  // attention logits (transposed GEMM) + softmax over time + weighted mean / std + asp_bn, fused
-            Step s;
-            s.kind = Step::ASP_FUSED;
-            rc = asp_fused_build(&s.ap, m->att2.W, m->buf.bufs[B_ATT], m->buf.bufs[B_MFA], m->buf.bufs[B_GSTAT], m->aspbn_scale, m->aspbn_shift,
-                                 m->buf.bufs[B_POOL], m->buf.pooled_raw, B, T, P, Tp, C3, m->att, 1e-12f);
+            PlanStep s;
+            s.kind = PlanStep::ASP_FUSED;
+            rc = asp_fused_build(&s.ap, att2.W, buf.att, buf.mfa, buf.gstat, aspbn_scale, aspbn_shift, buf.pool, buf.pooled_raw, B, T, P, Tp, C3,
+                                 att, 1e-12f);
             if (rc) return rc;
-            m->steps.push_back(s);
+            steps.push_back(s);
         }
     }
-    {  // fc: pooled [B, Kp] -> [B, embd]
-        Epilogue ep;
-        ep.out_mode = OUT_F32;
-        ep.out = m->emb_out;
-        ep.out_ld = m->cfg.embd_dim;
-        const int Kp = (pooling == PPV_POOL_ASP || pooling == PPV_POOL_TSP) ? 2 * C3 : C3;
-        rc = add_gemm(m->fc, {{B_POOL, 0, Kp, 0, 0, 0, 0}}, nullptr, 0, B, ep);
-        if (rc) return rc;
-    }
-    return PPV_OK;
+    // fc: pooled [B, Kp] -> [B, embd]
+    const int Kp = (pooling == PPV_POOL_ASP || pooling == PPV_POOL_TSP) ? 2 * C3 : C3;
+    return plan_row_linear(fc, GemmSource{buf.pool, 0, Kp, 0}, B, f32_out(emb_out, cfg.embd_dim));
 }
 
 // ------------------------------------------------------------------------------------------------ forward
@@ -551,143 +411,61 @@ int ecapa_forward(Model* m, const float* feat, Fbank* fb, const float* wav, cons
     return static_cast<EcapaModel*>(m)->forward_ex(feat, fb, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, st, lengths);
 }
 
-// Launches the plan's steps on features or, with `wav`, on the fbank of the waveforms.
+// Packs the features or, with `wav`, computes the fbank of the waveforms into the first layer's operand, then runs the plan.
 int EcapaModel::run(const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int L, const float* lengths, cudaStream_t st) {
-    EcapaModel* const m = this;
-    const int B = m->plan_B, T = m->plan_T;
-    const int Tp = m->Tp, P = m->P, C = m->C, C3 = m->C3;
-    const int64_t R = int64_t(B) * Tp;
-    int rc;
-    auto prof_mark = [&](int kind, bool begin) {
-        if (!m->prof_on) return;
-        if (begin) {
-            if (m->prof_used + 2 > m->prof_ev.size()) {
-                cudaEvent_t a, b;
-                cudaEventCreate(&a);
-                cudaEventCreate(&b);
-                m->prof_ev.push_back(a);
-                m->prof_ev.push_back(b);
-                m->prof_kind.push_back(kind);
-            }
-            m->prof_kind[m->prof_used / 2] = kind;
-            cudaEventRecord(m->prof_ev[m->prof_used], st);
-        } else {
-            cudaEventRecord(m->prof_ev[m->prof_used + 1], st);
-            m->prof_used += 2;
-        }
-    };
+    const int B = plan_B, T = plan_T;
     // `lengths` (ecapa_tdnn.py:245, relative lengths in (0,1]): SEBlock squeezes and ASP pools over the first
     // #{t : t < lengths[b] * T} frames of each utterance (ecapa_tdnn.py:71-75, pooling.py:96-115); everything else sees all T frames.
     const int* nv = nullptr;
     if (lengths) {
-        PPV_REQUIRE(m->cfg.pooling == PPV_POOL_ASP, "ecapa_forward: lengths is implemented for ASP pooling (the other heads ignore it in the reference)");
-        rc = launch_lengths_to_counts(lengths, B, T, m->buf.nvalid, st);
+        PPV_REQUIRE(cfg.pooling == PPV_POOL_ASP, "ecapa_forward: lengths is implemented for ASP pooling (the other heads ignore it in the reference)");
+        int rc = launch_lengths_to_counts(lengths, B, T, buf.nvalid, st);
         if (rc) return rc;
-        nv = m->buf.nvalid;
+        nv = buf.nvalid;
     }
-    prof_mark(1, true);
+    int rc;
+    prof_begin(1, st);
     if (wav) {
-        rc = fbank_run(fb, wav, lens_ratio, B, L, m->buf.raw_logmel, nullptr, m->buf.bufs[B_FEAT], P, Tp, st);
-        m->launches_other += 3;
+        rc = fbank_run(fb, wav, lens_ratio, B, L, buf.raw_logmel, nullptr, buf.feat, P, Tp, st);
+        launches_other += 3;
     } else {
-        rc = launch_pack_features(feat, B, T, m->cfg.input_size, m->buf.bufs[B_FEAT], P, Tp, st);
-        m->launches_other += 1;
+        rc = launch_pack_features(feat, B, T, cfg.input_size, buf.feat, P, Tp, st);
+        launches_other += 1;
     }
-    prof_mark(1, false);
-    if (rc) return rc;
-    for (const Step& s : m->steps) {
-        const bool tensor_step = (s.kind == Step::GEMM || s.kind == Step::ASP_FUSED || s.kind == Step::RES2 || s.kind == Step::RES2CHAIN);
-        // (SKINNY steps count as "other kernels": their FLOPs are not credited to the tensor-core roofline)
-        prof_mark(tensor_step ? 0 : 1, true);
-        if (tensor_step) m->launches_gemm += 1; else m->launches_other += 1;
-        switch (s.kind) {
-            case Step::GEMM: rc = gemm_launch(s.gp, m->precision, m->num_sms, st); break;
-            case Step::SKINNY: rc = skinny_linear_launch(s.sk_x, s.sk_col0, s.sk_w, s.sk_M, s.sk_N, s.sk_K, s.sk_ep, st); break;
-            case Step::RES2: rc = res2conv_launch(s.rp, m->precision, m->num_sms, st); break;
-            case Step::RES2CHAIN:
-                rc = res2chain_launch(s.cp, m->precision, m->num_sms, st);
-                if (s.cp.trace) {
-                    static int dumps = 0;
-                    if (++dumps == 10) res2chain_trace_dump(s.cp);  // a warm launch of the first block
-                }
-                break;
-            case Step::SE_SQUEEZE:
-                rc = launch_colstats(m->buf.bufs[B_Z], 0, C, B, T, P, Tp, 0, 0.f, nullptr, m->buf.bufs[B_SEM], st, 0.f, nv);
-                break;
-            case Step::SE_SCALE: {
-                const Planes& X = (s.blk == 1) ? m->buf.bufs[B_X0] : m->buf.bufs[B_CAT];
-                const int xcol = (s.blk == 1) ? 0 : (s.blk - 2) * C;
-                rc = launch_se_scale_res(m->buf.bufs[B_Z], m->buf.se_scale, X, xcol, m->buf.bufs[B_CAT], (s.blk - 1) * C, C, Tp, R, m->num_sms, st);
-                break;
-            }
-            case Step::ASP_GLOBAL:
-                rc = launch_colstats(m->buf.bufs[B_MFA], 0, C3, B, T, P, Tp, 1, 1e-12f, nullptr, m->buf.bufs[B_GSTAT], st, 0.f, nv);
-                break;
-            case Step::ASP_FUSED: {
-                AspFusedParams ap = s.ap;
-                ap.nvalid = nv;
-                rc = asp_fused_launch(ap, m->precision, m->num_sms, st);
-                break;
-            }
-            case Step::POOL_STATS:
-                rc = launch_colstats(m->buf.bufs[B_MFA], 0, C3, B, T, P, Tp, m->cfg.pooling == PPV_POOL_TAP ? 0 : 3, 0.f, nullptr, m->buf.bufs[B_POOL], st);
-                break;
-        }
-        prof_mark(0, false);
-        if (rc) return rc;
-    }
-    return PPV_OK;
+    prof_end(st);
+    return rc ? rc : run_plan(feat, nv, st);
 }
 
 int ecapa_profile(Model* model, int enable) {
-    EcapaModel* m = static_cast<EcapaModel*>(model);
-    m->prof_on = enable != 0;
-    m->prof_used = 0;
-    m->launches_gemm = m->launches_other = 0;
+    static_cast<EcapaModel*>(model)->profile(enable != 0);
     return PPV_OK;
 }
 
-// Sums the event-pair durations recorded since ecapa_profile(m, 1); synchronises on the last event.
 int ecapa_profile_read(Model* model, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
-    EcapaModel* m = static_cast<EcapaModel*>(model);
     PPV_REQUIRE(gemm_ms && other_ms && gemm_launches && other_launches, "ecapa_profile_read: null argument");
-    double g = 0, o = 0;
-    if (m->prof_used >= 2) PPV_CUDA_OK(cudaEventSynchronize(m->prof_ev[m->prof_used - 1]));
-    for (size_t i = 0; i + 1 < m->prof_used; i += 2) {
-        float ms = 0.f;
-        PPV_CUDA_OK(cudaEventElapsedTime(&ms, m->prof_ev[i], m->prof_ev[i + 1]));
-        (m->prof_kind[i / 2] == 0 ? g : o) += ms;
-    }
-    *gemm_ms = g;
-    *other_ms = o;
-    *gemm_launches = m->launches_gemm;
-    *other_launches = m->launches_other;
-    m->prof_used = 0;
-    m->launches_gemm = m->launches_other = 0;
-    return PPV_OK;
+    return static_cast<EcapaModel*>(model)->profile_read(gemm_ms, other_ms, gemm_launches, other_launches);
 }
 
 int EcapaModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {
-    EcapaModel* const m = this;
-    const int B = m->plan_B, T = m->plan_T, P = m->P, Tp = m->Tp, C = m->C, C3 = m->C3;
+    const int B = plan_B, T = plan_T;
     const Planes* src = nullptr;
     int col0 = 0, cols = 0;
     if (n == "feat") {
-        src = &m->buf.bufs[B_FEAT];
-        cols = m->cfg.input_size;
+        src = &buf.feat;
+        cols = cfg.input_size;
     } else if (n == "blocks.0") {
-        src = &m->buf.bufs[B_X0];
+        src = &buf.x0;
         cols = C;
     } else if (n == "blocks.1" || n == "blocks.2" || n == "blocks.3") {
-        src = &m->buf.bufs[B_CAT];
+        src = &buf.cat;
         col0 = (n.back() - '1') * C;
         cols = C;
     } else if (n == "mfa") {
-        src = &m->buf.bufs[B_MFA];
+        src = &buf.mfa;
         cols = C3;
     } else if (n == "asp") {
         PPV_REQUIRE(out_elems >= size_t(B) * 2 * C3, "ecapa_read_tap: output too small");
-        PPV_CUDA_OK(cudaMemcpyAsync(out, m->buf.pooled_raw, size_t(B) * 2 * C3 * 4, cudaMemcpyDeviceToDevice, st));
+        PPV_CUDA_OK(cudaMemcpyAsync(out, buf.pooled_raw, size_t(B) * 2 * C3 * 4, cudaMemcpyDeviceToDevice, st));
         return PPV_OK;
     } else {
         return fail(PPV_EINVAL, "ecapa_read_tap: unknown tap " + n);

@@ -40,7 +40,7 @@ struct EFuseW {  // layerN_downsample + fuse_modeXYZ
 
 }  // namespace
 
-struct ERes2NetModel : ImagePlanModel {
+struct ERes2NetModel : PlanModel {
     ppv_eres2net_cfg cfg;
     float *stem_w = nullptr, *stem_b = nullptr;
     std::vector<EBlockW> blocks;
@@ -52,7 +52,7 @@ struct ERes2NetModel : ImagePlanModel {
     ImageGeo geo[5];
     Planes stats, stage_out[5], fuse_out[3];
 
-    explicit ERes2NetModel(const ppv_eres2net_cfg& c) : ImagePlanModel("eres2net", c.precision), cfg(c) {}
+    explicit ERes2NetModel(const ppv_eres2net_cfg& c) : PlanModel("eres2net", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
     size_t workspace_bytes(int B, int T) const override;
 
@@ -311,7 +311,7 @@ int ERes2NetModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
             if (rc) return rc;
             res = eb.sc[i];
         }
-        m->steps.push_back(scale_res_step(eb.o3[i], nullptr, res, eb.out[i], C, go, B, ER_RELU_MAX));
+        m->steps.push_back(scale_res_step(eb.o3[i], nullptr, res, 0, eb.out[i], 0, C, go.Hp * go.Wp, go.rows(B), true, ER_RELU_MAX));
         x = eb.out[i];
         m->stage_out[bw.stage] = x;
     }

@@ -1,5 +1,5 @@
-// The 2-D models' shared plan pieces (image_plan.h): image-grid geometry and epilogues, conv routing, the plan step executor, and the
-// kernels every 2-D model runs: the stem conv, the flatten of the last grid to a time-major matrix, and the fp32 image tap.
+// The 2-D models' shared plan pieces (image_plan.h): image-grid geometry, epilogues and taps, 3x3 conv routing, and the kernels every
+// 2-D model runs: the stem conv, the flatten of the last grid to a time-major matrix, and the fp32 image tap.
 #include <stdlib.h>
 
 #include "image_plan.h"
@@ -152,97 +152,8 @@ void image_taps(std::vector<GemmSource>* v, const Planes& p, int col0, int ncols
         for (int dw = -1; dw <= 1; ++dw) v->push_back(GemmSource{p, col0, ncols, dh * g.Wp + dw});
 }
 
-// ------------------------------------------------------------------------------------------------ steps
-PlanStep stem_step(const float* w9, const float* bias, int C0, const Planes& out, const ImageGeo& g, int B) {
-    PlanStep s;
-    s.kind = PlanStep::STEM;
-    s.vec[0] = w9;
-    s.vec[1] = bias;
-    s.C = C0;
-    s.out = out;
-    s.g = g;
-    s.B = B;
-    return s;
-}
-PlanStep scale_res_step(const Planes& z, const float* scale, const Planes& res, const Planes& out, int C, const ImageGeo& g, int B, float relu_max) {
-    PlanStep s;
-    s.kind = PlanStep::SCALE_RES;
-    s.x = z;
-    s.vec[0] = scale;
-    s.y = res;
-    s.out = out;
-    s.C = C;
-    s.g = g;
-    s.B = B;
-    s.relu_max = relu_max;
-    return s;
-}
-PlanStep aff_combine_step(const Planes& x, int xc0, const Planes& y, int yc0, const Planes& t, const Planes& out, int C, int64_t rows) {
-    PlanStep s;
-    s.kind = PlanStep::AFF_COMBINE;
-    s.x = x;
-    s.xc0 = xc0;
-    s.y = y;
-    s.yc0 = yc0;
-    s.t = t;
-    s.out = out;
-    s.C = C;
-    s.rows = rows;
-    return s;
-}
-PlanStep flatten_step(const Planes& in, const ImageGeo& g, int B, int C, const Planes& out) {
-    PlanStep s;
-    s.kind = PlanStep::FLATTEN_IMAGE;
-    s.x = in;
-    s.g = g;
-    s.B = B;
-    s.C = C;
-    s.out = out;
-    return s;
-}
-PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int mode, float eps, const Planes& out, float inv_count) {
-    PlanStep s;
-    s.kind = PlanStep::COLSTATS;
-    s.x = x;
-    s.C = C;
-    s.B = B;
-    s.T = T;
-    s.P = P;
-    s.Tp = Tp;
-    s.mode = mode;
-    s.eps = eps;
-    s.out = out;
-    s.inv_count = inv_count;
-    return s;
-}
-PlanStep model_step(int model_kind) {
-    PlanStep s;
-    s.kind = PlanStep::MODEL;
-    s.model_kind = model_kind;
-    return s;
-}
-
-// ------------------------------------------------------------------------------------------------ conv routing
-int ImagePlanModel::plan_gemm(const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) {
-    ep.bias = gw.bias;
-    PlanStep s;
-    s.kind = PlanStep::GEMM;
-    int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N));
-    if (rc) return rc;
-    steps.push_back(s);
-    return PPV_OK;
-}
-
-int ImagePlanModel::plan_conv(const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) {
-    ep.bias = gw.bias;
-    PlanStep s;
-    if (!pointwise_step_build(&s.pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) return plan_gemm(gw, srcs, M, ep);
-    s.kind = PlanStep::POINTWISE;
-    steps.push_back(s);
-    return PPV_OK;
-}
-
-int ImagePlanModel::plan_conv3x3(const GemmWeights& gw, const Planes& x, int col0, int ncols, const ImageGeo& g, int B, Epilogue ep) {
+// ------------------------------------------------------------------------------------------------ 3x3 conv routing
+int PlanModel::plan_conv3x3(const GemmWeights& gw, const Planes& x, int col0, int ncols, const ImageGeo& g, int B, Epilogue ep) {
     const char* e = getenv("PPV_CONV3X3");  // 0 = every 3x3 conv on the gather-GEMM (debugging / A-B timing)
     const bool patch = !(e && e[0] == '0') && ncols == 32 && gw.N == 32 && gw.Ktot == 9 * 32 && conv3x3_c32_supported(ncols, gw.N, g.H, g.W);
     if (!patch) {
@@ -259,42 +170,15 @@ int ImagePlanModel::plan_conv3x3(const GemmWeights& gw, const Planes& x, int col
     return PPV_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ executor
-int ImagePlanModel::run_steps(const float* feat, cudaStream_t st) {
-    for (const PlanStep& s : steps) {
-        int rc = PPV_OK;
-        switch (s.kind) {
-            case PlanStep::GEMM: rc = gemm_launch(s.gp, precision, num_sms, st); break;
-            case PlanStep::CONV3X3: rc = conv3x3_launch(s.c3, precision, num_sms, st); break;
-            case PlanStep::POINTWISE: rc = pointwise_launch(s.pw, num_sms, st); break;
-            case PlanStep::STEM: rc = launch_stem_conv(feat, s.B, s.g.W, s.g.H, s.vec[0], s.vec[1], s.C, s.out, s.g.Hp, s.g.Wp, st); break;
-            case PlanStep::SCALE_RES:
-                rc = launch_se_scale_res(s.x, s.vec[0], s.y, 0, s.out, 0, s.C, s.g.Hp * s.g.Wp, s.g.rows(s.B), num_sms, st, 1, s.relu_max);
-                break;
-            case PlanStep::AFF_COMBINE: rc = launch_aff_combine(s.x, s.xc0, s.y, s.yc0, s.t, s.out, s.C, s.rows, num_sms, st); break;
-            case PlanStep::FLATTEN_IMAGE: rc = launch_flatten_image(s.x, s.B, s.g.H, s.g.W, s.g.Hp, s.g.Wp, s.C, s.out, num_sms, st); break;
-            case PlanStep::COLSTATS:
-                rc = launch_colstats(s.x, 0, s.C, s.B, s.T, s.P, s.Tp, s.mode, s.eps, nullptr, s.out, st, s.inv_count);
-                break;
-            case PlanStep::ASP_FUSED: rc = asp_fused_launch(s.ap, precision, num_sms, st); break;
-            case PlanStep::MODEL: rc = run_model_step(s, st); break;
-        }
-        if (rc) return rc;
-    }
-    return PPV_OK;
-}
-
-int ImagePlanModel::run_model_step(const PlanStep&, cudaStream_t) { return fail(PPV_EINVAL, std::string(prefix) + ": plan step of unknown kind"); }
-
 // ------------------------------------------------------------------------------------------------ taps
-int ImagePlanModel::name_index(const std::string& n, const char* base, int lo, int hi) {
+int PlanModel::name_index(const std::string& n, const char* base, int lo, int hi) {
     const size_t len = strlen(base);
     if (n.size() != len + 1 || n.compare(0, len, base) != 0) return 0;
     const int i = n[len] - '0';
     return i >= lo && i <= hi ? i : 0;
 }
 
-int ImagePlanModel::image_tap(const Planes& src, const ImageGeo& g, int C, float* out, size_t out_elems, cudaStream_t st) const {
+int PlanModel::image_tap(const Planes& src, const ImageGeo& g, int C, float* out, size_t out_elems, cudaStream_t st) const {
     PPV_REQUIRE(out_elems >= size_t(plan_B) * g.H * g.W * C, std::string(prefix) + "_read_tap: output too small");
     return launch_image_to_f32(src, plan_B, g.H, g.W, g.Hp, g.Wp, C, out, st);
 }

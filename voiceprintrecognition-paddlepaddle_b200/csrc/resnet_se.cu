@@ -28,7 +28,7 @@ struct BlockW {
 
 }  // namespace
 
-struct ResNetSEModel : ImagePlanModel {
+struct ResNetSEModel : PlanModel {
     ppv_resnetse_cfg cfg;
     // weights
     float* conv1_w = nullptr;  // [32][9] BN folded
@@ -42,7 +42,7 @@ struct ResNetSEModel : ImagePlanModel {
     Planes conv1_out, flat, stage_out[5];
     float* pooled_raw = nullptr;
 
-    explicit ResNetSEModel(const ppv_resnetse_cfg& c) : ImagePlanModel("resnetse", c.precision), cfg(c) {}
+    explicit ResNetSEModel(const ppv_resnetse_cfg& c) : PlanModel("resnetse", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
     size_t workspace_bytes(int B, int T) const override;
 
@@ -303,7 +303,7 @@ int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
         e2.sigmoid_ = 1;
         rc = plan_gemm(bw.se2, {GemmSource{rb.se_hid, 0, 64, 0}}, B, e2);
         if (rc) return rc;
-        m->steps.push_back(scale_res_step(rb.out3[i], rb.se_scale, res, rb.blk_out[i], C, gout, B));
+        m->steps.push_back(scale_res_step(rb.out3[i], rb.se_scale, res, 0, rb.blk_out[i], 0, C, gout.Hp * gout.Wp, gout.rows(B), true));
         x = rb.blk_out[i];
         m->stage_out[bw.stage] = x;
     }
