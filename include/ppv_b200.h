@@ -290,6 +290,18 @@ int ppv_cosine_pairlist(const float* E, const int32_t* idx, int64_t P, int n, in
 size_t ppv_audio_prep_workspace_bytes(int B, int max_new_len);
 int ppv_audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, int B,
                    int max_new_len, float target_db, int normalize, int Lout, float* out, void* ws, size_t ws_bytes, void* stream);
+/* The same with reverberation (yeaudio ReverbPerturbAugmentor: full convolution with a room impulse response, not truncated, the
+ * response not normalised) after the noise and before the dB normalisation.  rir_bank = concatenated responses (rir_bank_len samples,
+ * device); rparams [B][2] int32 (device) = {rir_off, rir_len}, rir_len 0 = no reverb for that item, otherwise 1 <= rir_len <= max_rir_len
+ * and rir_off + rir_len <= rir_bank_len.  For an item with a response, crop_start / crop_len in iparams are on its reverberant length
+ * new_len + rir_len - 1.  Items without one come out exactly as from ppv_audio_prep.  rparams live on the device, so a violating entry
+ * cannot be reported here: the kernels read nothing for it and write NaN over that item's output row.  ws: scratch of
+ * ppv_audio_prep_reverb_workspace_bytes(B, max_new_len, max_rir_len) bytes, 256-byte aligned (~2 KB per 256 samples of every
+ * utterance and response). */
+size_t ppv_audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len);
+int ppv_audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise,
+                          const float* rir_bank, int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len,
+                          float target_db, int normalize, int Lout, float* out, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Verification metrics and enrol-DB retrieval on the device.  Replaces ppvector/metric/metrics.py:4-37

@@ -6,13 +6,16 @@
 //   speed   change_speed(r): new_len = int(len / r), samples = np.interp(linspace(0, len, new_len), arange(len), samples)
 //   volume  samples *= 10^(gain_dB / 20)
 //   noise   noise gain = min(rms_dB(signal) - rms_dB(noise) - snr_dB, 300) dB; samples += noise * gain (noise tiled over the utterance)
+//   reverb  samples = fftconvolve(samples, rir, "full"): new_len + R - 1 samples, response not normalised (audio_prep_reverb only)
 //   norm    gain = min(target_dB - rms_dB(samples), 300) dB over the WHOLE utterance (before the crop), rms_dB = 10 log10(mean x^2)
 //   crop    [start, start + crop_len) of the result, zero-padded to the batch's output length
 // Two passes over the samples: (1) per-utterance sums  S_xx, S_nn, S_xn  of the speed-changed signal and its noise segment, from
 // which every gain follows in closed form (the mixture's energy is g^2 S_xx + 2 g g_n S_xn + g_n^2 S_nn); (2) the output.  HBM-bound:
-// ~2 reads of the raw samples + 1 write of the crop.
+// ~2 reads of the raw samples + 1 write of the crop.  Items with a room response take the volume and noise gains from pass 1, and their
+// normalisation from the energy of the reverberant signal, which reverb.cu computes between the two passes.
 #include <math.h>
 
+#include "audio_prep.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -22,51 +25,17 @@ namespace {
 
 constexpr int AP_CHUNK = 8192;  // samples per block in pass 1
 
-struct PrepItem {
-    int raw_len, new_len, crop_start, crop_len, noise_off, noise_len, has_noise;
-    float pos_step, vol_gain_db, snr_db;
-};
-
-__device__ __forceinline__ PrepItem load_item(const int32_t* ip, const float* fp, int b) {
-    PrepItem it;
-    const int32_t* i = ip + b * PPV_PREP_NI;
-    const float* f = fp + b * PPV_PREP_NF;
-    it.raw_len = i[0];
-    it.new_len = i[1];
-    it.crop_start = i[2];
-    it.crop_len = i[3];
-    it.noise_off = i[4];
-    it.noise_len = i[5];
-    it.has_noise = i[6];
-    it.pos_step = f[0];
-    it.vol_gain_db = f[1];
-    it.snr_db = f[2];
-    return it;
-}
-
-// sample j of the speed-changed signal: np.interp(j * pos_step, arange(raw_len), x) with np.interp's clamping beyond the last index
-__device__ __forceinline__ float speed_sample(const float* __restrict__ x, const PrepItem& it, int j) {
-    if (it.new_len == it.raw_len) return x[j];
-    // linspace(0, raw_len, new_len)[j] in double (a float position loses the fraction beyond ~1e6 samples)
-    const double pos = double(j) * (double(it.raw_len) / double(max(it.new_len - 1, 1)));
-    int i0 = int(pos);
-    if (i0 >= it.raw_len - 1) return x[it.raw_len - 1];
-    const float fr = float(pos - double(i0));
-    const float a = x[i0], c = x[i0 + 1];
-    return a + fr * (c - a);
-}
-
 __global__ void __launch_bounds__(256) prep_stats_kernel(const float* __restrict__ wav, int64_t wav_ld, const int32_t* __restrict__ ip,
                                                          const float* __restrict__ fp, const float* __restrict__ noise, int nchunk,
                                                          double* __restrict__ partial) {
     __shared__ double red[3][8];
     const int b = blockIdx.y, chunk = blockIdx.x;
-    const PrepItem it = load_item(ip, fp, b);
+    const PrepItem it = prep_load_item(ip, fp, b);
     const float* x = wav + int64_t(b) * wav_ld;
     double sxx = 0.0, snn = 0.0, sxn = 0.0;
     const int j0 = chunk * AP_CHUNK, j1 = min(it.new_len, j0 + AP_CHUNK);
     for (int j = j0 + threadIdx.x; j < j1; j += blockDim.x) {
-        const float v = speed_sample(x, it, j);
+        const float v = prep_speed_sample(x, it, j);
         sxx += double(v) * double(v);
         if (it.has_noise) {
             const float n = noise[it.noise_off + (j % it.noise_len)];
@@ -93,12 +62,13 @@ __global__ void __launch_bounds__(256) prep_stats_kernel(const float* __restrict
     }
 }
 
-// gains[b] = {signal gain, noise gain} including the dB normalisation
+// gains[b] = {signal gain, noise gain} including the dB normalisation -- except for items with a room response (rparams, may be null):
+// their normalisation follows the convolution (reverb.cu)
 __global__ void prep_gains_kernel(const int32_t* __restrict__ ip, const float* __restrict__ fp, const double* __restrict__ partial, int nchunk,
-                                  int B, float target_db, int normalize, float* __restrict__ gains) {
+                                  int B, float target_db, int normalize, const int32_t* __restrict__ rparams, float* __restrict__ gains) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const PrepItem it = load_item(ip, fp, b);
+    const PrepItem it = prep_load_item(ip, fp, b);
     double sxx = 0.0, snn = 0.0, sxn = 0.0;
     const int used = (it.new_len + AP_CHUNK - 1) / AP_CHUNK;
     for (int c = 0; c < used; ++c) {
@@ -114,7 +84,7 @@ __global__ void prep_gains_kernel(const int32_t* __restrict__ ip, const float* _
         gn = pow(10.0, fmin(sig_db - noise_db - double(it.snr_db), 300.0) / 20.0);
     }
     double gnorm = 1.0;
-    if (normalize) {
+    if (normalize && prep_rir_len(rparams, b) == 0) {
         const double ms = (g * g * sxx + 2.0 * g * gn * sxn + gn * gn * snn) / n;
         if (ms > 0.0) gnorm = pow(10.0, fmin(double(target_db) - 10.0 * log10(ms), 300.0) / 20.0);
     }
@@ -122,21 +92,27 @@ __global__ void prep_gains_kernel(const int32_t* __restrict__ ip, const float* _
     gains[2 * b + 1] = float(gn * gnorm);
 }
 
+// out[b] = the crop window of the prepared signal, zero-padded to Lout.  Items with a room response (rparams, may be null) find their
+// un-normalised reverberant crop window in out already (reverb.cu) and gains[2b] = its normalisation gain.
 __global__ void __launch_bounds__(256) prep_apply_kernel(const float* __restrict__ wav, int64_t wav_ld, const int32_t* __restrict__ ip,
                                                          const float* __restrict__ fp, const float* __restrict__ noise,
-                                                         const float* __restrict__ gains, int Lout, float* __restrict__ out) {
+                                                         const float* __restrict__ gains, const int32_t* __restrict__ rparams, int Lout,
+                                                         float* __restrict__ out) {
     const int b = blockIdx.y;
-    const PrepItem it = load_item(ip, fp, b);
+    const PrepItem it = prep_load_item(ip, fp, b);
     const float* x = wav + int64_t(b) * wav_ld;
     const float gs = gains[2 * b], gn = gains[2 * b + 1];
     float* dst = out + int64_t(b) * Lout;
+    const int rlen = prep_rir_len(rparams, b);
+    if (rlen != 0) {
+        const int ly = it.new_len + rlen - 1;
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lout; i += gridDim.x * blockDim.x)
+            dst[i] = (i < it.crop_len && it.crop_start + i < ly) ? dst[i] * gs : 0.f;
+        return;
+    }
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lout; i += gridDim.x * blockDim.x) {
         float v = 0.f;
-        if (i < it.crop_len) {
-            const int j = it.crop_start + i;
-            v = speed_sample(x, it, j) * gs;
-            if (it.has_noise) v = fmaf(noise[it.noise_off + (j % it.noise_len)], gn, v);
-        }
+        if (i < it.crop_len) v = prep_mixed_sample(x, noise, it, it.crop_start + i, gs, gn);
         dst[i] = v;
     }
 }
@@ -161,10 +137,43 @@ int audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, const f
     double* partial = static_cast<double*>(ws);
     float* gains = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + ((size_t(B) * nchunk * 3 * sizeof(double) + 255) / 256) * 256);
     prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, partial);
-    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, partial, nchunk, B, target_db, normalize, gains);
+    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, partial, nchunk, B, target_db, normalize, nullptr, gains);
     const int gx = std::max(1, std::min((Lout + 255) / 256, 64));
-    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, Lout, out);
+    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, nullptr, Lout, out);
     PPV_LAUNCH_OK("audio_prep kernels");
+    return PPV_OK;
+}
+
+size_t audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len) {
+    if (B <= 0 || max_new_len <= 0 || max_rir_len <= 0) return 0;
+    return audio_prep_workspace_bytes(B, max_new_len) + reverb_workspace_bytes(B, max_new_len, max_rir_len);
+}
+
+// audio_prep with reverberation after the noise: rparams [B][2] = {rir_off, rir_len} into rir_bank (rir_bank_len samples), rir_len 0 = no
+// reverb for that item.  An item with a response has crop_start / crop_len on its reverberant length new_len + rir_len - 1.  Same stats
+// and gains passes (reverb items leave the normalisation out), then reverb.cu's convolution and normalisation, then the same apply pass.
+int audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
+                      int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
+                      int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    PPV_REQUIRE(wav && iparams && fparams && rir_bank && rparams && out && ws, "audio_prep_reverb: null argument");
+    PPV_REQUIRE(B > 0 && max_new_len > 0 && Lout > 0, "audio_prep_reverb: empty batch");
+    PPV_REQUIRE(max_rir_len > 0 && int64_t(max_rir_len) <= rir_bank_len, "audio_prep_reverb: max_rir_len outside [1, rir_bank_len]");
+    PPV_REQUIRE(int64_t(max_new_len) + max_rir_len - 1 <= INT32_MAX - 512, "audio_prep_reverb: reverberant length exceeds int32");
+    PPV_REQUIRE(ws_bytes >= audio_prep_reverb_workspace_bytes(B, max_new_len, max_rir_len) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0,
+                "audio_prep_reverb: workspace too small / unaligned");
+    const size_t base = audio_prep_workspace_bytes(B, max_new_len);
+    const int nchunk = (max_new_len + AP_CHUNK - 1) / AP_CHUNK;
+    double* partial = static_cast<double*>(ws);
+    float* gains = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + ((size_t(B) * nchunk * 3 * sizeof(double) + 255) / 256) * 256);
+    prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, partial);
+    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, partial, nchunk, B, target_db, normalize, rparams, gains);
+    PPV_LAUNCH_OK("audio_prep_reverb stats / gains");
+    const int rc = reverb_run(wav, wav_ld, iparams, fparams, noise, rir_bank, rir_bank_len, rparams, B, max_new_len, max_rir_len, target_db,
+                              normalize, Lout, out, gains, static_cast<uint8_t*>(ws) + base, st);
+    if (rc != PPV_OK) return rc;
+    const int gx = std::max(1, std::min((Lout + 255) / 256, 64));
+    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, rparams, Lout, out);
+    PPV_LAUNCH_OK("audio_prep_reverb apply");
     return PPV_OK;
 }
 

@@ -143,6 +143,18 @@ int ppv_audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, con
     PPV_GUARD_END
 }
 
+size_t ppv_audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len) {
+    return audio_prep_reverb_workspace_bytes(B, max_new_len, max_rir_len);
+}
+int ppv_audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise,
+                          const float* rir_bank, int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len,
+                          float target_db, int normalize, int Lout, float* out, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    return audio_prep_reverb(wav, wav_ld, iparams, fparams, noise, rir_bank, rir_bank_len, rparams, B, max_new_len, max_rir_len, target_db,
+                             normalize, Lout, out, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+
 // ---------------------------------------------------------------- model
 void ppv_ecapa_default_cfg(ppv_ecapa_cfg* c) {
     if (c) ppv_ecapa_default_cfg_impl(c);

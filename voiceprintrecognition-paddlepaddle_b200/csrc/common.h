@@ -306,6 +306,16 @@ int fbank_run(Fbank* h, const float* wav, const float* lens_ratio, int B, int L,
 size_t audio_prep_workspace_bytes(int B, int max_new_len);
 int audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, int B, int max_new_len,
                float target_db, int normalize, int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+size_t audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len);
+int audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
+                      int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
+                      int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+
+// ---- reverb.cu: the convolution stage of audio_prep_reverb (gains [B][2] in: signal / noise gains, out: normalisation gain of reverb items)
+size_t reverb_workspace_bytes(int B, int max_new_len, int max_rir_len);
+int reverb_run(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
+               int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
+               int Lout, float* out, float* gains, void* ws, cudaStream_t st);
 
 // ---- spectral.cu ------------------------------------------------------------------------------------
 struct Spectral;

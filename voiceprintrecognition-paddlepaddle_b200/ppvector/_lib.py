@@ -122,6 +122,9 @@ SIGNATURES = {
     "ppv_fbank_forward_ragged": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P]),
     "ppv_audio_prep_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "ppv_audio_prep": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
+    "ppv_audio_prep_reverb_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "ppv_audio_prep_reverb": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_int64, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int,
+                                        _P, _P, C.c_size_t, _P]),
     "ppv_eer_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "ppv_eer_mindcf": (C.c_int, [_P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, _P, _P, C.c_size_t, _P]),
     "ppv_eer_mindcf_matrix": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, C.c_size_t, _P]),

@@ -3,10 +3,11 @@
 List file lines are ``path\\tlabel``; items are ``(feature [T,F] float32 CUDA tensor, speaker id)``.  Audio goes
 wav -> float32 -> (resample) -> dB normalise -> crop (eval: from 0; train: random start; extract_feature: no crop) ->
 ``AudioFeaturizer`` on the GPU -> SpecAugment (train mode, reader.py:105-107, ``ppv_spec_augment``).  ``.npy`` entries are
-pre-extracted features (reader.py:78-83).  Waveform augmentation (reader.py:143-163: speed / volume / noise), dB normalisation and
-the crop run on the GPU (``ppvector.data_utils.audio_batch``, ``ppv_audio_prep``); ``load_batch`` prepares a whole batch with one
-launch sequence (decode on the host, then audio prep -> ragged Fbank -> SpecAugment), which is what ``PPVectorTrainer.train`` uses.
-Reverb augmentation raises."""
+pre-extracted features (reader.py:78-83).  Waveform augmentation (reader.py:143-163: speed / volume / noise / reverb), dB normalisation
+and the crop run on the GPU (``ppvector.data_utils.audio_batch``, ``ppv_audio_prep`` / ``ppv_audio_prep_reverb``); ``load_batch`` prepares
+a whole batch with one launch sequence (decode on the host, then audio prep -> ragged Fbank -> SpecAugment), which is what
+``PPVectorTrainer.train`` uses.  With reverb the utterance grows by the response's length - 1 before the crop, as in the reference, so
+the crop decision and its random start are taken on the reverberant length."""
 import random
 
 import numpy as np
@@ -14,7 +15,7 @@ import torch
 from tqdm import tqdm
 
 from ppvector.data_utils.audio import AudioSegment
-from ppvector.data_utils.audio_batch import WaveAugmentor, prepare_batch
+from ppvector.data_utils.audio_batch import WaveAugmentor, augmented_len, prepare_batch
 from ppvector.data_utils.featurizer import AudioFeaturizer
 from ppvector.data_utils.spec_aug import SpecAugmentor
 
@@ -62,14 +63,21 @@ class PPVectorDataset(torch.utils.data.Dataset):
 
     def _plan(self, x, spk_id):
         """The random decisions of one utterance, in the reference's order: augmentation draws (reader.py:153-163), then the crop start
-        (reader.py:100-101).  -> (draw dict or None, (crop_start, crop_len or None), label)"""
+        (reader.py:100-101) on the augmented length (speed-changed, plus a drawn room response's length - 1).
+        -> (draw dict or None, (crop_start, crop_len or None), label)"""
         draw = self.wave_augment.draw(x.shape[0], spk_id) if self.wave_augment is not None else None
-        new_len = x.shape[0] if not draw or draw['speed_rate'] == 1.0 else int(x.shape[0] / draw['speed_rate'])
+        new_len = augmented_len(x.shape[0], draw)
         crop = (0, None)
         n = int(self.max_duration * self._target_sample_rate)
         if self.mode != 'extract_feature' and new_len / float(self._target_sample_rate) > self.max_duration:
             crop = (random.randint(0, new_len - n) if self.mode == 'train' else 0, n)
         return draw, crop, (draw['spk_id'] if draw else spk_id)
+
+    def _banks(self):
+        """(noise bank, room response bank) of the wave augmentor, None where absent"""
+        if self.wave_augment is None:
+            return None, None
+        return self.wave_augment.noise_bank, self.wave_augment.rir_bank
 
     def _npy_feature(self, idx):
         feature = np.load(self.lines[idx].strip().split('\t')[0])
@@ -86,9 +94,9 @@ class PPVectorDataset(torch.utils.data.Dataset):
         if any(x is None for x, _ in decoded):
             return collate_fn([self[int(i)] for i in indices])
         plans = [self._plan(x, spk) for x, spk in decoded]
-        noise_bank = self.wave_augment.noise_bank if self.wave_augment is not None else None
+        noise_bank, rir_bank = self._banks()
         wav, lens = prepare_batch([x for x, _ in decoded], [p[0] for p in plans], [p[1] for p in plans], target_db=self._target_dB,
-                                  normalize=self._use_dB_normalization, noise_bank=noise_bank, device=self.device)
+                                  normalize=self._use_dB_normalization, noise_bank=noise_bank, device=self.device, rir_bank=rir_bank)
         feats, frames = self.audio_featurizer.forward_ragged(wav, lens)
         if self.mode == 'train' and self.spec_augment is not None:  # reader.py:105-107
             feats = self.spec_augment(feats, num_frames=frames)
@@ -100,9 +108,9 @@ class PPVectorDataset(torch.utils.data.Dataset):
             feature = self._npy_feature(idx)
         else:
             draw, crop, spk_id = self._plan(x, spk_id)
-            noise_bank = self.wave_augment.noise_bank if self.wave_augment is not None else None
+            noise_bank, rir_bank = self._banks()
             wav, lens = prepare_batch([x], [draw], [crop], target_db=self._target_dB, normalize=self._use_dB_normalization,
-                                      noise_bank=noise_bank, device=self.device)
+                                      noise_bank=noise_bank, device=self.device, rir_bank=rir_bank)
             feature = self.audio_featurizer(wav[0, :lens[0]]).squeeze(0)
         if self.mode == 'train' and self.spec_augment is not None:  # reader.py:105-107
             feature = self.spec_augment(feature)
