@@ -426,6 +426,22 @@ size_t ppv_gemm_test_workspace_bytes(int M, int N, int K) {
     const size_t Kp = au(size_t(K), 64);
     return au(au(size_t(M), 128) * Kp * 4, 256) + au(au(size_t(N), 256) * Kp * 4, 256) + 256;
 }
+// Both hooks' operands in the workspace, zero-padded: A as planes [2][pad128(M)][Kp], then W as planes [2][pad256(N)][Kp], Kp = pad64(K).
+static int gemm_test_stage(const float* A, const float* W, int M, int N, int K, void* ws, cudaStream_t st, Planes* pa, Planes* pw) {
+    const int Kp = int(au(size_t(K), 64));
+    pa->rows = int64_t(au(size_t(M), 128));
+    pa->ld = Kp;
+    pa->plane_stride = pa->rows * Kp;
+    pa->base = static_cast<__nv_bfloat16*>(ws);
+    pw->rows = int64_t(au(size_t(N), 256));
+    pw->ld = Kp;
+    pw->plane_stride = pw->rows * Kp;
+    pw->base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + au(size_t(pa->plane_stride) * 4, 256));
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, ppv_gemm_test_workspace_bytes(M, N, K), st));
+    int rc = launch_f32_to_planes(A, M, K, *pa, st);
+    if (rc) return rc;
+    return launch_f32_to_planes(W, N, K, *pw, st);
+}
 int ppv_gemm_test(const float* A, const float* W, const float* bias, const float* bn_scale, const float* bn_shift, int relu, int M,
                   int N, int K, int block_n, int block_k, int precision, float* out, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
@@ -434,22 +450,10 @@ int ppv_gemm_test(const float* A, const float* W, const float* bias, const float
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Kp = int(au(size_t(K), 64));
     Planes pa, pw;
-    pa.rows = int64_t(au(size_t(M), 128));
-    pa.ld = Kp;
-    pa.plane_stride = pa.rows * Kp;
-    pa.base = static_cast<__nv_bfloat16*>(ws);
-    pw.rows = int64_t(au(size_t(N), 256));
-    pw.ld = Kp;
-    pw.plane_stride = pw.rows * Kp;
-    pw.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + au(size_t(pa.plane_stride) * 4, 256));
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, ppv_gemm_test_workspace_bytes(M, N, K), st));
-    rc = launch_f32_to_planes(A, M, K, pa, st);
+    rc = gemm_test_stage(A, W, M, N, K, ws, st, &pa, &pw);
     if (rc) return rc;
-    rc = launch_f32_to_planes(W, N, K, pw, st);
-    if (rc) return rc;
-    GemmSource src{pa, 0, Kp, 0};
+    GemmSource src{pa, 0, pa.ld, 0};
     Epilogue ep;
     ep.bias = bias;
     ep.relu = relu;
@@ -478,22 +482,10 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Kp = int(au(size_t(K), 64));
     Planes pa, pw;
-    pa.rows = int64_t(au(size_t(M), 128));
-    pa.ld = Kp;
-    pa.plane_stride = pa.rows * Kp;
-    pa.base = static_cast<__nv_bfloat16*>(ws);
-    pw.rows = int64_t(au(size_t(N), 256));
-    pw.ld = Kp;
-    pw.plane_stride = pw.rows * Kp;
-    pw.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + au(size_t(pa.plane_stride) * 4, 256));
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, ppv_gemm_test_workspace_bytes(M, N, K), st));
-    rc = launch_f32_to_planes(A, M, K, pa, st);
+    rc = gemm_test_stage(A, W, M, N, K, ws, st, &pa, &pw);
     if (rc) return rc;
-    rc = launch_f32_to_planes(W, N, K, pw, st);
-    if (rc) return rc;
-    GemmSource src{pa, 0, Kp, 0};
+    GemmSource src{pa, 0, pa.ld, 0};
     Epilogue ep;
     ep.bias = bias;
     ep.rowgrp_bias = rowgrp_bias;

@@ -29,6 +29,21 @@
 
 namespace ppv {
 
+constexpr int GEMM_MAX_STAGES = 8;  // barrier slots
+
+// The shared-memory ring of an n-tile BN wide with BK-element k-steps: bytes per stage (the A and W tiles, hi and, for
+// bf16x3, lo planes), as many stages as fit the 227 KB opt-in beside 1024 bytes of alignment slack and 256 of barriers, and
+// the dynamic shared memory that takes.
+struct GemmRing {
+    int stage_bytes, stages, smem_bytes;
+};
+constexpr GemmRing gemm_ring(int BN, int BK, int nsplit) {
+    const int stage_bytes = (nsplit == 3 ? 2 : 1) * (GEMM_BM + BN) * BK * 2;
+    const int fit = (232448 - 1024 - 256) / stage_bytes;
+    const int stages = fit > GEMM_MAX_STAGES ? GEMM_MAX_STAGES : fit;
+    return {stage_bytes, stages, 1024 + stages * stage_bytes + 256};
+}
+
 // BK = K elements per pipeline stage: 64 (128-byte rows, SWIZZLE_128B) or 32 (64-byte rows, SWIZZLE_64B).  The smaller
 // stage keeps the same bytes per MMA but doubles the number of ring slots, i.e. more TMA bytes in flight for the same
 // shared memory.
@@ -38,13 +53,11 @@ struct GemmCfg {
     static constexpr int NB = NA;
     static constexpr int A_BYTES = GEMM_BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = NA * A_BYTES + NB * B_BYTES;
-    static constexpr int BAR_BYTES = 256;
-    static constexpr int MAX_SMEM = 232448;  // 227 KB
-    static constexpr int STAGES_RAW = (MAX_SMEM - 1024 - BAR_BYTES) / STAGE_BYTES;
-    static constexpr int MAX_STAGES = 8;  // barrier slots
-    static constexpr int STAGES = STAGES_RAW > MAX_STAGES ? MAX_STAGES : STAGES_RAW;
-    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + BAR_BYTES;
+    static constexpr GemmRing RING = gemm_ring(BN, BK, NSPLIT);
+    static constexpr int STAGE_BYTES = RING.stage_bytes;
+    static constexpr int STAGES = RING.stages;
+    static constexpr int SMEM_BYTES = RING.smem_bytes;
+    static_assert(STAGE_BYTES == NA * A_BYTES + NB * B_BYTES, "stage layout");
     // Ping-pong schedule (each MMA warpgroup owns whole tiles, two m64 x BN accumulators) where a tile fits in registers: BN <= 128.
     // BN = 256 would need 256 accumulator registers per thread and keeps the cooperative schedule (both warpgroups share every tile).
     static constexpr bool PINGPONG = BN <= 128;
@@ -69,7 +82,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     const uint32_t tiles_base = smem_base;
     const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
     // barrier layout (8 B each): full[8], empty[8], resident-weights barrier
-    constexpr int MAXST = Cfg::MAX_STAGES;
+    constexpr int MAXST = GEMM_MAX_STAGES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (MAXST + s); };
     const uint32_t w_full = bar_base + 8u * (2 * MAXST);
@@ -178,27 +191,38 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                 }
             }
         }
-    } else if constexpr (Cfg::PINGPONG) {
+    } else {
         setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
-        // ===================== MMA + epilogue, ping-pong: warpgroup g owns the CTA's tiles g, g + 2, g + 4, ... =====================
-        // A tile is two m64 x BN accumulators (rows 0-63 and 64-127).  The producer fills the ring in tile order and the warpgroup that
-        // consumes a slot releases it.  Ordered hand-off: a warpgroup starts its k-loop only once the other has waited for every k-step of
-        // the tile before (named barrier 1 + g, arrived at by the other warpgroup).  So the k-loops run one after the other, one
-        // warpgroup's epilogue runs under the other's MMAs, and no warpgroup ever waits for a ring slot more than one fill ahead of the
-        // last completed one (an mbarrier parity wait cannot tell fill k from fill k + 2).
+        // ===================== MMA + epilogue =====================
+        // Ping-pong (BN <= 128): warpgroup g owns the CTA's tiles g, g + 2, g + 4, ... whole, as two m64 x BN accumulators (rows 0-63
+        // and 64-127), and skips the ring positions of the other's tiles.  The producer fills the ring in tile order and the warpgroup
+        // that consumes a slot releases it.  Ordered hand-off: a warpgroup starts its k-loop only once the other has waited for every
+        // k-step of the tile before (named barrier 1 + g, arrived at by the other warpgroup).  So the k-loops run one after the other,
+        // one warpgroup's epilogue runs under the other's MMAs, and no warpgroup ever waits for a ring slot more than one fill ahead of
+        // the last completed one (an mbarrier parity wait cannot tell fill k from fill k + 2).
+        // Cooperative (BN = 256): warpgroup g owns rows [64 g, 64 g + 64) of every tile, one accumulator; both release each slot.
+        constexpr bool PP = Cfg::PINGPONG;
+        constexpr int NACC = PP ? 2 : 1;  // m64 x BN accumulators per warpgroup: acc0[, acc1]
         const int g = (warp - 4) >> 2;
         const int t = threadIdx.x & 127;
-        constexpr uint32_t A_HALF = 64 * BK * 2;  // 64 rows of the A tile (a whole number of 8-row swizzle groups)
+        constexpr uint32_t A_M64 = 64 * BK * 2;  // 64 rows of the A tile (a whole number of 8-row swizzle groups)
+        auto m64 = [&](int h) { return PP ? h : g; };  // the 64-row block of the tile that accumulator h holds
         const int my_tiles = blockIdx.x < num_tiles ? (num_tiles - 1 - int(blockIdx.x)) / int(gridDim.x) + 1 : 0;
         int stage = 0;
         uint32_t phase = 0;
         float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+        // the MMAs of one 16-wide K slice: acc0, then acc1.  K advance inside the swizzle atom: +32 B (16 bf16) per MMA => +2 in the
+        // descriptor's start field
+        auto mma = [&](uint64_t a0, uint64_t a1, uint64_t b, int k, uint32_t scale_d) {
+            wgmma_bf16<BN>(acc0, a0 + 2 * k, b + 2 * k, scale_d);
+            if (PP) wgmma_bf16<BN>(acc1, a1 + 2 * k, b + 2 * k, scale_d);
+        };
         if (gp.ws) mbar_wait(w_full, 0);
         int local = 0;  // index of the tile among this CTA's tiles
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-            if ((local & 1) != g) {  // the other warpgroup's tile: skip its nk ring positions
+            if (PP && (local & 1) != g) {  // the other warpgroup's tile: skip its nk ring positions
                 const int adv = stage + nk;
                 phase ^= uint32_t((adv / nst) & 1);
                 stage = adv % nst;
@@ -207,38 +231,30 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             const int m0 = tile_m(tile) * GEMM_BM;
             const int n0 = tile_n(tile) * BN;
             const bool tr = trace_cta && t == 0 && local < GEMM_TRACE_TILES;
-            named_bar_sync_if(local > 0, 1 + g, 2 * 128);  // the other warpgroup has taken every k-step of tile local - 1
+            if (PP) named_bar_sync_if(local > 0, 1 + g, 2 * 128);  // the other warpgroup has taken every k-step of tile local - 1
             stamp(tr, 1 + g, local, 0);
             int prev = -1;
             wgmma_fence_acc(acc0);
-            wgmma_fence_acc(acc1);
+            if (PP) wgmma_fence_acc(acc1);
             for (int s = 0; s < nk; ++s) {
                 mbar_wait(full_bar(stage), phase);
                 stamp(tr && s == 0, 1 + g, local, 1);
                 const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
                 const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
-                const uint64_t a0_hi = make_kmajor_desc<BK>(sa), a1_hi = make_kmajor_desc<BK>(sa + A_HALF);
+                const uint64_t a0_hi = make_kmajor_desc<BK>(sa + m64(0) * A_M64), a1_hi = make_kmajor_desc<BK>(sa + m64(1) * A_M64);
                 const uint64_t b_hi = make_kmajor_desc<BK>(sb);
                 wgmma_fence();
-                // per accumulator the same order as the cooperative schedule: hi*hi, lo*hi, hi*lo, k ascending in each
+                // per accumulator hi*hi, lo*hi, hi*lo, k ascending in each
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    wgmma_bf16<BN>(acc0, a0_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
-                    wgmma_bf16<BN>(acc1, a1_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
-                }
+                for (int k = 0; k < BK / 16; ++k) mma(a0_hi, a1_hi, b_hi, k, (s > 0 || k > 0) ? 1u : 0u);
                 if (NSPLIT == 3) {
-                    const uint64_t a0_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES), a1_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES + A_HALF);
+                    const uint32_t sa_lo = sa + Cfg::A_BYTES;
+                    const uint64_t a0_lo = make_kmajor_desc<BK>(sa_lo + m64(0) * A_M64), a1_lo = make_kmajor_desc<BK>(sa_lo + m64(1) * A_M64);
                     const uint64_t b_lo = make_kmajor_desc<BK>(sb + Cfg::B_BYTES);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        wgmma_bf16<BN>(acc0, a0_lo + 2 * k, b_hi + 2 * k, 1u);
-                        wgmma_bf16<BN>(acc1, a1_lo + 2 * k, b_hi + 2 * k, 1u);
-                    }
+                    for (int k = 0; k < BK / 16; ++k) mma(a0_lo, a1_lo, b_hi, k, 1u);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        wgmma_bf16<BN>(acc0, a0_hi + 2 * k, b_lo + 2 * k, 1u);
-                        wgmma_bf16<BN>(acc1, a1_hi + 2 * k, b_lo + 2 * k, 1u);
-                    }
+                    for (int k = 0; k < BK / 16; ++k) mma(a0_hi, a1_hi, b_lo, k, 1u);
                 }
                 wgmma_commit();
                 stamp(tr && s == nk - 1, 1 + g, local, 2);
@@ -253,83 +269,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             }
             wgmma_wait<0>();
             stamp(tr, 1 + g, local, 3);
-            // the other warpgroup may start tile local + 1
-            named_bar_arrive_if(local + 1 < my_tiles, 1 + (g ^ 1), 2 * 128);
+            if (PP) named_bar_arrive_if(local + 1 < my_tiles, 1 + (g ^ 1), 2 * 128);  // the other warpgroup may start tile local + 1
             wgmma_fence_acc(acc0);
-            wgmma_fence_acc(acc1);
+            if (PP) wgmma_fence_acc(acc1);
             if (t == 0) mbar_arrive(empty_bar(prev));
             stamp_release(tr, 1 + g, local, nk - 1);
             stamp(tr, 1 + g, local, 4);
             const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
-            // rows 0-63 from acc0, then rows 64-127 moved down into acc0: one copy of the epilogue code
+            // acc0, then (ping-pong) acc1 moved down into acc0: one copy of the epilogue code
 #pragma unroll 1
-            for (int h = 0; h < 2; ++h) {
-                const int rbase = m0 + 64 * h;
+            for (int h = 0; h < NACC; ++h) {
+                const int rbase = m0 + 64 * m64(h);
                 gemm_epilogue<BN>(gp.epi, gp.N, n0, acc0, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
+                if (PP)
 #pragma unroll
-                for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
+                    for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
             }
-            stamp(tr, 1 + g, local, 5);
-        }
-    } else {
-        setmaxnreg_inc<232>();  // 128 x 40 + 256 x 232 <= 64 K registers
-        // ===================== MMA + epilogue: warpgroup g owns rows [64 g, 64 g + 64) of every tile =====================
-        const int g = (warp - 4) >> 2;
-        const int t = threadIdx.x & 127;
-        constexpr uint32_t A_WG_OFF = 64 * BK * 2;  // 64 rows of the A tile (a whole number of 8-row swizzle groups)
-        int stage = 0;
-        uint32_t phase = 0;
-        float acc[BN / 2];
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-        if (gp.ws) mbar_wait(w_full, 0);
-        int local = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-            const int m0 = tile_m(tile) * GEMM_BM;
-            const int n0 = tile_n(tile) * BN;
-            const bool tr = trace_cta && t == 0 && local < GEMM_TRACE_TILES;
-            stamp(tr, 1 + g, local, 0);
-            int prev = -1;
-            wgmma_fence_acc(acc);
-            for (int s = 0; s < nk; ++s) {
-                mbar_wait(full_bar(stage), phase);
-                stamp(tr && s == 0, 1 + g, local, 1);
-                const uint32_t sa = tiles_base + stage * Cfg::STAGE_BYTES;
-                const uint32_t sb = gp.ws ? w_res + s * Cfg::NB * Cfg::B_BYTES : sa + Cfg::NA * Cfg::A_BYTES;
-                const uint64_t a_hi = make_kmajor_desc<BK>(sa + g * A_WG_OFF);
-                const uint64_t b_hi = make_kmajor_desc<BK>(sb);
-                wgmma_fence();
-                // K advance inside the swizzle atom: +32 B (16 bf16) per MMA => +2 in the descriptor's start field
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, (s > 0 || k > 0) ? 1u : 0u);
-                if (NSPLIT == 3) {
-                    const uint64_t a_lo = make_kmajor_desc<BK>(sa + Cfg::A_BYTES + g * A_WG_OFF);
-                    const uint64_t b_lo = make_kmajor_desc<BK>(sb + Cfg::B_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
-                }
-                wgmma_commit();
-                stamp(tr && s == nk - 1, 1 + g, local, 2);
-                wgmma_wait<1>();  // the previous k-step's MMAs have retired: its ring slot is free
-                if (prev >= 0 && t == 0) mbar_arrive(empty_bar(prev));
-                stamp_release(tr, 1 + g, local, s - 1);
-                prev = stage;
-                if (++stage == nst) {
-                    stage = 0;
-                    phase ^= 1u;
-                }
-            }
-            wgmma_wait<0>();
-            stamp(tr, 1 + g, local, 3);
-            wgmma_fence_acc(acc);
-            if (t == 0) mbar_arrive(empty_bar(prev));
-            stamp_release(tr, 1 + g, local, nk - 1);
-            stamp(tr, 1 + g, local, 4);
-            const int64_t shift = int64_t(tile / mn_tiles) * gp.lin_split_rows;
-            const int rbase = m0 + 64 * g;
-            gemm_epilogue<BN>(gp.epi, gp.N, n0, acc, [&](int r) -> int64_t { return rbase + r < gp.M ? int64_t(rbase + r) : -1; }, t, shift);
             stamp(tr, 1 + g, local, 5);
         }
     }
@@ -373,6 +328,25 @@ int encode_planes_map_ex(CUtensorMap* m, const Planes& t, int box_cols, int box_
 // 3-D map over split planes [2][rows][ld] bf16, box = {64 cols, box_rows, 1 plane}, SWIZZLE_128B.
 int encode_planes_map(CUtensorMap* m, const Planes& t, int box_rows) { return encode_planes_map_ex(m, t, GEMM_BK, box_rows, 128); }
 
+// The set-up both builders share: zeroed parameters; A map 0 in every A-map slot, since the producer prefetches all of them
+// (gemm_build overwrites the slots of further A tensors); the tiling and n-tile width; the epilogue, with the test for paired fp32 stores.
+static int gemm_params_init(GemmParams* gp, const Planes& a0, int M, int N, int BN, int BK, const Epilogue& epi) {
+    memset(gp, 0, sizeof(*gp));
+    int rc = encode_planes_map_ex(&gp->mapA[0], a0, BK, GEMM_BM, BK * 2);
+    if (rc) return rc;
+    for (int j = 1; j < GEMM_MAX_MAPS; ++j) gp->mapA[j] = gp->mapA[0];
+    gp->bk = BK;
+    gp->M = M;
+    gp->N = N;
+    gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
+    gp->n_tiles = (N + BN - 1) / BN;
+    gp->bn = BN;
+    gp->epi = epi;
+    if (epi.out_mode == OUT_F32)
+        gp->epi.f32_vec_ok = ((epi.out_ld % 2) == 0 && (epi.out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(epi.out) & 7) == 0) ? 1 : 0;
+    return PPV_OK;
+}
+
 int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W, int M, int N, const Epilogue& epi,
                int BN, int BK) {
     if (BK == 0) {
@@ -384,10 +358,12 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
     PPV_REQUIRE(BN == 64 || BN == 128 || BN == 256, "gemm_build: BN must be 64/128/256");
     PPV_REQUIRE(epi.out_mode == OUT_F32 || N % 32 == 0, "gemm_build: planes output needs N % 32 == 0");
     PPV_REQUIRE(!epi.rowgrp_bias || N % 32 == 0, "gemm_build: row-group bias needs N % 32 == 0");
-    memset(gp, 0, sizeof(*gp));
-    // distinct A tensors -> maps
-    const __nv_bfloat16* bases[GEMM_MAX_MAPS];
-    int nmaps = 0;
+    PPV_REQUIRE(nsrc > 0, "gemm_build: empty K");
+    int rc = gemm_params_init(gp, srcs[0].t, M, N, BN, BK, epi);
+    if (rc) return rc;
+    // distinct A tensors -> maps, the first one map 0
+    const __nv_bfloat16* bases[GEMM_MAX_MAPS] = {srcs[0].t.base};
+    int nmaps = 1;
     int ks = 0;
     for (int i = 0; i < nsrc; ++i) {
         const GemmSource& s = srcs[i];
@@ -400,7 +376,7 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
             PPV_REQUIRE(nmaps < GEMM_MAX_MAPS, "gemm_build: too many distinct A tensors");
             mi = nmaps++;
             bases[mi] = s.t.base;
-            int rc = encode_planes_map_ex(&gp->mapA[mi], s.t, BK, GEMM_BM, BK * 2);
+            rc = encode_planes_map_ex(&gp->mapA[mi], s.t, BK, GEMM_BM, BK * 2);
             if (rc) return rc;
         }
         for (int c = 0; c < s.ncols; c += BK) {
@@ -411,29 +387,20 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
             ++ks;
         }
     }
-    for (int j = nmaps; j < GEMM_MAX_MAPS; ++j) gp->mapA[j] = gp->mapA[0];
     PPV_REQUIRE(ks > 0, "gemm_build: empty K");
     PPV_REQUIRE(W.ld == ks * BK, "gemm_build: weight K does not match the k-steps");
     PPV_REQUIRE(W.rows >= N, "gemm_build: weight rows < N");
-    int rc = encode_planes_map_ex(&gp->mapB, W, BK, BN, BK * 2);
+    rc = encode_planes_map_ex(&gp->mapB, W, BK, BN, BK * 2);
     if (rc) return rc;
     gp->num_ksteps = ks;
-    gp->bk = BK;
-    gp->M = M;
-    gp->N = N;
-    gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
-    gp->n_tiles = (N + BN - 1) / BN;
-    gp->bn = BN;
-    gp->epi = epi;
     {
-        // weight-stationary: one n-tile, all k-slices of W (both planes) fit next to a 4-slot ring, and enough tiles per CTA to pay
-        // (two per SM of a 132-SM H100)
-        const size_t stage_bytes = size_t(2) * GEMM_BM * BK * 2 + size_t(2) * BN * BK * 2;
-        const size_t stages_full = std::min<size_t>(8, (232448 - 1024 - 256) / stage_bytes);
+        // weight-stationary: one n-tile, all k-slices of W (both planes) fit next to a GEMM_WS_STAGES-slot ring, and enough tiles per
+        // CTA to pay (two per SM of a 132-SM H100).  Sized on the bf16x3 ring: the bf16 ring holds half the bytes in at least as many stages.
+        const GemmRing ring = gemm_ring(BN, BK, 3);
         const size_t w_bytes = size_t(ks) * 2 * BN * BK * 2;
         const char* wsenv = getenv("PPV_GEMM_WS");
-        gp->ws = (gp->n_tiles == 1 && stages_full > GEMM_WS_STAGES && w_bytes <= (stages_full - GEMM_WS_STAGES) * stage_bytes && gp->m_tiles >= 264 &&
-                  !(wsenv && wsenv[0] == '0'))
+        gp->ws = (gp->n_tiles == 1 && ring.stages > GEMM_WS_STAGES && w_bytes <= size_t(ring.stages - GEMM_WS_STAGES) * ring.stage_bytes &&
+                  gp->m_tiles >= 264 && !(wsenv && wsenv[0] == '0'))
                      ? 1
                      : 0;
     }
@@ -458,8 +425,6 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
                         !(epi.relu && epi.relu_max > 0.f) && !gp->epi.debug_nostore)
                            ? 1
                            : 0;
-    } else {
-        gp->epi.f32_vec_ok = ((epi.out_ld % 2) == 0 && (epi.out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(epi.out) & 7) == 0) ? 1 : 0;
     }
     return PPV_OK;
 }
@@ -471,10 +436,13 @@ int gemm_build_wgrad(GemmParams* gp, const Planes& At, const Planes& Bt, int M, 
                      int64_t out_ld, int out_col0, int64_t split_rows, int BN) {
     PPV_REQUIRE(BN == 64 || BN == 128 || BN == 256, "gemm_build_wgrad: BN must be 64/128/256");
     PPV_REQUIRE(At.ld == Bt.ld && splits >= 1, "gemm_build_wgrad: operands must share the contraction length");
-    memset(gp, 0, sizeof(*gp));
-    int rc = encode_planes_map_ex(&gp->mapA[0], At, GEMM_BK, GEMM_BM, 128);
+    Epilogue ep;
+    ep.out_mode = OUT_F32;
+    ep.out = out;
+    ep.out_ld = out_ld;
+    ep.out_col0 = out_col0;
+    int rc = gemm_params_init(gp, At, M, N, BN, GEMM_BK, ep);
     if (rc) return rc;
-    for (int j = 1; j < GEMM_MAX_MAPS; ++j) gp->mapA[j] = gp->mapA[0];
     rc = encode_planes_map_ex(&gp->mapB, Bt, GEMM_BK, BN, 128);
     if (rc) return rc;
     const int nk_total = (At.ld + GEMM_BK - 1) / GEMM_BK;
@@ -483,19 +451,6 @@ int gemm_build_wgrad(GemmParams* gp, const Planes& At, const Planes& Bt, int M, 
     gp->lin_b_row0 = b_row0;
     gp->lin_b_col0 = b_col0;
     gp->lin_split_rows = split_rows;
-    gp->bk = GEMM_BK;
-    gp->M = M;
-    gp->N = N;
-    gp->m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
-    gp->n_tiles = (N + BN - 1) / BN;
-    gp->bn = BN;
-    Epilogue ep;
-    ep.out_mode = OUT_F32;
-    ep.out = out;
-    ep.out_ld = out_ld;
-    ep.out_col0 = out_col0;
-    gp->epi = ep;
-    gp->epi.f32_vec_ok = ((out_ld % 2) == 0 && (out_col0 % 2) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0) ? 1 : 0;
     PPV_REQUIRE(N % 32 == 0, "gemm_build_wgrad: N % 32 == 0 required");
     return PPV_OK;
 }
