@@ -1,12 +1,14 @@
 """Training-step throughput of the ECAPA-TDNN CUDA trainer (SURVEY.md §8d config 3 shape: per-GPU batch 64 x 298 frames, 2796
 speakers, AAM margin 0.2, Adam) -- a tuning aid; features resident in HBM.  python tools/train_bench.py [--batch 64] [--frames 298]
-[--steps 10] [--once]  (--once: one warm step only, for an ncu launch list).  Under torchrun every rank trains its own batch and the
+[--steps 10] [--once] [--dump DIR]  (--once: one warm step only, for an ncu launch list; --dump: the state after one step, to
+compare two builds bit for bit).  Under torchrun every rank trains its own batch and the
 gradient all-reduce runs over NCCL."""
 import argparse
 import json
 import os
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,6 +24,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--speakers", type=int, default=2796)
     ap.add_argument("--once", action="store_true")
+    ap.add_argument("--dump", metavar="DIR", help="run one forward_backward and adam_step, write the loss, logits, params, grads, stats "
+                    "and Adam moments to DIR/<name>.npy and exit")
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "bf16"], help="bf16 = train_conf.enable_amp")
     a = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -46,6 +50,14 @@ def main():
         eng.adam_step(lr=1e-3, weight_decay=1e-6, grad_scale=eng.all_reduce_grads())
         return loss
 
+    if a.dump:
+        loss, logits = eng.forward_backward(x, y, margin=0.2, return_logits=True)
+        eng.adam_step(lr=1e-3, weight_decay=1e-6, grad_scale=eng.all_reduce_grads())
+        os.makedirs(a.dump, exist_ok=True)
+        for name, t in {"loss": loss, "logits": logits, "params": eng.params, "grads": eng.grads, "stats": eng.stats, "exp_avg": eng.exp_avg,
+                        "exp_avg_sq": eng.exp_avg_sq}.items():
+            np.save(os.path.join(a.dump, name + ".npy"), t.cpu().numpy())
+        return
     for _ in range(3):
         loss = step()
     torch.cuda.synchronize()

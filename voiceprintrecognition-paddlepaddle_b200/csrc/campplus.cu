@@ -215,7 +215,7 @@ struct CamppModel : PlanModel {
   protected:
     bool prepare_weights(ArenaBuilder& ab) override;
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
-    int run_model_step(const PlanStep& s, cudaStream_t st) override;
+    int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) override;
     int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
@@ -381,15 +381,7 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     const int M2 = int(int64_t(B) * Tp);
 
     auto time_epi = [&](const Planes& out, int col0) {
-        Epilogue ep;
-        ep.out_mode = OUT_PLANES;
-        ep.out = out.base;
-        ep.out_ld = out.ld;
-        ep.out_plane_stride = out.plane_stride;
-        ep.out_col0 = col0;
-        ep.Tp = Tp;
-        ep.P = CP_P;
-        ep.T = T2;
+        Epilogue ep = planes_epilogue(out, col0, Tp, CP_P, T2);
         ep.zero_invalid = 1;
         return ep;
     };
@@ -507,7 +499,7 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int CamppModel::run_model_step(const PlanStep& s, cudaStream_t st) {
+int CamppModel::run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) {
     switch (s.model_kind) {
         case CP_FLATTEN_PAIRS: {
             const ImageGeo& g = s.g;
@@ -529,7 +521,7 @@ int CamppModel::run_model_step(const PlanStep& s, cudaStream_t st) {
                        "cp_context_kernel");
             return PPV_OK;
     }
-    return PlanModel::run_model_step(s, st);
+    return PlanModel::run_model_step(s, in, st);
 }
 
 // taps: "head.layer1", "head.layer2" -> fp32 [B,H,W,32]; "tdnn" [B,T2,128]; "block1".."block3" [B,T2,C]; "transit1", "transit2"

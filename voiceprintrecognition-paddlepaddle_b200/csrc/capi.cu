@@ -486,22 +486,14 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
     rc = gemm_test_stage(A, W, M, N, K, ws, st, &pa, &pw);
     if (rc) return rc;
     GemmSource src{pa, 0, pa.ld, 0};
-    Epilogue ep;
+    const Planes po{static_cast<__nv_bfloat16*>(out), 0, N, int64_t(M) * N};
+    Epilogue ep = Tp > 0 ? planes_epilogue(po, 0, Tp, P, Tp - 2 * P) : planes_epilogue(po);
     ep.bias = bias;
     ep.rowgrp_bias = rowgrp_bias;
     ep.relu = relu;
     ep.tanh_ = tanh_;
     ep.bn_scale = bn_scale;
     ep.bn_shift = bn_shift;
-    ep.out_mode = OUT_PLANES;
-    ep.out = out;
-    ep.out_ld = N;
-    ep.out_plane_stride = int64_t(M) * N;
-    if (Tp > 0) {
-        ep.Tp = Tp;
-        ep.P = P;
-        ep.T = Tp - 2 * P;
-    }
     GemmParams gp;
     rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, 64);
     if (rc) return rc;
@@ -638,17 +630,16 @@ int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision,
     PPV_CUDA_OK(cudaMemsetAsync(vec, 0x3c, v_bytes, st));  // small finite floats (0.0115)
     GemmSource src{pa, 0, int(Kp), 0};
     Epilogue ep;
-    ep.relu = 1;
-    if (planes_out) {
-        ep.out_mode = OUT_PLANES; ep.out = po.base; ep.out_ld = po.ld; ep.out_plane_stride = po.plane_stride;
-        if (planes_out >= 2) {
-            ep.Tp = kTp; ep.P = kP; ep.T = kTp - 2 * kP;
-            ep.bias = vec; ep.bn_scale = vec + N; ep.bn_shift = vec + 2 * N;
-            if (planes_out == 3) { ep.rowgrp_bias = vec + 3 * N; ep.tanh_ = 1; }
-        }
+    if (planes_out >= 2) {
+        ep = planes_epilogue(po, 0, kTp, kP, kTp - 2 * kP);
+        ep.bias = vec; ep.bn_scale = vec + N; ep.bn_shift = vec + 2 * N;
+        if (planes_out == 3) { ep.rowgrp_bias = vec + 3 * N; ep.tanh_ = 1; }
+    } else if (planes_out) {
+        ep = planes_epilogue(po);
     } else {
         ep.out_mode = OUT_F32; ep.out = po.base; ep.out_ld = N;
     }
+    ep.relu = 1;
     GemmParams gp;
     int rc = gemm_build(&gp, &src, 1, pw, M, N, ep, block_n, block_k);
     if (rc) return rc;

@@ -144,6 +144,21 @@ struct Epilogue {
     int lean = 0;  // set by gemm_build: the epilogue needs only what epilogue_frag_lean does (gemm_epilogue.cuh)
 };
 
+// An epilogue that writes split-bf16 planes `out` from column col0: on every row, or with Tp > 0 on the padded time layout (the T
+// valid rows of every Tp = T + 2P).
+inline Epilogue planes_epilogue(const Planes& out, int col0 = 0, int Tp = 0, int P = 0, int T = 0) {
+    Epilogue ep;
+    ep.out_mode = OUT_PLANES;
+    ep.out = out.base;
+    ep.out_ld = out.ld;
+    ep.out_plane_stride = out.plane_stride;
+    ep.out_col0 = col0;
+    ep.Tp = Tp;
+    ep.P = P;
+    ep.T = T;
+    return ep;
+}
+
 constexpr int GEMM_TRACE_TILES = 16;   // PPV_GEMM_TRACE: the traced CTA's first tiles stamped
 constexpr int GEMM_TRACE_EVENTS = 16;  // stamps per role and tile
 

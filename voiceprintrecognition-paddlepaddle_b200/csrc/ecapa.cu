@@ -35,9 +35,8 @@ struct EcBuffers {  // the workspace of a plan
 
 }  // namespace
 
-struct EcapaModel : PlanModel {
+struct EcapaModel : PlanModel, EcapaGeometry {
     ppv_ecapa_cfg cfg;
-    int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0;
     // device weights
     ConvW conv0, tdnn1[3], res2[3][8], tdnn2[3], se1[3], se2[3], mfa, fold, att1, att2, fc;
     float *aspbn_scale = nullptr, *aspbn_shift = nullptr;
@@ -45,7 +44,7 @@ struct EcapaModel : PlanModel {
     EcBuffers buf;
     int Tp = 0;
 
-    explicit EcapaModel(const ppv_ecapa_cfg& c) : PlanModel("ecapa", c.precision), cfg(c) {
+    EcapaModel(const ppv_ecapa_cfg& c, const EcapaGeometry& g) : PlanModel("ecapa", c.precision), EcapaGeometry(g), cfg(c) {
         // 128-wide n-tiles even where N allows 256: on an H100 SXM at 700 W (tools/gemm_bench.py, M = 78 336,
         // profiles/gemm_bench_after.txt) BN = 128 with 64-wide k-steps takes 15-18 % less time than BN = 256 at every large layer of
         // the model (N x K = 512 x 512 / 640, 1536 x 1536, split-bf16 x3), and no BN = 256 variant beats it by more than run-to-run noise.
@@ -84,32 +83,14 @@ void ppv_ecapa_default_cfg_impl(ppv_ecapa_cfg* c) {
 
 int ecapa_create(const ppv_ecapa_cfg* cfg, Model** out) {
     PPV_REQUIRE(cfg && out, "ecapa_create: null argument");
-    const int C = cfg->channels[0];
-    if (cfg->channels[1] != C || cfg->channels[2] != C || cfg->channels[3] != C)
-        return fail(PPV_EUNSUPPORTED, "ecapa: channels[0..3] must be equal (no shortcut conv path)");
-    if (cfg->channels[4] != 3 * C) return fail(PPV_EUNSUPPORTED, "ecapa: channels[4] must equal 3 * channels[0] (MFA concat)");
-    if (cfg->res2net_scale < 2 || cfg->res2net_scale > 8 || C % cfg->res2net_scale)
-        return fail(PPV_EUNSUPPORTED, "ecapa: res2net_scale must divide channels and be in [2,8]");
-    const int width = C / cfg->res2net_scale;
-    if (width % 64) return fail(PPV_EUNSUPPORTED, "ecapa: channels / res2net_scale must be a multiple of 64");
-    if (cfg->kernel_sizes[1] != 3 || cfg->kernel_sizes[2] != 3 || cfg->kernel_sizes[3] != 3 || cfg->kernel_sizes[4] != 1 ||
-        (cfg->kernel_sizes[0] % 2) == 0 || cfg->dilations[4] != 1)
-        return fail(PPV_EUNSUPPORTED, "ecapa: kernel sizes must be [odd,3,3,3,1]");
+    EcapaGeometry g;
+    int rc = ecapa_geometry(*cfg, &g);
+    if (rc) return rc;
+    if (cfg->dilations[4] != 1) return fail(PPV_EUNSUPPORTED, "ecapa: kernel sizes must be [odd,3,3,3,1]");
     if (cfg->attention_channels % 64 || cfg->embd_dim % 32 || cfg->se_channels <= 0 || cfg->se_channels % 64)
         return fail(PPV_EUNSUPPORTED, "ecapa: attention_channels % 64, se_channels % 64, embd_dim % 32 required");
     if (cfg->pooling < PPV_POOL_ASP || cfg->pooling > PPV_POOL_TSP) return fail(PPV_EUNSUPPORTED, "ecapa: pooling must be PPV_POOL_ASP / SAP / TAP / TSP");
-    EcapaModel* m = new EcapaModel(*cfg);
-    m->C = C;
-    m->C3 = 3 * C;
-    m->width = width;
-    m->scale = cfg->res2net_scale;
-    m->Fp = int(mc_align_up(cfg->input_size, 64));
-    m->att = cfg->attention_channels;
-    m->se = cfg->se_channels;
-    int P = (cfg->kernel_sizes[0] - 1) / 2 * cfg->dilations[0];
-    for (int i = 1; i <= 3; ++i) P = std::max(P, cfg->dilations[i]);
-    m->P = P;
-    *out = m;
+    *out = new EcapaModel(*cfg, g);
     return PPV_OK;
 }
 
@@ -270,15 +251,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
 
     // planes output in the padded time layout: ReLU, then the layer's BatchNorm
     auto planes_out = [&](const Planes& p, int col0, bool halo, const ConvW& cw) {
-        Epilogue ep;
-        ep.out_mode = OUT_PLANES;
-        ep.out = p.base;
-        ep.out_ld = p.ld;
-        ep.out_plane_stride = p.plane_stride;
-        ep.out_col0 = col0;
-        ep.Tp = Tp;
-        ep.P = P;
-        ep.T = T;
+        Epilogue ep = planes_epilogue(p, col0, Tp, P, T);
         ep.halo = halo ? 1 : 0;
         ep.relu = 1;
         ep.bn_scale = cw.bn_scale;
@@ -338,11 +311,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         if (rc) return rc;
         steps.push_back(colstats_step(buf.z, C, B, T, P, Tp, 0, 0.f, buf.sem, 0.f, true));
         {  // s = sigmoid(W2 relu(W1 mean + b1) + b2): [B,C] -> [B,S] -> [B,C], plain (un-padded) row layout
-            Epilogue e1;
-            e1.out_mode = OUT_PLANES;
-            e1.out = buf.seh.base;
-            e1.out_ld = buf.seh.ld;
-            e1.out_plane_stride = buf.seh.plane_stride;
+            Epilogue e1 = planes_epilogue(buf.seh);
             e1.relu = 1;
             rc = plan_row_linear(se1[b - 1], GemmSource{buf.sem, 0, C, 0}, B, e1);
             if (rc) return rc;
@@ -433,7 +402,7 @@ int EcapaModel::run(const float* feat, Fbank* fb, const float* wav, const float*
         launches_other += 1;
     }
     prof_end(st);
-    return rc ? rc : run_plan(feat, nv, st);
+    return rc ? rc : run_plan(PlanInputs{feat, nv}, st);
 }
 
 int ecapa_profile(Model* model, int enable) {

@@ -22,8 +22,7 @@
 #include <vector>
 
 #include "common.h"
-#include "model_common.h"
-#include "train.h"
+#include "plan.h"
 
 namespace ppv {
 
@@ -49,29 +48,11 @@ struct TLayer {  // TDNNBlock
     TBN bn;
 };
 
-struct TStep {
-    enum Kind {
-        REPACK, PACK, GEMM, BN_FWD, SE_FWD, SCALE_RES, ASP_HEAD_FWD, ASP_TAIL_FWD, LOSS,
-        HEAD_BWD, ASP_BWD, COLSUM, BN_BWD, WGRAD, ASP_CTX_BWD, GRAD_SUM, SE_BWD
-    } kind;
-    GemmParams gp;
-    int a = 0, b = 0;  // small integer arguments (block index, split counts)
-    GradSrcList gl;
-    BnApplyArgs ap;
-    Planes p0, p1;
-    int c0 = 0, c1 = 0, C = 0;
-    float* f0 = nullptr;
-    // WGRAD
-    std::vector<GemmParams> wg;
-    struct Tr {
-        Planes in;
-        int col0, C, row0;  // row0: first row of the transposed buffer to write
-        int which;          // 0 = TA, 1 = TB
-        int shift = 0;      // row shift of the input (first conv tap)
-        int ntaps = 1, shift_step = 0, row_step = 0;  // all taps of a conv in one launch
-    };
-    std::vector<Tr> trs;
-    int layer = -1;
+// The trainer's own plan steps (PlanStep::MODEL), one per launcher call: run_model_step passes each launcher its arguments from the
+// step's fields as plan.h lays them out.
+enum TrKind {
+    TR_REPACK, TR_PACK, TR_BN_FWD, TR_DENSE_FWD, TR_PLANES_TO_F32, TR_ASP_POOL, TR_BN1D_FWD, TR_AAM_FWD, TR_AAM_BWD, TR_DENSE_BWD,
+    TR_BN1D_BWD, TR_ASP_BWD, TR_GRAD_SUM, TR_BN_BWD, TR_TRANSPOSE, TR_WGRAD_UNPACK, TR_ASP_GLOBAL_BWD, TR_GRAD_DOT, TR_ACT_BWD
 };
 
 // The workspace views of one plan (tr_carve).  `layer` is indexed like Trainer::conv: the TDNN layers, then asp.conv.
@@ -90,7 +71,7 @@ struct TrBuffers {
     float *d_emb = nullptr, *dpn = nullptr, *dpooled = nullptr, *dgs = nullptr, *rs = nullptr, *rb = nullptr, *dg2 = nullptr, *dg1 = nullptr, *ds = nullptr,
           *part = nullptr, *wpart = nullptr;
     size_t part_elems = 0;
-    void* aam_ws = nullptr;
+    float* aam_ws = nullptr;
     size_t aam_ws_bytes = 0;
 };
 
@@ -106,10 +87,10 @@ struct TrTap {
 
 }  // namespace
 
-struct Trainer : PlanOwner {
+struct Trainer : PlanOwner, EcapaGeometry {
     ppv_ecapa_cfg cfg;
     int S = 0;  // classes
-    int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0, D = 0;
+    int D = 0;  // embedding size
     // (PlanOwner::precision PPV_PREC_BF16: single-pass bf16 operands for every forward / data-gradient / weight-gradient GEMM, AMP mode)
     // flat layout
     std::map<std::string, std::pair<int64_t, int64_t>> pmap, smap;  // name -> (offset, numel)
@@ -121,18 +102,22 @@ struct Trainer : PlanOwner {
     TConv att2;
     int64_t se1_w[3], se1_b[3], se2_w[3], se2_b[3], aspbn_g = 0, aspbn_b = 0, aspbn_rm = 0, aspbn_rv = 0, fc_w = 0, fc_b = 0, cls_w = 0;
     // plan
-    std::vector<TStep> steps;
     TrBuffers buf;
     std::map<std::string, TrTap> taps;
 
-    Trainer() : PlanOwner("trainer", "ppv_trainer_workspace_bytes", PPV_PREC_BF16X3) {}
+    Trainer(const ppv_ecapa_cfg& c, const EcapaGeometry& g, int num_classes)
+        : PlanOwner("trainer", "ppv_trainer_workspace_bytes", PPV_PREC_BF16X3), EcapaGeometry(g), cfg(c), S(num_classes), D(c.embd_dim) {
+        sync_each_step = getenv("PPV_TRAIN_DEBUG") != nullptr;  // localise a faulting kernel
+    }
     // convs by layer index: L's, then asp.conv
     int l_att2() const { return int(L.size()); }
     const TConv& conv(int layer) const { return layer == l_att2() ? att2 : L[layer].conv; }
     size_t workspace_bytes(int B, int T) const override;
+    using PlanOwner::run_plan;
 
   protected:
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
+    int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) override;
 };
 
 // ------------------------------------------------------------------------------------------------ create: flat layout
@@ -155,20 +140,10 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
         return fail(PPV_EUNSUPPORTED, "trainer: attention_channels % 64, se_channels % 8, embd_dim % 8 required");
     if (cfg->pooling != PPV_POOL_ASP || !cfg->global_context)
         return fail(PPV_EUNSUPPORTED, "trainer: the training step implements pooling_type ASP with global_context");
-    Trainer* t = new Trainer();
-    t->cfg = *cfg;
-    t->S = num_classes;
-    t->C = C;
-    t->C3 = 3 * C;
-    t->scale = 8;
-    t->width = C / 8;
-    t->Fp = int(mc_align_up(size_t(cfg->input_size), 64));
-    t->att = cfg->attention_channels;
-    t->se = cfg->se_channels;
-    t->D = cfg->embd_dim;
-    int P = (cfg->kernel_sizes[0] - 1) / 2 * cfg->dilations[0];
-    for (int i = 1; i <= 3; ++i) P = std::max(P, cfg->dilations[i]);
-    t->P = P;
+    EcapaGeometry g;  // its checks pass where the ones above do
+    int rc = ecapa_geometry(*cfg, &g);
+    if (rc) return rc;
+    Trainer* t = new Trainer(*cfg, g, num_classes);
 
     auto add_layer = [&](const std::string& p, int cin, int cout, int k, int dil, bool dgrad) {
         TLayer l;
@@ -360,7 +335,7 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     }
     f->wpart = f32(wmax);
     f->aam_ws_bytes = aam_workspace_bytes(B, t->D, t->S);
-    f->aam_ws = cv.take(f->aam_ws_bytes);
+    f->aam_ws = static_cast<float*>(cv.take(f->aam_ws_bytes));
 }
 
 // The taps trainer_read_tap serves, by name without the "pad:" prefix and the block suffix.
@@ -440,40 +415,42 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     tr_carve(t, cv, B, T, &f);
     t->taps = tr_tap_table(t, f, B);
     t->steps.clear();
-    const int C = t->C, C3 = t->C3, W = t->width, P = t->P, Tp = f.Tp;
+    const int C = t->C, C3 = t->C3, W = t->width, P = t->P, Tp = f.Tp, se = t->se, att = t->att, D = t->D;
     const int M = int(f.R);
     float* const par = t->params;
     float* const grd = t->grads;
+    float* const sta = t->stats;
 
-    auto push = [&](const TStep& s) { t->steps.push_back(s); };
-    // forward conv: bias + ReLU -> post-activation planes (valid frames)
+    auto model = [&](TrKind kind) {
+        PlanStep s = model_step(kind);
+        s.B = B;
+        s.T = T;
+        s.P = P;
+        s.Tp = Tp;
+        return s;
+    };
+    auto push = [&](const PlanStep& s) { t->steps.push_back(s); };
+    auto gemm = [&](const std::vector<GemmSource>& srcs, const Planes& w, int N, const Epilogue& ep) -> int {
+        PlanStep s;
+        s.kind = PlanStep::GEMM;
+        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), w, M, N, ep, gemm_pick_bn(N));
+        if (!r) push(s);
+        return r;
+    };
+    // forward conv: bias + ReLU -> post-activation planes (valid frames), or fp32 rows
     auto fwd_gemm = [&](int li, const std::vector<GemmSource>& srcs, const Planes& out, int out_col0, bool relu, const float* rowgrp,
                         float* out_f32) -> int {
         const TConv& c = t->conv(li);
-        Epilogue ep;
-        ep.bias = par + c.b_off;
-        ep.rowgrp_bias = rowgrp;
-        ep.relu = relu ? 1 : 0;
+        Epilogue ep = planes_epilogue(out, out_col0, Tp, P, T);
         if (out_f32) {
             ep.out_mode = OUT_F32;
             ep.out = out_f32;
             ep.out_ld = c.Cout;
-        } else {
-            ep.out_mode = OUT_PLANES;
-            ep.out = out.base;
-            ep.out_ld = out.ld;
-            ep.out_plane_stride = out.plane_stride;
-            ep.out_col0 = out_col0;
         }
-        ep.Tp = Tp;
-        ep.P = P;
-        ep.T = T;
-        TStep s;
-        s.kind = TStep::GEMM;
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), f.layer[li].wf, M, c.Cout, ep, gemm_pick_bn(c.Cout));
-        if (r) return r;
-        push(s);
-        return PPV_OK;
+        ep.bias = par + c.b_off;
+        ep.rowgrp_bias = rowgrp;
+        ep.relu = relu ? 1 : 0;
+        return gemm(srcs, f.layer[li].wf, c.Cout, ep);
     };
     auto taps_of = [&](const TConv& c, const Planes& x, int col0, int sign) {
         std::vector<GemmSource> v;
@@ -482,62 +459,87 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     };
     auto bn_fwd = [&](int li, const Planes& a, int a_col0, const Planes& y, int y_col0, int tanh_, const Planes* add, int add_col0,
                       const Planes* out2, int out2_col0) {
-        TStep s;
-        s.kind = TStep::BN_FWD;
-        s.layer = li;
-        s.p0 = a;
-        s.c0 = a_col0;
-        s.ap.y = y;
-        s.ap.y_col0 = y_col0;
-        s.ap.tanh_ = tanh_;
+        const TBN& bn = t->L[li].bn;
+        const TrBuffers::Layer& w = f.layer[li];
+        PlanStep s = model(TR_BN_FWD);
+        s.x = a;
+        s.xc0 = a_col0;
+        s.C = bn.C;
+        s.vec = {par + bn.g_off, par + bn.b_off};
+        s.f32 = {w.mean, w.rstd, w.scale, w.shift, sta + bn.rm_off, sta + bn.rv_off, f.part};
+        s.apply.y = y;
+        s.apply.y_col0 = y_col0;
+        s.apply.tanh_ = tanh_;
         if (out2) {
-            s.ap.add = *add;
-            s.ap.add_col0 = add_col0;
-            s.ap.out2 = *out2;
-            s.ap.out2_col0 = out2_col0;
+            s.apply.add = *add;
+            s.apply.add_col0 = add_col0;
+            s.apply.out2 = *out2;
+            s.apply.out2_col0 = out2_col0;
         }
+        push(s);
+    };
+    auto dense_fwd = [&](const float* X, int x_ld, const float* Wt, int w_ld, const float* bias, int Mr, int N, int K, int act, float* Y, int y_ld) {
+        PlanStep s = model(TR_DENSE_FWD);
+        s.vec = {X, Wt, bias};
+        s.dim = {x_ld, w_ld, Mr, N, K, act, y_ld};
+        s.f32 = {Y};
+        push(s);
+    };
+    auto dense_bwd = [&](const float* dY, int dy_ld, const float* X, int x_ld, const float* Wt, int w_ld, int Mr, int N, int K, float* dX,
+                         int dx_ld, float* dW, int dw_ld, float* db) {
+        PlanStep s = model(TR_DENSE_BWD);
+        s.vec = {dY, X, Wt};
+        s.dim = {dy_ld, x_ld, w_ld, Mr, N, K, dx_ld, dw_ld};
+        s.f32 = {dX, dW, db};
+        push(s);
+    };
+    auto act_bwd = [&](float* dy, const float* y, int64_t n, int act, float alpha) {
+        PlanStep s = model(TR_ACT_BWD);
+        s.f32 = {dy};
+        s.vec = {y};
+        s.dim = {n, act};
+        s.inv_count = alpha;
         push(s);
     };
     // data gradient: dx_pad[r, cin] = sum_tap dz[r - off_tap, :] . W[:, cin, tap]  -> planes on every row
     auto dgrad_gemm = [&](int li, const Planes& dz, int dz_col0, const Planes& out, int out_col0) -> int {
         const TConv& c = t->conv(li);
-        Epilogue ep;
-        ep.out_mode = OUT_PLANES;
-        ep.out = out.base;
-        ep.out_ld = out.ld;
-        ep.out_plane_stride = out.plane_stride;
-        ep.out_col0 = out_col0;
-        TStep s;
-        s.kind = TStep::GEMM;
-        std::vector<GemmSource> srcs = taps_of(c, dz, dz_col0, -1);
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), f.layer[li].wd, M, c.Cinp, ep, gemm_pick_bn(c.Cinp));
-        if (r) return r;
+        return gemm(taps_of(c, dz, dz_col0, -1), f.layer[li].wd, c.Cinp, planes_epilogue(out, out_col0));
+    };
+    // out[c][row0 + r] = in[r + shift][col0 + c]; ntaps > 1: tap z shifted by z * shift_step into rows z * row_step on
+    auto transpose = [&](const Planes& in, int col0, int Cn, Planes out, int row0, int shift, int ntaps, int shift_step, int row_step) {
+        PlanStep s = model(TR_TRANSPOSE);
+        s.x = in;
+        s.xc0 = col0;
+        s.C = Cn;
+        s.rows = f.R;
+        out.base += int64_t(row0) * out.ld;
+        out.rows -= row0;
+        s.out = out;
+        s.dim = {shift, ntaps, shift_step, row_step};
         push(s);
-        return PPV_OK;
     };
     // weight gradient: dz^T -> TA; one row-shifted transpose of the layer input per tap -> TB rows [tap * Cinp, ...); ONE GEMM
     // [Cout] x [taps * Cinp] over the frames (split-K partials); unpack into the flat gradient buffer
-    auto wgrad = [&](int li, const Planes& dz, int dz_col0, const std::vector<TStep::Tr>& xs) -> int {
+    struct WgradInput {
+        Planes x;
+        int col0, C, row0;  // row0: first row of TB to write
+    };
+    auto wgrad = [&](int li, const Planes& dz, int dz_col0, const std::vector<WgradInput>& xs) -> int {
         const TConv& c = t->conv(li);
-        TStep s;
-        s.kind = TStep::WGRAD;
-        s.layer = li;
-        s.trs.push_back(TStep::Tr{dz, dz_col0, c.Cout, 0, 0, 0});
-        for (const TStep::Tr& x : xs) {
-            TStep::Tr tr{x.in, x.col0, x.C, x.row0, 1, -((c.taps - 1) / 2) * c.dil};
-            tr.ntaps = c.taps;
-            tr.shift_step = c.dil;
-            tr.row_step = c.Cinp;
-            s.trs.push_back(tr);
-        }
+        transpose(dz, dz_col0, c.Cout, f.TA, 0, 0, 1, 0, 0);
+        for (const WgradInput& x : xs) transpose(x.x, x.col0, x.C, f.TB, x.row0, -((c.taps - 1) / 2) * c.dil, c.taps, c.dil, c.Cinp);
         const int N = c.taps * c.Cinp;
         const WgradSplit sp = tr_wgrad_split(t, c, f.Rp);
-        GemmParams gp;
-        int r = gemm_build_wgrad(&gp, f.TA, f.TB, c.Cout, N, 0, 0, sp.splits, f.wpart, N, 0, sp.Mpad, sp.BN);
+        PlanStep g;
+        g.kind = PlanStep::GEMM;
+        int r = gemm_build_wgrad(&g.gp, f.TA, f.TB, c.Cout, N, 0, 0, sp.splits, f.wpart, N, 0, sp.Mpad, sp.BN);
         if (r) return r;
-        s.wg.push_back(gp);
-        s.a = gp.lin_splits;
-        s.b = sp.Mpad;
+        push(g);
+        PlanStep s = model(TR_WGRAD_UNPACK);
+        s.vec = {f.wpart};
+        s.dim = {g.gp.lin_splits, sp.Mpad, c.Cout, c.Cin, c.Cinp, c.taps, int64_t(c.CinTotal) * c.taps};
+        s.f32 = {grd + c.w_off};
         push(s);
         return PPV_OK;
     };
@@ -548,28 +550,47 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         g.fold = fold;
         return g;
     };
-    auto bn_bwd = [&](int layer, const GradSrcList& gl, const Planes& a, int a_col0, const Planes& dz, int dz_col0) {
-        TStep s;
-        s.kind = TStep::BN_BWD;
-        s.layer = layer;
+    auto bn_bwd = [&](int li, const GradSrcList& gl, const Planes& a, int a_col0, const Planes& dz, int dz_col0) {
+        const TLayer& l = t->L[li];
+        const TrBuffers::Layer& w = f.layer[li];
+        PlanStep s = model(TR_BN_BWD);
         s.gl = gl;
-        s.p0 = a;
-        s.c0 = a_col0;
-        s.p1 = dz;
-        s.c1 = dz_col0;
-        s.a = tr_bn_bwd_tsplit(t, layer, B);
+        s.x = a;
+        s.xc0 = a_col0;
+        s.C = l.bn.C;
+        s.vec = {w.mean, w.rstd, par + l.bn.g_off};
+        s.f32 = {grd + l.bn.g_off, grd + l.bn.b_off, grd + l.conv.b_off, f.part};
+        s.out = dz;
+        s.oc0 = dz_col0;
+        s.dim = {int64_t(f.part_elems), tr_bn_bwd_tsplit(t, li, B)};
         push(s);
     };
-    auto simple = [&](TStep::Kind kd, int a = 0) {
-        TStep s;
-        s.kind = kd;
-        s.a = a;
+    // out (optional planes, valid frames) = summed sources, per-utterance column sums -> part, colsum (optional) [Cn]
+    auto grad_sum = [&](const GradSrcList& gl, int Cn, const Planes& out, float* colsum) {
+        PlanStep s = model(TR_GRAD_SUM);
+        s.gl = gl;
+        s.C = Cn;
+        s.out = out;
+        s.f32 = {f.part, colsum};
         push(s);
     };
 
     // ================================================================= forward
-    simple(TStep::REPACK);
-    simple(TStep::PACK);
+    for (int l = 0; l <= t->l_att2(); ++l) {
+        const TConv& c = t->conv(l);
+        PlanStep s = model(TR_REPACK);
+        s.vec = {par + c.w_off};
+        s.dim = {int64_t(c.CinTotal) * c.taps, c.Cout, c.Cin, c.Cinp, c.taps};
+        s.x = f.layer[l].wf;
+        s.y = f.layer[l].wd;
+        push(s);
+    }
+    {
+        PlanStep s = model(TR_PACK);
+        s.C = t->cfg.input_size;
+        s.out = f.X0;
+        push(s);
+    }
     {
         const int li = t->l_conv0;
         rc = fwd_gemm(li, taps_of(t->conv(li), f.X0, 0, +1), f.A0, 0, true, nullptr, nullptr);
@@ -602,22 +623,31 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
             if (rc) return rc;
             bn_fwd(li, f.At2[b], 0, f.Yt2[b], 0, 0, nullptr, 0, nullptr, 0);
         }
-        simple(TStep::SE_FWD, b);
-        {
-            TStep s;
-            s.kind = TStep::SCALE_RES;
-            s.a = b;
-            s.p0 = u;
-            s.c0 = uc;
-            push(s);
-        }
+        // SE: squeeze, excite, then scale + residual into OUTCAT's window b
+        PlanStep sq = colstats_step(f.Yt2[b], C, B, T, P, Tp, 0, 0.f, Planes());
+        sq.out_f32 = f.se_s[b];
+        push(sq);
+        dense_fwd(f.se_s[b], C, par + t->se1_w[b], C, par + t->se1_b[b], B, se, C, 1, f.se_g1[b], se);
+        dense_fwd(f.se_g1[b], se, par + t->se2_w[b], se, par + t->se2_b[b], B, C, se, 2, f.se_g2[b], C);
+        push(scale_res_step(f.Yt2[b], f.se_g2[b], u, uc, f.OUTCAT, C * b, C, Tp, f.R, false));
     }
     {
         rc = fwd_gemm(t->l_mfa, {GemmSource{f.OUTCAT, 0, C3, 0}}, f.Amfa, 0, true, nullptr, nullptr);
         if (rc) return rc;
         bn_fwd(t->l_mfa, f.Amfa, 0, f.M, 0, 0, nullptr, 0, nullptr, 0);
     }
-    simple(TStep::ASP_HEAD_FWD);  // global stats -> per-utterance bias of the attention TDNN
+    {
+        // global stats -> per-utterance bias of the attention TDNN: its weight [att][3*C3], columns C3.. multiply [mean | std]
+        push(colstats_step(f.M, C3, B, T, P, Tp, 1, TR_ASP_EPS, f.gstat_pl));
+        PlanStep s = model(TR_PLANES_TO_F32);
+        s.x = f.gstat_pl;
+        s.C = 2 * C3;
+        s.T = s.Tp = 1;  // one row per utterance
+        s.P = 0;
+        s.f32 = {f.gstat};
+        push(s);
+        dense_fwd(f.gstat, 2 * C3, par + t->L[t->l_att1].conv.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, f.fold, att);
+    }
     {
         rc = fwd_gemm(t->l_att1, {GemmSource{f.M, 0, C3, 0}}, f.Aatt, 0, true, f.fold, nullptr);
         if (rc) return rc;
@@ -625,35 +655,78 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         rc = fwd_gemm(t->l_att2(), {GemmSource{f.A4, 0, t->att, 0}}, Planes(), 0, false, nullptr, f.logits);
         if (rc) return rc;
     }
-    simple(TStep::ASP_TAIL_FWD);  // softmax pooling, asp_bn (batch statistics), fc
-    simple(TStep::LOSS);
+    {
+        // softmax pooling, asp_bn (batch statistics), fc, AAM-softmax loss
+        PlanStep s = model(TR_ASP_POOL);
+        s.vec = {f.logits};
+        s.dim = {C3};
+        s.x = f.M;
+        s.C = C3;
+        s.f32 = {f.pooled};
+        push(s);
+        s = model(TR_BN1D_FWD);
+        s.vec = {f.pooled, par + t->aspbn_g, par + t->aspbn_b};
+        s.C = 2 * C3;
+        s.f32 = {f.pn, f.aspbn_mean, f.aspbn_rstd, sta + t->aspbn_rm, sta + t->aspbn_rv};
+        push(s);
+        dense_fwd(f.pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, f.emb, D);
+        s = model(TR_AAM_FWD);
+        s.vec = {f.emb, par + t->cls_w};
+        s.dim = {D, t->S, int64_t(f.aam_ws_bytes)};
+        s.f32 = {f.cls_logits, f.loss, f.aam_ws};
+        push(s);
+    }
 
     // ================================================================= backward
-    simple(TStep::HEAD_BWD);  // AAM, fc, asp_bn -> dpooled
-    simple(TStep::ASP_BWD);   // -> dlogits, dMd
+    {
+        // AAM, fc, asp_bn -> dpooled; ASP -> dlogits, dMd
+        PlanStep s = model(TR_AAM_BWD);
+        s.vec = {f.emb, par + t->cls_w, f.cls_logits};
+        s.dim = {D, t->S, int64_t(f.aam_ws_bytes)};
+        s.f32 = {f.d_emb, grd + t->cls_w, f.aam_ws};
+        push(s);
+        dense_bwd(f.d_emb, D, f.pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, f.dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b);
+        s = model(TR_BN1D_BWD);
+        s.vec = {f.dpn, f.pooled, par + t->aspbn_g, f.aspbn_mean, f.aspbn_rstd};
+        s.C = 2 * C3;
+        s.f32 = {f.dpooled, grd + t->aspbn_g, grd + t->aspbn_b};
+        push(s);
+        s = model(TR_ASP_BWD);
+        s.vec = {f.logits, f.pooled, f.dpooled};
+        s.dim = {C3};
+        s.x = f.M;
+        s.C = C3;
+        s.out = f.dlogits;
+        s.t = f.dMd;
+        push(s);
+    }
     {
         // asp.conv: bias, weight, data gradients
-        TStep s;
-        s.kind = TStep::COLSUM;
-        s.gl.n = 1;
-        s.gl.s[0] = src1(f.dlogits, 0, 0);
-        s.C = C3;
-        s.f0 = grd + t->att2.b_off;
-        push(s);
-        rc = wgrad(t->l_att2(), f.dlogits, 0, {TStep::Tr{f.A4, 0, t->att, 0, 1}});
+        GradSrcList gl;
+        gl.n = 1;
+        gl.s[0] = src1(f.dlogits, 0, 0);
+        grad_sum(gl, C3, Planes(), grd + t->att2.b_off);
+        rc = wgrad(t->l_att2(), f.dlogits, 0, {{f.A4, 0, t->att, 0}});
         if (rc) return rc;
         rc = dgrad_gemm(t->l_att2(), f.dlogits, 0, f.dA4, 0);
         if (rc) return rc;
     }
     {
-        // attention TDNN: tanh, BN, ReLU backward; frame-level weight / data gradients; per-utterance context gradients
+        // attention TDNN: tanh, BN, ReLU backward; per-utterance context gradients (from the sums the BN backward leaves in f.part
+        // [B][att]); frame-level weight / data gradients
         GradSrcList gl;
         gl.n = 1;
         gl.s[0] = src1(f.dA4, 0, 0);
         gl.s[0].dtanh = f.A4;
         bn_bwd(t->l_att1, gl, f.Aatt, 0, f.dZatt, 0);
-        simple(TStep::ASP_CTX_BWD);
-        rc = wgrad(t->l_att1, f.dZatt, 0, {TStep::Tr{f.M, 0, C3, 0, 1}});
+        const TConv& c = t->L[t->l_att1].conv;
+        dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3, nullptr);
+        PlanStep s = model(TR_ASP_GLOBAL_BWD);
+        s.vec = {f.gstat, f.dgs};
+        s.C = C3;
+        s.f32 = {f.rs, f.rb};
+        push(s);
+        rc = wgrad(t->l_att1, f.dZatt, 0, {{f.M, 0, C3, 0}});
         if (rc) return rc;
         rc = dgrad_gemm(t->l_att1, f.dZatt, 0, f.dMatt, 0);
         if (rc) return rc;
@@ -669,7 +742,7 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         gl.s[2].rowbias = f.rb;
         gl.s[2].row_ld = C3;
         bn_bwd(t->l_mfa, gl, f.Amfa, 0, f.dZmfa, 0);
-        rc = wgrad(t->l_mfa, f.dZmfa, 0, {TStep::Tr{f.OUTCAT, 0, C3, 0, 1}});
+        rc = wgrad(t->l_mfa, f.dZmfa, 0, {{f.OUTCAT, 0, C3, 0}});
         if (rc) return rc;
         rc = dgrad_gemm(t->l_mfa, f.dZmfa, 0, f.dOUTCAT, 0);
         if (rc) return rc;
@@ -677,33 +750,43 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     for (int b = 2; b >= 0; --b) {
         const Planes u = b == 0 ? f.Y0 : f.OUTCAT;
         const int uc = b == 0 ? 0 : C * (b - 1);
-        const Planes& D = f.Dbuf[b];
+        const Planes& Dg = f.Dbuf[b];
         {
             // d(out_b) = MFA window + (next block: tdnn1 data gradient + its own residual gradient)
-            TStep s;
-            s.kind = TStep::GRAD_SUM;
-            s.gl.n = 1;
-            s.gl.s[0] = src1(f.dOUTCAT, C * b, 0);
+            GradSrcList gl;
+            gl.n = 1;
+            gl.s[0] = src1(f.dOUTCAT, C * b, 0);
             if (b < 2) {
-                s.gl.n = 3;
-                s.gl.s[1] = src1(f.dXt1[b + 1], 0, 0);
-                s.gl.s[2] = src1(f.Dbuf[b + 1], 0, 0);
+                gl.n = 3;
+                gl.s[1] = src1(f.dXt1[b + 1], 0, 0);
+                gl.s[2] = src1(f.Dbuf[b + 1], 0, 0);
             }
-            s.C = C;
-            s.p0 = D;
-            s.c0 = 0;
-            push(s);
+            grad_sum(gl, C, Dg, nullptr);
         }
-        simple(TStep::SE_BWD, b);  // -> dg2 ... ds (scaled by 1/T), SE weight gradients
+        {
+            // SE backward -> dg2 ... ds (scaled by 1/T), SE weight gradients
+            PlanStep s = model(TR_GRAD_DOT);
+            s.gl.n = 1;
+            s.gl.s[0].t = Dg;
+            s.x = f.Yt2[b];
+            s.C = C;
+            s.f32 = {f.dg2};
+            push(s);
+            act_bwd(f.dg2, f.se_g2[b], int64_t(B) * C, 2, 0.f);
+            dense_bwd(f.dg2, C, f.se_g1[b], se, par + t->se2_w[b], se, B, C, se, f.dg1, se, grd + t->se2_w[b], se, grd + t->se2_b[b]);
+            act_bwd(f.dg1, f.se_g1[b], int64_t(B) * se, 1, 0.f);
+            dense_bwd(f.dg1, se, f.se_s[b], C, par + t->se1_w[b], C, B, se, C, f.ds, C, grd + t->se1_w[b], C, grd + t->se1_b[b]);
+            act_bwd(f.ds, nullptr, int64_t(B) * C, 0, 1.f / float(T));
+        }
         {
             GradSrcList gl;
             gl.n = 1;
-            gl.s[0] = src1(D, 0, 0);
+            gl.s[0] = src1(Dg, 0, 0);
             gl.s[0].rowscale = f.se_g2[b];
             gl.s[0].rowbias = f.ds;
             gl.s[0].row_ld = C;
             bn_bwd(t->l_tdnn2[b], gl, f.At2[b], 0, f.dZt2[b], 0);
-            rc = wgrad(t->l_tdnn2[b], f.dZt2[b], 0, {TStep::Tr{f.Yt1[b], 0, W, 0, 1}, TStep::Tr{f.RC[b], W, C - W, W, 1}});
+            rc = wgrad(t->l_tdnn2[b], f.dZt2[b], 0, {{f.Yt1[b], 0, W, 0}, {f.RC[b], W, C - W, W}});
             if (rc) return rc;
             rc = dgrad_gemm(t->l_tdnn2[b], f.dZt2[b], 0, f.dRC[b], 0);
             if (rc) return rc;
@@ -718,28 +801,24 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
             }
             const int li = t->l_res[b][j];
             bn_bwd(li, gl, f.Ares[b], W * j, f.dZres[b], W * j);
-            rc = wgrad(li, f.dZres[b], W * j, {TStep::Tr{j == 1 ? f.Yt1[b] : f.IN[b], W * j, W, 0, 1}});
+            rc = wgrad(li, f.dZres[b], W * j, {{j == 1 ? f.Yt1[b] : f.IN[b], W * j, W, 0}});
             if (rc) return rc;
             rc = dgrad_gemm(li, f.dZres[b], W * j, f.DIN[b], W * j);
             if (rc) return rc;
         }
         {
             // chunk 0 of the tdnn1 output went straight into tdnn2: copy its gradient next to the others
-            TStep s;
-            s.kind = TStep::GRAD_SUM;
-            s.gl.n = 1;
-            s.gl.s[0] = src1(f.dRC[b], 0, 0);
-            s.C = W;
-            s.p0 = f.DIN[b];
-            s.c0 = 0;
-            push(s);
+            GradSrcList gl;
+            gl.n = 1;
+            gl.s[0] = src1(f.dRC[b], 0, 0);
+            grad_sum(gl, W, f.DIN[b], nullptr);
         }
         {
             GradSrcList gl;
             gl.n = 1;
             gl.s[0] = src1(f.DIN[b], 0, 1);
             bn_bwd(t->l_tdnn1[b], gl, f.At1[b], 0, f.dZt1[b], 0);
-            rc = wgrad(t->l_tdnn1[b], f.dZt1[b], 0, {TStep::Tr{u, uc, C, 0, 1}});
+            rc = wgrad(t->l_tdnn1[b], f.dZt1[b], 0, {{u, uc, C, 0}});
             if (rc) return rc;
             rc = dgrad_gemm(t->l_tdnn1[b], f.dZt1[b], 0, f.dXt1[b], 0);
             if (rc) return rc;
@@ -751,154 +830,57 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         gl.s[0] = src1(f.dXt1[0], 0, 0);
         gl.s[1] = src1(f.Dbuf[0], 0, 0);
         bn_bwd(t->l_conv0, gl, f.A0, 0, f.dZ0, 0);
-        rc = wgrad(t->l_conv0, f.dZ0, 0, {TStep::Tr{f.X0, 0, t->Fp, 0, 1}});
+        rc = wgrad(t->l_conv0, f.dZ0, 0, {{f.X0, 0, t->Fp, 0}});
         if (rc) return rc;
     }
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ step
+int Trainer::run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) {
+    const auto& v = s.vec;
+    const auto& o = s.f32;
+    const auto& d = s.dim;
+    switch (s.model_kind) {
+        case TR_REPACK: return tr_repack_conv(v[0], d[0], d[1], d[2], d[3], d[4], s.x, s.y, st);
+        case TR_PACK: return launch_pack_features(in.feat, s.B, s.T, s.C, s.out, s.P, s.Tp, st);
+        case TR_BN_FWD:
+            return tr_bn_forward(s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, TR_BN_EPS, TR_BN_MOMENTUM, v[0], v[1], o[0], o[1], o[2], o[3], o[4], o[5], o[6],
+                                 s.apply, num_sms, st);
+        case TR_DENSE_FWD: return tr_dense_fwd(v[0], d[0], v[1], d[1], v[2], d[2], d[3], d[4], d[5], o[0], d[6], st);
+        case TR_PLANES_TO_F32: return launch_planes_to_f32(s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, o[0], st);
+        case TR_ASP_POOL: return launch_asp_pool(v[0], d[0], s.x, s.C, s.B, s.T, s.P, s.Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), o[0], st);
+        case TR_BN1D_FWD: return tr_bn1d_fwd(v[0], s.B, s.C, TR_BN_EPS, TR_BN_MOMENTUM, v[1], v[2], o[0], o[1], o[2], o[3], o[4], st);
+        case TR_AAM_FWD:
+            return aam_forward(v[0], v[1], in.labels, s.B, d[0], d[1], in.margin, in.scale, in.easy_margin, in.label_smoothing, o[0], o[1], o[2],
+                               d[2], st);
+        case TR_AAM_BWD:
+            return aam_backward(v[0], v[1], in.labels, v[2], s.B, d[0], d[1], in.margin, in.scale, in.easy_margin, in.label_smoothing, o[0], o[1],
+                                o[2], d[2], st);
+        case TR_DENSE_BWD: return tr_dense_bwd(v[0], d[0], v[1], d[1], v[2], d[2], d[3], d[4], d[5], o[0], d[6], o[1], d[7], o[2], st);
+        case TR_BN1D_BWD: return tr_bn1d_bwd(v[0], v[1], s.B, s.C, v[2], v[3], v[4], o[0], o[1], o[2], st);
+        case TR_ASP_BWD: return tr_asp_bwd(v[0], d[0], s.x, s.C, s.B, s.T, s.P, s.Tp, TR_ASP_EPS, v[1], v[2], s.out, s.t, st);
+        case TR_GRAD_SUM: return tr_grad_sum(s.gl, s.C, s.B, s.T, s.P, s.Tp, s.out, s.oc0, o[0], o[1], st);
+        case TR_BN_BWD:
+            return tr_bn_backward(s.gl, s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, v[0], v[1], v[2], o[0], o[1], s.out, s.oc0, o[2], o[3], d[0], st, d[1]);
+        case TR_TRANSPOSE: return tr_transpose(s.x, s.xc0, s.C, s.rows, s.out, d[0], st, d[1], d[2], d[3]);
+        case TR_WGRAD_UNPACK: return tr_wgrad_unpack(v[0], d[0], d[1], d[2], d[3], d[4], d[5], o[0], d[6], st);
+        case TR_ASP_GLOBAL_BWD: return tr_asp_global_bwd(v[0], v[1], s.B, s.C, s.T, TR_ASP_EPS, o[0], o[1], st);
+        case TR_GRAD_DOT: return tr_grad_dot(s.gl, s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, o[0], st);
+        case TR_ACT_BWD: return tr_act_bwd(o[0], v[0], d[0], d[1], s.inv_count, st);
+    }
+    return PlanOwner::run_model_step(s, in, st);
+}
+
 int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* labels, int B, int T, float margin, float scale, int easy_margin,
                              float label_smoothing, float* loss_out, float* logits_out, void* ws, size_t ws_bytes, cudaStream_t st) {
     PPV_REQUIRE(t && feat && labels, "trainer_forward_backward: null argument");
     PPV_REQUIRE(B > 1 && T > 0, "trainer_forward_backward: batch of at least 2 required (batch statistics)");
     int rc = t->update_plan(B, T, ws, ws_bytes, st);
+    if (!rc) rc = t->run_plan(PlanInputs{feat, nullptr, labels, margin, scale, label_smoothing, easy_margin}, st);
     if (rc) return rc;
-    const TrBuffers& f = t->buf;
-    float* const par = t->params;
-    float* const grd = t->grads;
-    float* const sta = t->stats;
-    const int C = t->C, C3 = t->C3, P = t->P, Tp = f.Tp, se = t->se, att = t->att, D = t->D;
-    static const bool debug_sync = getenv("PPV_TRAIN_DEBUG") != nullptr;  // localise a faulting kernel: sync after every step
-    int step_idx = 0;
-    for (const TStep& s : t->steps) {
-        if (debug_sync) {
-            cudaError_t e = cudaStreamSynchronize(st);
-            if (e != cudaSuccess)
-                return fail(PPV_ECUDA, "trainer: step " + std::to_string(step_idx - 1) + " (kind " + std::to_string(int(t->steps[std::max(step_idx - 1, 0)].kind)) +
-                                           ", layer " + std::to_string(t->steps[std::max(step_idx - 1, 0)].layer) + ") failed: " + cudaGetErrorString(e));
-        }
-        ++step_idx;
-        switch (s.kind) {
-            case TStep::REPACK: {
-                for (int l = 0; l <= t->l_att2() && !rc; ++l) {
-                    const TConv& c = t->conv(l);
-                    rc = tr_repack_conv(par + c.w_off, int64_t(c.CinTotal) * c.taps, c.Cout, c.Cin, c.Cinp, c.taps, f.layer[l].wf, f.layer[l].wd, st);
-                }
-                break;
-            }
-            case TStep::PACK: rc = launch_pack_features(feat, B, T, t->cfg.input_size, f.X0, P, Tp, st); break;
-            case TStep::GEMM: rc = gemm_launch(s.gp, t->precision, t->num_sms, st); break;
-            case TStep::BN_FWD: {
-                const TBN& bn = t->L[s.layer].bn;
-                const TrBuffers::Layer& w = f.layer[s.layer];
-                rc = tr_bn_forward(s.p0, s.c0, bn.C, B, T, P, Tp, TR_BN_EPS, TR_BN_MOMENTUM, par + bn.g_off, par + bn.b_off, w.mean, w.rstd, w.scale,
-                                   w.shift, sta + bn.rm_off, sta + bn.rv_off, f.part, s.ap, t->num_sms, st);
-                break;
-            }
-            case TStep::SE_FWD: {
-                const int b = s.a;
-                rc = launch_colstats(f.Yt2[b], 0, C, B, T, P, Tp, 0, 0.f, f.se_s[b], Planes(), st);
-                if (rc) return rc;
-                rc = tr_dense_fwd(f.se_s[b], C, par + t->se1_w[b], C, par + t->se1_b[b], B, se, C, 1, f.se_g1[b], se, st);
-                if (rc) return rc;
-                rc = tr_dense_fwd(f.se_g1[b], se, par + t->se2_w[b], se, par + t->se2_b[b], B, C, se, 2, f.se_g2[b], C, st);
-                break;
-            }
-            case TStep::SCALE_RES:
-                rc = launch_se_scale_res(f.Yt2[s.a], f.se_g2[s.a], s.p0, s.c0, f.OUTCAT, C * s.a, C, Tp, f.R, t->num_sms, st);
-                break;
-            case TStep::ASP_HEAD_FWD: {
-                rc = launch_colstats(f.M, 0, C3, B, T, P, Tp, 1, TR_ASP_EPS, nullptr, f.gstat_pl, st);
-                if (rc) return rc;
-                rc = launch_planes_to_f32(f.gstat_pl, 0, 2 * C3, B, 1, 0, 1, f.gstat, st);
-                if (rc) return rc;
-                const TConv& c = t->L[t->l_att1].conv;  // weight [att][3*C3]: columns C3.. multiply [mean | std]
-                rc = tr_dense_fwd(f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, f.fold, att, st);
-                break;
-            }
-            case TStep::ASP_TAIL_FWD: {
-                rc = launch_asp_pool(f.logits, C3, f.M, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), f.pooled, st);
-                if (rc) return rc;
-                rc = tr_bn1d_fwd(f.pooled, B, 2 * C3, TR_BN_EPS, TR_BN_MOMENTUM, par + t->aspbn_g, par + t->aspbn_b, f.pn, f.aspbn_mean, f.aspbn_rstd,
-                                 sta + t->aspbn_rm, sta + t->aspbn_rv, st);
-                if (rc) return rc;
-                rc = tr_dense_fwd(f.pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, f.emb, D, st);
-                break;
-            }
-            case TStep::LOSS:
-                rc = aam_forward(f.emb, par + t->cls_w, labels, B, D, t->S, margin, scale, easy_margin, label_smoothing, f.cls_logits, f.loss,
-                                 f.aam_ws, f.aam_ws_bytes, st);
-                break;
-            case TStep::HEAD_BWD: {
-                rc = aam_backward(f.emb, par + t->cls_w, labels, f.cls_logits, B, D, t->S, margin, scale, easy_margin, label_smoothing, f.d_emb,
-                                  grd + t->cls_w, f.aam_ws, f.aam_ws_bytes, st);
-                if (rc) return rc;
-                rc = tr_dense_bwd(f.d_emb, D, f.pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, f.dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b, st);
-                if (rc) return rc;
-                rc = tr_bn1d_bwd(f.dpn, f.pooled, B, 2 * C3, par + t->aspbn_g, f.aspbn_mean, f.aspbn_rstd, f.dpooled, grd + t->aspbn_g,
-                                 grd + t->aspbn_b, st);
-                break;
-            }
-            case TStep::ASP_BWD:
-                rc = tr_asp_bwd(f.logits, C3, f.M, C3, B, T, P, Tp, TR_ASP_EPS, f.pooled, f.dpooled, f.dlogits, f.dMd, st);
-                break;
-            case TStep::COLSUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, Planes(), 0, f.part, s.f0, st); break;
-            case TStep::GRAD_SUM: rc = tr_grad_sum(s.gl, s.C, B, T, P, Tp, s.p0, s.c0, f.part, nullptr, st); break;
-            case TStep::BN_BWD: {
-                const TLayer& l = t->L[s.layer];
-                rc = tr_bn_backward(s.gl, s.p0, s.c0, l.bn.C, B, T, P, Tp, f.layer[s.layer].mean, f.layer[s.layer].rstd, par + l.bn.g_off, grd + l.bn.g_off, grd + l.bn.b_off,
-                                    s.p1, s.c1, grd + l.conv.b_off, f.part, f.part_elems, st, s.a);
-                break;
-            }
-            case TStep::ASP_CTX_BWD: {
-                // f.part holds sum_t dz per utterance [B][att] (left by the BN backward of the attention TDNN)
-                const TConv& c = t->L[t->l_att1].conv;
-                rc = tr_dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3,
-                                  nullptr, st);
-                if (rc) return rc;
-                rc = tr_asp_global_bwd(f.gstat, f.dgs, B, C3, T, TR_ASP_EPS, f.rs, f.rb, st);
-                break;
-            }
-            case TStep::SE_BWD: {
-                const int b = s.a;
-                GradSrcList gl;
-                gl.n = 1;
-                gl.s[0].t = f.Dbuf[b];
-                rc = tr_grad_dot(gl, f.Yt2[b], 0, C, B, T, P, Tp, f.dg2, st);
-                if (rc) return rc;
-                rc = tr_act_bwd(f.dg2, f.se_g2[b], int64_t(B) * C, 2, 0.f, st);
-                if (rc) return rc;
-                rc = tr_dense_bwd(f.dg2, C, f.se_g1[b], se, par + t->se2_w[b], se, B, C, se, f.dg1, se, grd + t->se2_w[b], se, grd + t->se2_b[b], st);
-                if (rc) return rc;
-                rc = tr_act_bwd(f.dg1, f.se_g1[b], int64_t(B) * se, 1, 0.f, st);
-                if (rc) return rc;
-                rc = tr_dense_bwd(f.dg1, se, f.se_s[b], C, par + t->se1_w[b], C, B, se, C, f.ds, C, grd + t->se1_w[b], C, grd + t->se1_b[b], st);
-                if (rc) return rc;
-                rc = tr_act_bwd(f.ds, nullptr, int64_t(B) * C, 0, 1.f / float(T), st);
-                break;
-            }
-            case TStep::WGRAD: {
-                const TConv& c = t->conv(s.layer);
-                for (const TStep::Tr& tr : s.trs) {
-                    Planes dst = tr.which == 0 ? f.TA : f.TB;
-                    dst.base += int64_t(tr.row0) * dst.ld;
-                    dst.rows -= tr.row0;
-                    rc = tr_transpose(tr.in, tr.col0, tr.C, f.R, dst, tr.shift, st, tr.ntaps, tr.shift_step, tr.row_step);
-                    if (rc) return rc;
-                }
-                for (const GemmParams& gp : s.wg) {
-                    rc = gemm_launch(gp, t->precision, t->num_sms, st);
-                    if (rc) return rc;
-                }
-                rc = tr_wgrad_unpack(f.wpart, s.a, s.b, c.Cout, c.Cin, c.Cinp, c.taps, grd + c.w_off, int64_t(c.CinTotal) * c.taps, st);
-                break;
-            }
-        }
-        if (rc) return rc;
-    }
-    if (loss_out) PPV_CUDA_OK(cudaMemcpyAsync(loss_out, f.loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (logits_out) PPV_CUDA_OK(cudaMemcpyAsync(logits_out, f.cls_logits, size_t(B) * t->S * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (loss_out) PPV_CUDA_OK(cudaMemcpyAsync(loss_out, t->buf.loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (logits_out) PPV_CUDA_OK(cudaMemcpyAsync(logits_out, t->buf.cls_logits, size_t(B) * t->S * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return PPV_OK;
 }
 

@@ -131,11 +131,7 @@ void image_pyramid(ImageGeo* levels, int n, int H, int W, bool halve_w) {
 }
 
 Epilogue image_epilogue(const Planes& out, const ImageGeo& gin, const ImageGeo& gout, int stride_h, int stride_w) {
-    Epilogue ep;
-    ep.out_mode = OUT_PLANES;
-    ep.out = out.base;
-    ep.out_ld = out.ld;
-    ep.out_plane_stride = out.plane_stride;
+    Epilogue ep = planes_epilogue(out);
     ep.img_Hp = gin.Hp;
     ep.img_Wp = gin.Wp;
     ep.img_H = gin.H;

@@ -1,5 +1,5 @@
 // How the 2-D models (ResNetSE, ERes2Net, CAM++) plan their convolutions over image grids, in one place (image_plan.cu).  The plan
-// itself (PlanStep, PlanModel and its executor) is shared with ECAPA-TDNN: plan.h.
+// itself (PlanStep, PlanModel and the executor) is shared with ECAPA-TDNN: plan.h.
 //
 // Layout: every activation is split-bf16 planes over rows (b, h+1, w+1) of a [B, H+2, W+2] grid whose border rows are zero and
 // are never written (freq = H, time = W, channels last).  With that layout

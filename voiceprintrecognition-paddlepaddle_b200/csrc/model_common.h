@@ -1,5 +1,5 @@
 // Host-side helpers shared by the model plans: named fp32 weights as loaded through the C ABI, an arena image that is
-// built on the host (split-bf16 weight planes, fp32 vectors) and uploaded once, and the workspace carver.
+// built on the host (split-bf16 weight planes, fp32 vectors) and uploaded once, the workspace carver, and the ECAPA-TDNN geometry.
 #pragma once
 #include <string.h>
 
@@ -217,116 +217,31 @@ struct WsCarver {
     }
 };
 
-// A plan of launches over a caller-owned workspace, built for (workspace, B, T) and rebuilt whenever one of them changes: the
-// inference models and the training step.
-struct PlanOwner {
-    const char* prefix;    // error-message prefix, e.g. "resnetse"
-    const char* ws_query;  // the C ABI entry point that sizes the workspace, named in the "workspace too small" error
-    int precision;
-    int num_sms;
-    void* plan_ws = nullptr;  // the plan's key (plan_ws, plan_B, plan_T); null and zeros when no plan is built
-    int plan_B = 0, plan_T = 0;
-
-    PlanOwner(const char* prefix, const char* ws_query, int precision)
-        : prefix(prefix), ws_query(ws_query), precision(precision), num_sms(device_sm_count()) {}
-    virtual ~PlanOwner() = default;
-    // Bytes of workspace a plan for B utterances of T frames carves; computed without touching the current plan.
-    virtual size_t workspace_bytes(int B, int T) const = 0;
-
-    // No plan: B > 0 in every run, so no key matches this one and the next run rebuilds.
-    void invalidate_plan() {
-        plan_ws = nullptr;
-        plan_B = plan_T = 0;
-    }
-    int update_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
-        if (plan_ws == ws && plan_B == B && plan_T == T) return PPV_OK;
-        int rc = build_plan(B, T, ws, ws_bytes, st);
-        if (rc) {
-            invalidate_plan();
-            return rc;
-        }
-        plan_ws = ws;
-        plan_B = B;
-        plan_T = T;
-        return PPV_OK;
-    }
-
-  protected:
-    // The opening of build_plan: `ws` must hold workspace_bytes(B, T) bytes at 256-byte alignment; it is zeroed on `st`, because the
-    // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
-    int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
-        const size_t need = workspace_bytes(B, T);
-        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see " + ws_query + ")");
-        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
-        PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
-        return PPV_OK;
-    }
-    // Carves `ws` and plans the launches of a run over B utterances of T frames.
-    virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
+// The geometry of an ECAPA-TDNN config, shared by the inference plan and the training step, after the checks both need:
+// channels [C, C, C, C, 3C], res2net_scale in [2, 8] with chunks of a multiple of 64 channels, kernel sizes [odd, 3, 3, 3, 1].
+struct EcapaGeometry {
+    int C = 0, C3 = 0, width = 0, scale = 0, Fp = 0, P = 0, att = 0, se = 0;  // P: the reflect padding of the time axis
 };
-
-// An inference model behind ppv_model_*: weights are loaded by name, prepared into one device arena by finalize(), and each
-// forward runs the plan.
-struct Model : PlanOwner {
-    WeightMap raw;
-    bool finalized = false;
-    void* arena = nullptr;
-    float* emb_out = nullptr;  // workspace buffer the plan's last step writes the embeddings [B][embd_dim] to
-
-    Model(const char* prefix, int precision) : PlanOwner(prefix, "ppv_model_workspace_bytes", precision) {}
-    ~Model() override { cudaFree(arena); }
-    virtual int embd_dim() const = 0;
-
-    int load_weight(const char* name, const float* data, const int64_t* shape, int ndim) {
-        if (finalized) return fail(PPV_ESTATE, std::string(prefix) + "_load_weight: model already finalized");
-        return weight_map_load(&raw, name, data, shape, ndim);
-    }
-    int set_precision(int p) {
-        PPV_REQUIRE(p == PPV_PREC_BF16X3 || p == PPV_PREC_BF16, "bad precision");
-        precision = p;
-        return PPV_OK;
-    }
-    int finalize() {
-        if (finalized) return PPV_OK;
-        ArenaBuilder ab;
-        ab.wm = &raw;
-        if (!prepare_weights(ab))
-            return fail(PPV_EINVAL, std::string(prefix) + "_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
-        int rc = ab.upload(&arena);
-        if (rc) return rc;
-        raw.clear();
-        finalized = true;
-        return PPV_OK;
-    }
-    int forward(const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
-        int rc = forward_begin(emb, B, T);
-        if (!rc) rc = update_plan(B, T, ws, ws_bytes, st);
-        if (!rc) rc = run_steps(feat, st);
-        return rc ? rc : copy_embeddings(emb, st);
-    }
-    int read_tap(const char* name, float* out, size_t out_elems, cudaStream_t st) {
-        PPV_REQUIRE(name && out, std::string(prefix) + "_read_tap: null argument");
-        if (!plan_ws) return fail(PPV_ESTATE, std::string(prefix) + "_read_tap: no forward has run");
-        return tap(name, out, out_elems, st);
-    }
-
-  protected:
-    // The steps of forward(), for models whose forward takes more inputs.
-    int forward_begin(const float* emb, int B, int T) {
-        PPV_REQUIRE(emb, std::string(prefix) + "_forward: null argument");
-        if (!finalized) return fail(PPV_ESTATE, std::string(prefix) + "_forward: call ppv_model_finalize first");
-        PPV_REQUIRE(B > 0 && T > 0, std::string(prefix) + "_forward: empty batch");
-        return PPV_OK;
-    }
-    int copy_embeddings(float* emb, cudaStream_t st) {
-        PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(plan_B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        return PPV_OK;
-    }
-    // Puts the prepared weights into the arena image; false, with ab.err set where known, on a missing or misshapen weight.
-    virtual bool prepare_weights(ArenaBuilder& ab) = 0;
-    // Launches the planned steps on features [plan_B, plan_T, input_size].
-    virtual int run_steps(const float* feat, cudaStream_t st) = 0;
-    virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
-};
+inline int ecapa_geometry(const ppv_ecapa_cfg& cfg, EcapaGeometry* g) {
+    const int C = cfg.channels[0];
+    if (cfg.channels[1] != C || cfg.channels[2] != C || cfg.channels[3] != C)
+        return fail(PPV_EUNSUPPORTED, "ecapa: channels[0..3] must be equal (no shortcut conv path)");
+    if (cfg.channels[4] != 3 * C) return fail(PPV_EUNSUPPORTED, "ecapa: channels[4] must equal 3 * channels[0] (MFA concat)");
+    if (cfg.res2net_scale < 2 || cfg.res2net_scale > 8 || C % cfg.res2net_scale)
+        return fail(PPV_EUNSUPPORTED, "ecapa: res2net_scale must divide channels and be in [2,8]");
+    if ((C / cfg.res2net_scale) % 64) return fail(PPV_EUNSUPPORTED, "ecapa: channels / res2net_scale must be a multiple of 64");
+    if (cfg.kernel_sizes[1] != 3 || cfg.kernel_sizes[2] != 3 || cfg.kernel_sizes[3] != 3 || cfg.kernel_sizes[4] != 1 || (cfg.kernel_sizes[0] % 2) == 0)
+        return fail(PPV_EUNSUPPORTED, "ecapa: kernel sizes must be [odd,3,3,3,1]");
+    g->C = C;
+    g->C3 = 3 * C;
+    g->scale = cfg.res2net_scale;
+    g->width = C / cfg.res2net_scale;
+    g->Fp = int(mc_align_up(size_t(cfg.input_size), 64));
+    g->att = cfg.attention_channels;
+    g->se = cfg.se_channels;
+    g->P = (cfg.kernel_sizes[0] - 1) / 2 * cfg.dilations[0];
+    for (int i = 1; i <= 3; ++i) g->P = std::max(g->P, cfg.dilations[i]);
+    return PPV_OK;
+}
 
 }  // namespace ppv

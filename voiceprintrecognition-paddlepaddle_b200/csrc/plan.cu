@@ -1,4 +1,4 @@
-// The inference models' plan (plan.h): step constructors, layer routing, the step executor and its launch profile.
+// The plans (plan.h): step constructors, layer routing, the step executor and its launch profile.
 #include "plan.h"
 
 namespace ppv {
@@ -114,8 +114,9 @@ int PlanModel::plan_row_linear(const GemmWeights& gw, const GemmSource& src, int
 }
 
 // ------------------------------------------------------------------------------------------------ executor
-int PlanModel::run_plan(const float* feat, const int* nvalid, cudaStream_t st) {
-    for (const PlanStep& s : steps) {
+int PlanOwner::run_plan(const PlanInputs& in, cudaStream_t st) {
+    for (size_t i = 0; i < steps.size(); ++i) {
+        const PlanStep& s = steps[i];
         const bool tensor_step = s.kind == PlanStep::GEMM || s.kind == PlanStep::CONV3X3 || s.kind == PlanStep::RES2 ||
                                  s.kind == PlanStep::RES2CHAIN || s.kind == PlanStep::ASP_FUSED;
         // (SKINNY and POINTWISE steps count as "other kernels": their FLOPs are not credited to the tensor-core roofline)
@@ -137,43 +138,49 @@ int PlanModel::run_plan(const float* feat, const int* nvalid, cudaStream_t st) {
                 break;
             case PlanStep::CONV3X3: rc = conv3x3_launch(s.c3, precision, num_sms, st); break;
             case PlanStep::POINTWISE: rc = pointwise_launch(s.pw, num_sms, st); break;
-            case PlanStep::STEM: rc = launch_stem_conv(feat, s.B, s.g.W, s.g.H, s.vec[0], s.vec[1], s.C, s.out, s.g.Hp, s.g.Wp, st); break;
+            case PlanStep::STEM: rc = launch_stem_conv(in.feat, s.B, s.g.W, s.g.H, s.vec[0], s.vec[1], s.C, s.out, s.g.Hp, s.g.Wp, st); break;
             case PlanStep::SCALE_RES:
                 rc = launch_se_scale_res(s.x, s.vec[0], s.y, s.yc0, s.out, s.oc0, s.C, s.utt_rows, s.rows, num_sms, st, s.relu ? 1 : 0, s.relu_max);
                 break;
             case PlanStep::AFF_COMBINE: rc = launch_aff_combine(s.x, s.xc0, s.y, s.yc0, s.t, s.out, s.C, s.rows, num_sms, st); break;
             case PlanStep::FLATTEN_IMAGE: rc = launch_flatten_image(s.x, s.B, s.g.H, s.g.W, s.g.Hp, s.g.Wp, s.C, s.out, num_sms, st); break;
             case PlanStep::COLSTATS:
-                rc = launch_colstats(s.x, 0, s.C, s.B, s.T, s.P, s.Tp, s.mode, s.eps, nullptr, s.out, st, s.inv_count, s.masked ? nvalid : nullptr);
+                rc = launch_colstats(s.x, 0, s.C, s.B, s.T, s.P, s.Tp, s.mode, s.eps, s.out_f32, s.out, st, s.inv_count, s.masked ? in.nvalid : nullptr);
                 break;
             case PlanStep::ASP_FUSED: {
                 AspFusedParams ap = s.ap;
-                ap.nvalid = nvalid;
+                ap.nvalid = in.nvalid;
                 rc = asp_fused_launch(ap, precision, num_sms, st);
                 break;
             }
-            case PlanStep::MODEL: rc = run_model_step(s, st); break;
+            case PlanStep::MODEL: rc = run_model_step(s, in, st); break;
         }
         prof_end(st);
         if (rc) return rc;
+        if (sync_each_step) {
+            const cudaError_t e = cudaStreamSynchronize(st);
+            const std::string model = s.kind == PlanStep::MODEL ? ", model kind " + std::to_string(s.model_kind) : "";
+            if (e != cudaSuccess)
+                return fail(PPV_ECUDA, std::string(prefix) + ": step " + std::to_string(i) + " (kind " + std::to_string(int(s.kind)) + model + ") failed: " + cudaGetErrorString(e));
+        }
     }
     return PPV_OK;
 }
 
-int PlanModel::run_model_step(const PlanStep&, cudaStream_t) { return fail(PPV_EINVAL, std::string(prefix) + ": plan step of unknown kind"); }
+int PlanOwner::run_model_step(const PlanStep&, const PlanInputs&, cudaStream_t) { return fail(PPV_EINVAL, std::string(prefix) + ": plan step of unknown kind"); }
 
 // ------------------------------------------------------------------------------------------------ profile
-PlanModel::~PlanModel() {
+PlanOwner::~PlanOwner() {
     for (cudaEvent_t e : prof_ev) cudaEventDestroy(e);
 }
 
-void PlanModel::profile(bool enable) {
+void PlanOwner::profile(bool enable) {
     prof_on = enable;
     prof_used = 0;
     launches_gemm = launches_other = 0;
 }
 
-void PlanModel::prof_begin(int kind, cudaStream_t st) {
+void PlanOwner::prof_begin(int kind, cudaStream_t st) {
     if (!prof_on) return;
     if (prof_used + 2 > prof_ev.size()) {
         cudaEvent_t a, b;
@@ -187,13 +194,13 @@ void PlanModel::prof_begin(int kind, cudaStream_t st) {
     cudaEventRecord(prof_ev[prof_used], st);
 }
 
-void PlanModel::prof_end(cudaStream_t st) {
+void PlanOwner::prof_end(cudaStream_t st) {
     if (!prof_on) return;
     cudaEventRecord(prof_ev[prof_used + 1], st);
     prof_used += 2;
 }
 
-int PlanModel::profile_read(double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
+int PlanOwner::profile_read(double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
     double g = 0, o = 0;
     if (prof_used >= 2) PPV_CUDA_OK(cudaEventSynchronize(prof_ev[prof_used - 1]));
     for (size_t i = 0; i + 1 < prof_used; i += 2) {

@@ -1,12 +1,14 @@
-// The inference models' plans, in one place (plan.cu): ECAPA-TDNN, ResNetSE, ERes2Net(V2) and CAM++ each plan their forward as a
-// list of PlanSteps, each holding every argument of its launch, and PlanModel::run_plan launches them in order.  The routing helpers
-// choose a layer's kernel; what is about zero-bordered image grids (the 2-D models) is in image_plan.h.
+// The plans, in one place (plan.cu): ECAPA-TDNN, ResNetSE, ERes2Net(V2) and CAM++ each plan their forward, and the ECAPA-TDNN
+// trainer its training step, as a list of PlanSteps, each holding every argument of its launch; PlanOwner::run_plan launches them in
+// order.  The routing helpers choose a layer's kernel; what is about zero-bordered image grids (the 2-D models) is in image_plan.h.
 #pragma once
+#include <array>
 #include <string>
 #include <vector>
 
 #include "common.h"
 #include "model_common.h"
+#include "train.h"
 
 namespace ppv {
 
@@ -23,11 +25,11 @@ struct PlanStep {
     // SCALE_RES: out[:, oc0 + c] = x[:, c] * vec[0][utterance][c] + y[:, yc0 + c] (vec[0] null: no scale), then, if relu, ReLU clipped
     // at relu_max > 0, over `rows` rows of utt_rows rows per utterance (Tp frames, or an image's Hp x Wp grid);
     // AFF_COMBINE: out = x (1 + t) + y (1 - t) over `rows`;  FLATTEN_IMAGE: x on grid g -> out;
-    // COLSTATS: launch_colstats of x's first C columns into out, over each utterance's first nvalid frames if `masked` and the forward
-    // has them;  MODEL: what the model puts here.
+    // COLSTATS: launch_colstats of x's first C columns into the planes `out` or, if set, out_f32, over each utterance's first nvalid
+    // frames if `masked` and the run has them;  MODEL: what the model puts here.
     Planes x, y, t, out;
     int xc0 = 0, yc0 = 0, oc0 = 0;
-    const float* vec[4] = {};
+    std::array<const float*, 6> vec{};
     float* out_f32 = nullptr;
     ImageGeo g;
     int B = 0, C = 0, T = 0, P = 0, Tp = 0, mode = 0, n = 0;
@@ -35,6 +37,13 @@ struct PlanStep {
     int utt_rows = 0;
     float eps = 0.f, inv_count = 0.f, relu_max = 0.f;
     bool relu = false, masked = false;
+    // The trainer's MODEL steps (ecapa_train.cu) take their launcher's arguments from the fields above and these: the Planes it reads
+    // from x, y (column offsets xc0, yc0) and those it writes from out, t (oc0); the fp32 arrays it reads from vec and those it writes
+    // from f32, each in the launcher's order; B, C, T, P, Tp; every other integer from dim, in the launcher's order.
+    std::array<float*, 8> f32{};
+    std::array<int64_t, 8> dim{};
+    GradSrcList gl;
+    BnApplyArgs apply;
 };
 
 PlanStep stem_step(const float* w9, const float* bias, int C0, const Planes& out, const ImageGeo& g, int B);
@@ -46,13 +55,50 @@ PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int 
                        bool masked = false);
 PlanStep model_step(int model_kind);
 
-// A model whose forward is a plan of PlanSteps.
-struct PlanModel : Model {
-    std::vector<PlanStep> steps;
-    int max_bn = 256;  // widest gather-GEMM n-tile plan_gemm picks
+// What a run of a plan reads besides the plan itself.
+struct PlanInputs {
+    const float* feat = nullptr;      // features [plan_B, plan_T, input_size]
+    const int* nvalid = nullptr;      // inference: [plan_B] valid-frame counts for masked COLSTATS and ASP_FUSED steps (null: every frame)
+    const int64_t* labels = nullptr;  // training: [plan_B] class labels and the AAM-softmax settings
+    float margin = 0.f, scale = 0.f, label_smoothing = 0.f;
+    int easy_margin = 0;
+};
 
-    using Model::Model;
-    ~PlanModel() override;
+// A plan of launches over a caller-owned workspace, built for (workspace, B, T) and rebuilt whenever one of them changes: the
+// inference models and the training step.
+struct PlanOwner {
+    const char* prefix;    // error-message prefix, e.g. "resnetse"
+    const char* ws_query;  // the C ABI entry point that sizes the workspace, named in the "workspace too small" error
+    int precision;
+    int num_sms;
+    void* plan_ws = nullptr;  // the plan's key (plan_ws, plan_B, plan_T); null and zeros when no plan is built
+    int plan_B = 0, plan_T = 0;
+    std::vector<PlanStep> steps;
+    bool sync_each_step = false;  // run_plan synchronises after every step and names the one that failed (localises a faulting kernel)
+
+    PlanOwner(const char* prefix, const char* ws_query, int precision)
+        : prefix(prefix), ws_query(ws_query), precision(precision), num_sms(device_sm_count()) {}
+    virtual ~PlanOwner();
+    // Bytes of workspace a plan for B utterances of T frames carves; computed without touching the current plan.
+    virtual size_t workspace_bytes(int B, int T) const = 0;
+
+    // No plan: B > 0 in every run, so no key matches this one and the next run rebuilds.
+    void invalidate_plan() {
+        plan_ws = nullptr;
+        plan_B = plan_T = 0;
+    }
+    int update_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
+        if (plan_ws == ws && plan_B == B && plan_T == T) return PPV_OK;
+        int rc = build_plan(B, T, ws, ws_bytes, st);
+        if (rc) {
+            invalidate_plan();
+            return rc;
+        }
+        plan_ws = ws;
+        plan_B = B;
+        plan_T = T;
+        return PPV_OK;
+    }
 
     // Launch profile (ppv_model_profile): with it on, run_plan records a CUDA event pair around each launch group; the launch counters
     // count every run.  Tensor-core steps (GEMM, CONV3X3, RES2, RES2CHAIN, ASP_FUSED) are one kind, every other launch the other.
@@ -61,16 +107,103 @@ struct PlanModel : Model {
     int profile_read(double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches);
 
   protected:
-    int run_steps(const float* feat, cudaStream_t st) override { return run_plan(feat, nullptr, st); }
-    // The executor: feat [plan_B, plan_T, input_size] for STEM steps, nvalid [plan_B] valid-frame counts for masked COLSTATS and
-    // ASP_FUSED steps (null: every frame).
-    int run_plan(const float* feat, const int* nvalid, cudaStream_t st);
-    virtual int run_model_step(const PlanStep& s, cudaStream_t st);
+    // The opening of build_plan: `ws` must hold workspace_bytes(B, T) bytes at 256-byte alignment; it is zeroed on `st`, because the
+    // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
+    int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
+        const size_t need = workspace_bytes(B, T);
+        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see " + ws_query + ")");
+        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
+        PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
+        return PPV_OK;
+    }
+    // Carves `ws` and plans the launches of a run over B utterances of T frames.
+    virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
+    // The executor: launches the planned steps in order.
+    int run_plan(const PlanInputs& in, cudaStream_t st);
+    virtual int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st);
     // an event pair around launches of kind 0 (tensor cores) or 1 (other), recorded while the profile is on
     void prof_begin(int kind, cudaStream_t st);
     void prof_end(cudaStream_t st);
     int64_t launches_gemm = 0, launches_other = 0;
 
+  private:
+    bool prof_on = false;
+    std::vector<cudaEvent_t> prof_ev;  // pairs
+    std::vector<int> prof_kind;        // per pair: 0 = tensor cores, 1 = other
+    size_t prof_used = 0;
+};
+
+// An inference model behind ppv_model_*: weights are loaded by name, prepared into one device arena by finalize(), and each
+// forward runs the plan.
+struct Model : PlanOwner {
+    WeightMap raw;
+    bool finalized = false;
+    void* arena = nullptr;
+    float* emb_out = nullptr;  // workspace buffer the plan's last step writes the embeddings [B][embd_dim] to
+
+    Model(const char* prefix, int precision) : PlanOwner(prefix, "ppv_model_workspace_bytes", precision) {}
+    ~Model() override { cudaFree(arena); }
+    virtual int embd_dim() const = 0;
+
+    int load_weight(const char* name, const float* data, const int64_t* shape, int ndim) {
+        if (finalized) return fail(PPV_ESTATE, std::string(prefix) + "_load_weight: model already finalized");
+        return weight_map_load(&raw, name, data, shape, ndim);
+    }
+    int set_precision(int p) {
+        PPV_REQUIRE(p == PPV_PREC_BF16X3 || p == PPV_PREC_BF16, "bad precision");
+        precision = p;
+        return PPV_OK;
+    }
+    int finalize() {
+        if (finalized) return PPV_OK;
+        ArenaBuilder ab;
+        ab.wm = &raw;
+        if (!prepare_weights(ab))
+            return fail(PPV_EINVAL, std::string(prefix) + "_finalize: " + (ab.err.empty() ? std::string("bad weights") : ab.err));
+        int rc = ab.upload(&arena);
+        if (rc) return rc;
+        raw.clear();
+        finalized = true;
+        return PPV_OK;
+    }
+    int forward(const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
+        int rc = forward_begin(emb, B, T);
+        if (!rc) rc = update_plan(B, T, ws, ws_bytes, st);
+        if (!rc) rc = run_steps(feat, st);
+        return rc ? rc : copy_embeddings(emb, st);
+    }
+    int read_tap(const char* name, float* out, size_t out_elems, cudaStream_t st) {
+        PPV_REQUIRE(name && out, std::string(prefix) + "_read_tap: null argument");
+        if (!plan_ws) return fail(PPV_ESTATE, std::string(prefix) + "_read_tap: no forward has run");
+        return tap(name, out, out_elems, st);
+    }
+
+  protected:
+    // The steps of forward(), for models whose forward takes more inputs.
+    int forward_begin(const float* emb, int B, int T) {
+        PPV_REQUIRE(emb, std::string(prefix) + "_forward: null argument");
+        if (!finalized) return fail(PPV_ESTATE, std::string(prefix) + "_forward: call ppv_model_finalize first");
+        PPV_REQUIRE(B > 0 && T > 0, std::string(prefix) + "_forward: empty batch");
+        return PPV_OK;
+    }
+    int copy_embeddings(float* emb, cudaStream_t st) {
+        PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(plan_B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        return PPV_OK;
+    }
+    // Puts the prepared weights into the arena image; false, with ab.err set where known, on a missing or misshapen weight.
+    virtual bool prepare_weights(ArenaBuilder& ab) = 0;
+    // Launches the planned steps on features [plan_B, plan_T, input_size].
+    virtual int run_steps(const float* feat, cudaStream_t st) { return run_plan(PlanInputs{feat}, st); }
+    virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
+};
+
+// An inference model with the layer routing helpers.
+struct PlanModel : Model {
+    int max_bn = 256;  // widest gather-GEMM n-tile plan_gemm picks
+
+    using Model::Model;
+
+  protected:
     // Routing, one entry per kind of layer; each appends its step.  M = GEMM rows; ep.bias is set from gw.
     // gather-GEMM only, n-tile up to max_bn
     int plan_gemm(const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep);
@@ -89,12 +222,6 @@ struct PlanModel : Model {
     static int name_index(const std::string& n, const char* base, int lo, int hi);
     // fp32 [B, H, W, C] copy of image planes, after checking out_elems
     int image_tap(const Planes& src, const ImageGeo& g, int C, float* out, size_t out_elems, cudaStream_t st) const;
-
-  private:
-    bool prof_on = false;
-    std::vector<cudaEvent_t> prof_ev;  // pairs
-    std::vector<int> prof_kind;        // per pair: 0 = tensor cores, 1 = other
-    size_t prof_used = 0;
 };
 
 }  // namespace ppv

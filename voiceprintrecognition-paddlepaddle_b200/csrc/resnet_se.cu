@@ -253,11 +253,7 @@ int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
     m->steps.clear();
 
     auto plain_planes = [&](const Planes& p, bool relu) {
-        Epilogue ep;
-        ep.out_mode = OUT_PLANES;
-        ep.out = p.base;
-        ep.out_ld = p.ld;
-        ep.out_plane_stride = p.plane_stride;
+        Epilogue ep = planes_epilogue(p);
         ep.relu = relu ? 1 : 0;
         return ep;
     };
