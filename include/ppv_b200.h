@@ -319,6 +319,29 @@ int ppv_eer_mindcf_matrix(const float* scores, const int32_t* trial_labels, cons
 int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* best, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Speaker diarization: spectral clustering of the chunk embeddings.  Replaces
+ * ppvector/infer_utils/speaker_diarization.py:219-310 (SpectralCluster: pruning, Laplacian, scipy.linalg.eigh,
+ * sklearn k_means).  The affinity is ppv_cosine_matrix of the [N, D] embeddings.  One stage per entry point, so that each
+ * can be fed the previous stage's stored output.  All arithmetic after the affinity is fp64 and every sum runs in a fixed
+ * order: results are bitwise reproducible.  N (windows) must be 1 <= N <= 8192, else PPV_EINVAL.
+ * ------------------------------------------------------------------------------------------- */
+/* In place on affinity [N,N] fp32: pval' = 6/N if N*pval < 6 else pval; each row zeroes its int((1-pval')*N) smallest entries
+ * (exact ties: the lower column index first). */
+int ppv_cluster_prune(float* affinity, int N, double pval, void* stream);
+/* pruned [N,N] fp32 -> L [N,N] fp64 = diag(D) - M, M = (P + P^T)/2 with a zero diagonal, D_i = sum_j |M_ij|. */
+int ppv_cluster_laplacian(const float* pruned, int N, double* L, void* stream);
+/* The m (1 <= m <= min(N, 32)) smallest eigenvalues of the symmetric L [N,N] fp64 (overwritten), ascending -> evals [m], and
+ * their eigenvectors -> evecs [N,m] (row-major).  ws: ppv_sym_eig_workspace_bytes(N, m) bytes, 256-byte aligned. */
+size_t ppv_sym_eig_workspace_bytes(int N, int m);
+int ppv_sym_eig_smallest(double* L, int N, int m, double* evals, double* evecs, void* ws, size_t ws_bytes, void* stream);
+/* sklearn k_means(X, k, n_init="auto") of the rows of X [N, >= k] fp64 (row stride ld) -> labels [N] int32, inertia (device
+ * double).  k-means++ consumes uniforms [1 + (k-1)(2 + int(log k))] fp64 in [0, 1) in numpy's draw order; 1 <= k <= min(N, 32).
+ * ws: ppv_kmeans_workspace_bytes(N, k) bytes, 256-byte aligned. */
+size_t ppv_kmeans_workspace_bytes(int N, int k);
+int ppv_kmeans(const double* X, int ld, int N, int k, const double* uniforms, int n_uniforms, int max_iter, int32_t* labels, double* inertia,
+               void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Cosine classifier + AAMLoss.  Replaces ppvector/models/fc.py:41-53 (Cosine, num_blocks=0) and
  * ppvector/loss/aamloss.py:28-46 (mean softmax-CE over scale * margin-adjusted cosines).
  * W is [D,S] (Paddle layout, fc.py:31).  logits [B,S] receives the plain cosines

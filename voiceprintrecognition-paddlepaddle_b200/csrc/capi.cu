@@ -267,6 +267,31 @@ int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* be
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- speaker diarization
+int ppv_cluster_prune(float* affinity, int N, double pval, void* stream) {
+    PPV_GUARD_BEGIN
+    return cluster_prune(affinity, N, pval, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+int ppv_cluster_laplacian(const float* pruned, int N, double* L, void* stream) {
+    PPV_GUARD_BEGIN
+    return cluster_laplacian(pruned, N, L, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+size_t ppv_sym_eig_workspace_bytes(int N, int m) { return sym_eig_workspace_bytes(N, m); }
+int ppv_sym_eig_smallest(double* L, int N, int m, double* evals, double* evecs, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    return sym_eig_smallest(L, N, m, evals, evecs, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+size_t ppv_kmeans_workspace_bytes(int N, int k) { return kmeans_workspace_bytes(N, k); }
+int ppv_kmeans(const double* X, int ld, int N, int k, const double* uniforms, int n_uniforms, int max_iter, int32_t* labels, double* inertia,
+               void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    return kmeans(X, ld, N, k, uniforms, n_uniforms, max_iter, labels, inertia, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+
 int ppv_model_profile(ppv_model_t* h, int enable) {
     PPV_REQUIRE(ecapa_of(h), "ppv_model_profile: ECAPA-TDNN model required");
     return ecapa_profile(h->m, enable);

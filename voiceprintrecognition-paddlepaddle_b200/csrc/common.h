@@ -407,6 +407,15 @@ int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_la
                double p_target, double c_miss, double c_fa, double* out, void* ws, size_t ws_bytes, cudaStream_t st);
 int row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* best, cudaStream_t st);
 
+// ---- cluster.cu -------------------------------------------------------------------------------------
+int cluster_prune(float* A, int N, double pval, cudaStream_t st);
+int cluster_laplacian(const float* P, int N, double* L, cudaStream_t st);
+size_t sym_eig_workspace_bytes(int N, int m);
+int sym_eig_smallest(double* L, int N, int m, double* evals, double* evecs, void* ws, size_t ws_bytes, cudaStream_t st);
+size_t kmeans_workspace_bytes(int N, int k);
+int kmeans(const double* X, int ld, int N, int k, const double* uniforms, int n_uniforms, int max_iter, int32_t* labels, double* inertia, void* ws,
+           size_t ws_bytes, cudaStream_t st);
+
 int device_sm_count();
 
 }  // namespace ppv

@@ -7,8 +7,8 @@ would run past the segment end is moved back so that it ends at the segment end 
 window gives one zero-padded window.  All windows have the same length, so the whole recording becomes ONE [n_chunks, chunk_len] batch for the
 embedding path -- no per-chunk padding ratios, no ragged batch.
 
-Voice-activity detection (yeaudio's silero VAD) and the spectral clustering / post-processing after the embeddings are outside the hot path and
-are not part of this package: callers pass the VAD segments (or none: the whole recording is one segment).
+Voice-activity detection (yeaudio's silero VAD) is not part of this package: callers pass the VAD segments (or none: the whole recording is
+one segment).  The clustering and post-processing after the embeddings are infer_utils/speaker_diarization.py.
 """
 import numpy as np
 

@@ -6,10 +6,14 @@ Same constructor arguments and the same ``predict`` / ``predict_batch`` / ``cont
     embedding is ONE library call (``ppv_model_forward_wav``); the reference featurises per utterance in a Python
     loop and runs the model in chunks of 32 (predict.py:262-267);
   * cosine scoring runs on the GPU (``ppvector.metric.cosine``);
-  * ``use_gpu=False`` raises: this build has no CPU path.
-Not carried over (SURVEY.md §2 rows 12, 21: out of scope): the enrolment DB, recognition and diarization.
+  * ``use_gpu=False`` raises: this build has no CPU path;
+  * ``speaker_diarization`` clusters on the GPU (infer_utils/speaker_diarization.py) and takes the voice-activity segments as an
+    argument (the reference's silero VAD is not part of this build).
+The enrolment database is read (``audio_db_path``: ``recognition``, ``get_users``, ``search_audio_db``); ``register`` and
+``remove_user``, which write into it, are not carried over.
 """
 import os
+import pickle
 from io import BufferedReader
 
 import numpy as np
@@ -53,8 +57,80 @@ class PPVectorPredictor:
         self.predictor = backbone.eval().to(self.device)
         self._pinned = None
         self._pinned_out = None
+        self.audio_db_path = audio_db_path
+        self.users_name, self.users_audio_path, self.users_name_mean = [], [], []
+        self.audio_feature, self.audio_feature_mean = None, None
         if audio_db_path is not None:
-            logger.warning('audio_db_path: the enrolment database is out of scope of the CUDA hot path (ignored)')
+            self.audio_indexes_path = os.path.join(audio_db_path, 'audio_indexes.bin')
+            self._load_audio_db(audio_db_path)
+
+    # ---- enrolment database: predict.py:89-187 (read side) ----------------------------------------------------
+    def _load_audio_indexes(self):
+        """predict.py:89-102: the pickled index of embedded enrolment files; entries whose file is gone are dropped."""
+        if not os.path.exists(self.audio_indexes_path):
+            return
+        with open(self.audio_indexes_path, 'rb') as f:
+            indexes = pickle.load(f)
+        for name, feature, path in zip(indexes['users_name'], indexes['faces_feature'], indexes['users_image_path']):
+            if not os.path.exists(path):
+                continue
+            self.users_name.append(name)
+            self.users_audio_path.append(path)
+            self.audio_feature = feature[None] if self.audio_feature is None else np.vstack((self.audio_feature, feature))
+
+    def _write_index(self):
+        """predict.py:105-109 (same keys, same pickle layout)."""
+        with open(self.audio_indexes_path, 'wb') as f:
+            pickle.dump({'users_name': self.users_name, 'faces_feature': self.audio_feature, 'users_image_path': self.users_audio_path}, f)
+
+    def _load_audio_db(self, audio_db_path):
+        """predict.py:112-165: embed <db>/<user>/* files not yet in the index (predict_batch, eval batch size), rewrite the index,
+        keep one mean embedding per user (on the device as well, for retrieval)."""
+        self._load_audio_indexes()
+        os.makedirs(audio_db_path, exist_ok=True)
+        audios_path = []
+        for name in os.listdir(audio_db_path):
+            audio_dir = os.path.join(audio_db_path, name)
+            if os.path.isdir(audio_dir):
+                audios_path.extend(os.path.join(audio_dir, f).replace('\\', '/') for f in os.listdir(audio_dir))
+        if len(audios_path) == 0:
+            return
+        new = [p for p in audios_path if p not in self.users_audio_path]
+        bs = self.configs.dataset_conf.eval_conf.batch_size
+        for i in range(0, len(new), bs):
+            features = self.predict_batch(new[i:i + bs])
+            self.audio_feature = features if self.audio_feature is None else np.vstack((self.audio_feature, features))
+        for p in new:
+            self.users_name.append(os.path.basename(os.path.dirname(p)))
+            self.users_audio_path.append(p)
+        assert len(self.audio_feature) == len(self.users_name) == len(self.users_audio_path), '加载的数量对不上！'
+        self._write_index()
+        for name in set(self.users_name):
+            idx = [i for i, v in enumerate(self.users_name) if v == name]
+            feature = self.audio_feature[idx].mean(axis=0)
+            self.audio_feature_mean = feature[None] if self.audio_feature_mean is None else np.vstack((self.audio_feature_mean, feature))
+            self.users_name_mean.append(name)
+        self._audio_feature_mean_dev = torch.from_numpy(np.ascontiguousarray(self.audio_feature_mean, dtype=np.float32)).to(self.device)
+        logger.info(f'声纹库数据加载完成，一共有{len(self.audio_feature_mean)}个用户，分别是：{self.users_name_mean}')
+
+    def _retrieval(self, np_feature):
+        """predict.py:173-187: [name, similarity] of the best-matching user per query, [None, None] under the threshold (GPU cosine
+        + row arg-max, ppvector.metric.cosine.retrieval)."""
+        from ppvector.metric.cosine import retrieval
+        feats = np.asarray(np_feature, dtype=np.float32)
+        feats = feats / np.linalg.norm(feats, axis=1, keepdims=True)
+        return retrieval(feats, self._audio_feature_mean_dev, self.threshold, names=self.users_name_mean)
+
+    def recognition(self, audio_data, threshold=None, sample_rate=16000):
+        """predict.py:324-335 -> [name, similarity], or [None, None] under the threshold."""
+        if threshold:
+            self.threshold = threshold
+        feature = self.predict(audio_data, sample_rate=sample_rate)
+        return self._retrieval(feature[None])[0]
+
+    def get_users(self):
+        """predict.py:337-342"""
+        return self.users_name
 
     # ---- audio loading: predict.py:189-216 ----------------------------------------------------------------
     def _load_audio(self, audio_data, sample_rate=16000):
@@ -276,11 +352,36 @@ class PPVectorPredictor:
         window goes through the embedding path as ONE equal-length batch.  Returns (times [n, 2] seconds, embeddings [n, embd]).  VAD and the
         clustering after it are outside the hot path: pass ``vad_segments`` from your VAD; None takes the whole recording as one segment."""
         from ppvector.infer_utils.chunking import fan_out_embeddings
+        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments)
+        return fan_out_embeddings(segs, self.extract_embeddings, seg_duration, seg_shift, sr, batch_size)
+
+    def _voiced_segments(self, audio_data, sample_rate, vad_segments):
+        """-> (sample rate, [(start_s, end_s, samples), ...]) of the given voice-activity segments, or of the whole recording."""
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
         sr, x = seg.sample_rate, seg.samples
         spans = [(0.0, len(x) / sr)] if vad_segments is None else [(round(float(a), 3), round(float(b), 3)) for a, b in vad_segments]
-        segs = [(a, b, x[int(a * sr):int(b * sr)]) for a, b in spans]
-        return fan_out_embeddings(segs, self.extract_embeddings, seg_duration, seg_shift, sr, batch_size)
+        return sr, [(a, b, x[int(a * sr):int(b * sr)]) for a, b in spans]
+
+    def speaker_diarization(self, audio_data, sample_rate=16000, speaker_num=None, search_audio_db=False, vad_segments=None):
+        """reference: predict.py:366-396 -> [{'speaker', 'start', 'end'}, ...].  The recording (or the given voice-activity segments
+        [(start_s, end_s), ...]; None = the whole recording) is cut into 1.5 s windows every 0.75 s and embedded as one batch
+        (diarization_embeddings); the windows are clustered on the GPU (infer_utils/speaker_diarization.py: spectral clustering,
+        ``speaker_num`` fixes the speaker count) and the segments post-processed as in the reference.  The voiced speech must total
+        more than 5 s.  search_audio_db=True names each speaker from the enrolment database (``audio_db_path``)."""
+        from ppvector.infer_utils.chunking import fan_out_embeddings
+        from ppvector.infer_utils.speaker_diarization import SpeakerDiarization
+        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments)
+        sd = SpeakerDiarization(sample_rate=sr)
+        sd._check_audio_list([list(s) for s in segs])
+        times, features = fan_out_embeddings(segs, self.extract_embeddings, sd.seg_duration, sd.seg_shift, sr, 256)
+        labels, spk_center_embeddings = sd.clustering(features, speaker_num=speaker_num)
+        outputs = sd.postprocess([list(t) for t in times.tolist()], labels)
+        if search_audio_db:
+            assert getattr(self, 'audio_feature', None) is not None, "数据库中没有音频数据，请先指定说话人特征数据库或者注册说话人"
+            names = self._retrieval(spk_center_embeddings)  # indexed with the post-merge labels, as the reference does
+            outputs = [{'speaker': names[o['speaker']][0] if names[o['speaker']][0] else f"陌生人{o['speaker']}",
+                        'start': o['start'], 'end': o['end']} for o in outputs]
+        return outputs
 
     def contrast(self, audio_data1, audio_data2):
         """reference: predict.py:271-283 -> cosine similarity of the two embeddings"""
