@@ -402,6 +402,16 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
                     int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
                     size_t ws_bytes, void* stream);
 
+/* Test hook for the fused attentive-statistics pooling kernel (not a reference entry point): the kernel the ECAPA-TDNN and ResNetSE
+ * plans run, on operands given in fp32 and split into planes here.  W [C,K] (attention conv weight), att [B*Tp,K] and x [B*Tp,C] in
+ * the padded time layout (row b*Tp + P + t), bn_scale / bn_shift [2C], nvalid [B] int32 (may be NULL: T valid frames).
+ * C % 128 == 0, K in {64, 128}.  max_ctas: the grid's CTA count cap (0: every SM).  The 64 plane rows behind att and x hold a large finite value.  out_raw [B,2C] fp32 (mean | std), out [B,2C]: the asp_bn'd split
+ * planes decoded as hi + lo.  ws >= ppv_asp_fused_test_workspace_bytes. */
+size_t ppv_asp_fused_test_workspace_bytes(int B, int Tp, int C, int K);
+int ppv_asp_fused_test(const float* W, const float* att, const float* x, const float* bn_scale, const float* bn_shift,
+                       const int* nvalid, int B, int T, int P, int Tp, int C, int K, int precision, int max_ctas,
+                       float* out_raw, float* out, void* ws, size_t ws_bytes, void* stream);
+
 /* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N)
  * bytes + 4*(3 + M/306)*N rounded up to 256.  planes_out: 0 ReLU to fp32, 1 ReLU to planes, 2 bias + ReLU + BN to planes over the
  * padded time layout (Tp = 306, P = 4), 3 the same + per-utterance bias + tanh (ASP attention TDNN); 2 and 3 need M % 306 == 0. */

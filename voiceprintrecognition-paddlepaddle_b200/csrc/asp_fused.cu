@@ -10,8 +10,10 @@
 // (wgmma fragment, ptx.cuh).  The softmax over time and the weighted moments are per-thread running sums over the thread's
 // frames, merged across the four threads that share a channel at the end of the utterance -- no atomics, deterministic.
 //   * online softmax (running max, rescale once per tile)
-//   * moments about the channel's global mean g (from asp_global): S0 = sum e, S1 = sum e (x-g), S2 = sum e (x-g)^2,
-//     mean = g + S1/S0, var = S2/S0 - (S1/S0)^2   (shifted one-pass; the reference is two-pass)
+//   * moments merged, not subtracted: a thread keeps S0 = sum e, the weighted mean mu and M2 = sum e (x - mu)^2; each tile's
+//     own (w, mean, M2) is computed two-pass over the thread's frames and merged by Chan's formula, and so are the four
+//     threads of a channel.  A one-pass var = S2/S0 - (S1/S0)^2 cancels when attention sits on a few frames far from the
+//     shift; this stays at the grade of the reference's two-pass variance (and of asp_pool_kernel, the training forward).
 //   * the conv bias is constant over time and cancels in the softmax: it is not even loaded.
 // Work item = (utterance b, 128-channel slab); a CTA keeps the weight slab in smem for the item and streams the
 // utterance in 64-frame tiles through a 2-deep TMA ring.  A ring stage carries BOTH the attention activations (the
@@ -138,13 +140,11 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
             }
             const int nitem = item + gridDim.x;
             const bool last_of_slab = (nitem >= items) || (nitem % slabs != slab);
-            float gm[2], m[2], S0[2], S1[2], S2[2];
+            float m[2], S0[2], mu[2], M2[2];  // running max, sum of weights, weighted mean, weighted sum of squared deviations
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
-                const int64_t goff = int64_t(b) * p.gstat.ld + slab * 128 + cl0 + 8 * rr;
-                gm[rr] = __bfloat162float(p.gstat.hi()[goff]) + __bfloat162float(p.gstat.lo()[goff]);
                 m[rr] = -INFINITY;
-                S0[rr] = S1[rr] = S2[rr] = 0.f;
+                S0[rr] = mu[rr] = M2[rr] = 0.f;
             }
             const int Tb = p.nvalid ? max(1, min(p.T, p.nvalid[b])) : p.T;  // masked frames: softmax weight exactly 0
             for (int ft = 0; ft < ntiles; ++ft) {
@@ -184,12 +184,16 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
                     if (cm > m[rr]) {
                         const float r = exp2f((m[rr] - cm) * LOG2E);  // exp(-inf) = 0 on the first frames
                         S0[rr] *= r;
-                        S1[rr] *= r;
-                        S2[rr] *= r;
+                        M2[rr] *= r;
                         m[rr] = cm;
                     }
                     const float ms = m[rr] * LOG2E;
                     const int cl = cl0 + 8 * rr;
+                    // the tile's own weight wt, mean mt and M2 over this thread's <= 16 frames, two-pass: the weights overwrite acc and x
+                    // stays in xr.  The mean is taken about the thread's first frame x0, so a constant channel's comes out exact.
+                    const float x0 = __bfloat162float(xs_hi[2 * (l & 3) * 128 + cl]) + __bfloat162float(xs_lo[2 * (l & 3) * 128 + cl]);
+                    float xr[AF_NT / 8][2];
+                    float wt = 0.f, sx = 0.f;
 #pragma unroll
                     for (int i = 0; i < AF_NT / 8; ++i)
 #pragma unroll
@@ -197,15 +201,30 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
                             const int fl = 8 * i + 2 * (l & 3) + e;
                             if (f0 + fl < Tb) {
                                 const int o = fl * 128 + cl;
-                                const float xv = __bfloat162float(xs_hi[o]) + __bfloat162float(xs_lo[o]);
+                                xr[i][e] = __bfloat162float(xs_hi[o]) + __bfloat162float(xs_lo[o]);
                                 const float ev = exp2f(fmaf(acc[4 * i + 2 * rr + e], LOG2E, -ms));
-                                const float d = xv - gm[rr];
-                                const float ed = ev * d;
-                                S0[rr] += ev;
-                                S1[rr] += ed;
-                                S2[rr] = fmaf(ed, d, S2[rr]);
+                                acc[4 * i + 2 * rr + e] = ev;
+                                wt += ev;
+                                sx = fmaf(ev, xr[i][e] - x0, sx);
                             }
                         }
+                    if (wt > 0.f) {  // the thread's first frame is its earliest: wt = 0 iff none of its frames is valid
+                        const float mt = x0 + sx / wt;
+                        float m2 = 0.f;
+#pragma unroll
+                        for (int i = 0; i < AF_NT / 8; ++i)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e)
+                                if (f0 + 8 * i + 2 * (l & 3) + e < Tb) {
+                                    const float d = xr[i][e] - mt;
+                                    m2 = fmaf(acc[4 * i + 2 * rr + e] * d, d, m2);
+                                }
+                        // merge (S0, mu, M2) with (wt, mt, m2), Chan et al.: M2 += m2 + delta^2 S0 wt / (S0 + wt)
+                        const float n = S0[rr] + wt, f = wt / n, dl = mt - mu[rr];
+                        mu[rr] = fmaf(dl, f, mu[rr]);
+                        M2[rr] += m2 + dl * dl * (S0[rr] * f);
+                        S0[rr] = n;
+                    }
                 }
                 mbar_arrive(b_empty(stage));  // done with the att and x tiles of this stage
                 if (++stage == AF_STAGES) {
@@ -219,12 +238,14 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
 #pragma unroll
                 for (int off = 1; off <= 2; off <<= 1) {
                     const float om = __shfl_xor_sync(0xffffffffu, m[rr], off), o0 = __shfl_xor_sync(0xffffffffu, S0[rr], off),
-                                o1 = __shfl_xor_sync(0xffffffffu, S1[rr], off), o2 = __shfl_xor_sync(0xffffffffu, S2[rr], off);
+                                omu = __shfl_xor_sync(0xffffffffu, mu[rr], off), o2 = __shfl_xor_sync(0xffffffffu, M2[rr], off);
                     const float mm = fmaxf(m[rr], om);
                     const float ra = S0[rr] > 0.f ? exp2f((m[rr] - mm) * LOG2E) : 0.f, rb = o0 > 0.f ? exp2f((om - mm) * LOG2E) : 0.f;
-                    S0[rr] = S0[rr] * ra + o0 * rb;
-                    S1[rr] = S1[rr] * ra + o1 * rb;
-                    S2[rr] = S2[rr] * ra + o2 * rb;
+                    const float wa = S0[rr] * ra, wb = o0 * rb, n = wa + wb;
+                    const float f = n > 0.f ? wb / n : 0.f, dl = omu - mu[rr];
+                    mu[rr] = fmaf(dl, f, mu[rr]);
+                    M2[rr] = M2[rr] * ra + o2 * rb + dl * dl * (wa * f);
+                    S0[rr] = n;
                     m[rr] = mm;
                 }
             }
@@ -233,10 +254,8 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int c = slab * 128 + cl0 + 8 * rr;
-                const float inv = 1.f / S0[rr];
-                const float dm = S1[rr] * inv;
-                const float mean = gm[rr] + dm;
-                const float sd = sqrtf(fmaxf(S2[rr] * inv - dm * dm, p.eps));
+                const float mean = mu[rr];
+                const float sd = sqrtf(fmaxf(M2[rr] / S0[rr], p.eps));
                 if (p.out_raw) {
                     p.out_raw[int64_t(b) * 2 * C + c] = mean;
                     p.out_raw[int64_t(b) * 2 * C + C + c] = sd;
@@ -253,7 +272,7 @@ __global__ void __launch_bounds__(384, 1) asp_fused_kernel(const __grid_constant
     }
 }
 
-int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const Planes& x, const Planes& gstat, const float* bn_scale,
+int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const Planes& x, const float* bn_scale,
                     const float* bn_shift, const Planes& out, float* out_raw, int B, int T, int P, int Tp, int C, int K, float eps) {
     PPV_REQUIRE(C % 128 == 0 && K % 64 == 0 && K <= 128, "asp_fused: C % 128 == 0 and K in {64,128} required");
     memset(p, 0, sizeof(*p));
@@ -265,7 +284,6 @@ int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const
     rc = encode_planes_map_ex(&p->mapX, x, 128, AF_NT, 0);
     if (rc) return rc;
     p->x = x;
-    p->gstat = gstat;
     p->bn_scale = bn_scale;
     p->bn_shift = bn_shift;
     p->out = out;

@@ -625,6 +625,56 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- fused attentive-statistics pooling test hook
+// Workspace: W planes [2][C][K], att planes [2][B Tp + 64][K], x planes [2][B Tp + 64][C], out planes [2][B][2C].  The tensor
+// maps of att and x end at row B Tp; the 64 rows behind hold 0x4646 (12672 in bf16) in both planes.
+static size_t asp_test_sizes(int B, int Tp, int C, int K, size_t* off) {
+    const size_t rows = size_t(B) * Tp + 64;
+    const size_t sz[4] = {size_t(C) * K, rows * K, rows * C, size_t(B) * 2 * C};
+    size_t o = 0;
+    for (int i = 0; i < 4; ++i) {
+        off[i] = o;
+        o += au(2 * sz[i] * sizeof(__nv_bfloat16), 256);
+    }
+    return o;
+}
+size_t ppv_asp_fused_test_workspace_bytes(int B, int Tp, int C, int K) {
+    size_t off[4];
+    return asp_test_sizes(B, Tp, C, K, off);
+}
+int ppv_asp_fused_test(const float* W, const float* att, const float* x, const float* bn_scale, const float* bn_shift,
+                       const int* nvalid, int B, int T, int P, int Tp, int C, int K, int precision, int max_ctas, float* out_raw,
+                       float* out, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(W && att && x && bn_scale && bn_shift && out_raw && out && ws, "ppv_asp_fused_test: null argument");
+    PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P && max_ctas >= 0, "ppv_asp_fused_test: bad shape");
+    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "ppv_asp_fused_test: bad precision");
+    size_t off[4];
+    PPV_REQUIRE(ws_bytes >= asp_test_sizes(B, Tp, C, K, off), "ppv_asp_fused_test: workspace too small");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint8_t* w8 = static_cast<uint8_t*>(ws);
+    const int64_t rows = int64_t(B) * Tp;
+    auto planes = [&](int i, int64_t nrows, int ld, int64_t alloc_rows) {
+        return Planes{reinterpret_cast<__nv_bfloat16*>(w8 + off[i]), nrows, ld, alloc_rows * ld};
+    };
+    const Planes pw = planes(0, C, K, C), pa = planes(1, rows, K, rows + 64), px = planes(2, rows, C, rows + 64),
+                 po = planes(3, B, 2 * C, B);
+    PPV_CUDA_OK(cudaMemsetAsync(w8 + off[1], 0x46, off[3] - off[1], st));
+    if ((rc = launch_f32_to_planes(W, C, K, pw, st)) || (rc = launch_f32_to_planes(att, rows, K, pa, st)) ||
+        (rc = launch_f32_to_planes(x, rows, C, px, st)))
+        return rc;
+    AspFusedParams ap;
+    rc = asp_fused_build(&ap, pw, pa, px, bn_scale, bn_shift, po, out_raw, B, T, P, Tp, C, K, 1e-12f);
+    if (rc) return rc;
+    ap.nvalid = nvalid;
+    rc = asp_fused_launch(ap, precision, max_ctas > 0 ? max_ctas : device_sm_count(), st);
+    if (rc) return rc;
+    return launch_planes_to_f32(po, 0, 2 * C, B, 1, 0, 1, out, st);
+    PPV_GUARD_END
+}
+
 // Kernel-only timing of the gather-GEMM (tools/gemm_bench.py): operands are converted once, the kernel is launched
 // `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  planes_out selects the epilogue:
 //   0  ReLU, fp32 [M,N];   1  ReLU, split-bf16 planes (the layout every model layer writes);

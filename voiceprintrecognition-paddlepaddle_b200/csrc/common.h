@@ -282,7 +282,6 @@ struct AspFusedParams {
     CUtensorMap mapAtt;  // planes [2][rows][K] box {64, 64, 1}
     CUtensorMap mapX;    // planes [2][rows][C] box {128, 64, 1}, no swizzle
     Planes x;            // MFA output, padded time layout, ld = C
-    Planes gstat;        // [B, 2C] (global mean | std): mean used as the shift
     const float* bn_scale;  // asp_bn folded, [2C]
     const float* bn_shift;
     Planes out;          // [B, 2C] (mean | std) after asp_bn -> fc GEMM operand
@@ -292,7 +291,7 @@ struct AspFusedParams {
     const int* nvalid;  // optional [B]: frames t >= nvalid[b] get attention weight 0 (`lengths`, pooling.py:112-115); set per launch
 };
 
-int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const Planes& x, const Planes& gstat, const float* bn_scale,
+int asp_fused_build(AspFusedParams* p, const Planes& W, const Planes& att, const Planes& x, const float* bn_scale,
                     const float* bn_shift, const Planes& out, float* out_raw, int B, int T, int P, int Tp, int C, int K, float eps);
 int asp_fused_launch(const AspFusedParams& p, int precision, int num_sms, cudaStream_t st);
 

@@ -327,7 +327,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     const int pooling = cfg.pooling;
     if (pooling == PPV_POOL_TAP || pooling == PPV_POOL_TSP)  // mean (TAP) or mean | unbiased variance (TSP) over time, straight into the fc operand
         steps.push_back(colstats_step(buf.mfa, C3, B, T, P, Tp, pooling == PPV_POOL_TAP ? 0 : 3, 0.f, buf.pool));
-    else  // global mean | std: ASP's context statistics and the fused pooling's shift
+    else  // global mean | std: ASP's context statistics
         steps.push_back(colstats_step(buf.mfa, C3, B, T, P, Tp, 1, 1e-12f, buf.gstat, 0.f, true));
     if (pooling == PPV_POOL_ASP && cfg.global_context) {  // fold: [B, 2*C3] . W[:, C3:3*C3]^T -> per-utterance bias [B, att]  (no conv bias here)
         rc = plan_row_linear(fold, GemmSource{buf.gstat, 0, 2 * C3, 0}, B, f32_out(buf.fold_out, att));
@@ -348,7 +348,7 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         {  // attention logits (transposed GEMM) + softmax over time + weighted mean / std + asp_bn, fused
             PlanStep s;
             s.kind = PlanStep::ASP_FUSED;
-            rc = asp_fused_build(&s.ap, att2.W, buf.att, buf.mfa, buf.gstat, aspbn_scale, aspbn_shift, buf.pool, buf.pooled_raw, B, T, P, Tp, C3,
+            rc = asp_fused_build(&s.ap, att2.W, buf.att, buf.mfa, aspbn_scale, aspbn_shift, buf.pool, buf.pooled_raw, B, T, P, Tp, C3,
                                  att, 1e-12f);
             if (rc) return rc;
             steps.push_back(s);

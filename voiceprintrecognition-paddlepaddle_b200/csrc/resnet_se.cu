@@ -331,7 +331,7 @@ int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
     {
         PlanStep s;
         s.kind = PlanStep::ASP_FUSED;
-        rc = asp_fused_build(&s.ap, m->att2.W, rb.attp, rb.flat, rb.gstat, m->bn2_scale, m->bn2_shift, rb.pooled, rb.pooled_raw, B, Tf, 0, Tf, cat,
+        rc = asp_fused_build(&s.ap, m->att2.W, rb.attp, rb.flat, m->bn2_scale, m->bn2_shift, rb.pooled, rb.pooled_raw, B, Tf, 0, Tf, cat,
                              m->att, 1e-12f);
         if (rc) return rc;
         m->steps.push_back(s);
