@@ -412,6 +412,51 @@ int ppv_asp_fused_test(const float* W, const float* att, const float* x, const f
                        const int* nvalid, int B, int T, int P, int Tp, int C, int K, int precision, int max_ctas,
                        float* out_raw, float* out, void* ws, size_t ws_bytes, void* stream);
 
+/* Test hook for the column-statistics kernel (not a reference entry point): launch_colstats, as the model plans call it, over x
+ * [B*Tp, ld] fp32 split into planes here (rows b*Tp + P + t, t < T, of columns [col0, col0 + C); C % 64 == 0, col0 % 8 == 0,
+ * ld % 8 == 0).  mode 0: mean; 1: mean | sqrt(max(var, eps)); 2: mean | sqrt(var_unbiased + eps); 3: mean | var_unbiased.
+ * inv_count > 0: mean = sum * inv_count.  nvalid [B] int32 (may be NULL): frames pooled per utterance, clamped to [1, T].
+ * out [B, C] (mode 0) or [B, 2C]: the output planes decoded as hi + lo; out_f32 [B, C] (mode 0 only, may be NULL otherwise).
+ * ws >= ppv_colstats_test_workspace_bytes. */
+size_t ppv_colstats_test_workspace_bytes(int B, int Tp, int ld, int C);
+int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int col0, int C, int mode, float eps, float inv_count,
+                      const int* nvalid, float* out, float* out_f32, void* ws, size_t ws_bytes, void* stream);
+
+/* Test hook for CAM++'s context mask (not a reference entry point): the dense layers' context kernel over h [B*Tp, 128] fp32 split
+ * into planes here (frames t < T at rows b*Tp + P + t), with the MLP w1 [64,128], b1 [64], w2 [32,64], b2 [32] in the reference
+ * layout, transposed on the host as the model prepares them.  out [B * ceil(T/100), 32] fp32.  T > 6400 (more than 64 segments)
+ * is an error.  ws >= ppv_campplus_context_test_workspace_bytes.  Synchronises `stream` while it prepares the weights. */
+size_t ppv_campplus_context_test_workspace_bytes(int B, int Tp);
+int ppv_campplus_context_test(const float* h, int B, int T, int P, int Tp, const float* w1, const float* b1, const float* w2,
+                              const float* b2, float* out, void* ws, size_t ws_bytes, void* stream);
+
+/* Test hook for the gather-GEMM on the padded time layout (not a reference entry point): one case as a model plans it.
+ * x[i] [rows[i], ld[i]] fp32 (every row given, padding rows included) are split into planes here; source j reads columns
+ * [src_col0[j], src_col0[j] + src_ncols[j]) of x[src_input[j]] at row offset src_row_off[j].  W [N, sum ncols] fp32 in k-step order.
+ * Epilogue: + bias, * seg_scale[(b * nseg + t / seg_len) * N + n] (may be NULL), ReLU, BN affine (may be NULL) on the T valid rows of
+ * every Tp = T + 2P (Tp 0: every row valid); halo: also the reflect mirror rows; zero_invalid: zeros on the other rows.  out_f32 0:
+ * planes out [2][out_rows][out_ld] bf16, 1: fp32 out [out_rows][out_ld], written from column out_col0; the hook does not clear it.
+ * block_n 0: the plans' choice; block_k 0: gemm_build's.  ws >= ppv_gemm_test_taps_workspace_bytes. */
+#define PPV_TAPS_MAX_INPUTS 4
+#define PPV_TAPS_MAX_SOURCES 16
+typedef struct {
+    const float* x[PPV_TAPS_MAX_INPUTS];
+    int64_t rows[PPV_TAPS_MAX_INPUTS];
+    int ld[PPV_TAPS_MAX_INPUTS];
+    int ninputs, nsrc;
+    int src_input[PPV_TAPS_MAX_SOURCES], src_col0[PPV_TAPS_MAX_SOURCES], src_ncols[PPV_TAPS_MAX_SOURCES],
+        src_row_off[PPV_TAPS_MAX_SOURCES];
+    const float* W;
+    const float *bias, *bn_scale, *bn_shift, *seg_scale;
+    int M, N, relu, seg_len, nseg, Tp, P, T, halo, zero_invalid;
+    int out_f32;
+    void* out;
+    int64_t out_rows;
+    int out_ld, out_col0, block_n, block_k, precision;
+} ppv_gemm_taps_case;
+size_t ppv_gemm_test_taps_workspace_bytes(const ppv_gemm_taps_case* c);
+int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, void* stream);
+
 /* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N)
  * bytes + 4*(3 + M/306)*N rounded up to 256.  planes_out: 0 ReLU to fp32, 1 ReLU to planes, 2 bias + ReLU + BN to planes over the
  * padded time layout (Tp = 306, P = 4), 3 the same + per-utterance bias + tanh (ASP attention TDNN); 2 and 3 need M % 306 == 0. */

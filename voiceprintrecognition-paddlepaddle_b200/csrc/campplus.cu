@@ -57,7 +57,7 @@ struct TransitW {
 // CAM++'s own plan steps (PlanStep::MODEL):
 //   FLATTEN_PAIRS  x on grid g -> frame-pair matrix `out` (C channels, Tp / P time layout)
 //   BN_RELU        out = relu(x * vec[0] + vec[1]) over C columns of `rows` rows
-//   CONTEXT        x [B * Tp, 128] -> context mask out_f32 [B * n, 32] (MLP vec[0..3]), T frames from row P of each utterance
+//   CONTEXT        x [B * Tp, 128] -> context mask out_f32 [B * ceil(T / 100), 32] (MLP vec[0..3]), T frames from row P of each utterance
 enum CpKind { CP_FLATTEN_PAIRS, CP_BN_RELU, CP_CONTEXT };
 
 // ------------------------------------------------------------------------------------------------ kernels
@@ -190,7 +190,32 @@ __global__ void __launch_bounds__(256) cp_flatten_pairs_kernel(Planes in, int B,
     }
 }
 
+int cp_segments(int T2, int* nseg) {
+    *nseg = (T2 + CP_SEG - 1) / CP_SEG;
+    PPV_REQUIRE(*nseg <= CP_MAX_SEG, "campplus: utterance too long (more than 64 context segments of 100 frames)");
+    return PPV_OK;
+}
+
 }  // namespace
+
+void campplus_context_weights(const float* w1, const float* w2, std::vector<float>* w1t, std::vector<float>* w2t) {
+    constexpr int BC = 128, H = 64, G = 32;
+    w1t->assign(size_t(BC) * H, 0.f);
+    w2t->assign(size_t(H) * G, 0.f);
+    for (int j = 0; j < H; ++j)
+        for (int c = 0; c < BC; ++c) (*w1t)[size_t(c) * H + j] = w1[size_t(j) * BC + c];
+    for (int n = 0; n < G; ++n)
+        for (int k = 0; k < H; ++k) (*w2t)[size_t(k) * G + n] = w2[size_t(n) * H + k];
+}
+
+int campplus_context_launch(const Planes& h, int B, int T, int P, int Tp, const float* w1t, const float* b1, const float* w2t,
+                            const float* b2, float* out, cudaStream_t st) {
+    int nseg = 0;
+    int rc = cp_segments(T, &nseg);
+    if (rc) return rc;
+    PPV_PDL_OK(launch_pdl(cp_context_kernel, dim3(B), dim3(256), 0, st, h, T, P, Tp, nseg, w1t, b1, w2t, b2, out), "cp_context_kernel");
+    return PPV_OK;
+}
 
 struct CamppModel : PlanModel {
     ppv_campplus_cfg cfg;
@@ -288,11 +313,8 @@ bool CamppModel::prepare_weights(ArenaBuilder& ab) {
                 ok = false;
                 break;
             }
-            std::vector<float> w1t(size_t(BC) * (BC / 2)), w2t(size_t(BC / 2) * G);
-            for (int j = 0; j < BC / 2; ++j)
-                for (int c = 0; c < BC; ++c) w1t[size_t(c) * (BC / 2) + j] = w1->v[size_t(j) * BC + c];
-            for (int n = 0; n < G; ++n)
-                for (int k = 0; k < BC / 2; ++k) w2t[size_t(k) * G + n] = w2->v[size_t(n) * (BC / 2) + k];
+            std::vector<float> w1t, w2t;
+            campplus_context_weights(w1->v.data(), w2->v.data(), &w1t, &w2t);
             ab.put_f32(&lw.w1t, w1t);
             ab.put_f32(&lw.b1, b1->v);
             ab.put_f32(&lw.w2t, w2t);
@@ -366,12 +388,14 @@ size_t CamppModel::workspace_bytes(int B, int T) const {
 int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {
     CamppModel* const m = this;
     PPV_REQUIRE(T >= 3, "campplus: too few frames (the statistics pooling needs at least two frames after the stride-2 TDNN)");
-    const int T2 = (T - 1) / 2 + 1, Tp = T2 + 2 * CP_P, nseg = (T2 + CP_SEG - 1) / CP_SEG;
-    PPV_REQUIRE(nseg <= CP_MAX_SEG, "campplus: utterance too long (more than 64 context segments of 100 frames)");
+    const int T2 = (T - 1) / 2 + 1, Tp = T2 + 2 * CP_P;
+    int nseg = 0;
+    int rc = cp_segments(T2, &nseg);
+    if (rc) return rc;
     PPV_REQUIRE(T + 3 < 32768, "campplus: utterance too long for 16-bit tap offsets");
     image_pyramid(m->geo, 4, m->cfg.input_size, T, false);
     PPV_REQUIRE(m->geo[0].rows(B) < (int64_t(1) << 31), "campplus: batch too large for 32-bit row indices");
-    int rc = claim_workspace(B, T, ws, ws_bytes, st);
+    rc = claim_workspace(B, T, ws, ws_bytes, st);
     if (rc) return rc;
     WsCarver cv;
     cv.base = static_cast<uint8_t*>(ws);
@@ -456,7 +480,6 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             c.T = T2;
             c.P = CP_P;
             c.Tp = Tp;
-            c.n = nseg;
             c.vec[0] = lw.w1t;
             c.vec[1] = lw.b1;
             c.vec[2] = lw.w2t;
@@ -515,11 +538,7 @@ int CamppModel::run_model_step(const PlanStep& s, const PlanInputs& in, cudaStre
             PPV_PDL_OK(launch_pdl(cp_bn_relu_kernel, dim3(grid), dim3(256), 0, st, s.x, s.vec[0], s.vec[1], s.out, s.C, s.rows), "cp_bn_relu_kernel");
             return PPV_OK;
         }
-        case CP_CONTEXT:
-            PPV_PDL_OK(launch_pdl(cp_context_kernel, dim3(s.B), dim3(256), 0, st, s.x, s.T, s.P, s.Tp, s.n, s.vec[0], s.vec[1], s.vec[2], s.vec[3],
-                                  s.out_f32),
-                       "cp_context_kernel");
-            return PPV_OK;
+        case CP_CONTEXT: return campplus_context_launch(s.x, s.B, s.T, s.P, s.Tp, s.vec[0], s.vec[1], s.vec[2], s.vec[3], s.out_f32, st);
     }
     return PlanModel::run_model_step(s, in, st);
 }

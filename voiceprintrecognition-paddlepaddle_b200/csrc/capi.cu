@@ -675,6 +675,157 @@ int ppv_asp_fused_test(const float* W, const float* att, const float* x, const f
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- column statistics test hook
+// Workspace: x planes [2][B Tp][ld], then the output planes [2][B][C or 2C].
+static size_t colstats_test_sizes(int B, int Tp, int ld, int C, size_t* x_bytes) {
+    *x_bytes = au(size_t(B) * Tp * ld * 2 * sizeof(__nv_bfloat16), 256);
+    return *x_bytes + au(size_t(B) * 2 * C * 2 * sizeof(__nv_bfloat16), 256);
+}
+size_t ppv_colstats_test_workspace_bytes(int B, int Tp, int ld, int C) {
+    size_t x_bytes;
+    return colstats_test_sizes(B, Tp, ld, C, &x_bytes);
+}
+int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int col0, int C, int mode, float eps, float inv_count,
+                      const int* nvalid, float* out, float* out_f32, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && out && ws, "ppv_colstats_test: null argument");
+    PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P && C > 0 && col0 >= 0 && col0 + C <= ld, "ppv_colstats_test: bad shape");
+    PPV_REQUIRE(mode >= 0 && mode <= 3 && (mode == 0 || !out_f32), "ppv_colstats_test: mode must be 0-3, out_f32 with mode 0 only");
+    size_t x_bytes;
+    PPV_REQUIRE(ws_bytes >= colstats_test_sizes(B, Tp, ld, C, &x_bytes), "ppv_colstats_test: workspace too small");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t rows = int64_t(B) * Tp;
+    const int oc = mode == 0 ? C : 2 * C;
+    __nv_bfloat16* base = static_cast<__nv_bfloat16*>(ws);
+    const Planes px{base, rows, ld, rows * ld};
+    const Planes po{reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + x_bytes), B, oc, int64_t(B) * oc};
+    if ((rc = launch_f32_to_planes(x, rows, ld, px, st))) return rc;
+    if ((rc = launch_colstats(px, col0, C, B, T, P, Tp, mode, eps, out_f32, po, st, inv_count, nvalid))) return rc;
+    return launch_planes_to_f32(po, 0, oc, B, 1, 0, 1, out, st);
+    PPV_GUARD_END
+}
+
+// ---------------------------------------------------------------- CAM++ context mask test hook
+// Workspace: h planes [2][B Tp][128], then w1t [128][64], b1 [64], w2t [64][32], b2 [32] fp32.
+static size_t cp_context_test_h_bytes(int B, int Tp) { return au(size_t(B) * Tp * 128 * 2 * sizeof(__nv_bfloat16), 256); }
+size_t ppv_campplus_context_test_workspace_bytes(int B, int Tp) {
+    return cp_context_test_h_bytes(B, Tp) + au((128 * 64 + 64 + 64 * 32 + 32) * sizeof(float), 256);
+}
+int ppv_campplus_context_test(const float* h, int B, int T, int P, int Tp, const float* w1, const float* b1, const float* w2,
+                              const float* b2, float* out, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(h && w1 && b1 && w2 && b2 && out && ws, "ppv_campplus_context_test: null argument");
+    PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P, "ppv_campplus_context_test: bad shape");
+    PPV_REQUIRE(ws_bytes >= ppv_campplus_context_test_workspace_bytes(B, Tp), "ppv_campplus_context_test: workspace too small");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t rows = int64_t(B) * Tp;
+    const Planes ph{static_cast<__nv_bfloat16*>(ws), rows, 128, rows * 128};
+    if ((rc = launch_f32_to_planes(h, rows, 128, ph, st))) return rc;
+    std::vector<float> w1h(64 * 128), w2h(32 * 64), w1t, w2t;
+    PPV_CUDA_OK(cudaMemcpyAsync(w1h.data(), w1, w1h.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(w2h.data(), w2, w2h.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    PPV_CUDA_OK(cudaStreamSynchronize(st));
+    campplus_context_weights(w1h.data(), w2h.data(), &w1t, &w2t);
+    float* wdev = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + cp_context_test_h_bytes(B, Tp));
+    float *dw1t = wdev, *db1 = dw1t + 128 * 64, *dw2t = db1 + 64, *db2 = dw2t + 64 * 32;
+    PPV_CUDA_OK(cudaMemcpyAsync(dw1t, w1t.data(), w1t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(dw2t, w2t.data(), w2t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(db1, b1, 64 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(db2, b2, 32 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    rc = campplus_context_launch(ph, B, T, P, Tp, dw1t, db1, dw2t, db2, out, st);
+    if (rc) return rc;
+    PPV_CUDA_OK(cudaStreamSynchronize(st));  // the host copies of the weights die here
+    return PPV_OK;
+    PPV_GUARD_END
+}
+
+// ---------------------------------------------------------------- time-axis gather-GEMM test hook
+// Workspace: each input's planes [2][rows][ld], then W planes [2][pad256(N)][sum ncols] (zero rows past N).
+static size_t taps_test_sizes(const ppv_gemm_taps_case* c, size_t* off) {
+    size_t o = 0;
+    int K = 0;
+    for (int i = 0; i < c->ninputs; ++i) {
+        off[i] = o;
+        o += au(size_t(c->rows[i]) * c->ld[i] * 2 * sizeof(__nv_bfloat16), 256);
+    }
+    for (int j = 0; j < c->nsrc; ++j) K += c->src_ncols[j];
+    off[PPV_TAPS_MAX_INPUTS] = o;
+    return o + au(au(size_t(c->N), 256) * K * 2 * sizeof(__nv_bfloat16), 256);
+}
+size_t ppv_gemm_test_taps_workspace_bytes(const ppv_gemm_taps_case* c) {
+    size_t off[PPV_TAPS_MAX_INPUTS + 1];
+    return c ? taps_test_sizes(c, off) : 0;
+}
+int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(c && c->W && c->out && ws, "ppv_gemm_test_taps: null argument");
+    PPV_REQUIRE(c->ninputs > 0 && c->ninputs <= PPV_TAPS_MAX_INPUTS && c->nsrc > 0 && c->nsrc <= PPV_TAPS_MAX_SOURCES,
+                "ppv_gemm_test_taps: 1-4 inputs and 1-16 sources");
+    for (int i = 0; i < c->ninputs; ++i) PPV_REQUIRE(c->x[i] && c->rows[i] > 0 && c->ld[i] > 0, "ppv_gemm_test_taps: bad input");
+    for (int j = 0; j < c->nsrc; ++j)
+        PPV_REQUIRE(c->src_input[j] >= 0 && c->src_input[j] < c->ninputs && c->src_col0[j] >= 0 && c->src_ncols[j] > 0,
+                    "ppv_gemm_test_taps: bad source");
+    PPV_REQUIRE(c->M > 0 && c->N > 0 && c->out_rows > 0 && c->out_col0 >= 0 && c->out_col0 + c->N <= c->out_ld,
+                "ppv_gemm_test_taps: bad output shape");
+    PPV_REQUIRE(c->Tp == 0 || (c->T > 0 && c->P >= 0 && c->Tp >= c->T + 2 * c->P && c->M % c->Tp == 0 && c->out_rows >= c->M),
+                "ppv_gemm_test_taps: bad time layout");
+    PPV_REQUIRE(!c->seg_scale || (c->Tp > 0 && c->seg_len > 0 && c->nseg == (c->T + c->seg_len - 1) / c->seg_len),
+                "ppv_gemm_test_taps: seg_scale needs the time layout and nseg = ceil(T / seg_len)");
+    PPV_REQUIRE(c->precision == PPV_PREC_BF16X3 || c->precision == PPV_PREC_BF16, "ppv_gemm_test_taps: bad precision");
+    size_t off[PPV_TAPS_MAX_INPUTS + 1];
+    PPV_REQUIRE(ws_bytes >= taps_test_sizes(c, off), "ppv_gemm_test_taps: workspace too small");
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint8_t* w8 = static_cast<uint8_t*>(ws);
+    Planes in[PPV_TAPS_MAX_INPUTS];
+    for (int i = 0; i < c->ninputs; ++i) {
+        in[i] = Planes{reinterpret_cast<__nv_bfloat16*>(w8 + off[i]), c->rows[i], c->ld[i], c->rows[i] * c->ld[i]};
+        if ((rc = launch_f32_to_planes(c->x[i], c->rows[i], c->ld[i], in[i], st))) return rc;
+    }
+    std::vector<GemmSource> srcs;
+    int K = 0;
+    for (int j = 0; j < c->nsrc; ++j) {
+        srcs.push_back(GemmSource{in[c->src_input[j]], c->src_col0[j], c->src_ncols[j], c->src_row_off[j]});
+        K += c->src_ncols[j];
+    }
+    const int64_t wrows = int64_t(au(size_t(c->N), 256));
+    const Planes pw{reinterpret_cast<__nv_bfloat16*>(w8 + off[PPV_TAPS_MAX_INPUTS]), wrows, K, wrows * K};
+    PPV_CUDA_OK(cudaMemsetAsync(pw.base, 0, size_t(2 * wrows * K) * sizeof(__nv_bfloat16), st));
+    if ((rc = launch_f32_to_planes(c->W, c->N, K, pw, st))) return rc;
+    Epilogue ep;
+    if (c->out_f32) {
+        ep.out_mode = OUT_F32;
+        ep.out = c->out;
+        ep.out_ld = c->out_ld;
+        ep.out_col0 = c->out_col0;
+        ep.Tp = c->Tp;
+        ep.P = c->P;
+        ep.T = c->T;
+    } else {
+        const Planes po{static_cast<__nv_bfloat16*>(c->out), c->out_rows, c->out_ld, c->out_rows * c->out_ld};
+        ep = planes_epilogue(po, c->out_col0, c->Tp, c->P, c->T);
+    }
+    ep.bias = c->bias;
+    ep.bn_scale = c->bn_scale;
+    ep.bn_shift = c->bn_shift;
+    ep.relu = c->relu ? 1 : 0;
+    ep.seg_scale = c->seg_scale;
+    ep.seg_len = c->seg_len;
+    ep.nseg = c->nseg;
+    ep.halo = c->halo ? 1 : 0;
+    ep.zero_invalid = c->zero_invalid ? 1 : 0;
+    GemmParams gp;
+    rc = gemm_build(&gp, srcs.data(), int(srcs.size()), pw, c->M, c->N, ep, c->block_n > 0 ? c->block_n : gemm_pick_bn(c->N), c->block_k);
+    if (rc) return rc;
+    return gemm_launch(gp, c->precision, device_sm_count(), st);
+    PPV_GUARD_END
+}
+
 // Kernel-only timing of the gather-GEMM (tools/gemm_bench.py): operands are converted once, the kernel is launched
 // `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  planes_out selects the epilogue:
 //   0  ReLU, fp32 [M,N];   1  ReLU, split-bf16 planes (the layout every model layer writes);

@@ -10,6 +10,7 @@
 #include <algorithm>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "../../include/ppv_b200.h"
 
@@ -356,6 +357,13 @@ void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c);
 int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out);
 void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);
 int campplus_create(const ppv_campplus_cfg* cfg, Model** out);
+// CAM++'s context-mask MLP weights in the reference layout, w1 [64][128] and w2 [32][64], -> the transposed [128][64] and [64][32]
+// the context kernel reads
+void campplus_context_weights(const float* w1, const float* w2, std::vector<float>* w1t, std::vector<float>* w2t);
+// The context mask of CAM++'s dense layers: h [B Tp, 128] planes (T frames from row P of each utterance) -> out [B nseg, 32] fp32,
+// nseg = ceil(T / 100) <= 64
+int campplus_context_launch(const Planes& h, int B, int T, int P, int Tp, const float* w1t, const float* b1, const float* w2t,
+                            const float* b2, float* out, cudaStream_t st);
 
 // ---- conv2d models: zero-bordered NHWC image grids (image_plan.h / image_plan.cu) ------------------------
 struct ImageGeo {

@@ -86,13 +86,25 @@ __device__ __forceinline__ float2 block_colsum(float2 v, float2 (*s_part)[32], i
 // mode 1: mean and std = sqrt(clip(var, eps)) -> planes [B, 2C] (mean | std)             (ASP global context)
 // mode 2: mean and std = sqrt(var_unbiased + eps) -> planes [B, 2C]                       (TSTP, pooling.py:138-146)
 // mode 3: mean and var_unbiased -> planes [B, 2C]                                          (TSP, pooling.py:42-45)
-// Single pass with a per-channel shift K = x[first frame]: sum(x-K), sum((x-K)^2); var = (Q - S^2/T)/T.
+// One pass: each thread keeps Welford's running (count, mean, M2) over its frames; the lanes and then the warps are merged with Chan's
+// formula in a fixed order (deterministic, no atomics).  A sum of squares about a fixed shift would cancel in fp32 when the shift
+// sits far from the channel's mean (a frame 0 at the ReLU floor under a channel 20-50 std above it).
 // Each lane owns 8 channels (one 16-byte load per plane), 4 frames per warp, 32 frames per block iteration.
+__device__ __forceinline__ void chan_merge(float& na, float& ma, float& qa, float nb, float mb, float qb) {
+    const float n = na + nb;
+    const float d = mb - ma;
+    const float f = n > 0.f ? nb / n : 0.f;
+    ma = fmaf(d, f, ma);
+    qa = qa + qb + d * d * na * f;
+    na = n;
+}
+
 __global__ void __launch_bounds__(STAT_WARPS * 32)
     colstats_kernel(Planes x, int col0, int C, int T_all, int P, int Tp, int mode, float eps, float inv_count, float* __restrict__ out_f32,
                     Planes out_pl, const int* __restrict__ nvalid) {
-    __shared__ float s_s[STAT_WARPS][64];
+    __shared__ float s_m[STAT_WARPS][64];
     __shared__ float s_q[STAT_WARPS][64];
+    __shared__ float s_n[STAT_WARPS];
     griddep_launch_dependents();
     griddep_wait();
     const int b = blockIdx.y;
@@ -114,49 +126,50 @@ __global__ void __launch_bounds__(STAT_WARPS * 32)
             v[2 * i + 1] = hf.y + lf.y;
         }
     };
-    float k[8], s[8], q[8];
-    load8(row0, k);
+    float n = 0.f, m[8], q[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
+    for (int i = 0; i < 8; ++i) m[i] = q[i] = 0.f;
 #pragma unroll 4
     for (int t = warp * 4 + rsub; t < T; t += STAT_WARPS * 4) {
         float v[8];
         load8(row0 + t, v);
+        n += 1.f;
+        const float rn = 1.f / n;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const float d = v[i] - k[i];
-            s[i] += d;
-            q[i] = fmaf(d, d, q[i]);
+            const float d = v[i] - m[i];
+            m[i] = fmaf(d, rn, m[i]);  // the first frame: m = v exactly
+            q[i] = fmaf(d, v[i] - m[i], q[i]);
         }
     }
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 8);
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 16);
-        q[i] += __shfl_xor_sync(0xffffffffu, q[i], 8);
-        q[i] += __shfl_xor_sync(0xffffffffu, q[i], 16);
-    }
-    if (rsub == 0) {
+    for (int sh = 8; sh <= 16; sh *= 2) {
+        const float nb = __shfl_xor_sync(0xffffffffu, n, sh);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            s_s[warp][cg * 8 + i] = s[i];
+            const float mb = __shfl_xor_sync(0xffffffffu, m[i], sh), qb = __shfl_xor_sync(0xffffffffu, q[i], sh);
+            float na = n;
+            chan_merge(na, m[i], q[i], nb, mb, qb);
+        }
+        n += nb;
+    }
+    if (rsub == 0) {
+        if (cg == 0) s_n[warp] = n;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            s_m[warp][cg * 8 + i] = m[i];
             s_q[warp][cg * 8 + i] = q[i];
         }
     }
     __syncthreads();
     if (threadIdx.x < 64) {
         const int ch = threadIdx.x;  // channel within the slab
-        float S = 0.f, Q = 0.f;
+        float N = s_n[0], M = s_m[0][ch], Q = s_q[0][ch];
 #pragma unroll
-        for (int w = 0; w < STAT_WARPS; ++w) {
-            S += s_s[w][ch];
-            Q += s_q[w][ch];
-        }
-        // shift of this channel: lane (ch / 8) of warp 0 holds k[ch % 8]; re-read instead of shuffling
-        const int64_t off0 = row0 * x.ld + col0 + blockIdx.x * 64 + ch;
-        const float K = __bfloat162float(x.hi()[off0]) + __bfloat162float(x.lo()[off0]);
+        for (int w = 1; w < STAT_WARPS; ++w) chan_merge(N, M, Q, s_n[w], s_m[w][ch], s_q[w][ch]);
         const float inv = inv_count > 0.f ? inv_count : 1.f / float(T);  // inv_count: zero-bordered images are summed whole
-        const float mean = (inv_count > 0.f ? K * float(T) * inv : K) + S * inv;
+        const float mean = inv_count > 0.f ? M * float(T) * inv : M;
+        const float ssq = Q;  // sum of squared deviations from the mean
         const int cc = blockIdx.x * 64 + ch;
         if (mode == 0) {
             if (out_f32) out_f32[int64_t(b) * C + cc] = mean;
@@ -168,7 +181,6 @@ __global__ void __launch_bounds__(STAT_WARPS * 32)
             }
         } else {
             // mode 1: ASP global std = sqrt(clip(var_biased, eps)); mode 2: TSTP std = sqrt(var_unbiased + eps)
-            const float ssq = Q - S * S * inv;
             // mode 3: unbiased VARIANCE, no square root (TemporalStatisticsPooling, pooling.py:44)
             const float sd = (mode == 2)   ? sqrtf(fmaxf(ssq, 0.f) / float(T > 1 ? T - 1 : 1) + eps)
                              : (mode == 3) ? fmaxf(ssq, 0.f) / float(T > 1 ? T - 1 : 1)

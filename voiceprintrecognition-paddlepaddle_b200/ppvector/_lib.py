@@ -66,8 +66,24 @@ class CamPPlusCfg(C.Structure):
                 ("init_channels", C.c_int), ("precision", C.c_int)]
 
 
+TAPS_MAX_INPUTS, TAPS_MAX_SOURCES = 4, 16
+
+
+class GemmTapsCase(C.Structure):
+    """ppv_gemm_taps_case: one time-axis gather-GEMM case of ppv_gemm_test_taps"""
+    _fields_ = [("x", C.c_void_p * TAPS_MAX_INPUTS), ("rows", C.c_int64 * TAPS_MAX_INPUTS), ("ld", C.c_int * TAPS_MAX_INPUTS),
+                ("ninputs", C.c_int), ("nsrc", C.c_int),
+                ("src_input", C.c_int * TAPS_MAX_SOURCES), ("src_col0", C.c_int * TAPS_MAX_SOURCES),
+                ("src_ncols", C.c_int * TAPS_MAX_SOURCES), ("src_row_off", C.c_int * TAPS_MAX_SOURCES),
+                ("W", C.c_void_p), ("bias", C.c_void_p), ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p), ("seg_scale", C.c_void_p),
+                ("M", C.c_int), ("N", C.c_int), ("relu", C.c_int), ("seg_len", C.c_int), ("nseg", C.c_int), ("Tp", C.c_int), ("P", C.c_int),
+                ("T", C.c_int), ("halo", C.c_int), ("zero_invalid", C.c_int), ("out_f32", C.c_int), ("out", C.c_void_p),
+                ("out_rows", C.c_int64), ("out_ld", C.c_int), ("out_col0", C.c_int), ("block_n", C.c_int), ("block_k", C.c_int),
+                ("precision", C.c_int)]
+
+
 _P = C.c_void_p
-# name -> (restype, argtypes); this table is also what tests/test_abi.py checks against include/ppv_b200.h
+# name ->(restype, argtypes); this table is also what tests/test_abi.py checks against include/ppv_b200.h
 SIGNATURES = {
     "ppv_version": (C.c_int, []),
     "ppv_last_error": (C.c_int, [C.c_char_p, C.c_size_t]),
@@ -151,6 +167,12 @@ SIGNATURES = {
     "ppv_conv2d_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 13 + [_P, _P, C.c_size_t, _P]),
     "ppv_asp_fused_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "ppv_asp_fused_test": (C.c_int, [_P] * 6 + [C.c_int] * 8 + [_P, _P, _P, C.c_size_t, _P]),
+    "ppv_colstats_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "ppv_colstats_test": (C.c_int, [_P] + [C.c_int] * 8 + [C.c_float, C.c_float] + [_P, _P, _P, _P, C.c_size_t, _P]),
+    "ppv_campplus_context_test_workspace_bytes": (C.c_size_t, [C.c_int] * 2),
+    "ppv_campplus_context_test": (C.c_int, [_P] + [C.c_int] * 4 + [_P] * 6 + [C.c_size_t, _P]),
+    "ppv_gemm_test_taps_workspace_bytes": (C.c_size_t, [C.POINTER(GemmTapsCase)]),
+    "ppv_gemm_test_taps": (C.c_int, [C.POINTER(GemmTapsCase), _P, C.c_size_t, _P]),
 }
 
 _lib = None
