@@ -54,12 +54,6 @@ struct TransitW {
     int C = 0;
 };
 
-// CAM++'s own plan steps (PlanStep::MODEL):
-//   FLATTEN_PAIRS  x on grid g -> frame-pair matrix `out` (C channels, Tp / P time layout)
-//   BN_RELU        out = relu(x * vec[0] + vec[1]) over C columns of `rows` rows
-//   CONTEXT        x [B * Tp, 128] -> context mask out_f32 [B * ceil(T / 100), 32] (MLP vec[0..3]), T frames from row P of each utterance
-enum CpKind { CP_FLATTEN_PAIRS, CP_BN_RELU, CP_CONTEXT };
-
 // ------------------------------------------------------------------------------------------------ kernels
 // out[r, c] = relu(x[r, c] * scale[c] + shift[c]) for c < C (C % 8 == 0), every row
 __global__ void __launch_bounds__(256)
@@ -240,7 +234,6 @@ struct CamppModel : PlanModel {
   protected:
     bool prepare_weights(ArenaBuilder& ab) override;
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
-    int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) override;
     int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
@@ -413,15 +406,15 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
         ep.relu = 1;
         return ep;
     };
+    // cb.tmp = relu(x * scale + shift) over C columns of every row
     auto bn_relu = [&](const Planes& x, const float* scale, const float* shift, int C) {
-        PlanStep s = model_step(CP_BN_RELU);
-        s.x = x;
-        s.out = cb.tmp;
-        s.vec[0] = scale;
-        s.vec[1] = shift;
-        s.C = C;
-        s.rows = M2;
-        m->steps.push_back(s);
+        m->steps.push_back({"cp_bn_relu_kernel", false, [x, scale, shift, out = cb.tmp, C, rows = int64_t(M2)](const StepRun& r) {
+                                const int64_t total = rows * (C / 8);
+                                const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(r.num_sms) * 16));
+                                PPV_PDL_OK(launch_pdl(cp_bn_relu_kernel, dim3(grid), dim3(256), 0, r.st, x, scale, shift, out, C, rows),
+                                           "cp_bn_relu_kernel");
+                                return PPV_OK;
+                            }});
     };
     // ---- FCM head: its convs stride the frequency axis only
     m->steps.push_back(stem_step(m->stem_w, m->stem_b, 32, cb.stem_out, m->geo[0], B));
@@ -447,15 +440,15 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     {
         rc = plan_conv3x3(m->head_conv2, x, 0, 32, m->geo[2], B, relu(image_epilogue(cb.head_out, m->geo[2], m->geo[3], 2, 1)));
         if (rc) return rc;
-        PlanStep s = model_step(CP_FLATTEN_PAIRS);
-        s.x = cb.head_out;
-        s.g = m->geo[3];
-        s.B = B;
-        s.C = 32;
-        s.out = cb.flat;
-        s.Tp = Tp;
-        s.P = CP_P;
-        m->steps.push_back(s);
+        // head output on grid 3 -> frame-pair matrix
+        m->steps.push_back({"cp_flatten_pairs_kernel", false, [in = cb.head_out, g = m->geo[3], B, C = 32, out = cb.flat, Tp](const StepRun& r) {
+                                const int64_t total = int64_t(B) * g.W * C * g.H;
+                                const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(r.num_sms) * 16));
+                                PPV_PDL_OK(launch_pdl(cp_flatten_pairs_kernel, dim3(grid), dim3(256), 0, r.st, in, B, g.H, g.W, g.Hp, g.Wp, C, out,
+                                                      Tp, CP_P),
+                                           "cp_flatten_pairs_kernel");
+                                return PPV_OK;
+                            }});
     }
     // ---- TDNN (k5, stride 2) over the frame-pair matrix -> first 128 columns of block 1's buffer
     {
@@ -474,18 +467,10 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             bn_relu(xb, lw.bn1_scale, lw.bn1_shift, lw.Kp);
             rc = plan_conv(lw.linear1, {GemmSource{cb.tmp, 0, lw.Kp, 0}}, M2, relu(time_epi(cb.hbuf, 0)));
             if (rc) return rc;
-            PlanStep c = model_step(CP_CONTEXT);
-            c.x = cb.hbuf;
-            c.B = B;
-            c.T = T2;
-            c.P = CP_P;
-            c.Tp = Tp;
-            c.vec[0] = lw.w1t;
-            c.vec[1] = lw.b1;
-            c.vec[2] = lw.w2t;
-            c.vec[3] = lw.b2;
-            c.out_f32 = cb.mask;
-            m->steps.push_back(c);
+            m->steps.push_back({"campplus_context_launch", false,
+                                [h = cb.hbuf, B, T2, Tp, w1t = lw.w1t, b1 = lw.b1, w2t = lw.w2t, b2 = lw.b2, mask = cb.mask](const StepRun& r) {
+                                    return campplus_context_launch(h, B, T2, CP_P, Tp, w1t, b1, w2t, b2, mask, r.st);
+                                }});
             Epilogue ep = time_epi(xb, lw.in_ch);
             ep.seg_scale = cb.mask;
             ep.seg_len = CP_SEG;
@@ -519,28 +504,6 @@ int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
     m->T2 = T2;
     m->Tp = Tp;
     return PPV_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ forward
-int CamppModel::run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) {
-    switch (s.model_kind) {
-        case CP_FLATTEN_PAIRS: {
-            const ImageGeo& g = s.g;
-            const int64_t total = int64_t(s.B) * g.W * s.C * g.H;
-            const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(num_sms) * 16));
-            PPV_PDL_OK(launch_pdl(cp_flatten_pairs_kernel, dim3(grid), dim3(256), 0, st, s.x, s.B, g.H, g.W, g.Hp, g.Wp, s.C, s.out, s.Tp, s.P),
-                       "cp_flatten_pairs_kernel");
-            return PPV_OK;
-        }
-        case CP_BN_RELU: {
-            const int64_t total = s.rows * (s.C / 8);
-            const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(num_sms) * 16));
-            PPV_PDL_OK(launch_pdl(cp_bn_relu_kernel, dim3(grid), dim3(256), 0, st, s.x, s.vec[0], s.vec[1], s.out, s.C, s.rows), "cp_bn_relu_kernel");
-            return PPV_OK;
-        }
-        case CP_CONTEXT: return campplus_context_launch(s.x, s.B, s.T, s.P, s.Tp, s.vec[0], s.vec[1], s.vec[2], s.vec[3], s.out_f32, st);
-    }
-    return PlanModel::run_model_step(s, in, st);
 }
 
 // taps: "head.layer1", "head.layer2" -> fp32 [B,H,W,32]; "tdnn" [B,T2,128]; "block1".."block3" [B,T2,C]; "transit1", "transit2"

@@ -281,11 +281,17 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
                 sj[j - 1] = cw.bn_scale;
                 hj[j - 1] = cw.bn_shift;
             }
-            PlanStep s;
-            s.kind = PlanStep::RES2CHAIN;
-            rc = res2chain_build(&s.cp, buf.h, buf.y, Wj, bj, sj, hj, scale - 1, B, T, P, Tp, d, res2_paired);
+            Res2ChainParams cp;
+            rc = res2chain_build(&cp, buf.h, buf.y, Wj, bj, sj, hj, scale - 1, B, T, P, Tp, d, res2_paired);
             if (rc) return rc;
-            steps.push_back(s);
+            steps.push_back({"res2chain_launch", true, [cp](const StepRun& r) {
+                                 const int rc = res2chain_launch(cp, r.precision, r.num_sms, r.st);
+                                 if (cp.trace) {
+                                     static int dumps = 0;
+                                     if (++dumps == 10) res2chain_trace_dump(cp);  // a warm launch of the first block
+                                 }
+                                 return rc;
+                             }});
         }
         for (int j = 1; j < scale && !use_res2_chain; ++j) {
             const ConvW& cw = res2[b - 1][j];
@@ -293,11 +299,10 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             if (use_res2_kernel) {  // weight-stationary kernel, one tall tile per source (res2conv.cu)
                 const GemmSource srcs[2] = {GemmSource{buf.h, j * w, w, 0}, GemmSource{buf.y, (j - 1) * w, w, 0}};
                 ep.bias = cw.bias;
-                PlanStep s;
-                s.kind = PlanStep::RES2;
-                rc = res2conv_build(&s.rp, srcs, j >= 2 ? 2 : 1, cw.W, R, d, ep);
+                Res2Params rp;
+                rc = res2conv_build(&rp, srcs, j >= 2 ? 2 : 1, cw.W, R, d, ep);
                 if (rc) return rc;
-                steps.push_back(s);
+                steps.push_back({"res2conv_launch", true, [rp](const StepRun& r) { return res2conv_launch(rp, r.precision, r.num_sms, r.st); }});
             } else {  // the gather-GEMM over the three taps of chunk j and, from j = 2, of conv j-1's output
                 std::vector<GemmSource> srcs;
                 for (int tap = 0; tap < 3; ++tap) srcs.push_back(GemmSource{buf.h, j * w, w, (tap - 1) * d});
@@ -345,14 +350,9 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
             rc = plan_gemm(att1, {GemmSource{buf.mfa, 0, C3, 0}}, R, ep);
             if (rc) return rc;
         }
-        {  // attention logits (transposed GEMM) + softmax over time + weighted mean / std + asp_bn, fused
-            PlanStep s;
-            s.kind = PlanStep::ASP_FUSED;
-            rc = asp_fused_build(&s.ap, att2.W, buf.att, buf.mfa, aspbn_scale, aspbn_shift, buf.pool, buf.pooled_raw, B, T, P, Tp, C3,
-                                 att, 1e-12f);
-            if (rc) return rc;
-            steps.push_back(s);
-        }
+        // attention logits (transposed GEMM) + softmax over time + weighted mean / std + asp_bn, fused
+        rc = plan_asp_fused(att2.W, buf.att, buf.mfa, aspbn_scale, aspbn_shift, buf.pool, buf.pooled_raw, B, T, P, Tp, C3, att, 1e-12f);
+        if (rc) return rc;
     }
     // fc: pooled [B, Kp] -> [B, embd]
     const int Kp = (pooling == PPV_POOL_ASP || pooling == PPV_POOL_TSP) ? 2 * C3 : C3;

@@ -23,6 +23,7 @@
 
 #include "common.h"
 #include "plan.h"
+#include "train.h"
 
 namespace ppv {
 
@@ -48,13 +49,6 @@ struct TLayer {  // TDNNBlock
     TBN bn;
 };
 
-// The trainer's own plan steps (PlanStep::MODEL), one per launcher call: run_model_step passes each launcher its arguments from the
-// step's fields as plan.h lays them out.
-enum TrKind {
-    TR_REPACK, TR_PACK, TR_BN_FWD, TR_DENSE_FWD, TR_PLANES_TO_F32, TR_ASP_POOL, TR_BN1D_FWD, TR_AAM_FWD, TR_AAM_BWD, TR_DENSE_BWD,
-    TR_BN1D_BWD, TR_ASP_BWD, TR_GRAD_SUM, TR_BN_BWD, TR_TRANSPOSE, TR_WGRAD_UNPACK, TR_ASP_GLOBAL_BWD, TR_GRAD_DOT, TR_ACT_BWD
-};
-
 // The workspace views of one plan (tr_carve).  `layer` is indexed like Trainer::conv: the TDNN layers, then asp.conv.
 struct TrBuffers {
     int Tp = 0;          // rows per utterance: T + 2P
@@ -78,7 +72,7 @@ struct TrBuffers {
 // One readable tap (trainer_read_tap): planes read as fp32 [B, T, cols] from column col0, or `count` fp32 values as stored.  A
 // per-block tap has one buffer per block; the others use index 0.
 struct TrTap {
-    bool per_block = false, f32 = false;
+    bool per_block = false, fp32 = false;
     Planes pl[3];
     int col0 = 0, cols = 0;
     const float* vec[3] = {};
@@ -117,7 +111,6 @@ struct Trainer : PlanOwner, EcapaGeometry {
 
   protected:
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
-    int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) override;
 };
 
 // ------------------------------------------------------------------------------------------------ create: flat layout
@@ -352,7 +345,7 @@ std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, 
     auto vec = [&](const std::string& name, float* const* p, bool per_block, size_t count) {
         TrTap& e = m[name];
         e.per_block = per_block;
-        e.f32 = true;
+        e.fp32 = true;
         for (int b = 0; b < (per_block ? 3 : 1); ++b) e.vec[b] = p[b];
         e.count = count;
     };
@@ -421,21 +414,13 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     float* const grd = t->grads;
     float* const sta = t->stats;
 
-    auto model = [&](TrKind kind) {
-        PlanStep s = model_step(kind);
-        s.B = B;
-        s.T = T;
-        s.P = P;
-        s.Tp = Tp;
-        return s;
-    };
-    auto push = [&](const PlanStep& s) { t->steps.push_back(s); };
+    // the trainer's own steps: one launcher call each, none on the tensor cores
+    auto push = [&](const char* name, std::function<int(const StepRun&)> launch) { t->steps.push_back({name, false, std::move(launch)}); };
     auto gemm = [&](const std::vector<GemmSource>& srcs, const Planes& w, int N, const Epilogue& ep) -> int {
-        PlanStep s;
-        s.kind = PlanStep::GEMM;
-        int r = gemm_build(&s.gp, srcs.data(), int(srcs.size()), w, M, N, ep, gemm_pick_bn(N));
-        if (!r) push(s);
-        return r;
+        GemmParams gp;
+        int err = gemm_build(&gp, srcs.data(), int(srcs.size()), w, M, N, ep, gemm_pick_bn(N));
+        if (!err) t->steps.push_back(gemm_step(gp));
+        return err;
     };
     // forward conv: bias + ReLU -> post-activation planes (valid frames), or fp32 rows
     auto fwd_gemm = [&](int li, const std::vector<GemmSource>& srcs, const Planes& out, int out_col0, bool relu, const float* rowgrp,
@@ -461,45 +446,36 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
                       const Planes* out2, int out2_col0) {
         const TBN& bn = t->L[li].bn;
         const TrBuffers::Layer& w = f.layer[li];
-        PlanStep s = model(TR_BN_FWD);
-        s.x = a;
-        s.xc0 = a_col0;
-        s.C = bn.C;
-        s.vec = {par + bn.g_off, par + bn.b_off};
-        s.f32 = {w.mean, w.rstd, w.scale, w.shift, sta + bn.rm_off, sta + bn.rv_off, f.part};
-        s.apply.y = y;
-        s.apply.y_col0 = y_col0;
-        s.apply.tanh_ = tanh_;
+        BnApplyArgs apply;
+        apply.y = y;
+        apply.y_col0 = y_col0;
+        apply.tanh_ = tanh_;
         if (out2) {
-            s.apply.add = *add;
-            s.apply.add_col0 = add_col0;
-            s.apply.out2 = *out2;
-            s.apply.out2_col0 = out2_col0;
+            apply.add = *add;
+            apply.add_col0 = add_col0;
+            apply.out2 = *out2;
+            apply.out2_col0 = out2_col0;
         }
-        push(s);
+        push("tr_bn_forward", [a, a_col0, Cn = bn.C, B, T, P, Tp, gamma = par + bn.g_off, beta = par + bn.b_off, mean = w.mean, rstd = w.rstd,
+                               scale = w.scale, shift = w.shift, run_mean = sta + bn.rm_off, run_var = sta + bn.rv_off, part = f.part,
+                               apply](const StepRun& r) {
+            return tr_bn_forward(a, a_col0, Cn, B, T, P, Tp, TR_BN_EPS, TR_BN_MOMENTUM, gamma, beta, mean, rstd, scale, shift, run_mean, run_var,
+                                 part, apply, r.num_sms, r.st);
+        });
     };
     auto dense_fwd = [&](const float* X, int x_ld, const float* Wt, int w_ld, const float* bias, int Mr, int N, int K, int act, float* Y, int y_ld) {
-        PlanStep s = model(TR_DENSE_FWD);
-        s.vec = {X, Wt, bias};
-        s.dim = {x_ld, w_ld, Mr, N, K, act, y_ld};
-        s.f32 = {Y};
-        push(s);
+        push("tr_dense_fwd", [X, x_ld, Wt, w_ld, bias, Mr, N, K, act, Y, y_ld](const StepRun& r) {
+            return tr_dense_fwd(X, x_ld, Wt, w_ld, bias, Mr, N, K, act, Y, y_ld, r.st);
+        });
     };
     auto dense_bwd = [&](const float* dY, int dy_ld, const float* X, int x_ld, const float* Wt, int w_ld, int Mr, int N, int K, float* dX,
                          int dx_ld, float* dW, int dw_ld, float* db) {
-        PlanStep s = model(TR_DENSE_BWD);
-        s.vec = {dY, X, Wt};
-        s.dim = {dy_ld, x_ld, w_ld, Mr, N, K, dx_ld, dw_ld};
-        s.f32 = {dX, dW, db};
-        push(s);
+        push("tr_dense_bwd", [dY, dy_ld, X, x_ld, Wt, w_ld, Mr, N, K, dX, dx_ld, dW, dw_ld, db](const StepRun& r) {
+            return tr_dense_bwd(dY, dy_ld, X, x_ld, Wt, w_ld, Mr, N, K, dX, dx_ld, dW, dw_ld, db, r.st);
+        });
     };
     auto act_bwd = [&](float* dy, const float* y, int64_t n, int act, float alpha) {
-        PlanStep s = model(TR_ACT_BWD);
-        s.f32 = {dy};
-        s.vec = {y};
-        s.dim = {n, act};
-        s.inv_count = alpha;
-        push(s);
+        push("tr_act_bwd", [dy, y, n, act, alpha](const StepRun& r) { return tr_act_bwd(dy, y, n, act, alpha, r.st); });
     };
     // data gradient: dx_pad[r, cin] = sum_tap dz[r - off_tap, :] . W[:, cin, tap]  -> planes on every row
     auto dgrad_gemm = [&](int li, const Planes& dz, int dz_col0, const Planes& out, int out_col0) -> int {
@@ -508,16 +484,11 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     };
     // out[c][row0 + r] = in[r + shift][col0 + c]; ntaps > 1: tap z shifted by z * shift_step into rows z * row_step on
     auto transpose = [&](const Planes& in, int col0, int Cn, Planes out, int row0, int shift, int ntaps, int shift_step, int row_step) {
-        PlanStep s = model(TR_TRANSPOSE);
-        s.x = in;
-        s.xc0 = col0;
-        s.C = Cn;
-        s.rows = f.R;
         out.base += int64_t(row0) * out.ld;
         out.rows -= row0;
-        s.out = out;
-        s.dim = {shift, ntaps, shift_step, row_step};
-        push(s);
+        push("tr_transpose", [in, col0, Cn, rows = f.R, out, shift, ntaps, shift_step, row_step](const StepRun& r) {
+            return tr_transpose(in, col0, Cn, rows, out, shift, r.st, ntaps, shift_step, row_step);
+        });
     };
     // weight gradient: dz^T -> TA; one row-shifted transpose of the layer input per tap -> TB rows [tap * Cinp, ...); ONE GEMM
     // [Cout] x [taps * Cinp] over the frames (split-K partials); unpack into the flat gradient buffer
@@ -531,16 +502,14 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         for (const WgradInput& x : xs) transpose(x.x, x.col0, x.C, f.TB, x.row0, -((c.taps - 1) / 2) * c.dil, c.taps, c.dil, c.Cinp);
         const int N = c.taps * c.Cinp;
         const WgradSplit sp = tr_wgrad_split(t, c, f.Rp);
-        PlanStep g;
-        g.kind = PlanStep::GEMM;
-        int r = gemm_build_wgrad(&g.gp, f.TA, f.TB, c.Cout, N, 0, 0, sp.splits, f.wpart, N, 0, sp.Mpad, sp.BN);
-        if (r) return r;
-        push(g);
-        PlanStep s = model(TR_WGRAD_UNPACK);
-        s.vec = {f.wpart};
-        s.dim = {g.gp.lin_splits, sp.Mpad, c.Cout, c.Cin, c.Cinp, c.taps, int64_t(c.CinTotal) * c.taps};
-        s.f32 = {grd + c.w_off};
-        push(s);
+        GemmParams gp;
+        int err = gemm_build_wgrad(&gp, f.TA, f.TB, c.Cout, N, 0, 0, sp.splits, f.wpart, N, 0, sp.Mpad, sp.BN);
+        if (err) return err;
+        t->steps.push_back(gemm_step(gp));
+        push("tr_wgrad_unpack", [part = f.wpart, splits = gp.lin_splits, split_rows = sp.Mpad, Cout = c.Cout, Cin = c.Cin, Cinp = c.Cinp, taps = c.taps,
+                                 grad = grd + c.w_off, g_ld = int64_t(c.CinTotal) * c.taps](const StepRun& r) {
+            return tr_wgrad_unpack(part, splits, split_rows, Cout, Cin, Cinp, taps, grad, g_ld, r.st);
+        });
         return PPV_OK;
     };
     auto src1 = [](const Planes& p, int col0, int fold) {
@@ -553,44 +522,31 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     auto bn_bwd = [&](int li, const GradSrcList& gl, const Planes& a, int a_col0, const Planes& dz, int dz_col0) {
         const TLayer& l = t->L[li];
         const TrBuffers::Layer& w = f.layer[li];
-        PlanStep s = model(TR_BN_BWD);
-        s.gl = gl;
-        s.x = a;
-        s.xc0 = a_col0;
-        s.C = l.bn.C;
-        s.vec = {w.mean, w.rstd, par + l.bn.g_off};
-        s.f32 = {grd + l.bn.g_off, grd + l.bn.b_off, grd + l.conv.b_off, f.part};
-        s.out = dz;
-        s.oc0 = dz_col0;
-        s.dim = {int64_t(f.part_elems), tr_bn_bwd_tsplit(t, li, B)};
-        push(s);
+        push("tr_bn_backward", [gl, a, a_col0, Cn = l.bn.C, B, T, P, Tp, mean = w.mean, rstd = w.rstd, gamma = par + l.bn.g_off,
+                                dgamma = grd + l.bn.g_off, dbeta = grd + l.bn.b_off, dz, dz_col0, dbias = grd + l.conv.b_off, part = f.part,
+                                part_elems = f.part_elems, tsplit = tr_bn_bwd_tsplit(t, li, B)](const StepRun& r) {
+            return tr_bn_backward(gl, a, a_col0, Cn, B, T, P, Tp, mean, rstd, gamma, dgamma, dbeta, dz, dz_col0, dbias, part, part_elems, r.st,
+                                  tsplit);
+        });
     };
     // out (optional planes, valid frames) = summed sources, per-utterance column sums -> part, colsum (optional) [Cn]
     auto grad_sum = [&](const GradSrcList& gl, int Cn, const Planes& out, float* colsum) {
-        PlanStep s = model(TR_GRAD_SUM);
-        s.gl = gl;
-        s.C = Cn;
-        s.out = out;
-        s.f32 = {f.part, colsum};
-        push(s);
+        push("tr_grad_sum", [gl, Cn, B, T, P, Tp, out, part = f.part, colsum](const StepRun& r) {
+            return tr_grad_sum(gl, Cn, B, T, P, Tp, out, 0, part, colsum, r.st);
+        });
     };
 
     // ================================================================= forward
     for (int l = 0; l <= t->l_att2(); ++l) {
         const TConv& c = t->conv(l);
-        PlanStep s = model(TR_REPACK);
-        s.vec = {par + c.w_off};
-        s.dim = {int64_t(c.CinTotal) * c.taps, c.Cout, c.Cin, c.Cinp, c.taps};
-        s.x = f.layer[l].wf;
-        s.y = f.layer[l].wd;
-        push(s);
+        push("tr_repack_conv", [w = par + c.w_off, w_ld = int64_t(c.CinTotal) * c.taps, Cout = c.Cout, Cin = c.Cin, Cinp = c.Cinp, taps = c.taps,
+                                wf = f.layer[l].wf, wd = f.layer[l].wd](const StepRun& r) {
+            return tr_repack_conv(w, w_ld, Cout, Cin, Cinp, taps, wf, wd, r.st);
+        });
     }
-    {
-        PlanStep s = model(TR_PACK);
-        s.C = t->cfg.input_size;
-        s.out = f.X0;
-        push(s);
-    }
+    push("launch_pack_features", [B, T, F = t->cfg.input_size, X0 = f.X0, P, Tp](const StepRun& r) {
+        return launch_pack_features(r.in.feat, B, T, F, X0, P, Tp, r.st);
+    });
     {
         const int li = t->l_conv0;
         rc = fwd_gemm(li, taps_of(t->conv(li), f.X0, 0, +1), f.A0, 0, true, nullptr, nullptr);
@@ -624,12 +580,10 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
             bn_fwd(li, f.At2[b], 0, f.Yt2[b], 0, 0, nullptr, 0, nullptr, 0);
         }
         // SE: squeeze, excite, then scale + residual into OUTCAT's window b
-        PlanStep sq = colstats_step(f.Yt2[b], C, B, T, P, Tp, 0, 0.f, Planes());
-        sq.out_f32 = f.se_s[b];
-        push(sq);
+        t->steps.push_back(colstats_step(f.Yt2[b], C, B, T, P, Tp, 0, 0.f, Planes(), 0.f, false, f.se_s[b]));
         dense_fwd(f.se_s[b], C, par + t->se1_w[b], C, par + t->se1_b[b], B, se, C, 1, f.se_g1[b], se);
         dense_fwd(f.se_g1[b], se, par + t->se2_w[b], se, par + t->se2_b[b], B, C, se, 2, f.se_g2[b], C);
-        push(scale_res_step(f.Yt2[b], f.se_g2[b], u, uc, f.OUTCAT, C * b, C, Tp, f.R, false));
+        t->steps.push_back(scale_res_step(f.Yt2[b], f.se_g2[b], u, uc, f.OUTCAT, C * b, C, Tp, f.R, false));
     }
     {
         rc = fwd_gemm(t->l_mfa, {GemmSource{f.OUTCAT, 0, C3, 0}}, f.Amfa, 0, true, nullptr, nullptr);
@@ -638,14 +592,10 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     }
     {
         // global stats -> per-utterance bias of the attention TDNN: its weight [att][3*C3], columns C3.. multiply [mean | std]
-        push(colstats_step(f.M, C3, B, T, P, Tp, 1, TR_ASP_EPS, f.gstat_pl));
-        PlanStep s = model(TR_PLANES_TO_F32);
-        s.x = f.gstat_pl;
-        s.C = 2 * C3;
-        s.T = s.Tp = 1;  // one row per utterance
-        s.P = 0;
-        s.f32 = {f.gstat};
-        push(s);
+        t->steps.push_back(colstats_step(f.M, C3, B, T, P, Tp, 1, TR_ASP_EPS, f.gstat_pl));
+        push("launch_planes_to_f32", [x = f.gstat_pl, Cn = 2 * C3, B, out = f.gstat](const StepRun& r) {
+            return launch_planes_to_f32(x, 0, Cn, B, 1, 0, 1, out, r.st);  // one row per utterance
+        });
         dense_fwd(f.gstat, 2 * C3, par + t->L[t->l_att1].conv.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, f.fold, att);
     }
     {
@@ -657,48 +607,40 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     }
     {
         // softmax pooling, asp_bn (batch statistics), fc, AAM-softmax loss
-        PlanStep s = model(TR_ASP_POOL);
-        s.vec = {f.logits};
-        s.dim = {C3};
-        s.x = f.M;
-        s.C = C3;
-        s.f32 = {f.pooled};
-        push(s);
-        s = model(TR_BN1D_FWD);
-        s.vec = {f.pooled, par + t->aspbn_g, par + t->aspbn_b};
-        s.C = 2 * C3;
-        s.f32 = {f.pn, f.aspbn_mean, f.aspbn_rstd, sta + t->aspbn_rm, sta + t->aspbn_rv};
-        push(s);
+        push("launch_asp_pool", [logits = f.logits, C3, x = f.M, B, T, P, Tp, pooled = f.pooled](const StepRun& r) {
+            return launch_asp_pool(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), pooled, r.st);
+        });
+        push("tr_bn1d_fwd", [x = f.pooled, B, Cn = 2 * C3, gamma = par + t->aspbn_g, beta = par + t->aspbn_b, y = f.pn, mean = f.aspbn_mean,
+                             rstd = f.aspbn_rstd, run_mean = sta + t->aspbn_rm, run_var = sta + t->aspbn_rv](const StepRun& r) {
+            return tr_bn1d_fwd(x, B, Cn, TR_BN_EPS, TR_BN_MOMENTUM, gamma, beta, y, mean, rstd, run_mean, run_var, r.st);
+        });
         dense_fwd(f.pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, f.emb, D);
-        s = model(TR_AAM_FWD);
-        s.vec = {f.emb, par + t->cls_w};
-        s.dim = {D, t->S, int64_t(f.aam_ws_bytes)};
-        s.f32 = {f.cls_logits, f.loss, f.aam_ws};
-        push(s);
+        push("aam_forward", [emb = f.emb, cls_w = par + t->cls_w, B, D, S = t->S, logits = f.cls_logits, loss = f.loss, aam_ws = f.aam_ws,
+                             aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
+            const PlanInputs& in = r.in;
+            return aam_forward(emb, cls_w, in.labels, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, logits, loss, aam_ws,
+                               aam_ws_bytes, r.st);
+        });
     }
 
     // ================================================================= backward
     {
         // AAM, fc, asp_bn -> dpooled; ASP -> dlogits, dMd
-        PlanStep s = model(TR_AAM_BWD);
-        s.vec = {f.emb, par + t->cls_w, f.cls_logits};
-        s.dim = {D, t->S, int64_t(f.aam_ws_bytes)};
-        s.f32 = {f.d_emb, grd + t->cls_w, f.aam_ws};
-        push(s);
+        push("aam_backward", [emb = f.emb, cls_w = par + t->cls_w, logits = f.cls_logits, B, D, S = t->S, d_emb = f.d_emb, d_cls_w = grd + t->cls_w,
+                              aam_ws = f.aam_ws, aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
+            const PlanInputs& in = r.in;
+            return aam_backward(emb, cls_w, in.labels, logits, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, d_emb, d_cls_w,
+                                aam_ws, aam_ws_bytes, r.st);
+        });
         dense_bwd(f.d_emb, D, f.pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, f.dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b);
-        s = model(TR_BN1D_BWD);
-        s.vec = {f.dpn, f.pooled, par + t->aspbn_g, f.aspbn_mean, f.aspbn_rstd};
-        s.C = 2 * C3;
-        s.f32 = {f.dpooled, grd + t->aspbn_g, grd + t->aspbn_b};
-        push(s);
-        s = model(TR_ASP_BWD);
-        s.vec = {f.logits, f.pooled, f.dpooled};
-        s.dim = {C3};
-        s.x = f.M;
-        s.C = C3;
-        s.out = f.dlogits;
-        s.t = f.dMd;
-        push(s);
+        push("tr_bn1d_bwd", [dy = f.dpn, x = f.pooled, B, Cn = 2 * C3, gamma = par + t->aspbn_g, mean = f.aspbn_mean, rstd = f.aspbn_rstd,
+                             dx = f.dpooled, dgamma = grd + t->aspbn_g, dbeta = grd + t->aspbn_b](const StepRun& r) {
+            return tr_bn1d_bwd(dy, x, B, Cn, gamma, mean, rstd, dx, dgamma, dbeta, r.st);
+        });
+        push("tr_asp_bwd", [logits = f.logits, C3, x = f.M, B, T, P, Tp, pooled = f.pooled, dpooled = f.dpooled, dlogits = f.dlogits,
+                            dx = f.dMd](const StepRun& r) {
+            return tr_asp_bwd(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, pooled, dpooled, dlogits, dx, r.st);
+        });
     }
     {
         // asp.conv: bias, weight, data gradients
@@ -721,11 +663,9 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         bn_bwd(t->l_att1, gl, f.Aatt, 0, f.dZatt, 0);
         const TConv& c = t->L[t->l_att1].conv;
         dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3, nullptr);
-        PlanStep s = model(TR_ASP_GLOBAL_BWD);
-        s.vec = {f.gstat, f.dgs};
-        s.C = C3;
-        s.f32 = {f.rs, f.rb};
-        push(s);
+        push("tr_asp_global_bwd", [gstat = f.gstat, dgs = f.dgs, B, C3, T, rs = f.rs, rb = f.rb](const StepRun& r) {
+            return tr_asp_global_bwd(gstat, dgs, B, C3, T, TR_ASP_EPS, rs, rb, r.st);
+        });
         rc = wgrad(t->l_att1, f.dZatt, 0, {{f.M, 0, C3, 0}});
         if (rc) return rc;
         rc = dgrad_gemm(t->l_att1, f.dZatt, 0, f.dMatt, 0);
@@ -765,13 +705,12 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         }
         {
             // SE backward -> dg2 ... ds (scaled by 1/T), SE weight gradients
-            PlanStep s = model(TR_GRAD_DOT);
-            s.gl.n = 1;
-            s.gl.s[0].t = Dg;
-            s.x = f.Yt2[b];
-            s.C = C;
-            s.f32 = {f.dg2};
-            push(s);
+            GradSrcList gl;
+            gl.n = 1;
+            gl.s[0].t = Dg;
+            push("tr_grad_dot", [gl, y = f.Yt2[b], C, B, T, P, Tp, out = f.dg2](const StepRun& r) {
+                return tr_grad_dot(gl, y, 0, C, B, T, P, Tp, out, r.st);
+            });
             act_bwd(f.dg2, f.se_g2[b], int64_t(B) * C, 2, 0.f);
             dense_bwd(f.dg2, C, f.se_g1[b], se, par + t->se2_w[b], se, B, C, se, f.dg1, se, grd + t->se2_w[b], se, grd + t->se2_b[b]);
             act_bwd(f.dg1, f.se_g1[b], int64_t(B) * se, 1, 0.f);
@@ -836,42 +775,6 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     return PPV_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ step
-int Trainer::run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st) {
-    const auto& v = s.vec;
-    const auto& o = s.f32;
-    const auto& d = s.dim;
-    switch (s.model_kind) {
-        case TR_REPACK: return tr_repack_conv(v[0], d[0], d[1], d[2], d[3], d[4], s.x, s.y, st);
-        case TR_PACK: return launch_pack_features(in.feat, s.B, s.T, s.C, s.out, s.P, s.Tp, st);
-        case TR_BN_FWD:
-            return tr_bn_forward(s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, TR_BN_EPS, TR_BN_MOMENTUM, v[0], v[1], o[0], o[1], o[2], o[3], o[4], o[5], o[6],
-                                 s.apply, num_sms, st);
-        case TR_DENSE_FWD: return tr_dense_fwd(v[0], d[0], v[1], d[1], v[2], d[2], d[3], d[4], d[5], o[0], d[6], st);
-        case TR_PLANES_TO_F32: return launch_planes_to_f32(s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, o[0], st);
-        case TR_ASP_POOL: return launch_asp_pool(v[0], d[0], s.x, s.C, s.B, s.T, s.P, s.Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), o[0], st);
-        case TR_BN1D_FWD: return tr_bn1d_fwd(v[0], s.B, s.C, TR_BN_EPS, TR_BN_MOMENTUM, v[1], v[2], o[0], o[1], o[2], o[3], o[4], st);
-        case TR_AAM_FWD:
-            return aam_forward(v[0], v[1], in.labels, s.B, d[0], d[1], in.margin, in.scale, in.easy_margin, in.label_smoothing, o[0], o[1], o[2],
-                               d[2], st);
-        case TR_AAM_BWD:
-            return aam_backward(v[0], v[1], in.labels, v[2], s.B, d[0], d[1], in.margin, in.scale, in.easy_margin, in.label_smoothing, o[0], o[1],
-                                o[2], d[2], st);
-        case TR_DENSE_BWD: return tr_dense_bwd(v[0], d[0], v[1], d[1], v[2], d[2], d[3], d[4], d[5], o[0], d[6], o[1], d[7], o[2], st);
-        case TR_BN1D_BWD: return tr_bn1d_bwd(v[0], v[1], s.B, s.C, v[2], v[3], v[4], o[0], o[1], o[2], st);
-        case TR_ASP_BWD: return tr_asp_bwd(v[0], d[0], s.x, s.C, s.B, s.T, s.P, s.Tp, TR_ASP_EPS, v[1], v[2], s.out, s.t, st);
-        case TR_GRAD_SUM: return tr_grad_sum(s.gl, s.C, s.B, s.T, s.P, s.Tp, s.out, s.oc0, o[0], o[1], st);
-        case TR_BN_BWD:
-            return tr_bn_backward(s.gl, s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, v[0], v[1], v[2], o[0], o[1], s.out, s.oc0, o[2], o[3], d[0], st, d[1]);
-        case TR_TRANSPOSE: return tr_transpose(s.x, s.xc0, s.C, s.rows, s.out, d[0], st, d[1], d[2], d[3]);
-        case TR_WGRAD_UNPACK: return tr_wgrad_unpack(v[0], d[0], d[1], d[2], d[3], d[4], d[5], o[0], d[6], st);
-        case TR_ASP_GLOBAL_BWD: return tr_asp_global_bwd(v[0], v[1], s.B, s.C, s.T, TR_ASP_EPS, o[0], o[1], st);
-        case TR_GRAD_DOT: return tr_grad_dot(s.gl, s.x, s.xc0, s.C, s.B, s.T, s.P, s.Tp, o[0], st);
-        case TR_ACT_BWD: return tr_act_bwd(o[0], v[0], d[0], d[1], s.inv_count, st);
-    }
-    return PlanOwner::run_model_step(s, in, st);
-}
-
 int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* labels, int B, int T, float margin, float scale, int easy_margin,
                              float label_smoothing, float* loss_out, float* logits_out, void* ws, size_t ws_bytes, cudaStream_t st) {
     PPV_REQUIRE(t && feat && labels, "trainer_forward_backward: null argument");
@@ -907,11 +810,11 @@ int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems,
         PPV_REQUIRE(b < 3, "trainer_read_tap: bad block");
     }
     const auto it = t->taps.find(n);
-    if (it == t->taps.end() || (b >= 0 && !it->second.per_block) || (padded && it->second.f32))
+    if (it == t->taps.end() || (b >= 0 && !it->second.per_block) || (padded && it->second.fp32))
         return fail(PPV_EINVAL, std::string("trainer_read_tap: unknown tap ") + name);
     const TrTap& e = it->second;
     const int bk = std::max(b, 0);
-    if (e.f32) {
+    if (e.fp32) {
         PPV_REQUIRE(out_elems >= e.count, "trainer_read_tap: output too small");
         PPV_CUDA_OK(cudaMemcpyAsync(out, e.vec[bk], e.count * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return PPV_OK;

@@ -158,11 +158,10 @@ int PlanModel::plan_conv3x3(const GemmWeights& gw, const Planes& x, int col0, in
         return plan_gemm(gw, taps, int(g.rows(B)), ep);
     }
     ep.bias = gw.bias;
-    PlanStep s;
-    s.kind = PlanStep::CONV3X3;
-    int rc = conv3x3_build(&s.c3, x, col0, gw.W, B, g.H, g.W, g.Hp, g.Wp, ep);
+    Conv3x3Params c3;
+    int rc = conv3x3_build(&c3, x, col0, gw.W, B, g.H, g.W, g.Hp, g.Wp, ep);
     if (rc) return rc;
-    steps.push_back(s);
+    steps.push_back({"conv3x3_launch", true, [c3](const StepRun& r) { return conv3x3_launch(c3, r.precision, r.num_sms, r.st); }});
     return PPV_OK;
 }
 

@@ -4,170 +4,94 @@
 namespace ppv {
 
 // ------------------------------------------------------------------------------------------------ steps
+PlanStep gemm_step(const GemmParams& gp) {
+    return {"gemm_launch", true, [gp](const StepRun& r) { return gemm_launch(gp, r.precision, r.num_sms, r.st); }};
+}
 PlanStep stem_step(const float* w9, const float* bias, int C0, const Planes& out, const ImageGeo& g, int B) {
-    PlanStep s;
-    s.kind = PlanStep::STEM;
-    s.vec[0] = w9;
-    s.vec[1] = bias;
-    s.C = C0;
-    s.out = out;
-    s.g = g;
-    s.B = B;
-    return s;
+    return {"launch_stem_conv", false,
+            [w9, bias, C0, out, g, B](const StepRun& r) { return launch_stem_conv(r.in.feat, B, g.W, g.H, w9, bias, C0, out, g.Hp, g.Wp, r.st); }};
 }
 PlanStep scale_res_step(const Planes& z, const float* scale, const Planes& res, int rc0, const Planes& out, int oc0, int C, int rows_per_utt,
                         int64_t rows, bool relu, float relu_max) {
-    PlanStep s;
-    s.kind = PlanStep::SCALE_RES;
-    s.x = z;
-    s.vec[0] = scale;
-    s.y = res;
-    s.yc0 = rc0;
-    s.out = out;
-    s.oc0 = oc0;
-    s.C = C;
-    s.utt_rows = rows_per_utt;
-    s.rows = rows;
-    s.relu = relu;
-    s.relu_max = relu_max;
-    return s;
+    return {"launch_se_scale_res", false, [z, scale, res, rc0, out, oc0, C, rows_per_utt, rows, relu, relu_max](const StepRun& r) {
+                return launch_se_scale_res(z, scale, res, rc0, out, oc0, C, rows_per_utt, rows, r.num_sms, r.st, relu ? 1 : 0, relu_max);
+            }};
 }
 PlanStep aff_combine_step(const Planes& x, int xc0, const Planes& y, int yc0, const Planes& t, const Planes& out, int C, int64_t rows) {
-    PlanStep s;
-    s.kind = PlanStep::AFF_COMBINE;
-    s.x = x;
-    s.xc0 = xc0;
-    s.y = y;
-    s.yc0 = yc0;
-    s.t = t;
-    s.out = out;
-    s.C = C;
-    s.rows = rows;
-    return s;
+    return {"launch_aff_combine", false, [x, xc0, y, yc0, t, out, C, rows](const StepRun& r) {
+                return launch_aff_combine(x, xc0, y, yc0, t, out, C, rows, r.num_sms, r.st);
+            }};
 }
 PlanStep flatten_step(const Planes& in, const ImageGeo& g, int B, int C, const Planes& out) {
-    PlanStep s;
-    s.kind = PlanStep::FLATTEN_IMAGE;
-    s.x = in;
-    s.g = g;
-    s.B = B;
-    s.C = C;
-    s.out = out;
-    return s;
+    return {"launch_flatten_image", false,
+            [in, g, B, C, out](const StepRun& r) { return launch_flatten_image(in, B, g.H, g.W, g.Hp, g.Wp, C, out, r.num_sms, r.st); }};
 }
-PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int mode, float eps, const Planes& out, float inv_count, bool masked) {
-    PlanStep s;
-    s.kind = PlanStep::COLSTATS;
-    s.x = x;
-    s.C = C;
-    s.B = B;
-    s.T = T;
-    s.P = P;
-    s.Tp = Tp;
-    s.mode = mode;
-    s.eps = eps;
-    s.out = out;
-    s.inv_count = inv_count;
-    s.masked = masked;
-    return s;
-}
-PlanStep model_step(int model_kind) {
-    PlanStep s;
-    s.kind = PlanStep::MODEL;
-    s.model_kind = model_kind;
-    return s;
+PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int mode, float eps, const Planes& out, float inv_count, bool masked,
+                       float* out_f32) {
+    return {"launch_colstats", false, [x, C, B, T, P, Tp, mode, eps, out, inv_count, masked, out_f32](const StepRun& r) {
+                return launch_colstats(x, 0, C, B, T, P, Tp, mode, eps, out_f32, out, r.st, inv_count, masked ? r.in.nvalid : nullptr);
+            }};
 }
 
 // ------------------------------------------------------------------------------------------------ routing
 int PlanModel::plan_gemm(const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) {
     ep.bias = gw.bias;
-    PlanStep s;
-    s.kind = PlanStep::GEMM;
-    int rc = gemm_build(&s.gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N, max_bn));
+    GemmParams gp;
+    int rc = gemm_build(&gp, srcs.data(), int(srcs.size()), gw.W, M, gw.N, ep, gemm_pick_bn(gw.N, max_bn));
     if (rc) return rc;
-    steps.push_back(s);
+    steps.push_back(gemm_step(gp));
     return PPV_OK;
 }
 
 int PlanModel::plan_conv(const GemmWeights& gw, const std::vector<GemmSource>& srcs, int M, Epilogue ep) {
     ep.bias = gw.bias;
-    PlanStep s;
-    if (!pointwise_step_build(&s.pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) return plan_gemm(gw, srcs, M, ep);
-    s.kind = PlanStep::POINTWISE;
-    steps.push_back(s);
+    PwStep pw;
+    if (!pointwise_step_build(&pw, srcs.data(), int(srcs.size()), gw.W, gw.N, M, ep)) return plan_gemm(gw, srcs, M, ep);
+    steps.push_back({"pointwise_launch", false, [pw](const StepRun& r) { return pointwise_launch(pw, r.num_sms, r.st); }});
     return PPV_OK;
 }
 
 int PlanModel::plan_row_linear(const GemmWeights& gw, const GemmSource& src, int M, Epilogue ep) {
     ep.bias = gw.bias;
     if (src.row_off != 0 || gw.Ktot != src.ncols || !skinny_linear_supported(M, gw.N, src.ncols, ep)) return plan_gemm(gw, {src}, M, ep);
-    PlanStep s;
-    s.kind = PlanStep::SKINNY;
-    s.pw.srcs[0] = src;
-    s.pw.nsrc = 1;
-    s.pw.W = gw.W;
-    s.pw.M = M;
-    s.pw.N = gw.N;
-    s.pw.ep = ep;
-    steps.push_back(s);
+    steps.push_back({"skinny_linear_launch", false, [x = src.t, col0 = src.col0, W = gw.W, M, N = gw.N, K = src.ncols, ep](const StepRun& r) {
+                         return skinny_linear_launch(x, col0, W, M, N, K, ep, r.st);
+                     }});
+    return PPV_OK;
+}
+
+int PlanModel::plan_asp_fused(const Planes& W, const Planes& att, const Planes& x, const float* bn_scale, const float* bn_shift,
+                              const Planes& out, float* out_raw, int B, int T, int P, int Tp, int C, int K, float eps) {
+    AspFusedParams ap;
+    int rc = asp_fused_build(&ap, W, att, x, bn_scale, bn_shift, out, out_raw, B, T, P, Tp, C, K, eps);
+    if (rc) return rc;
+    steps.push_back({"asp_fused_launch", true, [ap](const StepRun& r) {
+                         AspFusedParams p = ap;
+                         p.nvalid = r.in.nvalid;
+                         return asp_fused_launch(p, r.precision, r.num_sms, r.st);
+                     }});
     return PPV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ executor
 int PlanOwner::run_plan(const PlanInputs& in, cudaStream_t st) {
+    const StepRun run{in, precision, num_sms, st};
     for (size_t i = 0; i < steps.size(); ++i) {
         const PlanStep& s = steps[i];
-        const bool tensor_step = s.kind == PlanStep::GEMM || s.kind == PlanStep::CONV3X3 || s.kind == PlanStep::RES2 ||
-                                 s.kind == PlanStep::RES2CHAIN || s.kind == PlanStep::ASP_FUSED;
-        // (SKINNY and POINTWISE steps count as "other kernels": their FLOPs are not credited to the tensor-core roofline)
-        prof_begin(tensor_step ? 0 : 1, st);
-        if (tensor_step) launches_gemm += 1; else launches_other += 1;
-        int rc = PPV_OK;
-        switch (s.kind) {
-            case PlanStep::GEMM: rc = gemm_launch(s.gp, precision, num_sms, st); break;
-            case PlanStep::SKINNY:
-                rc = skinny_linear_launch(s.pw.srcs[0].t, s.pw.srcs[0].col0, s.pw.W, int(s.pw.M), s.pw.N, s.pw.srcs[0].ncols, s.pw.ep, st);
-                break;
-            case PlanStep::RES2: rc = res2conv_launch(s.rp, precision, num_sms, st); break;
-            case PlanStep::RES2CHAIN:
-                rc = res2chain_launch(s.cp, precision, num_sms, st);
-                if (s.cp.trace) {
-                    static int dumps = 0;
-                    if (++dumps == 10) res2chain_trace_dump(s.cp);  // a warm launch of the first block
-                }
-                break;
-            case PlanStep::CONV3X3: rc = conv3x3_launch(s.c3, precision, num_sms, st); break;
-            case PlanStep::POINTWISE: rc = pointwise_launch(s.pw, num_sms, st); break;
-            case PlanStep::STEM: rc = launch_stem_conv(in.feat, s.B, s.g.W, s.g.H, s.vec[0], s.vec[1], s.C, s.out, s.g.Hp, s.g.Wp, st); break;
-            case PlanStep::SCALE_RES:
-                rc = launch_se_scale_res(s.x, s.vec[0], s.y, s.yc0, s.out, s.oc0, s.C, s.utt_rows, s.rows, num_sms, st, s.relu ? 1 : 0, s.relu_max);
-                break;
-            case PlanStep::AFF_COMBINE: rc = launch_aff_combine(s.x, s.xc0, s.y, s.yc0, s.t, s.out, s.C, s.rows, num_sms, st); break;
-            case PlanStep::FLATTEN_IMAGE: rc = launch_flatten_image(s.x, s.B, s.g.H, s.g.W, s.g.Hp, s.g.Wp, s.C, s.out, num_sms, st); break;
-            case PlanStep::COLSTATS:
-                rc = launch_colstats(s.x, 0, s.C, s.B, s.T, s.P, s.Tp, s.mode, s.eps, s.out_f32, s.out, st, s.inv_count, s.masked ? in.nvalid : nullptr);
-                break;
-            case PlanStep::ASP_FUSED: {
-                AspFusedParams ap = s.ap;
-                ap.nvalid = in.nvalid;
-                rc = asp_fused_launch(ap, precision, num_sms, st);
-                break;
-            }
-            case PlanStep::MODEL: rc = run_model_step(s, in, st); break;
-        }
+        // (skinny and pointwise steps count as "other kernels": their FLOPs are not credited to the tensor-core roofline)
+        prof_begin(s.tensor ? 0 : 1, st);
+        if (s.tensor) launches_gemm += 1; else launches_other += 1;
+        const int rc = s.launch(run);
         prof_end(st);
         if (rc) return rc;
         if (sync_each_step) {
             const cudaError_t e = cudaStreamSynchronize(st);
-            const std::string model = s.kind == PlanStep::MODEL ? ", model kind " + std::to_string(s.model_kind) : "";
             if (e != cudaSuccess)
-                return fail(PPV_ECUDA, std::string(prefix) + ": step " + std::to_string(i) + " (kind " + std::to_string(int(s.kind)) + model + ") failed: " + cudaGetErrorString(e));
+                return fail(PPV_ECUDA, std::string(prefix) + ": step " + std::to_string(i) + " (" + s.name + ") failed: " + cudaGetErrorString(e));
         }
     }
     return PPV_OK;
 }
-
-int PlanOwner::run_model_step(const PlanStep&, const PlanInputs&, cudaStream_t) { return fail(PPV_EINVAL, std::string(prefix) + ": plan step of unknown kind"); }
 
 // ------------------------------------------------------------------------------------------------ profile
 PlanOwner::~PlanOwner() {

@@ -1,68 +1,56 @@
 // The plans, in one place (plan.cu): ECAPA-TDNN, ResNetSE, ERes2Net(V2) and CAM++ each plan their forward, and the ECAPA-TDNN
-// trainer its training step, as a list of PlanSteps, each holding every argument of its launch; PlanOwner::run_plan launches them in
-// order.  The routing helpers choose a layer's kernel; what is about zero-bordered image grids (the 2-D models) is in image_plan.h.
+// trainer its training step, as a list of PlanSteps, each a launch with its arguments bound when the plan is built; PlanOwner::run_plan
+// launches them in order.  The routing helpers choose a layer's kernel; what is about zero-bordered image grids (the 2-D models) is in
+// image_plan.h.
 #pragma once
-#include <array>
+#include <functional>
 #include <string>
 #include <vector>
 
 #include "common.h"
 #include "model_common.h"
-#include "train.h"
 
 namespace ppv {
-
-struct PlanStep {
-    enum Kind { GEMM, SKINNY, RES2, RES2CHAIN, CONV3X3, POINTWISE, STEM, SCALE_RES, AFF_COMBINE, FLATTEN_IMAGE, COLSTATS, ASP_FUSED, MODEL } kind;
-    int model_kind = 0;   // MODEL: a model's own step, launched by its run_model_step
-    GemmParams gp;        // GEMM
-    Res2Params rp;        // RES2
-    Res2ChainParams cp;   // RES2CHAIN
-    Conv3x3Params c3;     // CONV3X3
-    PwStep pw;            // POINTWISE; SKINNY: srcs[0] is the input, its ncols the K
-    AspFusedParams ap;    // ASP_FUSED; nvalid is set per launch
-    // STEM: feat -> out on grid g, weights vec[0] / vec[1], C0 = C;
-    // SCALE_RES: out[:, oc0 + c] = x[:, c] * vec[0][utterance][c] + y[:, yc0 + c] (vec[0] null: no scale), then, if relu, ReLU clipped
-    // at relu_max > 0, over `rows` rows of utt_rows rows per utterance (Tp frames, or an image's Hp x Wp grid);
-    // AFF_COMBINE: out = x (1 + t) + y (1 - t) over `rows`;  FLATTEN_IMAGE: x on grid g -> out;
-    // COLSTATS: launch_colstats of x's first C columns into the planes `out` or, if set, out_f32, over each utterance's first nvalid
-    // frames if `masked` and the run has them;  MODEL: what the model puts here.
-    Planes x, y, t, out;
-    int xc0 = 0, yc0 = 0, oc0 = 0;
-    std::array<const float*, 6> vec{};
-    float* out_f32 = nullptr;
-    ImageGeo g;
-    int B = 0, C = 0, T = 0, P = 0, Tp = 0, mode = 0, n = 0;
-    int64_t rows = 0;
-    int utt_rows = 0;
-    float eps = 0.f, inv_count = 0.f, relu_max = 0.f;
-    bool relu = false, masked = false;
-    // The trainer's MODEL steps (ecapa_train.cu) take their launcher's arguments from the fields above and these: the Planes it reads
-    // from x, y (column offsets xc0, yc0) and those it writes from out, t (oc0); the fp32 arrays it reads from vec and those it writes
-    // from f32, each in the launcher's order; B, C, T, P, Tp; every other integer from dim, in the launcher's order.
-    std::array<float*, 8> f32{};
-    std::array<int64_t, 8> dim{};
-    GradSrcList gl;
-    BnApplyArgs apply;
-};
-
-PlanStep stem_step(const float* w9, const float* bias, int C0, const Planes& out, const ImageGeo& g, int B);
-PlanStep scale_res_step(const Planes& z, const float* scale, const Planes& res, int rc0, const Planes& out, int oc0, int C, int rows_per_utt,
-                        int64_t rows, bool relu, float relu_max = 0.f);
-PlanStep aff_combine_step(const Planes& x, int xc0, const Planes& y, int yc0, const Planes& t, const Planes& out, int C, int64_t rows);
-PlanStep flatten_step(const Planes& in, const ImageGeo& g, int B, int C, const Planes& out);
-PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int mode, float eps, const Planes& out, float inv_count = 0.f,
-                       bool masked = false);
-PlanStep model_step(int model_kind);
 
 // What a run of a plan reads besides the plan itself.
 struct PlanInputs {
     const float* feat = nullptr;      // features [plan_B, plan_T, input_size]
-    const int* nvalid = nullptr;      // inference: [plan_B] valid-frame counts for masked COLSTATS and ASP_FUSED steps (null: every frame)
+    const int* nvalid = nullptr;      // inference: [plan_B] valid-frame counts for masked column statistics and fused ASP (null: every frame)
     const int64_t* labels = nullptr;  // training: [plan_B] class labels and the AAM-softmax settings
     float margin = 0.f, scale = 0.f, label_smoothing = 0.f;
     int easy_margin = 0;
 };
+
+// What only the run knows.  Precision is one of them: set_precision switches a live plan without rebuilding it.
+struct StepRun {
+    const PlanInputs& in;
+    int precision, num_sms;
+    cudaStream_t st;
+};
+
+// One launch of a plan.  `launch` owns copies of every argument the plan fixes (its closure captures values only: the builder's
+// locals are gone when it runs) and takes the rest from the run.
+struct PlanStep {
+    const char* name;  // the launcher; named when a step fails under sync_each_step
+    bool tensor;       // the launch profile's tensor-core class: GEMM, 3x3 conv, Res2Net conv / chain, fused ASP
+    std::function<int(const StepRun&)> launch;
+};
+
+PlanStep gemm_step(const GemmParams& gp);  // a gather-GEMM built by gemm_build or gemm_build_wgrad
+// feat -> out on grid g: the 1 -> C0 channel stem conv
+PlanStep stem_step(const float* w9, const float* bias, int C0, const Planes& out, const ImageGeo& g, int B);
+// out[:, oc0 + c] = z[:, c] * scale[utterance][c] + res[:, rc0 + c] (scale null: no scale), then, if relu, ReLU clipped at relu_max > 0,
+// over `rows` rows of rows_per_utt rows per utterance (Tp frames, or an image's Hp x Wp grid)
+PlanStep scale_res_step(const Planes& z, const float* scale, const Planes& res, int rc0, const Planes& out, int oc0, int C, int rows_per_utt,
+                        int64_t rows, bool relu, float relu_max = 0.f);
+// out = x (1 + t) + y (1 - t) over `rows`
+PlanStep aff_combine_step(const Planes& x, int xc0, const Planes& y, int yc0, const Planes& t, const Planes& out, int C, int64_t rows);
+// `in` on grid g -> time-major `out`
+PlanStep flatten_step(const Planes& in, const ImageGeo& g, int B, int C, const Planes& out);
+// launch_colstats of x's first C columns into the planes `out` or, if set, out_f32, over each utterance's first nvalid frames if
+// `masked` and the run has them
+PlanStep colstats_step(const Planes& x, int C, int B, int T, int P, int Tp, int mode, float eps, const Planes& out, float inv_count = 0.f,
+                       bool masked = false, float* out_f32 = nullptr);
 
 // A plan of launches over a caller-owned workspace, built for (workspace, B, T) and rebuilt whenever one of them changes: the
 // inference models and the training step.
@@ -101,7 +89,7 @@ struct PlanOwner {
     }
 
     // Launch profile (ppv_model_profile): with it on, run_plan records a CUDA event pair around each launch group; the launch counters
-    // count every run.  Tensor-core steps (GEMM, CONV3X3, RES2, RES2CHAIN, ASP_FUSED) are one kind, every other launch the other.
+    // count every run.  Tensor-core steps (PlanStep::tensor) are one kind, every other launch the other.
     void profile(bool enable);
     // Sums the event-pair durations recorded since profile(true) by kind, synchronising on the last event, and resets the record.
     int profile_read(double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches);
@@ -120,7 +108,6 @@ struct PlanOwner {
     virtual int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) = 0;
     // The executor: launches the planned steps in order.
     int run_plan(const PlanInputs& in, cudaStream_t st);
-    virtual int run_model_step(const PlanStep& s, const PlanInputs& in, cudaStream_t st);
     // an event pair around launches of kind 0 (tensor cores) or 1 (other), recorded while the profile is on
     void prof_begin(int kind, cudaStream_t st);
     void prof_end(cudaStream_t st);
@@ -214,6 +201,9 @@ struct PlanModel : Model {
     // CTAs walking a latency-bound k-loop on the tensor cores.  The caller guarantees the one row per utterance: the skinny kernel
     // reads plain rows, with no padded time layout and no halo, so a per-frame layer goes to plan_gemm.
     int plan_row_linear(const GemmWeights& gw, const GemmSource& src, int M, Epilogue ep);
+    // Attentive statistics pooling in one kernel (asp_fused_build's arguments); the run supplies the valid-frame counts.
+    int plan_asp_fused(const Planes& W, const Planes& att, const Planes& x, const float* bn_scale, const float* bn_shift, const Planes& out,
+                       float* out_raw, int B, int T, int P, int Tp, int C, int K, float eps);
 
     // image-grid helpers (image_plan.cu)
     // 3x3 conv over columns [col0, col0 + ncols) of x on grid g: the patch kernel for a 32 -> 32 channel conv, else nine taps

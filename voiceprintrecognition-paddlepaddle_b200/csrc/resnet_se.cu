@@ -328,14 +328,8 @@ int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
         rc = plan_gemm(m->att1, {GemmSource{rb.flat, 0, cat, 0}}, B * Tf, ep);
         if (rc) return rc;
     }
-    {
-        PlanStep s;
-        s.kind = PlanStep::ASP_FUSED;
-        rc = asp_fused_build(&s.ap, m->att2.W, rb.attp, rb.flat, m->bn2_scale, m->bn2_shift, rb.pooled, rb.pooled_raw, B, Tf, 0, Tf, cat,
-                             m->att, 1e-12f);
-        if (rc) return rc;
-        m->steps.push_back(s);
-    }
+    rc = plan_asp_fused(m->att2.W, rb.attp, rb.flat, m->bn2_scale, m->bn2_shift, rb.pooled, rb.pooled_raw, B, Tf, 0, Tf, cat, m->att, 1e-12f);
+    if (rc) return rc;
     {
         Epilogue ep;
         ep.out_mode = OUT_F32;
