@@ -319,6 +319,28 @@ int ppv_eer_mindcf_matrix(const float* scores, const int32_t* trial_labels, cons
 int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* best, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Speaker index: the enrolment database's per-user mean embeddings, searched by cosine top-k.  Replaces the per-user mean loop of
+ * ppvector/predict.py:154-163 (__load_audio_db; register :311-320 and remove_user :360-362 update the same means) and the
+ * retrieval of :173-187 (__retrieval: sklearn cosine_similarity of the normalised queries against the means, then numpy.argmax).
+ * The index is an opaque device buffer of ppv_speaker_index_bytes(U, D) bytes, 256-byte aligned, written by
+ * ppv_speaker_index_build and read by ppv_speaker_index_search; its layout belongs to the library.  Limits: 1 <= D <= 256,
+ * U >= 1, Q >= 1, 1 <= k <= min(8, U); anything else is PPV_EINVAL.
+ * ------------------------------------------------------------------------------------------- */
+/* Bytes of the index of U users of dimension D (0 when out of range). */
+size_t ppv_speaker_index_bytes(int U, int D);
+/* E [n, D] fp32 enrolment embeddings; order [n] int32 = row indices grouped by user (enrolment order within a user), offsets [U+1]
+ * int32 (user u owns order[offsets[u] .. offsets[u+1]), every user at least one row) -> means [U, D] fp32, each the fp32 sum of the
+ * user's rows in that order divided by the count (bitwise numpy's E[rows].mean(axis=0)), and the index.  Deterministic; one launch. */
+int ppv_speaker_index_build(const float* E, int n, int D, const int32_t* order, const int32_t* offsets, int U, float* means, void* index,
+                            size_t index_bytes, void* stream);
+/* Scratch of ppv_speaker_index_search, 256-byte aligned: O(Q * k * splits), never O(Q * U). */
+size_t ppv_speaker_index_search_workspace_bytes(int Q, int U, int D, int k);
+/* queries [Q, D] fp32 -> idx [Q, k] int32, sim [Q, k] fp32: per query the k users of highest cosine similarity, descending, equal
+ * similarities lowest index first (k = 1: numpy.argmax's first maximum).  A zero-norm query or mean scores 0.  Deterministic. */
+int ppv_speaker_index_search(const float* queries, int Q, int D, const void* index, size_t index_bytes, int U, int k, int32_t* idx,
+                             float* sim, void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Speaker diarization: spectral clustering of the chunk embeddings.  Replaces
  * ppvector/infer_utils/speaker_diarization.py:219-310 (SpectralCluster: pruning, Laplacian, scipy.linalg.eigh,
  * sklearn k_means).  The affinity is ppv_cosine_matrix of the [N, D] embeddings.  One stage per entry point, so that each

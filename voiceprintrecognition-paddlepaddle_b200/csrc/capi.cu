@@ -267,6 +267,26 @@ int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* be
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- speaker index
+size_t ppv_speaker_index_bytes(int U, int D) { return speaker_index_bytes(U, D); }
+int ppv_speaker_index_build(const float* E, int n, int D, const int32_t* order, const int32_t* offsets, int U, float* means, void* index,
+                            size_t index_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    int rc = check_device();
+    if (rc) return rc;
+    return speaker_index_build(E, n, D, order, offsets, U, means, index, index_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+size_t ppv_speaker_index_search_workspace_bytes(int Q, int U, int D, int k) { return speaker_index_search_workspace_bytes(Q, U, D, k); }
+int ppv_speaker_index_search(const float* queries, int Q, int D, const void* index, size_t index_bytes, int U, int k, int32_t* idx,
+                             float* sim, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    int rc = check_device();
+    if (rc) return rc;
+    return speaker_index_search(queries, Q, D, index, index_bytes, U, k, idx, sim, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+
 // ---------------------------------------------------------------- speaker diarization
 int ppv_cluster_prune(float* affinity, int N, double pval, void* stream) {
     PPV_GUARD_BEGIN

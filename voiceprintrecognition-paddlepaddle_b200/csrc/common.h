@@ -408,6 +408,14 @@ int aam_backward(const float* emb, const float* W, const int64_t* labels, const 
                  float scale, int easy_margin, float label_smoothing, float* d_emb, float* d_W, void* ws, size_t ws_bytes,
                  cudaStream_t st);
 
+// ---- speaker_index.cu ---------------------------------------------------------------------------------
+size_t speaker_index_bytes(int U, int D);
+int speaker_index_build(const float* E, int n, int D, const int32_t* order, const int32_t* offsets, int U, float* means, void* index,
+                        size_t index_bytes, cudaStream_t st);
+size_t speaker_index_search_workspace_bytes(int Q, int U, int D, int k);
+int speaker_index_search(const float* queries, int Q, int D, const void* index, size_t index_bytes, int U, int k, int32_t* idx, float* sim,
+                         void* ws, size_t ws_bytes, cudaStream_t st);
+
 // ---- metrics.cu -------------------------------------------------------------------------------------
 size_t eer_workspace_bytes(int64_t n);
 int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_labels, const int32_t* col_labels, int ncols, int64_t n,

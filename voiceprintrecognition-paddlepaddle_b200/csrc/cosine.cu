@@ -6,29 +6,12 @@
 //              gather-GEMM as the model (K = D, fp32 out).  Tensor-core bound, 384 FLOP / pair.
 //   pair-list  idx[P,2] -> [P]        : 8 lanes per pair, gather both rows (1536 B / pair), HBM/L2-bound.
 #include "common.h"
+#include "normalize_rows.cuh"
 #include "ptx.cuh"
 
 namespace ppv {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-// one warp per row: x / max(|x|, tiny) -> planes [rows_pad, Dp] (columns >= D zero)
-__global__ void normalize_rows_kernel(const float* __restrict__ X, int rows, int D, Planes out) {
-    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (row >= rows) return;
-    const float* x = X + int64_t(row) * D;
-    float ss = 0.f;
-    for (int i = lane; i < D; i += 32) ss = fmaf(x[i], x[i], ss);
-    ss = warp_sum(ss);
-    const float inv = 1.f / fmaxf(sqrtf(ss), 1e-30f);
-    for (int i = lane; i < out.ld; i += 32) {
-        __nv_bfloat16 h, l;
-        split_bf16(i < D ? x[i] * inv : 0.f, h, l);
-        out.hi()[int64_t(row) * out.ld + i] = h;
-        out.lo()[int64_t(row) * out.ld + i] = l;
-    }
-}
 
 size_t cosine_workspace_bytes(int M, int N, int D) {
     const size_t Dp = align_up(size_t(D), 64);

@@ -145,6 +145,10 @@ SIGNATURES = {
     "ppv_eer_mindcf": (C.c_int, [_P, _P, C.c_int64, C.c_double, C.c_double, C.c_double, _P, _P, C.c_size_t, _P]),
     "ppv_eer_mindcf_matrix": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, _P, _P, C.c_size_t, _P]),
     "ppv_row_argmax": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),
+    "ppv_speaker_index_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "ppv_speaker_index_build": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, C.c_size_t, _P]),
+    "ppv_speaker_index_search_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "ppv_speaker_index_search": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t, C.c_int, C.c_int, _P, _P, _P, C.c_size_t, _P]),
     "ppv_cluster_prune": (C.c_int, [_P, C.c_int, C.c_double, _P]),
     "ppv_cluster_laplacian": (C.c_int, [_P, C.c_int, _P, _P]),
     "ppv_sym_eig_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),

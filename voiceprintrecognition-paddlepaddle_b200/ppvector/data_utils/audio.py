@@ -139,3 +139,12 @@ class AudioSegment:
 
     def normalize(self, target_db=-20.0, max_gain_db=300.0):
         self.samples = normalize_db(self.samples, target_db, max_gain_db)
+
+    def to_wav_file(self, filepath):
+        """Mono 32-bit IEEE-float WAV (format tag 3, yeaudio's default): read back by read_wav bit for bit."""
+        data = np.ascontiguousarray(self.samples, dtype='<f4').tobytes()
+        fmt = struct.pack('<HHIIHH', 3, 1, self.sample_rate, self.sample_rate * 4, 4, 32)
+        with open(filepath, 'wb') as f:
+            f.write(b'RIFF' + struct.pack('<I', 4 + 8 + len(fmt) + 8 + len(data)) + b'WAVE')
+            f.write(b'fmt ' + struct.pack('<I', len(fmt)) + fmt)
+            f.write(b'data' + struct.pack('<I', len(data)) + data)

@@ -55,16 +55,20 @@ def cosine_pairlist(E, idx):
 def retrieval(features, db_features, threshold, names=None):
     """Enrol-DB lookup of ppvector/predict.py:173-187 (``__retrieval``): cosine of each query against the per-user mean embeddings,
     arg-max per query, accepted when the similarity reaches ``threshold``.  features [Q,D], db_features [U,D] ->
-    list of [name_or_index, similarity rounded to 5 places] or [None, None] -- scoring and arg-max on the GPU
-    (``ppv_cosine_matrix`` + ``ppv_row_argmax``)."""
-    sim = cosine_matrix(features, db_features)
-    Q, U = sim.shape
-    idx = torch.empty((Q,), dtype=torch.int32, device=sim.device)
-    best = torch.empty((Q,), dtype=torch.float32, device=sim.device)
-    with torch.cuda.device(sim.device):
-        _lib.check(_lib.load().ppv_row_argmax(_lib.ptr(sim), Q, U, _lib.ptr(idx), _lib.ptr(best), _lib.current_stream()), 'ppv_row_argmax')
+    list of [name_or_index, similarity rounded to 5 places] or [None, None] -- a transient speaker index of ``db_features`` searched
+    for the top-1 on the GPU (ppvector.infer_utils.speaker_index; equal similarities: the lowest index, as numpy.argmax)."""
+    from ppvector.infer_utils.speaker_index import SpeakerIndex
+    db = _prep(db_features)
+    index = SpeakerIndex(db, torch.arange(db.shape[0], device=db.device), db.shape[0], device=db.device)
+    idx, best = index.search(_prep(features, db.device), k=1)
+    return threshold_top1(idx[:, 0].cpu().tolist(), best[:, 0].cpu().tolist(), threshold, names)
+
+
+def threshold_top1(idx, best, threshold, names=None):
+    """[name_or_index, round(similarity, 5)] per query whose best similarity reaches ``threshold``, else [None, None]
+    (predict.py:179-186)."""
     out = []
-    for i, s in zip(idx.cpu().tolist(), best.cpu().tolist()):
+    for i, s in zip(idx, best):
         if s >= threshold:
             out.append([names[i] if names is not None else i, round(float(s), 5)])
         else:

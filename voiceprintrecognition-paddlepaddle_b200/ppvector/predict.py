@@ -8,12 +8,15 @@ Same constructor arguments and the same ``predict`` / ``predict_batch`` / ``cont
   * cosine scoring runs on the GPU (``ppvector.metric.cosine``);
   * ``use_gpu=False`` raises: this build has no CPU path;
   * ``speaker_diarization`` clusters on the GPU (infer_utils/speaker_diarization.py) and takes the voice-activity segments as an
-    argument (the reference's silero VAD is not part of this build).
-The enrolment database is read (``audio_db_path``: ``recognition``, ``get_users``, ``search_audio_db``); ``register`` and
-``remove_user``, which write into it, are not carried over.
+    argument (the reference's silero VAD is not part of this build);
+  * the enrolment database (``audio_db_path``: ``register``, ``remove_user``, ``recognition``, ``get_users``, ``search_audio_db``) keeps
+    its per-user mean embeddings in a device-resident speaker index (infer_utils/speaker_index.py), rebuilt in one launch whenever a
+    user is registered or removed and searched by a fused top-k kernel; ``recognition_batch`` (extension) identifies a whole batch of
+    utterances with one search.
 """
 import os
 import pickle
+import shutil
 from io import BufferedReader
 
 import numpy as np
@@ -24,7 +27,8 @@ from loguru import logger
 from ppvector import _lib
 from ppvector.data_utils.audio import AudioSegment
 from ppvector.data_utils.featurizer import AudioFeaturizer
-from ppvector.metric.cosine import cosine_matrix
+from ppvector.infer_utils.speaker_index import SpeakerIndex
+from ppvector.metric.cosine import cosine_matrix, threshold_top1
 from ppvector.models import build_model
 from ppvector.utils.checkpoint import load_state_dict_file
 from ppvector.utils.utils import dict_to_object, print_arguments
@@ -60,11 +64,12 @@ class PPVectorPredictor:
         self.audio_db_path = audio_db_path
         self.users_name, self.users_audio_path, self.users_name_mean = [], [], []
         self.audio_feature, self.audio_feature_mean = None, None
+        self._index = None
         if audio_db_path is not None:
             self.audio_indexes_path = os.path.join(audio_db_path, 'audio_indexes.bin')
             self._load_audio_db(audio_db_path)
 
-    # ---- enrolment database: predict.py:89-187 (read side) ----------------------------------------------------
+    # ---- enrolment database: predict.py:89-187, 285-364 ------------------------------------------------------
     def _load_audio_indexes(self):
         """predict.py:89-102: the pickled index of embedded enrolment files; entries whose file is gone are dropped."""
         if not os.path.exists(self.audio_indexes_path):
@@ -85,7 +90,7 @@ class PPVectorPredictor:
 
     def _load_audio_db(self, audio_db_path):
         """predict.py:112-165: embed <db>/<user>/* files not yet in the index (predict_batch, eval batch size), rewrite the index,
-        keep one mean embedding per user (on the device as well, for retrieval)."""
+        keep one mean embedding per user (users_name_mean in the reference's set() order; the means from the speaker index)."""
         self._load_audio_indexes()
         os.makedirs(audio_db_path, exist_ok=True)
         audios_path = []
@@ -95,7 +100,8 @@ class PPVectorPredictor:
                 audios_path.extend(os.path.join(audio_dir, f).replace('\\', '/') for f in os.listdir(audio_dir))
         if len(audios_path) == 0:
             return
-        new = [p for p in audios_path if p not in self.users_audio_path]
+        known = set(self.users_audio_path)
+        new = [p for p in audios_path if p not in known]
         bs = self.configs.dataset_conf.eval_conf.batch_size
         for i in range(0, len(new), bs):
             features = self.predict_batch(new[i:i + bs])
@@ -105,21 +111,33 @@ class PPVectorPredictor:
             self.users_audio_path.append(p)
         assert len(self.audio_feature) == len(self.users_name) == len(self.users_audio_path), '加载的数量对不上！'
         self._write_index()
-        for name in set(self.users_name):
-            idx = [i for i, v in enumerate(self.users_name) if v == name]
-            feature = self.audio_feature[idx].mean(axis=0)
-            self.audio_feature_mean = feature[None] if self.audio_feature_mean is None else np.vstack((self.audio_feature_mean, feature))
-            self.users_name_mean.append(name)
-        self._audio_feature_mean_dev = torch.from_numpy(np.ascontiguousarray(self.audio_feature_mean, dtype=np.float32)).to(self.device)
+        self.users_name_mean = list(set(self.users_name))
+        self._rebuild_index()
         logger.info(f'声纹库数据加载完成，一共有{len(self.audio_feature_mean)}个用户，分别是：{self.users_name_mean}')
 
+    def _rebuild_index(self):
+        """The speaker index of the enrolment rows: user i of users_name_mean owns the rows named users_name_mean[i]; audio_feature_mean
+        is its [users, D] means (each user's rows summed in enrolment order, then divided: bitwise the reference's
+        audio_feature[rows].mean(axis=0))."""
+        if not self.users_name_mean:
+            self._index = None
+            self.audio_feature_mean = None if self.audio_feature is None else self.audio_feature[:0].copy()
+            return
+        user_id = {name: i for i, name in enumerate(self.users_name_mean)}
+        self._index = SpeakerIndex(np.ascontiguousarray(self.audio_feature, dtype=np.float32), [user_id[n] for n in self.users_name],
+                                   len(self.users_name_mean), self.device)
+        self.audio_feature_mean = self._index.means.cpu().numpy()
+
+    def _search(self, np_feature, k):
+        assert self._index is not None, "数据库中没有音频数据，请先指定说话人特征数据库或者注册说话人"
+        idx, sim = self._index.search(np.asarray(np_feature, dtype=np.float32), k=min(int(k), self._index.num_users))
+        return idx.cpu().tolist(), sim.cpu().tolist()
+
     def _retrieval(self, np_feature):
-        """predict.py:173-187: [name, similarity] of the best-matching user per query, [None, None] under the threshold (GPU cosine
-        + row arg-max, ppvector.metric.cosine.retrieval)."""
-        from ppvector.metric.cosine import retrieval
-        feats = np.asarray(np_feature, dtype=np.float32)
-        feats = feats / np.linalg.norm(feats, axis=1, keepdims=True)
-        return retrieval(feats, self._audio_feature_mean_dev, self.threshold, names=self.users_name_mean)
+        """predict.py:173-187: [name, similarity] of the best-matching user per query, [None, None] under the threshold (top-1 search
+        of the speaker index)."""
+        idx, sim = self._search(np_feature, 1)
+        return threshold_top1([i[0] for i in idx], [s[0] for s in sim], self.threshold, names=self.users_name_mean)
 
     def recognition(self, audio_data, threshold=None, sample_rate=16000):
         """predict.py:324-335 -> [name, similarity], or [None, None] under the threshold."""
@@ -127,6 +145,58 @@ class PPVectorPredictor:
             self.threshold = threshold
         feature = self.predict(audio_data, sample_rate=sample_rate)
         return self._retrieval(feature[None])[0]
+
+    def recognition_batch(self, audios_data, threshold=None, sample_rate=16000, top_k=1):
+        """Identification of a batch of utterances (extension): embedded together (predict_batch), then ONE top-k search of the speaker
+        index.  Per utterance a list of up to ``top_k`` (<= 8) [name, similarity rounded to 5 places], most similar first, holding the
+        users at or above ``threshold`` (None: the predictor's threshold, which this call does not change)."""
+        threshold = self.threshold if threshold is None else threshold
+        features = self.predict_batch(audios_data, sample_rate=sample_rate)
+        idx, sim = self._search(features, top_k)
+        return [[[self.users_name_mean[i], round(float(s), 5)] for i, s in zip(ri, rs) if s >= threshold] for ri, rs in zip(idx, sim)]
+
+    def register(self, audio_data, user_name: str, sample_rate=16000):
+        """predict.py:285-322 -> (True, "注册成功").  The audio goes through _load_audio (resample, dB normalisation) and the embedding
+        path; the processed samples are stored as <db>/<user_name>/<n>.wav (32-bit float WAV), the index file is rewritten and the
+        user's mean (or a new user) goes into the speaker index.  Deviations from the reference:
+          * registering into an empty database works (the reference's np.vstack((None, feature)) raises there);
+          * an existing file is never overwritten: n is the smallest unused number >= the number of files in the user's directory (the
+            reference takes that number as is, which overwrites a file after a manual delete);
+          * a predictor without a database (audio_db_path=None) raises ValueError (the reference fails with a TypeError)."""
+        if self.audio_db_path is None:
+            raise ValueError('register: this predictor has no enrolment database (audio_db_path=None)')
+        audio_segment = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
+        feature = self.predict(audio_data=audio_segment)
+        self.audio_feature = feature[None] if self.audio_feature is None else np.vstack((self.audio_feature, feature))
+        user_dir = os.path.join(self.audio_db_path, user_name)
+        n = len(os.listdir(user_dir)) if os.path.exists(user_dir) else 0
+        while os.path.exists(os.path.join(user_dir, f'{n}.wav')):
+            n += 1
+        audio_path = os.path.join(user_dir, f'{n}.wav')
+        os.makedirs(user_dir, exist_ok=True)
+        audio_segment.to_wav_file(audio_path)
+        self.users_audio_path.append(audio_path.replace('\\', '/'))
+        self.users_name.append(user_name)
+        self._write_index()
+        if user_name not in self.users_name_mean:
+            self.users_name_mean.append(user_name)
+        self._rebuild_index()
+        return True, "注册成功"
+
+    def remove_user(self, user_name):
+        """predict.py:344-364 -> True, or False for an unknown user: drops every row of the user, rewrites the index file, deletes
+        <db>/<user_name>/ and takes the user out of the speaker index."""
+        if user_name not in self.users_name:
+            return False
+        keep = [i for i, v in enumerate(self.users_name) if v != user_name]
+        self.users_name[:] = [self.users_name[i] for i in keep]
+        self.users_audio_path[:] = [self.users_audio_path[i] for i in keep]
+        self.audio_feature = self.audio_feature[keep]
+        self._write_index()
+        shutil.rmtree(os.path.join(self.audio_db_path, user_name))
+        del self.users_name_mean[self.users_name_mean.index(user_name)]
+        self._rebuild_index()
+        return True
 
     def get_users(self):
         """predict.py:337-342"""
