@@ -1,5 +1,6 @@
 """Equal error rate, minDCF and the EER threshold of a checkpoint on the enrolment / trials lists named in the config
-(counterpart of the reference's eval.py; same options)."""
+(counterpart of the reference's eval.py; same options).  When the config sets dataset_conf.eval_conf.score_norm
+({cohort_list, top_n, cohort}), the scores are AS-normalised against that cohort list first and the threshold is in normalised units."""
 import time
 
 from cli_common import parse_options

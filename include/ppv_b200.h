@@ -341,6 +341,21 @@ int ppv_speaker_index_search(const float* queries, int Q, int D, const void* ind
                              float* sim, void* ws, size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Adaptive score normalisation (AS-norm) against a cohort; no counterpart in the reference.  For a query row q (a trial or an
+ * enrolment) scored against the cohort, S_q is the multiset of its top_n largest scores (ties by value only: equal scores at the cut
+ * count with multiplicity), mean_q = mean(S_q) and std_q = sqrt(sum((x - mean_q)^2) / (top_n - 1)) floored at 1e-6; then
+ * s'(t, e) = 0.5 * ((s - mean_e) / std_e + (s - mean_t) / std_t).  Scores must be finite.
+ * ------------------------------------------------------------------------------------------- */
+/* scores [rows, cols] fp32, row r at scores + r * ld -> mean [rows], std [rows] fp32 of each row's top_n largest values.  Exact
+ * selection; fp64 sums about the top_n-th value.  Bitwise reproducible and independent of how rows are batched.  Rows of up to 10240
+ * columns are read from HBM once, wider rows four times.  PPV_EINVAL unless rows, cols >= 1, ld >= cols, 2 <= top_n <= cols. */
+int ppv_topn_row_stats(const float* scores, int rows, int cols, int64_t ld, int top_n, float* mean, float* std, void* stream);
+/* In place on scores [M, N] fp32 (row-major, ld = N) of trials x enrolments: s' from the trial statistics [M] and the enrolment
+ * statistics [N] (std floored at 1e-6 again).  One pass. */
+int ppv_as_norm_apply(float* scores, int M, int N, const float* trial_mean, const float* trial_std, const float* enroll_mean,
+                      const float* enroll_std, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Speaker diarization: spectral clustering of the chunk embeddings.  Replaces
  * ppvector/infer_utils/speaker_diarization.py:219-310 (SpectralCluster: pruning, Laplacian, scipy.linalg.eigh,
  * sklearn k_means).  The affinity is ppv_cosine_matrix of the [N, D] embeddings.  One stage per entry point, so that each

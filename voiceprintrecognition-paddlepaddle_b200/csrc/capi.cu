@@ -267,6 +267,23 @@ int ppv_row_argmax(const float* sim, int rows, int cols, int32_t* idx, float* be
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- AS-norm
+int ppv_topn_row_stats(const float* scores, int rows, int cols, int64_t ld, int top_n, float* mean, float* std, void* stream) {
+    PPV_GUARD_BEGIN
+    int rc = check_device();
+    if (rc) return rc;
+    return topn_row_stats(scores, rows, cols, ld, top_n, mean, std, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+int ppv_as_norm_apply(float* scores, int M, int N, const float* trial_mean, const float* trial_std, const float* enroll_mean,
+                      const float* enroll_std, void* stream) {
+    PPV_GUARD_BEGIN
+    int rc = check_device();
+    if (rc) return rc;
+    return as_norm_apply(scores, M, N, trial_mean, trial_std, enroll_mean, enroll_std, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+
 // ---------------------------------------------------------------- speaker index
 size_t ppv_speaker_index_bytes(int U, int D) { return speaker_index_bytes(U, D); }
 int ppv_speaker_index_build(const float* E, int n, int D, const int32_t* order, const int32_t* offsets, int U, float* means, void* index,

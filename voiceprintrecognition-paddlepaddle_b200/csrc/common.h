@@ -416,6 +416,11 @@ size_t speaker_index_search_workspace_bytes(int Q, int U, int D, int k);
 int speaker_index_search(const float* queries, int Q, int D, const void* index, size_t index_bytes, int U, int k, int32_t* idx, float* sim,
                          void* ws, size_t ws_bytes, cudaStream_t st);
 
+// ---- score_norm.cu ------------------------------------------------------------------------------------
+int topn_row_stats(const float* scores, int rows, int cols, int64_t ld, int top_n, float* mean, float* std, cudaStream_t st);
+int as_norm_apply(float* scores, int M, int N, const float* trial_mean, const float* trial_std, const float* enroll_mean,
+                  const float* enroll_std, cudaStream_t st);
+
 // ---- metrics.cu -------------------------------------------------------------------------------------
 size_t eer_workspace_bytes(int64_t n);
 int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_labels, const int32_t* col_labels, int ncols, int64_t n,

@@ -149,6 +149,8 @@ SIGNATURES = {
     "ppv_speaker_index_build": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_speaker_index_search_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "ppv_speaker_index_search": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t, C.c_int, C.c_int, _P, _P, _P, C.c_size_t, _P]),
+    "ppv_topn_row_stats": (C.c_int, [_P, C.c_int, C.c_int, C.c_int64, C.c_int, _P, _P, _P]),
+    "ppv_as_norm_apply": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "ppv_cluster_prune": (C.c_int, [_P, C.c_int, C.c_double, _P]),
     "ppv_cluster_laplacian": (C.c_int, [_P, C.c_int, _P, _P]),
     "ppv_sym_eig_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),

@@ -2,7 +2,8 @@
 
 ``extract_features`` (trainer.py:134-157) and ``evaluate`` (trainer.py:367-447) keep their signatures, list-file formats and
 return values; featurisation, the backbone, the trial x enrol cosine matrix and EER / minDCF (radix sort + sweep) run on the GPU
-through libppv_b200.  ``train`` (trainer.py:281-365 with the step of :206-229) runs the CUDA training step of
+through libppv_b200; with the optional ``dataset_conf.eval_conf.score_norm`` key the matrix is AS-normalised against a cohort list first
+(ppvector/metric/score_norm.py).  ``train`` (trainer.py:281-365 with the step of :206-229) runs the CUDA training step of
 ``ppvector.train_engine.TrainEngine`` (train-mode forward, AAM loss, backward, one gradient all-reduce over NCCL, Adam) with the
 reference's schedules; it is implemented for EcapaTdnn + AAMLoss + Adam + WarmupCosineSchedulerLR (configs/ecapa_tdnn.yml) and
 raises for other combinations.  Checkpoints follow the reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}``
@@ -22,6 +23,7 @@ from ppvector.data_utils.featurizer import AudioFeaturizer
 from ppvector.data_utils.reader import PPVectorDataset
 from ppvector.metric.cosine import cosine_matrix
 from ppvector.metric.metrics import compute_dcf, compute_eer, compute_fnr_fpr, eer_mindcf_from_matrix_gpu  # noqa: F401
+from ppvector.metric.score_norm import as_norm, cohort_stats, score_norm_config, speaker_cohort
 from ppvector.models import build_model
 from ppvector.utils.checkpoint import find_resume_dir, load_checkpoint_dir, load_state_dict_file, save_checkpoint
 from ppvector.utils.utils import dict_to_object, print_arguments
@@ -111,14 +113,22 @@ class PPVectorTrainer(object):
 
     # ---- trainer.py:367-447 ------------------------------------------------------------------------------------
     def evaluate(self, resume_model=None, save_image_path=None):
+        norm = score_norm_config(self.configs.dataset_conf.eval_conf.get('score_norm'))
         self._setup_model(resume_model)
         with torch.no_grad():
             enroll_features, enroll_labels = self._embed_list(self.configs.dataset_conf.enroll_list, '注册音频声纹特征')
             trials_features, trials_labels = self._embed_list(self.configs.dataset_conf.trials_list, '验证音频声纹特征')
+            if norm is not None and not self.stop_eval:
+                cohort_features, cohort_labels = self._embed_list(norm['cohort_list'], '归一化集合声纹特征')
         if self.stop_eval:
             return -1, -1, -1
         # the reference scores one trial against all enrolments per Python iteration (trainer.py:416-423): one GEMM here
         scores = cosine_matrix(trials_features, enroll_features)
+        if norm is not None:  # extension: AS-norm against the cohort list (ppvector/metric/score_norm.py)
+            cohort = speaker_cohort(cohort_features, cohort_labels) if norm['cohort'] == 'speaker' else cohort_features
+            as_norm(scores, cohort_stats(trials_features, cohort, norm['top_n']), cohort_stats(enroll_features, cohort, norm['top_n']))
+            logger.info(f"AS-norm against {cohort.shape[0]} cohort rows ({norm['cohort']}, top_n {norm['top_n']}): "
+                        f"the threshold is in normalised score units")
         # EER / minDCF on the device too (metrics.py:4-37 definitions; csrc/metrics.cu): the M x N scores never visit the host
         eer, min_dcf, threshold = eer_mindcf_from_matrix_gpu(scores, trials_labels, enroll_labels)
         if save_image_path:
