@@ -356,6 +356,41 @@ int ppv_as_norm_apply(float* scores, int M, int N, const float* trial_mean, cons
                       const float* enroll_std, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Energy voice-activity detection: Kaldi's compute-vad (src/ivector/voice-activity-detection.cc, ComputeVadEnergy) on the raw log
+ * energy of each snip_edges frame, in front of speaker diarization.  The reference runs silero-vad there (a neural network whose
+ * weights ship inside yeaudio); this is the classical energy VAD of Kaldi's x-vector recipes instead.  Per recording of L samples:
+ * T = 0 if L < window else 1 + (L - window) / shift frames;
+ * e_t = ln(max(32768^2 * sum_{n < window} (x[t * shift + n] - mean_t)^2, FLT_EPSILON)) (mean_t the frame's own mean; fp64 sums; no
+ * dither, pre-emphasis or window function); thr = energy_threshold + energy_mean_scale * (sum_t e_t) / T (fp64); frame t is voiced iff
+ * num >= den * proportion_threshold (product in fp32), where den counts the frames in [t - frames_context, t + frames_context] ∩ [0, T)
+ * and num those of them with e_t2 > thr.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+    int window;                 /* samples per frame: sample_rate * 25 / 1000 (400 at 16 kHz); 1..2048 */
+    int shift;                  /* samples between frames: sample_rate * 10 / 1000 (160 at 16 kHz); 1..window */
+    float energy_threshold;     /* 5.5 */
+    float energy_mean_scale;    /* 0.5; >= 0 */
+    int frames_context;         /* 2; >= 0 */
+    float proportion_threshold; /* 0.12; in (0, 1) */
+} ppv_vad_cfg;
+/* The defaults of Kaldi's VoxCeleb / SRE16 x-vector recipes (conf/vad.conf) with 25 ms / 10 ms frames at sample_rate. */
+void ppv_vad_default_cfg(ppv_vad_cfg* cfg, int sample_rate);
+/* T for a recording of L samples; -1 for a configuration out of range or L < 0. */
+int64_t ppv_vad_num_frames(const ppv_vad_cfg* cfg, int64_t L);
+/* Workspace for R recordings of total_samples samples in all (the last sample offset); 0 for arguments out of range. */
+size_t ppv_vad_workspace_bytes(const ppv_vad_cfg* cfg, int R, int64_t total_samples);
+/* R recordings, recording r at wav[sample_offsets[r] .. sample_offsets[r + 1]) (fp32, device; sample_offsets is a HOST array of R + 1
+ * non-decreasing values).  Frame outputs are concatenated in recording order (recording r's frames start at the sum of the earlier
+ * recordings' T): voiced [sum T] uint8 (0 / 1) and, if log_energy != NULL, e_t [sum T] fp64.  runs [run_cap, 3] int32 receives the
+ * maximal runs of voiced frames as (recording, first_frame, end_frame) in recording and frame order, frame indices within the
+ * recording; *n_runs (device int32) their count.  run_cap >= sum_r ceil(T_r / 2) (the alternating worst case).  A recording with
+ * T = 0 yields no run.  ws: ppv_vad_workspace_bytes(cfg, R, sample_offsets[R]) bytes, 256-byte aligned.  Bitwise reproducible and
+ * independent of how recordings are batched.  PPV_EINVAL for null pointers, R < 1, decreasing offsets, too small a workspace or run
+ * capacity, and configurations out of range. */
+int ppv_vad_energy(const ppv_vad_cfg* cfg, const float* wav, const int64_t* sample_offsets, int R, double* log_energy, uint8_t* voiced,
+                   int32_t* runs, int64_t run_cap, int32_t* n_runs, void* ws, size_t ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Speaker diarization: spectral clustering of the chunk embeddings.  Replaces
  * ppvector/infer_utils/speaker_diarization.py:219-310 (SpectralCluster: pruning, Laplacian, scipy.linalg.eigh,
  * sklearn k_means).  The affinity is ppv_cosine_matrix of the [N, D] embeddings.  One stage per entry point, so that each

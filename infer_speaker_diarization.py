@@ -13,6 +13,10 @@ OPTIONS = [
     ('threshold', float, 0.6, 'similarity at or above which a speaker is taken to be an enrolled user'),
     ('model_path', str, 'models/CAMPPlus_Fbank/best_model/', 'directory or file holding the weights'),
 ]
+# options of this build beyond the reference's
+EXTENSION_OPTIONS = [
+    ('vad', bool, False, "find the speech first with Kaldi's energy VAD on the GPU (otherwise the whole recording is taken as speech)"),
+]
 
 
 def main(opt):
@@ -23,7 +27,8 @@ def main(opt):
         assert opt.audio_db_path is not None, '请指定音频库的路径'
     predictor = PPVectorPredictor(configs=opt.configs, model_path=opt.model_path, threshold=opt.threshold, audio_db_path=opt.audio_db_path,
                                   use_gpu=opt.use_gpu)
-    results = predictor.speaker_diarization(opt.audio_path, speaker_num=opt.speaker_num, search_audio_db=opt.search_audio_db)
+    results = predictor.speaker_diarization(opt.audio_path, speaker_num=opt.speaker_num, search_audio_db=opt.search_audio_db,
+                                              vad=opt.vad)
     print('识别结果：')
     for result in results:
         print(result)
@@ -32,4 +37,4 @@ def main(opt):
 
 
 if __name__ == '__main__':
-    main(parse_options(__doc__, OPTIONS))
+    main(parse_options(__doc__, OPTIONS + EXTENSION_OPTIONS))

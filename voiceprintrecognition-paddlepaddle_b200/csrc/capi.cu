@@ -284,6 +284,30 @@ int ppv_as_norm_apply(float* scores, int M, int N, const float* trial_mean, cons
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- energy VAD
+void ppv_vad_default_cfg(ppv_vad_cfg* cfg, int sample_rate) {
+    if (!cfg) return;
+    cfg->window = int(int64_t(sample_rate) * 25 / 1000);
+    cfg->shift = int(int64_t(sample_rate) * 10 / 1000);
+    cfg->energy_threshold = 5.5f;
+    cfg->energy_mean_scale = 0.5f;
+    cfg->frames_context = 2;
+    cfg->proportion_threshold = 0.12f;
+}
+int64_t ppv_vad_num_frames(const ppv_vad_cfg* cfg, int64_t L) { return cfg ? vad_num_frames(*cfg, L) : -1; }
+size_t ppv_vad_workspace_bytes(const ppv_vad_cfg* cfg, int R, int64_t total_samples) {
+    return cfg ? vad_workspace_bytes(*cfg, R, total_samples) : 0;
+}
+int ppv_vad_energy(const ppv_vad_cfg* cfg, const float* wav, const int64_t* sample_offsets, int R, double* log_energy, uint8_t* voiced,
+                   int32_t* runs, int64_t run_cap, int32_t* n_runs, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    int rc = check_device();
+    if (rc) return rc;
+    if (!cfg) return fail(PPV_EINVAL, "ppv_vad_energy: null cfg");
+    return vad_energy(*cfg, wav, sample_offsets, R, log_energy, voiced, runs, run_cap, n_runs, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+
 // ---------------------------------------------------------------- speaker index
 size_t ppv_speaker_index_bytes(int U, int D) { return speaker_index_bytes(U, D); }
 int ppv_speaker_index_build(const float* E, int n, int D, const int32_t* order, const int32_t* offsets, int U, float* means, void* index,

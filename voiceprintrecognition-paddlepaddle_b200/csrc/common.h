@@ -421,6 +421,12 @@ int topn_row_stats(const float* scores, int rows, int cols, int64_t ld, int top_
 int as_norm_apply(float* scores, int M, int N, const float* trial_mean, const float* trial_std, const float* enroll_mean,
                   const float* enroll_std, cudaStream_t st);
 
+// ---- vad.cu -----------------------------------------------------------------------------------------
+int64_t vad_num_frames(const ppv_vad_cfg& cfg, int64_t L);
+size_t vad_workspace_bytes(const ppv_vad_cfg& cfg, int R, int64_t total_samples);
+int vad_energy(const ppv_vad_cfg& cfg, const float* wav, const int64_t* sample_offsets, int R, double* log_energy, uint8_t* voiced,
+               int32_t* runs, int64_t run_cap, int32_t* n_runs, void* ws, size_t ws_bytes, cudaStream_t st);
+
 // ---- metrics.cu -------------------------------------------------------------------------------------
 size_t eer_workspace_bytes(int64_t n);
 int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_labels, const int32_t* col_labels, int ncols, int64_t n,

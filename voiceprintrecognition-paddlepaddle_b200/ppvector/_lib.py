@@ -66,6 +66,11 @@ class CamPPlusCfg(C.Structure):
                 ("init_channels", C.c_int), ("precision", C.c_int)]
 
 
+class VadCfg(C.Structure):
+    _fields_ = [("window", C.c_int), ("shift", C.c_int), ("energy_threshold", C.c_float), ("energy_mean_scale", C.c_float),
+                ("frames_context", C.c_int), ("proportion_threshold", C.c_float)]
+
+
 TAPS_MAX_INPUTS, TAPS_MAX_SOURCES = 4, 16
 
 
@@ -151,6 +156,10 @@ SIGNATURES = {
     "ppv_speaker_index_search": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t, C.c_int, C.c_int, _P, _P, _P, C.c_size_t, _P]),
     "ppv_topn_row_stats": (C.c_int, [_P, C.c_int, C.c_int, C.c_int64, C.c_int, _P, _P, _P]),
     "ppv_as_norm_apply": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "ppv_vad_default_cfg": (None, [C.POINTER(VadCfg), C.c_int]),
+    "ppv_vad_num_frames": (C.c_int64, [C.POINTER(VadCfg), C.c_int64]),
+    "ppv_vad_workspace_bytes": (C.c_size_t, [C.POINTER(VadCfg), C.c_int, C.c_int64]),
+    "ppv_vad_energy": (C.c_int, [C.POINTER(VadCfg), _P, C.POINTER(C.c_int64), C.c_int, _P, _P, _P, C.c_int64, _P, _P, C.c_size_t, _P]),
     "ppv_cluster_prune": (C.c_int, [_P, C.c_int, C.c_double, _P]),
     "ppv_cluster_laplacian": (C.c_int, [_P, C.c_int, _P, _P]),
     "ppv_sym_eig_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),

@@ -108,7 +108,7 @@ def normalize_db(x, target_db=-20.0, max_gain_db=300.0):
 
 class AudioSegment:
     """The slice of yeaudio.audio.AudioSegment the predictor uses: samples / sample_rate / duration /
-    resample / normalize / from_file / from_ndarray / from_bytes."""
+    resample / normalize / vad / from_file / from_ndarray / from_bytes."""
 
     def __init__(self, samples, sample_rate):
         self.samples = np.ascontiguousarray(samples, dtype=np.float32)
@@ -139,6 +139,12 @@ class AudioSegment:
 
     def normalize(self, target_db=-20.0, max_gain_db=300.0):
         self.samples = normalize_db(self.samples, target_db, max_gain_db)
+
+    def vad(self, return_seconds=False, **opts):
+        """The speech in the recording: [{'start', 'end'}, ...] in samples, or in seconds with return_seconds=True.  yeaudio runs silero-vad
+        here; this build runs Kaldi's energy VAD on the GPU (infer_utils/vad.py, options as vad_options there)."""
+        from ppvector.infer_utils import vad
+        return vad.energy_vad([self.samples], self.sample_rate, return_seconds=return_seconds, **opts)[0]
 
     def to_wav_file(self, filepath):
         """Mono 32-bit IEEE-float WAV (format tag 3, yeaudio's default): read back by read_wav bit for bit."""

@@ -11,7 +11,8 @@ At most 8192 windows (about 1.7 h of speech) per call; more raise ``PPVError``.
 
 ``SpeakerDiarization``: the label and segment post-processing (:89-216) is list logic over a few thousand segments and stays on
 the host, quirks of the reference included (see ``_merge_by_cos``).  Windowing is infer_utils/chunking.py.  Voice-activity detection
-(yeaudio's silero VAD, ``segments_audio``) is not part of this build: callers pass the voiced segments.
+(``segments_audio``) runs Kaldi's energy VAD on the GPU (infer_utils/vad.py) where the reference runs yeaudio's silero VAD; callers
+may also pass voiced segments of their own.
 """
 import ctypes as C
 
@@ -34,6 +35,18 @@ class SpeakerDiarization(object):
         self.sample_rate = sample_rate
         self.merge_threshold = merge_threshold
         self.spectral_cluster = SpectralCluster()
+
+    def segments_audio(self, audio_segment) -> list:
+        """reference :26-45: the voiced spans of the recording (AudioSegment.vad, here the energy VAD), rounded to milliseconds, checked
+        and cut into seg_duration windows -> [[start_s, end_s, window samples], ...]."""
+        vad_segments = []
+        samples = audio_segment.samples
+        self.sample_rate = audio_segment.sample_rate
+        for t in audio_segment.vad(return_seconds=True):
+            st, ed = round(t['start'], 3), round(t['end'], 3)
+            vad_segments.append([st, ed, samples[int(st * self.sample_rate):int(ed * self.sample_rate)]])
+        self._check_audio_list(vad_segments)
+        return self._chunk(vad_segments)
 
     def _check_audio_list(self, audio: list):
         """reference :47-57: ordered, consistent [start_s, end_s, samples] segments with more than 5 s of speech in all."""

@@ -7,8 +7,8 @@ Same constructor arguments and the same ``predict`` / ``predict_batch`` / ``cont
     loop and runs the model in chunks of 32 (predict.py:262-267);
   * cosine scoring runs on the GPU (``ppvector.metric.cosine``);
   * ``use_gpu=False`` raises: this build has no CPU path;
-  * ``speaker_diarization`` clusters on the GPU (infer_utils/speaker_diarization.py) and takes the voice-activity segments as an
-    argument (the reference's silero VAD is not part of this build);
+  * ``speaker_diarization`` clusters on the GPU (infer_utils/speaker_diarization.py); the voice-activity segments come from the caller
+    or, with ``vad=True``, from Kaldi's energy VAD on the GPU (infer_utils/vad.py) where the reference runs silero-vad;
   * the enrolment database (``audio_db_path``: ``register``, ``remove_user``, ``recognition``, ``get_users``, ``search_audio_db``) keeps
     its per-user mean embeddings in a device-resident speaker index (infer_utils/speaker_index.py), rebuilt in one launch whenever a
     user is registered or removed and searched by a fused top-k kernel; ``recognition_batch`` (extension) identifies a whole batch of
@@ -416,31 +416,39 @@ class PPVectorPredictor:
         return np.concatenate([self.extract_embeddings(inputs[i:i + batch_size], ratio[i:i + batch_size])
                                for i in range(0, len(segs), batch_size)], axis=0)
 
-    def diarization_embeddings(self, audio_data, sample_rate=16000, vad_segments=None, seg_duration=1.5, seg_shift=0.75, batch_size=256):
+    def diarization_embeddings(self, audio_data, sample_rate=16000, vad_segments=None, seg_duration=1.5, seg_shift=0.75, batch_size=256,
+                               vad=False):
         """The embedding fan-out of the reference's ``speaker_diarization`` (predict.py:378-381): the recording (or the given voice-activity
         segments [(start_s, end_s), ...]) is cut into ``seg_duration`` windows every ``seg_shift`` seconds (infer_utils/chunking.py) and every
-        window goes through the embedding path as ONE equal-length batch.  Returns (times [n, 2] seconds, embeddings [n, embd]).  VAD and the
-        clustering after it are outside the hot path: pass ``vad_segments`` from your VAD; None takes the whole recording as one segment."""
+        window goes through the embedding path as ONE equal-length batch.  Returns (times [n, 2] seconds, embeddings [n, embd]).  Pass
+        ``vad_segments`` from your VAD, or ``vad=True`` to find them with the energy VAD (infer_utils/vad.py) on the loaded audio; with
+        neither, the whole recording is one segment."""
         from ppvector.infer_utils.chunking import fan_out_embeddings
-        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments)
+        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments, vad)
         return fan_out_embeddings(segs, self.extract_embeddings, seg_duration, seg_shift, sr, batch_size)
 
-    def _voiced_segments(self, audio_data, sample_rate, vad_segments):
-        """-> (sample rate, [(start_s, end_s, samples), ...]) of the given voice-activity segments, or of the whole recording."""
+    def _voiced_segments(self, audio_data, sample_rate, vad_segments, vad=False):
+        """-> (sample rate, [(start_s, end_s, samples), ...]) of the given voice-activity segments, of the segments the energy VAD finds
+        on the loaded (resampled, dB-normalised) audio (vad=True), or of the whole recording."""
+        if vad and vad_segments is not None:
+            raise ValueError('pass either vad=True or vad_segments, not both')
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
         sr, x = seg.sample_rate, seg.samples
+        if vad:
+            vad_segments = [(t['start'], t['end']) for t in seg.vad(return_seconds=True)]
         spans = [(0.0, len(x) / sr)] if vad_segments is None else [(round(float(a), 3), round(float(b), 3)) for a, b in vad_segments]
         return sr, [(a, b, x[int(a * sr):int(b * sr)]) for a, b in spans]
 
-    def speaker_diarization(self, audio_data, sample_rate=16000, speaker_num=None, search_audio_db=False, vad_segments=None):
+    def speaker_diarization(self, audio_data, sample_rate=16000, speaker_num=None, search_audio_db=False, vad_segments=None, vad=False):
         """reference: predict.py:366-396 -> [{'speaker', 'start', 'end'}, ...].  The recording (or the given voice-activity segments
-        [(start_s, end_s), ...]; None = the whole recording) is cut into 1.5 s windows every 0.75 s and embedded as one batch
+        [(start_s, end_s), ...]; None = the whole recording; vad=True: the segments the energy VAD finds, as the reference's
+        segments_audio does with silero-vad) is cut into 1.5 s windows every 0.75 s and embedded as one batch
         (diarization_embeddings); the windows are clustered on the GPU (infer_utils/speaker_diarization.py: spectral clustering,
         ``speaker_num`` fixes the speaker count) and the segments post-processed as in the reference.  The voiced speech must total
         more than 5 s.  search_audio_db=True names each speaker from the enrolment database (``audio_db_path``)."""
         from ppvector.infer_utils.chunking import fan_out_embeddings
         from ppvector.infer_utils.speaker_diarization import SpeakerDiarization
-        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments)
+        sr, segs = self._voiced_segments(audio_data, sample_rate, vad_segments, vad)
         sd = SpeakerDiarization(sample_rate=sr)
         sd._check_audio_list([list(s) for s in segs])
         times, features = fan_out_embeddings(segs, self.extract_embeddings, sd.seg_duration, sd.seg_shift, sr, 256)
