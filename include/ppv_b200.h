@@ -309,7 +309,8 @@ int ppv_audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* ipara
  * ppvector/predict.py:173-187 (__retrieval).
  * ------------------------------------------------------------------------------------------- */
 size_t ppv_eer_workspace_bytes(int64_t n);
-/* scores [n] fp32, labels [n] int32 (1 = target trial) -> out4 (device double[4]) = {EER, threshold at the EER, minDCF, number of targets}. */
+/* scores [n] fp32, labels [n] int32 (1 = target trial) -> out4 (device double[4]) = {EER, threshold at the EER, minDCF, number of targets}.
+ * ws: ppv_eer_workspace_bytes(n) bytes, 256-byte aligned (both forms). */
 int ppv_eer_mindcf(const float* scores, const int32_t* labels, int64_t n, double p_target, double c_miss, double c_fa, double* out4,
                    void* ws, size_t ws_bytes, void* stream);
 /* The evaluation loop's form (trainer.py:416-423): scores [M,N] of trials x enrolments, label = (trial_labels[i] == enroll_labels[j]). */
@@ -434,6 +435,7 @@ int ppv_kmeans(const double* X, int ld, int N, int k, const double* uniforms, in
  * [| 1 for margin_type 'A'; default 'C'], the `label_smoothing` argument carries lanbuda (the positive / negative weight); the loss's
  * bias stays at its initial 0 as in the reference (it is not among the optimizer's parameters). */
 #define PPV_HEAD_SPHEREFACE2 8
+/* ws: ppv_aam_workspace_bytes(B, D, S) bytes, 256-byte aligned. */
 int ppv_aam_forward(const float* emb, const float* W, const int64_t* labels, int B, int D, int S, float margin,
                     float scale, int easy_margin, float label_smoothing, float* logits, float* loss,
                     void* ws, size_t ws_bytes, void* stream);

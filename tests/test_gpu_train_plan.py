@@ -116,9 +116,10 @@ def test_bad_tap_names_fail_the_same_way(cuda):
 
 
 # ppv_trainer_workspace_bytes of the default config with 37 classes on a 132-SM H100 (the weight-gradient split-K partials and the
-# BatchNorm-backward frame splits scale with the SM count), recorded before the plan was moved onto the shared workspace helpers.
-WS_BYTES = {(2, 9): 87462144, (2, 298): 170561792, (3, 35): 108345088, (4, 40): 108453632, (8, 100): 212810496, (64, 9): 261409536,
-            (64, 40): 573033216, (64, 298): 3252996864}
+# BatchNorm-backward frame splits scale with the SM count), recorded before the plan was moved onto the shared workspace helpers, less
+# the 256 bytes of trailing slack the AAM block (the last buffer) stopped reserving when its size came from the AAM call's own carve.
+WS_BYTES = {(2, 9): 87461888, (2, 298): 170561536, (3, 35): 108344832, (4, 40): 108453376, (8, 100): 212810240, (64, 9): 261409280,
+            (64, 40): 573032960, (64, 298): 3252996608}
 
 
 def test_workspace_sizes_are_unchanged(cuda):

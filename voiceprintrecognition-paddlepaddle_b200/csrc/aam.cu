@@ -13,31 +13,21 @@
 
 namespace ppv {
 
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-// workspace layout (floats): e_hat [B,D] | inv_e [B] | inv_w [S] | row_loss [B] | G [B,S] | dE_hat [B,D]
+// The workspace of aam_forward and aam_backward: the backward reads the e_hat / inv_e / inv_w the forward left in the same workspace.
 struct AamWs {
-    float *e_hat, *inv_e, *inv_w, *row_loss, *G, *dEh;
+    float *e_hat, *inv_e, *inv_w, *row_loss, *G, *dEh;  // [B,D] | [B] | [S] | [B] | [B,S] | [B,D]
 };
-static AamWs carve_aam(void* ws, int B, int D, int S) {
-    float* p = static_cast<float*>(ws);
-    AamWs w;
-    auto take = [&](size_t n) {
-        float* r = p;
-        p += align_up(n, 64);
-        return r;
-    };
-    w.e_hat = take(size_t(B) * D);
-    w.inv_e = take(B);
-    w.inv_w = take(S);
-    w.row_loss = take(B);
-    w.G = take(size_t(B) * S);
-    w.dEh = take(size_t(B) * D);
-    return w;
+static void carve_aam(WsCarver& cv, int B, int D, int S, AamWs* w) {
+    auto take = [&](size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); };
+    w->e_hat = take(size_t(B) * D);
+    w->inv_e = take(B);
+    w->inv_w = take(S);
+    w->row_loss = take(B);
+    w->G = take(size_t(B) * S);
+    w->dEh = take(size_t(B) * D);
 }
 size_t aam_workspace_bytes(int B, int D, int S) {
-    size_t n = align_up(size_t(B) * D, 64) * 2 + align_up(size_t(B), 64) * 2 + align_up(size_t(S), 64) + align_up(size_t(B) * S, 64);
-    return n * sizeof(float) + 256;
+    return carve_extent([&](WsCarver& cv) { AamWs w; carve_aam(cv, B, D, S, &w); });
 }
 
 __global__ void aam_norm_rows_kernel(const float* __restrict__ emb, int B, int D, float* __restrict__ e_hat, float* __restrict__ inv_e) {
@@ -273,10 +263,12 @@ static void margin_consts(float margin, float* cos_m, float* sin_m, float* th, f
 
 int aam_forward(const float* emb, const float* W, const int64_t* labels, int B, int D, int S, float margin, float scale,
                 int easy_margin, float label_smoothing, float* logits, float* loss, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(emb && W && labels && logits && loss && ws, "aam_forward: null argument");
+    PPV_REQUIRE(emb && W && labels && logits && loss, "aam_forward: null argument");
     PPV_REQUIRE(B > 0 && D > 0 && S > 0, "aam_forward: empty input");
-    PPV_REQUIRE(ws_bytes >= aam_workspace_bytes(B, D, S), "aam_forward: workspace too small");
-    AamWs w = carve_aam(ws, B, D, S);
+    if (int rc = check_workspace("aam_forward", ws, ws_bytes, aam_workspace_bytes(B, D, S), "ppv_aam_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    AamWs w;
+    carve_aam(cv, B, D, S, &w);
     aam_norm_rows_kernel<<<(B + 7) / 8, 256, 0, st>>>(emb, B, D, w.e_hat, w.inv_e);
     PPV_LAUNCH_OK("aam_norm_rows_kernel");
     aam_norm_cols_kernel<<<(S + 255) / 256, 256, 0, st>>>(W, D, S, w.inv_w);
@@ -347,10 +339,12 @@ __global__ void __launch_bounds__(128)
 int aam_backward(const float* emb, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin,
                  float scale, int easy_margin, float label_smoothing, float* d_emb, float* d_W, void* ws, size_t ws_bytes,
                  cudaStream_t st) {
-    PPV_REQUIRE(emb && W && labels && logits && d_emb && d_W && ws, "aam_backward: null argument");
-    PPV_REQUIRE(ws_bytes >= aam_workspace_bytes(B, D, S), "aam_backward: workspace too small");
+    PPV_REQUIRE(emb && W && labels && logits && d_emb && d_W, "aam_backward: null argument");
+    if (int rc = check_workspace("aam_backward", ws, ws_bytes, aam_workspace_bytes(B, D, S), "ppv_aam_workspace_bytes")) return rc;
     PPV_REQUIRE(size_t(B) * D * sizeof(float) <= 200 * 1024, "aam_backward: B*D too large for the shared-memory dW kernel");
-    AamWs w = carve_aam(ws, B, D, S);  // e_hat / inv_e / inv_w are those of the forward call
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    AamWs w;
+    carve_aam(cv, B, D, S, &w);  // e_hat / inv_e / inv_w are those of the forward call
     float cm, sm, th, mmm;
     margin_consts(margin, &cm, &sm, &th, &mmm);
     int kind, K;

@@ -117,36 +117,48 @@ __global__ void __launch_bounds__(256) prep_apply_kernel(const float* __restrict
     }
 }
 
+struct PrepWs {
+    double* partial;  // [B][nchunk][3] per-chunk sums of pass 1
+    float* gains;     // [B][2]
+    ReverbViews rv;   // audio_prep_reverb only
+};
+// max_rir_len = 0: audio_prep's workspace; > 0: audio_prep_reverb's, the reverb views behind the shared ones
+void carve_prep(WsCarver& cv, int B, int max_new_len, int max_rir_len, PrepWs* w) {
+    const size_t nchunk = size_t((max_new_len + AP_CHUNK - 1) / AP_CHUNK);
+    w->partial = static_cast<double*>(cv.take(size_t(B) * nchunk * 3 * sizeof(double)));
+    w->gains = static_cast<float*>(cv.take(size_t(B) * 2 * sizeof(float)));
+    if (max_rir_len > 0) carve_reverb(cv, B, max_new_len, max_rir_len, &w->rv);
+}
+
 }  // namespace
 
-size_t audio_prep_workspace_bytes(int B, int max_len) {
-    if (B <= 0 || max_len <= 0) return 0;
-    const size_t nchunk = size_t((max_len + AP_CHUNK - 1) / AP_CHUNK);
-    return ((size_t(B) * nchunk * 3 * sizeof(double) + 255) / 256) * 256 + ((size_t(B) * 2 * sizeof(float) + 255) / 256) * 256;
+size_t audio_prep_workspace_bytes(int B, int max_new_len) {
+    if (B <= 0 || max_new_len <= 0) return 0;
+    return carve_extent([&](WsCarver& cv) { PrepWs w; carve_prep(cv, B, max_new_len, 0, &w); });
 }
 
 // wav [B][wav_ld] raw (resampled) samples; iparams [B][PPV_PREP_NI]; fparams [B][PPV_PREP_NF]; noise: concatenated noise clips (may be null
 // when no item has noise); out [B][Lout].  max_new_len >= every item's new_len (sizes the workspace).
 int audio_prep(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, int B, int max_new_len,
                float target_db, int normalize, int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(wav && iparams && fparams && out && ws, "audio_prep: null argument");
+    PPV_REQUIRE(wav && iparams && fparams && out, "audio_prep: null argument");
     PPV_REQUIRE(B > 0 && max_new_len > 0 && Lout > 0, "audio_prep: empty batch");
-    PPV_REQUIRE(ws_bytes >= audio_prep_workspace_bytes(B, max_new_len) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0,
-                "audio_prep: workspace too small / unaligned");
+    if (int rc = check_workspace("audio_prep", ws, ws_bytes, audio_prep_workspace_bytes(B, max_new_len), "ppv_audio_prep_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    PrepWs w;
+    carve_prep(cv, B, max_new_len, 0, &w);
     const int nchunk = (max_new_len + AP_CHUNK - 1) / AP_CHUNK;
-    double* partial = static_cast<double*>(ws);
-    float* gains = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + ((size_t(B) * nchunk * 3 * sizeof(double) + 255) / 256) * 256);
-    prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, partial);
-    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, partial, nchunk, B, target_db, normalize, nullptr, gains);
+    prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, w.partial);
+    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, w.partial, nchunk, B, target_db, normalize, nullptr, w.gains);
     const int gx = std::max(1, std::min((Lout + 255) / 256, 64));
-    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, nullptr, Lout, out);
+    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, w.gains, nullptr, Lout, out);
     PPV_LAUNCH_OK("audio_prep kernels");
     return PPV_OK;
 }
 
 size_t audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len) {
     if (B <= 0 || max_new_len <= 0 || max_rir_len <= 0) return 0;
-    return audio_prep_workspace_bytes(B, max_new_len) + reverb_workspace_bytes(B, max_new_len, max_rir_len);
+    return carve_extent([&](WsCarver& cv) { PrepWs w; carve_prep(cv, B, max_new_len, max_rir_len, &w); });
 }
 
 // audio_prep with reverberation after the noise: rparams [B][2] = {rir_off, rir_len} into rir_bank (rir_bank_len samples), rir_len 0 = no
@@ -155,24 +167,24 @@ size_t audio_prep_reverb_workspace_bytes(int B, int max_new_len, int max_rir_len
 int audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
                       int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
                       int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(wav && iparams && fparams && rir_bank && rparams && out && ws, "audio_prep_reverb: null argument");
+    PPV_REQUIRE(wav && iparams && fparams && rir_bank && rparams && out, "audio_prep_reverb: null argument");
     PPV_REQUIRE(B > 0 && max_new_len > 0 && Lout > 0, "audio_prep_reverb: empty batch");
     PPV_REQUIRE(max_rir_len > 0 && int64_t(max_rir_len) <= rir_bank_len, "audio_prep_reverb: max_rir_len outside [1, rir_bank_len]");
     PPV_REQUIRE(int64_t(max_new_len) + max_rir_len - 1 <= INT32_MAX - 512, "audio_prep_reverb: reverberant length exceeds int32");
-    PPV_REQUIRE(ws_bytes >= audio_prep_reverb_workspace_bytes(B, max_new_len, max_rir_len) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0,
-                "audio_prep_reverb: workspace too small / unaligned");
-    const size_t base = audio_prep_workspace_bytes(B, max_new_len);
+    if (int rc = check_workspace("audio_prep_reverb", ws, ws_bytes, audio_prep_reverb_workspace_bytes(B, max_new_len, max_rir_len),
+                                 "ppv_audio_prep_reverb_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    PrepWs w;
+    carve_prep(cv, B, max_new_len, max_rir_len, &w);
     const int nchunk = (max_new_len + AP_CHUNK - 1) / AP_CHUNK;
-    double* partial = static_cast<double*>(ws);
-    float* gains = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + ((size_t(B) * nchunk * 3 * sizeof(double) + 255) / 256) * 256);
-    prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, partial);
-    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, partial, nchunk, B, target_db, normalize, rparams, gains);
+    prep_stats_kernel<<<dim3(nchunk, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, nchunk, w.partial);
+    prep_gains_kernel<<<(B + 127) / 128, 128, 0, st>>>(iparams, fparams, w.partial, nchunk, B, target_db, normalize, rparams, w.gains);
     PPV_LAUNCH_OK("audio_prep_reverb stats / gains");
     const int rc = reverb_run(wav, wav_ld, iparams, fparams, noise, rir_bank, rir_bank_len, rparams, B, max_new_len, max_rir_len, target_db,
-                              normalize, Lout, out, gains, static_cast<uint8_t*>(ws) + base, st);
+                              normalize, Lout, out, w.gains, w.rv, st);
     if (rc != PPV_OK) return rc;
     const int gx = std::max(1, std::min((Lout + 255) / 256, 64));
-    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, rparams, Lout, out);
+    prep_apply_kernel<<<dim3(gx, B), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, w.gains, rparams, Lout, out);
     PPV_LAUNCH_OK("audio_prep_reverb apply");
     return PPV_OK;
 }

@@ -293,7 +293,7 @@ bool CamppModel::prepare_weights(ArenaBuilder& ab) {
             lw.block = bi;
             lw.dil = CP_DIL[bi];
             lw.in_ch = channels + li * G;
-            lw.Kp = int(mc_align_up(size_t(lw.in_ch), 64));
+            lw.Kp = int(align_up(size_t(lw.in_ch), 64));
             const std::string p = "xvector.block" + std::to_string(bi + 1) + ".tdnnd" + std::to_string(li + 1);
             ok &= ab.put_bn(&lw.bn1_scale, &lw.bn1_shift, p + ".nonlinear1.batchnorm", lw.in_ch, lw.Kp);
             ok &= ab.fold_conv(&lw.linear1, p + ".linear1", p + ".nonlinear2.batchnorm", BC, lw.in_ch, 1, 1, 0, {{1, lw.Kp, 0, lw.in_ch, 0}});
@@ -364,7 +364,7 @@ void cp_carve(const CamppModel* m, WsCarver& cv, int B, int T, ImageGeo* geo, Cp
     cb->final_x = cv.planes(R, m->final_ch);
     cb->stats = cv.planes(B, 2 * m->final_ch);
     cb->mask = static_cast<float*>(cv.take(size_t(B) * nseg * m->cfg.growth_rate * sizeof(float)));
-    cb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
+    cb->emb_out = static_cast<float*>(cv.take(align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
 }  // namespace
@@ -375,7 +375,7 @@ size_t CamppModel::workspace_bytes(int B, int T) const {
     ImageGeo g[4];
     CpBuffers cb;
     cp_carve(this, cv, B, T, g, &cb);
-    return mc_align_up(cv.off, 256);
+    return align_up(cv.off, 256);
 }
 
 int CamppModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {

@@ -507,23 +507,19 @@ int ppv_aam_backward(const float* emb, const float* W, const int64_t* labels, co
 }
 
 // ---------------------------------------------------------------- GEMM test hook
-static inline size_t au(size_t x, size_t a) { return (x + a - 1) / a * a; }
-size_t ppv_gemm_test_workspace_bytes(int M, int N, int K) {
-    const size_t Kp = au(size_t(K), 64);
-    return au(au(size_t(M), 128) * Kp * 4, 256) + au(au(size_t(N), 256) * Kp * 4, 256) + 256;
-}
 // Both hooks' operands in the workspace, zero-padded: A as planes [2][pad128(M)][Kp], then W as planes [2][pad256(N)][Kp], Kp = pad64(K).
-static int gemm_test_stage(const float* A, const float* W, int M, int N, int K, void* ws, cudaStream_t st, Planes* pa, Planes* pw) {
-    const int Kp = int(au(size_t(K), 64));
-    pa->rows = int64_t(au(size_t(M), 128));
-    pa->ld = Kp;
-    pa->plane_stride = pa->rows * Kp;
-    pa->base = static_cast<__nv_bfloat16*>(ws);
-    pw->rows = int64_t(au(size_t(N), 256));
-    pw->ld = Kp;
-    pw->plane_stride = pw->rows * Kp;
-    pw->base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + au(size_t(pa->plane_stride) * 4, 256));
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, ppv_gemm_test_workspace_bytes(M, N, K), st));
+static void carve_gemm_test(WsCarver& cv, int M, int N, int K, Planes* pa, Planes* pw) {
+    const int Kp = int(align_up(size_t(K), 64));
+    *pa = cv.planes(M, Kp);
+    *pw = cv.planes(int64_t(align_up(size_t(N), 256)), Kp);
+}
+size_t ppv_gemm_test_workspace_bytes(int M, int N, int K) {
+    return carve_extent([&](WsCarver& cv) { Planes pa, pw; carve_gemm_test(cv, M, N, K, &pa, &pw); });
+}
+static int gemm_test_stage(const float* A, const float* W, int M, int N, int K, void* ws, size_t need, cudaStream_t st, Planes* pa, Planes* pw) {
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    carve_gemm_test(cv, M, N, K, pa, pw);
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
     int rc = launch_f32_to_planes(A, M, K, *pa, st);
     if (rc) return rc;
     return launch_f32_to_planes(W, N, K, *pw, st);
@@ -531,13 +527,14 @@ static int gemm_test_stage(const float* A, const float* W, int M, int N, int K, 
 int ppv_gemm_test(const float* A, const float* W, const float* bias, const float* bn_scale, const float* bn_shift, int relu, int M,
                   int N, int K, int block_n, int block_k, int precision, float* out, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(A && W && out && ws, "ppv_gemm_test: null argument");
-    PPV_REQUIRE(ws_bytes >= ppv_gemm_test_workspace_bytes(M, N, K), "ppv_gemm_test: workspace too small");
+    PPV_REQUIRE(A && W && out, "ppv_gemm_test: null argument");
+    const size_t need = ppv_gemm_test_workspace_bytes(M, N, K);
+    if (int rc = check_workspace("ppv_gemm_test", ws, ws_bytes, need, "ppv_gemm_test_workspace_bytes")) return rc;
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Planes pa, pw;
-    rc = gemm_test_stage(A, W, M, N, K, ws, st, &pa, &pw);
+    rc = gemm_test_stage(A, W, M, N, K, ws, need, st, &pa, &pw);
     if (rc) return rc;
     GemmSource src{pa, 0, pa.ld, 0};
     Epilogue ep;
@@ -562,14 +559,15 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
                          const float* bn_shift, int relu, int tanh_, int Tp, int P, int M, int N, int K, int block_n, int precision,
                          void* out, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(A && W && out && ws, "ppv_gemm_test_planes: null argument");
-    PPV_REQUIRE(ws_bytes >= ppv_gemm_test_workspace_bytes(M, N, K), "ppv_gemm_test_planes: workspace too small");
+    PPV_REQUIRE(A && W && out, "ppv_gemm_test_planes: null argument");
+    const size_t need = ppv_gemm_test_workspace_bytes(M, N, K);
+    if (int rc = check_workspace("ppv_gemm_test_planes", ws, ws_bytes, need, "ppv_gemm_test_workspace_bytes")) return rc;
     PPV_REQUIRE(N % 32 == 0 && (Tp == 0 || (M % Tp == 0 && Tp > 2 * P)), "ppv_gemm_test_planes: bad shape");
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Planes pa, pw;
-    rc = gemm_test_stage(A, W, M, N, K, ws, st, &pa, &pw);
+    rc = gemm_test_stage(A, W, M, N, K, ws, need, st, &pa, &pw);
     if (rc) return rc;
     GemmSource src{pa, 0, pa.ld, 0};
     const Planes po{static_cast<__nv_bfloat16*>(out), 0, N, int64_t(M) * N};
@@ -590,25 +588,27 @@ int ppv_gemm_test_planes(const float* A, const float* W, const float* bias, cons
 // ---------------------------------------------------------------- conv2d test hook
 // One conv2d of the 2-D models (ResNetSE, ERes2Net, CAM++) on an input grid laid out as theirs, with their weight reorder, epilogue
 // and tap list (image_plan.h, model_common.h); exactly the kernel `path` names runs, or an error is returned.  Workspace: the input grid [2][pad128(B (H+2) (W+2))][x_ld], then the weight planes [2][pad256(Cout)][k k Cin].
-static size_t conv2d_test_x_bytes(int B, int H, int W, int x_ld) {
-    return au(au(size_t(B) * (H + 2) * (W + 2), 128) * size_t(x_ld) * 4, 256);
+static void carve_conv2d_test(WsCarver& cv, int B, int H, int W, int Cin, int Cout, int k, int x_ld, Planes* xp, Planes* wp) {
+    *xp = cv.planes(int64_t(B) * (H + 2) * (W + 2), x_ld);
+    *wp = cv.planes(int64_t(align_up(size_t(Cout), 256)), k * k * Cin);
 }
 size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, int k, int x_ld) {
     if (x_ld <= 0) x_ld = Cin;
-    return conv2d_test_x_bytes(B, H, W, x_ld) + au(au(size_t(Cout), 256) * k * k * Cin * 4, 256) + 256;
+    return carve_extent([&](WsCarver& cv) { Planes xp, wp; carve_conv2d_test(cv, B, H, W, Cin, Cout, k, x_ld, &xp, &wp); });
 }
 int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
                     int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws, size_t ws_bytes,
                     void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(x && w && out && ws, "ppv_conv2d_test: null argument");
+    PPV_REQUIRE(x && w && out, "ppv_conv2d_test: null argument");
     if (x_ld <= 0) x_ld = Cin;
     PPV_REQUIRE(B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && (k == 1 || k == 3) && stride_h >= 1 && stride_w >= 1,
                 "ppv_conv2d_test: bad shape");
     PPV_REQUIRE(x_col0 >= 0 && x_col0 + Cin <= x_ld, "ppv_conv2d_test: the input columns exceed x_ld");
     PPV_REQUIRE(path >= 0 && path <= 2, "ppv_conv2d_test: path must be 0 (3x3 patch kernel), 1 (pointwise kernel) or 2 (gather-GEMM)");
     PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "ppv_conv2d_test: bad precision");
-    PPV_REQUIRE(ws_bytes >= ppv_conv2d_test_workspace_bytes(B, H, W, Cin, Cout, k, x_ld), "ppv_conv2d_test: workspace too small");
+    if (int rc = check_workspace("ppv_conv2d_test", ws, ws_bytes, ppv_conv2d_test_workspace_bytes(B, H, W, Cin, Cout, k, x_ld),
+                                 "ppv_conv2d_test_workspace_bytes")) return rc;
     const int Hp = H + 2, Wp = W + 2, Ho = (H - 1) / stride_h + 1, Wo = (W - 1) / stride_w + 1;
     const int64_t M = int64_t(B) * Hp * Wp;
     PPV_REQUIRE(M < (int64_t(1) << 31) && Wp + 1 < 32768, "ppv_conv2d_test: grid too large for 32-bit rows / 16-bit tap offsets");
@@ -617,13 +617,10 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // input grid: zero border; x at columns [x_col0, x_col0 + Cin) of the interior; the other columns hold 0x3f3f (0.746 in bf16) in
     // both planes, so a kernel that reads outside its column window is visibly wrong
-    Planes xp;
-    xp.rows = int64_t(au(size_t(M), 128));
-    xp.ld = x_ld;
-    xp.plane_stride = xp.rows * x_ld;
-    xp.base = static_cast<__nv_bfloat16*>(ws);
-    const size_t x_bytes = conv2d_test_x_bytes(B, H, W, x_ld);
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, x_bytes, st));
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes xp, wp;
+    carve_conv2d_test(cv, B, H, W, Cin, Cout, k, x_ld, &xp, &wp);
+    PPV_CUDA_OK(cudaMemsetAsync(xp.base, 0, size_t(2 * xp.plane_stride) * sizeof(__nv_bfloat16), st));
     const size_t pitch = size_t(x_ld) * sizeof(__nv_bfloat16), rows2 = size_t(2 * xp.rows);
     if (x_col0 > 0) PPV_CUDA_OK(cudaMemset2DAsync(xp.base, pitch, 0x3f, size_t(x_col0) * sizeof(__nv_bfloat16), rows2, st));
     if (x_col0 + Cin < x_ld)
@@ -643,10 +640,9 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     ArenaBuilder ab;
     GemmWeights gw;
     ab.put_matrix(&gw, conv_weight_matrix(wh.data(), Cout, Cin, k * k, Cout, {{k * k, Cin, 0, Cin, 0}}), Cout, K);
-    uint8_t* wdev = static_cast<uint8_t*>(ws) + x_bytes;
-    PPV_CUDA_OK(cudaMemcpyAsync(wdev, ab.host.data(), ab.host.size(), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(wp.base, ab.host.data(), ab.host.size(), cudaMemcpyHostToDevice, st));
     PPV_CUDA_OK(cudaStreamSynchronize(st));
-    gw.W.base = reinterpret_cast<__nv_bfloat16*>(wdev + ab.patches[0].off);
+    gw.W.base = wp.base;
     // output grid, zeroed as a plan zeroes its workspace: the kernels store interior positions on the stride grid only
     const int64_t out_plane = int64_t(B) * (Ho + 2) * (Wo + 2) * Cout;
     PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2 * out_plane) * sizeof(__nv_bfloat16), st));
@@ -689,43 +685,42 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
 // ---------------------------------------------------------------- fused attentive-statistics pooling test hook
 // Workspace: W planes [2][C][K], att planes [2][B Tp + 64][K], x planes [2][B Tp + 64][C], out planes [2][B][2C].  The tensor
 // maps of att and x end at row B Tp; the 64 rows behind hold 0x4646 (12672 in bf16) in both planes.
-static size_t asp_test_sizes(int B, int Tp, int C, int K, size_t* off) {
-    const size_t rows = size_t(B) * Tp + 64;
-    const size_t sz[4] = {size_t(C) * K, rows * K, rows * C, size_t(B) * 2 * C};
-    size_t o = 0;
-    for (int i = 0; i < 4; ++i) {
-        off[i] = o;
-        o += au(2 * sz[i] * sizeof(__nv_bfloat16), 256);
-    }
-    return o;
+struct AspTestWs {
+    Planes w, att, x, out;
+};
+static void carve_asp_test(WsCarver& cv, int B, int Tp, int C, int K, AspTestWs* v) {
+    const int64_t rows = int64_t(B) * Tp;
+    auto planes = [&](int64_t nrows, int ld, int64_t alloc_rows) {
+        return Planes{static_cast<__nv_bfloat16*>(cv.take(size_t(2 * alloc_rows * ld) * sizeof(__nv_bfloat16))), nrows, ld, alloc_rows * ld};
+    };
+    v->w = planes(C, K, C);
+    v->att = planes(rows, K, rows + 64);
+    v->x = planes(rows, C, rows + 64);
+    v->out = planes(B, 2 * C, B);
 }
 size_t ppv_asp_fused_test_workspace_bytes(int B, int Tp, int C, int K) {
-    size_t off[4];
-    return asp_test_sizes(B, Tp, C, K, off);
+    return carve_extent([&](WsCarver& cv) { AspTestWs v; carve_asp_test(cv, B, Tp, C, K, &v); });
 }
 int ppv_asp_fused_test(const float* W, const float* att, const float* x, const float* bn_scale, const float* bn_shift,
                        const int* nvalid, int B, int T, int P, int Tp, int C, int K, int precision, int max_ctas, float* out_raw,
                        float* out, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(W && att && x && bn_scale && bn_shift && out_raw && out && ws, "ppv_asp_fused_test: null argument");
+    PPV_REQUIRE(W && att && x && bn_scale && bn_shift && out_raw && out, "ppv_asp_fused_test: null argument");
     PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P && max_ctas >= 0, "ppv_asp_fused_test: bad shape");
     PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "ppv_asp_fused_test: bad precision");
-    size_t off[4];
-    PPV_REQUIRE(ws_bytes >= asp_test_sizes(B, Tp, C, K, off), "ppv_asp_fused_test: workspace too small");
+    if (int rc = check_workspace("ppv_asp_fused_test", ws, ws_bytes, ppv_asp_fused_test_workspace_bytes(B, Tp, C, K),
+                                 "ppv_asp_fused_test_workspace_bytes")) return rc;
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    uint8_t* w8 = static_cast<uint8_t*>(ws);
     const int64_t rows = int64_t(B) * Tp;
-    auto planes = [&](int i, int64_t nrows, int ld, int64_t alloc_rows) {
-        return Planes{reinterpret_cast<__nv_bfloat16*>(w8 + off[i]), nrows, ld, alloc_rows * ld};
-    };
-    const Planes pw = planes(0, C, K, C), pa = planes(1, rows, K, rows + 64), px = planes(2, rows, C, rows + 64),
-                 po = planes(3, B, 2 * C, B);
-    PPV_CUDA_OK(cudaMemsetAsync(w8 + off[1], 0x46, off[3] - off[1], st));
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    AspTestWs v;
+    carve_asp_test(cv, B, Tp, C, K, &v);
+    const Planes &pw = v.w, &pa = v.att, &px = v.x, &po = v.out;
+    PPV_CUDA_OK(cudaMemsetAsync(pa.base, 0x46, reinterpret_cast<uint8_t*>(po.base) - reinterpret_cast<uint8_t*>(pa.base), st));
     if ((rc = launch_f32_to_planes(W, C, K, pw, st)) || (rc = launch_f32_to_planes(att, rows, K, pa, st)) ||
-        (rc = launch_f32_to_planes(x, rows, C, px, st)))
-        return rc;
+        (rc = launch_f32_to_planes(x, rows, C, px, st))) return rc;
     AspFusedParams ap;
     rc = asp_fused_build(&ap, pw, pa, px, bn_scale, bn_shift, po, out_raw, B, T, P, Tp, C, K, 1e-12f);
     if (rc) return rc;
@@ -738,30 +733,31 @@ int ppv_asp_fused_test(const float* W, const float* att, const float* x, const f
 
 // ---------------------------------------------------------------- column statistics test hook
 // Workspace: x planes [2][B Tp][ld], then the output planes [2][B][C or 2C].
-static size_t colstats_test_sizes(int B, int Tp, int ld, int C, size_t* x_bytes) {
-    *x_bytes = au(size_t(B) * Tp * ld * 2 * sizeof(__nv_bfloat16), 256);
-    return *x_bytes + au(size_t(B) * 2 * C * 2 * sizeof(__nv_bfloat16), 256);
+static void carve_colstats_test(WsCarver& cv, int B, int Tp, int ld, int C, __nv_bfloat16** x, __nv_bfloat16** out) {
+    *x = static_cast<__nv_bfloat16*>(cv.take(size_t(B) * Tp * ld * 2 * sizeof(__nv_bfloat16)));
+    *out = static_cast<__nv_bfloat16*>(cv.take(size_t(B) * 2 * C * 2 * sizeof(__nv_bfloat16)));
 }
 size_t ppv_colstats_test_workspace_bytes(int B, int Tp, int ld, int C) {
-    size_t x_bytes;
-    return colstats_test_sizes(B, Tp, ld, C, &x_bytes);
+    return carve_extent([&](WsCarver& cv) { __nv_bfloat16 *x, *out; carve_colstats_test(cv, B, Tp, ld, C, &x, &out); });
 }
 int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int col0, int C, int mode, float eps, float inv_count,
                       const int* nvalid, float* out, float* out_f32, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(x && out && ws, "ppv_colstats_test: null argument");
+    PPV_REQUIRE(x && out, "ppv_colstats_test: null argument");
     PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P && C > 0 && col0 >= 0 && col0 + C <= ld, "ppv_colstats_test: bad shape");
     PPV_REQUIRE(mode >= 0 && mode <= 3 && (mode == 0 || !out_f32), "ppv_colstats_test: mode must be 0-3, out_f32 with mode 0 only");
-    size_t x_bytes;
-    PPV_REQUIRE(ws_bytes >= colstats_test_sizes(B, Tp, ld, C, &x_bytes), "ppv_colstats_test: workspace too small");
+    if (int rc = check_workspace("ppv_colstats_test", ws, ws_bytes, ppv_colstats_test_workspace_bytes(B, Tp, ld, C),
+                                 "ppv_colstats_test_workspace_bytes")) return rc;
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int64_t rows = int64_t(B) * Tp;
     const int oc = mode == 0 ? C : 2 * C;
-    __nv_bfloat16* base = static_cast<__nv_bfloat16*>(ws);
-    const Planes px{base, rows, ld, rows * ld};
-    const Planes po{reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + x_bytes), B, oc, int64_t(B) * oc};
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    __nv_bfloat16 *xb, *ob;
+    carve_colstats_test(cv, B, Tp, ld, C, &xb, &ob);
+    const Planes px{xb, rows, ld, rows * ld};
+    const Planes po{ob, B, oc, int64_t(B) * oc};
     if ((rc = launch_f32_to_planes(x, rows, ld, px, st))) return rc;
     if ((rc = launch_colstats(px, col0, C, B, T, P, Tp, mode, eps, out_f32, po, st, inv_count, nvalid))) return rc;
     return launch_planes_to_f32(po, 0, oc, B, 1, 0, 1, out, st);
@@ -770,34 +766,46 @@ int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int c
 
 // ---------------------------------------------------------------- CAM++ context mask test hook
 // Workspace: h planes [2][B Tp][128], then w1t [128][64], b1 [64], w2t [64][32], b2 [32] fp32.
-static size_t cp_context_test_h_bytes(int B, int Tp) { return au(size_t(B) * Tp * 128 * 2 * sizeof(__nv_bfloat16), 256); }
+struct CpContextTestWs {
+    __nv_bfloat16* h;
+    float *w1t, *b1, *w2t, *b2;
+};
+static void carve_cp_context_test(WsCarver& cv, int B, int Tp, CpContextTestWs* v) {
+    v->h = static_cast<__nv_bfloat16*>(cv.take(size_t(B) * Tp * 128 * 2 * sizeof(__nv_bfloat16)));
+    v->w1t = static_cast<float*>(cv.take(128 * 64 * sizeof(float)));
+    v->b1 = static_cast<float*>(cv.take(64 * sizeof(float)));
+    v->w2t = static_cast<float*>(cv.take(64 * 32 * sizeof(float)));
+    v->b2 = static_cast<float*>(cv.take(32 * sizeof(float)));
+}
 size_t ppv_campplus_context_test_workspace_bytes(int B, int Tp) {
-    return cp_context_test_h_bytes(B, Tp) + au((128 * 64 + 64 + 64 * 32 + 32) * sizeof(float), 256);
+    return carve_extent([&](WsCarver& cv) { CpContextTestWs v; carve_cp_context_test(cv, B, Tp, &v); });
 }
 int ppv_campplus_context_test(const float* h, int B, int T, int P, int Tp, const float* w1, const float* b1, const float* w2,
                               const float* b2, float* out, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(h && w1 && b1 && w2 && b2 && out && ws, "ppv_campplus_context_test: null argument");
+    PPV_REQUIRE(h && w1 && b1 && w2 && b2 && out, "ppv_campplus_context_test: null argument");
     PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P, "ppv_campplus_context_test: bad shape");
-    PPV_REQUIRE(ws_bytes >= ppv_campplus_context_test_workspace_bytes(B, Tp), "ppv_campplus_context_test: workspace too small");
+    if (int rc = check_workspace("ppv_campplus_context_test", ws, ws_bytes, ppv_campplus_context_test_workspace_bytes(B, Tp),
+                                 "ppv_campplus_context_test_workspace_bytes")) return rc;
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int64_t rows = int64_t(B) * Tp;
-    const Planes ph{static_cast<__nv_bfloat16*>(ws), rows, 128, rows * 128};
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    CpContextTestWs v;
+    carve_cp_context_test(cv, B, Tp, &v);
+    const Planes ph{v.h, rows, 128, rows * 128};
     if ((rc = launch_f32_to_planes(h, rows, 128, ph, st))) return rc;
     std::vector<float> w1h(64 * 128), w2h(32 * 64), w1t, w2t;
     PPV_CUDA_OK(cudaMemcpyAsync(w1h.data(), w1, w1h.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
     PPV_CUDA_OK(cudaMemcpyAsync(w2h.data(), w2, w2h.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
     PPV_CUDA_OK(cudaStreamSynchronize(st));
     campplus_context_weights(w1h.data(), w2h.data(), &w1t, &w2t);
-    float* wdev = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + cp_context_test_h_bytes(B, Tp));
-    float *dw1t = wdev, *db1 = dw1t + 128 * 64, *dw2t = db1 + 64, *db2 = dw2t + 64 * 32;
-    PPV_CUDA_OK(cudaMemcpyAsync(dw1t, w1t.data(), w1t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-    PPV_CUDA_OK(cudaMemcpyAsync(dw2t, w2t.data(), w2t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-    PPV_CUDA_OK(cudaMemcpyAsync(db1, b1, 64 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    PPV_CUDA_OK(cudaMemcpyAsync(db2, b2, 32 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    rc = campplus_context_launch(ph, B, T, P, Tp, dw1t, db1, dw2t, db2, out, st);
+    PPV_CUDA_OK(cudaMemcpyAsync(v.w1t, w1t.data(), w1t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(v.w2t, w2t.data(), w2t.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(v.b1, b1, 64 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    PPV_CUDA_OK(cudaMemcpyAsync(v.b2, b2, 32 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    rc = campplus_context_launch(ph, B, T, P, Tp, v.w1t, v.b1, v.w2t, v.b2, out, st);
     if (rc) return rc;
     PPV_CUDA_OK(cudaStreamSynchronize(st));  // the host copies of the weights die here
     return PPV_OK;
@@ -806,24 +814,22 @@ int ppv_campplus_context_test(const float* h, int B, int T, int P, int Tp, const
 
 // ---------------------------------------------------------------- time-axis gather-GEMM test hook
 // Workspace: each input's planes [2][rows][ld], then W planes [2][pad256(N)][sum ncols] (zero rows past N).
-static size_t taps_test_sizes(const ppv_gemm_taps_case* c, size_t* off) {
-    size_t o = 0;
+static void carve_taps_test(WsCarver& cv, const ppv_gemm_taps_case* c, Planes* in, Planes* pw) {
     int K = 0;
     for (int i = 0; i < c->ninputs; ++i) {
-        off[i] = o;
-        o += au(size_t(c->rows[i]) * c->ld[i] * 2 * sizeof(__nv_bfloat16), 256);
+        in[i] = Planes{nullptr, c->rows[i], c->ld[i], c->rows[i] * c->ld[i]};
+        in[i].base = static_cast<__nv_bfloat16*>(cv.take(size_t(2 * in[i].plane_stride) * sizeof(__nv_bfloat16)));
     }
     for (int j = 0; j < c->nsrc; ++j) K += c->src_ncols[j];
-    off[PPV_TAPS_MAX_INPUTS] = o;
-    return o + au(au(size_t(c->N), 256) * K * 2 * sizeof(__nv_bfloat16), 256);
+    *pw = cv.planes(int64_t(align_up(size_t(c->N), 256)), K);
 }
 size_t ppv_gemm_test_taps_workspace_bytes(const ppv_gemm_taps_case* c) {
-    size_t off[PPV_TAPS_MAX_INPUTS + 1];
-    return c ? taps_test_sizes(c, off) : 0;
+    if (!c || c->ninputs > PPV_TAPS_MAX_INPUTS) return 0;
+    return carve_extent([&](WsCarver& cv) { Planes in[PPV_TAPS_MAX_INPUTS], pw; carve_taps_test(cv, c, in, &pw); });
 }
 int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(c && c->W && c->out && ws, "ppv_gemm_test_taps: null argument");
+    PPV_REQUIRE(c && c->W && c->out, "ppv_gemm_test_taps: null argument");
     PPV_REQUIRE(c->ninputs > 0 && c->ninputs <= PPV_TAPS_MAX_INPUTS && c->nsrc > 0 && c->nsrc <= PPV_TAPS_MAX_SOURCES,
                 "ppv_gemm_test_taps: 1-4 inputs and 1-16 sources");
     for (int i = 0; i < c->ninputs; ++i) PPV_REQUIRE(c->x[i] && c->rows[i] > 0 && c->ld[i] > 0, "ppv_gemm_test_taps: bad input");
@@ -837,27 +843,20 @@ int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, v
     PPV_REQUIRE(!c->seg_scale || (c->Tp > 0 && c->seg_len > 0 && c->nseg == (c->T + c->seg_len - 1) / c->seg_len),
                 "ppv_gemm_test_taps: seg_scale needs the time layout and nseg = ceil(T / seg_len)");
     PPV_REQUIRE(c->precision == PPV_PREC_BF16X3 || c->precision == PPV_PREC_BF16, "ppv_gemm_test_taps: bad precision");
-    size_t off[PPV_TAPS_MAX_INPUTS + 1];
-    PPV_REQUIRE(ws_bytes >= taps_test_sizes(c, off), "ppv_gemm_test_taps: workspace too small");
+    if (int rc = check_workspace("ppv_gemm_test_taps", ws, ws_bytes, ppv_gemm_test_taps_workspace_bytes(c),
+                                 "ppv_gemm_test_taps_workspace_bytes")) return rc;
     int rc = check_device();
     if (rc) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    uint8_t* w8 = static_cast<uint8_t*>(ws);
-    Planes in[PPV_TAPS_MAX_INPUTS];
-    for (int i = 0; i < c->ninputs; ++i) {
-        in[i] = Planes{reinterpret_cast<__nv_bfloat16*>(w8 + off[i]), c->rows[i], c->ld[i], c->rows[i] * c->ld[i]};
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes in[PPV_TAPS_MAX_INPUTS], pw;
+    carve_taps_test(cv, c, in, &pw);
+    for (int i = 0; i < c->ninputs; ++i)
         if ((rc = launch_f32_to_planes(c->x[i], c->rows[i], c->ld[i], in[i], st))) return rc;
-    }
     std::vector<GemmSource> srcs;
-    int K = 0;
-    for (int j = 0; j < c->nsrc; ++j) {
-        srcs.push_back(GemmSource{in[c->src_input[j]], c->src_col0[j], c->src_ncols[j], c->src_row_off[j]});
-        K += c->src_ncols[j];
-    }
-    const int64_t wrows = int64_t(au(size_t(c->N), 256));
-    const Planes pw{reinterpret_cast<__nv_bfloat16*>(w8 + off[PPV_TAPS_MAX_INPUTS]), wrows, K, wrows * K};
-    PPV_CUDA_OK(cudaMemsetAsync(pw.base, 0, size_t(2 * wrows * K) * sizeof(__nv_bfloat16), st));
-    if ((rc = launch_f32_to_planes(c->W, c->N, K, pw, st))) return rc;
+    for (int j = 0; j < c->nsrc; ++j) srcs.push_back(GemmSource{in[c->src_input[j]], c->src_col0[j], c->src_ncols[j], c->src_row_off[j]});
+    PPV_CUDA_OK(cudaMemsetAsync(pw.base, 0, size_t(2 * pw.plane_stride) * sizeof(__nv_bfloat16), st));
+    if ((rc = launch_f32_to_planes(c->W, c->N, pw.ld, pw, st))) return rc;
     Epilogue ep;
     if (c->out_f32) {
         ep.out_mode = OUT_F32;
@@ -887,6 +886,14 @@ int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, v
     PPV_GUARD_END
 }
 
+// ppv_gemm_bench's workspace: the GEMM test hooks' operands, then the output [2][pad128(M)][N] (planes or fp32) and the epilogue
+// vectors (bias, BN scale / shift, one bias per Tp-row utterance).
+static void carve_gemm_bench(WsCarver& cv, int M, int N, int K, int Tp, Planes* pa, Planes* pw, Planes* po, float** vec) {
+    carve_gemm_test(cv, M, N, K, pa, pw);
+    *po = cv.planes(M, N);
+    *vec = static_cast<float*>(cv.take((3 + size_t(M / Tp)) * size_t(N) * sizeof(float)));
+}
+
 // Kernel-only timing of the gather-GEMM (tools/gemm_bench.py): operands are converted once, the kernel is launched
 // `iters` times between two CUDA events on `stream`; *ms_per_launch receives the average.  planes_out selects the epilogue:
 //   0  ReLU, fp32 [M,N];   1  ReLU, split-bf16 planes (the layout every model layer writes);
@@ -896,26 +903,22 @@ int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, v
 int ppv_gemm_bench(int M, int N, int K, int block_n, int block_k, int precision, int planes_out, int iters, void* ws, size_t ws_bytes,
                    float* ms_per_launch, void* stream) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(ws && ms_per_launch && iters > 0, "ppv_gemm_bench: bad argument");
+    PPV_REQUIRE(ms_per_launch && iters > 0, "ppv_gemm_bench: bad argument");
     PPV_REQUIRE(planes_out >= 0 && planes_out <= 3, "ppv_gemm_bench: planes_out must be 0-3");
     constexpr int kTp = 306, kP = 4;
     PPV_REQUIRE(planes_out < 2 || M % kTp == 0, "ppv_gemm_bench: model epilogues need M % 306 == 0");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t Kp = au(size_t(K), 64);
-    const size_t a_bytes = au(au(size_t(M), 128) * Kp * 4, 256), w_bytes = au(au(size_t(N), 256) * Kp * 4, 256);
-    const size_t o_bytes = au(au(size_t(M), 128) * size_t(N) * 4, 256);
-    const size_t v_bytes = au((3 + size_t(M / kTp)) * size_t(N) * 4, 256);  // bias, BN scale / shift, per-utterance bias
-    PPV_REQUIRE(ws_bytes >= a_bytes + w_bytes + o_bytes + v_bytes, "ppv_gemm_bench: workspace too small");
+    WsCarver cv;
     Planes pa, pw, po;
-    pa.rows = int64_t(au(size_t(M), 128)); pa.ld = int(Kp); pa.plane_stride = pa.rows * pa.ld; pa.base = static_cast<__nv_bfloat16*>(ws);
-    pw.rows = int64_t(au(size_t(N), 256)); pw.ld = int(Kp); pw.plane_stride = pw.rows * pw.ld;
-    pw.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + a_bytes);
-    po.rows = pa.rows; po.ld = N; po.plane_stride = po.rows * po.ld;
-    po.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + a_bytes + w_bytes);
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0x11, a_bytes + w_bytes, st));  // small finite bf16 values
-    float* vec = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + a_bytes + w_bytes + o_bytes);
-    PPV_CUDA_OK(cudaMemsetAsync(vec, 0x3c, v_bytes, st));  // small finite floats (0.0115)
-    GemmSource src{pa, 0, int(Kp), 0};
+    float* vec;
+    carve_gemm_bench(cv, M, N, K, kTp, &pa, &pw, &po, &vec);
+    const size_t need = align_up(cv.off, 256);
+    if (int rc = check_workspace("ppv_gemm_bench", ws, ws_bytes, need, "see ppv_gemm_bench in ppv_b200.h")) return rc;
+    cv = WsCarver{static_cast<uint8_t*>(ws)};
+    carve_gemm_bench(cv, M, N, K, kTp, &pa, &pw, &po, &vec);
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0x11, reinterpret_cast<uint8_t*>(po.base) - static_cast<uint8_t*>(ws), st));  // small finite bf16 values
+    PPV_CUDA_OK(cudaMemsetAsync(vec, 0x3c, static_cast<uint8_t*>(ws) + need - reinterpret_cast<uint8_t*>(vec), st));  // small finite floats (0.0115)
+    GemmSource src{pa, 0, pa.ld, 0};
     Epilogue ep;
     if (planes_out >= 2) {
         ep = planes_epilogue(po, 0, kTp, kP, kTp - 2 * kP);

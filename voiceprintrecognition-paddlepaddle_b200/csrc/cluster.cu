@@ -34,8 +34,6 @@ constexpr int CL_MAX_N = 8192;
 constexpr int CL_MAX_K = 32;  // eigenpairs / clusters
 constexpr int CL_MAX_TRIALS = 2 + 3;  // 2 + int(log 32)
 
-inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
-
 __device__ __forceinline__ uint32_t ordered_key(float f) {
     const uint32_t u = __float_as_uint(f);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
@@ -731,38 +729,31 @@ __global__ void __launch_bounds__(KM_THREADS) kmeans_kernel(const double* __rest
     if (tid == 0) *inertia = in;
 }
 
-EigWs carve_eig(void* ws, int N, int m) {
-    uint8_t* p = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) { uint8_t* q = p; p += up256(bytes); return q; };
-    EigWs w;
-    w.d = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.e = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.e2 = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.tau = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.p = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.w = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.scal = reinterpret_cast<double*>(take(8 * 8));
-    w.u0 = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.u1 = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.u2 = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.mult = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.x = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.piv = reinterpret_cast<int*>(take(size_t(N) * 4));
-    w.Z = reinterpret_cast<double*>(take(size_t(N) * m * 8));
-    return w;
+void carve_eig(WsCarver& cv, int N, int m, EigWs* w) {
+    auto vec = [&] { return static_cast<double*>(cv.take(size_t(N) * 8)); };
+    w->d = vec();
+    w->e = vec();
+    w->e2 = vec();
+    w->tau = vec();
+    w->p = vec();
+    w->w = vec();
+    w->scal = static_cast<double*>(cv.take(8 * 8));
+    w->u0 = vec();
+    w->u1 = vec();
+    w->u2 = vec();
+    w->mult = vec();
+    w->x = vec();
+    w->piv = static_cast<int*>(cv.take(size_t(N) * 4));
+    w->Z = static_cast<double*>(cv.take(size_t(N) * m * 8));
 }
 
-KmWs carve_km(void* ws, int N, int k) {
-    uint8_t* p = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) { uint8_t* q = p; p += up256(bytes); return q; };
-    KmWs w;
-    w.X = reinterpret_cast<double*>(take(size_t(N) * k * 8));
-    w.xsq = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.closest = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.cum = reinterpret_cast<double*>(take(size_t(N) * 8));
-    w.dcand = reinterpret_cast<double*>(take(size_t(N) * CL_MAX_TRIALS * 8));
-    w.labels_old = reinterpret_cast<int*>(take(size_t(N) * 4));
-    return w;
+void carve_km(WsCarver& cv, int N, int k, KmWs* w) {
+    w->X = static_cast<double*>(cv.take(size_t(N) * k * 8));
+    w->xsq = static_cast<double*>(cv.take(size_t(N) * 8));
+    w->closest = static_cast<double*>(cv.take(size_t(N) * 8));
+    w->cum = static_cast<double*>(cv.take(size_t(N) * 8));
+    w->dcand = static_cast<double*>(cv.take(size_t(N) * CL_MAX_TRIALS * 8));
+    w->labels_old = static_cast<int*>(cv.take(size_t(N) * 4));
 }
 
 int check_n(int N, const char* what) {
@@ -795,16 +786,17 @@ int cluster_laplacian(const float* P, int N, double* L, cudaStream_t st) {
 
 size_t sym_eig_workspace_bytes(int N, int m) {
     if (N < 1 || m < 1) return 0;
-    return 12 * up256(size_t(N) * 8) + up256(64) + up256(size_t(N) * 4) + up256(size_t(N) * m * 8) + 256;
+    return carve_extent([&](WsCarver& cv) { EigWs w; carve_eig(cv, N, m, &w); });
 }
 
 int sym_eig_smallest(double* L, int N, int m, double* evals, double* evecs, void* ws, size_t ws_bytes, cudaStream_t st) {
     if (int rc = check_n(N, "ppv_sym_eig_smallest")) return rc;
-    PPV_REQUIRE(L && evals && evecs && ws, "ppv_sym_eig_smallest: null argument");
+    PPV_REQUIRE(L && evals && evecs, "ppv_sym_eig_smallest: null argument");
     PPV_REQUIRE(m >= 1 && m <= std::min(N, CL_MAX_K), "ppv_sym_eig_smallest: need 1 <= m <= min(N, 32)");
-    PPV_REQUIRE(ws_bytes >= sym_eig_workspace_bytes(N, m) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0,
-                "ppv_sym_eig_smallest: workspace too small / not 256-byte aligned");
-    const EigWs w = carve_eig(ws, N, m);
+    if (int rc = check_workspace("ppv_sym_eig_smallest", ws, ws_bytes, sym_eig_workspace_bytes(N, m), "ppv_sym_eig_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    EigWs w;
+    carve_eig(cv, N, m, &w);
     for (int k = 0; k < N; ++k) {
         house_kernel<<<1, 1024, 0, st>>>(L, N, k, w);
         if (k < N - 1) trail_update_symv_kernel<<<(N - k - 1 + TR_ROWS - 1) / TR_ROWS, 256, 0, st>>>(L, N, k, w);
@@ -821,19 +813,21 @@ int sym_eig_smallest(double* L, int N, int m, double* evals, double* evecs, void
 
 size_t kmeans_workspace_bytes(int N, int k) {
     if (N < 1 || k < 1) return 0;
-    return up256(size_t(N) * k * 8) + 3 * up256(size_t(N) * 8) + up256(size_t(N) * CL_MAX_TRIALS * 8) + up256(size_t(N) * 4) + 256;
+    return carve_extent([&](WsCarver& cv) { KmWs w; carve_km(cv, N, k, &w); });
 }
 
 int kmeans(const double* X, int ld, int N, int k, const double* uniforms, int n_uniforms, int max_iter, int32_t* labels, double* inertia, void* ws,
            size_t ws_bytes, cudaStream_t st) {
     if (int rc = check_n(N, "ppv_kmeans")) return rc;
-    PPV_REQUIRE(X && uniforms && labels && inertia && ws, "ppv_kmeans: null argument");
+    PPV_REQUIRE(X && uniforms && labels && inertia, "ppv_kmeans: null argument");
     PPV_REQUIRE(k >= 1 && k <= std::min(N, CL_MAX_K) && ld >= k && max_iter >= 1, "ppv_kmeans: need 1 <= k <= min(N, 32), ld >= k, max_iter >= 1");
     const int n_trials = 2 + int(log(double(k)));
     PPV_REQUIRE(n_uniforms >= 1 + (k - 1) * n_trials, "ppv_kmeans: need 1 + (k - 1) * (2 + int(log k)) uniforms");
-    PPV_REQUIRE(ws_bytes >= kmeans_workspace_bytes(N, k) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0,
-                "ppv_kmeans: workspace too small / not 256-byte aligned");
-    kmeans_kernel<<<1, KM_THREADS, 0, st>>>(X, ld, N, k, uniforms, max_iter, labels, inertia, carve_km(ws, N, k));
+    if (int rc = check_workspace("ppv_kmeans", ws, ws_bytes, kmeans_workspace_bytes(N, k), "ppv_kmeans_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    KmWs w;
+    carve_km(cv, N, k, &w);
+    kmeans_kernel<<<1, KM_THREADS, 0, st>>>(X, ld, N, k, uniforms, max_iter, labels, inertia, w);
     PPV_LAUNCH_OK("kmeans_kernel");
     return PPV_OK;
 }

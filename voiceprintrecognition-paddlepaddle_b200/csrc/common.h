@@ -1,4 +1,4 @@
-// Shared host/device declarations for libppv_b200: status codes, error reporting, tensor views,
+// Shared host/device declarations for libppv_b200: status codes, error reporting, tensor views, workspace carving,
 // the GEMM launch parameters and the kernel launchers each .cu file exports to the others.
 #pragma once
 #include <cuda.h>
@@ -97,6 +97,47 @@ struct TimeLayout {  // padded time layout of a batch
     int B = 0, T = 0, P = 0, Tp = 0;
     int64_t rows() const { return int64_t(B) * Tp; }
 };
+
+// ---- caller-owned workspaces --------------------------------------------------------------------------
+inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// Lays out a workspace: 256-byte aligned buffers in order from `base`.  Every call that takes a workspace has one carve function;
+// run on a null base it measures the extent its size query returns, run on the workspace it yields the views, so the size and the
+// layout cannot disagree.
+struct WsCarver {
+    uint8_t* base = nullptr;
+    size_t off = 0;
+    void* take(size_t bytes) {
+        off = align_up(off, 256);
+        void* p = base ? base + off : nullptr;
+        off += bytes;
+        return p;
+    }
+    Planes planes(int64_t rows, int ld) {
+        Planes p;
+        p.rows = int64_t(align_up(size_t(rows), 128));
+        p.ld = ld;
+        p.plane_stride = p.rows * ld;
+        p.base = static_cast<__nv_bfloat16*>(take(size_t(2) * p.plane_stride * sizeof(__nv_bfloat16)));
+        return p;
+    }
+};
+// What a size query returns: the extent of `carve(WsCarver&)` run on a null base.
+template <typename Carve>
+size_t carve_extent(const Carve& carve) {
+    WsCarver cv;
+    carve(cv);
+    return align_up(cv.off, 256);
+}
+
+// The check every call makes on its workspace before any launch: `ws` is non-null, 256-byte aligned and holds the `need` bytes the
+// call's carve takes, which the size query `query` returns.
+inline int check_workspace(const char* call, const void* ws, size_t ws_bytes, size_t need, const char* query) {
+    if (ws && ws_bytes >= need && (reinterpret_cast<uintptr_t>(ws) & 255) == 0) return PPV_OK;
+    return fail(PPV_EINVAL, std::string(call) + ": the workspace must be a non-null, 256-byte aligned buffer of at least " + std::to_string(need) +
+                                " bytes (" + query + "); got " + std::to_string(ws_bytes) + " bytes at " +
+                                std::to_string(reinterpret_cast<uintptr_t>(ws)));
+}
 
 // ---- GEMM -----------------------------------------------------------------------------------------
 constexpr int GEMM_BM = 128;
@@ -327,10 +368,14 @@ int audio_prep_reverb(const float* wav, int64_t wav_ld, const int32_t* iparams, 
                       int Lout, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 
 // ---- reverb.cu: the convolution stage of audio_prep_reverb (gains [B][2] in: signal / noise gains, out: normalisation gain of reverb items)
-size_t reverb_workspace_bytes(int B, int max_new_len, int max_rir_len);
+struct ReverbViews {  // per-output-block energies [B][nm], signal block spectra [B][nx][256], response partition spectra [B][nj][256]
+    double* ypart;
+    float2 *xspec, *hspec;
+};
+void carve_reverb(WsCarver& cv, int B, int max_new_len, int max_rir_len, ReverbViews* v);
 int reverb_run(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
                int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
-               int Lout, float* out, float* gains, void* ws, cudaStream_t st);
+               int Lout, float* out, float* gains, const ReverbViews& v, cudaStream_t st);
 
 // ---- spectral.cu ------------------------------------------------------------------------------------
 struct Spectral;

@@ -11,38 +11,32 @@
 
 namespace ppv {
 
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
+// The all-pairs workspace: the normalised rows of A and of B as split-bf16 planes [2][pad128(rows)][pad64(D)].
+static void carve_cosine(WsCarver& cv, int M, int N, int D, Planes* pa, Planes* pb) {
+    const int Dp = int(align_up(size_t(D), 64));
+    *pa = cv.planes(M, Dp);
+    *pb = cv.planes(N, Dp);
+}
 size_t cosine_workspace_bytes(int M, int N, int D) {
-    const size_t Dp = align_up(size_t(D), 64);
-    const size_t a = align_up(size_t(M), 128) * Dp * 2 * sizeof(__nv_bfloat16);
-    const size_t b = align_up(size_t(N), 128) * Dp * 2 * sizeof(__nv_bfloat16);
-    return align_up(a, 256) + align_up(b, 256) + 256;
+    return carve_extent([&](WsCarver& cv) { Planes pa, pb; carve_cosine(cv, M, N, D, &pa, &pb); });
 }
 
 int cosine_matrix(const float* A, const float* Bm, int M, int N, int D, float* out, void* ws, size_t ws_bytes, int precision,
                   cudaStream_t st) {
-    PPV_REQUIRE(A && Bm && out && ws, "cosine_matrix: null argument");
+    PPV_REQUIRE(A && Bm && out, "cosine_matrix: null argument");
     PPV_REQUIRE(M > 0 && N > 0 && D > 0, "cosine_matrix: empty input");
-    PPV_REQUIRE(ws_bytes >= cosine_workspace_bytes(M, N, D), "cosine_matrix: workspace too small");
-    PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "cosine_matrix: workspace must be 256-byte aligned");
-    const int Dp = int(align_up(size_t(D), 64));
+    const size_t need = cosine_workspace_bytes(M, N, D);
+    if (int rc = check_workspace("cosine_matrix", ws, ws_bytes, need, "ppv_cosine_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
     Planes pa, pb;
-    pa.rows = int64_t(align_up(size_t(M), 128));
-    pa.ld = Dp;
-    pa.plane_stride = pa.rows * Dp;
-    pa.base = static_cast<__nv_bfloat16*>(ws);
-    pb.rows = int64_t(align_up(size_t(N), 128));
-    pb.ld = Dp;
-    pb.plane_stride = pb.rows * Dp;
-    pb.base = reinterpret_cast<__nv_bfloat16*>(static_cast<uint8_t*>(ws) + align_up(size_t(pa.plane_stride) * 4, 256));
+    carve_cosine(cv, M, N, D, &pa, &pb);
     // rows beyond M / N must be finite (they only feed masked outputs, but keep them zero)
-    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, cosine_workspace_bytes(M, N, D), st));
+    PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
     normalize_rows_kernel<<<(M + 7) / 8, 256, 0, st>>>(A, M, D, pa);
     PPV_LAUNCH_OK("normalize_rows_kernel(A)");
     normalize_rows_kernel<<<(N + 7) / 8, 256, 0, st>>>(Bm, N, D, pb);
     PPV_LAUNCH_OK("normalize_rows_kernel(B)");
-    GemmSource src{pa, 0, Dp, 0};
+    GemmSource src{pa, 0, pa.ld, 0};
     Epilogue ep;
     ep.out_mode = OUT_F32;
     ep.out = out;

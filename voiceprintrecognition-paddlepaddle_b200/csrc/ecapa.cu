@@ -205,10 +205,10 @@ void carve(const EcapaModel* m, WsCarver& cv, int B, int T, EcBuffers* eb, float
     eb->seh = cv.planes(B, m->se);
     eb->se_mean = static_cast<float*>(cv.take(size_t(B) * C * 4));
     eb->se_scale = static_cast<float*>(cv.take(size_t(B) * C * 4));
-    eb->fold_out = static_cast<float*>(cv.take(mc_align_up(B, 128) * m->att * 4));
+    eb->fold_out = static_cast<float*>(cv.take(align_up(B, 128) * m->att * 4));
     eb->pooled_raw = static_cast<float*>(cv.take(size_t(B) * 2 * C3 * 4));
     eb->raw_logmel = static_cast<float*>(cv.take(size_t(B) * T * m->cfg.input_size * 4));
-    *emb_out = static_cast<float*>(cv.take(mc_align_up(B, 128) * m->cfg.embd_dim * 4));
+    *emb_out = static_cast<float*>(cv.take(align_up(B, 128) * m->cfg.embd_dim * 4));
     eb->nvalid = static_cast<int*>(cv.take(size_t(B) * sizeof(int)));
 }
 
@@ -228,7 +228,7 @@ size_t EcapaModel::workspace_bytes(int B, int T) const {
     EcBuffers eb;
     float* emb;
     carve(this, cv, B, T, &eb, &emb);
-    return mc_align_up(cv.off, 256);
+    return align_up(cv.off, 256);
 }
 
 // ------------------------------------------------------------------------------------------------ plan

@@ -117,7 +117,7 @@ struct Trainer : PlanOwner, EcapaGeometry {
 static int64_t tr_add(std::map<std::string, std::pair<int64_t, int64_t>>& m, int64_t& total, const std::string& name, int64_t numel) {
     const int64_t off = total;
     m[name] = {off, numel};
-    total += int64_t(mc_align_up(size_t(numel), 8));  // 32-byte aligned tensors (vector loads in the epilogues)
+    total += int64_t(align_up(size_t(numel), 8));  // 32-byte aligned tensors (vector loads in the epilogues)
     return off;
 }
 
@@ -143,7 +143,7 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
         l.conv.name = p + ".conv.conv";
         l.conv.Cout = cout;
         l.conv.Cin = l.conv.CinTotal = cin;
-        l.conv.Cinp = int(mc_align_up(size_t(cin), 64));
+        l.conv.Cinp = int(align_up(size_t(cin), 64));
         l.conv.taps = k;
         l.conv.dil = dil;
         l.conv.dgrad = dgrad;
@@ -256,7 +256,7 @@ WgradSplit tr_wgrad_split(const Trainer* t, const TConv& c, int64_t Rp) {
 void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     f->Tp = T + 2 * t->P;
     f->R = int64_t(B) * f->Tp;
-    f->Rp = int64_t(mc_align_up(size_t(f->R), 128));
+    f->Rp = int64_t(align_up(size_t(f->R), 128));
     const int64_t Rp = f->Rp;
     const int C = t->C, C3 = t->C3;
     auto f32 = [&](size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); };
@@ -264,8 +264,8 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     for (int l = 0; l <= t->l_att2(); ++l) {
         const TConv& c = t->conv(l);
         TrBuffers::Layer& w = f->layer[l];
-        w.wf = cv.planes(int64_t(mc_align_up(size_t(c.Cout), 256)), c.taps * c.Cinp);
-        if (c.dgrad) w.wd = cv.planes(int64_t(mc_align_up(size_t(c.Cinp), 256)), c.taps * c.Cout);
+        w.wf = cv.planes(int64_t(align_up(size_t(c.Cout), 256)), c.taps * c.Cinp);
+        if (c.dgrad) w.wd = cv.planes(int64_t(align_up(size_t(c.Cinp), 256)), c.taps * c.Cout);
         if (l == t->l_att2()) break;
         const int Cb = t->L[l].bn.C;
         w.mean = f32(Cb);
@@ -390,7 +390,7 @@ size_t Trainer::workspace_bytes(int B, int T) const {
     WsCarver cv;
     TrBuffers f;
     tr_carve(this, cv, B, T, &f);
-    return mc_align_up(cv.off, 256);
+    return align_up(cv.off, 256);
 }
 
 size_t trainer_workspace_bytes(const Trainer* t, int B, int T) { return t ? t->workspace_bytes(B, T) : 0; }

@@ -229,7 +229,7 @@ void er_carve(const ERes2NetModel* m, WsCarver& cv, int B, int T, ImageGeo* geo,
     const int Tf = geo[4].W;
     eb->flat = cv.planes(int64_t(B) * Tf, m->stats_ch);
     eb->stats = cv.planes(B, 2 * m->stats_ch);
-    eb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
+    eb->emb_out = static_cast<float*>(cv.take(align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
 }  // namespace
@@ -240,7 +240,7 @@ size_t ERes2NetModel::workspace_bytes(int B, int T) const {
     ImageGeo g[5];
     ErBuffers eb;
     er_carve(this, cv, B, T, g, &eb);
-    return mc_align_up(cv.off, 256);
+    return align_up(cv.off, 256);
 }
 
 int ERes2NetModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {

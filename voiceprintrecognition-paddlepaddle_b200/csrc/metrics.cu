@@ -302,50 +302,57 @@ __global__ void __launch_bounds__(256) row_argmax_kernel(const float* __restrict
     }
 }
 
-inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
+struct EerWs {
+    unsigned long long *ka, *kb;  // [n] sort keys, ping-pong
+    uint32_t *hist, *tsum, *tsum_raw;  // [256][nb] digit counts; [nb] per-tile target counts, scanned and raw
+    EerAcc* acc;
+};
+void carve_eer(WsCarver& cv, int64_t n, EerWs* w) {
+    const size_t nb = size_t((n + RS_TILE - 1) / RS_TILE);
+    w->ka = static_cast<unsigned long long*>(cv.take(size_t(n) * 8));
+    w->kb = static_cast<unsigned long long*>(cv.take(size_t(n) * 8));
+    w->hist = static_cast<uint32_t*>(cv.take(256 * nb * 4));
+    w->tsum = static_cast<uint32_t*>(cv.take(nb * 4));
+    w->tsum_raw = static_cast<uint32_t*>(cv.take(nb * 4));
+    w->acc = static_cast<EerAcc*>(cv.take(sizeof(EerAcc)));
+}
 
 }  // namespace
 
 size_t eer_workspace_bytes(int64_t n) {
     if (n <= 0) return 0;
-    const size_t nb = size_t((n + RS_TILE - 1) / RS_TILE);
-    return up256(size_t(n) * 8) * 2 + up256(256 * nb * 4) + up256(nb * 4) * 2 + up256(sizeof(EerAcc)) + 256;
+    return carve_extent([&](WsCarver& cv) { EerWs w; carve_eer(cv, n, &w); });
 }
 
 // Exactly one of `labels` [n] or (`row_labels` [n / ncols], `col_labels` [ncols]).  out: device double[4] = {eer, threshold, min_dcf, n_target}.
 int eer_mindcf(const float* scores, const int32_t* labels, const int32_t* row_labels, const int32_t* col_labels, int ncols, int64_t n,
                double p_target, double c_miss, double c_fa, double* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    PPV_REQUIRE(scores && out && ws, "eer_mindcf: null argument");
+    PPV_REQUIRE(scores && out, "eer_mindcf: null argument");
     PPV_REQUIRE(n >= 2 && n < (int64_t(1) << 32), "eer_mindcf: need 2 <= n < 2^32 scores");
     PPV_REQUIRE((labels != nullptr) != (row_labels != nullptr && col_labels != nullptr), "eer_mindcf: labels XOR (row_labels, col_labels)");
     if (!labels) PPV_REQUIRE(ncols > 0 && n % ncols == 0, "eer_mindcf: n must be rows x ncols");
-    PPV_REQUIRE(ws_bytes >= eer_workspace_bytes(n) && (reinterpret_cast<uintptr_t>(ws) & 255) == 0, "eer_mindcf: workspace too small / unaligned");
+    if (int rc = check_workspace("eer_mindcf", ws, ws_bytes, eer_workspace_bytes(n), "ppv_eer_workspace_bytes")) return rc;
     const int nb = int((n + RS_TILE - 1) / RS_TILE);
-    uint8_t* p = static_cast<uint8_t*>(ws);
-    auto take = [&](size_t bytes) { uint8_t* q = p; p += up256(bytes); return q; };
-    unsigned long long* ka = reinterpret_cast<unsigned long long*>(take(size_t(n) * 8));
-    unsigned long long* kb = reinterpret_cast<unsigned long long*>(take(size_t(n) * 8));
-    uint32_t* hist = reinterpret_cast<uint32_t*>(take(size_t(256) * nb * 4));
-    uint32_t* tsum = reinterpret_cast<uint32_t*>(take(size_t(nb) * 4));
-    uint32_t* tsum_raw = reinterpret_cast<uint32_t*>(take(size_t(nb) * 4));
-    EerAcc* acc = reinterpret_cast<EerAcc*>(take(sizeof(EerAcc)));
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    EerWs w;
+    carve_eer(cv, n, &w);
     const int pack_grid = int(std::min<int64_t>((n + 255) / 256, 132 * 8));
-    eer_pack_kernel<<<pack_grid, 256, 0, st>>>(scores, labels, row_labels, col_labels, ncols, n, ka);
+    eer_pack_kernel<<<pack_grid, 256, 0, st>>>(scores, labels, row_labels, col_labels, ncols, n, w.ka);
     PPV_LAUNCH_OK("eer_pack_kernel");
     for (int pass = 0; pass < RS_PASSES; ++pass) {
         const int shift = 8 * pass;
-        rs_hist_kernel<<<nb, RS_THREADS, 0, st>>>(ka, n, shift, nb, hist);
-        rs_scan_kernel<<<1, 1024, 0, st>>>(hist, 256 * nb);
-        rs_scatter_kernel<<<nb, RS_THREADS, 0, st>>>(ka, kb, n, shift, nb, hist);
+        rs_hist_kernel<<<nb, RS_THREADS, 0, st>>>(w.ka, n, shift, nb, w.hist);
+        rs_scan_kernel<<<1, 1024, 0, st>>>(w.hist, 256 * nb);
+        rs_scatter_kernel<<<nb, RS_THREADS, 0, st>>>(w.ka, w.kb, n, shift, nb, w.hist);
         PPV_LAUNCH_OK("radix sort pass");
-        std::swap(ka, kb);
+        std::swap(w.ka, w.kb);
     }
-    eer_count_kernel<<<nb, RS_THREADS, 0, st>>>(ka, n, tsum);
-    PPV_CUDA_OK(cudaMemcpyAsync(tsum_raw, tsum, size_t(nb) * 4, cudaMemcpyDeviceToDevice, st));
-    rs_scan_kernel<<<1, 1024, 0, st>>>(tsum, nb);
-    eer_init_kernel<<<1, 1, 0, st>>>(acc, tsum, tsum_raw + (nb - 1), nb);
-    eer_sweep_kernel<<<nb, RS_THREADS, 0, st>>>(ka, n, tsum, p_target, c_miss, c_fa, acc);
-    eer_finish_kernel<<<1, 1, 0, st>>>(ka, n, tsum, acc, p_target, c_miss, c_fa, out);
+    eer_count_kernel<<<nb, RS_THREADS, 0, st>>>(w.ka, n, w.tsum);
+    PPV_CUDA_OK(cudaMemcpyAsync(w.tsum_raw, w.tsum, size_t(nb) * 4, cudaMemcpyDeviceToDevice, st));
+    rs_scan_kernel<<<1, 1024, 0, st>>>(w.tsum, nb);
+    eer_init_kernel<<<1, 1, 0, st>>>(w.acc, w.tsum, w.tsum_raw + (nb - 1), nb);
+    eer_sweep_kernel<<<nb, RS_THREADS, 0, st>>>(w.ka, n, w.tsum, p_target, c_miss, c_fa, w.acc);
+    eer_finish_kernel<<<1, 1, 0, st>>>(w.ka, n, w.tsum, w.acc, p_target, c_miss, c_fa, out);
     PPV_LAUNCH_OK("eer sweep");
     return PPV_OK;
 }

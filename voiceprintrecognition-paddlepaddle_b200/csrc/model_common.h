@@ -1,5 +1,5 @@
 // Host-side helpers shared by the model plans: named fp32 weights as loaded through the C ABI, an arena image that is
-// built on the host (split-bf16 weight planes, fp32 vectors) and uploaded once, the workspace carver, and the ECAPA-TDNN geometry.
+// built on the host (split-bf16 weight planes, fp32 vectors) and uploaded once, and the ECAPA-TDNN geometry.
 #pragma once
 #include <string.h>
 
@@ -10,8 +10,6 @@
 #include "common.h"
 
 namespace ppv {
-
-inline size_t mc_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 struct HostWeight {
     std::vector<float> v;
@@ -85,7 +83,7 @@ struct ArenaBuilder {
     std::vector<Patch> patches;
 
     size_t reserve(size_t bytes) {
-        const size_t off = mc_align_up(host.size(), 256);
+        const size_t off = align_up(host.size(), 256);
         host.resize(off + bytes, 0);
         return off;
     }
@@ -109,7 +107,7 @@ struct ArenaBuilder {
     }
     // dense fp32 [N][K] (row-major) -> split planes [2][Npad][K]; rows N..Npad stay zero
     void put_matrix(GemmWeights* gw, const std::vector<double>& m, int N, int K, int n_align = 256) {
-        const int Npad = int(mc_align_up(size_t(N), size_t(n_align)));
+        const int Npad = int(align_up(size_t(N), size_t(n_align)));
         const size_t plane = size_t(Npad) * K;
         const size_t off = reserve(2 * plane * sizeof(__nv_bfloat16));
         __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(host.data() + off);
@@ -198,25 +196,6 @@ struct ArenaBuilder {
     }
 };
 
-struct WsCarver {
-    uint8_t* base = nullptr;
-    size_t off = 0;
-    void* take(size_t bytes) {
-        off = mc_align_up(off, 256);
-        void* p = base ? base + off : nullptr;
-        off += bytes;
-        return p;
-    }
-    Planes planes(int64_t rows, int ld) {
-        Planes p;
-        p.rows = int64_t(mc_align_up(size_t(rows), 128));
-        p.ld = ld;
-        p.plane_stride = p.rows * ld;
-        p.base = static_cast<__nv_bfloat16*>(take(size_t(2) * p.plane_stride * sizeof(__nv_bfloat16)));
-        return p;
-    }
-};
-
 // The geometry of an ECAPA-TDNN config, shared by the inference plan and the training step, after the checks both need:
 // channels [C, C, C, C, 3C], res2net_scale in [2, 8] with chunks of a multiple of 64 channels, kernel sizes [odd, 3, 3, 3, 1].
 struct EcapaGeometry {
@@ -236,7 +215,7 @@ inline int ecapa_geometry(const ppv_ecapa_cfg& cfg, EcapaGeometry* g) {
     g->C3 = 3 * C;
     g->scale = cfg.res2net_scale;
     g->width = C / cfg.res2net_scale;
-    g->Fp = int(mc_align_up(size_t(cfg.input_size), 64));
+    g->Fp = int(align_up(size_t(cfg.input_size), 64));
     g->att = cfg.attention_channels;
     g->se = cfg.se_channels;
     g->P = (cfg.kernel_sizes[0] - 1) / 2 * cfg.dilations[0];

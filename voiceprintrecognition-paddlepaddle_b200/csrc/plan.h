@@ -99,8 +99,7 @@ struct PlanOwner {
     // plans rely on zero borders, zero padding rows and zero padding columns that no step writes.
     int claim_workspace(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
         const size_t need = workspace_bytes(B, T);
-        PPV_REQUIRE(ws && ws_bytes >= need, std::string(prefix) + ": workspace too small (see " + ws_query + ")");
-        PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, std::string(prefix) + ": workspace must be 256-byte aligned");
+        if (int rc = check_workspace(prefix, ws, ws_bytes, need, ws_query)) return rc;
         PPV_CUDA_OK(cudaMemsetAsync(ws, 0, need, st));
         return PPV_OK;
     }

@@ -223,9 +223,9 @@ void rs_carve(const ResNetSEModel* m, WsCarver& cv, int B, int T, Geo* geo, RsBu
     rb->se_mean = cv.planes(B, maxC);
     rb->se_hid = cv.planes(B, 64);
     rb->se_scale = static_cast<float*>(cv.take(size_t(B) * maxC * 4));
-    rb->fold_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->att * 4));
+    rb->fold_out = static_cast<float*>(cv.take(align_up(size_t(B), 128) * m->att * 4));
     rb->pooled_raw = static_cast<float*>(cv.take(size_t(B) * 2 * m->cat * 4));
-    rb->emb_out = static_cast<float*>(cv.take(mc_align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
+    rb->emb_out = static_cast<float*>(cv.take(align_up(size_t(B), 128) * m->cfg.embd_dim * 4));
 }
 
 }  // namespace
@@ -236,7 +236,7 @@ size_t ResNetSEModel::workspace_bytes(int B, int T) const {
     Geo g[5];
     RsBuffers rb;
     rs_carve(this, cv, B, T, g, &rb);
-    return mc_align_up(cv.off, 256);
+    return align_up(cv.off, 256);
 }
 
 int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) {

@@ -241,45 +241,37 @@ __global__ void __launch_bounds__(256) rv_norm_kernel(const int32_t* __restrict_
     }
 }
 
-struct RvLayout {
+struct RvLayout {  // blocks per item at the batch's maximum lengths: signal blocks, response partitions, output blocks
     int nx, nj, nm;
-    size_t ypart, xspec, hspec, total;  // byte offsets from the reverb workspace's start
 };
 
-RvLayout rv_layout(int B, int max_new_len, int max_rir_len) {
+RvLayout rv_layout(int max_new_len, int max_rir_len) {
     RvLayout L;
     L.nx = (max_new_len + RV_P - 1) / RV_P + 1;
     L.nj = (max_rir_len + RV_P - 1) / RV_P;
     L.nm = int((int64_t(max_new_len) + max_rir_len - 1 + RV_P - 1) / RV_P);
-    auto up = [](size_t v) { return (v + 255) / 256 * 256; };
-    L.ypart = 0;
-    L.xspec = up(size_t(B) * L.nm * sizeof(double));
-    L.hspec = L.xspec + size_t(B) * L.nx * RV_P * sizeof(float2);
-    L.total = L.hspec + size_t(B) * L.nj * RV_P * sizeof(float2);
     return L;
 }
 
 }  // namespace
 
-size_t reverb_workspace_bytes(int B, int max_new_len, int max_rir_len) {
-    if (B <= 0 || max_new_len <= 0 || max_rir_len <= 0) return 0;
-    return rv_layout(B, max_new_len, max_rir_len).total;
+void carve_reverb(WsCarver& cv, int B, int max_new_len, int max_rir_len, ReverbViews* v) {
+    const RvLayout L = rv_layout(max_new_len, max_rir_len);
+    v->ypart = static_cast<double*>(cv.take(size_t(B) * L.nm * sizeof(double)));
+    v->xspec = static_cast<float2*>(cv.take(size_t(B) * L.nx * RV_P * sizeof(float2)));
+    v->hspec = static_cast<float2*>(cv.take(size_t(B) * L.nj * RV_P * sizeof(float2)));
 }
 
 int reverb_run(const float* wav, int64_t wav_ld, const int32_t* iparams, const float* fparams, const float* noise, const float* rir_bank,
                int64_t rir_bank_len, const int32_t* rparams, int B, int max_new_len, int max_rir_len, float target_db, int normalize,
-               int Lout, float* out, float* gains, void* ws, cudaStream_t st) {
-    const RvLayout L = rv_layout(B, max_new_len, max_rir_len);
-    uint8_t* base = static_cast<uint8_t*>(ws);
-    double* ypart = reinterpret_cast<double*>(base + L.ypart);
-    float2* xspec = reinterpret_cast<float2*>(base + L.xspec);
-    float2* hspec = reinterpret_cast<float2*>(base + L.hspec);
+               int Lout, float* out, float* gains, const ReverbViews& v, cudaStream_t st) {
+    const RvLayout L = rv_layout(max_new_len, max_rir_len);
     const int fx = (std::max(L.nx, L.nj) + RV_FRAMES - 1) / RV_FRAMES;
     rv_forward_kernel<<<dim3(fx, B, 2), 256, 0, st>>>(wav, wav_ld, iparams, fparams, noise, gains, rir_bank, rir_bank_len, rparams, max_new_len,
-                                                      max_rir_len, L.nx, L.nj, xspec, hspec);
+                                                      max_rir_len, L.nx, L.nj, v.xspec, v.hspec);
     rv_conv_kernel<<<dim3((L.nm + RV_TM - 1) / RV_TM, B), 256, 0, st>>>(iparams, fparams, rparams, rir_bank_len, max_new_len, max_rir_len, L.nx,
-                                                                        L.nj, L.nm, xspec, hspec, normalize, Lout, out, ypart);
-    rv_norm_kernel<<<B, 256, 0, st>>>(iparams, fparams, rparams, rir_bank_len, max_new_len, max_rir_len, L.nm, ypart, target_db, normalize,
+                                                                        L.nj, L.nm, v.xspec, v.hspec, normalize, Lout, out, v.ypart);
+    rv_norm_kernel<<<B, 256, 0, st>>>(iparams, fparams, rparams, rir_bank_len, max_new_len, max_rir_len, L.nm, v.ypart, target_db, normalize,
                                       gains);
     PPV_LAUNCH_OK("reverb kernels");
     return PPV_OK;

@@ -26,7 +26,6 @@ constexpr int SI_THREADS = 160;  // warps 0-3: MMA + top-k warpgroup, warp 4: TM
 constexpr int SI_MAX_D = 256;
 constexpr int SI_MAX_K = 8;
 
-inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 inline int padded_dim(int D) { return int(align_up(size_t(D), 64)); }
 inline int64_t padded_users(int U) { return int64_t(align_up(size_t(U), SI_ROWS)); }
 
@@ -141,7 +140,7 @@ struct SearchParams {
 
 struct SearchPlan {
     int Dp, nchunks, qblocks, ntiles, splits, stages;
-    size_t q_bytes, tile_bytes, smem, q_planes_bytes, cand_bytes;
+    size_t q_bytes, tile_bytes, smem;
 };
 
 SearchPlan plan_search(int Q, int U, int D, int kmax, int num_sms) {
@@ -171,9 +170,22 @@ SearchPlan plan_search(int Q, int U, int D, int kmax, int num_sms) {
         }
     }
     p.splits = best;
-    p.q_planes_bytes = align_up(size_t(p.qblocks) * SI_ROWS * p.Dp * 2 * sizeof(__nv_bfloat16), 256);
-    p.cand_bytes = align_up(size_t(Q) * p.splits * kmax * sizeof(float), 256);
     return p;
+}
+
+// The search workspace: the normalised queries as split-bf16 planes [2][qblocks * 64][Dp], then the per-split candidates
+// [Q][splits][kmax] (similarities, then indices).
+struct SearchWs {
+    Planes q;
+    float* cand_val;
+    int32_t* cand_idx;
+};
+void carve_search(WsCarver& cv, const SearchPlan& pl, int Q, int kmax, SearchWs* w) {
+    const int64_t rows = int64_t(pl.qblocks) * SI_ROWS;
+    w->q = Planes{static_cast<__nv_bfloat16*>(cv.take(size_t(2 * rows * pl.Dp) * sizeof(__nv_bfloat16))), rows, pl.Dp, rows * pl.Dp};
+    const size_t cand = size_t(Q) * pl.splits * kmax;
+    w->cand_val = static_cast<float*>(cv.take(cand * sizeof(float)));
+    w->cand_idx = static_cast<int32_t*>(cv.take(cand * sizeof(int32_t)));
 }
 
 // The three split-bf16 products of one 64 x 64 tile over the whole (padded) D: A = query block, B = index tile.
@@ -336,16 +348,12 @@ __global__ void __launch_bounds__(256) speaker_index_merge_kernel(const float* _
 template <int K>
 int search_launch(const float* queries, int Q, int D, const void* index, int U, int k, int32_t* idx, float* sim, void* ws, cudaStream_t st) {
     const SearchPlan pl = plan_search(Q, U, D, K, device_sm_count());
-    Planes qp;
-    qp.base = static_cast<__nv_bfloat16*>(ws);
-    qp.rows = int64_t(pl.qblocks) * SI_ROWS;
-    qp.ld = pl.Dp;
-    qp.plane_stride = qp.rows * qp.ld;
-    float* cand_val = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + pl.q_planes_bytes);
-    int32_t* cand_idx = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(ws) + pl.q_planes_bytes + pl.cand_bytes);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    SearchWs w;
+    carve_search(cv, pl, Q, K, &w);
     SearchParams p;
     memset(&p, 0, sizeof(p));
-    int rc = encode_planes_map_ex(&p.mapQ, qp, 64, SI_ROWS, 128);
+    int rc = encode_planes_map_ex(&p.mapQ, w.q, 64, SI_ROWS, 128);
     if (rc) return rc;
     rc = encode_planes_map_ex(&p.mapX, index_planes(const_cast<void*>(index), U, D), 64, SI_ROWS, 128);
     if (rc) return rc;
@@ -355,19 +363,19 @@ int search_launch(const float* queries, int Q, int D, const void* index, int U, 
     p.ntiles = pl.ntiles;
     p.splits = pl.splits;
     p.stages = pl.stages;
-    p.cand_val = cand_val;
-    p.cand_idx = cand_idx;
+    p.cand_val = w.cand_val;
+    p.cand_idx = w.cand_idx;
     // query rows past Q feed only rows that are never stored; keep them zero all the same
-    if (qp.rows > Q) {
-        PPV_CUDA_OK(cudaMemsetAsync(qp.hi() + int64_t(Q) * qp.ld, 0, size_t(qp.rows - Q) * qp.ld * sizeof(__nv_bfloat16), st));
-        PPV_CUDA_OK(cudaMemsetAsync(qp.lo() + int64_t(Q) * qp.ld, 0, size_t(qp.rows - Q) * qp.ld * sizeof(__nv_bfloat16), st));
+    if (w.q.rows > Q) {
+        PPV_CUDA_OK(cudaMemsetAsync(w.q.hi() + int64_t(Q) * w.q.ld, 0, size_t(w.q.rows - Q) * w.q.ld * sizeof(__nv_bfloat16), st));
+        PPV_CUDA_OK(cudaMemsetAsync(w.q.lo() + int64_t(Q) * w.q.ld, 0, size_t(w.q.rows - Q) * w.q.ld * sizeof(__nv_bfloat16), st));
     }
-    normalize_rows_kernel<<<(Q + 7) / 8, 256, 0, st>>>(queries, Q, D, qp);
+    normalize_rows_kernel<<<(Q + 7) / 8, 256, 0, st>>>(queries, Q, D, w.q);
     PPV_LAUNCH_OK("normalize_rows_kernel(queries)");
     PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(speaker_index_search_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, SI_SMEM_MAX)));
     speaker_index_search_kernel<K><<<dim3(pl.qblocks, pl.splits), SI_THREADS, pl.smem, st>>>(p);
     PPV_LAUNCH_OK("speaker_index_search_kernel");
-    speaker_index_merge_kernel<K><<<(Q + 7) / 8, 256, 0, st>>>(cand_val, cand_idx, Q, pl.splits, k, idx, sim);
+    speaker_index_merge_kernel<K><<<(Q + 7) / 8, 256, 0, st>>>(w.cand_val, w.cand_idx, Q, pl.splits, k, idx, sim);
     PPV_LAUNCH_OK("speaker_index_merge_kernel");
     return PPV_OK;
 }
@@ -403,19 +411,20 @@ int speaker_index_build(const float* E, int n, int D, const int32_t* order, cons
 
 size_t speaker_index_search_workspace_bytes(int Q, int U, int D, int k) {
     if (Q < 1 || U < 1 || D < 1 || D > SI_MAX_D || k < 1 || k > SI_MAX_K) return 0;
-    const SearchPlan pl = plan_search(Q, U, D, k == 1 ? 1 : SI_MAX_K, device_sm_count());
-    return pl.q_planes_bytes + 2 * pl.cand_bytes;
+    const int kmax = k == 1 ? 1 : SI_MAX_K;
+    const SearchPlan pl = plan_search(Q, U, D, kmax, device_sm_count());
+    return carve_extent([&](WsCarver& cv) { SearchWs w; carve_search(cv, pl, Q, kmax, &w); });
 }
 
 int speaker_index_search(const float* queries, int Q, int D, const void* index, size_t index_bytes, int U, int k, int32_t* idx, float* sim,
                          void* ws, size_t ws_bytes, cudaStream_t st) {
     int rc = check_search_shape(Q, U, D, k);
     if (rc) return rc;
-    PPV_REQUIRE(queries && index && idx && sim && ws, "speaker_index_search: null argument");
+    PPV_REQUIRE(queries && index && idx && sim, "speaker_index_search: null argument");
     PPV_REQUIRE(index_bytes >= speaker_index_bytes(U, D), "speaker_index_search: index buffer smaller than ppv_speaker_index_bytes(U, D)");
-    PPV_REQUIRE(ws_bytes >= speaker_index_search_workspace_bytes(Q, U, D, k), "speaker_index_search: workspace too small");
-    PPV_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0 && (reinterpret_cast<uintptr_t>(index) & 255) == 0,
-                "speaker_index_search: workspace and index must be 256-byte aligned");
+    PPV_REQUIRE((reinterpret_cast<uintptr_t>(index) & 255) == 0, "speaker_index_search: index must be 256-byte aligned");
+    if (int rc = check_workspace("speaker_index_search", ws, ws_bytes, speaker_index_search_workspace_bytes(Q, U, D, k),
+                                 "ppv_speaker_index_search_workspace_bytes")) return rc;
     return k == 1 ? search_launch<1>(queries, Q, D, index, U, k, idx, sim, ws, st) : search_launch<SI_MAX_K>(queries, Q, D, index, U, k, idx, sim, ws, st);
 }
 

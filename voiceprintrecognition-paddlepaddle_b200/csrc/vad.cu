@@ -262,30 +262,21 @@ int tile_frames_for(const ppv_vad_cfg& c) {
     return std::max(1, std::min(VAD_TILE_FRAMES, (VAD_STAGE_FLOATS - 3 - c.window) / c.shift + 1));
 }
 
-struct VadLayout {
-    size_t meta, energy, tile_sum, thr, count, base, total;
+struct VadWs {
+    int64_t* meta;  // [3][R + 1] sample, frame and tile offsets
+    double *energy, *tile_sum, *thr;
+    int2 *count, *base;
 };
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 // Sized from R and the sample total alone: T_r <= L_r / shift (window >= shift), tiles <= frames / tile_frames + R.
-VadLayout vad_layout(const ppv_vad_cfg& c, int R, int64_t total_samples) {
+void carve_vad(WsCarver& cv, const ppv_vad_cfg& c, int R, int64_t total_samples, VadWs* w) {
     const int64_t frames = total_samples / c.shift;
     const int64_t tiles = frames / tile_frames_for(c) + R;
-    VadLayout l;
-    size_t o = 0;
-    l.meta = o;
-    o += align256(size_t(3) * (R + 1) * sizeof(int64_t));
-    l.energy = o;
-    o += align256(size_t(frames) * sizeof(double));
-    l.tile_sum = o;
-    o += align256(size_t(tiles) * sizeof(double));
-    l.thr = o;
-    o += align256(size_t(R) * sizeof(double));
-    l.count = o;
-    o += align256(size_t(tiles) * sizeof(int2));
-    l.base = o;
-    o += align256(size_t(tiles) * sizeof(int2));
-    l.total = o;
-    return l;
+    w->meta = static_cast<int64_t*>(cv.take(size_t(3) * (R + 1) * sizeof(int64_t)));
+    w->energy = static_cast<double*>(cv.take(size_t(frames) * sizeof(double)));
+    w->tile_sum = static_cast<double*>(cv.take(size_t(tiles) * sizeof(double)));
+    w->thr = static_cast<double*>(cv.take(size_t(R) * sizeof(double)));
+    w->count = static_cast<int2*>(cv.take(size_t(tiles) * sizeof(int2)));
+    w->base = static_cast<int2*>(cv.take(size_t(tiles) * sizeof(int2)));
 }
 
 }  // namespace
@@ -297,17 +288,16 @@ int64_t vad_num_frames(const ppv_vad_cfg& c, int64_t L) {
 
 size_t vad_workspace_bytes(const ppv_vad_cfg& c, int R, int64_t total_samples) {
     if (!vad_cfg_ok(c, nullptr) || R < 1 || total_samples < 0) return 0;
-    return vad_layout(c, R, total_samples).total;
+    return carve_extent([&](WsCarver& cv) { VadWs w; carve_vad(cv, c, R, total_samples, &w); });
 }
 
 int vad_energy(const ppv_vad_cfg& c, const float* wav, const int64_t* sample_offsets, int R, double* log_energy, uint8_t* voiced,
                int32_t* runs, int64_t run_cap, int32_t* n_runs, void* ws, size_t ws_bytes, cudaStream_t st) {
     std::string why;
     PPV_REQUIRE(vad_cfg_ok(c, &why), "vad_energy: " + why);
-    PPV_REQUIRE(wav && sample_offsets && voiced && runs && n_runs && ws, "vad_energy: null argument");
+    PPV_REQUIRE(wav && sample_offsets && voiced && runs && n_runs, "vad_energy: null argument");
     PPV_REQUIRE(R >= 1, "vad_energy: R must be >= 1 (got " + std::to_string(R) + ")");
     PPV_REQUIRE(reinterpret_cast<uintptr_t>(wav) % 4 == 0, "vad_energy: wav must be 4-byte aligned");
-    PPV_REQUIRE(reinterpret_cast<uintptr_t>(ws) % 256 == 0, "vad_energy: workspace must be 256-byte aligned");
     PPV_REQUIRE(sample_offsets[0] >= 0, "vad_energy: sample_offsets[0] must be >= 0");
     const int tf = tile_frames_for(c);
     std::vector<int64_t> meta(size_t(3) * (R + 1));
@@ -329,34 +319,29 @@ int vad_energy(const ppv_vad_cfg& c, const float* wav, const int64_t* sample_off
     PPV_REQUIRE(frames < (int64_t(1) << 31), "vad_energy: more than 2^31 - 1 frames in the batch");
     PPV_REQUIRE(run_cap >= need_runs, "vad_energy: run capacity " + std::to_string(run_cap) + " < " + std::to_string(need_runs) +
                                           " (sum over recordings of ceil(T / 2))");
-    const VadLayout lay = vad_layout(c, R, so[R]);
-    PPV_REQUIRE(ws_bytes >= lay.total, "vad_energy: workspace of " + std::to_string(ws_bytes) + " bytes < " + std::to_string(lay.total) +
-                                           " (ppv_vad_workspace_bytes)");
-    char* w = static_cast<char*>(ws);
-    int64_t* d_meta = reinterpret_cast<int64_t*>(w + lay.meta);
-    double* energy = log_energy ? log_energy : reinterpret_cast<double*>(w + lay.energy);
-    double* tile_sum = reinterpret_cast<double*>(w + lay.tile_sum);
-    double* thr = reinterpret_cast<double*>(w + lay.thr);
-    int2* count = reinterpret_cast<int2*>(w + lay.count);
-    int2* base = reinterpret_cast<int2*>(w + lay.base);
+    if (int rc = check_workspace("vad_energy", ws, ws_bytes, vad_workspace_bytes(c, R, so[R]), "ppv_vad_workspace_bytes")) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    VadWs w;
+    carve_vad(cv, c, R, so[R], &w);
+    double* energy = log_energy ? log_energy : w.energy;
     if (tiles == 0) {
         PPV_CUDA_OK(cudaMemsetAsync(n_runs, 0, sizeof(int32_t), st));
         return PPV_OK;
     }
-    PPV_CUDA_OK(cudaMemcpyAsync(d_meta, meta.data(), meta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-    const VadGeom g{d_meta, d_meta + (R + 1), d_meta + 2 * (R + 1), R, c.window, c.shift, tf};
+    PPV_CUDA_OK(cudaMemcpyAsync(w.meta, meta.data(), meta.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    const VadGeom g{w.meta, w.meta + (R + 1), w.meta + 2 * (R + 1), R, c.window, c.shift, tf};
     const size_t smem = size_t((tf - 1) * c.shift + c.window + 3) * sizeof(float);
     PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(vad_energy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                          int(VAD_STAGE_FLOATS * sizeof(float)))));
-    vad_energy_kernel<<<unsigned(tiles), VAD_THREADS, smem, st>>>(wav, g, energy, tile_sum);
+    vad_energy_kernel<<<unsigned(tiles), VAD_THREADS, smem, st>>>(wav, g, energy, w.tile_sum);
     PPV_LAUNCH_OK("vad_energy_kernel");
-    vad_threshold_kernel<<<R, VAD_THREADS, 0, st>>>(g, tile_sum, c.energy_threshold, c.energy_mean_scale, thr);
+    vad_threshold_kernel<<<R, VAD_THREADS, 0, st>>>(g, w.tile_sum, c.energy_threshold, c.energy_mean_scale, w.thr);
     PPV_LAUNCH_OK("vad_threshold_kernel");
-    vad_decide_kernel<<<unsigned(tiles), VAD_TILE_THREADS, 0, st>>>(g, energy, thr, c.frames_context, c.proportion_threshold, voiced, count);
+    vad_decide_kernel<<<unsigned(tiles), VAD_TILE_THREADS, 0, st>>>(g, energy, w.thr, c.frames_context, c.proportion_threshold, voiced, w.count);
     PPV_LAUNCH_OK("vad_decide_kernel");
-    vad_scan_kernel<<<1, VAD_SCAN_THREADS, 0, st>>>(count, tiles, base, n_runs);
+    vad_scan_kernel<<<1, VAD_SCAN_THREADS, 0, st>>>(w.count, tiles, w.base, n_runs);
     PPV_LAUNCH_OK("vad_scan_kernel");
-    vad_emit_kernel<<<unsigned(tiles), VAD_TILE_THREADS, 0, st>>>(g, voiced, base, runs);
+    vad_emit_kernel<<<unsigned(tiles), VAD_TILE_THREADS, 0, st>>>(g, voiced, w.base, runs);
     PPV_LAUNCH_OK("vad_emit_kernel");
     return PPV_OK;
 }
