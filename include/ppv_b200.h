@@ -531,6 +531,33 @@ typedef struct {
 size_t ppv_gemm_test_taps_workspace_bytes(const ppv_gemm_taps_case* c);
 int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, void* stream);
 
+/* Test hook for the Res2Net convs of an SE-Res2Net block (not a reference entry point): y_1 = f_1(x_1), y_j = f_j(x_j + y_{j-1}),
+ * f_j = BN(ReLU(conv_k3,dil + bias)) on 64-channel chunks, for j = 1..nconv, through the launches the ECAPA-TDNN plan builds.
+ * variant PPV_RES2_CHAIN: res2chain_kernel (T + 8 <= 384); PPV_RES2_CHAIN_PAIRED: res2chain_pair_kernel (T + 8 <= 320);
+ * PPV_RES2_PER_CONV: one res2conv_kernel per conv.  x [B*Tp, ld_x] fp32 in the padded time layout (Tp = T + 8, P = 4: frame t of
+ * utterance b at row b*Tp + 4 + t), chunk c at columns [64c, 64c + 64); the chain builds its reflect halo rows itself, the per-conv
+ * path reads them from x.  w [nconv][64][64][3], bias / bn_scale / bn_shift [nconv][64] fp32.  y [B*Tp + 64, ld_y] fp32: conv j
+ * writes columns [64j, 64j + 64) of rows [0, B*Tp) (the chain: every row, the per-conv path: the valid rows and their reflect
+ * mirrors).  x and y are split into planes here and come back whole, decoded as hi + lo (y with PPV_PREC_BF16: its hi plane, the
+ * only one the convs read and the chain stores): a position no kernel stores keeps its value.  max_ctas: the grid's CTA count cap (0: every SM).  A case the builds reject is PPV_EINVAL before any launch.
+ * ws >= ppv_res2net_test_workspace_bytes.  Synchronises `stream` while it prepares the weights. */
+#define PPV_RES2_CHAIN 0
+#define PPV_RES2_CHAIN_PAIRED 1
+#define PPV_RES2_PER_CONV 2
+size_t ppv_res2net_test_workspace_bytes(int nconv, int B, int T, int ld_x, int ld_y);
+int ppv_res2net_test(float* x, int ld_x, const float* w, const float* bias, const float* bn_scale, const float* bn_shift, int nconv,
+                     int B, int T, int dil, int variant, int precision, int max_ctas, float* y, int ld_y, void* ws, size_t ws_bytes,
+                     void* stream);
+
+/* Test hook for the skinny linear kernel (not a reference entry point): out[m, out_col0 + n] = act(sum_k x[m, x_col0 + k] W[n, k]
+ * + bias[n]) through skinny_linear_launch, as the SE excitation runs it.  x [M, ld] and W [N, K] fp32 are split into planes here;
+ * bias [N] may be NULL; act 0: none, 1: ReLU, 2: sigmoid.  out [M, out_ld] fp32: out_planes 0 writes it directly, 1 writes
+ * split planes initialised from it and decodes them back whole as hi + lo.  A shape the kernel does not take is PPV_EINVAL before
+ * any launch.  ws >= ppv_skinny_linear_test_workspace_bytes. */
+size_t ppv_skinny_linear_test_workspace_bytes(int M, int ld, int N, int K, int out_ld);
+int ppv_skinny_linear_test(const float* x, int M, int ld, int x_col0, const float* W, int N, int K, const float* bias, int act,
+                           int out_planes, float* out, int out_ld, int out_col0, void* ws, size_t ws_bytes, void* stream);
+
 /* Kernel-only timing of the gather-GEMM (tools/gemm_bench.py); ws >= 4*(pad128(M)*pad64(K) + pad256(N)*pad64(K) + pad128(M)*N)
  * bytes + 4*(3 + M/306)*N rounded up to 256.  planes_out: 0 ReLU to fp32, 1 ReLU to planes, 2 bias + ReLU + BN to planes over the
  * padded time layout (Tp = 306, P = 4), 3 the same + per-utterance bias + tanh (ASP attention TDNN); 2 and 3 need M % 306 == 0. */

@@ -294,13 +294,41 @@ def case_gemm_test_taps():
     return lib.ppv_gemm_test_taps_workspace_bytes(C.byref(c)), run
 
 
+def case_res2net_test(variant):
+    lib = _lib.load()
+    nconv, B, T, dil, ld = 3, 3, 60, 2, 320
+    Tp = T + 8
+    w, bias = randn(nconv, 64, 64, 3, seed=39) * 0.07, randn(nconv, 64, seed=40)
+    scale, shift = randn(nconv, 64, seed=41), randn(nconv, 64, seed=42)
+
+    def run(ws, nb):  # x is read and written back: its FILL bytes are a small finite input
+        xo, y = out((B * Tp, ld), torch.float32), out((B * Tp + 64, ld), torch.float32)
+        return lib.ppv_res2net_test(_lib.ptr(xo), ld, _lib.ptr(w), _lib.ptr(bias), _lib.ptr(scale), _lib.ptr(shift), nconv, B, T, dil,
+                                    variant, _lib.PPV_PREC_BF16X3, 0, _lib.ptr(y), ld, V(ws), nb, stream()), [xo, y]
+    return lib.ppv_res2net_test_workspace_bytes(nconv, B, T, ld, ld), run
+
+
+def case_skinny_linear_test():
+    lib = _lib.load()
+    M, ld, x_col0, N, K, out_ld = 37, 272, 8, 130, 256, 136
+    x, W, bias = randn(M, ld, seed=43), randn(N, K, seed=44) * 0.1, randn(N, seed=45)
+
+    def run(ws, nb):
+        o = out((M, out_ld), torch.float32)
+        return lib.ppv_skinny_linear_test(_lib.ptr(x), M, ld, x_col0, _lib.ptr(W), N, K, _lib.ptr(bias), 1, 1, _lib.ptr(o), out_ld, 3, V(ws),
+                                          nb, stream()), [o]
+    return lib.ppv_skinny_linear_test_workspace_bytes(M, ld, N, K, out_ld), run
+
+
 CASES = {
     "aam_forward_backward": case_aam, "cosine_matrix": case_cosine, "eer_mindcf": case_eer, "sym_eig_smallest": case_sym_eig,
     "kmeans": case_kmeans, "vad_energy": case_vad, "audio_prep": case_audio_prep, "audio_prep_reverb": case_audio_prep_reverb,
     "speaker_index_search_k1": lambda: case_speaker_index_search(1), "speaker_index_search_k5": lambda: case_speaker_index_search(5),
     "gemm_test": case_gemm_test, "gemm_test_planes": case_gemm_test_planes, "conv2d_test": case_conv2d_test,
     "asp_fused_test": case_asp_fused_test, "colstats_test": case_colstats_test, "campplus_context_test": case_campplus_context_test,
-    "gemm_test_taps": case_gemm_test_taps,
+    "gemm_test_taps": case_gemm_test_taps, "res2net_test_chain": lambda: case_res2net_test(_lib.PPV_RES2_CHAIN),
+    "res2net_test_chain_paired": lambda: case_res2net_test(_lib.PPV_RES2_CHAIN_PAIRED),
+    "res2net_test_per_conv": lambda: case_res2net_test(_lib.PPV_RES2_PER_CONV), "skinny_linear_test": case_skinny_linear_test,
 }
 
 

@@ -5,7 +5,8 @@ the old byte formulas counted memory no carve takes:
   - aam, cosine, eer, k-means, sym-eig, gemm_test, conv2d_test: the trailing 256 bytes of slack (no kernel touches memory past
     the last buffer of its call);
   - sym-eig: also one N-double buffer that the carve never took.
-Every other size is unchanged, and every query still returns 0 where it returned 0 (shapes its call rejects)."""
+Every other size is unchanged, and every query still returns 0 where it returned 0 (shapes its call rejects).  The Res2Net and skinny
+linear test hooks came later: their entries are the sizes of their carves when they were added."""
 import ctypes as C
 
 import pytest
@@ -52,6 +53,8 @@ QUERY = {
     "asp_fused_test": "ppv_asp_fused_test_workspace_bytes",
     "colstats_test": "ppv_colstats_test_workspace_bytes",
     "campplus_context_test": "ppv_campplus_context_test_workspace_bytes",
+    "res2net_test": "ppv_res2net_test_workspace_bytes",
+    "skinny_linear_test": "ppv_skinny_linear_test_workspace_bytes",
 }
 
 
@@ -148,6 +151,17 @@ PARENT = {'aam': {(1, 1, 1): 1792,
  'asp_fused_test': {(1, 1, 1, 1): 1536, (1, 5, 64, 64): 52224, (3, 101, 1536, 128): 3266048, (4, 306, 1536, 128): 9408512},
  'colstats_test': {(1, 1, 1, 1): 512, (3, 101, 512, 100): 623104, (4, 306, 1536, 1536): 7569408},
  'campplus_context_test': {(1, 1): 41984, (3, 101): 196608, (4, 306): 668160},
+ 'res2net_test': {(1, 1, 5, 128, 128): 144384,
+                  (1, 2, 5, 128, 128): 157696,
+                  (7, 3, 120, 512, 576): 3096576,
+                  (2, 531, 120, 512, 576): 296239104,
+                  (7, 3, 3000, 512, 512): 38371328,
+                  (7, 256, 298, 512, 512): 322273280},
+ 'skinny_linear_test': {(1, 8, 1, 8, 1): 8704,
+                        (17, 528, 17, 520, 25): 549376,
+                        (256, 512, 128, 512, 128): 917504,
+                        (256, 128, 512, 128, 512): 917504,
+                        (4096, 1040, 520, 1024, 528): 28311552},
  'gemm_test_taps': {None: 0,
                     ((300,), (64,), (64, 64, 64), 100): 273408,
                     ((1000, 999), (128, 80), (128, 64), 512): 1224960,
@@ -173,4 +187,5 @@ def test_every_stateless_query_is_covered():
 
 
 # queries without an early return 0 (their calls reject shapes in other ways)
-ZERO_FREE = {"aam", "cosine", "gemm_test", "conv2d_test", "asp_fused_test", "colstats_test", "campplus_context_test"}
+ZERO_FREE = {"aam", "cosine", "gemm_test", "conv2d_test", "asp_fused_test", "colstats_test", "campplus_context_test", "res2net_test",
+             "skinny_linear_test"}

@@ -886,6 +886,142 @@ int ppv_gemm_test_taps(const ppv_gemm_taps_case* c, void* ws, size_t ws_bytes, v
     PPV_GUARD_END
 }
 
+// ---------------------------------------------------------------- Res2Net test hook
+// Workspace: x planes [2][B Tp][ld_x], y planes [2][B Tp + 64][ld_y], then per conv j the weight planes [2][128][(j ? 2 : 1) 192].
+// y's tensor maps take in its 64 tail rows, so a store past the last utterance lands where the caller sees it.
+struct Res2NetTestWs {
+    Planes x, y, w[RES2CHAIN_MAX];
+};
+static void carve_res2net_test(WsCarver& cv, int nconv, int B, int Tp, int ld_x, int ld_y, Res2NetTestWs* v) {
+    const int64_t rows = int64_t(B) * Tp;
+    auto planes = [&](int64_t nrows, int ld) {
+        return Planes{static_cast<__nv_bfloat16*>(cv.take(size_t(2 * nrows * ld) * sizeof(__nv_bfloat16))), nrows, ld, nrows * ld};
+    };
+    v->x = planes(rows, ld_x);
+    v->y = planes(rows + 64, ld_y);
+    for (int j = 0; j < nconv && j < RES2CHAIN_MAX; ++j) v->w[j] = cv.planes(64, (j ? 2 : 1) * 3 * 64);
+}
+size_t ppv_res2net_test_workspace_bytes(int nconv, int B, int T, int ld_x, int ld_y) {
+    return carve_extent([&](WsCarver& cv) { Res2NetTestWs v; carve_res2net_test(cv, nconv, B, T + 8, ld_x, ld_y, &v); });
+}
+int ppv_res2net_test(float* x, int ld_x, const float* w, const float* bias, const float* bn_scale, const float* bn_shift, int nconv, int B,
+                     int T, int dil, int variant, int precision, int max_ctas, float* y, int ld_y, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && w && bias && bn_scale && bn_shift && y, "ppv_res2net_test: null argument");
+    constexpr int P = 4;  // the padding of every ECAPA-TDNN layer's output: the largest dilation
+    PPV_REQUIRE(nconv >= 1 && nconv <= RES2CHAIN_MAX && B > 0 && T > P && max_ctas >= 0, "ppv_res2net_test: bad shape");
+    PPV_REQUIRE(ld_x >= 64 * (nconv + 1) && ld_y >= 64 * (nconv + 1) && ld_x % 8 == 0 && ld_y % 8 == 0,
+                "ppv_res2net_test: x and y need 64 (nconv + 1) columns and a 16-byte row pitch");
+    PPV_REQUIRE(variant >= PPV_RES2_CHAIN && variant <= PPV_RES2_PER_CONV, "ppv_res2net_test: bad variant");
+    PPV_REQUIRE(precision == PPV_PREC_BF16X3 || precision == PPV_PREC_BF16, "ppv_res2net_test: bad precision");
+    const int Tp = T + 2 * P;
+    if (int rc = check_workspace("ppv_res2net_test", ws, ws_bytes, ppv_res2net_test_workspace_bytes(nconv, B, T, ld_x, ld_y),
+                                 "ppv_res2net_test_workspace_bytes")) return rc;
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Res2NetTestWs v;
+    carve_res2net_test(cv, nconv, B, Tp, ld_x, ld_y, &v);
+    const int R = B * Tp;
+    // the launches, built as the ECAPA-TDNN plan builds them (ecapa.cu); the builds reject what the kernels do not take, before any launch
+    Res2ChainParams cp;
+    Res2Params rp[RES2CHAIN_MAX];
+    if (variant == PPV_RES2_PER_CONV) {
+        for (int j = 1; j <= nconv; ++j) {
+            Epilogue ep = planes_epilogue(v.y, j * 64, Tp, P, T);
+            ep.halo = 1;
+            ep.relu = 1;
+            ep.bias = bias + 64 * (j - 1);
+            ep.bn_scale = bn_scale + 64 * (j - 1);
+            ep.bn_shift = bn_shift + 64 * (j - 1);
+            const GemmSource srcs[2] = {GemmSource{v.x, j * 64, 64, 0}, GemmSource{v.y, (j - 1) * 64, 64, 0}};
+            if ((rc = res2conv_build(&rp[j - 1], srcs, j >= 2 ? 2 : 1, v.w[j - 1], R, dil, ep))) return rc;
+        }
+    } else {
+        const float *bj[RES2CHAIN_MAX], *sj[RES2CHAIN_MAX], *hj[RES2CHAIN_MAX];
+        for (int j = 0; j < nconv; ++j) bj[j] = bias + 64 * j, sj[j] = bn_scale + 64 * j, hj[j] = bn_shift + 64 * j;
+        if ((rc = res2chain_build(&cp, v.x, v.y, v.w, bj, sj, hj, nconv, B, T, P, Tp, dil, variant == PPV_RES2_CHAIN_PAIRED))) return rc;
+    }
+    // weights [nconv][64][64][3] -> the model's matrices: the three taps of chunk j, and from conv 2 the same weights again for the
+    // three taps of conv j-1's output
+    std::vector<float> wh(size_t(nconv) * 64 * 64 * 3);
+    PPV_CUDA_OK(cudaMemcpyAsync(wh.data(), w, wh.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    PPV_CUDA_OK(cudaStreamSynchronize(st));
+    ArenaBuilder ab;
+    GemmWeights gw[RES2CHAIN_MAX];
+    for (int j = 0; j < nconv; ++j) {
+        std::vector<ConvKGroup> groups = {{3, 64, 0, 64, 0}};
+        if (j >= 1) groups.push_back({3, 64, 0, 64, 0});
+        const std::vector<double> mtx = conv_weight_matrix(wh.data() + size_t(j) * 64 * 64 * 3, 64, 64, 3, 64, groups);
+        ab.put_matrix(&gw[j], mtx, 64, int(mtx.size() / 64), 128);
+        PPV_REQUIRE(gw[j].W.plane_stride == v.w[j].plane_stride, "ppv_res2net_test: weight layout mismatch");
+        PPV_CUDA_OK(cudaMemcpyAsync(v.w[j].base, ab.host.data() + ab.patches[j].off, size_t(2 * v.w[j].plane_stride) * sizeof(__nv_bfloat16),
+                                    cudaMemcpyHostToDevice, st));
+    }
+    PPV_CUDA_OK(cudaStreamSynchronize(st));  // the host matrices die here
+    if ((rc = launch_f32_to_planes(x, R, ld_x, v.x, st)) || (rc = launch_f32_to_planes(y, v.y.rows, ld_y, v.y, st))) return rc;
+    const int sms = max_ctas > 0 ? max_ctas : device_sm_count();
+    if (variant == PPV_RES2_PER_CONV) {
+        for (int j = 0; j < nconv; ++j)
+            if ((rc = res2conv_launch(rp[j], precision, sms, st))) return rc;
+    } else if ((rc = res2chain_launch(cp, precision, sms, st))) {
+        return rc;
+    }
+    if ((rc = launch_planes_to_f32(v.x, 0, ld_x, R, 1, 0, 1, x, st))) return rc;
+    // bf16: the convs read only the hi planes, and the chain stores no lo plane; y comes back as its hi plane
+    if (precision == PPV_PREC_BF16) PPV_CUDA_OK(cudaMemsetAsync(v.y.lo(), 0, size_t(v.y.plane_stride) * sizeof(__nv_bfloat16), st));
+    return launch_planes_to_f32(v.y, 0, ld_y, int(v.y.rows), 1, 0, 1, y, st);
+    PPV_GUARD_END
+}
+
+// ---------------------------------------------------------------- skinny linear test hook
+// Workspace: x planes [2][pad128(M)][ld], W planes [2][pad128(N)][K], output planes [2][pad128(M)][out_ld].
+static void carve_skinny_test(WsCarver& cv, int M, int ld, int N, int K, int out_ld, Planes* px, Planes* pw, Planes* po) {
+    *px = cv.planes(M, ld);
+    *pw = cv.planes(N, K);
+    *po = cv.planes(M, out_ld);
+}
+size_t ppv_skinny_linear_test_workspace_bytes(int M, int ld, int N, int K, int out_ld) {
+    return carve_extent([&](WsCarver& cv) { Planes px, pw, po; carve_skinny_test(cv, M, ld, N, K, out_ld, &px, &pw, &po); });
+}
+int ppv_skinny_linear_test(const float* x, int M, int ld, int x_col0, const float* W, int N, int K, const float* bias, int act, int out_planes,
+                           float* out, int out_ld, int out_col0, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && W && out, "ppv_skinny_linear_test: null argument");
+    PPV_REQUIRE(M > 0 && N > 0 && K > 0 && x_col0 >= 0 && x_col0 + K <= ld && out_col0 >= 0 && out_col0 + N <= out_ld,
+                "ppv_skinny_linear_test: bad shape");
+    PPV_REQUIRE(act >= 0 && act <= 2, "ppv_skinny_linear_test: act must be 0 (none), 1 (ReLU) or 2 (sigmoid)");
+    if (int rc = check_workspace("ppv_skinny_linear_test", ws, ws_bytes, ppv_skinny_linear_test_workspace_bytes(M, ld, N, K, out_ld),
+                                 "ppv_skinny_linear_test_workspace_bytes")) return rc;
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes px, pw, po;
+    carve_skinny_test(cv, M, ld, N, K, out_ld, &px, &pw, &po);
+    Epilogue ep;
+    if (out_planes) {
+        ep = planes_epilogue(po, out_col0);
+    } else {
+        ep.out_mode = OUT_F32;
+        ep.out = out;
+        ep.out_ld = out_ld;
+        ep.out_col0 = out_col0;
+    }
+    ep.bias = bias;
+    ep.relu = act == 1;
+    ep.sigmoid_ = act == 2;
+    // what skinny_linear_launch requires, checked before anything is launched: no other kernel stands in
+    PPV_REQUIRE(skinny_linear_supported(M, N, K, ep) && ld % 8 == 0 && x_col0 % 8 == 0,
+                "ppv_skinny_linear_test: the skinny kernel does not take this shape");
+    if ((rc = launch_f32_to_planes(x, M, ld, px, st)) || (rc = launch_f32_to_planes(W, N, K, pw, st))) return rc;
+    if (out_planes && (rc = launch_f32_to_planes(out, M, out_ld, po, st))) return rc;
+    if ((rc = skinny_linear_launch(px, x_col0, pw, M, N, K, ep, st))) return rc;
+    return out_planes ? launch_planes_to_f32(po, 0, out_ld, M, 1, 0, 1, out, st) : PPV_OK;
+    PPV_GUARD_END
+}
+
 // ppv_gemm_bench's workspace: the GEMM test hooks' operands, then the output [2][pad128(M)][N] (planes or fp32) and the epilogue
 // vectors (bias, BN scale / shift, one bias per Tp-row utterance).
 static void carve_gemm_bench(WsCarver& cv, int M, int N, int K, int Tp, Planes* pa, Planes* pw, Planes* po, float** vec) {

@@ -1,9 +1,10 @@
-// Skinny linear layers: out[b, n] = act(sum_k x[b, k] W[n, k] + bias[n]) for a handful of rows (one per utterance) -- the SE
-// excitation MLP (ppvector/models/ecapa_tdnn.py:79-80), ASP's global-context bias and the final fc of EcapaTdnn.forward
-// (ecapa_tdnn.py:274), each [256 x K] x [K x N] with K <= 3072, N <= 512.
+// Skinny linear layers: out[b, n] = act(sum_k x[b, k] W[n, k] + bias[n]) for a handful of rows (one per utterance), K <= 1024.
+// In ECAPA-TDNN that is the SE excitation MLP (ppvector/models/ecapa_tdnn.py:79-80): se1 [B x 512] x [512 x 128] with ReLU into
+// planes, se2 [B x 128] x [128 x 512] with sigmoid into fp32.  ASP's global-context fold (K = 3072) and the final fc (K = 1536 or
+// 3072) run on the gather-GEMM: plan_row_linear chooses by skinny_linear_supported.
 //
 // On the tensor-core gather-GEMM these layers would occupy 2-6 CTAs: with M = 256 rows there are only two 128-row tiles, and the
-// k-loop is a latency chain.  They are 17-150 MFLOP: here every SM takes a 16 x 16 output tile and walks K on the CUDA cores with fp32 FMAs over
+// k-loop is a latency chain.  Here every SM takes a 16 x 16 output tile and walks K on the CUDA cores with fp32 FMAs over
 // the exact hi + lo values of the split-bf16 operands (at least as accurate as the three-product tensor path).  128-192 CTAs, no
 // split-K, no atomics: deterministic.
 #include "common.h"

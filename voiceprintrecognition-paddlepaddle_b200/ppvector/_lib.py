@@ -13,6 +13,7 @@ PPV_PREC_BF16X3 = 0
 PPV_PREC_BF16 = 1
 PPV_MODEL_ECAPA_TDNN = 1
 PPV_POOL_ASP, PPV_POOL_SAP, PPV_POOL_TAP, PPV_POOL_TSP = 0, 1, 2, 3
+PPV_RES2_CHAIN, PPV_RES2_CHAIN_PAIRED, PPV_RES2_PER_CONV = 0, 1, 2
 
 
 class PPVError(RuntimeError):
@@ -188,6 +189,11 @@ SIGNATURES = {
     "ppv_campplus_context_test": (C.c_int, [_P] + [C.c_int] * 4 + [_P] * 6 + [C.c_size_t, _P]),
     "ppv_gemm_test_taps_workspace_bytes": (C.c_size_t, [C.POINTER(GemmTapsCase)]),
     "ppv_gemm_test_taps": (C.c_int, [C.POINTER(GemmTapsCase), _P, C.c_size_t, _P]),
+    "ppv_res2net_test_workspace_bytes": (C.c_size_t, [C.c_int] * 5),
+    "ppv_res2net_test": (C.c_int, [_P, C.c_int] + [_P] * 4 + [C.c_int] * 7 + [_P, C.c_int, _P, C.c_size_t, _P]),
+    "ppv_skinny_linear_test_workspace_bytes": (C.c_size_t, [C.c_int] * 5),
+    "ppv_skinny_linear_test": (C.c_int, [_P] + [C.c_int] * 3 + [_P] + [C.c_int] * 2 + [_P] + [C.c_int] * 2 + [_P] + [C.c_int] * 2
+                               + [_P, C.c_size_t, _P]),
 }
 
 _lib = None
