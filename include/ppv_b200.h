@@ -189,6 +189,23 @@ typedef struct {
     int precision;     /* PPV_PREC_* */
 } ppv_campplus_cfg;
 void ppv_campplus_default_cfg(ppv_campplus_cfg* cfg);
+
+/* kind PPV_MODEL_RES2NET: ppvector/models/res2net.py:90-167 (Bottle2neck :11-87), ASP head as ResNetSE's; the reference's configs/res2net.yml.
+ * scale 2 only (the sp = sp + spx[i] chain of scale > 2 is PPV_EUNSUPPORTED), m_channels 32, every chunk width
+ * m_channels * 2^l * base_width / 64 16 or a multiple of 32, and input_size must leave a final grid of input_size / base_width rows
+ * (the stem is 7x7 / stride 3 / padding 1 and a 3x3 / 2 max-pool; the reference sizes its head from input_size / base_width). */
+#define PPV_MODEL_RES2NET 5
+typedef struct {
+    int input_size;         /* 80 */
+    int embd_dim;           /* 192 */
+    int layers[4];          /* 3,4,6,3 */
+    int m_channels;         /* 32 */
+    int base_width;         /* 32 */
+    int scale;              /* 2 */
+    int attention_channels; /* 128 */
+    int precision;          /* PPV_PREC_* */
+} ppv_res2net_cfg;
+void ppv_res2net_default_cfg(ppv_res2net_cfg* cfg);
 int ppv_model_create(int kind, const void* cfg, ppv_model_t** out);
 int ppv_model_destroy(ppv_model_t* h);
 /* Weights are COPIED (and re-laid-out for the tensor cores) at finalize; names and shapes are the
@@ -208,17 +225,19 @@ int ppv_model_forward(ppv_model_t* h, const float* feat, int B, int T, float* em
  * #{t : t < lengths[b] * T} frames of each utterance.  lengths == NULL is ppv_model_forward. */
 int ppv_model_forward_lengths(ppv_model_t* h, const float* feat, const float* lengths, int B, int T, float* emb, void* ws,
                               size_t ws_bytes, void* stream);
-/* Fused front end + model: wav [B,L] fp32 -> emb [B,embd_dim]; the Fbank features go straight into the
- * first conv's operand layout and never exist as [B,T,F] fp32.  lens_ratio as ppv_fbank_forward. */
+/* Fused front end + model: wav [B,L] fp32 -> emb [B,embd_dim]; ECAPA-TDNN and Res2Net.  ECAPA-TDNN: the Fbank features go straight
+ * into the first conv's operand layout and never exist as [B,T,F] fp32; Res2Net: they go to the workspace, where its stem reads them.
+ * lens_ratio as ppv_fbank_forward. */
 int ppv_model_forward_wav(ppv_model_t* h, ppv_fbank_t* fb, const float* wav, const float* lens_ratio, int B, int L,
                           float* emb, void* ws, size_t ws_bytes, void* stream);
 /* Debug / parity taps: copy an internal activation (valid frames only) to out as fp32.
  * ECAPA: name in {"feat","blocks.0","blocks.1","blocks.2","blocks.3","mfa","asp"}; out is [B,T,C] ([B,C] for asp).
  * ResNetSE: {"conv1","layer1".."layer4"} -> [B,H,W,C] (H = frequency, W = time); "flat" -> [B,T',C*H]; "asp" -> [B,2*C*H].
- * ERes2Net: {"layer1".."layer4","fuse12","fuse123","fuse1234"} -> [B,H,W,C]; "stats" -> [B, 2*C*H]. */
+ * ERes2Net: {"layer1".."layer4","fuse12","fuse123","fuse1234"} -> [B,H,W,C]; "stats" -> [B, 2*C*H].
+ * Res2Net: "stem" (after the max-pool) and "layer1".."layer4" -> [B,H,W,C]; "flat" -> [B,T',C*H]; "asp" -> [B,2*C*H]. */
 int ppv_model_read_tap(ppv_model_t* h, const char* name, float* out, size_t out_elems, void* stream);
 
-/* Measurement hooks (bench.py): CUDA events around every kernel group of the forward, on the launching stream.
+/* Measurement hooks (bench.py; ECAPA-TDNN and Res2Net): CUDA events around every kernel group of the forward, on the launching stream.
  * profile(h,1) starts recording; profile_read sums the durations since then (tensor-core GEMM launches vs the
  * HBM-bound kernels), reports how many kernels were launched, synchronises on the last event and resets. */
 int ppv_model_profile(ppv_model_t* h, int enable);
@@ -475,6 +494,18 @@ size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, i
 int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
                     int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
                     size_t ws_bytes, void* stream);
+
+/* Test hooks for Res2Net's CUDA-core kernels (not reference entry points).
+ * stem: feat [B,T,F] fp32, w [32][49] and bias [32] fp32 with the BN folded in -> out: split-bf16 planes [2][B][Hq+2][Wq+2][32],
+ * H1 = (F-5)/3+1, W1 = (T-5)/3+1, Hq = (H1-1)/2+1, Wq = (W1-1)/2+1, 16-byte aligned; zeroed, then the kernel writes the interior
+ * (7x7 / 3 conv, ReLU, 3x3 / 2 max-pool).  F, T >= 5.
+ * avgpool: x fp32 [B][H+2][W+2][C] (a zero-bordered grid) -> out: split-bf16 planes [2][B][Ho+2][Wo+2][C], Ho = (H-1)/stride+1,
+ * Wo = (W-1)/stride+1; zeroed, then columns [col0, col0+ncols) of the interior get the exclusive 3x3 average (stride 1 or 2, padding 1)
+ * of the same columns of x.  col0, ncols, C multiples of 8; ws >= ppv_res2net_avgpool_test_workspace_bytes. */
+int ppv_res2net_stem_test(const float* feat, const float* w, const float* bias, int B, int T, int F, void* out, void* stream);
+size_t ppv_res2net_avgpool_test_workspace_bytes(int B, int H, int W, int C);
+int ppv_res2net_avgpool_test(const float* x, int B, int H, int W, int C, int col0, int ncols, int stride, void* out, void* ws,
+                             size_t ws_bytes, void* stream);
 
 /* Test hook for the fused attentive-statistics pooling kernel (not a reference entry point): the kernel the ECAPA-TDNN and ResNetSE
  * plans run, on operands given in fp32 and split into planes here.  W [C,K] (attention conv weight), att [B*Tp,K] and x [B*Tp,C] in

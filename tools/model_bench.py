@@ -1,10 +1,14 @@
 """Throughput of the backbone forwards (features resident in HBM) -- a tuning aid, not the contract bench (bench.py).
 
-python tools/model_bench.py [--models EcapaTdnn,ResNetSE,ERes2Net,CAMPPlus] [--batch 256] [--frames 298] [--iters 10]
+python tools/model_bench.py [--models EcapaTdnn,ResNetSE,ERes2Net,CAMPPlus,Res2Net] [--batch 256] [--frames 298] [--iters 10]
                             [--precision bf16x3] [--once MODEL]   (--once: one warm forward only, for ncu launch lists)
                             [--dump-outputs DIR]   (each model's last embeddings as float32 DIR/<model>.npy)
+                            [--profile]   (kernel-time split of one warm forward: ppv_model_profile's tensor-core / other time where the
+                                           model has it, and torch.profiler's device time per kernel name)
 Prints one JSON line per model.  Weights and inputs are seeded, so two builds can be compared output for output."""
 import argparse
+import collections
+import ctypes as C
 import json
 import os
 import sys
@@ -18,9 +22,11 @@ from ppvector import _lib  # noqa: E402
 from ppvector.models.campplus import CAMPPlus  # noqa: E402
 from ppvector.models.ecapa_tdnn import EcapaTdnn  # noqa: E402
 from ppvector.models.eres2net import ERes2Net, ERes2NetV2  # noqa: E402
+from ppvector.models.res2net import Res2Net  # noqa: E402
 from ppvector.models.resnet_se import ResNetSE  # noqa: E402
 
-MODELS = {"EcapaTdnn": EcapaTdnn, "ResNetSE": ResNetSE, "ERes2Net": ERes2Net, "ERes2NetV2": ERes2NetV2, "CAMPPlus": CAMPPlus}
+MODELS = {"EcapaTdnn": EcapaTdnn, "ResNetSE": ResNetSE, "ERes2Net": ERes2Net, "ERes2NetV2": ERes2NetV2, "CAMPPlus": CAMPPlus,
+          "Res2Net": Res2Net}
 
 
 def randomize(m, seed=0):
@@ -38,6 +44,30 @@ def randomize(m, seed=0):
     return m
 
 
+def kernel_split(m, x):
+    """ppv_model_profile's tensor-core / other split (ECAPA-TDNN and Res2Net) and the device time of each kernel name, in ms, of one
+    warm forward"""
+    out = {}
+    lib, h = _lib.load(), m._get_handle()
+    if lib.ppv_model_profile(h, 1) == 0:
+        m(x)
+        g_ms, o_ms, g_n, o_n = C.c_double(), C.c_double(), C.c_int64(), C.c_int64()
+        _lib.check(lib.ppv_model_profile_read(h, C.byref(g_ms), C.byref(o_ms), C.byref(g_n), C.byref(o_n)), "ppv_model_profile_read")
+        lib.ppv_model_profile(h, 0)
+        out["ppv_model_profile"] = {"tensor_ms": round(g_ms.value, 3), "other_ms": round(o_ms.value, 3), "tensor_launches": g_n.value,
+                                    "other_launches": o_n.value}
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        m(x)
+        torch.cuda.synchronize()
+    per = collections.Counter()
+    for e in prof.events():
+        if e.device_type == torch.autograd.DeviceType.CUDA:
+            per[e.name.split("<")[0].split("(")[0]] += e.device_time_total / 1e3
+    out["kernels_ms"] = {k: round(v, 3) for k, v in per.most_common()}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--models", default="EcapaTdnn,ResNetSE,ERes2Net,CAMPPlus")
@@ -47,6 +77,7 @@ def main():
     ap.add_argument("--precision", default="bf16x3")
     ap.add_argument("--once", default="")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write each model's last embeddings to DIR/<model>.npy")
+    ap.add_argument("--profile", action="store_true", help="add the kernel-time split of one warm forward")
     ap.add_argument("--lanes", type=int, default=1, help="batches in flight: replica models on their own streams (see PPVectorPredictor._lanes)")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
@@ -75,6 +106,8 @@ def main():
         ws = _lib.load().ppv_model_workspace_bytes(m._get_handle(), a.batch, a.frames)
         line = {"model": name, "precision": a.precision, "batch": a.batch, "frames": a.frames, "ms_per_forward": round(ms, 3),
                 "utt_per_s": round(a.batch / ms * 1e3, 1), "workspace_GB": round(ws / 2**30, 2), "finite": bool(torch.isfinite(e).all())}
+        if a.profile:
+            line["profile"] = kernel_split(m, x)
         if a.lanes > 1:  # the same forwards dealt round robin to replica models on their own streams
             reps = [m]
             for _ in range(a.lanes - 1):

@@ -59,6 +59,8 @@ struct ppv_model {
 
 // The model behind an ECAPA-TDNN handle, else null: the entry points that only ECAPA-TDNN has.
 static Model* ecapa_of(const ppv_model* h) { return h && h->kind == PPV_MODEL_ECAPA_TDNN ? h->m : nullptr; }
+// The models with the fused waveform path and the launch profile: ECAPA-TDNN and Res2Net.
+static Model* wav_model_of(const ppv_model* h) { return h && (h->kind == PPV_MODEL_ECAPA_TDNN || h->kind == PPV_MODEL_RES2NET) ? h->m : nullptr; }
 
 #define PPV_GUARD_BEGIN try {
 #define PPV_GUARD_END                                                        \
@@ -168,13 +170,17 @@ void ppv_campplus_default_cfg(ppv_campplus_cfg* c) {
 void ppv_resnetse_default_cfg(ppv_resnetse_cfg* c) {
     if (c) ppv_resnetse_default_cfg_impl(c);
 }
+void ppv_res2net_default_cfg(ppv_res2net_cfg* c) {
+    if (c) ppv_res2net_default_cfg_impl(c);
+}
 
 int ppv_model_create(int kind, const void* cfg, ppv_model_t** out) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(cfg && out, "ppv_model_create: null argument");
-    if (kind != PPV_MODEL_ECAPA_TDNN && kind != PPV_MODEL_RESNET_SE && kind != PPV_MODEL_ERES2NET && kind != PPV_MODEL_CAMPPLUS)
-        return fail(PPV_EUNSUPPORTED,
-                    "ppv_model_create: implemented kinds are PPV_MODEL_ECAPA_TDNN, PPV_MODEL_RESNET_SE, PPV_MODEL_ERES2NET, PPV_MODEL_CAMPPLUS");
+    if (kind != PPV_MODEL_ECAPA_TDNN && kind != PPV_MODEL_RESNET_SE && kind != PPV_MODEL_ERES2NET && kind != PPV_MODEL_CAMPPLUS &&
+        kind != PPV_MODEL_RES2NET)
+        return fail(PPV_EUNSUPPORTED, "ppv_model_create: implemented kinds are PPV_MODEL_ECAPA_TDNN, PPV_MODEL_RESNET_SE, PPV_MODEL_ERES2NET, "
+                                      "PPV_MODEL_CAMPPLUS, PPV_MODEL_RES2NET");
     int rc = check_device();
     if (rc) return rc;
     Model* m = nullptr;
@@ -182,6 +188,7 @@ int ppv_model_create(int kind, const void* cfg, ppv_model_t** out) {
         case PPV_MODEL_ECAPA_TDNN: rc = ecapa_create(static_cast<const ppv_ecapa_cfg*>(cfg), &m); break;
         case PPV_MODEL_RESNET_SE: rc = resnetse_create(static_cast<const ppv_resnetse_cfg*>(cfg), &m); break;
         case PPV_MODEL_ERES2NET: rc = eres2net_create(static_cast<const ppv_eres2net_cfg*>(cfg), &m); break;
+        case PPV_MODEL_RES2NET: rc = res2net_create(static_cast<const ppv_res2net_cfg*>(cfg), &m); break;
         default: rc = campplus_create(static_cast<const ppv_campplus_cfg*>(cfg), &m); break;
     }
     if (rc) return rc;
@@ -232,7 +239,10 @@ int ppv_model_forward_wav(ppv_model_t* h, ppv_fbank_t* fb, const float* wav, con
                           void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && fb && wav && emb, "ppv_model_forward_wav: null argument");
-    if (!ecapa_of(h)) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_wav: the fused waveform path exists for ECAPA-TDNN only; call ppv_fbank_forward + ppv_model_forward");
+    if (!wav_model_of(h))
+        return fail(PPV_EUNSUPPORTED, "ppv_model_forward_wav: the fused waveform path exists for ECAPA-TDNN and Res2Net only; call ppv_fbank_forward + ppv_model_forward");
+    if (h->kind == PPV_MODEL_RES2NET)
+        return res2net_forward_wav(h->m, fb->impl, wav, lens_ratio, B, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     const int T = fbank_num_frames(fb->impl, L);
     PPV_REQUIRE(T > 0, "ppv_model_forward_wav: waveform shorter than one frame");
     return ecapa_forward(h->m, nullptr, fb->impl, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
@@ -354,13 +364,15 @@ int ppv_kmeans(const double* X, int ld, int N, int k, const double* uniforms, in
 }
 
 int ppv_model_profile(ppv_model_t* h, int enable) {
-    PPV_REQUIRE(ecapa_of(h), "ppv_model_profile: ECAPA-TDNN model required");
-    return ecapa_profile(h->m, enable);
+    PPV_REQUIRE(wav_model_of(h), "ppv_model_profile: ECAPA-TDNN or Res2Net model required");
+    h->m->profile(enable != 0);
+    return PPV_OK;
 }
 int ppv_model_profile_read(ppv_model_t* h, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(ecapa_of(h), "ppv_model_profile_read: ECAPA-TDNN model required");
-    return ecapa_profile_read(h->m, gemm_ms, other_ms, gemm_launches, other_launches);
+    PPV_REQUIRE(wav_model_of(h), "ppv_model_profile_read: ECAPA-TDNN or Res2Net model required");
+    PPV_REQUIRE(gemm_ms && other_ms && gemm_launches && other_launches, "ppv_model_profile_read: null argument");
+    return h->m->profile_read(gemm_ms, other_ms, gemm_launches, other_launches);
     PPV_GUARD_END
 }
 
@@ -679,6 +691,55 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     rc = gemm_build(&gp, srcs.data(), int(srcs.size()), gw.W, int(M), Cout, ep, gemm_pick_bn(Cout));
     if (rc) return rc;
     return gemm_launch(gp, precision, sms, st);
+    PPV_GUARD_END
+}
+
+// Res2Net's fused stem + max-pool (res2net.cu) on features given here: w [32][49] and bias [32] with the BN already folded in.
+int ppv_res2net_stem_test(const float* feat, const float* w, const float* bias, int B, int T, int F, void* out, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(feat && w && bias && out && B > 0, "ppv_res2net_stem_test: bad argument");
+    if (int rc = check_device()) return rc;
+    int H1, W1, Hq, Wq;
+    res2net_stem_grids(F, T, &H1, &W1, &Hq, &Wq);
+    Planes o;
+    o.base = static_cast<__nv_bfloat16*>(out);
+    o.ld = 32;
+    o.rows = int64_t(B) * (Hq + 2) * (Wq + 2);
+    o.plane_stride = o.rows * o.ld;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2) * o.plane_stride * sizeof(__nv_bfloat16), st));
+    return launch_res2net_stem(feat, B, T, F, w, bias, 32, o, st);
+    PPV_GUARD_END
+}
+
+// Res2Net's exclusive 3x3 average pool (res2net.cu).  Workspace: the input grid [2][pad128(B (H+2) (W+2))][C].
+static void carve_avgpool_test(WsCarver& cv, int B, int H, int W, int C, Planes* xp) { *xp = cv.planes(int64_t(B) * (H + 2) * (W + 2), C); }
+size_t ppv_res2net_avgpool_test_workspace_bytes(int B, int H, int W, int C) {
+    if (B <= 0 || H <= 0 || W <= 0 || C <= 0) return 0;
+    return carve_extent([&](WsCarver& cv) { Planes xp; carve_avgpool_test(cv, B, H, W, C, &xp); });
+}
+int ppv_res2net_avgpool_test(const float* x, int B, int H, int W, int C, int col0, int ncols, int stride, void* out, void* ws, size_t ws_bytes,
+                             void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && out && B > 0 && H > 0 && W > 0 && C > 0 && col0 >= 0 && ncols > 0 && col0 + ncols <= C, "ppv_res2net_avgpool_test: bad argument");
+    if (int rc = check_workspace("ppv_res2net_avgpool_test", ws, ws_bytes, ppv_res2net_avgpool_test_workspace_bytes(B, H, W, C),
+                                 "ppv_res2net_avgpool_test_workspace_bytes"))
+        return rc;
+    if (int rc = check_device()) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes xp;
+    carve_avgpool_test(cv, B, H, W, C, &xp);
+    int rc = launch_f32_to_planes(x, int64_t(B) * (H + 2) * (W + 2), C, xp, st);
+    if (rc) return rc;
+    const int Ho = (H - 1) / std::max(stride, 1) + 1, Wo = (W - 1) / std::max(stride, 1) + 1;
+    Planes o;
+    o.base = static_cast<__nv_bfloat16*>(out);
+    o.ld = C;
+    o.rows = int64_t(B) * (Ho + 2) * (Wo + 2);
+    o.plane_stride = o.rows * o.ld;
+    PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2) * o.plane_stride * sizeof(__nv_bfloat16), st));
+    return launch_avgpool3x3(xp, col0, B, H, W, stride, ncols, o, col0, device_sm_count(), st);
     PPV_GUARD_END
 }
 

@@ -387,17 +387,20 @@ int spectral_feature_dim(const Spectral* h);
 int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st);
 int spec_augment_run(float* feat, const int32_t* params, int B, int T, int F, int n_freq_masks, int n_time_masks, int fill_mode, cudaStream_t st);
 
-// ---- model factories (ecapa.cu, resnet_se.cu, eres2net.cu, campplus.cu; the Model interface is in model_common.h) -------------
+// ---- model factories (ecapa.cu, resnet_se.cu, res2net.cu, eres2net.cu, campplus.cu; the Model interface is in model_common.h) -------------
 struct Model;
 void ppv_ecapa_default_cfg_impl(ppv_ecapa_cfg* c);
 int ecapa_create(const ppv_ecapa_cfg* cfg, Model** out);
-// ECAPA-TDNN only (m must be one): waveform input through `fb`, `lengths`, and the launch-group profile
+// ECAPA-TDNN only (m must be one): waveform input through `fb` and `lengths`
 int ecapa_forward(Model* m, const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb,
                   void* ws, size_t ws_bytes, cudaStream_t st, const float* lengths = nullptr);
-int ecapa_profile(Model* m, int enable);
-int ecapa_profile_read(Model* m, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches);
 void ppv_resnetse_default_cfg_impl(ppv_resnetse_cfg* c);
 int resnetse_create(const ppv_resnetse_cfg* cfg, Model** out);
+void ppv_res2net_default_cfg_impl(ppv_res2net_cfg* c);
+int res2net_create(const ppv_res2net_cfg* cfg, Model** out);
+// Res2Net only (m must be one): the Fbank of wav [B, L] into the workspace, then the forward
+int res2net_forward_wav(Model* m, Fbank* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb, void* ws, size_t ws_bytes,
+                        cudaStream_t st);
 void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c);
 int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out);
 void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);
@@ -418,6 +421,14 @@ struct ImageGeo {
 // stem: 1 -> C0 channels, 3x3, padding 1, folded BN, ReLU, from feats [B,T,F] (image = feats transposed: H = F, W = T)
 int launch_stem_conv(const float* feat, int B, int T, int F, const float* w9, const float* bias, int C0, const Planes& out, int Hp, int Wp,
                      cudaStream_t st);
+// Res2Net's stem (res2net.cu): 1 -> 32 channels, 7x7, stride 3, padding 1, folded BN (w [32][49]), ReLU, then MaxPool2D(3, 2, 1), from
+// feats [B,T,F] into the pooled grid Hq x Wq (zero-bordered, ld out.ld); res2net_stem_grids gives the conv grid H1 x W1 and Hq x Wq
+void res2net_stem_grids(int F, int T, int* H1, int* W1, int* Hq, int* Wq);
+int launch_res2net_stem(const float* feat, int B, int T, int F, const float* w, const float* bias, int C0, const Planes& out, cudaStream_t st);
+// AvgPool2D(3, stride 1 or 2, padding 1, exclusive): columns [in_col0, +ncols) of `in` on the H x W grid -> [out_col0, +ncols) of `out`
+// on the ((H-1)/stride+1) x ((W-1)/stride+1) grid; ncols and both column offsets multiples of 8
+int launch_avgpool3x3(const Planes& in, int in_col0, int B, int H, int W, int stride, int ncols, const Planes& out, int out_col0, int num_sms,
+                      cudaStream_t st);
 // [B,Hp,Wp,C] image -> [B*W, C*H] time-major matrix (channel index c*H + h)
 int launch_flatten_image(const Planes& in, int B, int H, int W, int Hp, int Wp, int C, const Planes& out, int num_sms, cudaStream_t st);
 int launch_image_to_f32(const Planes& in, int B, int H, int W, int Hp, int Wp, int C, float* out, cudaStream_t st);

@@ -405,16 +405,6 @@ int EcapaModel::run(const float* feat, Fbank* fb, const float* wav, const float*
     return rc ? rc : run_plan(PlanInputs{feat, nv}, st);
 }
 
-int ecapa_profile(Model* model, int enable) {
-    static_cast<EcapaModel*>(model)->profile(enable != 0);
-    return PPV_OK;
-}
-
-int ecapa_profile_read(Model* model, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
-    PPV_REQUIRE(gemm_ms && other_ms && gemm_launches && other_launches, "ecapa_profile_read: null argument");
-    return static_cast<EcapaModel*>(model)->profile_read(gemm_ms, other_ms, gemm_launches, other_launches);
-}
-
 int EcapaModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {
     const int B = plan_B, T = plan_T;
     const Planes* src = nullptr;

@@ -1,5 +1,6 @@
-// The 2-D models' shared plan pieces (image_plan.h): image-grid geometry, epilogues and taps, 3x3 conv routing, and the kernels every
-// 2-D model runs: the stem conv, the flatten of the last grid to a time-major matrix, and the fp32 image tap.
+// The 2-D models' shared plan pieces (image_plan.h): image-grid geometry, epilogues and taps, 3x3 conv routing, the ASP head of ResNetSE
+// and Res2Net, and the kernels every 2-D model runs: the stem conv, the flatten of the last grid to a time-major matrix, and the fp32
+// image tap.
 #include <stdlib.h>
 
 #include "image_plan.h"
@@ -163,6 +164,73 @@ int PlanModel::plan_conv3x3(const GemmWeights& gw, const Planes& x, int col0, in
     if (rc) return rc;
     steps.push_back({"conv3x3_launch", true, [c3](const StepRun& r) { return conv3x3_launch(c3, r.precision, r.num_sms, r.st); }});
     return PPV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ ASP head
+bool prepare_asp_head(ArenaBuilder& ab, AspHead* h, int cat, int A, int E) {
+    h->cat = cat;
+    h->att = A;
+    h->embd = E;
+    const HostWeight* wt = ab.get("pooling.tdnn.conv.conv.weight", {A, 3 * cat, 1});
+    const HostWeight* bt = ab.get("pooling.tdnn.conv.conv.bias", {A});
+    const HostWeight* wc = ab.get("pooling.conv.conv.weight", {cat, A, 1});
+    const HostWeight* wl = ab.get("linear.weight", {2 * cat, E});
+    const HostWeight* bl = ab.get("linear.bias", {E});
+    std::vector<double> s3, h3;
+    const bool ok = wt && bt && wc && wl && bl && ab.put_bn(&h->att1_bn_scale, &h->att1_bn_shift, "pooling.tdnn.norm.norm", A, A) &&
+                    ab.put_bn(&h->bn2_scale, &h->bn2_shift, "bn2.norm", 2 * cat, 2 * cat) && ab.bn_affine("bn3.norm", E, &s3, &h3);
+    if (!ok) return false;
+    std::vector<double> mx(size_t(A) * cat), mf(size_t(A) * 2 * cat), mc(size_t(cat) * A), ml(size_t(E) * 2 * cat);
+    for (int a = 0; a < A; ++a) {
+        for (int c = 0; c < cat; ++c) mx[size_t(a) * cat + c] = wt->v[size_t(a) * 3 * cat + c];
+        for (int c = 0; c < 2 * cat; ++c) mf[size_t(a) * 2 * cat + c] = wt->v[size_t(a) * 3 * cat + cat + c];
+    }
+    for (size_t i = 0; i < mc.size(); ++i) mc[i] = wc->v[i];
+    std::vector<float> bl2(E);
+    for (int n = 0; n < E; ++n) {
+        for (int k = 0; k < 2 * cat; ++k) ml[size_t(n) * 2 * cat + k] = double(wl->v[size_t(k) * E + n]) * s3[n];
+        bl2[n] = float(double(bl->v[n]) * s3[n] + h3[n]);
+    }
+    ab.put_matrix(&h->att1, mx, A, cat);
+    ab.put_f32(&h->att1.bias, bt->v);
+    ab.put_matrix(&h->fold, mf, A, 2 * cat);
+    ab.put_matrix(&h->att2, mc, cat, A);
+    ab.put_matrix(&h->fc, ml, E, 2 * cat);
+    ab.put_f32(&h->fc.bias, bl2);
+    return true;
+}
+
+int PlanModel::plan_asp_head(const AspHead& h, const AspHeadBuffers& hb, int B, int Tf) {
+    const int cat = h.cat;
+    steps.push_back(colstats_step(hb.flat, cat, B, Tf, 0, Tf, 1, 1e-12f, hb.gstat));
+    {
+        Epilogue ep;
+        ep.out_mode = OUT_F32;
+        ep.out = hb.fold_out;
+        ep.out_ld = h.att;
+        int rc = plan_gemm(h.fold, {GemmSource{hb.gstat, 0, 2 * cat, 0}}, B, ep);
+        if (rc) return rc;
+    }
+    {
+        Epilogue ep = planes_epilogue(hb.attp);
+        ep.relu = 1;
+        ep.Tp = Tf;
+        ep.P = 0;
+        ep.T = Tf;
+        ep.rowgrp_bias = hb.fold_out;
+        ep.bn_scale = h.att1_bn_scale;
+        ep.bn_shift = h.att1_bn_shift;
+        ep.tanh_ = 1;
+        int rc = plan_gemm(h.att1, {GemmSource{hb.flat, 0, cat, 0}}, B * Tf, ep);
+        if (rc) return rc;
+    }
+    int rc = plan_asp_fused(h.att2.W, hb.attp, hb.flat, h.bn2_scale, h.bn2_shift, hb.pooled, hb.pooled_raw, B, Tf, 0, Tf, cat, h.att, 1e-12f);
+    if (rc) return rc;
+    Epilogue ep;
+    ep.out_mode = OUT_F32;
+    ep.out = hb.emb_out;
+    ep.out_ld = h.embd;
+    return plan_gemm(h.fc, {GemmSource{hb.pooled, 0, 2 * cat, 0}}, B, ep);
 }
 
 // ------------------------------------------------------------------------------------------------ taps

@@ -160,15 +160,17 @@ struct ArenaBuilder {
         put_f32(&gw->bias, bias);
         return true;
     }
-    // The 1 -> C0 channel 3x3 stem conv with its BatchNorm folded in: weights [C0][9], bias [C0] (launch_stem_conv)
-    bool fold_stem(float** w9, float** bias, const std::string& conv, const std::string& bn, int C0) {
-        const HostWeight* w = get(conv + ".weight", {C0, 1, 3, 3});
+    // The 1 -> C0 channel k x k stem conv with its BatchNorm folded in: weights [C0][k k], bias [C0] (launch_stem_conv: k = 3;
+    // Res2Net's 7 x 7 stem: launch_res2net_stem)
+    bool fold_stem(float** w9, float** bias, const std::string& conv, const std::string& bn, int C0, int k = 3) {
+        const HostWeight* w = get(conv + ".weight", {C0, 1, k, k});
         const HostWeight* b = get(conv + ".bias", {C0});
         std::vector<double> sc, sh;
         if (!w || !b || !bn_affine(bn, C0, &sc, &sh)) return false;
-        std::vector<float> wf(size_t(C0) * 9), bf(C0);
+        const int kk = k * k;
+        std::vector<float> wf(size_t(C0) * kk), bf(C0);
         for (int c = 0; c < C0; ++c) {
-            for (int k = 0; k < 9; ++k) wf[c * 9 + k] = float(double(w->v[c * 9 + k]) * sc[c]);
+            for (int t = 0; t < kk; ++t) wf[c * kk + t] = float(double(w->v[c * kk + t]) * sc[c]);
             bf[c] = float(double(b->v[c]) * sc[c] + sh[c]);
         }
         put_f32(w9, wf);

@@ -1,4 +1,4 @@
-// The plans, in one place (plan.cu): ECAPA-TDNN, ResNetSE, ERes2Net(V2) and CAM++ each plan their forward, and the ECAPA-TDNN
+// The plans, in one place (plan.cu): ECAPA-TDNN, ResNetSE, Res2Net, ERes2Net(V2) and CAM++ each plan their forward, and the ECAPA-TDNN
 // trainer its training step, as a list of PlanSteps, each a launch with its arguments bound when the plan is built; PlanOwner::run_plan
 // launches them in order.  The routing helpers choose a layer's kernel; what is about zero-bordered image grids (the 2-D models) is in
 // image_plan.h.
@@ -183,6 +183,9 @@ struct Model : PlanOwner {
     virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
 };
 
+struct AspHead;
+struct AspHeadBuffers;
+
 // An inference model with the layer routing helpers.
 struct PlanModel : Model {
     int max_bn = 256;  // widest gather-GEMM n-tile plan_gemm picks
@@ -209,6 +212,8 @@ struct PlanModel : Model {
     int plan_conv3x3(const GemmWeights& gw, const Planes& x, int col0, int ncols, const ImageGeo& g, int B, Epilogue ep);
     // "<base><i>" with lo <= i <= hi (one digit) -> i, else 0
     static int name_index(const std::string& n, const char* base, int lo, int hi);
+    // the ASP head of ResNetSE and Res2Net over hb.flat (B utterances of Tf frames) -> hb.emb_out
+    int plan_asp_head(const AspHead& h, const AspHeadBuffers& hb, int B, int Tf);
     // fp32 [B, H, W, C] copy of image planes, after checking out_elems
     int image_tap(const Planes& src, const ImageGeo& g, int C, float* out, size_t out_elems, cudaStream_t st) const;
 };

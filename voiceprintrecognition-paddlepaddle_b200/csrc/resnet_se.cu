@@ -7,7 +7,8 @@
 //   * every conv runs on the gather-GEMM or the patch kernel, none on the pointwise kernel;
 //   * SE: global average pool = column sums over the whole zero-bordered image; the two Linear layers are small
 //     gather-GEMMs (ReLU / sigmoid epilogues); scale, residual add and ReLU are one elementwise pass.
-// The tail (flatten to [B, T', 512*F'], ASP with the global-context fold, bn2, Linear, bn3) reuses the ECAPA kernels.
+// The tail (flatten to [B, T', 512*F'], ASP with the global-context fold, bn2, Linear, bn3) is the ASP head of image_plan.h, on the
+// ECAPA kernels.
 #include "common.h"
 #include "image_plan.h"
 #include "model_common.h"
@@ -34,8 +35,7 @@ struct ResNetSEModel : PlanModel {
     float* conv1_w = nullptr;  // [32][9] BN folded
     float* conv1_b = nullptr;  // [32]
     std::vector<BlockW> blocks;
-    GemmWeights fold, att1, att2, fc;
-    float *att1_bn_scale = nullptr, *att1_bn_shift = nullptr, *bn2_scale = nullptr, *bn2_shift = nullptr;
+    AspHead head;
     int att = 128, cat = 0, Hf = 0;
     // plan (what the taps read)
     Geo geo[5];  // geo[l] = grid of stage l (1..4); geo[1] is also conv1's
@@ -134,36 +134,7 @@ bool ResNetSEModel::prepare_weights(ArenaBuilder& ab) {
             inplanes = C;
         }
     }
-    if (ok) {  // ASP + head
-        const int cat = m->cat, A = m->att, E = cf.embd_dim;
-        const HostWeight* wt = ab.get("pooling.tdnn.conv.conv.weight", {A, 3 * cat, 1});
-        const HostWeight* bt = ab.get("pooling.tdnn.conv.conv.bias", {A});
-        const HostWeight* wc = ab.get("pooling.conv.conv.weight", {cat, A, 1});
-        const HostWeight* wl = ab.get("linear.weight", {2 * cat, E});
-        const HostWeight* bl = ab.get("linear.bias", {E});
-        std::vector<double> s3, h3;
-        ok = wt && bt && wc && wl && bl && ab.put_bn(&m->att1_bn_scale, &m->att1_bn_shift, "pooling.tdnn.norm.norm", A, A) &&
-             ab.put_bn(&m->bn2_scale, &m->bn2_shift, "bn2.norm", 2 * cat, 2 * cat) && ab.bn_affine("bn3.norm", E, &s3, &h3);
-        if (ok) {
-            std::vector<double> mx(size_t(A) * cat), mf(size_t(A) * 2 * cat), mc(size_t(cat) * A), ml(size_t(E) * 2 * cat);
-            for (int a = 0; a < A; ++a) {
-                for (int c = 0; c < cat; ++c) mx[size_t(a) * cat + c] = wt->v[size_t(a) * 3 * cat + c];
-                for (int c = 0; c < 2 * cat; ++c) mf[size_t(a) * 2 * cat + c] = wt->v[size_t(a) * 3 * cat + cat + c];
-            }
-            for (size_t i = 0; i < mc.size(); ++i) mc[i] = wc->v[i];
-            std::vector<float> bl2(E);
-            for (int n = 0; n < E; ++n) {
-                for (int k = 0; k < 2 * cat; ++k) ml[size_t(n) * 2 * cat + k] = double(wl->v[size_t(k) * E + n]) * s3[n];
-                bl2[n] = float(double(bl->v[n]) * s3[n] + h3[n]);
-            }
-            ab.put_matrix(&m->att1, mx, A, cat);
-            ab.put_f32(&m->att1.bias, bt->v);
-            ab.put_matrix(&m->fold, mf, A, 2 * cat);
-            ab.put_matrix(&m->att2, mc, cat, A);
-            ab.put_matrix(&m->fc, ml, E, 2 * cat);
-            ab.put_f32(&m->fc.bias, bl2);
-        }
-    }
+    if (ok) ok = prepare_asp_head(ab, &m->head, m->cat, m->att, cf.embd_dim);
     return ok;
 }
 
@@ -305,39 +276,18 @@ int ResNetSEModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStrea
     }
     // tail: flatten, ASP, bn2, linear, bn3
     const Geo& g4 = m->geo[4];
-    const int Tf = g4.W, cat = m->cat;
+    const int Tf = g4.W;
     m->steps.push_back(flatten_step(x, g4, B, 2 * m->cfg.num_filters[3], rb.flat));
-    m->steps.push_back(colstats_step(rb.flat, cat, B, Tf, 0, Tf, 1, 1e-12f, rb.gstat));
-    {
-        Epilogue ep;
-        ep.out_mode = OUT_F32;
-        ep.out = rb.fold_out;
-        ep.out_ld = m->att;
-        rc = plan_gemm(m->fold, {GemmSource{rb.gstat, 0, 2 * cat, 0}}, B, ep);
-        if (rc) return rc;
-    }
-    {
-        Epilogue ep = plain_planes(rb.attp, true);
-        ep.Tp = Tf;
-        ep.P = 0;
-        ep.T = Tf;
-        ep.rowgrp_bias = rb.fold_out;
-        ep.bn_scale = m->att1_bn_scale;
-        ep.bn_shift = m->att1_bn_shift;
-        ep.tanh_ = 1;
-        rc = plan_gemm(m->att1, {GemmSource{rb.flat, 0, cat, 0}}, B * Tf, ep);
-        if (rc) return rc;
-    }
-    rc = plan_asp_fused(m->att2.W, rb.attp, rb.flat, m->bn2_scale, m->bn2_shift, rb.pooled, rb.pooled_raw, B, Tf, 0, Tf, cat, m->att, 1e-12f);
+    AspHeadBuffers hb;
+    hb.flat = rb.flat;
+    hb.gstat = rb.gstat;
+    hb.pooled = rb.pooled;
+    hb.attp = rb.attp;
+    hb.fold_out = rb.fold_out;
+    hb.pooled_raw = rb.pooled_raw;
+    hb.emb_out = rb.emb_out;
+    rc = plan_asp_head(m->head, hb, B, Tf);
     if (rc) return rc;
-    {
-        Epilogue ep;
-        ep.out_mode = OUT_F32;
-        ep.out = rb.emb_out;
-        ep.out_ld = m->cfg.embd_dim;
-        rc = plan_gemm(m->fc, {GemmSource{rb.pooled, 0, 2 * cat, 0}}, B, ep);
-        if (rc) return rc;
-    }
     m->conv1_out = rb.conv1_out;
     m->flat = rb.flat;
     m->pooled_raw = rb.pooled_raw;

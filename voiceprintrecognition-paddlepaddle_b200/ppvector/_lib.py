@@ -48,6 +48,14 @@ class ERes2NetCfg(C.Structure):
 
 
 PPV_MODEL_CAMPPLUS = 4
+PPV_MODEL_RES2NET = 5
+
+
+class Res2NetCfg(C.Structure):
+    _fields_ = [("input_size", C.c_int), ("embd_dim", C.c_int), ("layers", C.c_int * 4), ("m_channels", C.c_int), ("base_width", C.c_int),
+                ("scale", C.c_int), ("attention_channels", C.c_int), ("precision", C.c_int)]
+
+
 PPV_SPEC_SPECTROGRAM, PPV_SPEC_MEL, PPV_SPEC_LOGMEL, PPV_SPEC_MFCC = 1, 2, 3, 4
 PPV_SPECAUG_NPARAM = 16
 PPV_PREP_NI, PPV_PREP_NF = 8, 4
@@ -111,6 +119,7 @@ SIGNATURES = {
     "ppv_resnetse_default_cfg": (None, [C.POINTER(ResNetSECfg)]),
     "ppv_eres2net_default_cfg": (None, [C.POINTER(ERes2NetCfg)]),
     "ppv_campplus_default_cfg": (None, [C.POINTER(CamPPlusCfg)]),
+    "ppv_res2net_default_cfg": (None, [C.POINTER(Res2NetCfg)]),
     "ppv_model_create": (C.c_int, [C.c_int, _P, C.POINTER(_P)]),
     "ppv_model_destroy": (C.c_int, [_P]),
     "ppv_model_load_weight": (C.c_int, [_P, C.c_char_p, _P, C.POINTER(C.c_int64), C.c_int]),
@@ -181,6 +190,9 @@ SIGNATURES = {
                                        C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_conv2d_test_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
     "ppv_conv2d_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 13 + [_P, _P, C.c_size_t, _P]),
+    "ppv_res2net_stem_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 3 + [_P, _P]),
+    "ppv_res2net_avgpool_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "ppv_res2net_avgpool_test": (C.c_int, [_P] + [C.c_int] * 7 + [_P, _P, C.c_size_t, _P]),
     "ppv_asp_fused_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "ppv_asp_fused_test": (C.c_int, [_P] * 6 + [C.c_int] * 8 + [_P, _P, _P, C.c_size_t, _P]),
     "ppv_colstats_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

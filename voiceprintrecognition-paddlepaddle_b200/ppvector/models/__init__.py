@@ -5,13 +5,15 @@ from loguru import logger
 from .campplus import CAMPPlus
 from .ecapa_tdnn import EcapaTdnn
 from .eres2net import ERes2Net, ERes2NetV2
+from .res2net import Res2Net
 from .resnet_se import ResNetSE
 
-__all__ = ['build_model', 'CAMPPlus', 'EcapaTdnn', 'ERes2Net', 'ERes2NetV2', 'ResNetSE']
+__all__ = ['build_model', 'CAMPPlus', 'EcapaTdnn', 'ERes2Net', 'ERes2NetV2', 'Res2Net', 'ResNetSE']
 
-_BACKBONES = {'CAMPPlus': CAMPPlus, 'EcapaTdnn': EcapaTdnn, 'ERes2Net': ERes2Net, 'ERes2NetV2': ERes2NetV2, 'ResNetSE': ResNetSE}
+_BACKBONES = {'CAMPPlus': CAMPPlus, 'EcapaTdnn': EcapaTdnn, 'ERes2Net': ERes2Net, 'ERes2NetV2': ERes2NetV2, 'Res2Net': Res2Net,
+              'ResNetSE': ResNetSE}
 # backbones the reference also ships; not part of the accelerated path (SURVEY.md §8)
-_REFERENCE_ONLY = ('Res2Net', 'TDNN')
+_REFERENCE_ONLY = ('TDNN',)
 
 
 def build_model(input_size, configs):
