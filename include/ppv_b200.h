@@ -527,6 +527,15 @@ size_t ppv_colstats_test_workspace_bytes(int B, int Tp, int ld, int C);
 int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int col0, int C, int mode, float eps, float inv_count,
                       const int* nvalid, float* out, float* out_f32, void* ws, size_t ws_bytes, void* stream);
 
+/* Test hook for the training step's TAP / TSP pooling backward (not a reference entry point): the kernel the ECAPA-TDNN trainer runs,
+ * over x [B*Tp, C] fp32 split into planes here (frames t < T at rows b*Tp + P + t; C % 8 == 0).  pooled and dpooled are fp32
+ * [B, C] (var == 0: TAP's mean) or [B, 2C] (var != 0: TSP's mean | unbiased variance) and their gradients.  dx [B*Tp, C]: every row
+ * of the output planes decoded as hi + lo; the planes are filled with the bytes 0x46 before the launch, so a row the kernel does not
+ * write (halo, padding) reads back as 2 * bf16(0x4646).  ws >= ppv_pool_stats_bwd_test_workspace_bytes (0 for an empty shape). */
+size_t ppv_pool_stats_bwd_test_workspace_bytes(int B, int Tp, int C);
+int ppv_pool_stats_bwd_test(const float* x, const float* pooled, const float* dpooled, int B, int T, int P, int Tp, int C, int var, float* dx,
+                            void* ws, size_t ws_bytes, void* stream);
+
 /* Test hook for CAM++'s context mask (not a reference entry point): the dense layers' context kernel over h [B*Tp, 128] fp32 split
  * into planes here (frames t < T at rows b*Tp + P + t), with the MLP w1 [64,128], b1 [64], w2 [32,64], b2 [32] in the reference
  * layout, transposed on the host as the model prepares them.  out [B * ceil(T/100), 32] fp32.  T > 6400 (more than 64 segments)

@@ -1,6 +1,7 @@
 """Training-step throughput of the ECAPA-TDNN CUDA trainer (SURVEY.md §8d config 3 shape: per-GPU batch 64 x 298 frames, 2796
 speakers, AAM margin 0.2, Adam) -- a tuning aid; features resident in HBM.  python tools/train_bench.py [--batch 64] [--frames 298]
-[--steps 10] [--once] [--dump DIR]  (--once: one warm step only, for an ncu launch list; --dump: the state after one step, to
+[--steps 10] [--pooling ASP|SAP|TAP|TSP] [--no-global-context] [--once] [--dump DIR]  (--pooling: the ECAPA-TDNN head, as
+model_conf.model_args.pooling_type; --no-global-context: ASP without the global context; --once: one warm step only, for an ncu launch list; --dump: the state after one step, to
 compare two builds bit for bit).  Under torchrun every rank trains its own batch and the
 gradient all-reduce runs over NCCL."""
 import argparse
@@ -27,6 +28,8 @@ def main():
     ap.add_argument("--dump", metavar="DIR", help="run one forward_backward and adam_step, write the loss, logits, params, grads, stats "
                     "and Adam moments to DIR/<name>.npy and exit")
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "bf16"], help="bf16 = train_conf.enable_amp")
+    ap.add_argument("--pooling", default="ASP", choices=["ASP", "SAP", "TAP", "TSP"], help="the pooling head (pooling_type)")
+    ap.add_argument("--no-global-context", action="store_true", help="ASP without the global context statistics")
     a = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -37,9 +40,10 @@ def main():
         dist.init_process_group("nccl")
     dev = torch.device("cuda", local)
     torch.manual_seed(1000)
-    eng = TrainEngine(input_size=80, num_speakers=a.speakers, device=dev)
+    head = dict(pooling_type=a.pooling, global_context=not a.no_global_context)
+    eng = TrainEngine(input_size=80, num_speakers=a.speakers, device=dev, **head)
     eng.set_precision(a.precision)
-    eng.load_state_dict(EcapaTdnn(input_size=80).state_dict(), torch.nn.init.xavier_uniform_(torch.empty(192, a.speakers)))
+    eng.load_state_dict(EcapaTdnn(input_size=80, **head).state_dict(), torch.nn.init.xavier_uniform_(torch.empty(192, a.speakers)))
     g = torch.Generator().manual_seed(1000 + rank)
     x = torch.randn(a.batch, a.frames, 80, generator=g)
     x = (x - x.mean(1, keepdim=True)).to(dev)
@@ -98,10 +102,13 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
     if rank == 0:
-        # algorithmic work: training step ~ 3 x forward (SURVEY.md §8d), forward 2.857 GFLOP / utterance as executed
+        # algorithmic work: training step ~ 3 x forward (SURVEY.md §8d), forward 2.857 GFLOP / utterance as executed with the default
+        # head (ASP with global context); the other heads do less work after mfa, so the figure is given for that head only
+        default_head = a.pooling == "ASP" and not a.no_global_context
         print(json.dumps({"metric": "train_samples_per_s", "value": round(world * a.batch / ms * 1e3, 1), "n_gpus": world, "precision": a.precision, "ms_per_step": round(ms, 3),
-                          "batch_per_gpu": a.batch, "frames": a.frames, "speakers": a.speakers, "loss": float(loss),
-                          "algorithmic_tflops": round(world * a.batch * 3 * 2.857e9 / (ms * 1e-3) / 1e12, 1),
+                          "batch_per_gpu": a.batch, "frames": a.frames, "speakers": a.speakers, "pooling": a.pooling,
+                          "global_context": not a.no_global_context, "loss": float(loss),
+                          "algorithmic_tflops": round(world * a.batch * 3 * 2.857e9 / (ms * 1e-3) / 1e12, 1) if default_head else None,
                           "workspace_GB": round(eng._ws.numel() / 2**30, 2),
                           "breakdown_ms": {"forward_backward": round(phases[0], 3), "grad_all_reduce": round(phases[1], 3), "adam": round(phases[2], 3)},
                           "all_reduce_bytes": int(eng.grads.numel() * 4)}))

@@ -7,6 +7,7 @@
 #include "common.h"
 #include "image_plan.h"
 #include "model_common.h"
+#include "train.h"
 
 namespace ppv {
 
@@ -822,6 +823,37 @@ int ppv_colstats_test(const float* x, int B, int T, int P, int Tp, int ld, int c
     if ((rc = launch_f32_to_planes(x, rows, ld, px, st))) return rc;
     if ((rc = launch_colstats(px, col0, C, B, T, P, Tp, mode, eps, out_f32, po, st, inv_count, nvalid))) return rc;
     return launch_planes_to_f32(po, 0, oc, B, 1, 0, 1, out, st);
+    PPV_GUARD_END
+}
+
+// ---------------------------------------------------------------- TAP / TSP pooling backward test hook
+// Workspace: x planes [2][B Tp][C], then the dx planes [2][B Tp][C].
+static void carve_pool_stats_bwd_test(WsCarver& cv, int B, int Tp, int C, Planes* x, Planes* dx) {
+    *x = cv.planes(int64_t(B) * Tp, C);
+    *dx = cv.planes(int64_t(B) * Tp, C);
+}
+size_t ppv_pool_stats_bwd_test_workspace_bytes(int B, int Tp, int C) {
+    if (B <= 0 || Tp <= 0 || C <= 0) return 0;
+    return carve_extent([&](WsCarver& cv) { Planes x, dx; carve_pool_stats_bwd_test(cv, B, Tp, C, &x, &dx); });
+}
+int ppv_pool_stats_bwd_test(const float* x, const float* pooled, const float* dpooled, int B, int T, int P, int Tp, int C, int var, float* dx,
+                            void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && pooled && dpooled && dx, "ppv_pool_stats_bwd_test: null argument");
+    PPV_REQUIRE(B > 0 && T > 0 && P >= 0 && Tp >= T + 2 * P && C > 0 && C % 8 == 0, "ppv_pool_stats_bwd_test: bad shape");
+    if (int rc = check_workspace("ppv_pool_stats_bwd_test", ws, ws_bytes, ppv_pool_stats_bwd_test_workspace_bytes(B, Tp, C),
+                                 "ppv_pool_stats_bwd_test_workspace_bytes")) return rc;
+    int rc = check_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t rows = int64_t(B) * Tp;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes px, pd;
+    carve_pool_stats_bwd_test(cv, B, Tp, C, &px, &pd);
+    PPV_CUDA_OK(cudaMemsetAsync(pd.base, 0x46, size_t(2) * pd.plane_stride * sizeof(__nv_bfloat16), st));  // the rows the kernel must not write
+    if ((rc = launch_f32_to_planes(x, rows, C, px, st))) return rc;
+    if ((rc = tr_pool_stats_bwd(px, C, B, T, P, Tp, pooled, dpooled, var != 0, pd, st))) return rc;
+    return launch_planes_to_f32(pd, 0, C, 1, int(rows), 0, int(rows), dx, st);
     PPV_GUARD_END
 }
 

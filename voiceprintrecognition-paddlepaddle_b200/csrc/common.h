@@ -339,6 +339,7 @@ int asp_fused_launch(const AspFusedParams& p, int precision, int num_sms, cudaSt
 
 // ---- other kernels (elementwise.cu) ---------------------------------------------------------------
 int launch_pack_features(const float* feat, int B, int T, int F, const Planes& out, int P, int Tp, cudaStream_t st);
+// per-utterance column statistics into the planes out_pl and / or fp32 out_f32 ([B][C] in mode 0, [B][2C] in modes 1-3)
 int launch_colstats(const Planes& x, int col0, int C, int B, int T, int P, int Tp, int mode, float eps, float* out_f32,
                     const Planes& out_pl, cudaStream_t st, float inv_count = 0.f, const int* nvalid = nullptr);
 int launch_lengths_to_counts(const float* lengths, int B, int T, int* nvalid, cudaStream_t st);

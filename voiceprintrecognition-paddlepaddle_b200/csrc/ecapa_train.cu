@@ -49,7 +49,7 @@ struct TLayer {  // TDNNBlock
     TBN bn;
 };
 
-// The workspace views of one plan (tr_carve).  `layer` is indexed like Trainer::conv: the TDNN layers, then asp.conv.
+// The workspace views of one plan (tr_carve).  `layer` is indexed like Trainer::conv: the TDNN layers, then the head's convs.
 struct TrBuffers {
     int Tp = 0;          // rows per utterance: T + 2P
     int64_t R = 0, Rp = 0;  // rows of the padded time layout, B * Tp, and that rounded up to 128
@@ -63,7 +63,7 @@ struct TrBuffers {
     float *logits = nullptr, *se_s[3], *se_g1[3], *se_g2[3], *gstat = nullptr, *fold = nullptr, *pooled = nullptr, *pn = nullptr, *emb = nullptr,
           *cls_logits = nullptr, *loss = nullptr, *aspbn_mean = nullptr, *aspbn_rstd = nullptr;
     float *d_emb = nullptr, *dpn = nullptr, *dpooled = nullptr, *dgs = nullptr, *rs = nullptr, *rb = nullptr, *dg2 = nullptr, *dg1 = nullptr, *ds = nullptr,
-          *part = nullptr, *wpart = nullptr;
+          *part = nullptr, *wpart = nullptr, *sap_stats = nullptr, *dsap_stats = nullptr;
     size_t part_elems = 0;
     float* aam_ws = nullptr;
     size_t aam_ws_bytes = 0;
@@ -90,10 +90,14 @@ struct Trainer : PlanOwner, EcapaGeometry {
     std::map<std::string, std::pair<int64_t, int64_t>> pmap, smap;  // name -> (offset, numel)
     int64_t n_params = 0, n_stats = 0;
     float *params = nullptr, *grads = nullptr, *stats = nullptr;
-    // layers: 0 conv0; per block b (1..3): tdnn1, res2 x7, tdnn2; mfa; att1; (att2 conv only)
+    // layers: 0 conv0; per block b (1..3): tdnn1, res2 x7, tdnn2; mfa; ASP: att1 (asp.tdnn)
     std::vector<TLayer> L;
-    int l_conv0 = 0, l_tdnn1[3], l_res[3][8], l_tdnn2[3], l_mfa = 0, l_att1 = 0;
-    TConv att2;
+    int l_conv0 = 0, l_tdnn1[3], l_res[3][8], l_tdnn2[3], l_mfa = 0, l_att1 = -1;
+    // the pooling head's convs without a BatchNorm, numbered after L: ASP asp.conv.conv; SAP asp.linear1, asp.linear2; TAP / TSP none.
+    // c_att2 is the conv that writes the softmax logits, c_lin1 SAP's linear1 (-1 where the head has none).
+    std::vector<TConv> hconv;
+    int c_lin1 = -1, c_att2 = -1;
+    int Kp = 0;  // width of the pooled vector and of asp_bn: 2 * C3 (ASP, TSP) or C3 (SAP, TAP)
     int64_t se1_w[3], se1_b[3], se2_w[3], se2_b[3], aspbn_g = 0, aspbn_b = 0, aspbn_rm = 0, aspbn_rv = 0, fc_w = 0, fc_b = 0, cls_w = 0;
     // plan
     TrBuffers buf;
@@ -103,9 +107,11 @@ struct Trainer : PlanOwner, EcapaGeometry {
         : PlanOwner("trainer", "ppv_trainer_workspace_bytes", PPV_PREC_BF16X3), EcapaGeometry(g), cfg(c), S(num_classes), D(c.embd_dim) {
         sync_each_step = getenv("PPV_TRAIN_DEBUG") != nullptr;  // localise a faulting kernel
     }
-    // convs by layer index: L's, then asp.conv
-    int l_att2() const { return int(L.size()); }
-    const TConv& conv(int layer) const { return layer == l_att2() ? att2 : L[layer].conv; }
+    // convs by layer index: L's, then hconv
+    int n_conv() const { return int(L.size() + hconv.size()); }
+    const TConv& conv(int layer) const { return layer < int(L.size()) ? L[layer].conv : hconv[layer - L.size()]; }
+    bool attentive() const { return cfg.pooling == PPV_POOL_ASP || cfg.pooling == PPV_POOL_SAP; }  // softmax pooling over logits
+    bool context() const { return cfg.pooling == PPV_POOL_ASP && cfg.global_context; }
     size_t workspace_bytes(int B, int T) const override;
     using PlanOwner::run_plan;
 
@@ -131,8 +137,9 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
         return fail(PPV_EUNSUPPORTED, "trainer: kernel sizes must be [odd,3,3,3,1]");
     if (cfg->attention_channels % 64 || cfg->se_channels % 8 || cfg->embd_dim % 8)
         return fail(PPV_EUNSUPPORTED, "trainer: attention_channels % 64, se_channels % 8, embd_dim % 8 required");
-    if (cfg->pooling != PPV_POOL_ASP || !cfg->global_context)
-        return fail(PPV_EUNSUPPORTED, "trainer: the training step implements pooling_type ASP with global_context");
+    if (cfg->pooling < PPV_POOL_ASP || cfg->pooling > PPV_POOL_TSP) return fail(PPV_EUNSUPPORTED, "trainer: pooling must be PPV_POOL_ASP / SAP / TAP / TSP");
+    if (cfg->pooling == PPV_POOL_SAP && cfg->attention_channels != 128)  // as the inference model refuses it, so a trained model can be evaluated
+        return fail(PPV_EUNSUPPORTED, "trainer: SAP pooling uses a 128-channel bottleneck (ecapa_tdnn.py:222): attention_channels must be 128");
     EcapaGeometry g;  // its checks pass where the ones above do
     int rc = ecapa_geometry(*cfg, &g);
     if (rc) return rc;
@@ -172,22 +179,36 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
         t->se2_b[b] = tr_add(t->pmap, t->n_params, p + ".se_block.conv2.conv.bias", C);
     }
     t->l_mfa = add_layer("mfa", t->C3, t->C3, 1, 1, true);
-    t->l_att1 = add_layer("asp.tdnn", 3 * t->C3, t->att, 1, 1, true);
-    {
+    // a 1x1 conv of the head without a BatchNorm after it ("<name>.weight" [Cout, Cin, 1], "<name>.bias" [Cout])
+    auto add_head_conv = [&](const std::string& name, int cin, int cout) {
+        TConv c;
+        c.name = name;
+        c.Cout = cout;
+        c.Cin = c.CinTotal = c.Cinp = cin;
+        c.w_off = tr_add(t->pmap, t->n_params, name + ".weight", int64_t(cout) * cin);
+        c.b_off = tr_add(t->pmap, t->n_params, name + ".bias", cout);
+        t->hconv.push_back(c);
+        return int(t->L.size() + t->hconv.size()) - 1;
+    };
+    // the head and its asp_bn in the reference's state_dict order (ecapa_tdnn.py:212-241): ASP's BatchNorm1d wraps paddle's as `.norm`
+    const int pool = cfg->pooling;
+    t->Kp = (pool == PPV_POOL_ASP || pool == PPV_POOL_TSP) ? 2 * t->C3 : t->C3;
+    if (pool == PPV_POOL_ASP) {
+        t->l_att1 = add_layer("asp.tdnn", (cfg->global_context ? 3 : 1) * t->C3, t->att, 1, 1, true);
         TConv& c1 = t->L[t->l_att1].conv;  // only the first C3 input channels go through the frame-level GEMM
         c1.Cin = t->C3;
         c1.Cinp = t->C3;
+        t->c_att2 = add_head_conv("asp.conv.conv", t->att, t->C3);
+    } else if (pool == PPV_POOL_SAP) {
+        t->c_lin1 = add_head_conv("asp.linear1", t->C3, t->att);
+        t->c_att2 = add_head_conv("asp.linear2", t->att, t->C3);
     }
-    t->att2.name = "asp.conv.conv";
-    t->att2.Cout = t->C3;
-    t->att2.Cin = t->att2.CinTotal = t->att2.Cinp = t->att;
-    t->att2.w_off = tr_add(t->pmap, t->n_params, "asp.conv.conv.weight", int64_t(t->C3) * t->att);
-    t->att2.b_off = tr_add(t->pmap, t->n_params, "asp.conv.conv.bias", t->C3);
-    t->aspbn_g = tr_add(t->pmap, t->n_params, "asp_bn.norm.weight", 2 * t->C3);
-    t->aspbn_b = tr_add(t->pmap, t->n_params, "asp_bn.norm.bias", 2 * t->C3);
-    t->aspbn_rm = tr_add(t->smap, t->n_stats, "asp_bn.norm._mean", 2 * t->C3);
-    t->aspbn_rv = tr_add(t->smap, t->n_stats, "asp_bn.norm._variance", 2 * t->C3);
-    t->fc_w = tr_add(t->pmap, t->n_params, "fc.conv.weight", int64_t(t->D) * 2 * t->C3);
+    const std::string bn = pool == PPV_POOL_ASP ? "asp_bn.norm" : "asp_bn";
+    t->aspbn_g = tr_add(t->pmap, t->n_params, bn + ".weight", t->Kp);
+    t->aspbn_b = tr_add(t->pmap, t->n_params, bn + ".bias", t->Kp);
+    t->aspbn_rm = tr_add(t->smap, t->n_stats, bn + "._mean", t->Kp);
+    t->aspbn_rv = tr_add(t->smap, t->n_stats, bn + "._variance", t->Kp);
+    t->fc_w = tr_add(t->pmap, t->n_params, "fc.conv.weight", int64_t(t->D) * t->Kp);
     t->fc_b = tr_add(t->pmap, t->n_params, "fc.conv.bias", t->D);
     t->cls_w = tr_add(t->pmap, t->n_params, "classifier.weight", int64_t(t->D) * t->S);  // fc.py:30-36: [input_dim, num_speakers]
     *out = t;
@@ -260,13 +281,15 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     const int64_t Rp = f->Rp;
     const int C = t->C, C3 = t->C3;
     auto f32 = [&](size_t n) { return static_cast<float*>(cv.take(n * sizeof(float))); };
-    f->layer.assign(t->l_att2() + 1, TrBuffers::Layer());
-    for (int l = 0; l <= t->l_att2(); ++l) {
+    const int Kp = t->Kp;
+    const bool attn = t->attentive(), ctx = t->context(), asp = t->cfg.pooling == PPV_POOL_ASP;
+    f->layer.assign(t->n_conv(), TrBuffers::Layer());
+    for (int l = 0; l < t->n_conv(); ++l) {
         const TConv& c = t->conv(l);
         TrBuffers::Layer& w = f->layer[l];
         w.wf = cv.planes(int64_t(align_up(size_t(c.Cout), 256)), c.taps * c.Cinp);
         if (c.dgrad) w.wd = cv.planes(int64_t(align_up(size_t(c.Cinp), 256)), c.taps * c.Cout);
-        if (l == t->l_att2()) break;
+        if (l >= int(t->L.size())) continue;
         const int Cb = t->L[l].bn.C;
         w.mean = f32(Cb);
         w.rstd = f32(Cb);
@@ -285,32 +308,42 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
         f->se_g2[b] = f32(size_t(B) * C);
     }
     act({&f->OUTCAT, &f->Amfa, &f->M}, C3);
-    act({&f->Aatt, &f->A4}, t->att);
-    f->gstat_pl = cv.planes(B, 2 * C3);
-    f->logits = f32(size_t(Rp) * C3);
-    f->gstat = f32(size_t(B) * 2 * C3);
-    f->fold = f32(size_t(B) * t->att);
-    f->pooled = f32(size_t(B) * 2 * C3);
-    f->pn = f32(size_t(B) * 2 * C3);
+    // the head's buffers, carved only for the heads that use them; the attention of SAP (tanh(linear1)) lands in A4 like ASP's
+    if (asp) act({&f->Aatt}, t->att);
+    if (attn) act({&f->A4}, t->att);
+    if (ctx) f->gstat_pl = cv.planes(B, 2 * C3);
+    if (attn) f->logits = f32(size_t(Rp) * C3);
+    if (ctx) {
+        f->gstat = f32(size_t(B) * 2 * C3);
+        f->fold = f32(size_t(B) * t->att);
+    }
+    f->pooled = f32(size_t(B) * Kp);
+    f->pn = f32(size_t(B) * Kp);
     f->emb = f32(size_t(B) * t->D);
     f->cls_logits = f32(size_t(B) * t->S);
     f->loss = f32(8);
-    f->aspbn_mean = f32(2 * C3);
-    f->aspbn_rstd = f32(2 * C3);
+    f->aspbn_mean = f32(Kp);
+    f->aspbn_rstd = f32(Kp);
     // gradients
-    act({&f->dlogits, &f->dMd}, C3);
-    act({&f->dA4, &f->dZatt}, t->att);
-    act({&f->dMatt, &f->dZmfa, &f->dOUTCAT}, C3);
+    if (attn) act({&f->dlogits}, C3);
+    act({&f->dMd}, C3);
+    if (attn) {
+        act({&f->dA4, &f->dZatt}, t->att);
+        act({&f->dMatt}, C3);
+    }
+    act({&f->dZmfa, &f->dOUTCAT}, C3);
     for (int b = 0; b < 3; ++b) act({&f->Dbuf[b], &f->dZt2[b], &f->dRC[b], &f->dZres[b], &f->DIN[b], &f->dZt1[b], &f->dXt1[b]}, C);
     act({&f->dZ0}, C);
     f->TA = cv.planes(C3, int(Rp));
     f->TB = cv.planes(C3, int(Rp));
     f->d_emb = f32(size_t(B) * t->D);
-    f->dpn = f32(size_t(B) * 2 * C3);
-    f->dpooled = f32(size_t(B) * 2 * C3);
-    f->dgs = f32(size_t(B) * 2 * C3);
-    f->rs = f32(size_t(B) * C3);
-    f->rb = f32(size_t(B) * C3);
+    f->dpn = f32(size_t(B) * Kp);
+    f->dpooled = f32(size_t(B) * Kp);
+    if (ctx) {
+        f->dgs = f32(size_t(B) * 2 * C3);
+        f->rs = f32(size_t(B) * C3);
+        f->rb = f32(size_t(B) * C3);
+    }
     f->dg2 = f32(size_t(B) * C);
     f->dg1 = f32(size_t(B) * t->se);
     f->ds = f32(size_t(B) * C);
@@ -321,7 +354,7 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     f->part = f32(f->part_elems);
     // weight-gradient partials: the largest split-K output of any conv
     size_t wmax = 0;
-    for (int l = 0; l <= t->l_att2(); ++l) {
+    for (int l = 0; l < t->n_conv(); ++l) {
         const TConv& c = t->conv(l);
         const WgradSplit w = tr_wgrad_split(t, c, Rp);
         wmax = std::max(wmax, size_t(w.splits) * w.Mpad * c.taps * c.Cinp);
@@ -329,13 +362,19 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
     f->wpart = f32(wmax);
     f->aam_ws_bytes = aam_workspace_bytes(B, t->D, t->S);
     f->aam_ws = static_cast<float*>(cv.take(f->aam_ws_bytes));
+    if (t->cfg.pooling == PPV_POOL_SAP) {  // the softmax pooling's [mean | std] and the gradient it reads back (std half: zero)
+        f->sap_stats = f32(size_t(B) * 2 * C3);
+        f->dsap_stats = f32(size_t(B) * 2 * C3);
+    }
 }
 
-// The taps trainer_read_tap serves, by name without the "pad:" prefix and the block suffix.
+// The taps trainer_read_tap serves, by name without the "pad:" prefix and the block suffix.  A buffer the head does not carve
+// has no tap.
 std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, int B) {
     const int C = t->C, C3 = t->C3;
     std::map<std::string, TrTap> m;
     auto planes = [&](const std::string& name, const Planes* p, bool per_block, int cols, int col0 = 0) {
+        if (!p[0].base) return;
         TrTap& e = m[name];
         e.per_block = per_block;
         for (int b = 0; b < (per_block ? 3 : 1); ++b) e.pl[b] = p[b];
@@ -343,6 +382,7 @@ std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, 
         e.col0 = col0;
     };
     auto vec = [&](const std::string& name, float* const* p, bool per_block, size_t count) {
+        if (!p[0]) return;
         TrTap& e = m[name];
         e.per_block = per_block;
         e.fp32 = true;
@@ -370,11 +410,12 @@ std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, 
                                      {"g:dXt1", f.dXt1}})
         planes(e.first, e.second, true, C);
     // fp32 as stored
-    vec("asp", &f.pooled, false, size_t(B) * 2 * C3);
+    vec("asp", &f.pooled, false, size_t(B) * t->Kp);
     for (const auto& e : NamedVec{{"emb", &f.emb}, {"d_emb", &f.d_emb}}) vec(e.first, e.second, false, size_t(B) * t->D);
     vec("logits", &f.logits, false, size_t(f.R) * C3);
-    for (const auto& e : NamedVec{{"gstat", &f.gstat}, {"dgs", &f.dgs}, {"pn", &f.pn}, {"dpn", &f.dpn}, {"dpooled", &f.dpooled}})
+    for (const auto& e : NamedVec{{"gstat", &f.gstat}, {"dgs", &f.dgs}, {"sap_stats", &f.sap_stats}, {"dsap_stats", &f.dsap_stats}})
         vec(e.first, e.second, false, size_t(B) * 2 * C3);
+    for (const auto& e : NamedVec{{"pn", &f.pn}, {"dpn", &f.dpn}, {"dpooled", &f.dpooled}}) vec(e.first, e.second, false, size_t(B) * t->Kp);
     for (const auto& e : NamedVec{{"rs", &f.rs}, {"rb", &f.rb}}) vec(e.first, e.second, false, size_t(B) * C3);
     for (const auto& e : NamedVec{{"dg2", &f.dg2}, {"ds", &f.ds}}) vec(e.first, e.second, false, size_t(B) * C);
     vec("dg1", &f.dg1, false, size_t(B) * t->se);
@@ -537,7 +578,7 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
     };
 
     // ================================================================= forward
-    for (int l = 0; l <= t->l_att2(); ++l) {
+    for (int l = 0; l < t->n_conv(); ++l) {
         const TConv& c = t->conv(l);
         push("tr_repack_conv", [w = par + c.w_off, w_ld = int64_t(c.CinTotal) * c.taps, Cout = c.Cout, Cin = c.Cin, Cinp = c.Cinp, taps = c.taps,
                                 wf = f.layer[l].wf, wd = f.layer[l].wd](const StepRun& r) {
@@ -590,7 +631,16 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         if (rc) return rc;
         bn_fwd(t->l_mfa, f.Amfa, 0, f.M, 0, 0, nullptr, 0, nullptr, 0);
     }
-    {
+    const int pool = t->cfg.pooling, Kp = t->Kp;
+    // copies the [B, C3] mean half of a [B, 2*C3] softmax-pooling row block to or from a plain [B, C3] matrix (SAP)
+    auto mean_half = [&](float* dst, int dst_ld, const float* src, int src_ld) {
+        push("cudaMemcpy2DAsync", [dst, dst_ld, src, src_ld, B, C3](const StepRun& r) {
+            PPV_CUDA_OK(cudaMemcpy2DAsync(dst, size_t(dst_ld) * sizeof(float), src, size_t(src_ld) * sizeof(float), size_t(C3) * sizeof(float), B,
+                                          cudaMemcpyDeviceToDevice, r.st));
+            return PPV_OK;
+        });
+    };
+    if (t->context()) {
         // global stats -> per-utterance bias of the attention TDNN: its weight [att][3*C3], columns C3.. multiply [mean | std]
         t->steps.push_back(colstats_step(f.M, C3, B, T, P, Tp, 1, TR_ASP_EPS, f.gstat_pl));
         push("launch_planes_to_f32", [x = f.gstat_pl, Cn = 2 * C3, B, out = f.gstat](const StepRun& r) {
@@ -598,23 +648,37 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         });
         dense_fwd(f.gstat, 2 * C3, par + t->L[t->l_att1].conv.w_off + C3, 3 * C3, nullptr, B, att, 2 * C3, 0, f.fold, att);
     }
-    {
+    if (pool == PPV_POOL_ASP) {
         rc = fwd_gemm(t->l_att1, {GemmSource{f.M, 0, C3, 0}}, f.Aatt, 0, true, f.fold, nullptr);
         if (rc) return rc;
         bn_fwd(t->l_att1, f.Aatt, 0, f.A4, 0, 1, nullptr, 0, nullptr, 0);
-        rc = fwd_gemm(t->l_att2(), {GemmSource{f.A4, 0, t->att, 0}}, Planes(), 0, false, nullptr, f.logits);
+    } else if (pool == PPV_POOL_SAP) {  // tanh(linear1(M)) (pooling.py:62): no ReLU, no BatchNorm
+        const TConv& c = t->conv(t->c_lin1);
+        Epilogue ep = planes_epilogue(f.A4, 0, Tp, P, T);
+        ep.bias = par + c.b_off;
+        ep.tanh_ = 1;
+        rc = gemm({GemmSource{f.M, 0, C3, 0}}, f.layer[t->c_lin1].wf, c.Cout, ep);
         if (rc) return rc;
     }
-    {
-        // softmax pooling, asp_bn (batch statistics), fc, AAM-softmax loss
-        push("launch_asp_pool", [logits = f.logits, C3, x = f.M, B, T, P, Tp, pooled = f.pooled](const StepRun& r) {
-            return launch_asp_pool(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), pooled, r.st);
+    if (t->attentive()) {
+        rc = fwd_gemm(t->c_att2, {GemmSource{f.A4, 0, t->att, 0}}, Planes(), 0, false, nullptr, f.logits);
+        if (rc) return rc;
+        // softmax pooling: ASP keeps [mean | std]; SAP pools the mean alone (pooling.py:63-65)
+        float* const out = pool == PPV_POOL_SAP ? f.sap_stats : f.pooled;
+        push("launch_asp_pool", [logits = f.logits, C3, x = f.M, B, T, P, Tp, out](const StepRun& r) {
+            return launch_asp_pool(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, nullptr, nullptr, Planes(), out, r.st);
         });
-        push("tr_bn1d_fwd", [x = f.pooled, B, Cn = 2 * C3, gamma = par + t->aspbn_g, beta = par + t->aspbn_b, y = f.pn, mean = f.aspbn_mean,
+        if (pool == PPV_POOL_SAP) mean_half(f.pooled, C3, f.sap_stats, 2 * C3);
+    } else {  // TAP: mean over time; TSP: mean | unbiased variance (pooling.py:8-47)
+        t->steps.push_back(colstats_step(f.M, C3, B, T, P, Tp, pool == PPV_POOL_TAP ? 0 : 3, 0.f, Planes(), 0.f, false, f.pooled));
+    }
+    {
+        // asp_bn (batch statistics), fc, AAM-softmax loss
+        push("tr_bn1d_fwd", [x = f.pooled, B, Cn = Kp, gamma = par + t->aspbn_g, beta = par + t->aspbn_b, y = f.pn, mean = f.aspbn_mean,
                              rstd = f.aspbn_rstd, run_mean = sta + t->aspbn_rm, run_var = sta + t->aspbn_rv](const StepRun& r) {
             return tr_bn1d_fwd(x, B, Cn, TR_BN_EPS, TR_BN_MOMENTUM, gamma, beta, y, mean, rstd, run_mean, run_var, r.st);
         });
-        dense_fwd(f.pn, 2 * C3, par + t->fc_w, 2 * C3, par + t->fc_b, B, D, 2 * C3, 0, f.emb, D);
+        dense_fwd(f.pn, Kp, par + t->fc_w, Kp, par + t->fc_b, B, D, Kp, 0, f.emb, D);
         push("aam_forward", [emb = f.emb, cls_w = par + t->cls_w, B, D, S = t->S, logits = f.cls_logits, loss = f.loss, aam_ws = f.aam_ws,
                              aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
             const PlanInputs& in = r.in;
@@ -632,28 +696,41 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
             return aam_backward(emb, cls_w, in.labels, logits, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, d_emb, d_cls_w,
                                 aam_ws, aam_ws_bytes, r.st);
         });
-        dense_bwd(f.d_emb, D, f.pn, 2 * C3, par + t->fc_w, 2 * C3, B, D, 2 * C3, f.dpn, 2 * C3, grd + t->fc_w, 2 * C3, grd + t->fc_b);
-        push("tr_bn1d_bwd", [dy = f.dpn, x = f.pooled, B, Cn = 2 * C3, gamma = par + t->aspbn_g, mean = f.aspbn_mean, rstd = f.aspbn_rstd,
+        dense_bwd(f.d_emb, D, f.pn, Kp, par + t->fc_w, Kp, B, D, Kp, f.dpn, Kp, grd + t->fc_w, Kp, grd + t->fc_b);
+        push("tr_bn1d_bwd", [dy = f.dpn, x = f.pooled, B, Cn = Kp, gamma = par + t->aspbn_g, mean = f.aspbn_mean, rstd = f.aspbn_rstd,
                              dx = f.dpooled, dgamma = grd + t->aspbn_g, dbeta = grd + t->aspbn_b](const StepRun& r) {
             return tr_bn1d_bwd(dy, x, B, Cn, gamma, mean, rstd, dx, dgamma, dbeta, r.st);
         });
-        push("tr_asp_bwd", [logits = f.logits, C3, x = f.M, B, T, P, Tp, pooled = f.pooled, dpooled = f.dpooled, dlogits = f.dlogits,
-                            dx = f.dMd](const StepRun& r) {
-            return tr_asp_bwd(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, pooled, dpooled, dlogits, dx, r.st);
-        });
+        if (t->attentive()) {
+            // SAP: the softmax pooling backward reads [d mean | d std] with the std half zero (never written since the workspace
+            // was cleared), so its std terms add exactly zero
+            const float* pooled = f.pooled;
+            const float* dpooled = f.dpooled;
+            if (pool == PPV_POOL_SAP) {
+                mean_half(f.dsap_stats, 2 * C3, f.dpooled, C3);
+                pooled = f.sap_stats;
+                dpooled = f.dsap_stats;
+            }
+            push("tr_asp_bwd", [logits = f.logits, C3, x = f.M, B, T, P, Tp, pooled, dpooled, dlogits = f.dlogits, dx = f.dMd](const StepRun& r) {
+                return tr_asp_bwd(logits, C3, x, C3, B, T, P, Tp, TR_ASP_EPS, pooled, dpooled, dlogits, dx, r.st);
+            });
+        } else {
+            push("tr_pool_stats_bwd", [x = f.M, C3, B, T, P, Tp, pooled = f.pooled, dpooled = f.dpooled, var = pool == PPV_POOL_TSP,
+                                       dx = f.dMd](const StepRun& r) { return tr_pool_stats_bwd(x, C3, B, T, P, Tp, pooled, dpooled, var, dx, r.st); });
+        }
     }
-    {
-        // asp.conv: bias, weight, data gradients
+    if (t->attentive()) {
+        // asp.conv / asp.linear2: bias, weight, data gradients
         GradSrcList gl;
         gl.n = 1;
         gl.s[0] = src1(f.dlogits, 0, 0);
-        grad_sum(gl, C3, Planes(), grd + t->att2.b_off);
-        rc = wgrad(t->l_att2(), f.dlogits, 0, {{f.A4, 0, t->att, 0}});
+        grad_sum(gl, C3, Planes(), grd + t->conv(t->c_att2).b_off);
+        rc = wgrad(t->c_att2, f.dlogits, 0, {{f.A4, 0, t->att, 0}});
         if (rc) return rc;
-        rc = dgrad_gemm(t->l_att2(), f.dlogits, 0, f.dA4, 0);
+        rc = dgrad_gemm(t->c_att2, f.dlogits, 0, f.dA4, 0);
         if (rc) return rc;
     }
-    {
+    if (pool == PPV_POOL_ASP) {
         // attention TDNN: tanh, BN, ReLU backward; per-utterance context gradients (from the sums the BN backward leaves in f.part
         // [B][att]); frame-level weight / data gradients
         GradSrcList gl;
@@ -661,26 +738,42 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
         gl.s[0] = src1(f.dA4, 0, 0);
         gl.s[0].dtanh = f.A4;
         bn_bwd(t->l_att1, gl, f.Aatt, 0, f.dZatt, 0);
-        const TConv& c = t->L[t->l_att1].conv;
-        dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3, nullptr);
-        push("tr_asp_global_bwd", [gstat = f.gstat, dgs = f.dgs, B, C3, T, rs = f.rs, rb = f.rb](const StepRun& r) {
-            return tr_asp_global_bwd(gstat, dgs, B, C3, T, TR_ASP_EPS, rs, rb, r.st);
-        });
+        if (t->context()) {
+            const TConv& c = t->L[t->l_att1].conv;
+            dense_bwd(f.part, att, f.gstat, 2 * C3, par + c.w_off + C3, 3 * C3, B, att, 2 * C3, f.dgs, 2 * C3, grd + c.w_off + C3, 3 * C3, nullptr);
+            push("tr_asp_global_bwd", [gstat = f.gstat, dgs = f.dgs, B, C3, T, rs = f.rs, rb = f.rb](const StepRun& r) {
+                return tr_asp_global_bwd(gstat, dgs, B, C3, T, TR_ASP_EPS, rs, rb, r.st);
+            });
+        }
         rc = wgrad(t->l_att1, f.dZatt, 0, {{f.M, 0, C3, 0}});
         if (rc) return rc;
         rc = dgrad_gemm(t->l_att1, f.dZatt, 0, f.dMatt, 0);
         if (rc) return rc;
+    } else if (pool == PPV_POOL_SAP) {
+        // linear1: tanh' straight after linear2's data gradient (no BatchNorm, no ReLU); the summed rows are linear1's bias gradient
+        GradSrcList gl;
+        gl.n = 1;
+        gl.s[0] = src1(f.dA4, 0, 0);
+        gl.s[0].dtanh = f.A4;
+        grad_sum(gl, att, f.dZatt, grd + t->conv(t->c_lin1).b_off);
+        rc = wgrad(t->c_lin1, f.dZatt, 0, {{f.M, 0, C3, 0}});
+        if (rc) return rc;
+        rc = dgrad_gemm(t->c_lin1, f.dZatt, 0, f.dMatt, 0);
+        if (rc) return rc;
     }
     {
-        // MFA: d(M) = ASP direct + attention path + global-context statistics (as row scale / bias on M itself)
+        // MFA: d(M) = pooling direct (+ attention path) (+ ASP's global-context statistics, as row scale / bias on M itself)
         GradSrcList gl;
-        gl.n = 3;
+        gl.n = 1;
         gl.s[0] = src1(f.dMd, 0, 0);
-        gl.s[1] = src1(f.dMatt, 0, 0);
-        gl.s[2] = src1(f.M, 0, 0);
-        gl.s[2].rowscale = f.rs;
-        gl.s[2].rowbias = f.rb;
-        gl.s[2].row_ld = C3;
+        if (t->attentive()) gl.s[gl.n++] = src1(f.dMatt, 0, 0);
+        if (t->context()) {
+            gl.s[gl.n] = src1(f.M, 0, 0);
+            gl.s[gl.n].rowscale = f.rs;
+            gl.s[gl.n].rowbias = f.rb;
+            gl.s[gl.n].row_ld = C3;
+            gl.n++;
+        }
         bn_bwd(t->l_mfa, gl, f.Amfa, 0, f.dZmfa, 0);
         rc = wgrad(t->l_mfa, f.dZmfa, 0, {{f.OUTCAT, 0, C3, 0}});
         if (rc) return rc;
@@ -792,9 +885,12 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
 //     forward   "blocks.0".."blocks.3", "mfa" (block outputs); X0, A0, Y0, OUTCAT, Amfa, M, Aatt, A4; per block ("<name>:<0..2>")
 //               At1, Yt1, Ares, RC, IN, At2, Yt2.  A* are the post-ReLU, pre-BatchNorm activations the BatchNorm backward reads.
 //     gradients "g:<name>": dZ0, dOUTCAT, dMd, dMatt, dZmfa, dlogits, dZatt, dA4; per block D, dZt2, dRC, dZres, DIN, dZt1, dXt1
-//   fp32 as stored: "asp" (pooled) [B, 2*C3], "emb" and "d_emb" [B, D], "logits" [B, Tp, C3] (every row), gstat, dgs, pn, dpn, dpooled
-//     [B, 2*C3], rs, rb [B, C3]; per block se_s, se_g2 [B, C], se_g1 [B, se]; dg2, ds [B, C] and dg1 [B, se] are scratch that every
-//     block's SE backward overwrites, so they hold block 0's values.
+//   fp32 as stored: "asp" (pooled) [B, Kp], "emb" and "d_emb" [B, D], "logits" [B, Tp, C3] (every row), gstat, dgs [B, 2*C3], pn, dpn,
+//     dpooled [B, Kp], rs, rb [B, C3]; SAP: sap_stats (the softmax pooling's [mean | std]) and dsap_stats (the [d mean | 0] its backward
+//     reads) [B, 2*C3]; per block se_s, se_g2 [B, C], se_g1 [B, se]; dg2, ds [B, C] and dg1 [B, se] are scratch that every block's SE
+//     backward overwrites, so they hold block 0's values.
+// Kp = 2*C3 for ASP and TSP, C3 for SAP and TAP.  A head has the taps of the buffers it uses: Aatt, gstat, dgs, rs, rb are ASP's (the last
+// four with global context), A4, logits and the attention gradients ASP's and SAP's.
 // A per-block name without a block suffix reads block 0.
 int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems, cudaStream_t st) {
     PPV_REQUIRE(t && name && out, "trainer_read_tap: null argument");

@@ -185,6 +185,11 @@ __global__ void __launch_bounds__(STAT_WARPS * 32)
             const float sd = (mode == 2)   ? sqrtf(fmaxf(ssq, 0.f) / float(T > 1 ? T - 1 : 1) + eps)
                              : (mode == 3) ? fmaxf(ssq, 0.f) / float(T > 1 ? T - 1 : 1)
                                            : sqrtf(fmaxf(ssq * inv, eps));
+            if (out_f32) {  // fp32 [B][2C] (the training step's TSP pooling)
+                out_f32[int64_t(b) * 2 * C + cc] = mean;
+                out_f32[int64_t(b) * 2 * C + C + cc] = sd;
+            }
+            if (!out_pl.base) return;
             __nv_bfloat16 h, l;
             split_bf16(mean, h, l);
             out_pl.hi()[int64_t(b) * out_pl.ld + cc] = h;

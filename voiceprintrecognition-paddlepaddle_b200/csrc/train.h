@@ -65,6 +65,11 @@ int tr_bn1d_bwd(const float* dy, const float* x, int B, int C, const float* gamm
                 float* dbeta, cudaStream_t st);
 int tr_asp_bwd(const float* logits, int64_t lg_ld, const Planes& x, int C, int B, int T, int P, int Tp, float eps, const float* pooled,
                const float* dpooled, const Planes& dlogits, const Planes& dx, cudaStream_t st);
+// Backward of temporal average / statistics pooling (TAP / TSP) over x's first C columns: given pooled = [mean | var] and dpooled =
+// [d mean | d var] as fp32 [B][var ? 2C : C], writes dx[b,t,c] = dmean[b,c] / T (+ dvar[b,c] * 2 (x[b,t,c] - mean[b,c]) / (T - 1) with
+// `var`, the unbiased variance) on the T valid frames of each utterance; no other row of dx is written.
+int tr_pool_stats_bwd(const Planes& x, int C, int B, int T, int P, int Tp, const float* pooled, const float* dpooled, bool var, const Planes& dx,
+                      cudaStream_t st);
 int tr_asp_global_bwd(const float* gstat, const float* dgstat, int B, int C, int T, float eps, float* rs, float* rb, cudaStream_t st);
 
 }  // namespace ppv

@@ -608,6 +608,36 @@ __global__ void asp_global_bwd_kernel(const float* __restrict__ gstat, const flo
     rb[i] = dmean / float(T) - s * mean;
 }
 
+// ---------------------------------------------------------------------------------------------- TAP / TSP backward
+// mean = (1/T) sum_t x_t, var = (1/(T-1)) sum_t (x_t - mean)^2 (pooling.py:8-47): dx_t = dmean / T + dvar * 2 (x_t - mean) / (T - 1)
+// (the mean's own gradient through var sums to zero over t).  8 channels per thread, valid frames only; TAP reads no x.  HBM-bound:
+// one pass over x and dx.
+template <bool VAR>
+__global__ void __launch_bounds__(256) pool_stats_bwd_kernel(Planes x, int C, int T, int P, int Tp, int64_t total, const float* __restrict__ pooled,
+                                                             const float* __restrict__ dpooled, Planes dx) {
+    const int groups = C >> 3, ld = VAR ? 2 * C : C;
+    const float inv_t = 1.f / float(T), two_inv_t1 = 2.f / float(T > 1 ? T - 1 : 1);
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+        const int c = int(i % groups) * 8;
+        const int64_t bt = i / groups;
+        const int b = int(bt / T), t = int(bt % T);
+        const int64_t row = int64_t(b) * Tp + P + t;
+        float dm[8], g[8];
+        tr_ld8f(dpooled + int64_t(b) * ld + c, dm);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) g[k] = dm[k] * inv_t;
+        if (VAR) {
+            float v[8], mu[8], dv[8];
+            tr_load8(x, row, c, v);
+            tr_ld8f(pooled + int64_t(b) * ld + c, mu);
+            tr_ld8f(dpooled + int64_t(b) * ld + C + c, dv);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) g[k] = fmaf(dv[k] * two_inv_t1, v[k] - mu[k], g[k]);
+        }
+        tr_store8(dx, row, c, g);
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- Adam
 // paddle.optimizer.Adam with weight_decay = coupled L2 (g += wd * p), bias-corrected step (optimizer/__init__.py:12-18)
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, int64_t n, float lr,
@@ -753,6 +783,18 @@ int tr_asp_bwd(const float* logits, int64_t lg_ld, const Planes& x, int C, int B
 int tr_asp_global_bwd(const float* gstat, const float* dgstat, int B, int C, int T, float eps, float* rs, float* rb, cudaStream_t st) {
     asp_global_bwd_kernel<<<unsigned((int64_t(B) * C + 255) / 256), 256, 0, st>>>(gstat, dgstat, B, C, T, eps, rs, rb);
     TR_LAUNCH_OK("asp_global_bwd_kernel");
+    return PPV_OK;
+}
+int tr_pool_stats_bwd(const Planes& x, int C, int B, int T, int P, int Tp, const float* pooled, const float* dpooled, bool var, const Planes& dx,
+                      cudaStream_t st) {
+    PPV_REQUIRE(C % 8 == 0 && B > 0 && T > 0 && Tp >= T + 2 * P, "pool_stats_bwd: C % 8 == 0 and Tp >= T + 2P required");
+    const int64_t total = int64_t(B) * T * (C / 8);
+    const int grid = int(std::min<int64_t>((total + 255) / 256, int64_t(device_sm_count()) * 16));
+    if (var)
+        pool_stats_bwd_kernel<true><<<grid, 256, 0, st>>>(x, C, T, P, Tp, total, pooled, dpooled, dx);
+    else
+        pool_stats_bwd_kernel<false><<<grid, 256, 0, st>>>(x, C, T, P, Tp, total, pooled, dpooled, dx);
+    TR_LAUNCH_OK("pool_stats_bwd_kernel");
     return PPV_OK;
 }
 int adam_step(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay,

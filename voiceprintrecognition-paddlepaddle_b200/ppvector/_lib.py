@@ -197,6 +197,8 @@ SIGNATURES = {
     "ppv_asp_fused_test": (C.c_int, [_P] * 6 + [C.c_int] * 8 + [_P, _P, _P, C.c_size_t, _P]),
     "ppv_colstats_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "ppv_colstats_test": (C.c_int, [_P] + [C.c_int] * 8 + [C.c_float, C.c_float] + [_P, _P, _P, _P, C.c_size_t, _P]),
+    "ppv_pool_stats_bwd_test_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "ppv_pool_stats_bwd_test": (C.c_int, [_P] * 3 + [C.c_int] * 6 + [_P, _P, C.c_size_t, _P]),
     "ppv_campplus_context_test_workspace_bytes": (C.c_size_t, [C.c_int] * 2),
     "ppv_campplus_context_test": (C.c_int, [_P] + [C.c_int] * 4 + [_P] * 6 + [C.c_size_t, _P]),
     "ppv_gemm_test_taps_workspace_bytes": (C.c_size_t, [C.POINTER(GemmTapsCase)]),

@@ -12,10 +12,17 @@ import torch
 
 from ppvector import _lib
 
+POOLING = {'ASP': _lib.PPV_POOL_ASP, 'SAP': _lib.PPV_POOL_SAP, 'TAP': _lib.PPV_POOL_TAP, 'TSP': _lib.PPV_POOL_TSP}
+
 
 class TrainEngine:
     def __init__(self, input_size=80, num_speakers=2796, embd_dim=192, channels=(512, 512, 512, 512, 1536), kernel_sizes=(5, 3, 3, 3, 1),
-                 dilations=(1, 2, 3, 4, 1), attention_channels=128, res2net_scale=8, se_channels=128, device='cuda'):
+                 dilations=(1, 2, 3, 4, 1), attention_channels=128, res2net_scale=8, se_channels=128, pooling_type='ASP', global_context=True,
+                 device='cuda'):
+        """pooling_type / global_context: the head, as EcapaTdnn's (ecapa_tdnn.py:212-241): 'ASP' (with or without the global context),
+        'SAP' (attention_channels must be 128), 'TAP' or 'TSP'."""
+        if pooling_type not in POOLING:
+            raise ValueError(f'pooling_type must be one of {sorted(POOLING)} (got {pooling_type})')
         self.device = torch.device(device)
         lib = _lib.load()
         cfg = _lib.EcapaCfg()
@@ -24,6 +31,7 @@ class TrainEngine:
         for i in range(5):
             cfg.channels[i], cfg.kernel_sizes[i], cfg.dilations[i] = channels[i], kernel_sizes[i], dilations[i]
         cfg.attention_channels, cfg.res2net_scale, cfg.se_channels = attention_channels, res2net_scale, se_channels
+        cfg.pooling, cfg.global_context = POOLING[pooling_type], int(bool(global_context))
         self.num_speakers, self.embd_dim, self.input_size = num_speakers, embd_dim, input_size
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):

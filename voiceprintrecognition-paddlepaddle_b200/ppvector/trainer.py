@@ -5,9 +5,9 @@ return values; featurisation, the backbone, the trial x enrol cosine matrix and 
 through libppv_b200; with the optional ``dataset_conf.eval_conf.score_norm`` key the matrix is AS-normalised against a cohort list first
 (ppvector/metric/score_norm.py).  ``train`` (trainer.py:281-365 with the step of :206-229) runs the CUDA training step of
 ``ppvector.train_engine.TrainEngine`` (train-mode forward, AAM loss, backward, one gradient all-reduce over NCCL, Adam) with the
-reference's schedules; it is implemented for EcapaTdnn + AAMLoss + Adam + WarmupCosineSchedulerLR (configs/ecapa_tdnn.yml) and
-raises for other combinations.  Checkpoints follow the reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}``
-with best-EER tracking, optimizer state and ``model.state``) and ``resume_model`` / an existing ``last_model`` restore the weights, the Adam
+reference's schedules; it is implemented for EcapaTdnn with any pooling head (ASP with or without the global context, SAP, TAP, TSP)
++ AAMLoss + Adam + WarmupCosineSchedulerLR (configs/ecapa_tdnn.yml) and raises for other combinations.  Checkpoints follow the
+reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}`` with best-EER tracking, optimizer state and ``model.state``) and ``resume_model`` / an existing ``last_model`` restore the weights, the Adam
 moments, the step counters of both schedules and the epoch.  VisualDL logging is out of scope."""
 import os
 
@@ -166,6 +166,15 @@ class PPVectorTrainer(object):
             raise NotImplementedError('training on the H100 path implements AAMLoss / AMLoss / ARMLoss / CELoss / SubCenterLoss / SphereFace2 + Adam (configs/ecapa_tdnn.yml)')
         if cf.dataset_conf.get('is_use_pksampler', False):
             raise NotImplementedError('PKSampler is out of scope of the H100 path')
+        model_args = dict(cf.model_conf.get('model_args', {}))
+        pooling_type = model_args.get('pooling_type', 'ASP')
+        if pooling_type not in ('ASP', 'SAP', 'TAP', 'TSP'):
+            raise Exception(f'没有{pooling_type}池化层！')  # ecapa_tdnn.py:242-243
+        if pooling_type == 'SAP' and int(model_args.get('attention_channels', 128)) != 128:  # the inference model refuses it too
+            raise NotImplementedError('SAP pooling uses a 128-channel bottleneck (ecapa_tdnn.py:222): attention_channels must be 128')
+        ch = list(model_args.get('channels', (512, 512, 512, 512, 1536)))
+        if len(ch) != 5 or ch[1:4] != [ch[0]] * 3 or ch[4] != 3 * ch[0]:
+            raise NotImplementedError(f'the CUDA training step implements channels [C, C, C, C, 3C] (got {ch})')
         torch.manual_seed(1000)  # trainer.py:290
         np.random.seed(1000)
         _random.seed(1000)
@@ -178,11 +187,8 @@ class PPVectorTrainer(object):
         sampler = cf.dataset_conf.get('sampler', {})
         batch_size = int(sampler.get('batch_size', 64))
         num_speakers = int(cf.model_conf.classifier.num_speakers)
-        model_args = dict(cf.model_conf.get('model_args', {}))
         backbone = build_model(input_size=fz.feature_dim, configs=cf)  # random init with the mirror's initialisers, names = state_dict
         cls_conf = dict(cf.model_conf.get('classifier', {}))
-        if model_args.get('pooling_type', 'ASP') != 'ASP' or not model_args.get('global_context', True):
-            raise NotImplementedError('the CUDA training step implements pooling_type="ASP" with global_context')
         if cls_conf.get('classifier_type', 'Cosine') != 'Cosine' or int(cls_conf.get('num_blocks', 0)) != 0:
             raise NotImplementedError('the CUDA training step implements classifier_type="Cosine", num_blocks=0')
         cls_K = int(cls_conf.get('K', 1))  # fc.py:33: K sub-centres per class (SubCenterLoss); the classifier has num_speakers * K columns
@@ -191,8 +197,8 @@ class PPVectorTrainer(object):
             raise ValueError(f'classifier K={cls_K} and loss K={loss_K} differ (SubCenterLoss needs model_conf.classifier.K == loss_args.K)')
         num_classes = num_speakers
         num_speakers = num_speakers * cls_K  # columns of the classifier from here on
-        engine_args = {k: model_args[k] for k in ('channels', 'kernel_sizes', 'dilations', 'attention_channels', 'res2net_scale', 'se_channels')
-                       if k in model_args}
+        engine_args = {k: model_args[k] for k in ('channels', 'kernel_sizes', 'dilations', 'attention_channels', 'res2net_scale', 'se_channels',
+                                                  'pooling_type', 'global_context') if k in model_args}
         engine = TrainEngine(input_size=fz.feature_dim, num_speakers=num_speakers, embd_dim=model_args.get('embd_dim', 192), device=self.device,
                              **engine_args)
         if cf.train_conf.get('enable_amp', False):
