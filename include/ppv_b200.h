@@ -51,7 +51,16 @@ int ppv_device_sm_count(void);
  * Fbank front end.  Replaces ppvector/data_utils/featurizer.py:88-101 (KaldiFbank.forward ->
  * paddleaudio.compliance.kaldi.fbank per utterance) and :33-60 (AudioFeaturizer.forward:
  * transpose, subtract the time mean, optional tail mask).
+ *
+ * The window is int(sample_rate * frame_length_ms / 1000) samples and is zero-padded to the next power of two, which must lie in
+ * [128, 4096].  A 512-point FFT with snip_edges, remove_dc_offset, use_power and use_log_fbank runs on a register-resident kernel
+ * built for that size; every other configuration runs on a general per-frame kernel.  ppv_fbank_create picks one from the config.
  * ------------------------------------------------------------------------------------------- */
+#define PPV_FBANK_WIN_POVEY 0
+#define PPV_FBANK_WIN_HANNING 1
+#define PPV_FBANK_WIN_HAMMING 2
+#define PPV_FBANK_WIN_RECTANGULAR 3
+#define PPV_FBANK_WIN_BLACKMAN 4
 typedef struct {
     int sample_rate;       /* 16000 */
     int n_mels;            /* 80 (<= 128) */
@@ -61,16 +70,31 @@ typedef struct {
     float low_freq;        /* 20 */
     float high_freq;       /* 0 => Nyquist */
     float log_floor;       /* 1.1920929e-07 (FLT_EPSILON) */
+    int window_type;       /* PPV_FBANK_WIN_POVEY */
+    float blackman_coeff;  /* 0.42 */
+    int remove_dc_offset;  /* 1: subtract each frame's mean */
+    int snip_edges;        /* 1: only frames that fit; 0: (L + shift/2) / shift frames over the edge-reflected waveform */
+    int use_power;         /* 1: power spectrum; 0: magnitude */
+    int use_log_fbank;     /* 1: log(max(mel, log_floor)); 0: linear mel energies */
+    float vtln_warp;       /* 1 => no warping */
+    float vtln_low;        /* 100 */
+    float vtln_high;       /* -500 => offset from Nyquist */
 } ppv_fbank_cfg;
 
 void ppv_fbank_default_cfg(ppv_fbank_cfg* cfg);
 int ppv_fbank_create(const ppv_fbank_cfg* cfg, ppv_fbank_t** out);
 int ppv_fbank_destroy(ppv_fbank_t* h);
-/* snip_edges frame count for L samples (0 if L < window). */
 /* As ppv_fbank_forward for a zero-padded batch of utterances of DIFFERENT lengths, each featurised as if alone (the training data
  * path, reader.py:101-104 + collate_fn.py:5-23): valid_frames[b] (device int32) frames of utterance b are real; the time mean is taken
- * over those only and frames beyond them are written as zeros. */
+ * over those only and frames beyond them are written as zeros.  With snip_edges = 0 the frames at an utterance's end reflect the
+ * padding instead of its own samples: use ppv_fbank_forward_ragged_samples there. */
 int ppv_fbank_forward_ragged(ppv_fbank_t* h, const float* wav, const int32_t* valid_frames, int B, int L, float* out, void* stream);
+/* As ppv_fbank_forward_ragged, and num_samples[b] (device int32, <= L) is utterance b's own length, where its right edge is reflected
+ * when snip_edges = 0; valid_frames[b] must be ppv_fbank_num_frames(h, num_samples[b]). */
+int ppv_fbank_forward_ragged_samples(ppv_fbank_t* h, const float* wav, const int32_t* valid_frames, const int32_t* num_samples, int B, int L,
+                                     float* out, void* stream);
+/* Frame count for L samples: snip_edges: 1 + (L - window) / shift (0 if L < window); otherwise (L + shift/2) / shift, or 0 when the
+ * reflected waveform is too short to hold the last frame (torchaudio's _get_strided cannot frame it either). */
 int ppv_fbank_num_frames(const ppv_fbank_t* h, int L);
 int ppv_fbank_feature_dim(const ppv_fbank_t* h);
 /* wav [B,L] fp32 in [-1,1] -> out [B,T,n_mels] fp32, time-mean subtracted; if lens_ratio != NULL,

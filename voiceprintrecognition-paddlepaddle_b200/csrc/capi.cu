@@ -97,6 +97,15 @@ void ppv_fbank_default_cfg(ppv_fbank_cfg* c) {
     c->low_freq = 20.f;
     c->high_freq = 0.f;
     c->log_floor = 1.1920928955078125e-07f;
+    c->window_type = PPV_FBANK_WIN_POVEY;
+    c->blackman_coeff = 0.42f;
+    c->remove_dc_offset = 1;
+    c->snip_edges = 1;
+    c->use_power = 1;
+    c->use_log_fbank = 1;
+    c->vtln_warp = 1.f;
+    c->vtln_low = 100.f;
+    c->vtln_high = -500.f;
 }
 
 int ppv_fbank_create(const ppv_fbank_cfg* cfg, ppv_fbank_t** out) {
@@ -134,6 +143,15 @@ int ppv_fbank_forward_ragged(ppv_fbank_t* h, const float* wav, const int32_t* va
     PPV_REQUIRE(h && wav && out && valid_frames, "ppv_fbank_forward_ragged: null argument");
     PPV_REQUIRE(B > 0 && L > 0, "ppv_fbank_forward_ragged: empty input");
     return fbank_run(h->impl, wav, nullptr, B, L, out, out, Planes(), 0, 0, static_cast<cudaStream_t>(stream), valid_frames);
+    PPV_GUARD_END
+}
+
+int ppv_fbank_forward_ragged_samples(ppv_fbank_t* h, const float* wav, const int32_t* valid_frames, const int32_t* num_samples, int B, int L,
+                                     float* out, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(h && wav && out && valid_frames && num_samples, "ppv_fbank_forward_ragged_samples: null argument");
+    PPV_REQUIRE(B > 0 && L > 0, "ppv_fbank_forward_ragged_samples: empty input");
+    return fbank_run(h->impl, wav, nullptr, B, L, out, out, Planes(), 0, 0, static_cast<cudaStream_t>(stream), valid_frames, num_samples);
     PPV_GUARD_END
 }
 

@@ -357,7 +357,7 @@ void fbank_destroy(Fbank* h);
 int fbank_num_frames(const Fbank* h, int L);
 int fbank_n_mels(const Fbank* h);
 int fbank_run(Fbank* h, const float* wav, const float* lens_ratio, int B, int L, float* raw, float* out_f32,
-              const Planes& out_pl, int P, int Tp, cudaStream_t st, const int* valid_frames = nullptr);
+              const Planes& out_pl, int P, int Tp, cudaStream_t st, const int* valid_frames = nullptr, const int* num_samples = nullptr);
 
 // ---- audio_prep.cu ----------------------------------------------------------------------------------
 size_t audio_prep_workspace_bytes(int B, int max_new_len);

@@ -14,12 +14,19 @@
 //     per frame plus a bank-conflicting bit-reversed round trip made it shuffle / LSU-issue bound at 4.6 % of the HBM roofline.)
 //   * log-mel rows of the item are staged in shared memory and leave as 16-byte coalesced stores, together with the item's
 //     column sums, so the separate mean pass over [B,T,F] is gone: fbank_finalize reads the partial sums.
+//
+// fbank_frame_kernel (every other configuration: FFT sizes 128..4096, snip_edges off, no DC removal, magnitude or linear output).
+//   One CTA per work item of 16 frames, the same items and the same output contract (raw rows + per-item column sums) as
+//   fbank_logmel_kernel, so fbank_finalize and the models' fused waveform path are shared.  The frames of an item go through the
+//   radix-2 shared-memory FFT of fft_radix2.cuh 4096 / n_fft at a time (one frame per pass at 4096 points, all 16 at <= 256).
+//   fbank_create chooses the kernel from the config; nothing else selects it.
 #include <math.h>
 
 #include <vector>
 
 #include "common.h"
 #include "fft512.cuh"
+#include "fft_radix2.cuh"
 #include "ptx.cuh"
 
 namespace ppv {
@@ -34,12 +41,15 @@ constexpr int FB_MAX_MELS = 128;
 constexpr int FB_PART_ROWS = 32768;   // handle-owned partial-sum rows ([row][FB_MAX_MELS]): utterances x items per launch group
 constexpr int FB_FIN_FRAMES = 32;     // frames per finalize block
 constexpr int FB_TW512 = 144;         // e^{-2 pi i k / 512} is needed for k <= 143 only (bins k and 256 - k share a pair)
+constexpr int FB_MIN_NFFT = 128, FB_MAX_NFFT = 4096;
+constexpr int FG_POINTS = 4096;       // complex points per FFT pass of fbank_frame_kernel
+constexpr int FG_THREADS = 256;
 
 struct FbankTables {
-    float* window = nullptr;    // [512] zero-padded
+    float* window = nullptr;    // [n_fft] zero-padded
     float2* tw = nullptr;       // [16][16]  exp(-2 pi i k1 n2 / 256) at [k1*16 + n2]
     float2* tw512 = nullptr;    // [256]  exp(-2 pi i k / 512)
-    float* mel_w = nullptr;     // [nnz]  (x 0.25: the kernel's spectrum is 2 X)
+    float* mel_w = nullptr;     // [nnz]  (x 0.25 for fbank_logmel_kernel: its spectrum is 2 X)
     int* mel_start = nullptr;   // [n_mels] first FFT bin
     int* mel_len = nullptr;     // [n_mels]
     int* mel_off = nullptr;     // [n_mels] offset into mel_w
@@ -48,8 +58,10 @@ struct FbankTables {
 
 struct Fbank {
     ppv_fbank_cfg cfg;
-    int win = 0, shift = 0;
+    int win = 0, shift = 0, nfft = 0, log2n = 0;
+    bool general = false;         // fbank_frame_kernel; otherwise fbank_logmel_kernel
     FbankTables tb;
+    float2* twiddle = nullptr;    // [n_fft / 2] exp(-2 pi i k / n_fft), fbank_frame_kernel only
     float* part = nullptr;   // [FB_PART_ROWS, FB_MAX_MELS] per-item column sums
     float* part2 = nullptr;  // [FB_PART_ROWS / 64, FB_MAX_MELS] per-utterance sums (long utterances)
 };
@@ -295,6 +307,114 @@ __global__ void __launch_bounds__(FB_THREADS, 3)
     }
 }
 
+// Where frame 0 starts in the waveform.  snip_edges: at sample 0.  Otherwise torchaudio's _get_strided frames the waveform with
+// min(pad, L) of its first samples prepended in reverse (pad = win / 2 - shift / 2 > 0; the edge sample repeats, unlike numpy's
+// 'reflect') or with its first min(-pad, L) samples dropped (pad <= 0), and the whole reversed waveform appended on the right.
+// Sample n of frame t is then index g = t * shift + n + origin of the waveform, mirrored as -1 - g below 0 and 2L - 1 - g from L on.
+__host__ __device__ inline int fbank_frame_origin(int L, int win, int shift, int snip_edges) {
+    if (snip_edges) return 0;
+    const int pad = win / 2 - shift / 2;
+    return pad > 0 ? -min(pad, L) : min(-pad, L);
+}
+
+struct FbankFrameArgs {
+    const float* window;    // [n_fft], zero beyond win
+    const float2* twiddle;  // [n_fft / 2]
+    const float* mel_w;
+    const int* mel_start;
+    const int* mel_len;
+    const int* mel_off;
+    int win, shift, log2n, n_mels, snip_edges, remove_dc, use_power, use_log;
+    float preemph, log_floor;
+};
+
+__host__ __device__ inline int fbank_frame_smem_bytes(int n_mels) {
+    return FG_POINTS * 8 + (FG_POINTS / 2) * 4 + FB_ITEM * n_mels * 4 + FB_ITEM * 4;
+}
+
+// The general Kaldi frame: framing (either snip_edges) -> DC removal (optional) -> pre-emphasis -> window -> zero-pad to n_fft ->
+// radix-2 FFT -> power or magnitude -> sparse mel -> log (optional).  Same output contract as fbank_logmel_kernel: raw rows
+// out_raw [B, T, n_mels] and per-item column sums part[(b * nitem + item) * FB_MAX_MELS + m].  num_samples (optional): utterance b's
+// own length, where its right edge is reflected (ragged batches); frames past an utterance's own count are computed from clamped
+// indices and only ever read as padding.
+__global__ void __launch_bounds__(FG_THREADS, 2)
+    fbank_frame_kernel(const float* __restrict__ wav, int L, int T, FbankFrameArgs a, const int* __restrict__ num_samples,
+                       float* __restrict__ out_raw, float* __restrict__ part, const int* __restrict__ valid_frames) {
+    extern __shared__ __align__(16) uint8_t fg_smem[];
+    float2* z = reinterpret_cast<float2*>(fg_smem);       // [FG_POINTS] the transforms of one pass, back to back
+    float* pw = reinterpret_cast<float*>(z + FG_POINTS);  // [FG_POINTS / 2] their spectra, bins 0 .. n_fft / 2 - 1
+    float* s_out = pw + FG_POINTS / 2;                    // [FB_ITEM][n_mels]
+    float* s_mu = s_out + FB_ITEM * a.n_mels;             // [FB_ITEM] frame means of the pass
+    griddep_launch_dependents();
+    griddep_wait();
+    const int N = 1 << a.log2n, half = N >> 1;
+    const int nitem = (T + FB_ITEM - 1) / FB_ITEM;
+    const int it = blockIdx.x, b = it / nitem, f0 = (it - b * nitem) * FB_ITEM, nf = min(FB_ITEM, T - f0);
+    const int Lb = num_samples ? min(max(num_samples[b], 1), L) : L;
+    const int origin = fbank_frame_origin(Lb, a.win, a.shift, a.snip_edges);
+    const float* x = wav + int64_t(b) * L;
+    const int shift = a.shift;
+    auto sample = [=](int t, int n) {
+        int g = t * shift + n + origin;
+        if (g < 0) g = -1 - g;
+        if (g >= Lb) g = 2 * Lb - 1 - g;
+        return __ldg(x + min(max(g, 0), Lb - 1));
+    };
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int fpp = min(FB_ITEM, FG_POINTS >> a.log2n);  // frames per pass
+    for (int p0 = 0; p0 < nf; p0 += fpp) {
+        const int np = min(fpp, nf - p0);
+        for (int fr = warp; fr < np; fr += FG_THREADS / 32) {
+            float s = 0.f;
+            if (a.remove_dc)
+                for (int n = lane; n < a.win; n += 32) s += sample(f0 + p0 + fr, n);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == 0) s_mu[fr] = s / float(a.win);
+        }
+        __syncthreads();
+        // ((x_n - mu) - p (x_{n-1} - mu)) w_n with x_{-1} := x_0, zero from win on; stored bit-reversed for the FFT
+        for (int i = threadIdx.x; i < np * N; i += FG_THREADS) {
+            const int fr = i >> a.log2n, n = i & (N - 1);
+            float y = 0.f;
+            if (n < a.win) {
+                const int t = f0 + p0 + fr;
+                const float mu = s_mu[fr];
+                const float cur = sample(t, n) - mu, prev = sample(t, n > 0 ? n - 1 : 0) - mu;
+                y = fmaf(-a.preemph, prev, cur) * __ldg(a.window + n);
+            }
+            z[(fr << a.log2n) + fft_bitrev(n, a.log2n)] = make_float2(y, 0.f);
+        }
+        __syncthreads();
+        fft_radix2(z, a.log2n, np, a.twiddle);
+        for (int i = threadIdx.x; i < np * half; i += FG_THREADS) {
+            const float2 c = z[((i >> (a.log2n - 1)) << a.log2n) + (i & (half - 1))];
+            const float p = fmaf(c.x, c.x, c.y * c.y);
+            pw[i] = a.use_power ? p : sqrtf(p);
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < np * a.n_mels; i += FG_THREADS) {
+            const int fr = i / a.n_mels, m = i - fr * a.n_mels;
+            const float* w = a.mel_w + __ldg(a.mel_off + m);
+            const float* p = pw + fr * half + __ldg(a.mel_start + m);
+            const int len = __ldg(a.mel_len + m);
+            float e = 0.f;
+            for (int j = 0; j < len; ++j) e = fmaf(__ldg(w + j), p[j], e);
+            s_out[(p0 + fr) * a.n_mels + m] = a.use_log ? logf(fmaxf(e, a.log_floor)) : e;
+        }
+        __syncthreads();
+    }
+    float* dst = out_raw + (int64_t(b) * T + f0) * a.n_mels;
+    for (int i = threadIdx.x; i < nf * a.n_mels; i += FG_THREADS) dst[i] = s_out[i];
+    if (int(threadIdx.x) < a.n_mels) {
+        // ragged batches: frames beyond the utterance's own count are padding and stay out of its time mean
+        const int nsum = valid_frames ? max(0, min(nf, valid_frames[b] - f0)) : nf;
+        float sum = 0.f;
+        for (int f = 0; f < nsum; ++f) sum += s_out[f * a.n_mels + threadIdx.x];
+        part[int64_t(it) * FB_MAX_MELS + threadIdx.x] = sum;
+    }
+}
+
 // long utterances: fold the per-item sums of each utterance into one row (nitem -> 1)
 __global__ void __launch_bounds__(128) fbank_part_reduce_kernel(const float* __restrict__ part, int nitem, float* __restrict__ out) {
     griddep_launch_dependents();
@@ -368,33 +488,55 @@ static int upload(T** dst, const std::vector<T>& v) {
     return PPV_OK;
 }
 
+// torchaudio kaldi.py:_feature_window_function, in double, rounded once
+static float fbank_window_value(int type, int i, int win, double blackman_coeff) {
+    const double c = cos(2.0 * M_PI * i / (win - 1));
+    switch (type) {
+        case PPV_FBANK_WIN_HANNING: return float(0.5 - 0.5 * c);
+        case PPV_FBANK_WIN_HAMMING: return float(0.54 - 0.46 * c);
+        case PPV_FBANK_WIN_RECTANGULAR: return 1.f;
+        case PPV_FBANK_WIN_BLACKMAN: {
+            const double a = 2.0 * M_PI / (win - 1);
+            return float(blackman_coeff - 0.5 * cos(a * i) + (0.5 - blackman_coeff) * cos(2.0 * a * i));
+        }
+        default: {  // povey: hann(periodic=False)^0.85
+            const double hann = 0.5 - 0.5 * cos(2.0 * M_PI * i / (win - 1));
+            return float(pow(hann, 0.85));
+        }
+    }
+}
+
 int fbank_create(const ppv_fbank_cfg* cfg, Fbank** out) {
     PPV_REQUIRE(cfg && out, "fbank_create: null argument");
     Fbank* h = new Fbank();
     h->cfg = *cfg;
     h->win = int(cfg->sample_rate * cfg->frame_length_ms * 0.001f);
     h->shift = int(cfg->sample_rate * cfg->frame_shift_ms * 0.001f);
-    if (next_pow2(h->win) != FB_NFFT || h->shift <= 0 || h->win < 2) {
+    if (cfg->sample_rate <= 0 || h->shift <= 0 || h->win < 2) {
         delete h;
-        return fail(PPV_EUNSUPPORTED, "fbank: only window sizes that pad to a 512-point FFT are implemented (16 kHz, 25 ms)");
+        return fail(PPV_EINVAL, "fbank: sample_rate, frame_length_ms and frame_shift_ms must give a window of >= 2 samples and a shift of >= 1");
     }
+    h->nfft = next_pow2(h->win);  // round_to_power_of_two
+    if (h->nfft < FB_MIN_NFFT || h->nfft > FB_MAX_NFFT) {
+        const int nfft = h->nfft, win = h->win;
+        delete h;
+        return fail(PPV_EUNSUPPORTED, "fbank: a " + std::to_string(win) + "-sample window pads to a " + std::to_string(nfft) +
+                                          "-point FFT; the FFT size must be a power of two in [128, 4096]");
+    }
+    while ((1 << h->log2n) < h->nfft) ++h->log2n;
     if (cfg->n_mels < 4 || cfg->n_mels > FB_MAX_MELS) {
         delete h;
         return fail(PPV_EUNSUPPORTED, "fbank: n_mels must be in [4,128]");
     }
-    const int win = h->win;
-    // povey window: hann(periodic=False)^0.85
-    std::vector<float> window(FB_NFFT, 0.f);  // zero beyond win: the kernel multiplies all 512 slots
-    for (int i = 0; i < win; ++i) {
-        const double hann = 0.5 - 0.5 * cos(2.0 * M_PI * i / (win - 1));
-        window[i] = float(pow(hann, 0.85));
+    if (cfg->window_type < PPV_FBANK_WIN_POVEY || cfg->window_type > PPV_FBANK_WIN_BLACKMAN) {
+        delete h;
+        return fail(PPV_EINVAL, "fbank: unknown window_type");
     }
-    std::vector<float2> tw(256), tw512(256);
-    for (int k1 = 0; k1 < 16; ++k1)
-        for (int n2 = 0; n2 < 16; ++n2)
-            tw[k1 * 16 + n2] = fft_twiddle(k1 * n2, 256);
-    for (int k = 0; k < 256; ++k) tw512[k] = fft_twiddle(k, 512);
-    // mel banks, evaluated in float32 like torchaudio kaldi.py:get_mel_banks (vtln_warp == 1)
+    h->general = !(h->nfft == FB_NFFT && cfg->snip_edges && cfg->remove_dc_offset && cfg->use_power && cfg->use_log_fbank);
+    const int win = h->win, nfft = h->nfft, half = nfft / 2;
+    std::vector<float> window(nfft, 0.f);  // zero beyond win: the kernels multiply all n_fft slots
+    for (int i = 0; i < win; ++i) window[i] = fbank_window_value(cfg->window_type, i, win, double(cfg->blackman_coeff));
+    // mel banks, evaluated in float32 like torchaudio kaldi.py:get_mel_banks
     const int nb = cfg->n_mels;
     const float sr = float(cfg->sample_rate);
     const float nyq = 0.5f * sr;
@@ -405,42 +547,84 @@ int fbank_create(const ppv_fbank_cfg* cfg, Fbank** out) {
         delete h;
         return fail(PPV_EINVAL, "fbank: bad low_freq / high_freq");
     }
+    const bool warp = cfg->vtln_warp != 1.f;
+    float vtln_high = cfg->vtln_high;
+    if (vtln_high < 0.f) vtln_high += nyq;
+    // the piecewise-linear VTLN warp of kaldi.py:vtln_warp_freq, inflection points l and h, slopes in double, applied in float32
+    const double wf = cfg->vtln_warp;
+    const double vl = double(cfg->vtln_low) * std::max(1.0, wf), vh = double(vtln_high) * std::min(1.0, wf);
+    if (warp && !(wf > 0.0 && low < cfg->vtln_low && cfg->vtln_low < high && 0.f < vtln_high && vtln_high < high &&
+                  cfg->vtln_low < vtln_high && vl > low && vh < high)) {
+        delete h;
+        return fail(PPV_EINVAL, "fbank: bad vtln_warp / vtln_low / vtln_high (need low_freq < vtln_low < vtln_high < high_freq)");
+    }
+    const double sd = 1.0 / wf;
+    const float scale = float(sd), scale_left = float((sd * vl - low) / (vl - low)), scale_right = float((high - sd * vh) / (high - vh));
+    auto warp_mel = [&](float mel) {
+        const float f = 700.0f * (expf(mel / 1127.0f) - 1.0f);
+        float r;
+        if (f < low || f > high) r = f;
+        else if (f < float(vl)) r = low + scale_left * (f - low);
+        else if (f < float(vh)) r = scale * f;
+        else r = high + scale_right * (f - high);
+        return 1127.0f * logf(1.0f + r / 700.0f);
+    };
     const double mel_low = 1127.0 * log(1.0 + double(low) / 700.0);
     const double mel_high = 1127.0 * log(1.0 + double(high) / 700.0);
     const double delta = (mel_high - mel_low) / (nb + 1);
-    const float bin_width = sr / float(FB_NFFT);
+    const float bin_width = sr / float(nfft);
+    // fbank_logmel_kernel's power spectrum is |2X|^2, so its weights carry the 1/4; the general kernel's spectrum is X itself
+    const float mel_scale = h->general ? 1.f : 0.25f;
     std::vector<float> melw;
     std::vector<int> mstart(nb), mlen(nb), moff(nb);
     for (int m = 0; m < nb; ++m) {
-        const float left = float(mel_low) + float(m) * float(delta);
-        const float center = float(mel_low) + (float(m) + 1.0f) * float(delta);
-        const float right = float(mel_low) + (float(m) + 2.0f) * float(delta);
+        float left = float(mel_low) + float(m) * float(delta);
+        float center = float(mel_low) + (float(m) + 1.0f) * float(delta);
+        float right = float(mel_low) + (float(m) + 2.0f) * float(delta);
+        if (warp) {
+            left = warp_mel(left);
+            center = warp_mel(center);
+            right = warp_mel(right);
+        }
         int first = -1, last = -1;
-        std::vector<float> row(FB_HALF, 0.f);
-        for (int k = 0; k < FB_HALF; ++k) {
+        std::vector<float> row(half, 0.f);
+        for (int k = 0; k < half; ++k) {
             const float mel = 1127.0f * logf(1.0f + (bin_width * float(k)) / 700.0f);
             const float up = (mel - left) / (center - left);
             const float down = (right - mel) / (right - center);
-            const float w = fmaxf(0.f, fminf(up, down));
+            // warped edges may come in any order: only the rising and falling flanks count (get_mel_banks, vtln_warp != 1)
+            const float w = !warp ? fmaxf(0.f, fminf(up, down)) : (mel > left && mel <= center) ? up : (mel > center && mel < right) ? down : 0.f;
             row[k] = w;
-            if (w > 0.f) {
+            if (w != 0.f) {
                 if (first < 0) first = k;
                 last = k;
             }
         }
         mstart[m] = first < 0 ? 0 : first;
         int len = first < 0 ? 0 : last - first + 1;
-        len = (len + 3) & ~3;  // the kernel's mel loop is unrolled by 4: pad with zero weights over valid power bins
-        if (mstart[m] + len > FB_HALF) mstart[m] = FB_HALF - len;
+        len = (len + 3) & ~3;  // fbank_logmel_kernel's mel loop is unrolled by 4: pad with zero weights over valid power bins
+        if (mstart[m] + len > half) mstart[m] = half - len;
         mlen[m] = len;
         moff[m] = int(melw.size());
-        for (int k = 0; k < len; ++k) melw.push_back(0.25f * row[mstart[m] + k]);  // the kernel's power spectrum is |2X|^2
+        for (int k = 0; k < len; ++k) melw.push_back(mel_scale * row[mstart[m] + k]);
     }
     if (melw.empty()) melw.push_back(0.f);
     h->tb.nnz = int(melw.size());
     int rc = upload(&h->tb.window, window);
-    if (!rc) rc = upload(&h->tb.tw, tw);
-    if (!rc) rc = upload(&h->tb.tw512, tw512);
+    if (!rc && !h->general) {
+        std::vector<float2> tw(256), tw512(256);
+        for (int k1 = 0; k1 < 16; ++k1)
+            for (int n2 = 0; n2 < 16; ++n2)
+                tw[k1 * 16 + n2] = fft_twiddle(k1 * n2, 256);
+        for (int k = 0; k < 256; ++k) tw512[k] = fft_twiddle(k, 512);
+        rc = upload(&h->tb.tw, tw);
+        if (!rc) rc = upload(&h->tb.tw512, tw512);
+    }
+    if (!rc && h->general) {
+        std::vector<float2> tw(half);
+        for (int k = 0; k < half; ++k) tw[k] = fft_twiddle(k, nfft);
+        rc = upload(&h->twiddle, tw);
+    }
     if (!rc) rc = upload(&h->tb.mel_w, melw);
     if (!rc) rc = upload(&h->tb.mel_start, mstart);
     if (!rc) rc = upload(&h->tb.mel_len, mlen);
@@ -449,7 +633,7 @@ int fbank_create(const ppv_fbank_cfg* cfg, Fbank** out) {
                 cudaMalloc(reinterpret_cast<void**>(&h->part2), size_t(FB_PART_ROWS / 64) * FB_MAX_MELS * sizeof(float)) != cudaSuccess))
         rc = fail(PPV_ECUDA, "fbank: cudaMalloc(partial sums) failed");
     if (rc) {
-        delete h;
+        fbank_destroy(h);
         return rc;
     }
     *out = h;
@@ -465,12 +649,20 @@ void fbank_destroy(Fbank* h) {
     cudaFree(h->tb.mel_start);
     cudaFree(h->tb.mel_len);
     cudaFree(h->tb.mel_off);
+    cudaFree(h->twiddle);
     cudaFree(h->part);
     cudaFree(h->part2);
     delete h;
 }
 
 int fbank_num_frames(const Fbank* h, int L) {
+    if (!h->cfg.snip_edges) {
+        if (L <= 0) return 0;
+        const int m = int((int64_t(L) + h->shift / 2) / h->shift);
+        // the last frame must end inside the reflected waveform (2L samples from the origin on), as _get_strided's view must
+        const int64_t end = int64_t(m - 1) * h->shift + h->win + fbank_frame_origin(L, h->win, h->shift, 0);
+        return m > 0 && end <= 2 * int64_t(L) ? m : 0;
+    }
     if (L < h->win) return 0;
     return 1 + (L - h->win) / h->shift;
 }
@@ -478,34 +670,52 @@ int fbank_n_mels(const Fbank* h) { return h->cfg.n_mels; }
 
 // raw: scratch [B,T,F] (may equal out_f32).  Exactly one or both of out_f32 / out_pl.
 int fbank_run(Fbank* h, const float* wav, const float* lens_ratio, int B, int L, float* raw, float* out_f32,
-              const Planes& out_pl, int P, int Tp, cudaStream_t st, const int* valid_frames) {
+              const Planes& out_pl, int P, int Tp, cudaStream_t st, const int* valid_frames, const int* num_samples) {
     PPV_REQUIRE(h && wav && raw, "fbank_run: null argument");
     PPV_REQUIRE(B > 0, "fbank_run: empty batch");
     const int T = fbank_num_frames(h, L);
     PPV_REQUIRE(T > 0, "fbank_run: waveform shorter than one frame");
     const int F = h->cfg.n_mels;
-    const FbankSmem lay = fbank_smem_layout(h->tb.nnz, F, h->win, h->shift);
-    PPV_REQUIRE(lay.total <= 200 * 1024, "fbank_run: shared memory budget exceeded (frame shift too large)");
-    // three CTAs per SM need <= 76 800 B each (228 KB - 1 KB reserved per CTA): 76 784 B for 16 kHz / 25 ms / 10 ms / 80 bins
-    const bool vec = (h->shift % 2) == 0;
-    auto kern = (h->win == 400) ? (vec ? fbank_logmel_kernel<true, 400> : fbank_logmel_kernel<false, 400>)
-                                : (vec ? fbank_logmel_kernel<true, 0> : fbank_logmel_kernel<false, 0>);
-    PPV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));  // per device: cheap, set every call
-    // TMA 1-D bulk copies need 16-byte aligned sources and sizes: every item starts at b * L + 16 k * shift samples
-    const int use_tma = (reinterpret_cast<uintptr_t>(wav) % 16 == 0) && (L % 4 == 0) && ((FB_ITEM * h->shift) % 4 == 0) &&
-                        (h->shift % 4 == 0) && (h->win % 4 == 0);
     const int nitem = (T + FB_ITEM - 1) / FB_ITEM;
     PPV_REQUIRE(nitem <= FB_PART_ROWS, "fbank_run: utterance too long (more than 524288 frames)");
     const int group = std::max(1, std::min(B, FB_PART_ROWS / nitem));  // utterances per launch group (partial-sum rows)
     const int sms = device_sm_count();
+    FbankSmem lay{};
+    void (*kern)(const float*, int, int, int, int, int, int, float, float, FbankTables, int, float*, float*, const int*) = nullptr;
+    int use_tma = 0, smem = 0;
+    FbankFrameArgs fa{};
+    if (h->general) {
+        smem = fbank_frame_smem_bytes(F);
+        PPV_CUDA_OK(cudaFuncSetAttribute(fbank_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        fa = FbankFrameArgs{h->tb.window, h->twiddle, h->tb.mel_w, h->tb.mel_start, h->tb.mel_len, h->tb.mel_off, h->win, h->shift, h->log2n, F,
+                            h->cfg.snip_edges, h->cfg.remove_dc_offset, h->cfg.use_power, h->cfg.use_log_fbank, h->cfg.preemph, h->cfg.log_floor};
+    } else {
+        lay = fbank_smem_layout(h->tb.nnz, F, h->win, h->shift);
+        PPV_REQUIRE(lay.total <= 200 * 1024, "fbank_run: shared memory budget exceeded (frame shift too large)");
+        // three CTAs per SM need <= 76 800 B each (228 KB - 1 KB reserved per CTA): 76 784 B for 16 kHz / 25 ms / 10 ms / 80 bins
+        const bool vec = (h->shift % 2) == 0;
+        kern = (h->win == 400) ? (vec ? fbank_logmel_kernel<true, 400> : fbank_logmel_kernel<false, 400>)
+                               : (vec ? fbank_logmel_kernel<true, 0> : fbank_logmel_kernel<false, 0>);
+        PPV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));  // per device: cheap, set every call
+        // TMA 1-D bulk copies need 16-byte aligned sources and sizes: every item starts at b * L + 16 k * shift samples
+        use_tma = (reinterpret_cast<uintptr_t>(wav) % 16 == 0) && (L % 4 == 0) && ((FB_ITEM * h->shift) % 4 == 0) && (h->shift % 4 == 0) &&
+                  (h->win % 4 == 0);
+    }
     for (int b0 = 0; b0 < B; b0 += group) {
         const int nb = std::min(group, B - b0);
         const float* w = wav + int64_t(b0) * L;
         float* r = raw + int64_t(b0) * T * F;
-        const int grid = std::min(nb * nitem, 3 * sms);
-        PPV_PDL_OK(launch_pdl(kern, dim3(grid), dim3(FB_THREADS), size_t(lay.total), st, w, nb, L, T, h->win, h->shift, F, h->cfg.preemph,
-                              h->cfg.log_floor, h->tb, use_tma, r, h->part, valid_frames ? valid_frames + b0 : (const int*)nullptr),
-                   "fbank_logmel_kernel");
+        const int* vf = valid_frames ? valid_frames + b0 : (const int*)nullptr;
+        if (h->general) {
+            PPV_PDL_OK(launch_pdl(fbank_frame_kernel, dim3(nb * nitem), dim3(FG_THREADS), size_t(smem), st, w, L, T, fa,
+                                  num_samples ? num_samples + b0 : (const int*)nullptr, r, h->part, vf),
+                       "fbank_frame_kernel");
+        } else {
+            const int grid = std::min(nb * nitem, 3 * sms);
+            PPV_PDL_OK(launch_pdl(kern, dim3(grid), dim3(FB_THREADS), size_t(lay.total), st, w, nb, L, T, h->win, h->shift, F, h->cfg.preemph,
+                                  h->cfg.log_floor, h->tb, use_tma, r, h->part, vf),
+                       "fbank_logmel_kernel");
+        }
         const float* sums = h->part;
         int nsum = nitem;
         if (nitem > 64 && nb <= FB_PART_ROWS / 64) {  // long utterances: one row of sums per utterance instead of nitem per finalize block
@@ -519,7 +729,7 @@ int fbank_run(Fbank* h, const float* wav, const float* lens_ratio, int B, int L,
             pl.base += int64_t(b0) * Tp * pl.ld;
         }
         PPV_PDL_OK(launch_pdl(fbank_finalize_kernel, dim3((T + FB_FIN_FRAMES - 1) / FB_FIN_FRAMES, nb), dim3(256), 0, st, (const float*)r, sums,
-                              nsum, lens_ratio ? lens_ratio + b0 : (const float*)nullptr, valid_frames ? valid_frames + b0 : (const int*)nullptr, nb, T, F,
+                              nsum, lens_ratio ? lens_ratio + b0 : (const float*)nullptr, vf, nb, T, F,
                               out_f32 ? out_f32 + int64_t(b0) * T * F : (float*)nullptr, pl, P, Tp),
                    "fbank_finalize_kernel");
     }

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "common.h"
+#include "fft_radix2.cuh"
 #include "ptx.cuh"
 
 namespace ppv {
@@ -64,25 +65,11 @@ __global__ void __launch_bounds__(SP_THREADS) spectral_frame_kernel(const float*
     const int N = a.n_fft;
     const int start = t * a.hop - (a.center ? N / 2 : 0);
     for (int i = threadIdx.x; i < N; i += SP_THREADS) {
-        const int j = int(__brev(unsigned(i)) >> (32 - a.log2n));
         const int src = a.center ? sp_reflect(start + i, L) : start + i;
-        z[j] = make_float2(x[src] * a.window[i], 0.f);
+        z[fft_bitrev(i, a.log2n)] = make_float2(x[src] * a.window[i], 0.f);
     }
     __syncthreads();
-    for (int s = 1; s <= a.log2n; ++s) {
-        const int half = 1 << (s - 1);
-        const int tw_stride = N >> s;
-        for (int bf = threadIdx.x; bf < N / 2; bf += SP_THREADS) {
-            const int pos = bf & (half - 1);
-            const int i0 = ((bf >> (s - 1)) << s) + pos;
-            const float2 w = __ldg(a.twiddle + pos * tw_stride);
-            const float2 u = z[i0], v0 = z[i0 + half];
-            const float2 v = make_float2(v0.x * w.x - v0.y * w.y, v0.x * w.y + v0.y * w.x);
-            z[i0] = make_float2(u.x + v.x, u.y + v.y);
-            z[i0 + half] = make_float2(u.x - v.x, u.y - v.y);
-        }
-        __syncthreads();
-    }
+    fft_radix2(z, a.log2n, 1, a.twiddle);
     float* dst = out_raw + (int64_t(b) * T + t) * F;
     for (int k = threadIdx.x; k < a.n_bins; k += SP_THREADS) {
         const float m2 = z[k].x * z[k].x + z[k].y * z[k].y;

@@ -20,10 +20,15 @@ class PPVError(RuntimeError):
     pass
 
 
+PPV_FBANK_WIN_POVEY, PPV_FBANK_WIN_HANNING, PPV_FBANK_WIN_HAMMING, PPV_FBANK_WIN_RECTANGULAR, PPV_FBANK_WIN_BLACKMAN = 0, 1, 2, 3, 4
+
+
 class FbankCfg(C.Structure):
     _fields_ = [("sample_rate", C.c_int), ("n_mels", C.c_int), ("frame_length_ms", C.c_float),
                 ("frame_shift_ms", C.c_float), ("preemph", C.c_float), ("low_freq", C.c_float),
-                ("high_freq", C.c_float), ("log_floor", C.c_float)]
+                ("high_freq", C.c_float), ("log_floor", C.c_float), ("window_type", C.c_int), ("blackman_coeff", C.c_float),
+                ("remove_dc_offset", C.c_int), ("snip_edges", C.c_int), ("use_power", C.c_int), ("use_log_fbank", C.c_int),
+                ("vtln_warp", C.c_float), ("vtln_low", C.c_float), ("vtln_high", C.c_float)]
 
 
 class EcapaCfg(C.Structure):
@@ -151,6 +156,7 @@ SIGNATURES = {
     "ppv_cosine_matrix": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_cosine_pairlist": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, _P]),
     "ppv_fbank_forward_ragged": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "ppv_fbank_forward_ragged_samples": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
     "ppv_audio_prep_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "ppv_audio_prep": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_audio_prep_reverb_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),

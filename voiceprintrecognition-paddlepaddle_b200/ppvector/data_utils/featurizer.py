@@ -61,20 +61,47 @@ class AudioFeaturizer(torch.nn.Module):
                 raise _lib.PPVError(f'{method} argument {k}={v!r} is not supported by the CUDA kernel')
         return cfg
 
-    @staticmethod
-    def _fbank_cfg(args):
+    # paddleaudio.compliance.kaldi.fbank keyword names (featurizer.py:97: Kaldi.fbank(waveform, **kwargs)); they are torchaudio's
+    # except sr (sample_frequency) and n_mels (num_mel_bins)
+    _FBANK_DIRECT = {'sr': 'sample_rate', 'n_mels': 'n_mels', 'frame_length': 'frame_length_ms', 'frame_shift': 'frame_shift_ms',
+                     'preemphasis_coefficient': 'preemph', 'low_freq': 'low_freq', 'high_freq': 'high_freq',
+                     'blackman_coeff': 'blackman_coeff', 'vtln_warp': 'vtln_warp', 'vtln_low': 'vtln_low', 'vtln_high': 'vtln_high'}
+    _FBANK_FLAGS = ('remove_dc_offset', 'snip_edges', 'use_power', 'use_log_fbank')
+    _FBANK_WINDOWS = {'povey': _lib.PPV_FBANK_WIN_POVEY, 'hanning': _lib.PPV_FBANK_WIN_HANNING, 'hamming': _lib.PPV_FBANK_WIN_HAMMING,
+                      'rectangular': _lib.PPV_FBANK_WIN_RECTANGULAR, 'blackman': _lib.PPV_FBANK_WIN_BLACKMAN}
+    # these only shape the energy column (use_energy) or repeat the time-mean subtraction forward() applies anyway
+    _FBANK_NO_EFFECT = ('htk_compat', 'raw_energy', 'energy_floor', 'subtract_mean')
+
+    @classmethod
+    def _fbank_cfg(cls, args):
         lib = _lib.load()
         cfg = _lib.FbankCfg()
         lib.ppv_fbank_default_cfg(C.byref(cfg))
         cfg.n_mels = 23  # paddleaudio kaldi.fbank default when n_mels is not given (cf. feature_dim, featurizer.py:77)
-        # paddleaudio.compliance.kaldi.fbank keyword names (featurizer.py:97: Kaldi.fbank(waveform, **kwargs))
-        known = {'sr': 'sample_rate', 'n_mels': 'n_mels', 'frame_length': 'frame_length_ms',
-                 'frame_shift': 'frame_shift_ms', 'preemphasis_coefficient': 'preemph', 'low_freq': 'low_freq',
-                 'high_freq': 'high_freq'}
         for k, v in args.items():
-            if k not in known:
+            if k in cls._FBANK_DIRECT:
+                setattr(cfg, cls._FBANK_DIRECT[k], type(getattr(cfg, cls._FBANK_DIRECT[k]))(v))
+            elif k in cls._FBANK_FLAGS:
+                setattr(cfg, k, int(bool(v)))
+            elif k == 'window_type':
+                if v not in cls._FBANK_WINDOWS:
+                    raise _lib.PPVError(f'Fbank: unknown window_type {v!r} (one of {", ".join(cls._FBANK_WINDOWS)})')
+                cfg.window_type = cls._FBANK_WINDOWS[v]
+            elif k in cls._FBANK_NO_EFFECT:
+                pass
+            elif k == 'dither':
+                if v != 0:
+                    raise _lib.PPVError('Fbank: dither != 0 is not supported: its noise comes from Paddle\'s random generator and cannot '
+                                        'be reproduced')
+            elif k == 'use_energy':
+                if v:
+                    raise _lib.PPVError('Fbank: use_energy=True is not supported: kaldi emits n_mels + 1 columns while feature_dim reports '
+                                        'n_mels, so the model\'s first layer would reject the features (the reference fails the same way)')
+            elif k == 'round_to_power_of_two':
+                if not v:
+                    raise _lib.PPVError('Fbank: round_to_power_of_two=False is not supported: the FFT size must be a power of two')
+            else:
                 raise _lib.PPVError(f'Fbank argument {k!r} is not supported by the CUDA kernel')
-            setattr(cfg, known[k], type(getattr(cfg, known[k]))(v))
         return cfg
 
     def _get_handle(self):
@@ -151,10 +178,11 @@ class AudioFeaturizer(torch.nn.Module):
         lib, h = _lib.load(), self._get_handle()
         T = lib.ppv_fbank_num_frames(h, L)
         vf = torch.tensor(frames, dtype=torch.int32, device=wav.device)
+        ns = torch.tensor([int(n) for n in lengths], dtype=torch.int32, device=wav.device)  # where snip_edges=False reflects each end
         out = torch.empty((B, T, self._cfg.n_mels), dtype=torch.float32, device=wav.device)
         with torch.cuda.device(wav.device):
-            _lib.check(lib.ppv_fbank_forward_ragged(h, _lib.ptr(wav), _lib.ptr(vf), B, L, _lib.ptr(out), _lib.current_stream()),
-                       'ppv_fbank_forward_ragged')
+            _lib.check(lib.ppv_fbank_forward_ragged_samples(h, _lib.ptr(wav), _lib.ptr(vf), _lib.ptr(ns), B, L, _lib.ptr(out),
+                                                            _lib.current_stream()), 'ppv_fbank_forward_ragged_samples')
         return out[:, :max(frames)], frames
 
     @property
