@@ -518,6 +518,30 @@ size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, i
 int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
                     int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
                     size_t ws_bytes, void* stream);
+/* Test hook (not a reference entry point): the same conv with the ReLU clipped at relu_max > 0 (ERes2Net's Hardtanh(0, 20)), as the
+ * ERes2Net plans ask the kernels for it.  Same workspace as ppv_conv2d_test. */
+int ppv_conv2d_test_clipped(const float* x, const float* w, const float* bias, float relu_max, int B, int H, int W, int Cin, int Cout,
+                            int k, int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
+                            size_t ws_bytes, void* stream);
+
+/* Test hooks for the 2-D models' stem conv and two elementwise kernels (not reference entry points).
+ * stem: feat [B,T,F] fp32, w [C0][9] and bias [C0] fp32 with the BN folded in -> out: split-bf16 planes [2][B][F+2][T+2][C0] (the image
+ * is the features transposed: frequency rows, frame columns), 16-byte aligned; zeroed, then the kernel writes the interior (3x3 conv,
+ * padding 1, ReLU).  C0 a multiple of 8 up to 2048.
+ * scale_res: out[r, oc0 + c] = z[r, c] * scale[r / rows_per_group, c] + res[r, rc0 + c] for the rows r < rows, then ReLU if relu, clipped
+ * at relu_max when relu_max > 0.  z [rows, C], res [rows, res_ld] fp32, split into planes here; scale [rows / rows_per_group, C] fp32
+ * (may be NULL: no scale).  out: split-bf16 planes [2][rows][out_ld], 16-byte aligned, not cleared: only columns [oc0, oc0 + C) are
+ * written.  C, rc0, oc0, res_ld, out_ld multiples of 8; ws >= ppv_scale_res_test_workspace_bytes.
+ * aff_combine: out[r, c] = x[r, xc0 + c] (1 + t[r, c]) + y[r, yc0 + c] (1 - t[r, c]).  x [rows, x_ld], y [rows, y_ld], t [rows, C] fp32,
+ * split into planes here.  out: split-bf16 planes [2][rows][C], 16-byte aligned.  C, xc0, yc0, x_ld, y_ld multiples of 8;
+ * ws >= ppv_aff_combine_test_workspace_bytes. */
+int ppv_stem_conv_test(const float* feat, const float* w, const float* bias, int B, int T, int F, int C0, void* out, void* stream);
+size_t ppv_scale_res_test_workspace_bytes(int rows, int C, int res_ld);
+int ppv_scale_res_test(const float* z, const float* scale, const float* res, int res_ld, int rc0, int C, int rows_per_group, int rows,
+                       int relu, float relu_max, void* out, int out_ld, int oc0, void* ws, size_t ws_bytes, void* stream);
+size_t ppv_aff_combine_test_workspace_bytes(int rows, int C, int x_ld, int y_ld);
+int ppv_aff_combine_test(const float* x, int x_ld, int xc0, const float* y, int y_ld, int yc0, const float* t, int C, int rows, void* out,
+                         void* ws, size_t ws_bytes, void* stream);
 
 /* Test hooks for Res2Net's CUDA-core kernels (not reference entry points).
  * stem: feat [B,T,F] fp32, w [32][49] and bias [32] fp32 with the BN folded in -> out: split-bf16 planes [2][B][Hq+2][Wq+2][32],

@@ -176,5 +176,25 @@ def make_eres2net_weights(seed=1000, dtype=torch.float32, **shape_args) -> Dict[
     return W
 
 
+def is_backbone_bn_gain(name: str) -> bool:
+    """the gain of a BatchNorm that feeds a Hardtanh(0, 20): the stem's `bn1`, and each block's `bn1`, `bns.N` and `bn3`"""
+    parts = name.split(".")
+    return parts[-1] == "weight" and len(parts) >= 2 and (parts[-2].startswith("bn") or (len(parts) >= 3 and parts[-3] == "bns"))
+
+
+def push_into_clip(W: Dict[str, torch.Tensor], gain: float, shift: float) -> Dict[str, torch.Tensor]:
+    """W with every backbone BatchNorm gain multiplied by `gain` and `shift` added to its bias.  The random weights of
+    make_eres2net_weights keep every activation far below 20, so Hardtanh(0, 20) never clips; raising the BatchNorm outputs moves a
+    share of each Hardtanh's inputs above 20."""
+    out = {}
+    for k, v in W.items():
+        if is_backbone_bn_gain(k):
+            v = v * gain
+        elif k.endswith(".bias") and is_backbone_bn_gain(k[:-len("bias")] + "weight"):
+            v = v + shift
+        out[k] = v
+    return out
+
+
 def count_params(W) -> int:
     return sum(v.numel() for k, v in W.items() if not (k.endswith("_mean") or k.endswith("_variance")))

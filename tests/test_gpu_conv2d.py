@@ -1,5 +1,5 @@
 """GPU: the conv2d kernels of ResNetSE, ERes2Net / ERes2NetV2 and CAM++, each on its own through the C ABI test hook
-(ppv_conv2d_test), against torch's conv2d in fp64.
+(ppv_conv2d_test; ppv_conv2d_test_clipped for ERes2Net's clipped ReLU), against torch's conv2d in fp64.
 
   path 0  the 3x3 patch kernel (conv3x3.cu): 32 -> 32 channels, 6 x 62 outputs per patch, one patch per work item;
   path 1  the pointwise kernel (pointwise.cu): 1x1, 32 input channels, 32 or 64 outputs, one thread per grid position;
@@ -38,8 +38,8 @@ def sm_count():
     return _lib.load().ppv_device_sm_count()
 
 
-def run_conv(x, w, bias, relu, stride, path, prec, x_col0=0, x_ld=0):
-    """-> the whole output grid as int16 bit patterns [2, B, Ho+2, Wo+2, Cout] (hi, lo planes)"""
+def run_conv(x, w, bias, relu, stride, path, prec, x_col0=0, x_ld=0, relu_max=0.0):
+    """-> the whole output grid as int16 bit patterns [2, B, Ho+2, Wo+2, Cout] (hi, lo planes); relu_max > 0 clips the ReLU there"""
     lib = _lib.load()
     B, H, W, Cin = x.shape
     Cout, _, k, _ = w.shape
@@ -49,8 +49,13 @@ def run_conv(x, w, bias, relu, stride, path, prec, x_col0=0, x_ld=0):
     buf = torch.full((2 * plane + GUARD,), -1, dtype=torch.int16, device=x.device)
     nbytes = lib.ppv_conv2d_test_workspace_bytes(B, H, W, Cin, Cout, k, x_ld)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-    _lib.check(lib.ppv_conv2d_test(_lib.ptr(x), _lib.ptr(w), _lib.ptr(bias), relu, B, H, W, Cin, Cout, k, sh, sw, x_col0, x_ld, path,
-                                   prec, _lib.ptr(buf), C.c_void_p(ws.data_ptr()), nbytes, _lib.current_stream()), "ppv_conv2d_test")
+    if relu_max > 0:  # the clipped ReLU implies the ReLU
+        _lib.check(lib.ppv_conv2d_test_clipped(_lib.ptr(x), _lib.ptr(w), _lib.ptr(bias), relu_max, B, H, W, Cin, Cout, k, sh, sw, x_col0,
+                                               x_ld, path, prec, _lib.ptr(buf), C.c_void_p(ws.data_ptr()), nbytes, _lib.current_stream()),
+                   "ppv_conv2d_test_clipped")
+    else:
+        _lib.check(lib.ppv_conv2d_test(_lib.ptr(x), _lib.ptr(w), _lib.ptr(bias), relu, B, H, W, Cin, Cout, k, sh, sw, x_col0, x_ld, path,
+                                       prec, _lib.ptr(buf), C.c_void_p(ws.data_ptr()), nbytes, _lib.current_stream()), "ppv_conv2d_test")
     torch.cuda.synchronize()
     assert (buf[2 * plane:] == -1).all(), "stored past the output grid"
     return buf[:2 * plane].view(2, B, Ho + 2, Wo + 2, Cout)
@@ -82,9 +87,10 @@ def make(cuda, B, H, W, Cin, Cout, k, seed, bias=True):
     return x, w, b
 
 
-def check(path, prec, got, ref, what):
+def check(path, prec, got, ref, what, scale_of=None):
+    """scale_of: the tensor whose magnitude sets the bound (default ref; a clipped conv's errors scale with its unclipped outputs)"""
     assert torch.isfinite(got).all(), what
-    scale = max(ref.abs().max().item(), 1.0)
+    scale = max((ref if scale_of is None else scale_of).abs().max().item(), 1.0)
     err = (got - ref).abs().max().item() / scale
     WORST[(path, prec)] = max(WORST.get((path, prec), 0.0), err)
     assert err < TOL, (what, err)
@@ -190,6 +196,31 @@ def test_patch_kernel_agrees_with_gather_gemm(cuda, B, H, W, stride, prec):
     assert err < TOL, err
 
 
+# ------------------------------------------------------------------------------------------------ clipped ReLU
+CLIP = 20.0  # ERes2Net's Hardtanh(0, 20)
+BF16_20 = 0x41A0  # 20.0 in bf16: exact, so a clipped output reads back as hi = 20, lo = 0
+
+
+@pytest.mark.parametrize("stride", [(1, 1), (2, 2)])
+@pytest.mark.parametrize("path, Cin, Cout, k", [(PATCH, 32, 32, 3), (POINTWISE, 32, 32, 1), (POINTWISE, 32, 64, 1), (GEMM, 64, 64, 3),
+                                                (GEMM, 64, 128, 1)])
+def test_clipped_relu(cuda, path, Cin, Cout, k, stride):
+    """relu_max = 20 on each kernel: the inputs are scaled by 25, so the pre-activations are ~N(0, 25^2) and about a fifth of the
+    outputs clip.  Each clipped output must be exactly 20.0 (hi = 20, lo = 0); the others as the unclipped conv, at the file's bound
+    relative to the largest unclipped pre-activation (~100): the clip bounds the outputs, not the sums the kernel accumulates."""
+    B, H, W = 2, 13, 63
+    x, w, b = make(cuda, B, H, W, Cin, Cout, k, seed=Cin + Cout + k + stride[0])
+    x = 25 * x
+    for prec in (X3, B16):
+        pre = ref_conv(x, w, b, False, stride, bf16_operands=(prec == B16 and path != POINTWISE))
+        assert (pre > CLIP).double().mean() >= 0.1 and ((pre > 0) & (pre < CLIP)).double().mean() >= 0.1
+        bits = run_conv(x, w, b, 1, stride, path, prec, relu_max=CLIP)
+        check(path, prec, interior(bits), pre.clamp(0, CLIP), ("clip", path, prec, Cin, Cout, k, stride), scale_of=pre)
+        clipped = pre > CLIP * (1 + TOL)
+        hi, lo = bits[0, :, 1:-1, 1:-1], bits[1, :, 1:-1, 1:-1]
+        assert (hi[clipped] == BF16_20).all() and (lo[clipped] == 0).all(), "a clipped output is not exactly 20.0"
+
+
 # ------------------------------------------------------------------------------------------------ refusals
 @pytest.mark.parametrize("path, Cin, Cout, k", [(PATCH, 64, 64, 3), (PATCH, 32, 64, 3), (PATCH, 32, 32, 1), (POINTWISE, 32, 32, 3),
                                                 (POINTWISE, 64, 32, 1), (POINTWISE, 32, 128, 1)])
@@ -198,6 +229,20 @@ def test_unsupported_conv_is_an_error(cuda, path, Cin, Cout, k):
     x, w, b = make(cuda, 1, 6, 62, Cin, Cout, k, seed=1)
     with pytest.raises(_lib.PPVError):
         run_conv(x, w, b, 1, (1, 1), path, X3)
+
+
+@pytest.mark.parametrize("relu_max", [0.0, -20.0])
+def test_clipped_hook_needs_a_positive_clip(cuda, relu_max):
+    x, w, b = make(cuda, 1, 6, 62, 32, 32, 3, seed=1)
+    lib = _lib.load()
+    nbytes = lib.ppv_conv2d_test_workspace_bytes(1, 6, 62, 32, 32, 3, 0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    buf = torch.full((2 * 8 * 64 * 32,), -1, dtype=torch.int16, device=x.device)
+    rc = lib.ppv_conv2d_test_clipped(_lib.ptr(x), _lib.ptr(w), _lib.ptr(b), relu_max, 1, 6, 62, 32, 32, 3, 1, 1, 0, 0, PATCH, X3,
+                                     _lib.ptr(buf), C.c_void_p(ws.data_ptr()), nbytes, _lib.current_stream())
+    torch.cuda.synchronize()
+    assert rc != 0 and "relu_max" in _lib.last_error()
+    assert (buf == -1).all()
 
 
 def test_pointwise_switch_is_an_error(cuda, monkeypatch):

@@ -70,3 +70,67 @@ def test_batch_independence(cuda, model):
     assert torch.isfinite(emb).all()
     for b in (0, 7):
         assert torch.equal(model(f[b:b + 1]), emb[b:b + 1])
+
+
+# ------------------------------------------------------------------------------------------------ m_channels = 64
+# The 64-channel ERes2Net takes other paths than the default 32: a 64-channel stem, stage 1's 1x1 convs on the gather-GEMM (the pointwise
+# kernel takes 32 input channels only), AFF blocks over 32 / 64 intermediate channels, bottom-up fusions over 256 / 512 / 1024 channels
+# and a 10240-wide flatten and TSTP.  Bounds as in test_gpu_conv_models.py: 1 - cos 1e-8 (bf16x3) or 2e-5 (bf16); stage taps 5e-5
+# relative in norm as above (bf16x3), 1e-2 in bf16 (one bf16 MMA per product, as test_gpu_res2net.py).  The embedding's relative error
+# bound is 2e-4, twice that of the 32-channel model.  Measured on an H100 SXM (700 W), bf16x3: taps 1.3e-5 - 1.4e-5, embedding
+# 9.6e-5 - 9.7e-5, against at most 5.0e-5 for the 32-channel models (test_gpu_conv_models.py).  The embedding layer computed in fp64 from the device's statistics lands within 1.2e-5
+# of the oracle; the other 9.0e-5 is the gather-GEMM's fp32 tensor-core accumulation over K = 20480 (10240 at 32 channels).  It is
+# almost all along the embedding itself (1 - cos 6e-10), so scores are unaffected.
+M64_TAP_TOL = {"bf16x3": 5e-5, "bf16": 1e-2}
+M64_COS_TOL = {"bf16x3": 1e-8, "bf16": 2e-5}
+M64_REL_TOL = 2e-4
+
+
+@pytest.fixture(scope="module")
+def W64_m64():
+    return oe.make_eres2net_weights(seed=1000, dtype=torch.float64, m_channels=64)
+
+
+def model_m64(cuda, W, precision):
+    m = ERes2Net(input_size=80, m_channels=64, precision=precision).eval()
+    m.load_state_dict({k: v.float() for k, v in W.items()}, strict=True)
+    return m.to(cuda)
+
+
+@pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
+@pytest.mark.parametrize("T", [64, 149, 298])
+def test_m_channels_64_taps_and_embedding(cuda, W64_m64, T, precision):
+    gi = torch.Generator().manual_seed(5000 + T)
+    f = torch.randn(2, T, 80, generator=gi, dtype=torch.float64)
+    f = f - f.mean(1, keepdim=True)
+    taps = {}
+    ref = oe.eres2net_forward(f, W64_m64, m_channels=64, taps=taps)
+    m = model_m64(cuda, W64_m64, precision)
+    emb = m(f.float().to(cuda))
+    torch.cuda.synchronize()
+    worst = 0.0
+    for name in ["layer1", "layer2", "layer3", "layer4", "fuse12", "fuse123", "fuse1234", "stats"]:
+        got = m.read_tap(name, 2, T).double().cpu()
+        want = taps[name] if name == "stats" else taps[name].permute(0, 2, 3, 1)
+        assert got.shape == want.shape, (name, got.shape, want.shape)
+        rel = ((got - want).norm() / want.norm()).item()
+        worst = max(worst, rel)
+        assert rel < M64_TAP_TOL[precision], (name, rel)
+    emb = emb.double().cpu()
+    assert emb.shape == (2, 192)
+    rel = ((emb - ref).norm(dim=1) / ref.norm(dim=1)).max().item()
+    one_minus_cos = (1 - torch.nn.functional.cosine_similarity(emb, ref)).max().item()
+    print(f"\nERes2Net m_channels=64 {precision} T={T}: taps worst rel {worst:.1e} (bound {M64_TAP_TOL[precision]:.0e}); embedding rel "
+          f"{rel:.1e} (bound {M64_REL_TOL:.0e} in bf16x3), 1 - cos {one_minus_cos:.1e} (bound {M64_COS_TOL[precision]:.0e})")
+    assert one_minus_cos < M64_COS_TOL[precision]
+    if precision == "bf16x3":
+        assert rel < M64_REL_TOL
+
+
+def test_m_channels_64_batch_independence(cuda, W64_m64):
+    m = model_m64(cuda, W64_m64, "bf16x3")
+    f = torch.randn(3, 298, 80, generator=torch.Generator().manual_seed(13)).to(cuda)
+    emb = m(f)
+    assert torch.isfinite(emb).all()
+    for b in range(3):
+        assert torch.equal(m(f[b:b + 1]), emb[b:b + 1])

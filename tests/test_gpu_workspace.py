@@ -320,6 +320,30 @@ def case_skinny_linear_test():
     return lib.ppv_skinny_linear_test_workspace_bytes(M, ld, N, K, out_ld), run
 
 
+def case_scale_res_test():
+    lib = _lib.load()
+    rows, rpg, Cc, res_ld, rc0, out_ld, oc0 = 3 * 45, 45, 64, 96, 32, 80, 16
+    z, res, scale = randn(rows, Cc, seed=46), randn(rows, res_ld, seed=47), randn(3, Cc, seed=48)
+
+    def run(ws, nb):
+        o = out((2, rows, out_ld), torch.int16)
+        return lib.ppv_scale_res_test(_lib.ptr(z), _lib.ptr(scale), _lib.ptr(res), res_ld, rc0, Cc, rpg, rows, 1, 20.0, _lib.ptr(o), out_ld,
+                                      oc0, V(ws), nb, stream()), [o]
+    return lib.ppv_scale_res_test_workspace_bytes(rows, Cc, res_ld), run
+
+
+def case_aff_combine_test():
+    lib = _lib.load()
+    rows, Cc, x_ld, xc0, y_ld, yc0 = 150, 64, 96, 32, 128, 64
+    x, y, t = randn(rows, x_ld, seed=49), randn(rows, y_ld, seed=50), torch.tanh(randn(rows, Cc, seed=51))
+
+    def run(ws, nb):
+        o = out((2, rows, Cc), torch.int16)
+        return lib.ppv_aff_combine_test(_lib.ptr(x), x_ld, xc0, _lib.ptr(y), y_ld, yc0, _lib.ptr(t), Cc, rows, _lib.ptr(o), V(ws), nb,
+                                        stream()), [o]
+    return lib.ppv_aff_combine_test_workspace_bytes(rows, Cc, x_ld, y_ld), run
+
+
 CASES = {
     "aam_forward_backward": case_aam, "cosine_matrix": case_cosine, "eer_mindcf": case_eer, "sym_eig_smallest": case_sym_eig,
     "kmeans": case_kmeans, "vad_energy": case_vad, "audio_prep": case_audio_prep, "audio_prep_reverb": case_audio_prep_reverb,
@@ -329,6 +353,7 @@ CASES = {
     "gemm_test_taps": case_gemm_test_taps, "res2net_test_chain": lambda: case_res2net_test(_lib.PPV_RES2_CHAIN),
     "res2net_test_chain_paired": lambda: case_res2net_test(_lib.PPV_RES2_CHAIN_PAIRED),
     "res2net_test_per_conv": lambda: case_res2net_test(_lib.PPV_RES2_PER_CONV), "skinny_linear_test": case_skinny_linear_test,
+    "scale_res_test": case_scale_res_test, "aff_combine_test": case_aff_combine_test,
 }
 
 

@@ -5,8 +5,8 @@ the old byte formulas counted memory no carve takes:
   - aam, cosine, eer, k-means, sym-eig, gemm_test, conv2d_test: the trailing 256 bytes of slack (no kernel touches memory past
     the last buffer of its call);
   - sym-eig: also one N-double buffer that the carve never took.
-Every other size is unchanged, and every query still returns 0 where it returned 0 (shapes its call rejects).  The Res2Net and skinny
-linear test hooks came later: their entries are the sizes of their carves when they were added."""
+Every other size is unchanged, and every query still returns 0 where it returned 0 (shapes its call rejects).  The Res2Net, skinny
+linear, scale-residual and AFF blend test hooks came later: their entries are the sizes of their carves when they were added."""
 import ctypes as C
 
 import pytest
@@ -55,6 +55,8 @@ QUERY = {
     "campplus_context_test": "ppv_campplus_context_test_workspace_bytes",
     "res2net_test": "ppv_res2net_test_workspace_bytes",
     "skinny_linear_test": "ppv_skinny_linear_test_workspace_bytes",
+    "scale_res_test": "ppv_scale_res_test_workspace_bytes",
+    "aff_combine_test": "ppv_aff_combine_test_workspace_bytes",
 }
 
 
@@ -162,6 +164,9 @@ PARENT = {'aam': {(1, 1, 1): 1792,
                         (256, 512, 128, 512, 128): 917504,
                         (256, 128, 512, 128, 512): 917504,
                         (4096, 1040, 520, 1024, 528): 28311552},
+ 'scale_res_test': {(0, 8, 8): 0, (1, 8, 0): 0, (1, 8, 8): 8192, (135, 64, 96): 163840, (196800, 32, 32): 50397184,
+                    (24600, 512, 512): 101187584},
+ 'aff_combine_test': {(0, 8, 8, 8): 0, (1, 8, 8, 8): 12288, (150, 64, 96, 128): 294912, (100000, 128, 256, 128): 204996608},
  'gemm_test_taps': {None: 0,
                     ((300,), (64,), (64, 64, 64), 100): 273408,
                     ((1000, 999), (128, 80), (128, 64), 512): 1224960,

@@ -627,9 +627,10 @@ size_t ppv_conv2d_test_workspace_bytes(int B, int H, int W, int Cin, int Cout, i
     if (x_ld <= 0) x_ld = Cin;
     return carve_extent([&](WsCarver& cv) { Planes xp, wp; carve_conv2d_test(cv, B, H, W, Cin, Cout, k, x_ld, &xp, &wp); });
 }
-int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
-                    int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws, size_t ws_bytes,
-                    void* stream) {
+// relu_max > 0: ReLU clipped at relu_max (ERes2Net's Hardtanh(0, 20)), the ppv_conv2d_test_clipped entry point
+static int conv2d_test(const float* x, const float* w, const float* bias, int relu, float relu_max, int B, int H, int W, int Cin, int Cout,
+                       int k, int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws, size_t ws_bytes,
+                       void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(x && w && out, "ppv_conv2d_test: null argument");
     if (x_ld <= 0) x_ld = Cin;
@@ -685,6 +686,7 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     Epilogue ep = image_epilogue(outp, gin, gout, stride_h, stride_w);
     ep.bias = bias;
     ep.relu = relu ? 1 : 0;
+    ep.relu_max = relu_max;
     const int sms = device_sm_count();
     if (path == 0) {
         PPV_REQUIRE(k == 3 && conv3x3_c32_supported(Cin, Cout, H, W), "ppv_conv2d_test: the patch kernel takes 3x3 convs with 32 -> 32 channels only");
@@ -712,6 +714,19 @@ int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu,
     return gemm_launch(gp, precision, sms, st);
     PPV_GUARD_END
 }
+int ppv_conv2d_test(const float* x, const float* w, const float* bias, int relu, int B, int H, int W, int Cin, int Cout, int k,
+                    int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws, size_t ws_bytes,
+                    void* stream) {
+    return conv2d_test(x, w, bias, relu, 0.f, B, H, W, Cin, Cout, k, stride_h, stride_w, x_col0, x_ld, path, precision, out, ws, ws_bytes,
+                       stream);
+}
+int ppv_conv2d_test_clipped(const float* x, const float* w, const float* bias, float relu_max, int B, int H, int W, int Cin, int Cout,
+                            int k, int stride_h, int stride_w, int x_col0, int x_ld, int path, int precision, void* out, void* ws,
+                            size_t ws_bytes, void* stream) {
+    if (!(relu_max > 0.f)) return fail(PPV_EINVAL, "ppv_conv2d_test_clipped: relu_max must be > 0");
+    return conv2d_test(x, w, bias, 1, relu_max, B, H, W, Cin, Cout, k, stride_h, stride_w, x_col0, x_ld, path, precision, out, ws, ws_bytes,
+                       stream);
+}
 
 // Res2Net's fused stem + max-pool (res2net.cu) on features given here: w [32][49] and bias [32] with the BN already folded in.
 int ppv_res2net_stem_test(const float* feat, const float* w, const float* bias, int B, int T, int F, void* out, void* stream) {
@@ -728,6 +743,91 @@ int ppv_res2net_stem_test(const float* feat, const float* w, const float* bias, 
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2) * o.plane_stride * sizeof(__nv_bfloat16), st));
     return launch_res2net_stem(feat, B, T, F, w, bias, 32, o, st);
+    PPV_GUARD_END
+}
+
+// ---------------------------------------------------------------- 2-D models' stem and elementwise test hooks
+// The 1 -> C0 stem conv of ResNetSE, ERes2Net and CAM++ (image_plan.cu) on features given here: w [C0][9] and bias [C0] with the BN
+// folded in.
+int ppv_stem_conv_test(const float* feat, const float* w, const float* bias, int B, int T, int F, int C0, void* out, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(feat && w && bias && out && B > 0 && T > 0 && F > 0, "ppv_stem_conv_test: bad argument");
+    if (int rc = check_device()) return rc;
+    Planes o;
+    o.base = static_cast<__nv_bfloat16*>(out);
+    o.ld = C0;
+    o.rows = int64_t(B) * (F + 2) * (T + 2);
+    o.plane_stride = o.rows * o.ld;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    PPV_CUDA_OK(cudaMemsetAsync(out, 0, size_t(2) * o.plane_stride * sizeof(__nv_bfloat16), st));
+    return launch_stem_conv(feat, B, T, F, w, bias, C0, o, F + 2, T + 2, st);
+    PPV_GUARD_END
+}
+
+// The residual add that ends every 2-D block and ECAPA's SE block (launch_se_scale_res).  Workspace: z planes [2][pad128(rows)][C],
+// then res planes [2][pad128(rows)][res_ld].
+static void carve_scale_res_test(WsCarver& cv, int rows, int C, int res_ld, Planes* zp, Planes* rp) {
+    *zp = cv.planes(rows, C);
+    *rp = cv.planes(rows, res_ld);
+}
+size_t ppv_scale_res_test_workspace_bytes(int rows, int C, int res_ld) {
+    if (rows <= 0 || C <= 0 || res_ld <= 0) return 0;
+    return carve_extent([&](WsCarver& cv) { Planes zp, rp; carve_scale_res_test(cv, rows, C, res_ld, &zp, &rp); });
+}
+int ppv_scale_res_test(const float* z, const float* scale, const float* res, int res_ld, int rc0, int C, int rows_per_group, int rows,
+                       int relu, float relu_max, void* out, int out_ld, int oc0, void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(z && res && out, "ppv_scale_res_test: null argument");
+    PPV_REQUIRE(rows > 0 && C > 0 && rows_per_group > 0 && rows % rows_per_group == 0 && rc0 >= 0 && rc0 + C <= res_ld && oc0 >= 0 &&
+                    oc0 + C <= out_ld && res_ld % 8 == 0 && out_ld % 8 == 0 && relu_max >= 0.f,
+                "ppv_scale_res_test: bad shape");
+    if (int rc = check_workspace("ppv_scale_res_test", ws, ws_bytes, ppv_scale_res_test_workspace_bytes(rows, C, res_ld),
+                                 "ppv_scale_res_test_workspace_bytes"))
+        return rc;
+    if (int rc = check_device()) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes zp, rp;
+    carve_scale_res_test(cv, rows, C, res_ld, &zp, &rp);
+    int rc = launch_f32_to_planes(z, rows, C, zp, st);
+    if (rc) return rc;
+    if ((rc = launch_f32_to_planes(res, rows, res_ld, rp, st))) return rc;
+    const Planes op{static_cast<__nv_bfloat16*>(out), rows, out_ld, int64_t(rows) * out_ld};
+    return launch_se_scale_res(zp, scale, rp, rc0, op, oc0, C, rows_per_group, rows, device_sm_count(), st, relu, relu_max);
+    PPV_GUARD_END
+}
+
+// AFF's blend (launch_aff_combine).  Workspace: x planes [2][pad128(rows)][x_ld], y planes [2][pad128(rows)][y_ld], t planes
+// [2][pad128(rows)][C].
+static void carve_aff_combine_test(WsCarver& cv, int rows, int C, int x_ld, int y_ld, Planes* xp, Planes* yp, Planes* tp) {
+    *xp = cv.planes(rows, x_ld);
+    *yp = cv.planes(rows, y_ld);
+    *tp = cv.planes(rows, C);
+}
+size_t ppv_aff_combine_test_workspace_bytes(int rows, int C, int x_ld, int y_ld) {
+    if (rows <= 0 || C <= 0 || x_ld <= 0 || y_ld <= 0) return 0;
+    return carve_extent([&](WsCarver& cv) { Planes xp, yp, tp; carve_aff_combine_test(cv, rows, C, x_ld, y_ld, &xp, &yp, &tp); });
+}
+int ppv_aff_combine_test(const float* x, int x_ld, int xc0, const float* y, int y_ld, int yc0, const float* t, int C, int rows, void* out,
+                         void* ws, size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(x && y && t && out, "ppv_aff_combine_test: null argument");
+    PPV_REQUIRE(rows > 0 && C > 0 && xc0 >= 0 && xc0 + C <= x_ld && yc0 >= 0 && yc0 + C <= y_ld && x_ld % 8 == 0 && y_ld % 8 == 0,
+                "ppv_aff_combine_test: bad shape");
+    if (int rc = check_workspace("ppv_aff_combine_test", ws, ws_bytes, ppv_aff_combine_test_workspace_bytes(rows, C, x_ld, y_ld),
+                                 "ppv_aff_combine_test_workspace_bytes"))
+        return rc;
+    if (int rc = check_device()) return rc;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    Planes xp, yp, tp;
+    carve_aff_combine_test(cv, rows, C, x_ld, y_ld, &xp, &yp, &tp);
+    int rc = launch_f32_to_planes(x, rows, x_ld, xp, st);
+    if (rc) return rc;
+    if ((rc = launch_f32_to_planes(y, rows, y_ld, yp, st))) return rc;
+    if ((rc = launch_f32_to_planes(t, rows, C, tp, st))) return rc;
+    const Planes op{static_cast<__nv_bfloat16*>(out), rows, C, int64_t(rows) * C};
+    return launch_aff_combine(xp, xc0, yp, yc0, tp, op, C, rows, device_sm_count(), st);
     PPV_GUARD_END
 }
 

@@ -142,15 +142,18 @@ inline int check_workspace(const char* call, const void* ws, size_t ws_bytes, si
 // ---- GEMM -----------------------------------------------------------------------------------------
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_MAX_KSTEPS = 192;
+constexpr int GEMM_MAX_KSTEPS = 320;  // K up to 20480: the embedding layer of the 64-channel ERes2Net reads 2 x 10240 TSTP statistics
 constexpr int GEMM_MAX_MAPS = 4;
 constexpr int GEMM_WS_STAGES = 4;  // ring slots in weight-stationary mode (the rest of the ring's shared memory holds W)
 
+// 4 bytes per k-step, so that the k-step table of GemmParams (a kernel parameter copied at every launch) stays small
 struct KStep {
-    int16_t map;      // which A tensor map
-    int16_t row_off;  // row offset (conv tap * dilation)
-    int32_t a_col;    // first column of the 64-wide K slice in that A tensor
+    int16_t row_off;   // row offset (conv tap * dilation)
+    uint16_t map_col;  // bits 14-15: which A tensor map; bits 0-13: first column of the K slice in that A tensor, in units of 8
+    __host__ __device__ int map() const { return map_col >> 14; }
+    __host__ __device__ int a_col() const { return (map_col & 0x3fff) << 3; }
 };
+static_assert(GEMM_MAX_MAPS <= 4, "KStep holds the map index in two bits");
 
 enum OutMode : int { OUT_PLANES = 0, OUT_F32 = 1 };
 

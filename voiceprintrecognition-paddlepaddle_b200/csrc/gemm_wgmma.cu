@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                         if (gp.ws) {
                             const KStep ks = gp.ksteps[s];
 #pragma unroll
-                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[ks.map], fb, ks.a_col, m0 + ks.row_off, p);
+                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, &gp.mapA[ks.map()], fb, ks.a_col(), m0 + ks.row_off, p);
                         } else if (gp.lin_splits > 0) {
                             const int kcol = (zsplit * nk + s) * BK;
 #pragma unroll
@@ -175,9 +175,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                                 tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, kcol + gp.lin_b_col0, gp.lin_b_row0 + n0, p);
                         } else {
                             const KStep ks = gp.ksteps[s];
-                            const CUtensorMap* ma = &gp.mapA[ks.map];
+                            const CUtensorMap* ma = &gp.mapA[ks.map()];
 #pragma unroll
-                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, ma, fb, ks.a_col, m0 + ks.row_off, p);
+                            for (int p = 0; p < Cfg::NA; ++p) tma_load_3d(sa + p * Cfg::A_BYTES, ma, fb, ks.a_col(), m0 + ks.row_off, p);
 #pragma unroll
                             for (int p = 0; p < Cfg::NB; ++p) tma_load_3d(sb + p * Cfg::B_BYTES, &gp.mapB, fb, s * BK, n0, p);
                         }
@@ -381,9 +381,9 @@ int gemm_build(GemmParams* gp, const GemmSource* srcs, int nsrc, const Planes& W
         }
         for (int c = 0; c < s.ncols; c += BK) {
             PPV_REQUIRE(ks < GEMM_MAX_KSTEPS, "gemm_build: too many k-steps");
-            gp->ksteps[ks].map = int16_t(mi);
+            PPV_REQUIRE(s.col0 + c < (1 << 17), "gemm_build: K slice starts past column 131064");
+            gp->ksteps[ks].map_col = uint16_t((mi << 14) | ((s.col0 + c) >> 3));
             gp->ksteps[ks].row_off = int16_t(s.row_off);
-            gp->ksteps[ks].a_col = s.col0 + c;
             ++ks;
         }
     }

@@ -196,6 +196,12 @@ SIGNATURES = {
                                        C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_conv2d_test_workspace_bytes": (C.c_size_t, [C.c_int] * 7),
     "ppv_conv2d_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 13 + [_P, _P, C.c_size_t, _P]),
+    "ppv_conv2d_test_clipped": (C.c_int, [_P, _P, _P, C.c_float] + [C.c_int] * 12 + [_P, _P, C.c_size_t, _P]),
+    "ppv_stem_conv_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 4 + [_P, _P]),
+    "ppv_scale_res_test_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "ppv_scale_res_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 6 + [C.c_float, _P, C.c_int, C.c_int, _P, C.c_size_t, _P]),
+    "ppv_aff_combine_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "ppv_aff_combine_test": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_res2net_stem_test": (C.c_int, [_P, _P, _P] + [C.c_int] * 3 + [_P, _P]),
     "ppv_res2net_avgpool_test_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "ppv_res2net_avgpool_test": (C.c_int, [_P] + [C.c_int] * 7 + [_P, _P, C.c_size_t, _P]),
