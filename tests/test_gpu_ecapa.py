@@ -7,6 +7,7 @@ import torch
 from oracle import ecapa as oe
 from oracle import fbank as ofb
 from oracle import head as oh
+from ppvector._lib import PPVError
 from ppvector.data_utils.featurizer import AudioFeaturizer
 from ppvector.models.ecapa_tdnn import EcapaTdnn
 
@@ -109,6 +110,17 @@ def test_batch_padding_semantics(cuda, model, W64):
     ref = oe.ecapa_forward(feat, W64)
     rel = (emb - ref).norm(dim=1) / ref.norm(dim=1)
     assert rel.max() < 5e-5, rel
+
+
+def test_forward_wav_refuses_training_mode(cuda, model):
+    """forward_wav is the eval-mode forward, as forward is: a model in training mode raises instead of embedding in eval mode"""
+    fz = AudioFeaturizer("Fbank", {"sr": 16000, "n_mels": 80})
+    model.train()
+    try:
+        with pytest.raises(PPVError, match=r"call \.eval\(\)"):
+            model.forward_wav(fz, torch.zeros(1, 16000, device=cuda))
+    finally:
+        model.eval()
 
 
 def test_bf16_fast_mode_is_close_but_flagged(cuda, W64):

@@ -229,6 +229,7 @@ struct CamppModel : PlanModel {
 
     explicit CamppModel(const ppv_campplus_cfg& c) : PlanModel("campplus", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
+    int input_size() const override { return cfg.input_size; }
     size_t workspace_bytes(int B, int T) const override;
 
   protected:

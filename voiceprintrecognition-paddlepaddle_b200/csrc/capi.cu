@@ -54,14 +54,8 @@ struct ppv_trainer {
 };
 
 struct ppv_model {
-    int kind;
     Model* m;
 };
-
-// The model behind an ECAPA-TDNN handle, else null: the entry points that only ECAPA-TDNN has.
-static Model* ecapa_of(const ppv_model* h) { return h && h->kind == PPV_MODEL_ECAPA_TDNN ? h->m : nullptr; }
-// The models with the fused waveform path and the launch profile: ECAPA-TDNN and Res2Net.
-static Model* wav_model_of(const ppv_model* h) { return h && (h->kind == PPV_MODEL_ECAPA_TDNN || h->kind == PPV_MODEL_RES2NET) ? h->m : nullptr; }
 
 #define PPV_GUARD_BEGIN try {
 #define PPV_GUARD_END                                                        \
@@ -211,7 +205,7 @@ int ppv_model_create(int kind, const void* cfg, ppv_model_t** out) {
         default: rc = campplus_create(static_cast<const ppv_campplus_cfg*>(cfg), &m); break;
     }
     if (rc) return rc;
-    *out = new ppv_model{kind, m};
+    *out = new ppv_model{m};
     return PPV_OK;
     PPV_GUARD_END
 }
@@ -243,28 +237,23 @@ size_t ppv_model_workspace_bytes(const ppv_model_t* h, int B, int T) { return h 
 int ppv_model_forward(ppv_model_t* h, const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && feat && emb, "ppv_model_forward: null argument");
-    return h->m->forward(feat, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    return h->m->forward(ModelInput{feat}, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 int ppv_model_forward_lengths(ppv_model_t* h, const float* feat, const float* lengths, int B, int T, float* emb, void* ws, size_t ws_bytes,
                               void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && feat && emb, "ppv_model_forward_lengths: null argument");
-    if (!ecapa_of(h)) return fail(PPV_EUNSUPPORTED, "ppv_model_forward_lengths: only EcapaTdnn.forward takes lengths in the reference");
-    return ecapa_forward(h->m, feat, nullptr, nullptr, nullptr, B, T, 0, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream), lengths);
+    ModelInput in{feat};
+    in.lengths = lengths;
+    return h->m->forward(in, B, T, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 int ppv_model_forward_wav(ppv_model_t* h, ppv_fbank_t* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb,
                           void* ws, size_t ws_bytes, void* stream) {
     PPV_GUARD_BEGIN
     PPV_REQUIRE(h && fb && wav && emb, "ppv_model_forward_wav: null argument");
-    if (!wav_model_of(h))
-        return fail(PPV_EUNSUPPORTED, "ppv_model_forward_wav: the fused waveform path exists for ECAPA-TDNN and Res2Net only; call ppv_fbank_forward + ppv_model_forward");
-    if (h->kind == PPV_MODEL_RES2NET)
-        return res2net_forward_wav(h->m, fb->impl, wav, lens_ratio, B, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
-    const int T = fbank_num_frames(fb->impl, L);
-    PPV_REQUIRE(T > 0, "ppv_model_forward_wav: waveform shorter than one frame");
-    return ecapa_forward(h->m, nullptr, fb->impl, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+    return h->m->forward(ModelInput{nullptr, fb->impl, wav, lens_ratio, L}, B, 0, emb, ws, ws_bytes, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
 int ppv_model_read_tap(ppv_model_t* h, const char* name, float* out, size_t out_elems, void* stream) {
@@ -383,13 +372,13 @@ int ppv_kmeans(const double* X, int ld, int N, int k, const double* uniforms, in
 }
 
 int ppv_model_profile(ppv_model_t* h, int enable) {
-    PPV_REQUIRE(wav_model_of(h), "ppv_model_profile: ECAPA-TDNN or Res2Net model required");
+    PPV_REQUIRE(h && h->m->takes_wav(), "ppv_model_profile: ECAPA-TDNN or Res2Net model required");
     h->m->profile(enable != 0);
     return PPV_OK;
 }
 int ppv_model_profile_read(ppv_model_t* h, double* gemm_ms, double* other_ms, int64_t* gemm_launches, int64_t* other_launches) {
     PPV_GUARD_BEGIN
-    PPV_REQUIRE(wav_model_of(h), "ppv_model_profile_read: ECAPA-TDNN or Res2Net model required");
+    PPV_REQUIRE(h && h->m->takes_wav(), "ppv_model_profile_read: ECAPA-TDNN or Res2Net model required");
     PPV_REQUIRE(gemm_ms && other_ms && gemm_launches && other_launches, "ppv_model_profile_read: null argument");
     return h->m->profile_read(gemm_ms, other_ms, gemm_launches, other_launches);
     PPV_GUARD_END

@@ -395,16 +395,10 @@ int spec_augment_run(float* feat, const int32_t* params, int B, int T, int F, in
 struct Model;
 void ppv_ecapa_default_cfg_impl(ppv_ecapa_cfg* c);
 int ecapa_create(const ppv_ecapa_cfg* cfg, Model** out);
-// ECAPA-TDNN only (m must be one): waveform input through `fb` and `lengths`
-int ecapa_forward(Model* m, const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb,
-                  void* ws, size_t ws_bytes, cudaStream_t st, const float* lengths = nullptr);
 void ppv_resnetse_default_cfg_impl(ppv_resnetse_cfg* c);
 int resnetse_create(const ppv_resnetse_cfg* cfg, Model** out);
 void ppv_res2net_default_cfg_impl(ppv_res2net_cfg* c);
 int res2net_create(const ppv_res2net_cfg* cfg, Model** out);
-// Res2Net only (m must be one): the Fbank of wav [B, L] into the workspace, then the forward
-int res2net_forward_wav(Model* m, Fbank* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb, void* ws, size_t ws_bytes,
-                        cudaStream_t st);
 void ppv_eres2net_default_cfg_impl(ppv_eres2net_cfg* c);
 int eres2net_create(const ppv_eres2net_cfg* cfg, Model** out);
 void ppv_campplus_default_cfg_impl(ppv_campplus_cfg* c);

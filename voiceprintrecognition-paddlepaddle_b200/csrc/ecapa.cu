@@ -51,16 +51,16 @@ struct EcapaModel : PlanModel, EcapaGeometry {
         max_bn = 128;
     }
     int embd_dim() const override { return cfg.embd_dim; }
+    int input_size() const override { return cfg.input_size; }
+    bool takes_wav() const override { return true; }
+    bool takes_lengths() const override { return true; }
     size_t workspace_bytes(int B, int T) const override;
-    int forward_ex(const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb, void* ws,
-                   size_t ws_bytes, cudaStream_t st, const float* lengths);
 
   protected:
     bool prepare_weights(ArenaBuilder& ab) override;
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
-    int run_steps(const float* feat, cudaStream_t st) override { return run(feat, nullptr, nullptr, nullptr, 0, nullptr, st); }
+    int stage_inputs(const ModelInput& in, PlanInputs* pin, cudaStream_t st) override;
     int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
-    int run(const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int L, const float* lengths, cudaStream_t st);
 };
 
 // ------------------------------------------------------------------------------------------------ create / load
@@ -360,49 +360,23 @@ int EcapaModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-int EcapaModel::forward_ex(const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb, void* ws,
-                           size_t ws_bytes, cudaStream_t st, const float* lengths) {
-    int rc = forward_begin(emb, B, T);
-    if (rc) return rc;
-    PPV_REQUIRE((feat != nullptr) != (wav != nullptr), "ecapa_forward: exactly one of feat / wav");
-    if (wav) {
-        PPV_REQUIRE(fb, "ecapa_forward: wav input needs a fbank handle");
-        PPV_REQUIRE(fbank_n_mels(fb) == cfg.input_size, "ecapa_forward: fbank n_mels != model input_size");
-        PPV_REQUIRE(fbank_num_frames(fb, L) == T, "ecapa_forward: frame count mismatch");
-    }
-    rc = update_plan(B, T, ws, ws_bytes, st);
-    if (!rc) rc = run(feat, fb, wav, lens_ratio, L, lengths, st);
-    return rc ? rc : copy_embeddings(emb, st);
-}
-
-int ecapa_forward(Model* m, const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int B, int T, int L, float* emb, void* ws,
-                  size_t ws_bytes, cudaStream_t st, const float* lengths) {
-    return static_cast<EcapaModel*>(m)->forward_ex(feat, fb, wav, lens_ratio, B, T, L, emb, ws, ws_bytes, st, lengths);
-}
-
-// Packs the features or, with `wav`, computes the fbank of the waveforms into the first layer's operand, then runs the plan.
-int EcapaModel::run(const float* feat, Fbank* fb, const float* wav, const float* lens_ratio, int L, const float* lengths, cudaStream_t st) {
+// Packs the features or, with `wav`, computes the fbank of the waveforms into the first layer's operand.
+int EcapaModel::stage_inputs(const ModelInput& in, PlanInputs* pin, cudaStream_t st) {
     const int B = plan_B, T = plan_T;
     // `lengths` (ecapa_tdnn.py:245, relative lengths in (0,1]): SEBlock squeezes and ASP pools over the first
     // #{t : t < lengths[b] * T} frames of each utterance (ecapa_tdnn.py:71-75, pooling.py:96-115); everything else sees all T frames.
-    const int* nv = nullptr;
-    if (lengths) {
+    if (in.lengths) {
         PPV_REQUIRE(cfg.pooling == PPV_POOL_ASP, "ecapa_forward: lengths is implemented for ASP pooling (the other heads ignore it in the reference)");
-        int rc = launch_lengths_to_counts(lengths, B, T, buf.nvalid, st);
+        int rc = launch_lengths_to_counts(in.lengths, B, T, buf.nvalid, st);
         if (rc) return rc;
-        nv = buf.nvalid;
+        pin->nvalid = buf.nvalid;
     }
-    int rc;
+    if (in.wav) return stage_fbank(in, buf.raw_logmel, nullptr, buf.feat, P, Tp, st);
     prof_begin(1, st);
-    if (wav) {
-        rc = fbank_run(fb, wav, lens_ratio, B, L, buf.raw_logmel, nullptr, buf.feat, P, Tp, st);
-        launches_other += 3;
-    } else {
-        rc = launch_pack_features(feat, B, T, cfg.input_size, buf.feat, P, Tp, st);
-        launches_other += 1;
-    }
+    const int rc = launch_pack_features(in.feat, B, T, cfg.input_size, buf.feat, P, Tp, st);
+    launches_other += 1;
     prof_end(st);
-    return rc ? rc : run_plan(PlanInputs{feat, nv}, st);
+    return rc;
 }
 
 int EcapaModel::tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) {

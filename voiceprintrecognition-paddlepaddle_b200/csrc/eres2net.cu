@@ -54,6 +54,7 @@ struct ERes2NetModel : PlanModel {
 
     explicit ERes2NetModel(const ppv_eres2net_cfg& c) : PlanModel("eres2net", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
+    int input_size() const override { return cfg.input_size; }
     size_t workspace_bytes(int B, int T) const override;
 
   protected:

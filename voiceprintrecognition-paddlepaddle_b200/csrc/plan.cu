@@ -1,4 +1,4 @@
-// The plans (plan.h): step constructors, layer routing, the step executor and its launch profile.
+// The plans (plan.h): step constructors, layer routing, the model forward, the step executor and its launch profile.
 #include "plan.h"
 
 namespace ppv {
@@ -71,6 +71,37 @@ int PlanModel::plan_asp_fused(const Planes& W, const Planes& att, const Planes& 
                          return asp_fused_launch(p, r.precision, r.num_sms, r.st);
                      }});
     return PPV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ forward
+int Model::forward(const ModelInput& in, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
+    const std::string fn = std::string(prefix) + "_forward";
+    PPV_REQUIRE(emb && (in.feat != nullptr) != (in.wav != nullptr), fn + ": null argument, or not exactly one of feat / wav");
+    if (in.wav && !takes_wav()) return fail(PPV_EUNSUPPORTED, fn + ": no fused waveform path; call ppv_fbank_forward + ppv_model_forward");
+    if (in.lengths && !takes_lengths()) return fail(PPV_EUNSUPPORTED, fn + ": takes no lengths (only EcapaTdnn.forward does in the reference)");
+    if (in.wav) {
+        PPV_REQUIRE(in.fb, fn + ": wav input needs a fbank handle");
+        PPV_REQUIRE(fbank_n_mels(in.fb) == input_size(), fn + ": fbank n_mels != model input_size");
+        T = fbank_num_frames(in.fb, in.L);
+        PPV_REQUIRE(T > 0, fn + ": waveform shorter than one frame");
+    }
+    if (!finalized) return fail(PPV_ESTATE, fn + ": call ppv_model_finalize first");
+    PPV_REQUIRE(B > 0 && T > 0, fn + ": empty batch");
+    PlanInputs pin{in.feat};
+    int rc = update_plan(B, T, ws, ws_bytes, st);
+    if (!rc) rc = stage_inputs(in, &pin, st);
+    if (!rc) rc = run_plan(pin, st);
+    if (rc) return rc;
+    PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return PPV_OK;
+}
+
+int Model::stage_fbank(const ModelInput& in, float* raw, float* out_f32, const Planes& out_pl, int P, int Tp, cudaStream_t st) {
+    prof_begin(1, st);
+    const int rc = fbank_run(in.fb, in.wav, in.lens_ratio, plan_B, in.L, raw, out_f32, out_pl, P, Tp, st);
+    launches_other += 3;
+    prof_end(st);
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------------------ executor

@@ -21,6 +21,16 @@ struct PlanInputs {
     int easy_margin = 0;
 };
 
+// What a caller hands Model::forward: features, or waveforms through the fused Fbank front end; and, optionally, `lengths`.
+struct ModelInput {
+    const float* feat = nullptr;     // features [B, T, input_size]; null when wav is set
+    Fbank* fb = nullptr;             // the front end of wav [B, L], with lens_ratio as ppv_fbank_forward takes it
+    const float* wav = nullptr;
+    const float* lens_ratio = nullptr;
+    int L = 0;
+    const float* lengths = nullptr;  // [B] relative lengths in (0, 1] (ppv_model_forward_lengths); null: every frame
+};
+
 // What only the run knows.  Precision is one of them: set_precision switches a live plan without rebuilding it.
 struct StepRun {
     const PlanInputs& in;
@@ -130,6 +140,11 @@ struct Model : PlanOwner {
     Model(const char* prefix, int precision) : PlanOwner(prefix, "ppv_model_workspace_bytes", precision) {}
     ~Model() override { cudaFree(arena); }
     virtual int embd_dim() const = 0;
+    virtual int input_size() const = 0;
+    // Which inputs forward() takes besides features: waveforms through the fused Fbank front end (the models ppv_model_profile takes
+    // too), and `lengths`.
+    virtual bool takes_wav() const { return false; }
+    virtual bool takes_lengths() const { return false; }
 
     int load_weight(const char* name, const float* data, const int64_t* shape, int ndim) {
         if (finalized) return fail(PPV_ESTATE, std::string(prefix) + "_load_weight: model already finalized");
@@ -152,12 +167,9 @@ struct Model : PlanOwner {
         finalized = true;
         return PPV_OK;
     }
-    int forward(const float* feat, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st) {
-        int rc = forward_begin(emb, B, T);
-        if (!rc) rc = update_plan(B, T, ws, ws_bytes, st);
-        if (!rc) rc = run_steps(feat, st);
-        return rc ? rc : copy_embeddings(emb, st);
-    }
+    // B utterances -> emb [B, embd_dim]: T frames of in.feat, or as many as the front end makes of in.wav's L samples (T is then
+    // ignored).  Plans for (ws, B, T) if the plan is not that one, stages the inputs, runs the plan and copies the embeddings out.
+    int forward(const ModelInput& in, int B, int T, float* emb, void* ws, size_t ws_bytes, cudaStream_t st);
     int read_tap(const char* name, float* out, size_t out_elems, cudaStream_t st) {
         PPV_REQUIRE(name && out, std::string(prefix) + "_read_tap: null argument");
         if (!plan_ws) return fail(PPV_ESTATE, std::string(prefix) + "_read_tap: no forward has run");
@@ -165,21 +177,14 @@ struct Model : PlanOwner {
     }
 
   protected:
-    // The steps of forward(), for models whose forward takes more inputs.
-    int forward_begin(const float* emb, int B, int T) {
-        PPV_REQUIRE(emb, std::string(prefix) + "_forward: null argument");
-        if (!finalized) return fail(PPV_ESTATE, std::string(prefix) + "_forward: call ppv_model_finalize first");
-        PPV_REQUIRE(B > 0 && T > 0, std::string(prefix) + "_forward: empty batch");
-        return PPV_OK;
-    }
-    int copy_embeddings(float* emb, cudaStream_t st) {
-        PPV_CUDA_OK(cudaMemcpyAsync(emb, emb_out, size_t(plan_B) * embd_dim() * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        return PPV_OK;
-    }
     // Puts the prepared weights into the arena image; false, with ab.err set where known, on a missing or misshapen weight.
     virtual bool prepare_weights(ArenaBuilder& ab) = 0;
-    // Launches the planned steps on features [plan_B, plan_T, input_size].
-    virtual int run_steps(const float* feat, cudaStream_t st) { return run_plan(PlanInputs{feat}, st); }
+    // Puts what the plan reads of `in` where it reads it and sets what else the run passes it in `pin` (pin->feat = in.feat on
+    // entry); by default the plan reads in.feat as it is.
+    virtual int stage_inputs(const ModelInput& in, PlanInputs* pin, cudaStream_t st) { return PPV_OK; }
+    // The fused front end for stage_inputs: the Fbank of in.wav as fbank_run writes it (raw log-mel, then CMN into out_f32 or the
+    // planes out_pl of the padded time layout), counted and timed as three other launches.
+    int stage_fbank(const ModelInput& in, float* raw, float* out_f32, const Planes& out_pl, int P, int Tp, cudaStream_t st);
     virtual int tap(const std::string& name, float* out, size_t out_elems, cudaStream_t st) = 0;
 };
 

@@ -230,12 +230,19 @@ struct Res2NetModel : PlanModel {
 
     explicit Res2NetModel(const ppv_res2net_cfg& c) : PlanModel("res2net", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
+    int input_size() const override { return cfg.input_size; }
+    bool takes_wav() const override { return true; }
     size_t workspace_bytes(int B, int T) const override;
-    int forward_wav(Fbank* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb, void* ws, size_t ws_bytes, cudaStream_t st);
 
   protected:
     bool prepare_weights(ArenaBuilder& ab) override;
     int build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) override;
+    // The fused front end: the Fbank of the waveforms into the workspace's feature buffer, where the stem reads them.
+    int stage_inputs(const ModelInput& in, PlanInputs* pin, cudaStream_t st) override {
+        if (!in.wav) return PPV_OK;
+        pin->feat = feat_buf;
+        return stage_fbank(in, feat_buf, feat_buf, Planes{}, 0, 0, st);
+    }
     int tap(const std::string& n, float* out, size_t out_elems, cudaStream_t st) override;
 };
 
@@ -326,7 +333,7 @@ bool Res2NetModel::prepare_weights(ArenaBuilder& ab) {
 namespace {
 
 struct R2Buffers {
-    float* feat;  // forward_wav's features [B, T, F]
+    float* feat;  // the fused front end's features [B, T, F]
     Planes stem_out;
     std::vector<Planes> c1, cat, o3, out;
     AspHeadBuffers head;
@@ -461,29 +468,6 @@ int Res2NetModel::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream
     emb_out = rb.head.emb_out;
     feat_buf = rb.feat;
     return PPV_OK;
-}
-
-// The fused front end: the Fbank of the waveforms into the workspace's feature buffer, then the plan on it.
-int Res2NetModel::forward_wav(Fbank* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb, void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
-    PPV_REQUIRE(fb && wav, "res2net_forward_wav: null argument");
-    PPV_REQUIRE(fbank_n_mels(fb) == cfg.input_size, "res2net_forward_wav: fbank n_mels != model input_size");
-    const int T = fbank_num_frames(fb, L);
-    PPV_REQUIRE(T > 0, "res2net_forward_wav: waveform shorter than one frame");
-    int rc = forward_begin(emb, B, T);
-    if (!rc) rc = update_plan(B, T, ws, ws_bytes, st);
-    if (rc) return rc;
-    prof_begin(1, st);
-    rc = fbank_run(fb, wav, lens_ratio, B, L, feat_buf, feat_buf, Planes{}, 0, 0, st);
-    launches_other += 3;
-    prof_end(st);
-    if (!rc) rc = run_plan(PlanInputs{feat_buf}, st);
-    return rc ? rc : copy_embeddings(emb, st);
-}
-
-int res2net_forward_wav(Model* m, Fbank* fb, const float* wav, const float* lens_ratio, int B, int L, float* emb, void* ws, size_t ws_bytes,
-                        cudaStream_t st) {
-    return static_cast<Res2NetModel*>(m)->forward_wav(fb, wav, lens_ratio, B, L, emb, ws, ws_bytes, st);
 }
 
 // taps: "stem" (after the max-pool), "layer1".."layer4" -> fp32 [B,H,W,C]; "flat" -> [B,T',cat]; "asp" -> [B, 2*cat]

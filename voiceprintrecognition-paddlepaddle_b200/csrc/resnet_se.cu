@@ -44,6 +44,7 @@ struct ResNetSEModel : PlanModel {
 
     explicit ResNetSEModel(const ppv_resnetse_cfg& c) : PlanModel("resnetse", c.precision), cfg(c) {}
     int embd_dim() const override { return cfg.embd_dim; }
+    int input_size() const override { return cfg.input_size; }
     size_t workspace_bytes(int B, int T) const override;
 
   protected:

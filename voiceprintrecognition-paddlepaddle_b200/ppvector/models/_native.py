@@ -12,6 +12,9 @@ from ppvector import _lib
 class NativeBackbone(nn.Module):
     """Subclasses implement ``_native_cfg() -> (kind, ctypes cfg struct)`` and set ``embd_dim`` / ``input_size``."""
 
+    # True: the library takes this model's waveforms through the Fbank front end in the same call (ppv_model_forward_wav)
+    _fused_wav = False
+
     def __init__(self, precision='bf16x3'):
         super().__init__()
         self.precision = precision
@@ -70,28 +73,58 @@ class NativeBackbone(nn.Module):
         except Exception:
             pass
 
-    def forward(self, x, lengths=None):
-        """x [N, time, freq] float32 CUDA -> [N, embd_dim]"""
-        if lengths is not None:
-            raise NotImplementedError('lengths masking is never used by the reference callers and is not implemented')
+    def _lengths_refusal(self):
+        """Why ``forward`` cannot take ``lengths``, or None where it can (ppv_model_forward_lengths)."""
+        return 'lengths masking is never used by the reference callers and is not implemented'
+
+    def _check_eval(self):
         if self.training:
             raise _lib.PPVError(f'{type(self).__name__} on the H100 path implements the eval-mode forward only; call .eval()')
+
+    def _embed(self, entry, args, device, B, T):
+        """[B, embd_dim] from the library call ``entry(handle, *args, emb, workspace, workspace_bytes, stream)``, on a workspace
+        sized for B utterances of T frames."""
+        with torch.cuda.device(device):
+            h = self._get_handle()
+            ws = self._workspace(B, T, device)
+            emb = torch.empty((B, self.embd_dim), dtype=torch.float32, device=device)
+            _lib.check(getattr(_lib.load(), entry)(h, *args, _lib.ptr(emb), C.c_void_p(ws.data_ptr()), ws.numel(),
+                                                    _lib.current_stream()), entry)
+        return emb
+
+    def forward(self, x, lengths=None):
+        """x [N, time, freq] float32 CUDA -> [N, embd_dim].  ``lengths`` [N], where the model takes it: relative lengths in (0, 1]."""
+        refusal = lengths is not None and self._lengths_refusal()
+        if refusal:
+            raise NotImplementedError(refusal)
+        self._check_eval()
         _lib.require_cuda(x, 'x')
         x = x.to(torch.float32).contiguous()
         B, T, F = x.shape
         assert F == self.input_size
-        with torch.cuda.device(x.device):
-            h = self._get_handle()
-            ws = self._workspace(B, T, x.device)
-            emb = torch.empty((B, self.embd_dim), dtype=torch.float32, device=x.device)
-            _lib.check(_lib.load().ppv_model_forward(h, _lib.ptr(x), B, T, _lib.ptr(emb), C.c_void_p(ws.data_ptr()),
-                                                      ws.numel(), _lib.current_stream()), 'ppv_model_forward')
-        return emb
+        if lengths is None:
+            return self._embed('ppv_model_forward', (_lib.ptr(x), B, T), x.device, B, T)
+        lengths = torch.as_tensor(lengths, dtype=torch.float32, device=x.device).contiguous()
+        assert lengths.shape == (B,)
+        return self._embed('ppv_model_forward_lengths', (_lib.ptr(x), _lib.ptr(lengths), B, T), x.device, B, T)
 
     def forward_wav(self, featurizer, waveforms, input_lens_ratio=None):
-        """waveforms [N, samples] -> [N, embd_dim]: featurise, then embed (two library calls).  EcapaTdnn overrides this with the
-        fused ``ppv_model_forward_wav`` path when the front end is Fbank."""
-        return self(featurizer(waveforms, input_lens_ratio))
+        """waveforms [N, samples] -> [N, embd_dim], equal to ``self(featurizer(waveforms, input_lens_ratio))``.  Models with
+        ``_fused_wav`` and an Fbank front end take one library call (``ppv_model_forward_wav``) that never materialises the
+        [N, time, freq] features; every other pairing featurises, then embeds (two calls)."""
+        if not self._fused_wav or getattr(featurizer, '_feature_method', 'Fbank') != 'Fbank':
+            return self(featurizer(waveforms, input_lens_ratio))
+        self._check_eval()
+        _lib.require_cuda(waveforms, 'waveforms')
+        if waveforms.dim() == 1:
+            waveforms = waveforms.unsqueeze(0)
+        wav = waveforms.to(torch.float32).contiguous()
+        B, L = wav.shape
+        ratio = None
+        if input_lens_ratio is not None:
+            ratio = torch.as_tensor(input_lens_ratio, dtype=torch.float32, device=wav.device).contiguous()
+        return self._embed('ppv_model_forward_wav', (featurizer._get_handle(), _lib.ptr(wav), _lib.ptr(ratio), B, L), wav.device,
+                           B, featurizer.num_frames(L))
 
     def _read_tap(self, name, shape):
         out = torch.empty(shape, dtype=torch.float32, device=self._ws.device)

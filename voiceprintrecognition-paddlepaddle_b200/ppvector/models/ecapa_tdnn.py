@@ -9,7 +9,6 @@ There is no torch fallback.
 """
 import ctypes as C
 
-import torch
 from torch import nn
 
 from ppvector import _lib
@@ -97,6 +96,7 @@ class SelfAttentivePooling(nn.Module):
 
 
 class EcapaTdnn(NativeBackbone):
+    _fused_wav = True  # the Fbank features go straight into the first conv's operand layout
     _POOLING = {"ASP": _lib.PPV_POOL_ASP, "SAP": _lib.PPV_POOL_SAP, "TAP": _lib.PPV_POOL_TAP, "TSP": _lib.PPV_POOL_TSP}
 
     def __init__(self, input_size, embd_dim=192, pooling_type="ASP", activation=None,
@@ -147,60 +147,16 @@ class EcapaTdnn(NativeBackbone):
         cfg.global_context = 1 if self.global_context else 0
         return _lib.PPV_MODEL_ECAPA_TDNN, cfg
 
-    def forward(self, x, lengths=None):
-        """reference: ecapa_tdnn.py:245-276.  x [N, time, freq] float32 CUDA -> [N, embd_dim].  ``lengths`` [N]: relative lengths in
-        (0, 1]; SEBlock and ASP then use the first #{t : t < lengths * T} frames only (ecapa_tdnn.py:71-75, pooling.py:96-115)."""
-        if lengths is None:
-            return super().forward(x)
+    def _lengths_refusal(self):
+        """reference: ecapa_tdnn.py:245-276.  ``lengths``: SEBlock and ASP use the first #{t : t < lengths * T} frames only
+        (ecapa_tdnn.py:71-75, pooling.py:96-115)."""
         if self.pooling_type != "ASP":  # pooling.py:17,39,60: the other pooling layers accept and ignore `lengths`; SEBlock does not
-            raise NotImplementedError('lengths with pooling_type != "ASP" is not implemented on the H100 path')
-        if self.training:
-            raise _lib.PPVError('EcapaTdnn on the H100 path implements the eval-mode forward only; call .eval()')
-        _lib.require_cuda(x, 'x')
-        x = x.to(torch.float32).contiguous()
-        B, T, F = x.shape
-        assert F == self.input_size
-        lengths = torch.as_tensor(lengths, dtype=torch.float32, device=x.device).contiguous()
-        assert lengths.shape == (B,)
-        with torch.cuda.device(x.device):
-            h = self._get_handle()
-            ws = self._workspace(B, T, x.device)
-            emb = torch.empty((B, self.embd_dim), dtype=torch.float32, device=x.device)
-            _lib.check(_lib.load().ppv_model_forward_lengths(h, _lib.ptr(x), _lib.ptr(lengths), B, T, _lib.ptr(emb),
-                                                              C.c_void_p(ws.data_ptr()), ws.numel(), _lib.current_stream()),
-                       'ppv_model_forward_lengths')
-        return emb
-
-    def forward_wav(self, featurizer, waveforms, input_lens_ratio=None):
-        """Fused waveform -> embedding path (``ppv_model_forward_wav``): equals
-        ``self(featurizer(waveforms, input_lens_ratio))`` without materialising the [B,T,F] features."""
-        if getattr(featurizer, '_feature_method', 'Fbank') != 'Fbank':  # the fused path is Fbank -> ECAPA; other front ends: two calls
-            return self(featurizer(waveforms, input_lens_ratio))
-        _lib.require_cuda(waveforms, 'waveforms')
-        if waveforms.dim() == 1:
-            waveforms = waveforms.unsqueeze(0)
-        wav = waveforms.to(torch.float32).contiguous()
-        B, L = wav.shape
-        T = featurizer.num_frames(L)
-        ratio = None
-        if input_lens_ratio is not None:
-            ratio = torch.as_tensor(input_lens_ratio, dtype=torch.float32, device=wav.device).contiguous()
-        with torch.cuda.device(wav.device):
-            h = self._get_handle()
-            ws = self._workspace(B, T, wav.device)
-            emb = torch.empty((B, self.embd_dim), dtype=torch.float32, device=wav.device)
-            _lib.check(_lib.load().ppv_model_forward_wav(h, featurizer._get_handle(), _lib.ptr(wav), _lib.ptr(ratio), B, L,
-                                                          _lib.ptr(emb), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                                          _lib.current_stream()), 'ppv_model_forward_wav')
-        return emb
+            return 'lengths with pooling_type != "ASP" is not implemented on the H100 path'
+        return None
 
     def read_tap(self, name, B, T):
         """Debug / parity: an internal activation of the last forward as fp32 ([B,T,C], or [B,2C] for 'asp')."""
         C3 = self.channels[-1]
         cols = {'feat': self.input_size, 'blocks.0': self.channels[0], 'blocks.1': self.channels[1],
                 'blocks.2': self.channels[2], 'blocks.3': self.channels[3], 'mfa': C3}
-        dev = self._ws.device
-        out = torch.empty((B, 2 * C3) if name == 'asp' else (B, T, cols[name]), dtype=torch.float32, device=dev)
-        _lib.check(_lib.load().ppv_model_read_tap(self._get_handle(), name.encode(), _lib.ptr(out), out.numel(),
-                                                   _lib.current_stream()), 'ppv_model_read_tap')
-        return out
+        return self._read_tap(name, (B, 2 * C3) if name == 'asp' else (B, T, cols[name]))

@@ -8,7 +8,6 @@ head.  Eval mode only."""
 import ctypes as C
 import math
 
-import torch
 from torch import nn
 
 from ppvector import _lib
@@ -46,6 +45,8 @@ def _final_height(input_size):
 
 
 class Res2Net(NativeBackbone):
+    _fused_wav = True  # the Fbank features go to the workspace, where the stem reads them
+
     def __init__(self, input_size, m_channels=32, layers=[3, 4, 6, 3], base_width=32, scale=2, embd_dim=192, pooling_type="ASP",
                  precision='bf16x3'):
         super().__init__(precision)
@@ -94,31 +95,6 @@ class Res2Net(NativeBackbone):
         for i in range(4):
             cfg.layers[i] = self.layers_cfg[i]
         return _lib.PPV_MODEL_RES2NET, cfg
-
-    def forward_wav(self, featurizer, waveforms, input_lens_ratio=None):
-        """Fused waveform -> embedding path (``ppv_model_forward_wav``): equals ``self(featurizer(waveforms, input_lens_ratio))`` in one
-        library call; the Fbank features go to the workspace, where the stem reads them.  Other front ends: two calls."""
-        if getattr(featurizer, '_feature_method', 'Fbank') != 'Fbank':
-            return self(featurizer(waveforms, input_lens_ratio))
-        if self.training:
-            raise _lib.PPVError('Res2Net on the H100 path implements the eval-mode forward only; call .eval()')
-        _lib.require_cuda(waveforms, 'waveforms')
-        if waveforms.dim() == 1:
-            waveforms = waveforms.unsqueeze(0)
-        wav = waveforms.to(torch.float32).contiguous()
-        B, L = wav.shape
-        T = featurizer.num_frames(L)
-        ratio = None
-        if input_lens_ratio is not None:
-            ratio = torch.as_tensor(input_lens_ratio, dtype=torch.float32, device=wav.device).contiguous()
-        with torch.cuda.device(wav.device):
-            h = self._get_handle()
-            ws = self._workspace(B, T, wav.device)
-            emb = torch.empty((B, self.embd_dim), dtype=torch.float32, device=wav.device)
-            _lib.check(_lib.load().ppv_model_forward_wav(h, featurizer._get_handle(), _lib.ptr(wav), _lib.ptr(ratio), B, L,
-                                                          _lib.ptr(emb), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                                          _lib.current_stream()), 'ppv_model_forward_wav')
-        return emb
 
     def grids(self, T):
         """[(H, W)] of the pooled stem grid (= layer1's) and of layers 2..4 for T frames"""
