@@ -285,7 +285,21 @@ int ppv_model_profile_read(ppv_model_t* h, double* gemm_ms, double* other_ms, in
 int ppv_set_pdl(int enabled);
 
 typedef struct ppv_trainer ppv_trainer_t;
+/* The classifier of ppvector/models/fc.py (model_conf.classifier), Cosine with num_blocks = 0 unless created with
+ * ppv_trainer_create_classifier. */
 int ppv_trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, ppv_trainer_t** out);
+/* classifier_type: the output layer, fc.py:30-40 -- PPV_CLASSIFIER_COSINE ("classifier.weight" [in, num_classes], cosine logits) or
+ * PPV_CLASSIFIER_LINEAR ("classifier.output.weight" [in, num_classes] and "classifier.output.bias" [num_classes], logits = h W + b).
+ * num_blocks DenseLayers sit between the embedding and the output layer (fc.py:27-29), each Conv1D(in, inter_dim, 1) with bias then
+ * BatchNorm1D(inter_dim), no ReLU, batch statistics in training: "classifier.blocks.<i>.linear.{weight [inter_dim, in, 1], bias}",
+ * "classifier.blocks.<i>.nonlinear.batchnorm.{weight, bias, _mean, _variance}"; `in` is embd_dim for block 0 and inter_dim after it.
+ * A Linear classifier runs with the loss heads defined for any real logits: PPV_HEAD_AM, PPV_HEAD_ARM, PPV_HEAD_CE and SphereFace2
+ * type C; ppv_trainer_forward_backward refuses the others.  Taps "classifier.blocks.<i>" and "g:classifier.blocks.<i>" read a block's
+ * output and its gradient, [B, inter_dim]. */
+#define PPV_CLASSIFIER_COSINE 0
+#define PPV_CLASSIFIER_LINEAR 1
+int ppv_trainer_create_classifier(const ppv_ecapa_cfg* cfg, int num_classes, int classifier_type, int num_blocks, int inter_dim,
+                                  ppv_trainer_t** out);
 int ppv_trainer_destroy(ppv_trainer_t* h);
 int64_t ppv_trainer_param_count(const ppv_trainer_t* h); /* floats in the parameter / gradient buffers (tensors are 32-byte aligned) */
 int64_t ppv_trainer_stat_count(const ppv_trainer_t* h);  /* floats in the running-statistics buffer */
@@ -298,10 +312,11 @@ int ppv_trainer_bind(ppv_trainer_t* h, float* params, float* grads, float* stats
 int ppv_trainer_set_precision(ppv_trainer_t* h, int precision);
 size_t ppv_trainer_workspace_bytes(ppv_trainer_t* h, int B, int T);
 /* feat [B,T,F] fp32, labels [B] int64 (device).  Overwrites the whole gradient buffer with d(loss)/d(param), updates the
- * running statistics, writes the scalar loss and (optionally) the cosine logits [B, num_classes] (device pointers). */
+ * running statistics, writes the scalar loss and (optionally) the classifier's logits [B, num_classes] (device pointers). */
 int ppv_trainer_forward_backward(ppv_trainer_t* h, const float* feat, const int64_t* labels, int B, int T, float margin, float scale,
                                  int easy_margin, float label_smoothing, float* loss, float* logits, void* ws, size_t ws_bytes, void* stream);
-/* forward activations of the last step: "blocks.0".."blocks.3", "mfa" -> [B,T,C]; "asp" -> [B, 2*3C]; "emb" -> [B, embd_dim] */
+/* forward activations of the last step: "blocks.0".."blocks.3", "mfa" -> [B,T,C]; "asp" -> [B, 2*3C]; "emb" -> [B, embd_dim];
+ * "classifier.blocks.<i>" -> [B, inter_dim] */
 int ppv_trainer_read_tap(ppv_trainer_t* h, const char* name, float* out, size_t out_elems, void* stream);
 /* p -= lr * mhat / (sqrt(vhat) + eps) with g = grads * grad_scale + weight_decay * p; step counts from 1. */
 int ppv_adam_step(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,

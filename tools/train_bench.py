@@ -1,7 +1,8 @@
 """Training-step throughput of the ECAPA-TDNN CUDA trainer (SURVEY.md §8d config 3 shape: per-GPU batch 64 x 298 frames, 2796
 speakers, AAM margin 0.2, Adam) -- a tuning aid; features resident in HBM.  python tools/train_bench.py [--batch 64] [--frames 298]
-[--steps 10] [--pooling ASP|SAP|TAP|TSP] [--no-global-context] [--once] [--dump DIR]  (--pooling: the ECAPA-TDNN head, as
-model_conf.model_args.pooling_type; --no-global-context: ASP without the global context; --once: one warm step only, for an ncu launch list; --dump: the state after one step, to
+[--steps 10] [--pooling ASP|SAP|TAP|TSP] [--no-global-context] [--classifier Cosine|Linear] [--num-blocks N] [--inter-dim D] [--once]
+[--dump DIR]  (--pooling: the ECAPA-TDNN head, as model_conf.model_args.pooling_type; --no-global-context: ASP without the global context;
+--classifier / --num-blocks / --inter-dim: model_conf.classifier, a Linear classifier trains with CELoss, a Cosine one with AAMLoss; --once: one warm step only, for an ncu launch list; --dump: the state after one step, to
 compare two builds bit for bit).  Under torchrun every rank trains its own batch and the
 gradient all-reduce runs over NCCL."""
 import argparse
@@ -14,8 +15,10 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "voiceprintrecognition-paddlepaddle_b200"))
+from ppvector import _lib  # noqa: E402
 from ppvector.models.ecapa_tdnn import EcapaTdnn  # noqa: E402
 from ppvector.train_engine import TrainEngine  # noqa: E402
+from ppvector.trainer import init_classifier  # noqa: E402
 
 
 def main():
@@ -30,6 +33,9 @@ def main():
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "bf16"], help="bf16 = train_conf.enable_amp")
     ap.add_argument("--pooling", default="ASP", choices=["ASP", "SAP", "TAP", "TSP"], help="the pooling head (pooling_type)")
     ap.add_argument("--no-global-context", action="store_true", help="ASP without the global context statistics")
+    ap.add_argument("--classifier", default="Cosine", choices=["Cosine", "Linear"], help="the output layer (classifier_type)")
+    ap.add_argument("--num-blocks", type=int, default=0, help="DenseLayer blocks before the output layer (num_blocks)")
+    ap.add_argument("--inter-dim", type=int, default=512, help="width of the DenseLayer blocks (inter_dim)")
     a = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -41,21 +47,23 @@ def main():
     dev = torch.device("cuda", local)
     torch.manual_seed(1000)
     head = dict(pooling_type=a.pooling, global_context=not a.no_global_context)
-    eng = TrainEngine(input_size=80, num_speakers=a.speakers, device=dev, **head)
+    eng = TrainEngine(input_size=80, num_speakers=a.speakers, device=dev, classifier_type=a.classifier, num_blocks=a.num_blocks,
+                      inter_dim=a.inter_dim, **head)
     eng.set_precision(a.precision)
-    eng.load_state_dict(EcapaTdnn(input_size=80, **head).state_dict(), torch.nn.init.xavier_uniform_(torch.empty(192, a.speakers)))
+    eng.load_state_dict(dict(EcapaTdnn(input_size=80, **head).state_dict(), **init_classifier(eng.classifier_shapes)))
+    sel = _lib.PPV_HEAD_CE if a.classifier == "Linear" else _lib.PPV_HEAD_AAM  # AAMLoss reads cosines: a Linear classifier trains with CELoss
     g = torch.Generator().manual_seed(1000 + rank)
     x = torch.randn(a.batch, a.frames, 80, generator=g)
     x = (x - x.mean(1, keepdim=True)).to(dev)
     y = torch.randint(0, a.speakers, (a.batch,), generator=g).to(dev)
 
     def step():
-        loss = eng.forward_backward(x, y, margin=0.2)
+        loss = eng.forward_backward(x, y, margin=0.2, easy_margin=sel)
         eng.adam_step(lr=1e-3, weight_decay=1e-6, grad_scale=eng.all_reduce_grads())
         return loss
 
     if a.dump:
-        loss, logits = eng.forward_backward(x, y, margin=0.2, return_logits=True)
+        loss, logits = eng.forward_backward(x, y, margin=0.2, easy_margin=sel, return_logits=True)
         eng.adam_step(lr=1e-3, weight_decay=1e-6, grad_scale=eng.all_reduce_grads())
         os.makedirs(a.dump, exist_ok=True)
         for name, t in {"loss": loss, "logits": logits, "params": eng.params, "grads": eng.grads, "stats": eng.stats, "exp_avg": eng.exp_avg,
@@ -85,7 +93,7 @@ def main():
         dist.barrier()
     for i in range(a.steps):
         ev[i][0].record()
-        eng.forward_backward(x, y, margin=0.2)
+        eng.forward_backward(x, y, margin=0.2, easy_margin=sel)
         ev[i][1].record()
         scale = eng.all_reduce_grads()
         ev[i][2].record()
@@ -104,10 +112,11 @@ def main():
     if rank == 0:
         # algorithmic work: training step ~ 3 x forward (SURVEY.md §8d), forward 2.857 GFLOP / utterance as executed with the default
         # head (ASP with global context); the other heads do less work after mfa, so the figure is given for that head only
-        default_head = a.pooling == "ASP" and not a.no_global_context
+        default_head = a.pooling == "ASP" and not a.no_global_context and a.classifier == "Cosine" and a.num_blocks == 0
         print(json.dumps({"metric": "train_samples_per_s", "value": round(world * a.batch / ms * 1e3, 1), "n_gpus": world, "precision": a.precision, "ms_per_step": round(ms, 3),
                           "batch_per_gpu": a.batch, "frames": a.frames, "speakers": a.speakers, "pooling": a.pooling,
-                          "global_context": not a.no_global_context, "loss": float(loss),
+                          "global_context": not a.no_global_context, "classifier": a.classifier, "num_blocks": a.num_blocks,
+                          "inter_dim": a.inter_dim, "loss": float(loss),
                           "algorithmic_tflops": round(world * a.batch * 3 * 2.857e9 / (ms * 1e-3) / 1e12, 1) if default_head else None,
                           "workspace_GB": round(eng._ws.numel() / 2**30, 2),
                           "breakdown_ms": {"forward_backward": round(phases[0], 3), "grad_all_reduce": round(phases[1], 3), "adam": round(phases[2], 3)},

@@ -141,6 +141,9 @@ __device__ __forceinline__ float class_cosine(const float* __restrict__ c, int c
 // cosines (cos(theta + m) with the same th / mmm fallback on the target, cos(theta - m) on the others).  Entry loss:
 // target lambda * log(1 + exp(-z_p)), others (1 - lambda) * log(1 + exp(z_n)); the loss's bias parameter is created at 0 and is not
 // handed to the optimizer in the reference (trainer.py:186-190 passes model.parameters() only), so it stays 0.
+// kRaw: the logits are a Linear layer's, any real value: g is the plain polynomial (z < -1 included); otherwise they are cosines and
+// (z + 1) / 2 is clamped at 0 against rounding.
+template <bool kRaw>
 __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a, int t, float lambda, float cos_m, float sin_m, float th,
                                            float mmm, float margin, float scale, float* dl_dc) {
     float inner = c, dinner = 1.f, shift = 0.f;
@@ -162,7 +165,7 @@ __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a,
         shift = is_target ? -margin : margin;
     }
     const float h = 0.5f * (inner + 1.f);
-    const float hp = powf(fmaxf(h, 0.f), float(t - 1));  // ((z + 1) / 2)^(t - 1)
+    const float hp = powf(kRaw ? h : fmaxf(h, 0.f), float(t - 1));  // ((z + 1) / 2)^(t - 1); t - 1 is integral, so a negative h is exact
     const float g = 2.f * hp * h - 1.f;
     const float dg = float(t) * hp * dinner;  // d g / d c
     const float z = scale * (g + shift);
@@ -175,10 +178,11 @@ __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a,
 }
 
 // one block per row: loss_b and (optionally) G[b,s] = d loss / d cos[b,s].  S = classes, K = sub-centres per class (1: plain heads);
-// logits and G have S * K columns.
-__global__ void __launch_bounds__(256)
-    aam_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m, float sin_m,
-                   float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss, float* __restrict__ G, float margin) {
+// logits and G have S * K columns.  kRaw: Linear logits (see sf2_entry).
+template <bool kRaw>
+__device__ __forceinline__ void row_loss_body(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m,
+                                         float sin_m, float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss,
+                                         float* __restrict__ G, float margin) {
     __shared__ float s_red[8];
     const int b = blockIdx.x;
     const int64_t label = labels[b];
@@ -190,7 +194,7 @@ __global__ void __launch_bounds__(256)
         const float invB = 1.f / float(B);
         for (int s = threadIdx.x; s < S; s += blockDim.x) {
             float d;
-            acc += sf2_entry(c[s], s == label, type_a, t, ls, cos_m, sin_m, th, mmm, margin, scale, &d);
+            acc += sf2_entry<kRaw>(c[s], s == label, type_a, t, ls, cos_m, sin_m, th, mmm, margin, scale, &d);
             if (G) G[int64_t(b) * S + s] = d * invB;
         }
         acc = block_reduce(acc, s_red, false);
@@ -229,6 +233,17 @@ __global__ void __launch_bounds__(256)
             for (int k = 0; k < K; ++k) G[(int64_t(b) * S + s) * K + k] = k == arg ? (p - t) * invB * d : 0.f;
         }
     }
+}
+__global__ void __launch_bounds__(256)
+    aam_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m, float sin_m,
+                   float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss_out, float* __restrict__ G, float margin) {
+    row_loss_body<false>(logits, labels, B, S, K, cos_m, sin_m, th, mmm, easy, scale, ls, row_loss_out, G, margin);
+}
+// the same for the raw logits of a Linear classifier (K = 1)
+__global__ void __launch_bounds__(256)
+    lin_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, float cos_m, float sin_m, float th,
+                   float mmm, int easy, float scale, float ls, float* __restrict__ row_loss_out, float* __restrict__ G, float margin) {
+    row_loss_body<true>(logits, labels, B, S, 1, cos_m, sin_m, th, mmm, easy, scale, ls, row_loss_out, G, margin);
 }
 __global__ void aam_mean_kernel(const float* __restrict__ row_loss, int B, float* __restrict__ loss) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -361,6 +376,141 @@ int aam_backward(const float* emb, const float* W, const int64_t* labels, const 
     PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(aam_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)));
     aam_dw_kernel<<<(S + 127) / 128, 128, smem, st>>>(w.G, w.e_hat, W, w.inv_w, B, D, S, d_W);
     PPV_LAUNCH_OK("aam_dw_kernel");
+    return PPV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Linear output layer
+// fc.py:37-38, 50-51: logits = H @ W + b with W [D, S] (Paddle's Linear layout, the one the cosine head reads) and b [S], no
+// normalisation.  The same loss heads then run on the raw logits (lin_row_kernel: aam_row_kernel's body).  Every product below is a fixed-order fp32
+// loop: no atomics, the same bits on every run.
+constexpr int LIN_ROWS = 8;    // rows of H (or of G) one thread carries: W is read once per LIN_ROWS rows
+constexpr int LIN_DCHUNK = 16;  // dW: columns of H one thread carries
+constexpr int LIN_BCHUNK = 256; // dW: rows of H staged in shared memory at a time
+
+// logits[b,s] = sum_d H[b,d] W[d,s] + bias[s]: thread per column s, LIN_ROWS rows per block (those rows of H in shared memory)
+__global__ void __launch_bounds__(256)
+    lin_logits_kernel(const float* __restrict__ H, const float* __restrict__ W, const float* __restrict__ bias, int B, int D, int S,
+                      float* __restrict__ logits) {
+    extern __shared__ float s_h[];  // [LIN_ROWS][D]
+    const int b0 = blockIdx.y * LIN_ROWS, nb = min(LIN_ROWS, B - b0);
+    for (int i = threadIdx.x; i < nb * D; i += blockDim.x) s_h[i] = H[int64_t(b0) * D + i];
+    __syncthreads();
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= S) return;
+    float acc[LIN_ROWS] = {};
+    for (int d = 0; d < D; ++d) {
+        const float w = W[int64_t(d) * S + s];
+#pragma unroll
+        for (int r = 0; r < LIN_ROWS; ++r) acc[r] = fmaf(s_h[(r < nb ? r : 0) * D + d], w, acc[r]);
+    }
+    const float bs = bias[s];
+    for (int r = 0; r < nb; ++r) logits[int64_t(b0 + r) * S + s] = acc[r] + bs;
+}
+// dH[b,d] = sum_s G[b,s] W[d,s]: one warp per d (coalesced over s), LIN_ROWS rows of G per warp
+__global__ void __launch_bounds__(256)
+    lin_dh_kernel(const float* __restrict__ G, const float* __restrict__ W, int B, int D, int S, float* __restrict__ dH) {
+    const int d = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    const int b0 = blockIdx.y * LIN_ROWS, nb = min(LIN_ROWS, B - b0);
+    if (d >= D) return;
+    float acc[LIN_ROWS] = {};
+    for (int s = lane; s < S; s += 32) {
+        const float w = W[int64_t(d) * S + s];
+#pragma unroll
+        for (int r = 0; r < LIN_ROWS; ++r)
+            if (r < nb) acc[r] = fmaf(G[int64_t(b0 + r) * S + s], w, acc[r]);
+    }
+#pragma unroll
+    for (int r = 0; r < LIN_ROWS; ++r) {
+        const float v = warp_sum(acc[r]);
+        if (lane == 0 && r < nb) dH[int64_t(b0 + r) * D + d] = v;
+    }
+}
+// dW[d,s] = sum_b H[b,d] G[b,s] for LIN_DCHUNK columns d per thread; the blocks of the first d-chunk also write db[s] = sum_b G[b,s]
+__global__ void __launch_bounds__(128)
+    lin_dw_kernel(const float* __restrict__ G, const float* __restrict__ H, int B, int D, int S, float* __restrict__ dW, float* __restrict__ db) {
+    __shared__ float s_h[LIN_BCHUNK * LIN_DCHUNK];
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    const int d0 = blockIdx.y * LIN_DCHUNK, nd = min(LIN_DCHUNK, D - d0);
+    float acc[LIN_DCHUNK] = {};
+    float gs = 0.f;
+    for (int b0 = 0; b0 < B; b0 += LIN_BCHUNK) {
+        const int nb = min(LIN_BCHUNK, B - b0);
+        __syncthreads();
+        for (int i = threadIdx.x; i < nb * LIN_DCHUNK; i += blockDim.x) {
+            const int r = i / LIN_DCHUNK, j = i % LIN_DCHUNK;
+            s_h[i] = j < nd ? H[int64_t(b0 + r) * D + d0 + j] : 0.f;
+        }
+        __syncthreads();
+        if (s < S)
+            for (int r = 0; r < nb; ++r) {
+                const float g = G[int64_t(b0 + r) * S + s];
+                gs += g;
+#pragma unroll
+                for (int j = 0; j < LIN_DCHUNK; ++j) acc[j] = fmaf(g, s_h[r * LIN_DCHUNK + j], acc[j]);
+            }
+    }
+    if (s >= S) return;
+    for (int j = 0; j < nd; ++j) dW[int64_t(d0 + j) * S + s] = acc[j];
+    if (blockIdx.y == 0) db[s] = gs;
+}
+
+// AAMLoss, SubCenterLoss and SphereFace2 type A read the logits as cosines (sqrt(1 - z^2), and SubCenterLoss's K sub-centre columns):
+// on raw Linear logits the reference turns NaN as soon as one leaves [-1, 1].  CELoss, AMLoss, ARMLoss and SphereFace2 type C are
+// defined for any real logits.
+static int linear_head_check(int sel) {
+    const bool cosine_only = (sel & PPV_HEAD_SUBCENTER) || ((sel & PPV_HEAD_SPHEREFACE2) && (sel & 1)) ||
+                             (!(sel & PPV_HEAD_SPHEREFACE2) && sel <= PPV_HEAD_AAM_EASY);
+    if (cosine_only)
+        return fail(PPV_EUNSUPPORTED, "Linear classifier: AAMLoss, SubCenterLoss and SphereFace2 type A take sqrt(1 - z^2) of cosine logits; "
+                                      "use CELoss, AMLoss, ARMLoss or SphereFace2 type C");
+    return PPV_OK;
+}
+
+int linear_head_forward(const float* H, const float* W, const float* bias, const int64_t* labels, int B, int D, int S, float margin, float scale,
+                        int easy_margin, float label_smoothing, float* logits, float* loss, void* ws, size_t ws_bytes, cudaStream_t st) {
+    PPV_REQUIRE(H && W && bias && labels && logits && loss, "linear_head_forward: null argument");
+    PPV_REQUIRE(B > 0 && D > 0 && S > 0, "linear_head_forward: empty input");
+    if (int rc = check_workspace("linear_head_forward", ws, ws_bytes, aam_workspace_bytes(B, D, S), "ppv_aam_workspace_bytes")) return rc;
+    int kind, K;
+    int rc = decode_head(easy_margin, S, &kind, &K);
+    if (!rc) rc = linear_head_check(easy_margin);
+    if (rc) return rc;
+    PPV_REQUIRE(size_t(LIN_ROWS) * D * sizeof(float) <= 48 * 1024, "linear_head_forward: input width too large");
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    AamWs w;
+    carve_aam(cv, B, D, S, &w);
+    lin_logits_kernel<<<dim3((S + 255) / 256, (B + LIN_ROWS - 1) / LIN_ROWS), 256, size_t(LIN_ROWS) * D * sizeof(float), st>>>(H, W, bias, B, D, S,
+                                                                                                                                logits);
+    PPV_LAUNCH_OK("lin_logits_kernel");
+    float cm, sm, th, mmm;
+    margin_consts(margin, &cm, &sm, &th, &mmm);
+    lin_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, nullptr, margin);
+    PPV_LAUNCH_OK("lin_row_kernel");
+    aam_mean_kernel<<<1, 32, 0, st>>>(w.row_loss, B, loss);
+    PPV_LAUNCH_OK("aam_mean_kernel");
+    return PPV_OK;
+}
+
+int linear_head_backward(const float* H, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin, float scale,
+                         int easy_margin, float label_smoothing, float* d_H, float* d_W, float* d_bias, void* ws, size_t ws_bytes, cudaStream_t st) {
+    PPV_REQUIRE(H && W && labels && logits && d_H && d_W && d_bias, "linear_head_backward: null argument");
+    if (int rc = check_workspace("linear_head_backward", ws, ws_bytes, aam_workspace_bytes(B, D, S), "ppv_aam_workspace_bytes")) return rc;
+    int kind, K;
+    int rc = decode_head(easy_margin, S, &kind, &K);
+    if (!rc) rc = linear_head_check(easy_margin);
+    if (rc) return rc;
+    WsCarver cv{static_cast<uint8_t*>(ws)};
+    AamWs w;
+    carve_aam(cv, B, D, S, &w);
+    float cm, sm, th, mmm;
+    margin_consts(margin, &cm, &sm, &th, &mmm);
+    lin_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, w.G, margin);
+    PPV_LAUNCH_OK("lin_row_kernel(bwd)");
+    lin_dh_kernel<<<dim3((D + 7) / 8, (B + LIN_ROWS - 1) / LIN_ROWS), 256, 0, st>>>(w.G, W, B, D, S, d_H);
+    PPV_LAUNCH_OK("lin_dh_kernel");
+    lin_dw_kernel<<<dim3((S + 127) / 128, (D + LIN_DCHUNK - 1) / LIN_DCHUNK), 128, 0, st>>>(w.G, H, B, D, S, d_W, d_bias);
+    PPV_LAUNCH_OK("lin_dw_kernel");
     return PPV_OK;
 }
 

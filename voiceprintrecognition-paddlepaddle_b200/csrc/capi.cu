@@ -428,7 +428,20 @@ int ppv_trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, ppv_trainer_t*
     int rc = check_device();
     if (rc) return rc;
     Trainer* impl = nullptr;
-    rc = trainer_create(cfg, num_classes, &impl);
+    rc = trainer_create(cfg, num_classes, PPV_CLASSIFIER_COSINE, 0, 0, &impl);
+    if (rc) return rc;
+    *out = new ppv_trainer{impl};
+    return PPV_OK;
+    PPV_GUARD_END
+}
+int ppv_trainer_create_classifier(const ppv_ecapa_cfg* cfg, int num_classes, int classifier_type, int num_blocks, int inter_dim,
+                                  ppv_trainer_t** out) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(cfg && out, "ppv_trainer_create_classifier: null argument");
+    int rc = check_device();
+    if (rc) return rc;
+    Trainer* impl = nullptr;
+    rc = trainer_create(cfg, num_classes, classifier_type, num_blocks, inter_dim, &impl);
     if (rc) return rc;
     *out = new ppv_trainer{impl};
     return PPV_OK;

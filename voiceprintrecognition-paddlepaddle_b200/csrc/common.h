@@ -436,7 +436,7 @@ int launch_aff_combine(const Planes& x, int xc0, const Planes& y, int yc0, const
 
 // ---- ecapa_train.cu / train_kernels.cu ---------------------------------------------------------------
 struct Trainer;
-int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out);
+int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, int classifier_type, int num_blocks, int inter_dim, Trainer** out);
 void trainer_destroy(Trainer* t);
 int64_t trainer_param_count(const Trainer* t);
 int64_t trainer_stat_count(const Trainer* t);
@@ -461,6 +461,12 @@ int aam_forward(const float* emb, const float* W, const int64_t* labels, int B, 
 int aam_backward(const float* emb, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin,
                  float scale, int easy_margin, float label_smoothing, float* d_emb, float* d_W, void* ws, size_t ws_bytes,
                  cudaStream_t st);
+// The Linear output layer (fc.py:37-38, 50-51) in front of the same loss heads: logits = H W + b, H [B,D], W [D,S], b [S].  Takes
+// the workspace of aam_forward / aam_backward (aam_workspace_bytes(B, D, S)).  Heads that take sqrt(1 - z^2) of the logits are refused.
+int linear_head_forward(const float* H, const float* W, const float* bias, const int64_t* labels, int B, int D, int S, float margin, float scale,
+                        int easy_margin, float label_smoothing, float* logits, float* loss, void* ws, size_t ws_bytes, cudaStream_t st);
+int linear_head_backward(const float* H, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin, float scale,
+                         int easy_margin, float label_smoothing, float* d_H, float* d_W, float* d_bias, void* ws, size_t ws_bytes, cudaStream_t st);
 
 // ---- speaker_index.cu ---------------------------------------------------------------------------------
 size_t speaker_index_bytes(int U, int D);

@@ -1,7 +1,8 @@
 // ECAPA-TDNN training step: train-mode forward, AAM-softmax loss, full backward into one flat gradient buffer.
 // Reference: ppvector/trainer.py:206-229 (forward -> loss -> backward -> optimizer.step), ppvector/models/ecapa_tdnn.py:245-276,
 // ppvector/models/utils.py:96-148 (TDNNBlock = BatchNorm(ReLU(conv)), BatchNorm in TRAIN mode: batch statistics over all
-// B*T frames, momentum 0.9), ppvector/models/pooling.py:86-125, ppvector/models/fc.py:41-53, ppvector/loss/aamloss.py:28-53.
+// B*T frames, momentum 0.9), ppvector/models/pooling.py:86-125, ppvector/models/fc.py:6-90 (DenseLayer blocks, Cosine or Linear output
+// layer), ppvector/loss/aamloss.py:28-53.
 // lengths = None, as the reference trainer calls the model (trainer.py:210).
 //
 // Parameters, gradients and BatchNorm running statistics live in three caller-owned flat fp32 buffers (ppv_trainer_bind) laid
@@ -67,6 +68,10 @@ struct TrBuffers {
     size_t part_elems = 0;
     float* aam_ws = nullptr;
     size_t aam_ws_bytes = 0;
+    // classifier blocks (one entry per block, none without them): dense output z, BatchNorm output h (the block's output), its batch
+    // mean / rstd, and dL/dh; dcls_z is the dL/dz scratch every block's backward reuses
+    std::vector<float*> cls_z, cls_h, cls_mean, cls_rstd, dcls_h;
+    float* dcls_z = nullptr;
 };
 
 // One readable tap (trainer_read_tap): planes read as fp32 [B, T, cols] from column col0, or `count` fp32 values as stored.  A
@@ -99,6 +104,15 @@ struct Trainer : PlanOwner, EcapaGeometry {
     int c_lin1 = -1, c_att2 = -1;
     int Kp = 0;  // width of the pooled vector and of asp_bn: 2 * C3 (ASP, TSP) or C3 (SAP, TAP)
     int64_t se1_w[3], se1_b[3], se2_w[3], se2_b[3], aspbn_g = 0, aspbn_b = 0, aspbn_rm = 0, aspbn_rv = 0, fc_w = 0, fc_b = 0, cls_w = 0;
+    // the classifier (fc.py:6-53): num_blocks DenseLayers (Conv1D 1x1 + BatchNorm1D, no ReLU), then the Cosine or Linear output layer
+    struct ClsBlock {
+        int in = 0;  // input width: embd_dim for block 0, inter_dim after it
+        int64_t w = 0, b = 0, g = 0, beta = 0, rm = 0, rv = 0;
+    };
+    int cls_type = PPV_CLASSIFIER_COSINE, inter = 0;
+    std::vector<ClsBlock> cls_blocks;
+    int64_t cls_b = -1;  // Linear: classifier.output.bias
+    int head_dim() const { return cls_blocks.empty() ? D : inter; }  // width of the output layer's input
     // plan
     TrBuffers buf;
     std::map<std::string, TrTap> taps;
@@ -127,8 +141,11 @@ static int64_t tr_add(std::map<std::string, std::pair<int64_t, int64_t>>& m, int
     return off;
 }
 
-int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
+int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, int classifier_type, int num_blocks, int inter_dim, Trainer** out) {
     PPV_REQUIRE(cfg && out && num_classes > 1, "trainer_create: bad argument");
+    if (classifier_type != PPV_CLASSIFIER_COSINE && classifier_type != PPV_CLASSIFIER_LINEAR)
+        return fail(PPV_EUNSUPPORTED, "trainer: classifier_type must be PPV_CLASSIFIER_COSINE or PPV_CLASSIFIER_LINEAR");  // fc.py:39-40
+    PPV_REQUIRE(num_blocks >= 0 && (num_blocks == 0 || inter_dim > 0), "trainer: num_blocks >= 0 and inter_dim > 0 required");
     const int C = cfg->channels[0];
     if (cfg->channels[1] != C || cfg->channels[2] != C || cfg->channels[3] != C || cfg->channels[4] != 3 * C)
         return fail(PPV_EUNSUPPORTED, "trainer: channels must be [C,C,C,C,3C]");
@@ -210,7 +227,27 @@ int trainer_create(const ppv_ecapa_cfg* cfg, int num_classes, Trainer** out) {
     t->aspbn_rv = tr_add(t->smap, t->n_stats, bn + "._variance", t->Kp);
     t->fc_w = tr_add(t->pmap, t->n_params, "fc.conv.weight", int64_t(t->D) * t->Kp);
     t->fc_b = tr_add(t->pmap, t->n_params, "fc.conv.bias", t->D);
-    t->cls_w = tr_add(t->pmap, t->n_params, "classifier.weight", int64_t(t->D) * t->S);  // fc.py:30-36: [input_dim, num_speakers]
+    // the classifier in SpeakerIdentification's state_dict order (fc.py:25-38): the blocks, then the output layer
+    t->cls_type = classifier_type;
+    t->inter = num_blocks ? inter_dim : 0;
+    for (int i = 0; i < num_blocks; ++i) {
+        const std::string p = "classifier.blocks." + std::to_string(i);
+        Trainer::ClsBlock k;
+        k.in = i == 0 ? t->D : inter_dim;
+        k.w = tr_add(t->pmap, t->n_params, p + ".linear.weight", int64_t(inter_dim) * k.in);  // Conv1D [inter, in, 1]
+        k.b = tr_add(t->pmap, t->n_params, p + ".linear.bias", inter_dim);
+        k.g = tr_add(t->pmap, t->n_params, p + ".nonlinear.batchnorm.weight", inter_dim);
+        k.beta = tr_add(t->pmap, t->n_params, p + ".nonlinear.batchnorm.bias", inter_dim);
+        k.rm = tr_add(t->smap, t->n_stats, p + ".nonlinear.batchnorm._mean", inter_dim);
+        k.rv = tr_add(t->smap, t->n_stats, p + ".nonlinear.batchnorm._variance", inter_dim);
+        t->cls_blocks.push_back(k);
+    }
+    if (classifier_type == PPV_CLASSIFIER_COSINE) {
+        t->cls_w = tr_add(t->pmap, t->n_params, "classifier.weight", int64_t(t->head_dim()) * t->S);  // fc.py:30-36: [input_dim, num_speakers]
+    } else {
+        t->cls_w = tr_add(t->pmap, t->n_params, "classifier.output.weight", int64_t(t->head_dim()) * t->S);  // nn.Linear: [input_dim, num_speakers]
+        t->cls_b = tr_add(t->pmap, t->n_params, "classifier.output.bias", t->S);
+    }
     *out = t;
     return PPV_OK;
 }
@@ -360,12 +397,22 @@ void tr_carve(const Trainer* t, WsCarver& cv, int B, int T, TrBuffers* f) {
         wmax = std::max(wmax, size_t(w.splits) * w.Mpad * c.taps * c.Cinp);
     }
     f->wpart = f32(wmax);
-    f->aam_ws_bytes = aam_workspace_bytes(B, t->D, t->S);
+    f->aam_ws_bytes = aam_workspace_bytes(B, t->head_dim(), t->S);
     f->aam_ws = static_cast<float*>(cv.take(f->aam_ws_bytes));
     if (t->cfg.pooling == PPV_POOL_SAP) {  // the softmax pooling's [mean | std] and the gradient it reads back (std half: zero)
         f->sap_stats = f32(size_t(B) * 2 * C3);
         f->dsap_stats = f32(size_t(B) * 2 * C3);
     }
+    const size_t nblk = t->cls_blocks.size();
+    for (std::vector<float*>* v : {&f->cls_z, &f->cls_h, &f->cls_mean, &f->cls_rstd, &f->dcls_h}) v->assign(nblk, nullptr);
+    for (size_t i = 0; i < nblk; ++i) {
+        f->cls_z[i] = f32(size_t(B) * t->inter);
+        f->cls_h[i] = f32(size_t(B) * t->inter);
+        f->cls_mean[i] = f32(t->inter);
+        f->cls_rstd[i] = f32(t->inter);
+        f->dcls_h[i] = f32(size_t(B) * t->inter);
+    }
+    if (nblk) f->dcls_z = f32(size_t(B) * t->inter);
 }
 
 // The taps trainer_read_tap serves, by name without the "pad:" prefix and the block suffix.  A buffer the head does not carve
@@ -421,6 +468,11 @@ std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, 
     vec("dg1", &f.dg1, false, size_t(B) * t->se);
     for (const auto& e : NamedVec{{"se_s", f.se_s}, {"se_g2", f.se_g2}}) vec(e.first, e.second, true, size_t(B) * C);
     vec("se_g1", f.se_g1, true, size_t(B) * t->se);
+    for (size_t i = 0; i < t->cls_blocks.size(); ++i) {  // classifier block outputs and their gradients [B, inter_dim]
+        const std::string p = "classifier.blocks." + std::to_string(i);
+        vec(p, &f.cls_h[i], false, size_t(B) * t->inter);
+        vec("g:" + p, &f.dcls_h[i], false, size_t(B) * t->inter);
+    }
     return m;
 }
 
@@ -679,23 +731,64 @@ int Trainer::build_plan(int B, int T, void* ws, size_t ws_bytes, cudaStream_t st
             return tr_bn1d_fwd(x, B, Cn, TR_BN_EPS, TR_BN_MOMENTUM, gamma, beta, y, mean, rstd, run_mean, run_var, r.st);
         });
         dense_fwd(f.pn, Kp, par + t->fc_w, Kp, par + t->fc_b, B, D, Kp, 0, f.emb, D);
-        push("aam_forward", [emb = f.emb, cls_w = par + t->cls_w, B, D, S = t->S, logits = f.cls_logits, loss = f.loss, aam_ws = f.aam_ws,
+    }
+    // classifier blocks (fc.py:27-29, 44-45): h_i = BatchNorm1D(Conv1D_1x1(h_{i-1})) with batch statistics, h_{-1} = emb
+    const int Hd = t->head_dim(), nblk = int(t->cls_blocks.size());
+    const float* head_in = f.emb;
+    for (int i = 0; i < nblk; ++i) {
+        const Trainer::ClsBlock& k = t->cls_blocks[i];
+        dense_fwd(head_in, k.in, par + k.w, k.in, par + k.b, B, t->inter, k.in, 0, f.cls_z[i], t->inter);
+        push("tr_bn1d_fwd", [x = f.cls_z[i], B, Cn = t->inter, gamma = par + k.g, beta = par + k.beta, y = f.cls_h[i], mean = f.cls_mean[i],
+                             rstd = f.cls_rstd[i], run_mean = sta + k.rm, run_var = sta + k.rv](const StepRun& r) {
+            return tr_bn1d_fwd(x, B, Cn, TR_BN_EPS, TR_BN_MOMENTUM, gamma, beta, y, mean, rstd, run_mean, run_var, r.st);
+        });
+        head_in = f.cls_h[i];
+    }
+    // the output layer and the loss head: cosine logits (fc.py:48-49) or Linear logits (fc.py:50-51); the loss reads the logits alone
+    if (t->cls_type == PPV_CLASSIFIER_COSINE) {
+        push("aam_forward", [emb = head_in, cls_w = par + t->cls_w, B, D = Hd, S = t->S, logits = f.cls_logits, loss = f.loss, aam_ws = f.aam_ws,
                              aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
             const PlanInputs& in = r.in;
             return aam_forward(emb, cls_w, in.labels, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, logits, loss, aam_ws,
                                aam_ws_bytes, r.st);
         });
+    } else {
+        push("linear_head_forward", [h = head_in, w = par + t->cls_w, bias = par + t->cls_b, B, Hd, S = t->S, logits = f.cls_logits, loss = f.loss,
+                                     aam_ws = f.aam_ws, aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
+            const PlanInputs& in = r.in;
+            return linear_head_forward(h, w, bias, in.labels, B, Hd, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, logits, loss, aam_ws,
+                                       aam_ws_bytes, r.st);
+        });
     }
 
     // ================================================================= backward
     {
-        // AAM, fc, asp_bn -> dpooled; ASP -> dlogits, dMd
-        push("aam_backward", [emb = f.emb, cls_w = par + t->cls_w, logits = f.cls_logits, B, D, S = t->S, d_emb = f.d_emb, d_cls_w = grd + t->cls_w,
-                              aam_ws = f.aam_ws, aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
-            const PlanInputs& in = r.in;
-            return aam_backward(emb, cls_w, in.labels, logits, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, d_emb, d_cls_w,
-                                aam_ws, aam_ws_bytes, r.st);
-        });
+        // loss head -> the last block's dL/dh (d_emb without blocks); blocks -> d_emb; fc, asp_bn -> dpooled; ASP -> dlogits, dMd
+        float* const d_head = nblk ? f.dcls_h[nblk - 1] : f.d_emb;
+        if (t->cls_type == PPV_CLASSIFIER_COSINE) {
+            push("aam_backward", [emb = head_in, cls_w = par + t->cls_w, logits = f.cls_logits, B, D = Hd, S = t->S, d_emb = d_head,
+                                  d_cls_w = grd + t->cls_w, aam_ws = f.aam_ws, aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
+                const PlanInputs& in = r.in;
+                return aam_backward(emb, cls_w, in.labels, logits, B, D, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, d_emb, d_cls_w,
+                                    aam_ws, aam_ws_bytes, r.st);
+            });
+        } else {
+            push("linear_head_backward", [h = head_in, w = par + t->cls_w, logits = f.cls_logits, B, Hd, S = t->S, d_h = d_head, d_w = grd + t->cls_w,
+                                          d_b = grd + t->cls_b, aam_ws = f.aam_ws, aam_ws_bytes = f.aam_ws_bytes](const StepRun& r) {
+                const PlanInputs& in = r.in;
+                return linear_head_backward(h, w, in.labels, logits, B, Hd, S, in.margin, in.scale, in.easy_margin, in.label_smoothing, d_h, d_w, d_b,
+                                            aam_ws, aam_ws_bytes, r.st);
+            });
+        }
+        for (int i = nblk - 1; i >= 0; --i) {  // BatchNorm over the batch, then the 1x1 conv's dX / dW / db
+            const Trainer::ClsBlock& k = t->cls_blocks[i];
+            push("tr_bn1d_bwd", [dy = f.dcls_h[i], x = f.cls_z[i], B, Cn = t->inter, gamma = par + k.g, mean = f.cls_mean[i], rstd = f.cls_rstd[i],
+                                 dx = f.dcls_z, dgamma = grd + k.g, dbeta = grd + k.beta](const StepRun& r) {
+                return tr_bn1d_bwd(dy, x, B, Cn, gamma, mean, rstd, dx, dgamma, dbeta, r.st);
+            });
+            dense_bwd(f.dcls_z, t->inter, i ? f.cls_h[i - 1] : f.emb, k.in, par + k.w, k.in, B, t->inter, k.in, i ? f.dcls_h[i - 1] : f.d_emb, k.in,
+                      grd + k.w, k.in, grd + k.b);
+        }
         dense_bwd(f.d_emb, D, f.pn, Kp, par + t->fc_w, Kp, B, D, Kp, f.dpn, Kp, grd + t->fc_w, Kp, grd + t->fc_b);
         push("tr_bn1d_bwd", [dy = f.dpn, x = f.pooled, B, Cn = Kp, gamma = par + t->aspbn_g, mean = f.aspbn_mean, rstd = f.aspbn_rstd,
                              dx = f.dpooled, dgamma = grd + t->aspbn_g, dbeta = grd + t->aspbn_b](const StepRun& r) {
@@ -888,7 +981,8 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
 //   fp32 as stored: "asp" (pooled) [B, Kp], "emb" and "d_emb" [B, D], "logits" [B, Tp, C3] (every row), gstat, dgs [B, 2*C3], pn, dpn,
 //     dpooled [B, Kp], rs, rb [B, C3]; SAP: sap_stats (the softmax pooling's [mean | std]) and dsap_stats (the [d mean | 0] its backward
 //     reads) [B, 2*C3]; per block se_s, se_g2 [B, C], se_g1 [B, se]; dg2, ds [B, C] and dg1 [B, se] are scratch that every block's SE
-//     backward overwrites, so they hold block 0's values.
+//     backward overwrites, so they hold block 0's values.  With classifier blocks: "classifier.blocks.<i>" (block i's output) and
+//     "g:classifier.blocks.<i>" (its gradient) [B, inter_dim].
 // Kp = 2*C3 for ASP and TSP, C3 for SAP and TAP.  A head has the taps of the buffers it uses: Aatt, gstat, dgs, rs, rb are ASP's (the last
 // four with global context), A4, logits and the attention gradients ASP's and SAP's.
 // A per-block name without a block suffix reads block 0.

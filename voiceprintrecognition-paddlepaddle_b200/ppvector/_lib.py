@@ -13,6 +13,7 @@ PPV_PREC_BF16X3 = 0
 PPV_PREC_BF16 = 1
 PPV_MODEL_ECAPA_TDNN = 1
 PPV_POOL_ASP, PPV_POOL_SAP, PPV_POOL_TAP, PPV_POOL_TSP = 0, 1, 2, 3
+PPV_CLASSIFIER_COSINE, PPV_CLASSIFIER_LINEAR = 0, 1
 PPV_RES2_CHAIN, PPV_RES2_CHAIN_PAIRED, PPV_RES2_PER_CONV = 0, 1, 2
 
 
@@ -140,6 +141,7 @@ SIGNATURES = {
     "ppv_model_profile_read": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),
     "ppv_trainer_create": (C.c_int, [C.POINTER(EcapaCfg), C.c_int, C.POINTER(_P)]),
+    "ppv_trainer_create_classifier": (C.c_int, [C.POINTER(EcapaCfg), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "ppv_trainer_destroy": (C.c_int, [_P]),
     "ppv_trainer_param_count": (C.c_int64, [_P]),
     "ppv_trainer_stat_count": (C.c_int64, [_P]),

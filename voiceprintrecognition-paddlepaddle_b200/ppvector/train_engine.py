@@ -2,8 +2,9 @@
 
 Owns three flat fp32 CUDA tensors (parameters, gradients, BatchNorm running statistics) plus the two Adam moment tensors;
 ``libppv_b200`` works directly on them (``ppv_trainer_forward_backward``, ``ppv_adam_step``).  Named views follow the
-reference's state_dict (``blocks.1.tdnn1.conv.conv.weight`` ...) plus ``classifier.weight`` [embd_dim, num_speakers]
-(``SpeakerIdentification.weight``, fc.py:30-36).  Data-parallel training is one ``torch.distributed.all_reduce`` over the
+reference's state_dict (``blocks.1.tdnn1.conv.conv.weight`` ...) plus the classifier's tensors under ``classifier.``, named as
+``SpeakerIdentification``'s state_dict (fc.py:6-53): ``classifier.blocks.<i>.linear.weight`` ... for its DenseLayer blocks, then
+``classifier.weight`` [in, num_speakers] (Cosine) or ``classifier.output.weight`` / ``classifier.output.bias`` (Linear).  Data-parallel training is one ``torch.distributed.all_reduce`` over the
 gradient tensor (NCCL), as the reference's ``fleet.distributed_model`` does (trainer.py:318-320).  ECAPA-TDNN only.
 """
 import ctypes as C
@@ -13,16 +14,37 @@ import torch
 from ppvector import _lib
 
 POOLING = {'ASP': _lib.PPV_POOL_ASP, 'SAP': _lib.PPV_POOL_SAP, 'TAP': _lib.PPV_POOL_TAP, 'TSP': _lib.PPV_POOL_TSP}
+CLASSIFIER = {'Cosine': _lib.PPV_CLASSIFIER_COSINE, 'Linear': _lib.PPV_CLASSIFIER_LINEAR}
+
+
+def classifier_shapes(embd_dim, num_speakers, classifier_type='Cosine', num_blocks=0, inter_dim=512):
+    """name -> shape of every classifier tensor, running statistics included, in SpeakerIdentification's state_dict order
+    (fc.py:25-38) under ``classifier.``."""
+    out, d = {}, embd_dim
+    for i in range(num_blocks):
+        p = f'classifier.blocks.{i}.'
+        out[p + 'linear.weight'], out[p + 'linear.bias'] = (inter_dim, d, 1), (inter_dim,)
+        for n in ('weight', 'bias', '_mean', '_variance'):
+            out[p + 'nonlinear.batchnorm.' + n] = (inter_dim,)
+        d = inter_dim
+    if classifier_type == 'Cosine':
+        out['classifier.weight'] = (d, num_speakers)
+    else:
+        out['classifier.output.weight'], out['classifier.output.bias'] = (d, num_speakers), (num_speakers,)
+    return out
 
 
 class TrainEngine:
     def __init__(self, input_size=80, num_speakers=2796, embd_dim=192, channels=(512, 512, 512, 512, 1536), kernel_sizes=(5, 3, 3, 3, 1),
                  dilations=(1, 2, 3, 4, 1), attention_channels=128, res2net_scale=8, se_channels=128, pooling_type='ASP', global_context=True,
-                 device='cuda'):
+                 classifier_type='Cosine', num_blocks=0, inter_dim=512, device='cuda'):
         """pooling_type / global_context: the head, as EcapaTdnn's (ecapa_tdnn.py:212-241): 'ASP' (with or without the global context),
-        'SAP' (attention_channels must be 128), 'TAP' or 'TSP'."""
+        'SAP' (attention_channels must be 128), 'TAP' or 'TSP'.  classifier_type / num_blocks / inter_dim: the classifier, as
+        SpeakerIdentification's (fc.py:6-53): 'Cosine' or 'Linear' output layer after num_blocks DenseLayers of width inter_dim."""
         if pooling_type not in POOLING:
             raise ValueError(f'pooling_type must be one of {sorted(POOLING)} (got {pooling_type})')
+        if classifier_type not in CLASSIFIER:
+            raise ValueError(f'不支持该输出层：{classifier_type}')  # fc.py:39-40
         self.device = torch.device(device)
         lib = _lib.load()
         cfg = _lib.EcapaCfg()
@@ -33,9 +55,12 @@ class TrainEngine:
         cfg.attention_channels, cfg.res2net_scale, cfg.se_channels = attention_channels, res2net_scale, se_channels
         cfg.pooling, cfg.global_context = POOLING[pooling_type], int(bool(global_context))
         self.num_speakers, self.embd_dim, self.input_size = num_speakers, embd_dim, input_size
+        self.classifier_type, self.num_blocks, self.inter_dim = classifier_type, int(num_blocks), int(inter_dim)
+        self.classifier_shapes = classifier_shapes(embd_dim, num_speakers, classifier_type, self.num_blocks, self.inter_dim)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(lib.ppv_trainer_create(C.byref(cfg), num_speakers, C.byref(self._h)), 'ppv_trainer_create')
+            _lib.check(lib.ppv_trainer_create_classifier(C.byref(cfg), num_speakers, CLASSIFIER[classifier_type], self.num_blocks, self.inter_dim,
+                                                         C.byref(self._h)), 'ppv_trainer_create_classifier')
             n, ns = lib.ppv_trainer_param_count(self._h), lib.ppv_trainer_stat_count(self._h)
             self.params = torch.zeros(n, dtype=torch.float32, device=self.device)
             self.grads = torch.zeros(n, dtype=torch.float32, device=self.device)
@@ -78,7 +103,8 @@ class TrainEngine:
         return v.view(shape) if shape is not None else v
 
     def load_state_dict(self, state, classifier_weight=None):
-        """state: name -> tensor with the reference's names and shapes (backbone); classifier_weight [embd_dim, num_speakers]."""
+        """state: name -> tensor with the reference's names and shapes (backbone, and classifier tensors under ``classifier.``);
+        classifier_weight: the cosine classifier's weight [embd_dim, num_speakers]."""
         for name, t in state.items():
             self.view(name).copy_(torch.as_tensor(t).to(torch.float32).reshape(-1))
         if classifier_weight is not None:
@@ -90,7 +116,8 @@ class TrainEngine:
 
     # ---- step --------------------------------------------------------------------------------------------------
     def forward_backward(self, features, labels, margin=0.2, scale=32.0, easy_margin=False, label_smoothing=0.0, return_logits=False):
-        """features [B,T,F] float32 CUDA, labels [B] int64 -> loss (0-dim CUDA tensor) [, cosine logits [B,S]]; fills ``grads``."""
+        """features [B,T,F] float32 CUDA, labels [B] int64 -> loss (0-dim CUDA tensor) [, the classifier's logits [B,S]: cosines, or the
+        raw h W + b of a Linear classifier]; fills ``grads``."""
         _lib.require_cuda(features, 'features')
         x = features.to(torch.float32).contiguous()
         y = labels.to(device=x.device, dtype=torch.int64).contiguous()

@@ -5,8 +5,9 @@ return values; featurisation, the backbone, the trial x enrol cosine matrix and 
 through libppv_b200; with the optional ``dataset_conf.eval_conf.score_norm`` key the matrix is AS-normalised against a cohort list first
 (ppvector/metric/score_norm.py).  ``train`` (trainer.py:281-365 with the step of :206-229) runs the CUDA training step of
 ``ppvector.train_engine.TrainEngine`` (train-mode forward, AAM loss, backward, one gradient all-reduce over NCCL, Adam) with the
-reference's schedules; it is implemented for EcapaTdnn with any pooling head (ASP with or without the global context, SAP, TAP, TSP)
-+ AAMLoss + Adam + WarmupCosineSchedulerLR (configs/ecapa_tdnn.yml) and raises for other combinations.  Checkpoints follow the
+reference's schedules; it is implemented for EcapaTdnn with any pooling head (ASP with or without the global context, SAP, TAP, TSP),
+either classifier (Cosine or Linear, with any number of DenseLayer blocks) + AAMLoss + Adam + WarmupCosineSchedulerLR
+(configs/ecapa_tdnn.yml) and raises for other combinations.  Checkpoints follow the
 reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}`` with best-EER tracking, optimizer state and ``model.state``) and ``resume_model`` / an existing ``last_model`` restore the weights, the Adam
 moments, the step counters of both schedules and the epoch.  VisualDL logging is out of scope."""
 import os
@@ -27,6 +28,37 @@ from ppvector.metric.score_norm import as_norm, cohort_stats, score_norm_config,
 from ppvector.models import build_model
 from ppvector.utils.checkpoint import find_resume_dir, load_checkpoint_dir, load_state_dict_file, save_checkpoint
 from ppvector.utils.utils import dict_to_object, print_arguments
+
+
+def init_classifier(shapes):
+    """SpeakerIdentification's initial tensors (fc.py:25-38) with Paddle's default initialisers, in state_dict order: a block's Conv1D
+    weight Normal(0, sqrt(2 / fan_in)) and bias 0; its BatchNorm1D weight 1, bias 0, running mean 0, running variance 1; the output
+    weight Xavier uniform, a Linear bias 0.  Draws from torch's global generator."""
+    out = {}
+    for name, shape in shapes.items():
+        if name.endswith('linear.weight'):
+            out[name] = torch.randn(shape) * (2.0 / (shape[1] * shape[2])) ** 0.5
+        elif name in ('classifier.weight', 'classifier.output.weight'):
+            out[name] = torch.nn.init.xavier_uniform_(torch.empty(shape))  # fc.py:34-36 / nn.Linear
+        elif name.endswith(('batchnorm.weight', '_variance')):
+            out[name] = torch.ones(shape)
+        else:
+            out[name] = torch.zeros(shape)
+    return out
+
+
+def check_classifier_keys(loaded, shapes, path):
+    """Refuses a checkpoint whose classifier tensors (``classifier.<name>``) are not exactly the configured classifier's; one with no
+    classifier tensor (a backbone alone) passes."""
+    if not loaded:
+        return
+    missing = sorted(set(shapes) - set(loaded))
+    unexpected = sorted(set(loaded) - set(shapes))
+    wrong = sorted(k for k in set(loaded) & set(shapes) if tuple(np.shape(np.asarray(loaded[k]))) != tuple(shapes[k]))
+    if missing or unexpected or wrong:
+        fmt = lambda ks: [('1.' + k[len('classifier.'):]) for k in ks]  # noqa: E731
+        raise ValueError(f'{path}: the checkpoint\'s classifier does not match model_conf.classifier; missing keys {fmt(missing)}, '
+                         f'unexpected keys {fmt(unexpected)}, keys of another shape {fmt(wrong)}')
 
 
 class PPVectorTrainer(object):
@@ -189,10 +221,21 @@ class PPVectorTrainer(object):
         num_speakers = int(cf.model_conf.classifier.num_speakers)
         backbone = build_model(input_size=fz.feature_dim, configs=cf)  # random init with the mirror's initialisers, names = state_dict
         cls_conf = dict(cf.model_conf.get('classifier', {}))
-        if cls_conf.get('classifier_type', 'Cosine') != 'Cosine' or int(cls_conf.get('num_blocks', 0)) != 0:
-            raise NotImplementedError('the CUDA training step implements classifier_type="Cosine", num_blocks=0')
-        cls_K = int(cls_conf.get('K', 1))  # fc.py:33: K sub-centres per class (SubCenterLoss); the classifier has num_speakers * K columns
-        loss_K = int((cf.loss_conf.get('loss_args', {}) or {}).get('K', 3)) if cf.loss_conf.get('loss', 'AAMLoss') == 'SubCenterLoss' else 1
+        cls_type = cls_conf.get('classifier_type', 'Cosine')
+        if cls_type not in ('Cosine', 'Linear'):
+            raise ValueError(f'不支持该输出层：{cls_type}')  # fc.py:39-40
+        num_blocks, inter_dim = int(cls_conf.get('num_blocks', 0)), int(cls_conf.get('inter_dim', 512))
+        loss_name = cf.loss_conf.get('loss', 'AAMLoss')
+        loss_args = dict(cf.loss_conf.get('loss_args', {}) or {})
+        if cls_type == 'Linear' and (loss_name in ('AAMLoss', 'SubCenterLoss') or
+                                     (loss_name == 'SphereFace2' and loss_args.get('margin_type', 'C') == 'A')):
+            # aamloss.py / subcenterloss.py / sphereface2.py (type A) take sqrt(1 - z^2) of the logits: NaN once a Linear logit leaves [-1, 1]
+            raise NotImplementedError(f'{loss_name}{" (margin_type A)" if loss_name == "SphereFace2" else ""} reads the logits as cosines '
+                                      f'(sqrt(1 - z^2)) and cannot train a Linear classifier; use classifier_type Cosine, or CELoss / AMLoss / '
+                                      f'ARMLoss / SphereFace2 with margin_type C')
+        # fc.py:33: K sub-centres per class (SubCenterLoss); the cosine classifier has num_speakers * K columns, a Linear one ignores K
+        cls_K = int(cls_conf.get('K', 1)) if cls_type == 'Cosine' else 1
+        loss_K = int(loss_args.get('K', 3)) if loss_name == 'SubCenterLoss' else 1
         if cls_K != loss_K:
             raise ValueError(f'classifier K={cls_K} and loss K={loss_K} differ (SubCenterLoss needs model_conf.classifier.K == loss_args.K)')
         num_classes = num_speakers
@@ -200,7 +243,7 @@ class PPVectorTrainer(object):
         engine_args = {k: model_args[k] for k in ('channels', 'kernel_sizes', 'dilations', 'attention_channels', 'res2net_scale', 'se_channels',
                                                   'pooling_type', 'global_context') if k in model_args}
         engine = TrainEngine(input_size=fz.feature_dim, num_speakers=num_speakers, embd_dim=model_args.get('embd_dim', 192), device=self.device,
-                             **engine_args)
+                             classifier_type=cls_type, num_blocks=num_blocks, inter_dim=inter_dim, **engine_args)
         if cf.train_conf.get('enable_amp', False):
             # reference trainer.py:167, 209-229: auto_cast(level='O1') + GradScaler(1024).  Here: single-pass bf16 GEMM operands, everything else
             # fp32; bf16 has fp32's exponent range, so no loss scaling (nothing to unscale, no skipped steps)
@@ -208,8 +251,8 @@ class PPVectorTrainer(object):
             logger.info('enable_amp: bf16 operands in every GEMM of the step, fp32 accumulation / BatchNorm / loss / master weights')
         shapes = {k: tuple(v.shape) for k, v in backbone.state_dict().items()}
         sd = {k: v for k, v in backbone.state_dict().items()}
-        cls_w = torch.empty(engine.embd_dim, num_speakers)
-        torch.nn.init.xavier_uniform_(cls_w)  # fc.py:34-36
+        cls_shapes = engine.classifier_shapes
+        sd.update(init_classifier(cls_shapes))
         resume_dir = find_resume_dir(cf, save_model_path, resume_model)
         opt_state, run_state = None, {}
         for path, is_resume in ((pretrained_model, False), (resume_dir, True)):
@@ -219,12 +262,15 @@ class PPVectorTrainer(object):
                 loaded, opt_state, run_state = load_checkpoint_dir(path)
             else:
                 loaded = load_state_dict_file(path)
+            # Sequential(backbone, classifier) keys: "1.<name>" is the classifier's "classifier.<name>" (checked whole before anything loads)
+            cls_loaded = {'classifier.' + (k[2:] if k.startswith('1.') else k[len('classifier.'):]): v for k, v in loaded.items()
+                          if k.startswith(('1.', 'classifier.'))}
+            check_classifier_keys(cls_loaded, cls_shapes, path)
             for k, v in loaded.items():
-                if k.startswith('1.') or k == 'classifier.weight':
-                    cls_w = torch.as_tensor(np.asarray(v))
-                else:
+                if not k.startswith(('1.', 'classifier.')):
                     sd[k[2:] if k.startswith('0.') else k] = torch.as_tensor(np.asarray(v))
-        engine.load_state_dict(sd, cls_w)
+            sd.update({k: torch.as_tensor(np.asarray(v)) for k, v in cls_loaded.items()})
+        engine.load_state_dict(sd)
         last_epoch, best_eer = 0, 1.0
         if opt_state is not None:  # checkpoint.py:64-85: optimizer state, epoch counter, best EER
             engine.exp_avg.copy_(opt_state['exp_avg'])
@@ -257,9 +303,9 @@ class PPVectorTrainer(object):
 
         def checkpoint(epoch_no, best):
             self._state_dict = {k: v.cpu().numpy() for k, v in engine.state_dict(shapes).items()}
-            # keys as in the reference's Sequential(backbone, classifier) checkpoint: "0.<backbone tensor>", "1.weight"
+            # keys as in the reference's Sequential(backbone, classifier) checkpoint: "0.<backbone tensor>", "1.<classifier tensor>"
             ckpt = {'0.' + k: torch.from_numpy(v) for k, v in self._state_dict.items()}
-            ckpt['1.weight'] = engine.view('classifier.weight', (engine.embd_dim, num_speakers)).detach().cpu().clone()
+            ckpt.update({'1.' + k[len('classifier.'):]: v.cpu() for k, v in engine.state_dict(cls_shapes).items()})
             opt = {'exp_avg': engine.exp_avg.detach().cpu(), 'exp_avg_sq': engine.exp_avg_sq.detach().cpu(), 'step_count': engine.step_count,
                    'last_epoch': epoch_no, 'scheduler_last_epoch': getattr(scheduler, 'last_epoch', None),
                    'margin_step': getattr(margin_scheduler, 'current_step', None)}
