@@ -502,6 +502,18 @@ size_t ppv_aam_workspace_bytes(int B, int D, int S);
 int ppv_aam_backward(const float* emb, const float* W, const int64_t* labels, const float* logits, int B, int D,
                      int S, float margin, float scale, int easy_margin, float label_smoothing, float* d_emb,
                      float* d_W, void* ws, size_t ws_bytes, void* stream);
+/* Linear classifier + loss head (ppvector/models/fc.py:37-38, 50-51: logits = H @ W + b, no normalisation; H [B,D], W [D,S], b [S]),
+ * the output layer of the ECAPA-TDNN trainer's Linear classifier.  The same loss heads run on the raw logits; only those defined for
+ * any real logit are accepted: PPV_HEAD_CE, PPV_HEAD_AM, PPV_HEAD_ARM and PPV_HEAD_SPHEREFACE2 type C (the cosine-only heads return
+ * PPV_EUNSUPPORTED).  D <= 1536.  logits [B,S] receives H @ W + b; loss is a device scalar.
+ * ws: ppv_aam_workspace_bytes(B, D, S) bytes, 256-byte aligned. */
+int ppv_linear_head_forward(const float* H, const float* W, const float* bias, const int64_t* labels, int B, int D, int S, float margin,
+                            float scale, int easy_margin, float label_smoothing, float* logits, float* loss, void* ws, size_t ws_bytes,
+                            void* stream);
+/* Gradients of the mean loss w.r.t. H [B,D], W [D,S] and b [S]; uses logits from ppv_linear_head_forward. */
+int ppv_linear_head_backward(const float* H, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin,
+                             float scale, int easy_margin, float label_smoothing, float* d_H, float* d_W, float* d_bias, void* ws,
+                             size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Test hook for the tensor-core GEMM (not a reference entry point): out[M,N] = A[M,K] * W[N,K]^T

@@ -116,7 +116,10 @@ def margin_head_loss(logits: torch.Tensor, labels: torch.Tensor, kind: str, marg
         else:
             zp, zn = scale * (g(logits) - margin), scale * (g(logits) + margin)
         tm = F.one_hot(labels, logits.shape[1]).to(logits.dtype)
-        return (tm * lam * F.softplus(-zp) + (1 - tm) * (1 - lam) * F.softplus(zn)).sum(1).mean()
+        # the reference's log(1 + exp(x)): torch's default softplus is x itself past 20, exp(-x) (2e-9 at 20) away in value and slope;
+        # past 50 that gap is below fp64's resolution of x
+        sp = lambda x: F.softplus(x, threshold=50.0)  # noqa: E731
+        return (tm * lam * sp(-zp) + (1 - tm) * (1 - lam) * sp(zn)).sum(1).mean()
     if kind == "CE":
         pred = logits
     else:

@@ -141,9 +141,8 @@ __device__ __forceinline__ float class_cosine(const float* __restrict__ c, int c
 // cosines (cos(theta + m) with the same th / mmm fallback on the target, cos(theta - m) on the others).  Entry loss:
 // target lambda * log(1 + exp(-z_p)), others (1 - lambda) * log(1 + exp(z_n)); the loss's bias parameter is created at 0 and is not
 // handed to the optimizer in the reference (trainer.py:186-190 passes model.parameters() only), so it stays 0.
-// kRaw: the logits are a Linear layer's, any real value: g is the plain polynomial (z < -1 included); otherwise they are cosines and
-// (z + 1) / 2 is clamped at 0 against rounding.
-template <bool kRaw>
+// g is the plain polynomial for every z, as in the reference (sphereface2.py:40-42): a Linear layer's logits go below -1, and so does type
+// A's fallback c - mmm on the target (c <= th gives c - mmm <= -1), so the base (z + 1) / 2 is negative by design there.
 __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a, int t, float lambda, float cos_m, float sin_m, float th,
                                            float mmm, float margin, float scale, float* dl_dc) {
     float inner = c, dinner = 1.f, shift = 0.f;
@@ -165,7 +164,7 @@ __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a,
         shift = is_target ? -margin : margin;
     }
     const float h = 0.5f * (inner + 1.f);
-    const float hp = powf(kRaw ? h : fmaxf(h, 0.f), float(t - 1));  // ((z + 1) / 2)^(t - 1); t - 1 is integral, so a negative h is exact
+    const float hp = powf(h, float(t - 1));  // ((z + 1) / 2)^(t - 1); t - 1 is integral, so powf is exact for a negative h too
     const float g = 2.f * hp * h - 1.f;
     const float dg = float(t) * hp * dinner;  // d g / d c
     const float z = scale * (g + shift);
@@ -177,12 +176,11 @@ __device__ __forceinline__ float sf2_entry(float c, bool is_target, bool type_a,
     return w * sp;
 }
 
-// one block per row: loss_b and (optionally) G[b,s] = d loss / d cos[b,s].  S = classes, K = sub-centres per class (1: plain heads);
-// logits and G have S * K columns.  kRaw: Linear logits (see sf2_entry).
-template <bool kRaw>
-__device__ __forceinline__ void row_loss_body(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m,
-                                         float sin_m, float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss,
-                                         float* __restrict__ G, float margin) {
+// one block per row: loss_b and (optionally) G[b,s] = d loss / d logit[b,s].  S = classes, K = sub-centres per class (1: plain heads);
+// logits and G have S * K columns.  The same kernel reads a Linear layer's raw logits (K = 1).
+__global__ void __launch_bounds__(256)
+    aam_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m, float sin_m,
+                   float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss, float* __restrict__ G, float margin) {
     __shared__ float s_red[8];
     const int b = blockIdx.x;
     const int64_t label = labels[b];
@@ -194,7 +192,7 @@ __device__ __forceinline__ void row_loss_body(const float* __restrict__ logits, 
         const float invB = 1.f / float(B);
         for (int s = threadIdx.x; s < S; s += blockDim.x) {
             float d;
-            acc += sf2_entry<kRaw>(c[s], s == label, type_a, t, ls, cos_m, sin_m, th, mmm, margin, scale, &d);
+            acc += sf2_entry(c[s], s == label, type_a, t, ls, cos_m, sin_m, th, mmm, margin, scale, &d);
             if (G) G[int64_t(b) * S + s] = d * invB;
         }
         acc = block_reduce(acc, s_red, false);
@@ -233,17 +231,6 @@ __device__ __forceinline__ void row_loss_body(const float* __restrict__ logits, 
             for (int k = 0; k < K; ++k) G[(int64_t(b) * S + s) * K + k] = k == arg ? (p - t) * invB * d : 0.f;
         }
     }
-}
-__global__ void __launch_bounds__(256)
-    aam_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, int K, float cos_m, float sin_m,
-                   float th, float mmm, int easy, float scale, float ls, float* __restrict__ row_loss_out, float* __restrict__ G, float margin) {
-    row_loss_body<false>(logits, labels, B, S, K, cos_m, sin_m, th, mmm, easy, scale, ls, row_loss_out, G, margin);
-}
-// the same for the raw logits of a Linear classifier (K = 1)
-__global__ void __launch_bounds__(256)
-    lin_row_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B, int S, float cos_m, float sin_m, float th,
-                   float mmm, int easy, float scale, float ls, float* __restrict__ row_loss_out, float* __restrict__ G, float margin) {
-    row_loss_body<true>(logits, labels, B, S, 1, cos_m, sin_m, th, mmm, easy, scale, ls, row_loss_out, G, margin);
 }
 __global__ void aam_mean_kernel(const float* __restrict__ row_loss, int B, float* __restrict__ loss) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -381,7 +368,7 @@ int aam_backward(const float* emb, const float* W, const int64_t* labels, const 
 
 // ------------------------------------------------------------------------------------------------ Linear output layer
 // fc.py:37-38, 50-51: logits = H @ W + b with W [D, S] (Paddle's Linear layout, the one the cosine head reads) and b [S], no
-// normalisation.  The same loss heads then run on the raw logits (lin_row_kernel: aam_row_kernel's body).  Every product below is a fixed-order fp32
+// normalisation.  The same loss heads then run on the raw logits (aam_row_kernel with K = 1).  Every product below is a fixed-order fp32
 // loop: no atomics, the same bits on every run.
 constexpr int LIN_ROWS = 8;    // rows of H (or of G) one thread carries: W is read once per LIN_ROWS rows
 constexpr int LIN_DCHUNK = 16;  // dW: columns of H one thread carries
@@ -485,8 +472,8 @@ int linear_head_forward(const float* H, const float* W, const float* bias, const
     PPV_LAUNCH_OK("lin_logits_kernel");
     float cm, sm, th, mmm;
     margin_consts(margin, &cm, &sm, &th, &mmm);
-    lin_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, nullptr, margin);
-    PPV_LAUNCH_OK("lin_row_kernel");
+    aam_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, 1, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, nullptr, margin);
+    PPV_LAUNCH_OK("aam_row_kernel");
     aam_mean_kernel<<<1, 32, 0, st>>>(w.row_loss, B, loss);
     PPV_LAUNCH_OK("aam_mean_kernel");
     return PPV_OK;
@@ -505,8 +492,8 @@ int linear_head_backward(const float* H, const float* W, const int64_t* labels, 
     carve_aam(cv, B, D, S, &w);
     float cm, sm, th, mmm;
     margin_consts(margin, &cm, &sm, &th, &mmm);
-    lin_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, w.G, margin);
-    PPV_LAUNCH_OK("lin_row_kernel(bwd)");
+    aam_row_kernel<<<B, 256, 0, st>>>(logits, labels, B, S, 1, cm, sm, th, mmm, kind, scale, label_smoothing, w.row_loss, w.G, margin);
+    PPV_LAUNCH_OK("aam_row_kernel(bwd)");
     lin_dh_kernel<<<dim3((D + 7) / 8, (B + LIN_ROWS - 1) / LIN_ROWS), 256, 0, st>>>(w.G, W, B, D, S, d_H);
     PPV_LAUNCH_OK("lin_dh_kernel");
     lin_dw_kernel<<<dim3((S + 127) / 128, (D + LIN_DCHUNK - 1) / LIN_DCHUNK), 128, 0, st>>>(w.G, H, B, D, S, d_W, d_bias);

@@ -538,6 +538,22 @@ int ppv_aam_backward(const float* emb, const float* W, const int64_t* labels, co
                         static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
+int ppv_linear_head_forward(const float* H, const float* W, const float* bias, const int64_t* labels, int B, int D, int S, float margin,
+                            float scale, int easy_margin, float label_smoothing, float* logits, float* loss, void* ws, size_t ws_bytes,
+                            void* stream) {
+    PPV_GUARD_BEGIN
+    return linear_head_forward(H, W, bias, labels, B, D, S, margin, scale, easy_margin, label_smoothing, logits, loss, ws, ws_bytes,
+                               static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
+int ppv_linear_head_backward(const float* H, const float* W, const int64_t* labels, const float* logits, int B, int D, int S, float margin,
+                             float scale, int easy_margin, float label_smoothing, float* d_H, float* d_W, float* d_bias, void* ws,
+                             size_t ws_bytes, void* stream) {
+    PPV_GUARD_BEGIN
+    return linear_head_backward(H, W, labels, logits, B, D, S, margin, scale, easy_margin, label_smoothing, d_H, d_W, d_bias, ws, ws_bytes,
+                                static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
 
 // ---------------------------------------------------------------- GEMM test hook
 // Both hooks' operands in the workspace, zero-padded: A as planes [2][pad128(M)][Kp], then W as planes [2][pad256(N)][Kp], Kp = pad64(K).

@@ -468,11 +468,13 @@ std::map<std::string, TrTap> tr_tap_table(const Trainer* t, const TrBuffers& f, 
     vec("dg1", &f.dg1, false, size_t(B) * t->se);
     for (const auto& e : NamedVec{{"se_s", f.se_s}, {"se_g2", f.se_g2}}) vec(e.first, e.second, true, size_t(B) * C);
     vec("se_g1", f.se_g1, true, size_t(B) * t->se);
-    for (size_t i = 0; i < t->cls_blocks.size(); ++i) {  // classifier block outputs and their gradients [B, inter_dim]
+    for (size_t i = 0; i < t->cls_blocks.size(); ++i) {  // classifier block outputs, their dense outputs and gradients [B, inter_dim]
         const std::string p = "classifier.blocks." + std::to_string(i);
         vec(p, &f.cls_h[i], false, size_t(B) * t->inter);
+        vec(p + ".z", &f.cls_z[i], false, size_t(B) * t->inter);
         vec("g:" + p, &f.dcls_h[i], false, size_t(B) * t->inter);
     }
+    vec("g:classifier.z", &f.dcls_z, false, size_t(B) * t->inter);
     return m;
 }
 
@@ -981,8 +983,9 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
 //   fp32 as stored: "asp" (pooled) [B, Kp], "emb" and "d_emb" [B, D], "logits" [B, Tp, C3] (every row), gstat, dgs [B, 2*C3], pn, dpn,
 //     dpooled [B, Kp], rs, rb [B, C3]; SAP: sap_stats (the softmax pooling's [mean | std]) and dsap_stats (the [d mean | 0] its backward
 //     reads) [B, 2*C3]; per block se_s, se_g2 [B, C], se_g1 [B, se]; dg2, ds [B, C] and dg1 [B, se] are scratch that every block's SE
-//     backward overwrites, so they hold block 0's values.  With classifier blocks: "classifier.blocks.<i>" (block i's output) and
-//     "g:classifier.blocks.<i>" (its gradient) [B, inter_dim].
+//     backward overwrites, so they hold block 0's values.  With classifier blocks: "classifier.blocks.<i>" (block i's output),
+//     "classifier.blocks.<i>.z" (its dense output, the BatchNorm's input), "g:classifier.blocks.<i>" (dL/d output) and "g:classifier.z"
+//     (the dL/dz scratch every block's BatchNorm backward overwrites, so it holds block 0's) [B, inter_dim].
 // Kp = 2*C3 for ASP and TSP, C3 for SAP and TAP.  A head has the taps of the buffers it uses: Aatt, gstat, dgs, rs, rb are ASP's (the last
 // four with global context), A4, logits and the attention gradients ASP's and SAP's.
 // A per-block name without a block suffix reads block 0.

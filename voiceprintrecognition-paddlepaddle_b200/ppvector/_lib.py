@@ -189,6 +189,10 @@ SIGNATURES = {
                                   _P, _P, _P, C.c_size_t, _P]),
     "ppv_aam_backward": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int,
                                    C.c_float, _P, _P, _P, C.c_size_t, _P]),
+    "ppv_linear_head_forward": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_float,
+                                          _P, _P, _P, C.c_size_t, _P]),
+    "ppv_linear_head_backward": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_float,
+                                           _P, _P, _P, _P, C.c_size_t, _P]),
     "ppv_gemm_test_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "ppv_gemm_bench": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_size_t,
                                  C.POINTER(C.c_float), _P]),
