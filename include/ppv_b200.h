@@ -276,7 +276,7 @@ int ppv_model_profile_read(ppv_model_t* h, double* gemm_ms, double* other_ms, in
  * (coupled L2 weight decay).  Parameters / gradients / BatchNorm running statistics are three caller-owned flat fp32 device
  * buffers; ppv_trainer_lookup gives each state_dict tensor's offset ("blocks.1.tdnn1.conv.conv.weight", ...,
  * "classifier.weight" [embd_dim, num_classes]; "*._mean" / "*._variance" live in the statistics buffer).  Data-parallel
- * training is one all-reduce(sum) over the gradient buffer followed by ppv_adam_step(grad_scale = 1 / nranks)
+ * training is one all-reduce(sum) over the gradient buffer followed by ppv_optimizer_step(grad_scale = 1 / nranks)
  * (the reference's fleet.distributed_model, trainer.py:318-320).
  * ------------------------------------------------------------------------------------------- */
 /* Process-wide: 1 (default) = kernels are launched with programmatic dependent launch (the next kernel of a stream starts its prologue while
@@ -321,6 +321,36 @@ int ppv_trainer_read_tap(ppv_trainer_t* h, const char* name, float* out, size_t 
 /* p -= lr * mhat / (sqrt(vhat) + eps) with g = grads * grad_scale + weight_decay * p; step counts from 1. */
 int ppv_adam_step(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
                   float weight_decay, int64_t step, float grad_scale, void* stream);
+
+/* The optimizers ppvector/optimizer/__init__.py:12-18 builds by name (paddle.optimizer.<optimizer>(**optimizer_args)), as one fused
+ * elementwise step over the flat buffers.  g = grads * grad_scale; weight_decay is coupled L2 except for AdamW:
+ *   PPV_OPT_ADAM      the kernel of ppv_adam_step (bitwise the same); state0 = m, state1 = v
+ *   PPV_OPT_ADAMW     p *= 1 - lr wd, then the Adam update of ppv_adam_step on the undecayed g; state0 = m, state1 = v
+ *   PPV_OPT_SGD       p -= lr (g + wd p); no state
+ *   PPV_OPT_MOMENTUM  g' = g rescale_grad + wd p, v = momentum v + g', p -= lr v (use_nesterov: p -= lr (g' + momentum v)); state0 = v
+ *   PPV_OPT_RMSPROP   g' = g + wd p, ms = rho ms + (1 - rho) g'^2, centered: mg = rho mg + (1 - rho) g';
+ *                     mom = momentum mom + lr g' / sqrt(ms [- mg^2] + epsilon), p -= mom; state0 = ms, state1 = mom, state2 = mg (centered)
+ * ppv_optimizer_state_count(kind, centered) is the number of state buffers (n floats each, zero before the first step) the kind reads:
+ * state buffers beyond it may be NULL; negative for an unknown kind.  step counts from 1 (used by ADAM / ADAMW only).  Buffers whose
+ * addresses are all 16-byte aligned are read and written as float4. */
+#define PPV_OPT_ADAM 0
+#define PPV_OPT_ADAMW 1
+#define PPV_OPT_SGD 2
+#define PPV_OPT_MOMENTUM 3
+#define PPV_OPT_RMSPROP 4
+typedef struct ppv_optim_args {
+    float lr;
+    float weight_decay;
+    float beta1, beta2, epsilon; /* ADAM / ADAMW: epsilon also for RMSPROP */
+    float momentum;              /* MOMENTUM / RMSPROP */
+    float rho;                   /* RMSPROP */
+    float rescale_grad;          /* MOMENTUM */
+    int use_nesterov;            /* MOMENTUM */
+    int centered;                /* RMSPROP */
+} ppv_optim_args;
+int ppv_optimizer_state_count(int kind, int centered);
+int ppv_optimizer_step(int kind, float* params, const float* grads, float* state0, float* state1, float* state2, int64_t n,
+                       const ppv_optim_args* args, int64_t step, float grad_scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Cosine scoring.  Replaces ppvector/predict.py:279-283 (contrast), :173-187 (retrieval:

@@ -505,6 +505,14 @@ int ppv_adam_step(float* params, const float* grads, float* m, float* v, int64_t
     return adam_step(params, grads, m, v, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
+int ppv_optimizer_state_count(int kind, int centered) { return optimizer_state_count(kind, centered); }
+int ppv_optimizer_step(int kind, float* params, const float* grads, float* state0, float* state1, float* state2, int64_t n,
+                       const ppv_optim_args* args, int64_t step, float grad_scale, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(args, "ppv_optimizer_step: null args");
+    return optimizer_step(kind, params, grads, state0, state1, state2, n, *args, step, grad_scale, static_cast<cudaStream_t>(stream));
+    PPV_GUARD_END
+}
 
 // ---------------------------------------------------------------- cosine scoring
 size_t ppv_cosine_workspace_bytes(int M, int N, int D) { return cosine_workspace_bytes(M, N, D); }

@@ -449,6 +449,9 @@ int trainer_forward_backward(Trainer* t, const float* feat, const int64_t* label
 int trainer_read_tap(Trainer* t, const char* name, float* out, size_t out_elems, cudaStream_t st);
 int adam_step(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
               int64_t step, float grad_scale, cudaStream_t st);
+int optimizer_state_count(int kind, int centered);
+int optimizer_step(int kind, float* params, const float* grads, float* s0, float* s1, float* s2, int64_t n, const ppv_optim_args& args,
+                   int64_t step, float grad_scale, cudaStream_t st);
 
 // ---- cosine.cu / aam.cu -----------------------------------------------------------------------------
 size_t cosine_workspace_bytes(int M, int N, int D);

@@ -652,6 +652,86 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     p[i] -= lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
 }
 
+// ---------------------------------------------------------------------------------------------- AdamW / SGD / Momentum / RMSProp
+// paddle.optimizer.<name>(**optimizer_args) (optimizer/__init__.py:12-18), Paddle 2.x update rules (include/ppv_b200.h: PPV_OPT_*).  One
+// elementwise update per parameter; HBM-bound: (2 + 2 * states) floats moved per parameter.
+struct OptimStep {
+    float lr, wd, grad_scale, decay;  // decay = 1 - lr wd (AdamW)
+    float beta1, beta2, eps, bc1, bc2;
+    float mu, rho, rescale;
+    int nesterov, centered;
+};
+
+template <int KIND>
+__device__ __forceinline__ void optim_update(float& p, float g, float& s0, float& s1, float& s2, const OptimStep& a) {
+    g *= a.grad_scale;
+    if constexpr (KIND == PPV_OPT_SGD) {
+        p -= a.lr * (g + a.wd * p);
+    } else if constexpr (KIND == PPV_OPT_MOMENTUM) {
+        const float gd = g * a.rescale + a.wd * p;
+        s0 = a.mu * s0 + gd;
+        p -= a.nesterov ? a.lr * (gd + a.mu * s0) : a.lr * s0;
+    } else if constexpr (KIND == PPV_OPT_ADAMW) {
+        p *= a.decay;
+        s0 = a.beta1 * s0 + (1.f - a.beta1) * g;
+        s1 = a.beta2 * s1 + (1.f - a.beta2) * g * g;
+        p -= a.lr * (s0 / a.bc1) / (sqrtf(s1 / a.bc2) + a.eps);
+    } else {  // PPV_OPT_RMSPROP: epsilon inside the square root, lr inside the momentum buffer
+        const float gd = g + a.wd * p;
+        s0 = a.rho * s0 + (1.f - a.rho) * gd * gd;
+        float ms = s0;
+        if (a.centered) {
+            s2 = a.rho * s2 + (1.f - a.rho) * gd;
+            ms -= s2 * s2;
+        }
+        s1 = a.mu * s1 + a.lr * gd / sqrtf(ms + a.eps);
+        p -= s1;
+    }
+}
+
+// State buffers the kind reads and writes: s0 for all but SGD, s1 for AdamW and RMSProp, s2 for centered RMSProp.
+template <int KIND>
+__device__ __forceinline__ bool optim_uses(int k, const OptimStep& a) {
+    return KIND == PPV_OPT_SGD ? false : k == 0 ? true : k == 1 ? KIND != PPV_OPT_MOMENTUM : (KIND == PPV_OPT_RMSPROP && a.centered);
+}
+
+// VEC: every pointer is 16-byte aligned; the first n & ~3 elements go as float4, the tail element by element.  Grid-stride.
+template <int KIND, bool VEC>
+__global__ void __launch_bounds__(256) optim_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ s0,
+                                                    float* __restrict__ s1, float* __restrict__ s2, int64_t n, OptimStep a) {
+    const int64_t stride = int64_t(gridDim.x) * blockDim.x, tid = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    const bool u0 = optim_uses<KIND>(0, a), u1 = optim_uses<KIND>(1, a), u2 = optim_uses<KIND>(2, a);
+    int64_t done = 0;
+    if (VEC) {
+        const int64_t n4 = n >> 2;
+        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int64_t i = tid; i < n4; i += stride) {
+            float4 pv = reinterpret_cast<const float4*>(p)[i];
+            const float4 gv = reinterpret_cast<const float4*>(g)[i];
+            float4 a0 = u0 ? reinterpret_cast<const float4*>(s0)[i] : zero;
+            float4 a1 = u1 ? reinterpret_cast<const float4*>(s1)[i] : zero;
+            float4 a2 = u2 ? reinterpret_cast<const float4*>(s2)[i] : zero;
+            optim_update<KIND>(pv.x, gv.x, a0.x, a1.x, a2.x, a);
+            optim_update<KIND>(pv.y, gv.y, a0.y, a1.y, a2.y, a);
+            optim_update<KIND>(pv.z, gv.z, a0.z, a1.z, a2.z, a);
+            optim_update<KIND>(pv.w, gv.w, a0.w, a1.w, a2.w, a);
+            reinterpret_cast<float4*>(p)[i] = pv;
+            if (u0) reinterpret_cast<float4*>(s0)[i] = a0;
+            if (u1) reinterpret_cast<float4*>(s1)[i] = a1;
+            if (u2) reinterpret_cast<float4*>(s2)[i] = a2;
+        }
+        done = n4 << 2;
+    }
+    for (int64_t i = done + tid; i < n; i += stride) {
+        float pi = p[i], a0 = u0 ? s0[i] : 0.f, a1 = u1 ? s1[i] : 0.f, a2 = u2 ? s2[i] : 0.f;
+        optim_update<KIND>(pi, g[i], a0, a1, a2, a);
+        p[i] = pi;
+        if (u0) s0[i] = a0;
+        if (u1) s1[i] = a1;
+        if (u2) s2[i] = a2;
+    }
+}
+
 }  // namespace
 
 // ================================================================================================ launchers
@@ -804,6 +884,68 @@ int adam_step(float* params, const float* grads, float* m, float* v, int64_t n, 
     adam_kernel<<<unsigned((n + 255) / 256), 256, 0, st>>>(params, grads, m, v, n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale);
     TR_LAUNCH_OK("adam_kernel");
     return PPV_OK;
+}
+
+int optimizer_state_count(int kind, int centered) {
+    switch (kind) {
+        case PPV_OPT_ADAM:
+        case PPV_OPT_ADAMW: return 2;
+        case PPV_OPT_SGD: return 0;
+        case PPV_OPT_MOMENTUM: return 1;
+        case PPV_OPT_RMSPROP: return centered ? 3 : 2;
+        default: return PPV_EINVAL;
+    }
+}
+
+namespace {
+template <int KIND>
+int launch_optim(float* p, const float* g, float* s0, float* s1, float* s2, int64_t n, const OptimStep& a, cudaStream_t st) {
+    const bool vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(s0) |
+                       reinterpret_cast<uintptr_t>(s1) | reinterpret_cast<uintptr_t>(s2)) & 15) == 0;
+    const int64_t items = vec ? std::max<int64_t>(n >> 2, 1) : n;
+    const int grid = int(std::min<int64_t>((items + 255) / 256, int64_t(device_sm_count()) * 8));
+    if (vec)
+        optim_kernel<KIND, true><<<grid, 256, 0, st>>>(p, g, s0, s1, s2, n, a);
+    else
+        optim_kernel<KIND, false><<<grid, 256, 0, st>>>(p, g, s0, s1, s2, n, a);
+    TR_LAUNCH_OK("optim_kernel");
+    return PPV_OK;
+}
+}  // namespace
+
+int optimizer_step(int kind, float* params, const float* grads, float* s0, float* s1, float* s2, int64_t n, const ppv_optim_args& args,
+                   int64_t step, float grad_scale, cudaStream_t st) {
+    const int ns = optimizer_state_count(kind, args.centered);
+    PPV_REQUIRE(ns >= 0, "optimizer_step: kind must be one of PPV_OPT_ADAM / _ADAMW / _SGD / _MOMENTUM / _RMSPROP");
+    PPV_REQUIRE(params && grads && n > 0 && step >= 1, "optimizer_step: bad argument");
+    PPV_REQUIRE((ns < 1 || s0) && (ns < 2 || s1) && (ns < 3 || s2), "optimizer_step: a state buffer the optimizer needs is NULL");
+    if (kind == PPV_OPT_ADAM)
+        return adam_step(params, grads, s0, s1, n, args.lr, args.beta1, args.beta2, args.epsilon, args.weight_decay, step, grad_scale, st);
+    OptimStep a{};
+    a.lr = args.lr;
+    a.wd = args.weight_decay;
+    a.grad_scale = grad_scale;
+    a.decay = float(1.0 - double(args.lr) * double(args.weight_decay));
+    a.beta1 = args.beta1;
+    a.beta2 = args.beta2;
+    a.eps = args.epsilon;
+    a.bc1 = float(1.0 - pow(double(args.beta1), double(step)));
+    a.bc2 = float(1.0 - pow(double(args.beta2), double(step)));
+    a.mu = args.momentum;
+    a.rho = args.rho;
+    a.rescale = args.rescale_grad;
+    a.nesterov = args.use_nesterov != 0;
+    a.centered = args.centered != 0;
+    // the buffers the kind does not read take part in the alignment test as NULL
+    if (ns < 1) s0 = nullptr;
+    if (ns < 2) s1 = nullptr;
+    if (ns < 3) s2 = nullptr;
+    switch (kind) {
+        case PPV_OPT_ADAMW: return launch_optim<PPV_OPT_ADAMW>(params, grads, s0, s1, s2, n, a, st);
+        case PPV_OPT_SGD: return launch_optim<PPV_OPT_SGD>(params, grads, s0, s1, s2, n, a, st);
+        case PPV_OPT_MOMENTUM: return launch_optim<PPV_OPT_MOMENTUM>(params, grads, s0, s1, s2, n, a, st);
+        default: return launch_optim<PPV_OPT_RMSPROP>(params, grads, s0, s1, s2, n, a, st);
+    }
 }
 
 }  // namespace ppv

@@ -15,6 +15,7 @@ PPV_MODEL_ECAPA_TDNN = 1
 PPV_POOL_ASP, PPV_POOL_SAP, PPV_POOL_TAP, PPV_POOL_TSP = 0, 1, 2, 3
 PPV_CLASSIFIER_COSINE, PPV_CLASSIFIER_LINEAR = 0, 1
 PPV_RES2_CHAIN, PPV_RES2_CHAIN_PAIRED, PPV_RES2_PER_CONV = 0, 1, 2
+PPV_OPT_ADAM, PPV_OPT_ADAMW, PPV_OPT_SGD, PPV_OPT_MOMENTUM, PPV_OPT_RMSPROP = 0, 1, 2, 3, 4
 
 
 class PPVError(RuntimeError):
@@ -37,6 +38,12 @@ class EcapaCfg(C.Structure):
                 ("kernel_sizes", C.c_int * 5), ("dilations", C.c_int * 5), ("attention_channels", C.c_int),
                 ("res2net_scale", C.c_int), ("se_channels", C.c_int), ("precision", C.c_int), ("pooling", C.c_int),
                 ("global_context", C.c_int)]
+
+
+class OptimArgs(C.Structure):
+    """ppv_optim_args: the hyper-parameters of one ppv_optimizer_step"""
+    _fields_ = [("lr", C.c_float), ("weight_decay", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("epsilon", C.c_float),
+                ("momentum", C.c_float), ("rho", C.c_float), ("rescale_grad", C.c_float), ("use_nesterov", C.c_int), ("centered", C.c_int)]
 
 
 class ResNetSECfg(C.Structure):
@@ -154,6 +161,8 @@ SIGNATURES = {
                                                C.c_size_t, _P]),
     "ppv_trainer_read_tap": (C.c_int, [_P, C.c_char_p, _P, C.c_size_t, _P]),
     "ppv_adam_step": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, _P]),
+    "ppv_optimizer_state_count": (C.c_int, [C.c_int, C.c_int]),
+    "ppv_optimizer_step": (C.c_int, [C.c_int, _P, _P, _P, _P, _P, C.c_int64, C.POINTER(OptimArgs), C.c_int64, C.c_float, _P]),
     "ppv_cosine_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "ppv_cosine_matrix": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_size_t, _P]),
     "ppv_cosine_pairlist": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, _P]),

@@ -1,7 +1,9 @@
 """TrainEngine -- the CUDA training step behind PPVectorTrainer.train (reference: ppvector/trainer.py:206-229).
 
-Owns three flat fp32 CUDA tensors (parameters, gradients, BatchNorm running statistics) plus the two Adam moment tensors;
-``libppv_b200`` works directly on them (``ppv_trainer_forward_backward``, ``ppv_adam_step``).  Named views follow the
+Owns three flat fp32 CUDA tensors (parameters, gradients, BatchNorm running statistics) plus the state tensors of its optimizer
+(``optim_state``: Adam's and AdamW's two moments ``exp_avg`` / ``exp_avg_sq``, Momentum's ``velocity``, RMSProp's ``mean_square``,
+``moment`` and, centered, ``mean_grad``; none for SGD); ``libppv_b200`` works directly on them (``ppv_trainer_forward_backward``,
+``ppv_optimizer_step``).  Named views follow the
 reference's state_dict (``blocks.1.tdnn1.conv.conv.weight`` ...) plus the classifier's tensors under ``classifier.``, named as
 ``SpeakerIdentification``'s state_dict (fc.py:6-53): ``classifier.blocks.<i>.linear.weight`` ... for its DenseLayer blocks, then
 ``classifier.weight`` [in, num_speakers] (Cosine) or ``classifier.output.weight`` / ``classifier.output.bias`` (Linear).  Data-parallel training is one ``torch.distributed.all_reduce`` over the
@@ -12,6 +14,7 @@ import ctypes as C
 import torch
 
 from ppvector import _lib
+from ppvector.optimizer import OPTIMIZERS, resolve_optimizer
 
 POOLING = {'ASP': _lib.PPV_POOL_ASP, 'SAP': _lib.PPV_POOL_SAP, 'TAP': _lib.PPV_POOL_TAP, 'TSP': _lib.PPV_POOL_TSP}
 CLASSIFIER = {'Cosine': _lib.PPV_CLASSIFIER_COSINE, 'Linear': _lib.PPV_CLASSIFIER_LINEAR}
@@ -37,14 +40,18 @@ def classifier_shapes(embd_dim, num_speakers, classifier_type='Cosine', num_bloc
 class TrainEngine:
     def __init__(self, input_size=80, num_speakers=2796, embd_dim=192, channels=(512, 512, 512, 512, 1536), kernel_sizes=(5, 3, 3, 3, 1),
                  dilations=(1, 2, 3, 4, 1), attention_channels=128, res2net_scale=8, se_channels=128, pooling_type='ASP', global_context=True,
-                 classifier_type='Cosine', num_blocks=0, inter_dim=512, device='cuda'):
+                 classifier_type='Cosine', num_blocks=0, inter_dim=512, optimizer='Adam', optimizer_args=None, device='cuda'):
         """pooling_type / global_context: the head, as EcapaTdnn's (ecapa_tdnn.py:212-241): 'ASP' (with or without the global context),
         'SAP' (attention_channels must be 128), 'TAP' or 'TSP'.  classifier_type / num_blocks / inter_dim: the classifier, as
-        SpeakerIdentification's (fc.py:6-53): 'Cosine' or 'Linear' output layer after num_blocks DenseLayers of width inter_dim."""
+        SpeakerIdentification's (fc.py:6-53): 'Cosine' or 'Linear' output layer after num_blocks DenseLayers of width inter_dim.
+        optimizer / optimizer_args: optimizer_conf's, 'Adam', 'AdamW', 'SGD', 'Momentum' or 'RMSProp' with Paddle's arguments
+        (ppvector.optimizer.resolve_optimizer); optimizer_step applies them."""
         if pooling_type not in POOLING:
             raise ValueError(f'pooling_type must be one of {sorted(POOLING)} (got {pooling_type})')
         if classifier_type not in CLASSIFIER:
             raise ValueError(f'不支持该输出层：{classifier_type}')  # fc.py:39-40
+        self.optimizer, self.optimizer_args = optimizer, resolve_optimizer(optimizer, optimizer_args)
+        self._opt_kind, state_names = OPTIMIZERS[optimizer][:2]
         self.device = torch.device(device)
         lib = _lib.load()
         cfg = _lib.EcapaCfg()
@@ -65,8 +72,9 @@ class TrainEngine:
             self.params = torch.zeros(n, dtype=torch.float32, device=self.device)
             self.grads = torch.zeros(n, dtype=torch.float32, device=self.device)
             self.stats = torch.zeros(ns, dtype=torch.float32, device=self.device)
-            self.exp_avg = torch.zeros(n, dtype=torch.float32, device=self.device)
-            self.exp_avg_sq = torch.zeros(n, dtype=torch.float32, device=self.device)
+            ns = lib.ppv_optimizer_state_count(self._opt_kind, self.optimizer_args.get('centered', 0))
+            self.optim_state = {k: torch.zeros(n, dtype=torch.float32, device=self.device) for k in state_names[:ns]}
+            self.exp_avg, self.exp_avg_sq = self.optim_state.get('exp_avg'), self.optim_state.get('exp_avg_sq')
             _lib.check(lib.ppv_trainer_bind(self._h, _lib.ptr(self.params), _lib.ptr(self.grads), _lib.ptr(self.stats)), 'ppv_trainer_bind')
         self.step_count = 0
         self._ws = None
@@ -96,9 +104,9 @@ class TrainEngine:
         return off.value, numel.value, bool(is_stat.value)
 
     def view(self, name, shape=None, which='param'):
-        """Tensor view of one named tensor: which = 'param' | 'grad' | 'exp_avg' | 'exp_avg_sq' (statistics: 'param')."""
+        """Tensor view of one named tensor: which = 'param' | 'grad' | a name of optim_state, e.g. 'exp_avg' (statistics: 'param')."""
         off, numel, is_stat = self._lookup(name)
-        base = self.stats if is_stat else {'param': self.params, 'grad': self.grads, 'exp_avg': self.exp_avg, 'exp_avg_sq': self.exp_avg_sq}[which]
+        base = self.stats if is_stat else {'param': self.params, 'grad': self.grads, **self.optim_state}[which]
         v = base[off:off + numel]
         return v.view(shape) if shape is not None else v
 
@@ -145,7 +153,7 @@ class TrainEngine:
         return out
 
     def all_reduce_grads(self):
-        """One collective over the flat gradient buffer; returns the scale ppv_adam_step must apply (1 / world size)."""
+        """One collective over the flat gradient buffer; returns the scale the optimizer step must apply (1 / world size)."""
         from ppvector.parallel import allreduce_flat_grads
         return allreduce_flat_grads(self.grads)
 
@@ -155,3 +163,13 @@ class TrainEngine:
             _lib.check(_lib.load().ppv_adam_step(_lib.ptr(self.params), _lib.ptr(self.grads), _lib.ptr(self.exp_avg), _lib.ptr(self.exp_avg_sq),
                                                  self.params.numel(), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay),
                                                  self.step_count, float(grad_scale), _lib.current_stream()), 'ppv_adam_step')
+
+    def optimizer_step(self, lr, grad_scale=1.0):
+        """One step of the engine's optimizer at learning rate lr over the whole parameter buffer; grad_scale multiplies the gradients."""
+        self.step_count += 1
+        args = _lib.OptimArgs(lr=float(lr), **self.optimizer_args)
+        state = [_lib.ptr(t) for t in self.optim_state.values()] + [None] * (3 - len(self.optim_state))
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().ppv_optimizer_step(self._opt_kind, _lib.ptr(self.params), _lib.ptr(self.grads), *state, self.params.numel(),
+                                                      C.byref(args), self.step_count, float(grad_scale), _lib.current_stream()),
+                       'ppv_optimizer_step')

@@ -4,12 +4,12 @@
 return values; featurisation, the backbone, the trial x enrol cosine matrix and EER / minDCF (radix sort + sweep) run on the GPU
 through libppv_b200; with the optional ``dataset_conf.eval_conf.score_norm`` key the matrix is AS-normalised against a cohort list first
 (ppvector/metric/score_norm.py).  ``train`` (trainer.py:281-365 with the step of :206-229) runs the CUDA training step of
-``ppvector.train_engine.TrainEngine`` (train-mode forward, AAM loss, backward, one gradient all-reduce over NCCL, Adam) with the
-reference's schedules; it is implemented for EcapaTdnn with any pooling head (ASP with or without the global context, SAP, TAP, TSP),
-either classifier (Cosine or Linear, with any number of DenseLayer blocks) + AAMLoss + Adam + WarmupCosineSchedulerLR
-(configs/ecapa_tdnn.yml) and raises for other combinations.  Checkpoints follow the
-reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}`` with best-EER tracking, optimizer state and ``model.state``) and ``resume_model`` / an existing ``last_model`` restore the weights, the Adam
-moments, the step counters of both schedules and the epoch.  VisualDL logging is out of scope."""
+``ppvector.train_engine.TrainEngine`` (train-mode forward, AAM loss, backward, one gradient all-reduce over NCCL, the optimizer step)
+with the reference's schedules; it is implemented for EcapaTdnn with any pooling head (ASP with or without the global context, SAP, TAP,
+TSP), either classifier (Cosine or Linear, with any number of DenseLayer blocks) + AAMLoss + Adam, AdamW, SGD, Momentum or RMSProp +
+WarmupCosineSchedulerLR (configs/ecapa_tdnn.yml) and raises for other combinations.  Checkpoints follow the
+reference's directory layout (``<model>_<feature>/{epoch_N,last_model,best_model}`` with best-EER tracking, optimizer state and ``model.state``) and ``resume_model`` / an existing ``last_model`` restore the weights, the optimizer's
+state, the step counters of both schedules and the epoch.  VisualDL logging is out of scope."""
 import os
 
 import numpy as np
@@ -26,7 +26,7 @@ from ppvector.metric.cosine import cosine_matrix
 from ppvector.metric.metrics import compute_dcf, compute_eer, compute_fnr_fpr, eer_mindcf_from_matrix_gpu  # noqa: F401
 from ppvector.metric.score_norm import as_norm, cohort_stats, score_norm_config, speaker_cohort
 from ppvector.models import build_model
-from ppvector.utils.checkpoint import find_resume_dir, load_checkpoint_dir, load_state_dict_file, save_checkpoint
+from ppvector.utils.checkpoint import check_optimizer_state, find_resume_dir, load_checkpoint_dir, load_state_dict_file, save_checkpoint
 from ppvector.utils.utils import dict_to_object, print_arguments
 
 
@@ -182,20 +182,24 @@ class PPVectorTrainer(object):
     def train(self, save_model_path='models/', log_dir='log/', resume_model=None, pretrained_model=None, do_eval=True, max_steps=None):
         """reference: trainer.py:281-365.  ``max_steps`` (extension) stops early -- used by the tests and the bench tool.
         ``pretrained_model`` restores weights only (checkpoint.py:11-42); ``resume_model`` -- or ``<save_model_path>/<model>_<feature>/
-        last_model`` when it exists -- restores weights, Adam moments and step count, both schedules and the epoch (checkpoint.py:45-101)."""
+        last_model`` when it exists -- restores weights, the optimizer's state and step count, both schedules and the epoch
+        (checkpoint.py:45-101); a checkpoint written by another optimizer is refused."""
         import random as _random
 
         import torch.distributed as dist
 
         from ppvector.loss import build_loss
-        from ppvector.optimizer import MarginScheduler, build_lr_scheduler
+        from ppvector.optimizer import MarginScheduler, build_lr_scheduler, resolve_optimizer
         from ppvector.train_engine import TrainEngine
         cf = self.configs
         use_model = cf.model_conf.get('model', 'CAMPPlus')
         if use_model != 'EcapaTdnn':
             raise NotImplementedError(f'training on the H100 path is implemented for EcapaTdnn (got {use_model}); no fallback')
-        if cf.loss_conf.get('loss', 'AAMLoss') not in ('AAMLoss', 'AMLoss', 'ARMLoss', 'CELoss', 'SubCenterLoss', 'SphereFace2') or cf.optimizer_conf.get('optimizer', 'Adam') != 'Adam':
-            raise NotImplementedError('training on the H100 path implements AAMLoss / AMLoss / ARMLoss / CELoss / SubCenterLoss / SphereFace2 + Adam (configs/ecapa_tdnn.yml)')
+        if cf.loss_conf.get('loss', 'AAMLoss') not in ('AAMLoss', 'AMLoss', 'ARMLoss', 'CELoss', 'SubCenterLoss', 'SphereFace2'):
+            raise NotImplementedError('training on the H100 path implements AAMLoss / AMLoss / ARMLoss / CELoss / SubCenterLoss / SphereFace2 (configs/ecapa_tdnn.yml)')
+        # optimizer/__init__.py:12-18: paddle.optimizer.<optimizer>(**optimizer_args), checked here before any work
+        opt_name = cf.optimizer_conf.get('optimizer', 'Adam')
+        opt_args = resolve_optimizer(opt_name, cf.optimizer_conf.get('optimizer_args', {}))
         if cf.dataset_conf.get('is_use_pksampler', False):
             raise NotImplementedError('PKSampler is out of scope of the H100 path')
         model_args = dict(cf.model_conf.get('model_args', {}))
@@ -243,7 +247,8 @@ class PPVectorTrainer(object):
         engine_args = {k: model_args[k] for k in ('channels', 'kernel_sizes', 'dilations', 'attention_channels', 'res2net_scale', 'se_channels',
                                                   'pooling_type', 'global_context') if k in model_args}
         engine = TrainEngine(input_size=fz.feature_dim, num_speakers=num_speakers, embd_dim=model_args.get('embd_dim', 192), device=self.device,
-                             classifier_type=cls_type, num_blocks=num_blocks, inter_dim=inter_dim, **engine_args)
+                             classifier_type=cls_type, num_blocks=num_blocks, inter_dim=inter_dim, optimizer=opt_name, optimizer_args=opt_args,
+                             **engine_args)
         if cf.train_conf.get('enable_amp', False):
             # reference trainer.py:167, 209-229: auto_cast(level='O1') + GradScaler(1024).  Here: single-pass bf16 GEMM operands, everything else
             # fp32; bf16 has fp32's exponent range, so no loss scaling (nothing to unscale, no skipped steps)
@@ -266,6 +271,8 @@ class PPVectorTrainer(object):
             cls_loaded = {'classifier.' + (k[2:] if k.startswith('1.') else k[len('classifier.'):]): v for k, v in loaded.items()
                           if k.startswith(('1.', 'classifier.'))}
             check_classifier_keys(cls_loaded, cls_shapes, path)
+            if is_resume:
+                check_optimizer_state(opt_state, opt_name, engine.optim_state, path)
             for k, v in loaded.items():
                 if not k.startswith(('1.', 'classifier.')):
                     sd[k[2:] if k.startswith('0.') else k] = torch.as_tensor(np.asarray(v))
@@ -273,8 +280,8 @@ class PPVectorTrainer(object):
         engine.load_state_dict(sd)
         last_epoch, best_eer = 0, 1.0
         if opt_state is not None:  # checkpoint.py:64-85: optimizer state, epoch counter, best EER
-            engine.exp_avg.copy_(opt_state['exp_avg'])
-            engine.exp_avg_sq.copy_(opt_state['exp_avg_sq'])
+            for k, t in engine.optim_state.items():
+                t.copy_(opt_state[k])
             engine.step_count = int(opt_state['step_count'])
             last_epoch = int(run_state.get('last_epoch', opt_state.get('last_epoch', 0)))
             best_eer = float(run_state.get('eer', 1.0))
@@ -295,7 +302,7 @@ class PPVectorTrainer(object):
                 scheduler.step()
             if margin_scheduler is not None:
                 margin_scheduler.step(current_step=last_epoch * steps_per_epoch)
-        wd = float(dict(cf.optimizer_conf.get('optimizer_args', {})).get('weight_decay', 0.0))
+        logger.info(f'成功创建优化方法：{opt_name}，参数为：{opt_args}')
         logger.info('训练数据：{}'.format(len(train_dataset)))
         self.train_step, self.train_loss, self.train_acc = last_epoch * steps_per_epoch, None, None
         self.eval_eer = self.eval_min_dcf = self.eval_threshold = None
@@ -306,7 +313,7 @@ class PPVectorTrainer(object):
             # keys as in the reference's Sequential(backbone, classifier) checkpoint: "0.<backbone tensor>", "1.<classifier tensor>"
             ckpt = {'0.' + k: torch.from_numpy(v) for k, v in self._state_dict.items()}
             ckpt.update({'1.' + k[len('classifier.'):]: v.cpu() for k, v in engine.state_dict(cls_shapes).items()})
-            opt = {'exp_avg': engine.exp_avg.detach().cpu(), 'exp_avg_sq': engine.exp_avg_sq.detach().cpu(), 'step_count': engine.step_count,
+            opt = {'optimizer': opt_name, **{k: t.detach().cpu() for k, t in engine.optim_state.items()}, 'step_count': engine.step_count,
                    'last_epoch': epoch_no, 'scheduler_last_epoch': getattr(scheduler, 'last_epoch', None),
                    'margin_step': getattr(margin_scheduler, 'current_step', None)}
             return save_checkpoint(cf, ckpt, opt, save_model_path, epoch_no, eer=self.eval_eer, min_dcf=self.eval_min_dcf,
@@ -322,7 +329,7 @@ class PPVectorTrainer(object):
                 loss, logits = engine.forward_backward(features, label, margin=criterion.margin, scale=criterion.scale,
                                                        easy_margin=criterion.easy_margin, label_smoothing=criterion.label_smoothing,
                                                        return_logits=True)
-                engine.adam_step(lr=scheduler.get_lr(), weight_decay=wd, grad_scale=engine.all_reduce_grads())
+                engine.optimizer_step(lr=scheduler.get_lr(), grad_scale=engine.all_reduce_grads())
                 if cls_K > 1:  # trainer.py:231-234: a class's logit is the max over its sub-centres
                     logits = logits.reshape(logits.shape[0], num_classes, cls_K).amax(2)
                 accs.append((logits.argmax(1).cpu() == label.cpu()).float().mean().item())

@@ -45,8 +45,9 @@ def save_state_dict_npz(state_dict, path):
 
 # ---- training checkpoints: the reference's directory layout (ppvector/utils/checkpoint.py:104-159) ---------------------------------
 #   <save_model_path>/<model>_<feature_method>/{epoch_N, last_model, best_model}/{model.pt, optimizer.pt, model.state}
-# model.pt holds the reference's Sequential(backbone, classifier) keys ("0.<backbone tensor>", "1.weight"); optimizer.pt the Adam
-# moments, the step count and the LR / margin scheduler positions; model.state is the reference's json (last_epoch, eer, ...).
+# model.pt holds the reference's Sequential(backbone, classifier) keys ("0.<backbone tensor>", "1.weight"); optimizer.pt the optimizer's
+# name ("optimizer"), its state tensors by name (Adam's "exp_avg" / "exp_avg_sq", ...), the step count and the LR / margin scheduler
+# positions; model.state is the reference's json (last_epoch, eer, ...).
 def checkpoint_root(configs, save_model_path):
     return os.path.join(save_model_path, f'{configs.model_conf.model}_{configs.preprocess_conf.feature_method}')
 
@@ -84,6 +85,21 @@ def find_resume_dir(configs, save_model_path, resume_model):
     if all(os.path.exists(os.path.join(last, n)) for n in ('model.pt', 'optimizer.pt', 'model.state')):
         return last
     return None
+
+
+def check_optimizer_state(opt_state, name, state, path):
+    """Refuses an optimizer.pt (``opt_state``; None passes) that another optimizer than ``name`` wrote, or whose state tensors are not
+    exactly ``state``'s (name -> tensor) names and sizes.  An optimizer.pt without an ``optimizer`` entry was written by Adam."""
+    if opt_state is None:
+        return
+    saved = opt_state.get('optimizer', 'Adam')
+    if saved != name:
+        raise ValueError(f'{path}: the checkpoint was trained with the {saved} optimizer and optimizer_conf.optimizer is {name}; resume it '
+                         f'with {saved}, or start {name} from its weights with pretrained_model')
+    have = {k: tuple(v.shape) for k, v in opt_state.items() if hasattr(v, 'shape')}
+    want = {k: tuple(t.shape) for k, t in state.items()}
+    if have != want:
+        raise ValueError(f'{path}: optimizer.pt holds the {name} state {have}, the configured {name} needs {want}')
 
 
 def load_checkpoint_dir(path):
