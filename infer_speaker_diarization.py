@@ -1,5 +1,8 @@
 """Speaker diarization of one recording: who speaks when, optionally named from an enrolment database
-(counterpart of the reference's infer_speaker_diarization.py; same options).  Prints one {'speaker', 'start', 'end'} per segment."""
+(counterpart of the reference's infer_speaker_diarization.py; same options).  Prints one {'speaker', 'start', 'end'} per segment and, with
+--rttm_path, also writes them as RTTM (uri = the audio file's stem) for scoring by tools/eval_speaker_diarization/compute_metrics.py."""
+import os
+
 from cli_common import parse_options
 
 OPTIONS = [
@@ -16,12 +19,14 @@ OPTIONS = [
 # options of this build beyond the reference's
 EXTENSION_OPTIONS = [
     ('vad', bool, False, "find the speech first with Kaldi's energy VAD on the GPU (otherwise the whole recording is taken as speech)"),
+    ('rttm_path', str, None, "also write the result to this RTTM file, uri = the audio file's stem"),
 ]
 
 
 def main(opt):
     from loguru import logger
 
+    from ppvector.metric.der import write_rttm
     from ppvector.predict import PPVectorPredictor
     if opt.search_audio_db:
         assert opt.audio_db_path is not None, '请指定音频库的路径'
@@ -32,6 +37,9 @@ def main(opt):
     print('识别结果：')
     for result in results:
         print(result)
+    if opt.rttm_path is not None:
+        with open(opt.rttm_path, 'w', encoding='utf-8') as f:
+            write_rttm(f, os.path.splitext(os.path.basename(opt.audio_path))[0], [(r['start'], r['end'], r['speaker']) for r in results])
     if opt.show_plot:
         logger.info('show_plot: the matplotlib viewer is not part of this build')
 
