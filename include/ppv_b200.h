@@ -139,6 +139,14 @@ int ppv_spectral_num_frames(const ppv_spectral_t* h, int L);
 int ppv_spectral_feature_dim(const ppv_spectral_t* h);
 /* wav [B,L] fp32 -> out [B,T,F] fp32, time-mean subtracted, optional tail mask as in ppv_fbank_forward. */
 int ppv_spectral_forward(ppv_spectral_t* h, const float* wav, const float* lens_ratio, int B, int L, float* out, void* stream);
+/* A zero-padded batch of utterances of DIFFERENT lengths in one launch sequence, as ppv_fbank_forward_ragged_samples.  wav [B,L] fp32;
+ * num_samples[b] (device int32, <= L) is utterance b's own length; valid_frames[b] (device int32) must be
+ * ppv_spectral_num_frames(h, num_samples[b]).  out [B,T,F], T = ppv_spectral_num_frames(h, L): row b holds utterance b featurised
+ * as if alone (centre reflect padding at both of ITS ends, time mean over its own valid_frames[b] frames), zeros beyond.  Lengths
+ * out of range are clamped (valid_frames to [0, T], num_samples to [1, L]): that row's features are wrong, nothing outside it is
+ * read or written.  PPV_EINVAL for a null pointer, B outside [1, 65535] or L too short for one frame. */
+int ppv_spectral_forward_ragged_samples(ppv_spectral_t* h, const float* wav, const int32_t* valid_frames, const int32_t* num_samples,
+                                        int B, int L, float* out, void* stream);
 
 /* SpecAugment masking of a feature batch in place (ppvector/data_utils/reader.py:105-107, configs/augmentation.yml:36-48,
  * max_time_warp 0).  The random draws stay on the host, made with the reference's RNG calls; params is int32

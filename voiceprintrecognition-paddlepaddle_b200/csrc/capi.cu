@@ -415,6 +415,14 @@ int ppv_spectral_forward(ppv_spectral_t* h, const float* wav, const float* lens_
     return spectral_run(h->impl, wav, lens_ratio, B, L, out, static_cast<cudaStream_t>(stream));
     PPV_GUARD_END
 }
+int ppv_spectral_forward_ragged_samples(ppv_spectral_t* h, const float* wav, const int32_t* valid_frames, const int32_t* num_samples, int B,
+                                        int L, float* out, void* stream) {
+    PPV_GUARD_BEGIN
+    PPV_REQUIRE(h && wav && out && valid_frames && num_samples, "ppv_spectral_forward_ragged_samples: null argument");
+    PPV_REQUIRE(B > 0 && L > 0, "ppv_spectral_forward_ragged_samples: empty input");
+    return spectral_run(h->impl, wav, nullptr, B, L, out, static_cast<cudaStream_t>(stream), valid_frames, num_samples);
+    PPV_GUARD_END
+}
 int ppv_spec_augment(float* feat, const int32_t* params, int B, int T, int F, int n_freq_masks, int n_time_masks, int fill_mode, void* stream) {
     PPV_GUARD_BEGIN
     return spec_augment_run(feat, params, B, T, F, n_freq_masks, n_time_masks, fill_mode, static_cast<cudaStream_t>(stream));

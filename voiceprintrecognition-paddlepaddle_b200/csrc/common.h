@@ -388,7 +388,8 @@ int spectral_create(const ppv_spectral_cfg* cfg, Spectral** out);
 void spectral_destroy(Spectral* h);
 int spectral_num_frames(const Spectral* h, int L);
 int spectral_feature_dim(const Spectral* h);
-int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st);
+int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st,
+                 const int* valid_frames = nullptr, const int* num_samples = nullptr);
 int spec_augment_run(float* feat, const int32_t* params, int B, int T, int F, int n_freq_masks, int n_time_masks, int fill_mode, cudaStream_t st);
 
 // ---- model factories (ecapa.cu, resnet_se.cu, res2net.cu, eres2net.cu, campplus.cu; the Model interface is in model_common.h) -------------

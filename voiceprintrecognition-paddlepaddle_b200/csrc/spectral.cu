@@ -51,8 +51,11 @@ __device__ __forceinline__ int sp_reflect(int i, int L) {  // numpy 'reflect' (n
     return i;
 }
 
-// out_raw [B, T, F]
+// out_raw [B, T, F].  Ragged batches (both optional, nullptr: every row is L samples / T frames): row b is num_samples[b] samples
+// long, reflected at its own right edge when centred, and only its first valid_frames[b] frames are computed.  Both are clamped
+// ([1, L] and [0, T]) and every index stays inside the row, so a wrong length gives wrong features for that row, never a fault.
 __global__ void __launch_bounds__(SP_THREADS) spectral_frame_kernel(const float* __restrict__ wav, int L, int T, int F, SpecKernelArgs a,
+                                                                    const int* __restrict__ num_samples, const int* __restrict__ valid_frames,
                                                                     float* __restrict__ out_raw) {
     extern __shared__ __align__(16) uint8_t sp_smem[];
     float2* z = reinterpret_cast<float2*>(sp_smem);              // n_fft
@@ -61,11 +64,14 @@ __global__ void __launch_bounds__(SP_THREADS) spectral_frame_kernel(const float*
     griddep_launch_dependents();
     griddep_wait();
     const int t = blockIdx.x, b = blockIdx.y;
+    if (valid_frames && t >= min(max(valid_frames[b], 0), T)) return;
+    const int Lb = num_samples ? min(max(num_samples[b], 1), L) : L;
     const float* x = wav + int64_t(b) * L;
     const int N = a.n_fft;
     const int start = t * a.hop - (a.center ? N / 2 : 0);
     for (int i = threadIdx.x; i < N; i += SP_THREADS) {
-        const int src = a.center ? sp_reflect(start + i, L) : start + i;
+        // centred: an identity clamp whenever Lb > N / 2 frames it; non-centred: t < T keeps [start, start + N) inside [0, L)
+        const int src = a.center ? min(max(sp_reflect(start + i, Lb), 0), Lb - 1) : start + i;
         z[fft_bitrev(i, a.log2n)] = make_float2(x[src] * a.window[i], 0.f);
     }
     __syncthreads();
@@ -102,23 +108,27 @@ __global__ void __launch_bounds__(SP_THREADS) spectral_frame_kernel(const float*
 }
 
 // In place: x[b, t, f] -= mean_t x[b, :, f]; frames t >= int(ratio[b] * T) are zeroed after it (featurizer.py:48-59).
-// Block = (32-feature slab, utterance): 8 warps stride over time, lane = feature.
-__global__ void __launch_bounds__(256) spectral_cmn_kernel(float* __restrict__ x, const float* __restrict__ lens_ratio, int T, int F) {
+// Ragged batches (valid_frames, optional): the mean of row b runs over its first Tb = valid_frames[b] frames (clamped to [0, T]) in
+// the order of a call on that utterance alone, so the row is bitwise what that call gives; frames Tb .. T - 1 are written as zeros
+// without being read.  Block = (32-feature slab, utterance): 8 warps stride over time, lane = feature.
+__global__ void __launch_bounds__(256) spectral_cmn_kernel(float* __restrict__ x, const float* __restrict__ lens_ratio,
+                                                           const int* __restrict__ valid_frames, int T, int F) {
     __shared__ float s_part[8][32];
     griddep_launch_dependents();
     griddep_wait();
     const int b = blockIdx.y, f = blockIdx.x * 32 + (threadIdx.x & 31), warp = threadIdx.x >> 5;
+    const int Tb = valid_frames ? min(max(valid_frames[b], 0), T) : T;
     float* base = x + int64_t(b) * T * F;
     float acc = 0.f;
     if (f < F)
-        for (int t = warp; t < T; t += 8) acc += base[int64_t(t) * F + f];
+        for (int t = warp; t < Tb; t += 8) acc += base[int64_t(t) * F + f];
     s_part[warp][threadIdx.x & 31] = acc;
     __syncthreads();
     float mean = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) mean += s_part[w][threadIdx.x & 31];
-    mean /= float(T);
-    const int keep = lens_ratio ? int(lens_ratio[b] * float(T)) : T;
+    mean /= float(max(Tb, 1));
+    const int keep = min(lens_ratio ? int(lens_ratio[b] * float(T)) : T, Tb);
     if (f < F)
         for (int t = warp; t < T; t += 8) base[int64_t(t) * F + f] = t < keep ? base[int64_t(t) * F + f] - mean : 0.f;
 }
@@ -316,7 +326,8 @@ int spectral_num_frames(const Spectral* h, int L) {
 }
 int spectral_feature_dim(const Spectral* h) { return h->F; }
 
-int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st) {
+int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, int L, float* out, cudaStream_t st, const int* valid_frames,
+                 const int* num_samples) {
     PPV_REQUIRE(h && wav && out, "spectral_run: null argument");
     PPV_REQUIRE(B > 0 && B <= 65535, "spectral_run: batch must be in [1, 65535]");
     const int T = spectral_num_frames(h, L);
@@ -343,8 +354,10 @@ int spectral_run(Spectral* h, const float* wav, const float* lens_ratio, int B, 
     const size_t smem = size_t(h->n_fft) * sizeof(float2) + size_t(h->n_bins) * sizeof(float) + 512 * sizeof(float);
     PPV_ONCE_PER_DEVICE(PPV_CUDA_OK(cudaFuncSetAttribute(spectral_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)));
     PPV_REQUIRE(smem <= 64 * 1024, "spectral_run: shared memory budget exceeded");
-    PPV_PDL_OK(launch_pdl(spectral_frame_kernel, dim3(T, B), dim3(SP_THREADS), smem, st, wav, L, T, h->F, a, out), "spectral_frame_kernel");
-    PPV_PDL_OK(launch_pdl(spectral_cmn_kernel, dim3((h->F + 31) / 32, B), dim3(256), 0, st, out, lens_ratio, T, h->F), "spectral_cmn_kernel");
+    PPV_PDL_OK(launch_pdl(spectral_frame_kernel, dim3(T, B), dim3(SP_THREADS), smem, st, wav, L, T, h->F, a, num_samples, valid_frames, out),
+               "spectral_frame_kernel");
+    PPV_PDL_OK(launch_pdl(spectral_cmn_kernel, dim3((h->F + 31) / 32, B), dim3(256), 0, st, out, lens_ratio, valid_frames, T, h->F),
+               "spectral_cmn_kernel");
     return PPV_OK;
 }
 

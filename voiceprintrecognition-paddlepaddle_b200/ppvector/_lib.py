@@ -127,6 +127,7 @@ SIGNATURES = {
     "ppv_spectral_num_frames": (C.c_int, [_P, C.c_int]),
     "ppv_spectral_feature_dim": (C.c_int, [_P]),
     "ppv_spectral_forward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "ppv_spectral_forward_ragged_samples": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
     "ppv_spec_augment": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "ppv_ecapa_default_cfg": (None, [C.POINTER(EcapaCfg)]),
     "ppv_resnetse_default_cfg": (None, [C.POINTER(ResNetSECfg)]),

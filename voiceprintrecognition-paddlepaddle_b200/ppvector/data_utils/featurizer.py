@@ -162,27 +162,26 @@ class AudioFeaturizer(torch.nn.Module):
     def forward_ragged(self, waveforms, lengths):
         """A zero-padded batch of utterances of different lengths, each featurised as if alone (what the reference's training path
         computes sample by sample, reader.py:101-104, before collate_fn zero-pads the features): waveforms [B,L] CUDA, lengths [B]
-        samples -> (features [B,Tmax,F] with per-utterance CMN over its own frames and zeros beyond them, frames per utterance)."""
+        samples -> (features [B,Tmax,F] with per-utterance CMN over its own frames and zeros beyond them, frames per utterance).
+        One launch sequence for the whole batch, whatever the front end (``ppv_fbank_forward_ragged_samples`` /
+        ``ppv_spectral_forward_ragged_samples``)."""
         _lib.require_cuda(waveforms, 'waveforms')
         wav = waveforms.to(torch.float32).contiguous()
         B, L = wav.shape
         frames = [self.num_frames(int(n)) for n in lengths]
         if min(frames) <= 0:
             raise _lib.PPVError('an utterance is shorter than one frame')
-        if self._feature_method != 'Fbank':  # the STFT front ends have no ragged kernel: one call per utterance, then pad
-            T = max(frames)
-            out = torch.zeros((B, T, self.feature_dim), dtype=torch.float32, device=wav.device)
-            for b in range(B):
-                out[b, :frames[b]] = self.forward(wav[b, :int(lengths[b])])[0]
-            return out, frames
         lib, h = _lib.load(), self._get_handle()
-        T = lib.ppv_fbank_num_frames(h, L)
+        fbank = self._feature_method == 'Fbank'
+        T = (lib.ppv_fbank_num_frames if fbank else lib.ppv_spectral_num_frames)(h, L)
         vf = torch.tensor(frames, dtype=torch.int32, device=wav.device)
-        ns = torch.tensor([int(n) for n in lengths], dtype=torch.int32, device=wav.device)  # where snip_edges=False reflects each end
-        out = torch.empty((B, T, self._cfg.n_mels), dtype=torch.float32, device=wav.device)
+        # where snip_edges=False (Fbank) or center=True (the STFT front ends) reflects each utterance at its own end
+        ns = torch.tensor([int(n) for n in lengths], dtype=torch.int32, device=wav.device)
+        F = self._cfg.n_mels if fbank else lib.ppv_spectral_feature_dim(h)
+        out = torch.empty((B, T, F), dtype=torch.float32, device=wav.device)
+        name = 'ppv_fbank_forward_ragged_samples' if fbank else 'ppv_spectral_forward_ragged_samples'
         with torch.cuda.device(wav.device):
-            _lib.check(lib.ppv_fbank_forward_ragged_samples(h, _lib.ptr(wav), _lib.ptr(vf), _lib.ptr(ns), B, L, _lib.ptr(out),
-                                                            _lib.current_stream()), 'ppv_fbank_forward_ragged_samples')
+            _lib.check(getattr(lib, name)(h, _lib.ptr(wav), _lib.ptr(vf), _lib.ptr(ns), B, L, _lib.ptr(out), _lib.current_stream()), name)
         return out[:, :max(frames)], frames
 
     @property

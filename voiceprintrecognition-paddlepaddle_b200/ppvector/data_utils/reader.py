@@ -5,7 +5,7 @@ wav -> float32 -> (resample) -> dB normalise -> crop (eval: from 0; train: rando
 ``AudioFeaturizer`` on the GPU -> SpecAugment (train mode, reader.py:105-107, ``ppv_spec_augment``).  ``.npy`` entries are
 pre-extracted features (reader.py:78-83).  Waveform augmentation (reader.py:143-163: speed / volume / noise / reverb), dB normalisation
 and the crop run on the GPU (``ppvector.data_utils.audio_batch``, ``ppv_audio_prep`` / ``ppv_audio_prep_reverb``); ``load_batch`` prepares
-a whole batch with one launch sequence (decode on the host, then audio prep -> ragged Fbank -> SpecAugment), which is what
+a whole batch with one launch sequence (decode on the host, then audio prep -> ragged front end -> SpecAugment), which is what
 ``PPVectorTrainer.train`` uses.  With reverb the utterance grows by the response's length - 1 before the crop, as in the reference, so
 the crop decision and its random start are taken on the reverberant length."""
 import random

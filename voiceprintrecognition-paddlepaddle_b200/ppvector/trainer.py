@@ -137,7 +137,7 @@ class PPVectorTrainer(object):
         for i in tqdm(range(0, len(dataset), batch_size), desc=desc):
             if self.stop_eval:
                 break
-            # one launch sequence per batch (audio prep -> ragged Fbank); input_lens never reaches the model (trainer.py:392-395)
+            # one launch sequence per batch (audio prep -> ragged front end); input_lens never reaches the model (trainer.py:392-395)
             features, label, _input_lens = dataset.load_batch(range(i, min(i + batch_size, len(dataset))))
             feats.append(self.model(features))
             labels.append(label)
